@@ -4,6 +4,7 @@
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path (one process per GPU)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path (restated port) on host cores
     python bench.py --config c2a|c3|c4|c5                    # the other BASELINE.json configs at their full sizes
+    python bench.py ... --dump-outputs DIR                   # also write what the last timed step computed, as DIR/<name>.npy
 
 A "step" is one pass of the hot path over the whole workload: config C2b = enwik9-shaped text, 8192 independent
 128 KiB single-block frames (1 GiB), level 3, checksums on.  `value` is measured with compressed frames, block
@@ -35,7 +36,7 @@ def measured_peak():
     try:
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 class ClockSampler:
@@ -149,7 +150,7 @@ def workload_config(args, fs):
     return {"workload": WORKLOADS[args.config].format(n=fs.nframes, fb=args.frame_bytes), "config": args.config,
             "frames": fs.nframes, "D_bytes": fs.D, "C_bytes": fs.C, "ratio": fs.D / max(fs.C, 1), "sha256_plain": fs.sha256()[:16],
             "content_checksum_computed": True,
-            "l2": "inputs larger than L2 (C+D per pass = %.0f MB vs 126 MB L2)" % ((fs.C + fs.D) / 1e6),
+            "l2": "inputs larger than L2 (C+D per pass = %.0f MB vs 50 MB L2)" % ((fs.C + fs.D) / 1e6),
             "parallelism": "frames are independent: one process per GPU, no data-path collective"}
 
 
@@ -284,6 +285,29 @@ def run_reference(args):
     return 0
 
 
+DUMP_SAMPLE_BYTES = 1 << 21   # output bytes sampled at fixed, seeded positions
+DUMP_CHUNK = 1 << 16          # the whole output is also summarised as the byte sum of every 64 KiB chunk
+
+
+def dump_arrays(d_out, D, res, torch):
+    """What a caller of the timed path receives -- the decoded bytes and the per-frame results -- as float64 / float32 arrays
+    small enough to store (< 64 MB for any workload): a seeded sample of the output bytes, the byte sum of every 64 KiB chunk
+    of the whole output, and the per-frame result fields."""
+    rng = np.random.Generator(np.random.PCG64(0xD0E5))
+    idx = np.unique(rng.integers(0, D, min(D, DUMP_SAMPLE_BYTES), dtype=np.int64))
+    full = d_out[:D]
+    n = D // DUMP_CHUNK
+    sums = full[:n * DUMP_CHUNK].view(n, DUMP_CHUNK).sum(dim=1, dtype=torch.int64)
+    if D % DUMP_CHUNK:
+        sums = torch.cat([sums, full[n * DUMP_CHUNK:].sum(dtype=torch.int64).view(1)])
+    out = {"output_sample_index": idx.astype(np.float64),
+           "output_sample": full[torch.from_numpy(idx).to(full.device)].cpu().numpy().astype(np.float32),
+           "output_chunk_sums": sums.cpu().numpy().astype(np.float64)}
+    for f in ("status", "out_size", "bytes_read", "content_size", "calculated_checksum", "checksum_from_data"):
+        out["frame_" + f] = res[f].astype(np.float64)
+    return out
+
+
 def time_passes(batch, d_out, stream, steps, barrier, torch):
     """K passes of the device-resident path, CUDA events on the library's stream, barrier + synchronize on both sides."""
     barrier(); torch.cuda.synchronize()
@@ -315,6 +339,8 @@ def main():
     ap.add_argument("--c5-frames", type=int, default=100000)
     ap.add_argument("--e2e-steps", type=int, default=10)
     ap.add_argument("--skip-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed (output sample, per-chunk sums, per-frame results) as DIR/<name>.npy")
     args = ap.parse_args()
     args.steps_given = args.steps is not None
     if args.steps is None:
@@ -390,6 +416,8 @@ def main():
         assert (res["status"] == 0).all(), "a frame failed inside the timed region: %r" % (res[res["status"] != 0][:3],)
         out = {"fs": fs, "batch": batch, "d_out": d_out, "bit_exact": bit_exact, "ms": ms, "launches": launches, "clocks": clocks, "info": batch.info(),
                "sched": batch.debug_sched()}
+        if args.dump_outputs and rank == 0 and label == main_mode:
+            out["dump"] = dump_arrays(d_out, D, res, torch)
         # the same passes without the checksum stage (what round 1 timed)
         ctx.set_flags(0)
         batch.run(d_out); stream.synchronize()
@@ -420,6 +448,7 @@ def main():
     lo, hi = sharding.shard_frames(fs_all.src_size, world, rank) if world > 1 else (0, fs_all.nframes)
     fs_shard = fs_all.subset(lo, hi) if world > 1 else fs_all
     runs = {}
+    main_mode = args.scaling if world > 1 else "weak"
     order = ["weak", "strong"] if world > 1 else ["weak"]
     for mode in order:
         fs = fs_all if mode == "weak" else fs_shard
@@ -430,7 +459,6 @@ def main():
         m["D_total"] = fs_all.D * world if mode == "weak" else fs_all.D
         m["C_total"] = fs_all.C * world if mode == "weak" else fs_all.C
         runs[mode] = m
-    main_mode = args.scaling if world > 1 else "weak"
     M = runs[main_mode]
     fs, batch, d_out = M["fs"], M["batch"], M["d_out"]
     ms_per_step = M["ms_max"] / args.steps
@@ -449,12 +477,6 @@ def main():
         peak, peak_src = measured_peak()
         # roofline of THIS rank's pass (per-GPU quantity): algorithmic bytes of the rank's frames over the rank's pass time
         achieved = (fs.C + fs.D) / (M["ms"] / args.steps * 1e-3) / GB
-        traffic = None   # ncu DRAM bytes of one pass: captured for the C2b workload on one GPU only (profiles/traffic.py)
-        if args.config == "c2b" and fs.nframes == 8192:
-            try:
-                traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json"))).get("pipeline_dram_bytes_per_step")
-            except Exception:
-                pass
         cfg = workload_config(args, fs_all)   # identical in both arms
         run = {"frames_per_gpu": fs.nframes, "D_bytes_per_gpu": fs.D, "C_bytes_per_gpu": fs.C, "blocks_per_gpu": M["info"]["blocks"],
                "sequences_per_gpu": M["info"]["sequences"],
@@ -468,7 +490,7 @@ def main():
             "gpu_launches": int(M["launches"]),
             "clocks": M["clocks"],
             "value_without_checksum_stage": M["D_total"] / (max_over_ranks(M["ms_nochk"]) * 1e-3) / GB if world == 1 else None,
-            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
+            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                          "peak_source": peak_src, "algorithmic_bytes_per_step": fs.C + fs.D,
                          "kernel": "whole pass (k_setup, k_huf || k_fse, k_exec_cta / k_exec, k_xxh64), CUDA events over the timed region on the library stream",
                          "dominant_kernel": dominant, "kernel_ms": kern_ms, "completion_ms": timeline, "kernel_share": {k: v / tot for k, v in kern_ms.items()},
@@ -483,6 +505,10 @@ def main():
                                            "e2e": {"value": m["D_total"] / (m["e2e_ms"] * 1e-3) / GB, "unit": "GB/s", "ms_per_step": m["e2e_ms"]}}
         if numa is not None:
             line["cpu_affinity"] = numa
+        if args.dump_outputs:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            for name, a in M["dump"].items():
+                np.save(os.path.join(args.dump_outputs, name + ".npy"), a)
         if not args.skip_cpu and world == 1:   # the CPU baseline is a single-GPU-run companion (rank 0, N = 1 only)
             line["cpu_baseline"] = cpu_baseline(fs_all)
         print(json.dumps(line))

@@ -1,5 +1,5 @@
 /*
- * b200zstd.h -- C ABI of the B200-native zstd block decompressor (libb200zstd.so).
+ * b200zstd.h -- C ABI of the GPU-native (H100, sm_90a) zstd block decompressor (libb200zstd.so).
  *
  * Drop-in boundary for the decode hot path of ruzstd (KillingSpark/zstd-rs @ eb7e03cc, crate ruzstd 0.9.1).
  * Everything below replaces work that the reference does inside

@@ -22,7 +22,7 @@ for line in out.splitlines():
     m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(.*?);", line)
     if m and cur:
         funcs[cur].append(m.group(1).strip())
-lines = [f"# SASS of the shipped library (`cuobjdump -sass zstd-rs_b200/libb200zstd.so`, sm_100a), {tag}", "",
+lines = [f"# SASS of the shipped library (`cuobjdump -sass zstd-rs_b200/libb200zstd.so`, sm_90a), {tag}", "",
          "Per kernel: static instruction count, local-memory (spill) instructions, the asynchronous-copy / barrier mnemonics that show",
          "which hardware paths are used (`UBLKCP` = cp.async.bulk = TMA bulk copy, `SYNCS` = mbarrier, `LDGSTS` = cp.async), and the 14 most",
          "frequent opcodes.  Regenerate with `python profiles/sass_listing.py`.", ""]

@@ -4,7 +4,7 @@
 set -e
 cd "$(dirname "$0")/../zstd-rs_b200"
 mkdir -p variants build/var
-ARCH="-gencode arch=compute_100a,code=sm_100a"
+ARCH="-gencode arch=compute_90a,code=sm_90a"
 FL="$ARCH -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -cudart static"
 [ -f build/api.o ] && [ -f build/plan.o ] || make -s
 while [ $# -ge 2 ]; do

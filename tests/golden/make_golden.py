@@ -8,12 +8,15 @@ ones its own tests assert on (SURVEY.md section 8c):
   * ruzstd/test_fixtures/*.zst                    (tests/mod.rs:576-741; plaintexts generated in code)
   * ruzstd/fuzz/artifacts/*/*                     (tests/fuzz_regressions.rs, fse/mod.rs, huff0/mod.rs)
 Compressed inputs are copied verbatim (they are test DATA, not source); expected plaintexts are recorded as
-size + SHA-256 + XXH64-low32 in manifest.json so the repo stays small.  /root/reference does not exist on
-the GPU box, so every test reads tests/golden/ only.
+size + SHA-256 + XXH64-low32 in manifest.json, and the corpus originals as SHA-256 digests of every 64 KiB chunk in
+decodecorpus_originals.json, so the repo stays small.  Every test reads tests/golden/ only.
+
+    python tests/golden/make_golden.py <path to the ruzstd/ directory of a zstd-rs checkout>
 """
 import hashlib, json, os, shutil, sys
 
-REF = "/root/reference/ruzstd"
+REF = sys.argv[1] if len(sys.argv) > 1 else "ruzstd"
+CHUNK = 64 << 10
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "..", ".."))
 
@@ -25,6 +28,7 @@ def sha(b):
 def main():
     from oracle.oracle import xxh64
     man = {"source": "KillingSpark/zstd-rs eb7e03cc1b15705b94b93249ff7b05c4fc2c98b3", "corpus": {}, "dict": {}, "fixtures": {}, "fuzz": {}}
+    chunks = {"chunk_bytes": CHUNK, "files": {}}
     # corpus
     dst = os.path.join(HERE, "decodecorpus"); os.makedirs(dst, exist_ok=True)
     for f in sorted(os.listdir(f"{REF}/decodecorpus_files")):
@@ -32,6 +36,7 @@ def main():
             continue
         shutil.copyfile(f"{REF}/decodecorpus_files/{f}", f"{dst}/{f}")
         orig = open(f"{REF}/decodecorpus_files/{f[:-4]}", "rb").read()
+        chunks["files"][f] = [sha(orig[i:i + CHUNK]) for i in range(0, max(len(orig), 1), CHUNK)]
         man["corpus"][f] = {"size": len(orig), "sha256": sha(orig), "xxh64_low32": xxh64(orig) & 0xFFFFFFFF,
                             "compressed_size": os.path.getsize(f"{dst}/{f}")}
     # dict tests
@@ -61,6 +66,7 @@ def main():
             shutil.copyfile(f"{REF}/fuzz/artifacts/{sub}/{f}", f"{dst}/{f}")
             man["fuzz"][sub].append(f)
     json.dump(man, open(os.path.join(HERE, "manifest.json"), "w"), indent=1, sort_keys=True)
+    json.dump(chunks, open(os.path.join(HERE, "decodecorpus_originals.json"), "w"), indent=0, sort_keys=True)
     print("corpus", len(man["corpus"]), "dict", len(man["dict"]), "fixtures", len(man["fixtures"]),
           "fuzz", sum(len(v) for v in man["fuzz"].values()))
 

@@ -9,7 +9,7 @@ def _w(nseq, comp):
 
 def test_routing_crossover_on_similar_frames(pkg):
     """1 MiB Silesia-mix-shaped frames (~70 k sequences, ~410 KB compressed): few frames -> one CTA each, thousands -> one warp each
-    (measured crossover ~1,400 frames: 512 frames 4.0 vs 8.7 ms, 2048 frames 14.3 vs 10.2 ms, 4096 frames 28.0 vs 12.5 ms)."""
+    (the crossover of the cost model in csrc/plan.cpp lies between 1,024 and 2,048 frames on the 132 SMs of an H100)."""
     rng = np.random.Generator(np.random.PCG64(5))
     for n, expect_cta in ((8, True), (64, True), (512, True), (1024, True), (2048, False), (4096, False), (20000, False)):
         work = [_w(int(70000 * rng.uniform(0.1, 1.65)), int(410000 * rng.uniform(0.15, 2.3))) for _ in range(n)]

@@ -1,4 +1,4 @@
-"""zstd-rs_b200 -- B200-native zstd block decompressor behind ruzstd's FrameDecoder / StreamingDecoder API.
+"""zstd-rs_b200 -- GPU-native (H100, sm_90a) zstd block decompressor behind ruzstd's FrameDecoder / StreamingDecoder API.
 
 The product is the C-ABI library ``libb200zstd.so`` (include/b200zstd.h, sources in csrc/).  This package is the
 Python host-side mirror of the reference interface (same names, argument meaning and error behaviour as

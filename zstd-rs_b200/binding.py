@@ -58,7 +58,7 @@ def lib_path():
 
 
 def build(force=False):
-    """Compile libb200zstd.so for sm_100a in-tree (nvcc cross-compiles without a GPU)."""
+    """Compile libb200zstd.so for sm_90a in-tree (nvcc cross-compiles without a GPU)."""
     srcs = [os.path.join(_HERE, "csrc", f) for f in os.listdir(os.path.join(_HERE, "csrc"))] + [_HEADER, os.path.join(_HERE, "Makefile")]
     if force or not os.path.exists(_SO) or any(os.path.getmtime(s) > os.path.getmtime(_SO) for s in srcs):
         subprocess.check_call(["make", "-s", "-C", _HERE])
@@ -177,7 +177,7 @@ def xxh64(data):
     return lib().b200z_xxh64(b, len(b))
 
 
-def route_frames(work, eligible, sms=148):
+def route_frames(work, eligible, sms=132):
     """Host-only: the frames k_exec_cta would take (largest first) -- route_exec_frames, csrc/plan.cpp."""
     w = np.ascontiguousarray(work, dtype=np.uint64)
     el = np.ascontiguousarray(eligible, dtype=np.uint8)

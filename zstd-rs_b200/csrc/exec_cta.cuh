@@ -24,7 +24,7 @@
 // dependency, not the row order: every row publishes which of its bytes are still pending (four 32-bit planes per row,
 // plane k = ballot of "byte k of the lane's word is pending"); a byte is copied as soon as its source byte's bit is
 // clear.  Sources always precede destinations, so the lowest unfinished row can always complete; a row-to-row chain
-// (round 2's first version waited for whole rows: 400 k cycles per block) only forms where the data really chains.
+// (waiting for whole rows instead serialises every block) only forms where the data really chains.
 // Overlapping matches use source = start + (k mod offset), the byte-order-preserving form of repeat_in_chunks
 // (decode_buffer.rs:113-141).
 #pragma once

@@ -1,4 +1,4 @@
-// kernels.cu -- sm_100a kernels of the zstd block-decompression hot path.
+// kernels.cu -- sm_90a kernels of the zstd block-decompression hot path.
 //
 //   k_predefined : the three predefined FSE LUTs, built once per context
 //   k_setup      : per block: Huffman tree description -> huff0 LUT, FSE table descriptions -> LL/OF/ML LUTs
@@ -1007,8 +1007,10 @@ constexpr uint32_t EXEC_TMAX = B200Z_EXEC_TMAX;             // most bytes one ba
 #endif
 constexpr uint32_t EXEC_CHUNK_ROWS = B200Z_EXEC_CHUNK_ROWS;                    // rows (of 32 bytes) whose loads are in flight together
 constexpr uint32_t EXEC_MASK_WORDS = (EXEC_TMAX + 31) / 32 + EXEC_CHUNK_ROWS;
+// CTAs per SM the register budget must allow: 6 gives 80 registers (few spills).  On an H100 this runs k_exec ~19 % faster
+// than 8 (64 registers, ~190 bytes of spills per thread); 4 and 5 measure the same as 6.
 #ifndef B200Z_EXEC_MINB
-#define B200Z_EXEC_MINB 8
+#define B200Z_EXEC_MINB 6
 #endif
 
 __global__ void __launch_bounds__(EXEC_WARPS * 32, B200Z_EXEC_MINB) k_exec(const BlockDesc *__restrict__ descs, const BlockAux *__restrict__ aux,
@@ -1377,7 +1379,7 @@ __global__ void k_xxh64(const FrameDesc *__restrict__ frames, FrameState *__rest
     uint64_t v = k == 0 ? P1 + P2 : (k == 1 ? P2 : (k == 2 ? 0ull : 0ull - P1));
     const uint8_t *q = p + 8 * k;
     // the accumulator is a serial chain, the loads are not: 16 stripes' words are requested together (the loop is bound by
-    // memory latency otherwise: 1 ms per GiB with one load in flight per lane)
+    // memory latency otherwise, with one load in flight per lane)
     uint64_t s = 0;
     if ((((uintptr_t)q) & 7) == 0) {
         // software pipelined: the next 16 stripes' words are in flight while this batch goes through the (serial) rounds -- what a
@@ -1574,7 +1576,7 @@ int init_kernels() {
 
 uint32_t num_sms() {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64 || g_num_sms[dev] <= 0) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64 || g_num_sms[dev] <= 0) return 132;
     return (uint32_t)g_num_sms[dev];
 }
 
@@ -1591,8 +1593,8 @@ int launch_stage(const PipelineArgs &a, int stage, cudaStream_t s) {
         case 2:
             if (a.nblocks) {
                 // default: one warp walks chain and values (106 instructions per sequence).  B200Z_FSE=2: chain warp + value warp
-                // through a shared-memory queue (k_fse2) -- measured slower on B200 (1.34 vs 1.13 ms on C2b: the chain only drops to
-                // 92 instructions and pays for the queue hand-off), kept for A/B runs.
+                // through a shared-memory queue (k_fse2) -- the chain only drops to 92 instructions and pays for the queue hand-off;
+                // kept for A/B runs.
                 static const bool one_warp = [] { const char *e = getenv("B200Z_FSE"); return !(e && e[0] == '2'); }();
                 if (one_warp) k_fse<<<cdiv(a.nblocks, FSE_BLOCKS_PER_CTA), 32, kFseSmem, s>>>(a.descs, a.aux, a.input, a.seq_scratch, a.nblocks, a.fse_order);
                 else k_fse2<<<cdiv(a.nblocks, F2_LANES), 64, kFse2Smem, s>>>(a.descs, a.aux, a.input, a.seq_scratch, a.nblocks);

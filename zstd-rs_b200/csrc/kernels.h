@@ -42,7 +42,7 @@ int launch_pipeline(const PipelineArgs &a, cudaStream_t s);   // the stages one 
 // device-side header walk for device-resident input (k_walk): fill = 0 counts the blocks of every frame, fill = 1 writes the digests
 int launch_walk(const uint8_t *d_input, uint64_t input_len, const uint64_t *d_src_off, const uint64_t *d_src_size, uint32_t nframes, WalkFrame *d_wf,
                 const uint32_t *d_first_block, WalkBlock *d_wb, int fill, cudaStream_t s);
-uint32_t num_sms();   // of the current device (148 on B200)
+uint32_t num_sms();   // of the current device (132 on H100 SXM)
 int launch_checksum(const PipelineArgs &a, cudaStream_t s);   // optional 5th stage: XXH64 of every frame's plaintext
 struct PipelineStreams { cudaStream_t main, side; cudaEvent_t fork, join; };
 int launch_pipeline_overlapped(const PipelineArgs &a, const PipelineStreams &ps);   // the shipped order: k_exec beside k_fse (programmatic dependent launch)

@@ -196,13 +196,12 @@ uint64_t XXH64State::digest() const {
 // ---------------------------------------------------------------------------------------------------------------
 // Scheduling decisions (plan.h).  k_exec_cta puts a whole CTA on a frame's chain of blocks (~15x faster per frame), k_exec one warp --
 // but k_exec keeps ~4,700 frames in flight and needs fewer instructions per byte, so it wins once there are enough frames to fill
-// the machine.  Measured, 1 MiB Silesia-mix frames of 8 blocks, execution kernel alone: 512 frames 4.0 ms with CTAs / 8.7 ms with
-// warps, 2048 frames 14.3 / 10.2 ms, 4096 frames 28.0 / 12.5 ms; 64 chained 16 MiB text frames 17.4 ms with CTAs.  Model, fitted to
-// those:   t_cta  = max(sum w / SMs, largest w) * kCtaMs            (one CTA per frame, a frame at a time)
+// the machine (on 1 MiB Silesia-mix frames of 8 blocks the crossover lies between 1,024 and 2,048 frames).  Model:
+//          t_cta  = max(sum w / SMs, largest w) * kCtaMs            (one CTA per frame, a frame at a time)
 //          t_warp = largest w * kWarpChainMs + sum w * kWarpMs      (the longest chain, slowed down by everything else in flight)
 // The eligible frames are sorted by work; the k largest would go to CTAs and the rest to warps (the two kernels run one after the
-// other: each wants whole SMs).  A real split is taken only when the model promises a clear gain over both pure choices (measured on
-// 4096 similar frames: the 171 largest on CTAs shortened k_exec by 0.9 ms and cost 2.4 ms of k_exec_cta).
+// other: each wants whole SMs).  A real split is taken only when the model promises a clear gain over both pure choices: on similar
+// frames the time a split saves in k_exec is smaller than what it adds in k_exec_cta.
 // ---------------------------------------------------------------------------------------------------------------
 void route_exec_frames(const uint64_t *work, const uint8_t *eligible, size_t nframes, uint32_t sms_u, std::vector<uint32_t> &cta_frames) {
     cta_frames.clear();
