@@ -1,0 +1,138 @@
+#!/usr/bin/env python3
+"""bench_compress.py -- input GB/s of the batch compressor (b200z_compress_frames_batch, ruzstd's Fastest level, checksum on).
+
+    python bench_compress.py [--steps K] [--warmup W] [--skip-cpu]
+
+The workload is the C2b plaintext (1 GiB of enwik9-shaped text, datagen.c2_text_plain), device-resident, in two shapes:
+8192 frames of 128 KiB and one 1 GiB frame (C2a's plaintext shape, where the content checksum is four serial chains).
+Prints one JSON line: per shape the input GB/s (CUDA events around the call, median of the steps), the ratio, each kernel's
+milliseconds, (input + output bytes) / t against the HBM peak, the card's name and power limit, and `cpu_baseline`:
+libzstd 1.5.5 level 1 on the same 128 KiB pieces, one thread and all host threads.  Nothing is written to the tree.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, ROOT)
+
+import bench  # noqa: E402  (measured_peak, host_threads)
+
+GB = 1e9
+
+
+def card_info():
+    """Name and enforced power limit of GPU 0 (read-only NVML queries)."""
+    import torch
+    info = {"name": torch.cuda.get_device_name(0)}
+    try:
+        import pynvml
+        pynvml.nvmlInit()
+        info["power_limit_W"] = pynvml.nvmlDeviceGetEnforcedPowerLimit(pynvml.nvmlDeviceGetHandleByIndex(0)) / 1000.0
+    except Exception:
+        try:
+            out = subprocess.check_output(["nvidia-smi", "-i", "0", "--query-gpu=power.limit", "--format=csv,noheader,nounits"], text=True)
+            info["power_limit_W"] = float(out.strip().splitlines()[0])
+        except Exception as e:
+            info["power_limit_W"] = f"unknown ({str(e)[:60]})"
+    return info
+
+
+def libzstd_compress_baseline(datas):
+    """libzstd 1.5.5 level 1 (one frame per piece): one thread on the first 64 pieces, and all host threads on all of them."""
+    import datagen as G
+    from concurrent.futures import ThreadPoolExecutor
+    sub = datas[:64]
+    t0 = time.perf_counter()
+    n1 = sum(len(G.compress(d, level=1)) for d in sub)
+    one = sum(len(d) for d in sub) / (time.perf_counter() - t0) / GB
+    threads = bench.host_threads()
+    with ThreadPoolExecutor(max_workers=threads) as ex:
+        t0 = time.perf_counter()
+        sizes = list(ex.map(lambda d: len(G.compress(d, level=1)), datas))
+        dt = time.perf_counter() - t0
+    total = sum(len(d) for d in datas)
+    return {"kind": "libzstd 1.5.5 level 1", "one_core_GBps": one, "one_core_ratio": sum(len(d) for d in sub) / n1,
+            "all_cores_GBps": total / dt / GB, "cores": threads, "ratio": total / sum(sizes)}
+
+
+def run_compress(args):
+    """b200z_compress_frames_batch at the Fastest level on the 1 GiB C2b plaintext, device-resident, in two shapes:
+    8192 frames of 128 KiB (C2b) and one 1 GiB frame (C2a's plaintext shape).  Each output is first decoded on the GPU and must
+    equal the input; then the call is timed with CUDA events after warm-up, and one more run with a CUDA event between kernels
+    gives each kernel's time."""
+    import torch
+    import _pkg
+    import datagen
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_compress.py needs a CUDA device: the product path has no CPU fallback")
+    pkg = _pkg.load()
+    ctx = pkg.Context(0)
+    total = args.c2a_bytes
+    plain = datagen.c2_text_plain(total)
+    d_in = torch.from_numpy(plain).cuda()
+    peak, peak_src = bench.measured_peak()
+    line = {"metric": "compress_GBps", "unit": "GB/s", "level": "Fastest", "checksum": True, "card": card_info(), "input_bytes": total, "shapes": {}}
+    for shape, frame_bytes in (("c2b", args.frame_bytes), ("c2a", total)):
+        nfr = total // frame_bytes
+        io = np.zeros(nfr, dtype=pkg.binding.COMPRESS_IO_DTYPE)
+        cap = pkg.compress_bound(frame_bytes)
+        for i in range(nfr):
+            io[i] = (i * frame_bytes, frame_bytes, i * cap, cap)
+        d_out = torch.empty(nfr * cap, dtype=torch.uint8, device="cuda")
+        res = pkg.compress_frames(ctx, d_in, io, d_out)
+        assert (res["status"] == 0).all()
+        dio = np.zeros(nfr, dtype=pkg.binding.FRAME_IO_DTYPE)
+        dio["src_off"], dio["src_size"], dio["out_off"], dio["out_cap"] = io["dst_off"], res["dst_size"], io["src_off"], frame_bytes
+        back = torch.empty(total + 16, dtype=torch.uint8, device="cuda")
+        dres = pkg.decode_frames(ctx, d_out, dio, back)
+        assert (dres["status"] == 0).all() and torch.equal(back[:total], d_in), f"{shape}: GPU decode of the compressed frames differs from the input"
+        del back
+        for _ in range(args.warmup):
+            pkg.compress_frames(ctx, d_in, io, d_out)
+        stream = torch.cuda.ExternalStream(ctx.stream())
+        times = []
+        for _ in range(args.steps):
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record(stream)
+            pkg.compress_frames(ctx, d_in, io, d_out)
+            b.record(stream)
+            b.synchronize()
+            times.append(a.elapsed_time(b) / 1e3)
+        ctx.set_flags(pkg.binding.FLAG_PROFILE)
+        pkg.compress_frames(ctx, d_in, io, d_out)
+        prof = pkg.compress_profile(ctx)
+        ctx.set_flags(0)
+        t = float(np.median(times))
+        out_bytes = int(res["dst_size"].sum())
+        line["shapes"][shape] = {"frames": nfr, "frame_bytes": frame_bytes, "value": total / t / GB, "ms": t * 1e3,
+                                 "ms_min_max": [min(times) * 1e3, max(times) * 1e3], "ratio": total / out_bytes, "output_bytes": out_bytes,
+                                 "kernel_ms": prof, "roofline": {"bytes_per_call": total + out_bytes, "peak_GBps": peak, "peak_source": peak_src,
+                                                                 "fraction": (total + out_bytes) / t / GB / peak},
+                                 "raw_blocks": int(res["raw_blocks"].sum()), "rle_blocks": int(res["rle_blocks"].sum()), "blocks": int(res["blocks"].sum())}
+        del d_out
+    line["value"], line["ratio"] = line["shapes"]["c2b"]["value"], line["shapes"]["c2b"]["ratio"]
+    if not args.skip_cpu:
+        line["cpu_baseline"] = libzstd_compress_baseline([plain[i:i + args.frame_bytes] for i in range(0, total, args.frame_bytes)])
+    ctx.close()
+    print(json.dumps(line))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--frame-bytes", type=int, default=131072)
+    ap.add_argument("--c2a-bytes", type=int, default=1 << 30, help="total plaintext bytes (both shapes)")
+    ap.add_argument("--skip-cpu", action="store_true")
+    run_compress(ap.parse_args())
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

@@ -380,6 +380,50 @@ b200z_frame_decoder *b200z_streaming_decoder_frame_decoder(b200z_streaming_decod
 b200z_frame_decoder *b200z_streaming_decoder_into_frame_decoder(b200z_streaming_decoder *s);
 void b200z_streaming_decoder_free(b200z_streaming_decoder *s);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Batch compressor -- ruzstd's encoding::{compress, compress_to_vec, FrameCompressor::compress} (encoding/mod.rs:24-67,
+ * frame_compressor.rs:131-224) for many independent frames in one submission, every block of every frame encoded at once.
+ * Frames are standard zstd: Single_Segment = 0, a 128 KiB window, Frame_Content_Size always present (smallest legal field;
+ * the reference writes none), 128 KiB blocks, an optional content checksum (XXH64 seed 0, low 32 bits).  Blocks are RLE when
+ * all their bytes are equal, else Compressed when that is smaller, else Raw; a Compressed block never refers to another
+ * block's tables (no Treeless / Repeat modes, no repeat offsets).  The output need not equal the reference's byte for byte.
+ * ---------------------------------------------------------------------------------------------------------- */
+typedef struct b200z_compress_io {
+    uint64_t src_off;   /* the frame's plaintext inside `input`                                  */
+    uint64_t src_size;
+    uint64_t dst_off;   /* where the frame goes inside `output`                                  */
+    uint64_t dst_cap;   /* room reserved there; must be >= b200z_compress_bound(src_size)         */
+} b200z_compress_io;
+
+typedef struct b200z_compress_result {
+    uint64_t dst_size;  /* bytes of the frame written at dst_off                                 */
+    int32_t status;     /* 0 or b200z_error                                                      */
+    uint32_t blocks;    /* blocks in the frame                                                   */
+    uint32_t raw_blocks, rle_blocks;
+    uint32_t has_checksum, checksum;
+} b200z_compress_result;
+
+/* CompressionLevel (encoding/mod.rs:24-67): Default = 2, Better = 3, Best = 4 are unimplemented!() in the reference */
+#define B200Z_LEVEL_UNCOMPRESSED 0
+#define B200Z_LEVEL_FASTEST 1
+/* context flag: b200z_compress_frames_batch records a CUDA event between its kernels and keeps each kernel's milliseconds
+ * for b200z_compress_last_profile (profiling aid for bench.py; it synchronises anyway) */
+#define B200Z_FLAG_PROFILE 2u
+
+/* the largest frame b200z_compress_frames_batch can write for src_size bytes: src_size + 14 + 3 * max(1, ceil(src_size / 131072)) + 4 */
+size_t b200z_compress_bound(size_t src_size);
+/* Compresses `nframes` frames.  `input` / `output` are host or device memory (B200Z_MEM_*); `checksum` != 0 appends the
+ * content checksum.  Returns 0 when the submission ran (results[nframes] filled).  Checked before any launch:
+ * B200Z_ERR_INVALID_ARGUMENT for a range outside `input` / `output`, dst_cap < b200z_compress_bound(src_size), overlapping
+ * destination ranges or an unknown level; B200Z_ERR_REFERENCE_WOULD_PANIC for the levels the reference does not implement. */
+int b200z_compress_frames_batch(b200z_ctx *ctx, const uint8_t *input, size_t input_len, int input_mem,
+                                const b200z_compress_io *frames, size_t nframes, int level, int checksum,
+                                uint8_t *output, size_t output_cap, int output_mem, b200z_compress_result *results);
+int b200z_compress_num_stages(void);
+const char *b200z_compress_stage_name(int stage);
+/* each kernel's device milliseconds in the last b200z_compress_frames_batch run with B200Z_FLAG_PROFILE set */
+int b200z_compress_last_profile(const b200z_ctx *ctx, float *stage_ms, size_t n);
+
 /* XXH64(seed 0) of a host buffer -- the content-checksum hash the reference feeds on drain
  * (decode_buffer.rs:42,225,290,301); exposed so bindings can verify checksums like tests/decode_corpus.rs:61-74 */
 uint64_t b200z_xxh64(const uint8_t *data, size_t len);

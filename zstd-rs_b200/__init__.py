@@ -1,4 +1,5 @@
-"""zstd-rs_b200 -- GPU-native (H100, sm_90a) zstd block decompressor behind ruzstd's FrameDecoder / StreamingDecoder API.
+"""zstd-rs_b200 -- GPU-native (H100, sm_90a) zstd block decompressor behind ruzstd's FrameDecoder / StreamingDecoder API,
+and a batch compressor at ruzstd's Uncompressed and Fastest levels (compress_frames / compress_to_vec).
 
 The product is the C-ABI library ``libb200zstd.so`` (include/b200zstd.h, sources in csrc/).  This package is the
 Python host-side mirror of the reference interface (same names, argument meaning and error behaviour as
@@ -8,7 +9,7 @@ There is no CPU decode path: every decode call needs a CUDA device and fails lou
 Import name: ``zstd_rs_b200`` (the directory name has a hyphen; see ``_pkg.py`` at the repo root).
 """
 from .binding import (  # noqa: F401
-    ALL, UPTO_BLOCKS, UPTO_BYTES, B200ZError, Batch, Context, Dictionary, FrameDecoder, StreamingDecoder,
-    build, decode_blocks, decode_frames, error_names, lib, lib_path, xxh64,
+    ALL, FASTEST, UNCOMPRESSED, UPTO_BLOCKS, UPTO_BYTES, B200ZError, Batch, Context, Dictionary, FrameDecoder, StreamingDecoder,
+    build, compress_bound, compress_frames, compress_profile, compress_to_vec, decode_blocks, decode_frames, error_names, lib, lib_path, xxh64,
 )
 from . import binding  # noqa: F401

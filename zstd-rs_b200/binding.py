@@ -26,6 +26,8 @@ ALL, UPTO_BLOCKS, UPTO_BYTES = 0, 1, 2
 MEM_HOST, MEM_DEVICE = 0, 1
 ERR_SKIP_FRAME = 8
 FLAG_CHECKSUM = 1
+FLAG_PROFILE = 2
+UNCOMPRESSED, FASTEST = 0, 1   # CompressionLevel (ruzstd encoding/mod.rs:24-67); Default / Better / Best are not implemented there
 
 
 class FrameIO(C.Structure):
@@ -50,6 +52,9 @@ FRAME_RESULT_DTYPE = np.dtype([("out_size", "<u8"), ("bytes_read", "<u8"), ("con
                                ("status", "<i4"), ("stage", "<i4"), ("blocks_decoded", "<u4"), ("error_block", "<u4"),
                                ("has_checksum", "<u4"), ("checksum_from_data", "<u4"), ("has_dict_id", "<u4"), ("dict_id", "<u4"),
                                ("has_calculated_checksum", "<u4"), ("calculated_checksum", "<u4")])
+COMPRESS_IO_DTYPE = np.dtype([("src_off", "<u8"), ("src_size", "<u8"), ("dst_off", "<u8"), ("dst_cap", "<u8")])
+COMPRESS_RESULT_DTYPE = np.dtype([("dst_size", "<u8"), ("status", "<i4"), ("blocks", "<u4"), ("raw_blocks", "<u4"), ("rle_blocks", "<u4"),
+                                  ("has_checksum", "<u4"), ("checksum", "<u4")])
 assert FRAME_IO_DTYPE.itemsize == C.sizeof(FrameIO) and FRAME_RESULT_DTYPE.itemsize == C.sizeof(FrameResult)
 
 
@@ -143,6 +148,11 @@ def lib():
         "b200z_streaming_decoder_into_frame_decoder": (vp, [vp]),
         "b200z_streaming_decoder_free": (None, [vp]),
         "b200z_xxh64": (C.c_uint64, [vp, sz]),
+        "b200z_compress_bound": (sz, [sz]),
+        "b200z_compress_frames_batch": (C.c_int, [vp, vp, sz, C.c_int, vp, sz, C.c_int, C.c_int, vp, sz, C.c_int, vp]),
+        "b200z_compress_num_stages": (C.c_int, []),
+        "b200z_compress_stage_name": (C.c_char_p, [C.c_int]),
+        "b200z_compress_last_profile": (C.c_int, [vp, C.POINTER(C.c_float), sz]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)          # AttributeError here == a symbol the header declares is not exported
@@ -344,6 +354,43 @@ def decode_frames(ctx, input, frames, output, dicts=None, forced_dict=None, max_
                                         res.ctypes.data)
     ctx._chk(e)
     return res
+
+
+def compress_bound(n):
+    """b200z_compress_bound: the largest frame compress_frames can write for n input bytes."""
+    return lib().b200z_compress_bound(n)
+
+
+def compress_frames(ctx, input, io, output, level=FASTEST, checksum=True):
+    """b200z_compress_frames_batch: one zstd frame per COMPRESS_IO_DTYPE row (src_off, src_size, dst_off, dst_cap), every block of
+    every frame compressed at once.  input/output: bytes, numpy or torch (host or cuda).  Returns COMPRESS_RESULT_DTYPE rows."""
+    fr = np.ascontiguousarray(io, dtype=COMPRESS_IO_DTYPE)
+    res = np.zeros(len(fr), dtype=COMPRESS_RESULT_DTYPE)
+    ip, il, _k1 = _ptr(input)
+    op, ol, _k2 = _ptr(output)
+    e = ctx.L.b200z_compress_frames_batch(ctx.h, ip, il, MEM_DEVICE if _is_device(input) else MEM_HOST, fr.ctypes.data, len(fr), level,
+                                          1 if checksum else 0, op, ol, MEM_DEVICE if _is_device(output) else MEM_HOST, res.ctypes.data)
+    ctx._chk(e)
+    return res
+
+
+def compress_to_vec(ctx, data, level=FASTEST, checksum=True):
+    """Mirror of ruzstd::encoding::compress_to_vec (encoding/mod.rs): one frame holding `data`, as bytes."""
+    src = bytes(data)
+    cap = compress_bound(len(src))
+    out = np.zeros(cap, dtype=np.uint8)
+    io = np.array([(0, len(src), 0, cap)], dtype=COMPRESS_IO_DTYPE)
+    res = compress_frames(ctx, src, io, out, level, checksum)
+    return out[:int(res[0]["dst_size"])].tobytes()
+
+
+def compress_profile(ctx):
+    """{kernel name: ms} of the last compress_frames call made with FLAG_PROFILE set on the context."""
+    L = ctx.L
+    n = L.b200z_compress_num_stages()
+    ms = (C.c_float * n)()
+    ctx._chk(L.b200z_compress_last_profile(ctx.h, ms, n))
+    return {L.b200z_compress_stage_name(i).decode(): ms[i] for i in range(n)}
 
 
 class Batch:

@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "../../include/b200zstd.h"
+#include "compress.h"
 #include "kernels.h"
 #include "plan.h"
 #include "tables.cuh"
@@ -83,6 +84,7 @@ struct b200z_ctx {
     cudaStream_t side = nullptr;          // k_huf runs here, beside k_fse
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     struct PipeResources *pipe = nullptr;  // lazily created by the pipelined one-shot path
+    struct CompressResources *comp = nullptr;   // lazily created by the first compression
     FseSlot *d_predef = nullptr;
     std::string err;
     uint64_t launches = 0;
@@ -119,7 +121,7 @@ extern "C" int b200z_ctx_create(int device, b200z_ctx **out) {
     if (cudaStreamCreateWithPriority(&c->side, cudaStreamNonBlocking, prio_lo) != cudaSuccess || cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming) != cudaSuccess) { cudaGetLastError(); return B200Z_ERR_CUDA; }
     if (cudaMalloc((void **)&c->d_predef, sizeof(FseSlot)) != cudaSuccess) { cudaGetLastError(); return B200Z_ERR_OUT_OF_MEMORY; }
-    if (init_kernels()) { cudaGetLastError(); return B200Z_ERR_CUDA; }
+    if (init_kernels() || init_compress_kernels()) { cudaGetLastError(); return B200Z_ERR_CUDA; }
     int e = launch_predefined(c->d_predef, c->stream);
     if (e || cudaStreamSynchronize(c->stream) != cudaSuccess) { cudaGetLastError(); return B200Z_ERR_CUDA; }
     c->launches = 1;
@@ -127,10 +129,12 @@ extern "C" int b200z_ctx_create(int device, b200z_ctx **out) {
     return 0;
 }
 static void pipe_free(b200z_ctx *c);
+static void compress_free(b200z_ctx *c);
 extern "C" void b200z_ctx_destroy(b200z_ctx *c) {
     if (!c) return;
     cudaSetDevice(c->device);
     pipe_free(c);
+    compress_free(c);
     if (c->d_predef) cudaFree(c->d_predef);
     if (c->ev_fork) cudaEventDestroy(c->ev_fork);
     if (c->ev_join) cudaEventDestroy(c->ev_join);
@@ -1640,4 +1644,130 @@ extern "C" void b200z_streaming_decoder_free(b200z_streaming_decoder *s) {
     if (!s) return;
     if (s->owns) b200z_frame_decoder_free(s->dec);
     delete s;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// batch compressor (encoding::compress / compress_to_vec / FrameCompressor::compress at Uncompressed and Fastest):
+// host checks and the block plan, then k_cmatch -> k_cenc -> k_cxxh64 -> k_cassemble on the ctx stream
+// ---------------------------------------------------------------------------------------------------------------
+extern "C" size_t b200z_compress_bound(size_t n) {
+    const size_t blocks = std::max<size_t>(1, (n + ENC_BLOCK - 1) / ENC_BLOCK);
+    return n + 14 + 3 * blocks + 4;
+}
+extern "C" int b200z_compress_num_stages(void) { return kCompressStages; }
+extern "C" const char *b200z_compress_stage_name(int stage) { return stage >= 0 && stage < kCompressStages ? kCompressStageNames[stage] : ""; }
+
+struct CompressResources {
+    DevBuf frames, blocks, lit_stage, seq_stage, lits, seqs, info, res, csum, results, input, output;
+    cudaEvent_t ev[kCompressStages + 1] = {};
+    float stage_ms[kCompressStages] = {};
+    bool profiled = false;
+};
+static void compress_free(b200z_ctx *c) {
+    if (!c->comp) return;
+    for (cudaEvent_t e : c->comp->ev) if (e) cudaEventDestroy(e);
+    delete c->comp;
+    c->comp = nullptr;
+}
+extern "C" int b200z_compress_last_profile(const b200z_ctx *c, float *stage_ms, size_t n) {
+    if (!c || !stage_ms || !c->comp || !c->comp->profiled) return B200Z_ERR_INVALID_ARGUMENT;
+    for (size_t i = 0; i < n && i < (size_t)kCompressStages; i++) stage_ms[i] = c->comp->stage_ms[i];
+    return 0;
+}
+
+extern "C" int b200z_compress_frames_batch(b200z_ctx *c, const uint8_t *input, size_t input_len, int input_mem, const b200z_compress_io *frames,
+                                           size_t nframes, int level, int checksum, uint8_t *output, size_t output_cap, int output_mem,
+                                           b200z_compress_result *results) {
+    // ---- everything is checked before any device work
+    if (level >= 2 && level <= 4) return B200Z_ERR_REFERENCE_WOULD_PANIC;   // Default / Better / Best: unimplemented!() in the reference
+    if (!c || (level != B200Z_LEVEL_UNCOMPRESSED && level != B200Z_LEVEL_FASTEST)) return B200Z_ERR_INVALID_ARGUMENT;
+    if ((nframes && (!frames || !results)) || (input_mem != B200Z_MEM_HOST && input_mem != B200Z_MEM_DEVICE) ||
+        (output_mem != B200Z_MEM_HOST && output_mem != B200Z_MEM_DEVICE) || (input_len && !input) || (output_cap && !output) || nframes > 0xffffffffu) {
+        c->err = "invalid argument";
+        return B200Z_ERR_INVALID_ARGUMENT;
+    }
+    std::vector<std::pair<uint64_t, uint64_t>> dst;
+    uint64_t nblocks = 0;
+    for (size_t i = 0; i < nframes; i++) {
+        const b200z_compress_io &f = frames[i];
+        if (f.src_off > input_len || f.src_size > input_len - f.src_off || f.dst_off > output_cap || f.dst_cap > output_cap - f.dst_off ||
+            f.dst_cap < b200z_compress_bound(f.src_size)) {
+            c->err = "frame " + std::to_string(i) + ": range outside input/output or dst_cap < b200z_compress_bound(src_size)";
+            return B200Z_ERR_INVALID_ARGUMENT;
+        }
+        dst.push_back({f.dst_off, f.dst_cap});
+        nblocks += std::max<uint64_t>(1, (f.src_size + ENC_BLOCK - 1) / ENC_BLOCK);
+    }
+    std::sort(dst.begin(), dst.end());
+    for (size_t i = 1; i < dst.size(); i++)
+        if (dst[i - 1].first + dst[i - 1].second > dst[i].first) { c->err = "overlapping destination ranges"; return B200Z_ERR_INVALID_ARGUMENT; }
+    if (nblocks > 0xffffffffu) return B200Z_ERR_INVALID_ARGUMENT;
+    if (!nframes) return 0;
+    if (int e = c->use()) return e;
+    // ---- plan: frames -> 128 KiB blocks
+    std::vector<CFrame> hf(nframes);
+    std::vector<CBlock> hb;
+    hb.reserve(nblocks);
+    for (size_t i = 0; i < nframes; i++) {
+        const b200z_compress_io &f = frames[i];
+        hf[i] = CFrame{f.src_off, f.src_size, f.dst_off, (uint32_t)hb.size(), 0};
+        uint64_t pos = 0;
+        do {
+            const uint32_t size = (uint32_t)std::min<uint64_t>(ENC_BLOCK, f.src_size - pos);
+            hb.push_back(CBlock{f.src_off + pos, size, (uint32_t)std::min<uint64_t>(pos, ENC_WINDOW), (uint32_t)i, 0});
+            pos += size;
+        } while (pos < f.src_size);
+        hf[i].nblocks = (uint32_t)hb.size() - hf[i].first_block;
+    }
+    if (!c->comp) {
+        c->comp = new CompressResources();
+        for (cudaEvent_t &e : c->comp->ev) CU(c, cudaEventCreate(&e));
+    }
+    CompressResources &r = *c->comp;
+    const bool fast = level == B200Z_LEVEL_FASTEST;
+    int e = 0;
+    if ((e = r.frames.ensure(nframes * sizeof(CFrame))) || (e = r.blocks.ensure(nblocks * sizeof(CBlock))) ||
+        (e = r.res.ensure(nblocks * sizeof(CBlockInfo))) || (e = r.csum.ensure(nframes * 8)) ||
+        (e = r.results.ensure(nframes * sizeof(b200z_compress_result))))
+        return e;
+    if (fast && ((e = r.lit_stage.ensure(nblocks * ENC_BLOCK)) || (e = r.seq_stage.ensure(nblocks * CBLOCK_SEQS * sizeof(SeqRec))) ||
+                 (e = r.lits.ensure(nblocks * ENC_BLOCK)) || (e = r.seqs.ensure(nblocks * CBLOCK_SEQS * sizeof(SeqRec))) ||
+                 (e = r.info.ensure(nblocks * sizeof(CBlockInfo)))))
+        return e;
+    const uint8_t *d_in = input;
+    uint8_t *d_out = output;
+    cudaStream_t s = c->stream;
+    if (input_mem == B200Z_MEM_HOST) {
+        if ((e = r.input.ensure(input_len + 16))) return e;
+        CU(c, cudaMemcpyAsync(r.input.p, input, input_len, cudaMemcpyHostToDevice, s));
+        d_in = r.input.as<uint8_t>();
+    }
+    if (output_mem == B200Z_MEM_HOST) {
+        if ((e = r.output.ensure(output_cap + 16))) return e;
+        d_out = r.output.as<uint8_t>();
+    }
+    CU(c, cudaMemcpyAsync(r.frames.p, hf.data(), nframes * sizeof(CFrame), cudaMemcpyHostToDevice, s));
+    CU(c, cudaMemcpyAsync(r.blocks.p, hb.data(), nblocks * sizeof(CBlock), cudaMemcpyHostToDevice, s));
+    CompressArgs a{};
+    a.frames = r.frames.as<CFrame>(); a.blocks = r.blocks.as<CBlock>(); a.input = d_in; a.output = d_out;
+    a.lit_stage = r.lit_stage.as<uint8_t>(); a.seq_stage = r.seq_stage.as<SeqRec>(); a.lits = r.lits.as<uint8_t>(); a.seqs = r.seqs.as<SeqRec>();
+    a.enc = a.lit_stage; a.info = r.info.as<CBlockInfo>(); a.res = r.res.as<CBlockInfo>(); a.csum = r.csum.as<uint64_t>();
+    a.results = r.results.as<b200z_compress_result>(); a.nframes = (uint32_t)nframes; a.nblocks = (uint32_t)nblocks; a.level = level;
+    a.checksum = checksum ? 1 : 0;
+    const bool prof = (c->flags & B200Z_FLAG_PROFILE) != 0;
+    if (prof) CU(c, cudaEventRecord(r.ev[0], s));
+    for (int st = 0; st < kCompressStages; st++) {
+        if (int le = launch_compress_stage(a, st, s)) return c->set_cuda_err((cudaError_t)le, kCompressStageNames[st]);
+        if (prof) CU(c, cudaEventRecord(r.ev[st + 1], s));
+    }
+    c->launches += compress_launch_count(a);
+    CU(c, cudaMemcpyAsync(results, r.results.p, nframes * sizeof(b200z_compress_result), cudaMemcpyDeviceToHost, s));
+    CU(c, cudaStreamSynchronize(s));
+    if (output_mem == B200Z_MEM_HOST)
+        for (size_t i = 0; i < nframes; i++)
+            CU(c, cudaMemcpy(output + frames[i].dst_off, d_out + frames[i].dst_off, results[i].dst_size, cudaMemcpyDeviceToHost));
+    r.profiled = prof;
+    if (prof)
+        for (int st = 0; st < kCompressStages; st++) CU(c, cudaEventElapsedTime(&r.stage_ms[st], r.ev[st], r.ev[st + 1]));
+    return 0;
 }

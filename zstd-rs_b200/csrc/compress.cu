@@ -1,0 +1,250 @@
+// compress.cu -- sm_90a kernels of the batch compressor (ruzstd's encoding::compress at CompressionLevel::Fastest).
+//
+//   k_cmatch    : one CTA per 128 KiB block: greedy LZ77 parse into literals + sequences (two-table parallel parse)
+//   k_cenc      : one warp per block: Huffman literals, FSE sequences, the Raw / RLE / Compressed decision (encode.cuh)
+//   k_cxxh64    : content checksum of every frame's input (xxh64.cuh; four serial chains per frame)
+//   k_cassemble : one CTA per block: frame header, the block at its prefix-summed offset, the checksum, per-frame results
+//
+// Every block is encoded from its own literals and sequences only (no Repeat / Treeless modes, no repeat offsets), so all
+// blocks of all frames -- including the blocks of one huge frame -- run at the same time.  Matches may still reach back into
+// the previous block: the input is all there from the start.
+#include <cuda_runtime.h>
+#include <limits.h>
+#include <stdint.h>
+
+#include "compress.h"
+#include "encode.cuh"
+#include "xxh64.cuh"
+
+namespace b200z {
+
+constexpr uint32_t CM_THREADS = CM_WARPS * 32;
+constexpr uint32_t CM_T1_LOG = 14;   // block-wide first-occurrence table
+constexpr uint32_t CM_TP_LOG = 12;   // per-warp most-recent table
+constexpr uint32_t CM_SEED = 16384;  // bytes before its segment a warp's private table starts from
+constexpr uint32_t CM_CAP = 16;      // match bytes a lane verifies before the warp extends the chosen match together
+constexpr uint32_t CM_SMEM = (4u << CM_T1_LOG) + CM_WARPS * (4u << CM_TP_LOG);
+constexpr uint32_t CE_WARPS = 4;
+
+__device__ __forceinline__ uint64_t load5(const uint8_t *p) {
+    return (uint64_t)__ldg(p) | ((uint64_t)__ldg(p + 1) << 8) | ((uint64_t)__ldg(p + 2) << 16) | ((uint64_t)__ldg(p + 3) << 24) |
+           ((uint64_t)__ldg(p + 4) << 32);
+}
+__device__ __forceinline__ uint32_t hash5(const uint8_t *p, uint32_t log) { return (uint32_t)(((load5(p) << 24) * 889523592379ull) >> (64 - log)); }
+__device__ __forceinline__ uint32_t match_len(const uint8_t *a, const uint8_t *b, uint32_t lim) {
+    uint32_t n = 0;
+    while (n < lim && __ldg(a + n) == __ldg(b + n)) n++;
+    return n;
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// k_cmatch.  The CTA first builds a first-occurrence table of the block (5-byte hash -> smallest position, shared-memory
+// atomicMin: deterministic).  Warp w then parses segment w of the block greedily, 32 positions at a time: every lane looks
+// its position up in the first-occurrence table and in the warp's private most-recent table (seeded with the CM_SEED bytes
+// before the segment, which may lie in the previous block), keeps the longer verified candidate (candidate < position, offset
+// <= 128 KiB, inside the frame), and the first lane with a match of >= 5 bytes wins.  A match never crosses its segment's end.
+// Sequences and literals go to per-segment staging; the CTA then packs them, the trailing literals of a segment joining the
+// first sequence after them.
+// ------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(CM_THREADS, 1)
+k_cmatch(const CBlock *__restrict__ blocks, const uint8_t *__restrict__ input, uint8_t *__restrict__ lit_stage, SeqRec *__restrict__ seq_stage,
+         uint8_t *__restrict__ lits, SeqRec *__restrict__ seqs, CBlockInfo *__restrict__ info) {
+    extern __shared__ __align__(16) uint8_t smem_cm[];
+    uint32_t *t1 = reinterpret_cast<uint32_t *>(smem_cm);
+    int32_t *tp_all = reinterpret_cast<int32_t *>(smem_cm + (4u << CM_T1_LOG));
+    __shared__ uint32_t s_nseq[CM_WARPS], s_nlit[CM_WARPS], s_trail[CM_WARPS], s_add[CM_WARPS], s_soff[CM_WARPS], s_loff[CM_WARPS];
+    const uint32_t b = blockIdx.x, tid = threadIdx.x, w = tid >> 5, lane = tid & 31;
+    const CBlock blk = blocks[b];
+    const uint8_t *src = input + blk.src_off;
+    const uint32_t n = blk.size;
+    bool same = true;
+    for (uint32_t i = tid; i < n; i += CM_THREADS) same &= __ldg(src + i) == __ldg(src);
+    same = __syncthreads_and(same);
+    if (n == 0 || same) {
+        if (tid == 0) info[b] = CBlockInfo{n, 0, n ? 1u : 0u, 0};
+        return;
+    }
+    for (uint32_t i = tid; i < (1u << CM_T1_LOG); i += CM_THREADS) t1[i] = 0xffffffffu;
+    for (uint32_t i = tid; i < CM_WARPS << CM_TP_LOG; i += CM_THREADS) tp_all[i] = INT_MIN;
+    __syncthreads();
+    for (uint32_t q = tid; q + ENC_MIN_MATCH <= n; q += CM_THREADS) atomicMin(&t1[hash5(src + q, CM_T1_LOG)], q);
+    int32_t *tp = tp_all + (w << CM_TP_LOG);
+    const uint32_t seglen = (n + CM_WARPS - 1) / CM_WARPS;
+    const uint32_t s = min(n, w * seglen), e = min(n, s + seglen);
+    const int32_t seed_lo = max((int32_t)s - (int32_t)CM_SEED, -(int32_t)min(blk.back, CM_SEED));
+    for (int32_t q = seed_lo + (int32_t)lane; q < (int32_t)s && q + (int32_t)ENC_MIN_MATCH <= (int32_t)n; q += 32)   // inside the frame
+        atomicMax(&tp[hash5(src + q, CM_TP_LOG)], q);
+    __syncthreads();
+    SeqRec *stage = seq_stage + ((size_t)b * CM_WARPS + w) * CSEG_SEQS;
+    uint8_t *lstage = lit_stage + (size_t)b * ENC_BLOCK + s;
+    uint32_t p = s, anchor = s, nseq = 0, nlit = 0;
+    while (p + ENC_MIN_MATCH <= e) {
+        const uint32_t q = p + lane;
+        const bool valid = q + ENC_MIN_MATCH <= e;
+        uint32_t len = 0, cand = 0, h2 = 0;
+        if (valid) {
+            const uint32_t lim = min(CM_CAP, e - q);
+            const uint32_t c1 = t1[hash5(src + q, CM_T1_LOG)];
+            h2 = hash5(src + q, CM_TP_LOG);
+            const int32_t c2 = tp[h2];
+            if (c1 < q) { len = match_len(src + q, src + c1, lim); cand = q - c1; }
+            if (c2 != INT_MIN && c2 < (int32_t)q && (int32_t)q - c2 <= (int32_t)ENC_WINDOW) {
+                const uint32_t l2 = match_len(src + q, src + c2, lim);
+                if (l2 > len || (l2 == len && (uint32_t)((int32_t)q - c2) < cand)) { len = l2; cand = (uint32_t)((int32_t)q - c2); }
+            }
+        }
+        __syncwarp();
+        if (valid) atomicMax(&tp[h2], (int32_t)q);
+        const uint32_t m = __ballot_sync(0xffffffffu, len >= ENC_MIN_MATCH);
+        if (!m) { p += 32; __syncwarp(); continue; }
+        const uint32_t j = __ffs(m) - 1;
+        const uint32_t qj = p + j, off = __shfl_sync(0xffffffffu, cand, j);
+        uint32_t ml = __shfl_sync(0xffffffffu, len, j);
+        if (ml == CM_CAP) {   // extend the chosen match 32 bytes at a time
+            const uint32_t lim = e - qj;
+            while (ml < lim) {
+                const uint32_t i = ml + lane;
+                const bool stop = i >= lim || __ldg(src + qj + i) != __ldg(src + qj + i - off);
+                const uint32_t sm = __ballot_sync(0xffffffffu, stop);
+                if (sm) { ml += __ffs(sm) - 1; break; }
+                ml += 32;
+            }
+            ml = min(ml, lim);
+        }
+        for (uint32_t i = anchor + lane; i < qj; i += 32) lstage[nlit + i - anchor] = __ldg(src + i);
+        if (lane == 0) stage[nseq] = SeqRec{qj - anchor, ml, off};
+        nlit += qj - anchor;
+        nseq++;
+        anchor = p = qj + ml;
+        __syncwarp();
+    }
+    for (uint32_t i = anchor + lane; i < e; i += 32) lstage[nlit + i - anchor] = __ldg(src + i);
+    if (lane == 0) { s_nseq[w] = nseq; s_nlit[w] = nlit + (e - anchor); s_trail[w] = e - anchor; }
+    __syncthreads();
+    if (tid == 0) {
+        uint32_t carry = 0, so = 0, lo = 0;
+        for (uint32_t v = 0; v < CM_WARPS; v++) {
+            s_soff[v] = so; s_loff[v] = lo;
+            so += s_nseq[v]; lo += s_nlit[v];
+            if (s_nseq[v]) { s_add[v] = carry; carry = s_trail[v]; }
+            else { s_add[v] = 0; carry += s_trail[v]; }
+        }
+        info[b] = CBlockInfo{lo, so, 0, 0};
+    }
+    __syncthreads();
+    SeqRec *out = seqs + (size_t)b * CBLOCK_SEQS + s_soff[w];
+    for (uint32_t i = lane; i < s_nseq[w]; i += 32) {
+        SeqRec r = stage[i];
+        if (i == 0) r.ll += s_add[w];
+        out[i] = r;
+    }
+    uint8_t *lo = lits + (size_t)b * ENC_BLOCK + s_loff[w];
+    for (uint32_t i = lane; i < s_nlit[w]; i += 32) lo[i] = lstage[i];
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// k_cenc: one warp per block encodes its literals and sequences (encode_block) into the block's staging slot and decides the
+// block type: RLE when all bytes are equal, Compressed when smaller than the input block, else Raw.
+// ------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(CE_WARPS * 32)
+k_cenc(const CBlock *__restrict__ blocks, uint32_t nblocks, const CBlockInfo *__restrict__ info, const uint8_t *__restrict__ lits,
+       const SeqRec *__restrict__ seqs, uint8_t *__restrict__ enc, CBlockInfo *__restrict__ res) {
+    __shared__ EncScratch scratch[CE_WARPS];
+    const uint32_t w = threadIdx.x >> 5, lane = threadIdx.x & 31, b = blockIdx.x * CE_WARPS + w;
+    if (b >= nblocks) return;
+    const CBlockInfo in = info[b];
+    const uint32_t n = blocks[b].size;
+    uint32_t type = 0, csize = n;
+    if (in.type == 1) { type = 1; csize = 1; }
+    else if (n) {
+        const uint32_t size = encode_block(scratch[w], lits + (size_t)b * ENC_BLOCK, in.nlit, seqs + (size_t)b * CBLOCK_SEQS, in.nseq,
+                                           enc + (size_t)b * ENC_BLOCK, ENC_BLOCK, lane, 32);
+        if (size < n) { type = 2; csize = size; }
+    }
+    if (lane == 0) res[b] = CBlockInfo{in.nlit, in.nseq, type, csize};
+}
+
+__global__ void k_cxxh64(const CFrame *__restrict__ frames, const uint8_t *__restrict__ input, uint64_t *__restrict__ csum, uint32_t nframes) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t f = t >> 2, k = t & 3;
+    if (f >= nframes) return;
+    const uint64_t h = xxh64_group(input + frames[f].src_off, frames[f].src_size, k);
+    if (k == 0) csum[f] = h;
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// k_cassemble: one CTA per block.  Its offset inside the frame is the sum of the sizes of the blocks before it (read by the
+// whole CTA); the first block also writes the frame header, the last one the checksum and the frame's result.
+// ------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+k_cassemble(const CFrame *__restrict__ frames, const CBlock *__restrict__ blocks, const CBlockInfo *__restrict__ res, const uint8_t *__restrict__ enc,
+            const uint8_t *__restrict__ input, const uint64_t *__restrict__ csum, uint8_t *__restrict__ output, b200z_compress_result *__restrict__ results,
+            int level, int checksum) {
+    __shared__ uint64_t s_red[3][8];
+    const uint32_t b = blockIdx.x, tid = threadIdx.x;
+    const CBlock blk = blocks[b];
+    const CFrame fr = frames[blk.frame];
+    const bool last = b == fr.first_block + fr.nblocks - 1;
+    uint64_t before = 0, nraw = 0, nrle = 0;
+    for (uint32_t i = fr.first_block + tid; i < b + (last ? 1u : 0u); i += 256) {
+        const uint32_t t = level == 0 ? 0u : res[i].type;
+        const uint32_t sz = 3 + (t == 0 ? blocks[i].size : t == 1 ? 1u : res[i].csize);
+        if (i < b) before += sz;
+        nraw += t == 0;
+        nrle += t == 1;
+    }
+    for (int o = 16; o; o >>= 1) {
+        before += __shfl_xor_sync(0xffffffffu, before, o);
+        nraw += __shfl_xor_sync(0xffffffffu, nraw, o);
+        nrle += __shfl_xor_sync(0xffffffffu, nrle, o);
+    }
+    if ((tid & 31) == 0) { s_red[0][tid >> 5] = before; s_red[1][tid >> 5] = nraw; s_red[2][tid >> 5] = nrle; }
+    __syncthreads();
+    before = nraw = nrle = 0;
+    for (int i = 0; i < 8; i++) { before += s_red[0][i]; nraw += s_red[1][i]; nrle += s_red[2][i]; }
+    const uint32_t hdr = frame_header_size(fr.src_size);
+    uint8_t *dst = output + fr.dst_off + hdr + before;
+    const uint32_t type = level == 0 ? 0u : res[b].type;
+    const uint32_t csize = type == 0 ? blk.size : type == 1 ? 1u : res[b].csize;
+    const uint8_t *from = type == 2 ? enc + (size_t)b * ENC_BLOCK : input + blk.src_off;
+    if (tid == 0) {
+        const uint32_t bh = (last ? 1u : 0u) | (type << 1) | ((type == 1 ? blk.size : csize) << 3);
+        dst[0] = (uint8_t)bh; dst[1] = (uint8_t)(bh >> 8); dst[2] = (uint8_t)(bh >> 16);
+        if (b == fr.first_block) write_frame_header(output + fr.dst_off, fr.src_size, checksum != 0);
+    }
+    for (uint32_t i = tid; i < csize; i += 256) dst[3 + i] = from[i];
+    if (last && tid == 0) {
+        const uint32_t c = checksum ? (uint32_t)csum[blk.frame] : 0u;
+        uint64_t size = hdr + before + 3 + csize;
+        if (checksum) { for (int i = 0; i < 4; i++) dst[3 + csize + i] = (uint8_t)(c >> (8 * i)); size += 4; }
+        b200z_compress_result r;
+        r.dst_size = size; r.status = 0; r.blocks = fr.nblocks; r.raw_blocks = (uint32_t)nraw; r.rle_blocks = (uint32_t)nrle;
+        r.has_checksum = checksum ? 1u : 0u; r.checksum = c;
+        results[blk.frame] = r;
+    }
+}
+
+static uint32_t cdiv_u(uint64_t a, uint32_t b) { return (uint32_t)((a + b - 1) / b); }
+
+int init_compress_kernels() {
+    return (int)cudaFuncSetAttribute(k_cmatch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CM_SMEM);
+}
+
+const char *const kCompressStageNames[kCompressStages] = {"k_cmatch", "k_cenc", "k_cxxh64", "k_cassemble"};
+
+int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s) {
+    switch (stage) {
+    case 0: if (a.level && a.nblocks) k_cmatch<<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info); break;
+    case 1: if (a.level && a.nblocks) k_cenc<<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res); break;
+    case 2: if (a.checksum && a.nframes) k_cxxh64<<<cdiv_u((uint64_t)a.nframes * 4, 128), 128, 0, s>>>(a.frames, a.input, a.csum, a.nframes); break;
+    case 3: if (a.nblocks) k_cassemble<<<a.nblocks, 256, 0, s>>>(a.frames, a.blocks, a.res, a.enc, a.input, a.csum, a.output, a.results, a.level, a.checksum); break;
+    default: return (int)cudaErrorInvalidValue;
+    }
+    return (int)cudaGetLastError();
+}
+
+uint32_t compress_launch_count(const CompressArgs &a) {
+    return (a.level ? 2u : 0u) + (a.checksum ? 1u : 0u) + 1u;
+}
+
+}  // namespace b200z
