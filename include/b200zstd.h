@@ -247,7 +247,8 @@ int b200z_batch_run_timeline(b200z_batch *b, uint8_t *d_output, size_t output_ca
 int b200z_num_stages(void);
 const char *b200z_stage_kernel_name(int stage);
 /* facts about a prepared batch: [0] frames [1] blocks [2] compressed blocks [3] input bytes planned
- * [4] literal-scratch bytes [5] sequences [6] kernel launches per run */
+ * [4] literal-scratch bytes [5] sequences [6] kernels the most recent b200z_batch_run launched, k_xxh64 included (0 before the
+ * first run) */
 int b200z_batch_info(const b200z_batch *b, uint64_t out[8]);
 /* per-stage device pointers for kernel-level parity tests (tests/ only): literals scratch and sequence
  * scratch of the LAST run, laid out exactly as the oracle's trace (oracle/ruzstd_oracle.h zo_block_trace) */

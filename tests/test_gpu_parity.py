@@ -124,6 +124,39 @@ def test_gpu_checksum_stage(pkg, manifest):
     c2.close()
 
 
+def test_kernel_launch_counts(pkg, monkeypatch):
+    """ctx.kernel_launches() counts the kernels each path really launched, on single-block frames.  The warp kernel takes every
+    frame: k_exec_cta would add its own launches."""
+    import torch
+    import datagen as G
+    monkeypatch.setenv("B200Z_EXEC_MODE", "warp")
+    plains = [G.gen_text(20000, 70 + i).tobytes() for i in range(8)]
+    frames = [G.compress(p_) for p_ in plains]
+    c2 = pkg.Context(0)
+    dec = pkg.FrameDecoder(c2)
+    r = dec.reset(frames[0])
+    n0 = c2.kernel_launches()
+    assert dec.decode_blocks(r, pkg.ALL) is True
+    assert c2.kernel_launches() - n0 == 4   # k_setup, k_huf, k_fse; then k_exec once the output has grown
+    assert dec.collect() == plains[0]
+    del dec
+    io, comp, total = _io(pkg, frames, [len(p_) for p_ in plains])
+    d_out = torch.zeros(total + 64, dtype=torch.uint8, device="cuda")
+    b = pkg.Batch(c2, comp, io)
+    assert b.info()["compressed_blocks"] == len(frames) and b.info()["launches_per_run"] == 0
+    n0 = c2.kernel_launches()
+    b.run_profile(d_out)
+    assert c2.kernel_launches() - n0 == 4   # k_setup, k_huf, k_fse, k_exec, one after the other
+    c2.set_flags(pkg.binding.FLAG_CHECKSUM)
+    n0 = c2.kernel_launches()
+    b.run(d_out)
+    assert c2.kernel_launches() - n0 == b.info()["launches_per_run"] == 6   # two k_setup halves, k_huf, k_fse, k_exec, k_xxh64
+    res = b.finish()
+    assert (res["status"] == 0).all() and (res["has_calculated_checksum"] == 1).all()
+    b.close()
+    c2.close()
+
+
 def test_dict_corpus(pkg, ctx, manifest):
     """tests/dict_test.rs:77-262 via the mirror, then all 207 frames in one batch."""
     dic = read_golden("dict_tests", "dictionary")

@@ -433,6 +433,7 @@ class Batch:
         return res
 
     def info(self):
+        """Facts about the plan; launches_per_run is the kernels the most recent run() launched (0 before it)."""
         a = (C.c_uint64 * 8)()
         self.ctx.L.b200z_batch_info(self.h, a)
         k = ["frames", "blocks", "compressed_blocks", "planned_bytes", "literal_scratch_bytes", "sequences", "launches_per_run"]

@@ -122,9 +122,8 @@ extern "C" int b200z_ctx_create(int device, b200z_ctx **out) {
         cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming) != cudaSuccess) { cudaGetLastError(); return B200Z_ERR_CUDA; }
     if (cudaMalloc((void **)&c->d_predef, sizeof(FseSlot)) != cudaSuccess) { cudaGetLastError(); return B200Z_ERR_OUT_OF_MEMORY; }
     if (init_kernels() || init_compress_kernels()) { cudaGetLastError(); return B200Z_ERR_CUDA; }
-    int e = launch_predefined(c->d_predef, c->stream);
+    int e = launch_predefined(c->d_predef, c->stream, &c->launches);
     if (e || cudaStreamSynchronize(c->stream) != cudaSuccess) { cudaGetLastError(); return B200Z_ERR_CUDA; }
-    c->launches = 1;
     *out = c.release();
     return 0;
 }
@@ -242,7 +241,26 @@ extern "C" void b200z_dict_destroy(b200z_dict *d) { dict_free(d); }
 // ---------------------------------------------------------------------------------------------------------------
 namespace {
 
-struct CarrySet { const HufSlot *huf = nullptr; const FseTab *ll = nullptr, *of = nullptr, *ml = nullptr; };
+struct CarrySet {
+    const HufSlot *huf = nullptr;
+    const FseTab *ll = nullptr, *of = nullptr, *ml = nullptr;
+    const b200z_dict *dict = nullptr;   // the dictionary these tables belong to (null: the frame decoder's carried tables)
+};
+
+// initial cursor of a frame: fresh, or the dictionary's tables (scratch.rs:70-78)
+void cursor_from_carry(TableCursor &cur, const CarrySet &cs, uint32_t carry_idx) {
+    cur = TableCursor();
+    if (cs.huf) { cur.huf.kind = TabRef::CARRY; cur.huf.idx = carry_idx; }
+    if (cs.ll) { cur.ll.kind = TabRef::CARRY; cur.ll.idx = carry_idx; }
+    if (cs.of) { cur.of.kind = TabRef::CARRY; cur.of.idx = carry_idx; }
+    if (cs.ml) { cur.ml.kind = TabRef::CARRY; cur.ml.idx = carry_idx; }
+}
+CarrySet carry_of_dict(const b200z_dict *d) {
+    CarrySet cs;
+    cs.dict = d;
+    if (d && d->has_tables) { cs.huf = d->d_huf; cs.ll = &d->d_fse->ll; cs.of = &d->d_fse->of; cs.ml = &d->d_fse->ml; }
+    return cs;
+}
 
 struct Submission {
     std::vector<BlockDesc> descs;
@@ -260,6 +278,47 @@ struct Submission {
     void clear() {
         descs.clear(); refs.clear(); frames.clear(); states.clear(); carries.clear();
         n_huf = n_fse = 0; lit_bytes = 0; nseq = 0;
+    }
+    // TabRef::CARRY index of a dictionary's tables, added on first use; -1 for no dictionary
+    int carry_index(const b200z_dict *dict) {
+        if (!dict) return -1;
+        for (size_t i = 0; i < carries.size(); i++) if (carries[i].dict == dict) return (int)i;
+        carries.push_back(carry_of_dict(dict));
+        return (int)carries.size() - 1;
+    }
+    // Appends a frame whose blocks follow (the caller sets its nblocks), starting from the dictionary's offset history or {1, 4, 8}.
+    // Returns the table cursor of its first block: the dictionary's tables, if any.
+    TableCursor add_frame(const b200z_dict *dict, uint64_t out_off, uint64_t out_cap, uint64_t window) {
+        static const uint32_t fresh_hist[3] = {1, 4, 8};
+        FrameDesc fd;
+        memset(&fd, 0, sizeof fd);
+        fd.out_off = out_off; fd.out_cap = out_cap; fd.window_size = window;
+        fd.dict = dict ? dict->d_content : nullptr; fd.dict_len = dict ? dict->content_len : 0;
+        fd.first_block = (uint32_t)descs.size();
+        FrameState st;
+        memset(&st, 0, sizeof st);
+        memcpy(st.hist, dict ? dict->hist : fresh_hist, sizeof st.hist);
+        frames.push_back(fd); states.push_back(st);
+        TableCursor cur;
+        const int ci = carry_index(dict);
+        if (ci >= 0) cursor_from_carry(cur, carries[ci], (uint32_t)ci);
+        return cur;
+    }
+    // Appends a block.  A Compressed block is planned from its content, or from the section headers k_walk brought back (`view`);
+    // `cur` moves on to the tables it leaves current.
+    const BlockDesc &add_block(uint64_t src_off, const BlockHeader &bh, uint32_t frame, uint32_t block_in_frame, const uint8_t *content,
+                               const WalkBlock *view, TableCursor &cur) {
+        BlockDesc d;
+        memset(&d, 0, sizeof d);
+        BlockRefs r;
+        d.src_off = src_off; d.src_size = bh.content_size; d.frame = frame; d.btype = bh.type; d.raw_size = bh.decompressed_size;
+        d.block_in_frame = block_in_frame; d.last = bh.last;
+        if (bh.type == BT_COMPRESSED) {
+            if (view) plan_compressed_block_view(view->lit, view->seq, bh.content_size, d, r, cur, n_huf, n_fse, lit_bytes, nseq);
+            else plan_compressed_block(content, bh.content_size, d, r, cur, n_huf, n_fse, lit_bytes, nseq);
+        }
+        descs.push_back(d); refs.push_back(r);
+        return descs.back();
     }
     // resolve table references to device pointers and upload descriptors
     int upload(b200z_ctx *c, cudaStream_t stream = nullptr) {
@@ -360,20 +419,6 @@ struct Submission {
     }
 };
 
-// initial cursor of a frame: fresh, or the dictionary's tables (scratch.rs:70-78)
-void cursor_from_carry(TableCursor &cur, const CarrySet &cs, uint32_t carry_idx) {
-    cur = TableCursor();
-    if (cs.huf) { cur.huf.kind = TabRef::CARRY; cur.huf.idx = carry_idx; }
-    if (cs.ll) { cur.ll.kind = TabRef::CARRY; cur.ll.idx = carry_idx; }
-    if (cs.of) { cur.of.kind = TabRef::CARRY; cur.of.idx = carry_idx; }
-    if (cs.ml) { cur.ml.kind = TabRef::CARRY; cur.ml.idx = carry_idx; }
-}
-CarrySet carry_of_dict(const b200z_dict *d) {
-    CarrySet cs;
-    if (d && d->has_tables) { cs.huf = d->d_huf; cs.ll = &d->d_fse->ll; cs.of = &d->d_fse->of; cs.ml = &d->d_fse->ml; }
-    return cs;
-}
-
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -402,6 +447,7 @@ struct b200z_batch {
     size_t input_len = 0;
     bool ran = false;
     bool checksummed = false;
+    uint64_t run_launches = 0;               // kernels the most recent b200z_batch_run launched
 };
 
 // what k_walk brought back for a batch whose input lives in device memory (the planner then never sees the compressed bytes)
@@ -415,15 +461,6 @@ static int plan_batch(b200z_batch *b, const uint8_t *in, size_t in_len, const b2
     b->block_end_bytes.clear();
     if (max_window == 0) max_window = B200Z_DEFAULT_MAX_WINDOW_SIZE;
     max_window = std::min<uint64_t>(max_window, (1ull << 41) + 7 * (1ull << 38));
-    // carry sets: one per dictionary (+ forced)
-    std::vector<const b200z_dict *> dlist(dicts, dicts + ndicts);
-    int forced_idx = -1;
-    if (forced) {
-        auto it = std::find(dlist.begin(), dlist.end(), forced);
-        if (it == dlist.end()) { dlist.push_back(forced); forced_idx = (int)dlist.size() - 1; } else forced_idx = (int)(it - dlist.begin());
-    }
-    for (auto *d : dlist) s.carries.push_back(carry_of_dict(d));
-
     for (size_t i = 0; i < nframes; i++) {
         FramePlanInfo &fi = b->info[i];
         const b200z_frame_io &io = frames[i];
@@ -437,24 +474,16 @@ static int plan_batch(b200z_batch *b, const uint8_t *in, size_t in_len, const b2
         if (e) { fi.pre_status = e; fi.pre_stage = B200Z_STAGE_FRAME_HEADER; fi.bytes_read_full = consumed; continue; }
         if ((e = frame_window_size(fi.hdr, fi.window))) { fi.pre_status = e; fi.pre_stage = B200Z_STAGE_FRAME_HEADER; continue; }
         if (fi.window > max_window) { fi.pre_status = B200Z_ERR_WINDOW_SIZE_TOO_BIG; fi.pre_stage = B200Z_STAGE_FRAME_HEADER; continue; }
-        int dict_idx = -1;
+        const b200z_dict *dict = nullptr;
         if (fi.hdr.has_dict_id) {
-            for (size_t k = 0; k < dlist.size() && k < ndicts; k++) if (dlist[k]->id == fi.hdr.dict_id) dict_idx = (int)k;
-            if (dict_idx < 0) { fi.pre_status = B200Z_ERR_DICT_NOT_PROVIDED; fi.pre_stage = B200Z_STAGE_FRAME_HEADER; continue; }
+            for (size_t k = 0; k < ndicts; k++) if (dicts[k]->id == fi.hdr.dict_id) dict = dicts[k];
+            if (!dict) { fi.pre_status = B200Z_ERR_DICT_NOT_PROVIDED; fi.pre_stage = B200Z_STAGE_FRAME_HEADER; continue; }
         }
-        if (forced_idx >= 0) dict_idx = forced_idx;
-        const b200z_dict *dict = dict_idx >= 0 ? dlist[dict_idx] : nullptr;
+        if (forced) dict = forced;
 
-        FrameDesc fd;
-        memset(&fd, 0, sizeof fd);
-        fd.out_off = io.out_off; fd.out_cap = io.out_cap; fd.window_size = fi.window;
-        fd.dict = dict ? dict->d_content : nullptr; fd.dict_len = dict ? dict->content_len : 0;
-        fd.first_block = (uint32_t)s.descs.size();
-        FrameState st;
-        memset(&st, 0, sizeof st);
-        st.hist[0] = dict ? dict->hist[0] : 1; st.hist[1] = dict ? dict->hist[1] : 4; st.hist[2] = dict ? dict->hist[2] : 8;
-        TableCursor cur;
-        if (dict_idx >= 0) cursor_from_carry(cur, s.carries[dict_idx], (uint32_t)dict_idx);
+        fi.sub_frame = (int32_t)s.frames.size();
+        TableCursor cur = s.add_frame(dict, io.out_off, io.out_cap, fi.window);
+        FrameDesc &fd = s.frames.back();
         fi.first_block_end = b->block_end_bytes.size();
 
         uint64_t pos = consumed, bytes_read = consumed;
@@ -473,18 +502,9 @@ static int plan_batch(b200z_batch *b, const uint8_t *in, size_t in_len, const b2
                 fd.host_status = mk_status(bh.type == BT_COMPRESSED ? B200Z_ERR_BLOCK_CONTENT_READ : B200Z_ERR_BLOCK_BODY_READ, B200Z_STAGE_BLOCK_BODY);
                 break;
             }
-            BlockDesc d;
-            memset(&d, 0, sizeof d);
-            BlockRefs r;
-            d.src_off = io.src_off + pos; d.src_size = bh.content_size; d.frame = (uint32_t)s.frames.size();
-            d.btype = bh.type; d.raw_size = bh.decompressed_size; d.block_in_frame = bif++; d.last = bh.last;
-            if (bh.type == BT_COMPRESSED) {
-                if (wbk) plan_compressed_block_view(wbk->lit, wbk->seq, bh.content_size, d, r, cur, s.n_huf, s.n_fse, s.lit_bytes, s.nseq);
-                else plan_compressed_block(p + pos, bh.content_size, d, r, cur, s.n_huf, s.n_fse, s.lit_bytes, s.nseq);
-            }
+            const BlockDesc &d = s.add_block(io.src_off + pos, bh, (uint32_t)fi.sub_frame, bif++, wbk ? nullptr : p + pos, wbk, cur);
             pos += bh.content_size;
             bytes_read += 3 + bh.content_size;
-            s.descs.push_back(d); s.refs.push_back(r);
             b->block_end_bytes.push_back(bytes_read);
             if (d.host_status) break;  // the reference stops here; later blocks are never looked at
             if (bh.last) {
@@ -501,8 +521,6 @@ static int plan_batch(b200z_batch *b, const uint8_t *in, size_t in_len, const b2
         }
         fd.nblocks = (uint32_t)s.descs.size() - fd.first_block;
         fi.bytes_read_full = bytes_read;
-        fi.sub_frame = (int32_t)s.frames.size();
-        s.frames.push_back(fd); s.states.push_back(st);
     }
     return 0;
 }
@@ -519,23 +537,21 @@ static int device_walk(b200z_ctx *c, const uint8_t *d_input, size_t input_len, c
     if (int e = d_first.ensure(nframes * 4, false)) return e;
     CU(c, cudaMemcpyAsync(d_io.p, so.data(), so.size() * 8, cudaMemcpyHostToDevice, c->stream));
     const uint64_t *d_off = d_io.as<uint64_t>(), *d_sz = d_off + nframes;
-    int le = launch_walk(d_input, input_len, d_off, d_sz, (uint32_t)nframes, d_wf.as<WalkFrame>(), nullptr, nullptr, 0, c->stream);
+    int le = launch_walk(d_input, input_len, d_off, d_sz, (uint32_t)nframes, d_wf.as<WalkFrame>(), nullptr, nullptr, 0, c->stream, &c->launches);
     if (le) return c->set_cuda_err((cudaError_t)le, "k_walk");
     CU(c, cudaMemcpyAsync(w.wf.data(), d_wf.p, nframes * sizeof(WalkFrame), cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     uint64_t total = 0;
     for (size_t i = 0; i < nframes; i++) { w.first[i] = (uint32_t)total; total += w.wf[i].nblocks; }
     if (total > 0xFFFFFFF0ull) return B200Z_ERR_INVALID_ARGUMENT;
-    c->launches += 1;
     if (!total) return 0;
     w.wb.resize(total);
     if (int e = d_wb.ensure(total * sizeof(WalkBlock), false)) return e;
     CU(c, cudaMemcpyAsync(d_first.p, w.first.data(), nframes * 4, cudaMemcpyHostToDevice, c->stream));
-    le = launch_walk(d_input, input_len, d_off, d_sz, (uint32_t)nframes, d_wf.as<WalkFrame>(), d_first.as<uint32_t>(), d_wb.as<WalkBlock>(), 1, c->stream);
+    le = launch_walk(d_input, input_len, d_off, d_sz, (uint32_t)nframes, d_wf.as<WalkFrame>(), d_first.as<uint32_t>(), d_wb.as<WalkBlock>(), 1, c->stream, &c->launches);
     if (le) return c->set_cuda_err((cudaError_t)le, "k_walk");
     CU(c, cudaMemcpyAsync(w.wb.data(), d_wb.p, total * sizeof(WalkBlock), cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
-    c->launches += 1;
     return 0;
 }
 
@@ -580,24 +596,36 @@ extern "C" int b200z_batch_prepare(b200z_ctx *c, const uint8_t *input, size_t in
     return 0;
 }
 
+// One decode pass in the shipped overlapped order (launch_pipeline_overlapped), then, if `checksummed` is not null and the context has
+// B200Z_FLAG_CHECKSUM, k_xxh64 of every frame; *checksummed says whether it ran.  Adds the kernels launched to *launched.
+static int enqueue_pass(b200z_ctx *c, const PipelineArgs &a, const PipelineStreams &ps, bool *checksummed, uint64_t *launched) {
+    if (int e = launch_pipeline_overlapped(a, ps, launched)) return c->set_cuda_err((cudaError_t)e, "launch_pipeline");
+    if (!checksummed) return 0;
+    *checksummed = (c->flags & B200Z_FLAG_CHECKSUM) && a.nframes;
+    if (*checksummed)
+        if (int e = launch_checksum(a, ps.main, launched)) return c->set_cuda_err((cudaError_t)e, "launch_checksum");
+    return 0;
+}
+
+// every pass starts from the frame states b200z_batch_prepare planned
+static int restore_states(b200z_batch *b) {
+    b200z_ctx *c = b->ctx;
+    const Submission &s = b->sub;
+    if (!s.states.empty())
+        CU(c, cudaMemcpyAsync(s.d_states.p, b->d_states_init.p, s.states.size() * sizeof(FrameState), cudaMemcpyDeviceToDevice, c->stream));
+    return 0;
+}
+
 extern "C" int b200z_batch_run(b200z_batch *b, uint8_t *d_output, size_t output_cap) {
     if (!b) return B200Z_ERR_INVALID_ARGUMENT;
     b200z_ctx *c = b->ctx;
     if (int e = c->use()) return e;
-    Submission &s = b->sub;
-    if (!s.states.empty())
-        CU(c, cudaMemcpyAsync(s.d_states.p, b->d_states_init.p, s.states.size() * sizeof(FrameState), cudaMemcpyDeviceToDevice, c->stream));
-    PipelineArgs a = s.args(b->d_input, d_output, output_cap);
-    PipelineStreams ps{c->stream, c->side, c->ev_fork, c->ev_join};
-    int e = launch_pipeline_overlapped(a, ps);
-    if (e) return c->set_cuda_err((cudaError_t)e, "launch_pipeline");
-    c->launches += pipeline_launch_count(a);
-    b->checksummed = false;
-    if ((c->flags & B200Z_FLAG_CHECKSUM) && a.nframes) {
-        if ((e = launch_checksum(a, c->stream))) return c->set_cuda_err((cudaError_t)e, "launch_checksum");
-        c->launches += 1;
-        b->checksummed = true;
-    }
+    if (int e = restore_states(b)) return e;
+    PipelineArgs a = b->sub.args(b->d_input, d_output, output_cap);
+    b->run_launches = 0;
+    int e = enqueue_pass(c, a, PipelineStreams{c->stream, c->side, c->ev_fork, c->ev_join}, &b->checksummed, &b->run_launches);
+    c->launches += b->run_launches;
+    if (e) return e;
     b->ran = true;
     return 0;
 }
@@ -607,20 +635,17 @@ extern "C" int b200z_batch_run_profile(b200z_batch *b, uint8_t *d_output, size_t
     if (!b || !stage_ms) return B200Z_ERR_INVALID_ARGUMENT;
     b200z_ctx *c = b->ctx;
     if (int e = c->use()) return e;
-    Submission &s = b->sub;
-    if (!s.states.empty())
-        CU(c, cudaMemcpyAsync(s.d_states.p, b->d_states_init.p, s.states.size() * sizeof(FrameState), cudaMemcpyDeviceToDevice, c->stream));
-    PipelineArgs a = s.args(b->d_input, d_output, output_cap);
+    if (int e = restore_states(b)) return e;
+    PipelineArgs a = b->sub.args(b->d_input, d_output, output_cap);
     cudaEvent_t ev[kNumStages + 1];
     for (auto &e : ev) CU(c, cudaEventCreate(&e));
     if (int e = reset_sched(a, c->stream)) return c->set_cuda_err((cudaError_t)e, "reset_sched");
     CU(c, cudaEventRecord(ev[0], c->stream));
     for (int st = 0; st < kNumStages; st++) {
-        int e = launch_stage(a, st, c->stream);
+        int e = launch_stage(a, st, c->stream, &c->launches);
         if (e) return c->set_cuda_err((cudaError_t)e, "launch_stage");
         CU(c, cudaEventRecord(ev[st + 1], c->stream));
     }
-    c->launches += pipeline_launch_count(a);
     CU(c, cudaStreamSynchronize(c->stream));
     for (int st = 0; st < kNumStages && (size_t)st < nstages; st++) CU(c, cudaEventElapsedTime(&stage_ms[st], ev[st], ev[st + 1]));
     for (auto &e : ev) cudaEventDestroy(e);
@@ -634,10 +659,8 @@ extern "C" int b200z_batch_run_timeline(b200z_batch *b, uint8_t *d_output, size_
     if (!b || !out_ms || n < 4) return B200Z_ERR_INVALID_ARGUMENT;
     b200z_ctx *c = b->ctx;
     if (int e = c->use()) return e;
-    Submission &s = b->sub;
-    if (!s.states.empty())
-        CU(c, cudaMemcpyAsync(s.d_states.p, b->d_states_init.p, s.states.size() * sizeof(FrameState), cudaMemcpyDeviceToDevice, c->stream));
-    PipelineArgs a = s.args(b->d_input, d_output, output_cap);
+    if (int e = restore_states(b)) return e;
+    PipelineArgs a = b->sub.args(b->d_input, d_output, output_cap);
     if (int e = reset_sched(a, c->stream)) return c->set_cuda_err((cudaError_t)e, "reset_sched");
     cudaEvent_t ev[5];
     for (auto &e : ev) CU(c, cudaEventCreate(&e));
@@ -645,14 +668,13 @@ extern "C" int b200z_batch_run_timeline(b200z_batch *b, uint8_t *d_output, size_
     CU(c, cudaEventRecord(ev[0], c->stream));
     PipelineStreams ps{c->stream, c->side, c->ev_fork, c->ev_join};
     CU(c, cudaEventRecord(ev[1], c->stream));
-    int le = launch_tables_literals(a, ps);
+    int le = launch_tables_literals(a, ps, &c->launches);
     CU(c, cudaEventRecord(ev[2], c->stream));
-    if (!le) le = launch_fse_exec(a, c->stream);
+    if (!le) le = launch_fse_exec(a, c->stream, &c->launches);
     CU(c, cudaEventRecord(ev[3], c->stream));
-    if (!le) le = launch_cta_rest(a, c->stream);
+    if (!le) le = launch_cta_rest(a, c->stream, &c->launches);
     CU(c, cudaEventRecord(ev[4], c->stream));
     if (le) return c->set_cuda_err((cudaError_t)le, "launch_stage");
-    c->launches += pipeline_launch_count(a);
     CU(c, cudaStreamSynchronize(c->stream));
     for (int i = 0; i < 4; i++) CU(c, cudaEventElapsedTime(&out_ms[i], ev[0], ev[i + 1]));
     for (auto &e : ev) cudaEventDestroy(e);
@@ -726,7 +748,7 @@ extern "C" int b200z_batch_info(const b200z_batch *b, uint64_t out[8]) {
     uint64_t ncomp = 0, planned = 0;
     for (auto &d : s.descs) { ncomp += d.btype == BT_COMPRESSED; planned += d.src_size + 3; }
     out[0] = s.frames.size(); out[1] = s.descs.size(); out[2] = ncomp; out[3] = planned; out[4] = s.lit_bytes; out[5] = s.nseq;
-    out[6] = pipeline_launch_count(s.args(nullptr, nullptr, 0)); out[7] = 0;
+    out[6] = b->run_launches; out[7] = 0;
     return 0;
 }
 
@@ -915,16 +937,7 @@ static int decode_frames_pipelined(b200z_ctx *c, const uint8_t *input, size_t in
         cudaStream_t km = p->k_main[s];
         CU(c, cudaStreamWaitEvent(km, p->ev_h2d[s], 0));
         PipelineArgs a = b->sub.args(p->d_in[s].as<uint8_t>() - ilo, d_out, output_cap);
-        PipelineStreams ps{km, p->k_side[s], p->k_fork[s], p->k_join[s]};
-        int le = launch_pipeline_overlapped(a, ps);
-        if (le) return c->set_cuda_err((cudaError_t)le, "launch_pipeline");
-        c->launches += pipeline_launch_count(a);
-        b->checksummed = false;
-        if ((c->flags & B200Z_FLAG_CHECKSUM) && a.nframes) {
-            if ((le = launch_checksum(a, km))) return c->set_cuda_err((cudaError_t)le, "launch_checksum");
-            c->launches += 1;
-            b->checksummed = true;
-        }
+        if (int e = enqueue_pass(c, a, PipelineStreams{km, p->k_side[s], p->k_fork[s], p->k_join[s]}, &b->checksummed, &c->launches)) return e;
         CU(c, cudaEventRecord(p->ev_k[s], km));
         CU(c, cudaStreamWaitEvent(p->s_d2h, p->ev_k[s], 0));
         size_t nst = b->sub.states.size();
@@ -1004,50 +1017,29 @@ extern "C" int b200z_decode_blocks_batch(b200z_ctx *c, const b200z_block_desc *b
         hin = host_copy.data();
     }
     Submission s;
-    std::vector<const b200z_dict *> dlist;
     std::vector<int64_t> sub_of(nblocks, -1);      // caller's block index -> descriptor index in the submission
-    std::vector<uint32_t> frame_first(nframes, 0);
     for (size_t f = 0; f < nframes; f++) {
         const b200z_block_frame &bf = frames[f];
         if ((uint64_t)bf.first_block + bf.num_blocks > nblocks) return B200Z_ERR_INVALID_ARGUMENT;
-        int dict_idx = -1;
-        if (bf.dict) {
-            auto it = std::find(dlist.begin(), dlist.end(), bf.dict);
-            if (it == dlist.end()) { dlist.push_back(bf.dict); s.carries.push_back(carry_of_dict(bf.dict)); dict_idx = (int)dlist.size() - 1; }
-            else dict_idx = (int)(it - dlist.begin());
-        }
-        FrameDesc fd;
-        memset(&fd, 0, sizeof fd);
-        fd.out_off = bf.out_off; fd.out_cap = bf.out_cap; fd.window_size = bf.window_size;
-        fd.dict = bf.dict ? bf.dict->d_content : nullptr; fd.dict_len = bf.dict ? bf.dict->content_len : 0;
-        fd.first_block = (uint32_t)s.descs.size();
-        frame_first[f] = fd.first_block;
-        FrameState st;
-        memset(&st, 0, sizeof st);
-        st.hist[0] = bf.dict ? bf.dict->hist[0] : 1; st.hist[1] = bf.dict ? bf.dict->hist[1] : 4; st.hist[2] = bf.dict ? bf.dict->hist[2] : 8;
-        TableCursor cur;
-        if (dict_idx >= 0) cursor_from_carry(cur, s.carries[dict_idx], (uint32_t)dict_idx);
+        TableCursor cur = s.add_frame(bf.dict, bf.out_off, bf.out_cap, bf.window_size);
         for (uint32_t k = 0; k < bf.num_blocks; k++) {
             const b200z_block_desc &bd = blocks[bf.first_block + k];
             if (bd.block_type > BT_COMPRESSED || bd.src_off > compressed_len || bd.content_size > compressed_len - bd.src_off) return B200Z_ERR_INVALID_ARGUMENT;
-            BlockDesc d;
-            memset(&d, 0, sizeof d);
-            BlockRefs r;
-            d.src_off = bd.src_off; d.src_size = bd.content_size; d.frame = (uint32_t)f; d.btype = bd.block_type; d.raw_size = bd.decompressed_size;
-            d.block_in_frame = k; d.last = bd.last_block;
+            if (bd.block_type != BT_COMPRESSED && (bd.block_type == BT_RAW ? bd.content_size != bd.decompressed_size : bd.content_size != 1))
+                return B200Z_ERR_INVALID_ARGUMENT;
+            BlockHeader bh;
+            bh.last = bd.last_block; bh.type = bd.block_type; bh.decompressed_size = bd.decompressed_size; bh.content_size = bd.content_size;
+            sub_of[bf.first_block + k] = (int64_t)s.descs.size();
+            const BlockDesc &d = s.add_block(bd.src_off, bh, (uint32_t)f, k, hin + bd.src_off, nullptr, cur);
             if (bd.block_type == BT_COMPRESSED) {
-                plan_compressed_block(hin + bd.src_off, bd.content_size, d, r, cur, s.n_huf, s.n_fse, s.lit_bytes, s.nseq);
                 // the descriptor says what the caller's parsers found: it must be what the content says
                 const bool lit_seen = !(d.host_status && (d.host_status >> 24) == 1 && d.lit_type == 0 && d.regen_size == 0 && d.lit_off == 0);
                 if (lit_seen && (d.lit_type != bd.literals_type || d.regen_size != bd.regenerated_size)) return B200Z_ERR_INVALID_ARGUMENT;
                 if (!d.host_status && (d.nseq != bd.num_sequences || (d.nseq && d.modes != bd.modes))) return B200Z_ERR_INVALID_ARGUMENT;
-            } else if (bd.block_type == BT_RAW ? bd.content_size != bd.decompressed_size : bd.content_size != 1) return B200Z_ERR_INVALID_ARGUMENT;
-            sub_of[bf.first_block + k] = (int64_t)s.descs.size();
-            s.descs.push_back(d); s.refs.push_back(r);
+            }
             if (d.host_status) break;   // decompress_block would have returned here: later blocks of the frame are never reached
         }
-        fd.nblocks = (uint32_t)s.descs.size() - fd.first_block;
-        s.frames.push_back(fd); s.states.push_back(st);
+        s.frames.back().nblocks = (uint32_t)s.descs.size() - s.frames.back().first_block;
     }
     DevBuf d_in_own, d_out_own;
     const uint8_t *d_in = compressed;
@@ -1062,10 +1054,8 @@ extern "C" int b200z_decode_blocks_batch(b200z_ctx *c, const b200z_block_desc *b
         d_out = d_out_own.as<uint8_t>();
     }
     if (int e = s.upload(c)) return e;
-    PipelineArgs a = s.args(d_in, d_out, output_cap);
-    PipelineStreams ps{c->stream, c->side, c->ev_fork, c->ev_join};
-    if (int le = launch_pipeline_overlapped(a, ps)) return c->set_cuda_err((cudaError_t)le, "launch_pipeline");
-    c->launches += pipeline_launch_count(a);
+    if (int e = enqueue_pass(c, s.args(d_in, d_out, output_cap), PipelineStreams{c->stream, c->side, c->ev_fork, c->ev_join}, nullptr, &c->launches))
+        return e;
     std::vector<FrameState> st(s.states.size());
     std::vector<BlockAux> aux(s.descs.size());
     if (!st.empty()) CU(c, cudaMemcpyAsync(st.data(), s.d_states.p, st.size() * sizeof(FrameState), cudaMemcpyDeviceToHost, c->stream));
@@ -1312,9 +1302,8 @@ static int fd_submit(b200z_frame_decoder *d, const TableCursor &cur, uint32_t *f
     // stage A: tables + literals + sequences; sizes come back so the output can grow before execution
     PipelineArgs a = s.args(d->d_input.as<uint8_t>(), nullptr, 0);
     PipelineArgs a_dec = a; a_dec.nframes = 0;
-    int le = launch_pipeline(a_dec, c->stream);
+    int le = launch_pipeline(a_dec, c->stream, &c->launches);
     if (le) return c->set_cuda_err((cudaError_t)le, "launch decode");
-    c->launches += pipeline_launch_count(a_dec);
     std::vector<BlockAux> aux(s.descs.size());
     CU(c, cudaMemcpyAsync(aux.data(), s.d_aux.p, aux.size() * sizeof(BlockAux), cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
@@ -1329,9 +1318,8 @@ static int fd_submit(b200z_frame_decoder *d, const TableCursor &cur, uint32_t *f
     CU(c, cudaMemcpyAsync(s.d_frames.p, s.frames.data(), sizeof(FrameDesc), cudaMemcpyHostToDevice, c->stream));
     PipelineArgs a_ex = a; a_ex.nblocks = 0;
     a_ex.output = d->d_out.as<uint8_t>() - d->base; a_ex.output_cap = d->base + d->d_out.cap;
-    le = launch_pipeline(a_ex, c->stream);
+    le = launch_pipeline(a_ex, c->stream, &c->launches);
     if (le) return c->set_cuda_err((cudaError_t)le, "launch exec");
-    c->launches += pipeline_launch_count(a_ex);
     // carry the current tables over to the next submission (device-to-device, tables never visit the host)
     CarrySet next;
     if (cur.huf.kind == TabRef::SLOT) {
@@ -1409,13 +1397,7 @@ static int fd_decode_blocks_impl(b200z_frame_decoder *d, b200z_read_fn rd, void 
                 pending_err = bh.type == BT_COMPRESSED ? B200Z_ERR_BLOCK_CONTENT_READ : B200Z_ERR_BLOCK_BODY_READ; pending_stage = B200Z_STAGE_BLOCK_BODY;
                 break;
             }
-            BlockDesc bd;
-            memset(&bd, 0, sizeof bd);
-            BlockRefs r;
-            bd.src_off = off; bd.src_size = bh.content_size; bd.frame = 0; bd.btype = bh.type; bd.raw_size = bh.decompressed_size;
-            bd.block_in_frame = (uint32_t)(d->block_counter + s.descs.size()); bd.last = bh.last;
-            if (bh.type == BT_COMPRESSED) plan_compressed_block(d->staging.data() + off, bh.content_size, bd, r, cur, s.n_huf, s.n_fse, s.lit_bytes, s.nseq);
-            s.descs.push_back(bd); s.refs.push_back(r);
+            const BlockDesc &bd = s.add_block(off, bh, 0, (uint32_t)(d->block_counter + s.descs.size()), d->staging.data() + off, nullptr, cur);
             brc += bh.content_size;
             bytes_after.push_back(brc);
             if (bd.host_status) break;
@@ -1757,10 +1739,9 @@ extern "C" int b200z_compress_frames_batch(b200z_ctx *c, const uint8_t *input, s
     const bool prof = (c->flags & B200Z_FLAG_PROFILE) != 0;
     if (prof) CU(c, cudaEventRecord(r.ev[0], s));
     for (int st = 0; st < kCompressStages; st++) {
-        if (int le = launch_compress_stage(a, st, s)) return c->set_cuda_err((cudaError_t)le, kCompressStageNames[st]);
+        if (int le = launch_compress_stage(a, st, s, &c->launches)) return c->set_cuda_err((cudaError_t)le, kCompressStageNames[st]);
         if (prof) CU(c, cudaEventRecord(r.ev[st + 1], s));
     }
-    c->launches += compress_launch_count(a);
     CU(c, cudaMemcpyAsync(results, r.results.p, nframes * sizeof(b200z_compress_result), cudaMemcpyDeviceToHost, s));
     CU(c, cudaStreamSynchronize(s));
     if (output_mem == B200Z_MEM_HOST)

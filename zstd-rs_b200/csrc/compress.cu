@@ -232,19 +232,17 @@ int init_compress_kernels() {
 
 const char *const kCompressStageNames[kCompressStages] = {"k_cmatch", "k_cenc", "k_cxxh64", "k_cassemble"};
 
-int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s) {
+int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s, uint64_t *launched) {
     switch (stage) {
-    case 0: if (a.level && a.nblocks) k_cmatch<<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info); break;
-    case 1: if (a.level && a.nblocks) k_cenc<<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res); break;
-    case 2: if (a.checksum && a.nframes) k_cxxh64<<<cdiv_u((uint64_t)a.nframes * 4, 128), 128, 0, s>>>(a.frames, a.input, a.csum, a.nframes); break;
-    case 3: if (a.nblocks) k_cassemble<<<a.nblocks, 256, 0, s>>>(a.frames, a.blocks, a.res, a.enc, a.input, a.csum, a.output, a.results, a.level, a.checksum); break;
+    case 0: if (!a.level || !a.nblocks) return 0; k_cmatch<<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info); break;
+    case 1: if (!a.level || !a.nblocks) return 0; k_cenc<<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res); break;
+    case 2: if (!a.checksum || !a.nframes) return 0; k_cxxh64<<<cdiv_u((uint64_t)a.nframes * 4, 128), 128, 0, s>>>(a.frames, a.input, a.csum, a.nframes); break;
+    case 3: if (!a.nblocks) return 0; k_cassemble<<<a.nblocks, 256, 0, s>>>(a.frames, a.blocks, a.res, a.enc, a.input, a.csum, a.output, a.results, a.level, a.checksum); break;
     default: return (int)cudaErrorInvalidValue;
     }
-    return (int)cudaGetLastError();
-}
-
-uint32_t compress_launch_count(const CompressArgs &a) {
-    return (a.level ? 2u : 0u) + (a.checksum ? 1u : 0u) + 1u;
+    const int e = (int)cudaGetLastError();
+    if (!e) ++*launched;
+    return e;
 }
 
 }  // namespace b200z

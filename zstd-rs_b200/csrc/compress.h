@@ -47,7 +47,6 @@ struct CompressArgs {
 int init_compress_kernels();
 constexpr int kCompressStages = 4;
 extern const char *const kCompressStageNames[kCompressStages];
-int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s);
-uint32_t compress_launch_count(const CompressArgs &a);
+int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s, uint64_t *launched);   // adds the kernels it enqueued to *launched
 
 }  // namespace b200z

@@ -1466,7 +1466,6 @@ __global__ void k_walk(const uint8_t *__restrict__ input, uint64_t input_len, co
 
 }  // namespace b200z
 
-#include "fse2.cuh"
 #include "exec_cta.cuh"
 
 namespace b200z {
@@ -1476,9 +1475,16 @@ namespace b200z {
 // ------------------------------------------------------------------------------------------------------------
 static inline uint32_t cdiv(uint32_t a, uint32_t b) { return (a + b - 1) / b; }
 
-int launch_predefined(FseSlot *predef, cudaStream_t s) {
+// error of the launch just made; counts it in *launched when it was enqueued
+static int launched_one(uint64_t *launched) {
+    const int e = (int)cudaGetLastError();
+    if (!e) ++*launched;
+    return e;
+}
+
+int launch_predefined(FseSlot *predef, cudaStream_t s, uint64_t *launched) {
     k_predefined<<<1, 32, 0, s>>>(predef);
-    return (int)cudaGetLastError();
+    return launched_one(launched);
 }
 
 constexpr uint32_t kHufSmem = HUF_BLOCKS_PER_CTA * HUF_SMEM_PER_BLOCK + 32 * RING_STRIDE;
@@ -1490,10 +1496,6 @@ int init_kernels() {
     cudaError_t e = cudaFuncSetAttribute(k_fse, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFseSmem);
     if (e != cudaSuccess) return (int)e;
     e = cudaFuncSetAttribute(k_huf, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHufSmem);
-    if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(k_fse2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFse2Smem);
-    if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(k_fse2, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
     if (e != cudaSuccess) return (int)e;
     e = cudaFuncSetAttribute(k_exec_cta, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)XC_SMEM_BYTES);
     if (e != cudaSuccess) return (int)e;
@@ -1517,58 +1519,62 @@ uint32_t num_sms() {
 
 const char *const kStageNames[kNumStages] = {"k_setup", "k_huf", "k_fse", "k_exec_cta", "k_exec"};
 
+// k_exec, one warp per frame: every frame of the warp kernel, and whatever k_exec_cta left (resume[]).  `dependent_of_fse`
+// launches it as the programmatic dependent of the k_fse just before it in the stream (launch_pipeline_overlapped).
+static int launch_exec(const PipelineArgs &a, cudaStream_t s, bool dependent_of_fse, uint64_t *launched) {
+    if (!a.nframes) return 0;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(cdiv(a.nframes, EXEC_WARPS)); cfg.blockDim = dim3(EXEC_WARPS * 32); cfg.dynamicSmemBytes = 0; cfg.stream = s;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    static const bool no_pdl = [] { const char *e = getenv("B200Z_EXEC_PDL"); return e && e[0] == '0'; }();   // A/B knob: k_exec strictly after k_fse
+    cfg.attrs = attr; cfg.numAttrs = dependent_of_fse && !no_pdl ? 1 : 0;
+    const int e = (int)cudaLaunchKernelEx(&cfg, k_exec, a.descs, (const BlockAux *)a.aux, a.frames, a.states, a.input, (const uint8_t *)a.lit_scratch,
+                                          (const uint32_t *)a.seq_scratch, a.output, a.output_cap, a.nframes, a.resume, 0u);
+    if (!e) ++*launched;
+    return e;
+}
+
 // one stage of the pipeline; a stage with nothing to do launches nothing and returns 0
-int launch_stage(const PipelineArgs &a, int stage, cudaStream_t s) {
+int launch_stage(const PipelineArgs &a, int stage, cudaStream_t s, uint64_t *launched) {
     switch (stage) {
-        case 0: if (a.nblocks) k_setup<<<cdiv(a.nblocks, SETUP_WARPS), SETUP_WARPS * 32, 0, s>>>(a.descs, a.aux, a.input, a.nblocks, 3u); break;
+        case 0:
+            if (!a.nblocks) return 0;
+            k_setup<<<cdiv(a.nblocks, SETUP_WARPS), SETUP_WARPS * 32, 0, s>>>(a.descs, a.aux, a.input, a.nblocks, 3u);
+            break;
         case 1:
-            if (a.nblocks)
-                k_huf<<<cdiv(a.nblocks, HUF_BLOCKS_PER_CTA), 32, kHufSmem, s>>>(a.descs, a.aux, a.input, a.lit_scratch, a.nblocks);
+            if (!a.nblocks) return 0;
+            k_huf<<<cdiv(a.nblocks, HUF_BLOCKS_PER_CTA), 32, kHufSmem, s>>>(a.descs, a.aux, a.input, a.lit_scratch, a.nblocks);
             break;
         case 2:
-            if (a.nblocks) {
-                // default: one warp walks chain and values (106 instructions per sequence).  B200Z_FSE=2: chain warp + value warp
-                // through a shared-memory queue (k_fse2) -- the chain only drops to 92 instructions and pays for the queue hand-off;
-                // kept for A/B runs.
-                static const bool one_warp = [] { const char *e = getenv("B200Z_FSE"); return !(e && e[0] == '2'); }();
-                if (one_warp) k_fse<<<cdiv(a.nblocks, FSE_BLOCKS_PER_CTA), 32, kFseSmem, s>>>(a.descs, a.aux, a.input, a.seq_scratch, a.nblocks, a.fse_order);
-                else k_fse2<<<cdiv(a.nblocks, F2_LANES), 64, kFse2Smem, s>>>(a.descs, a.aux, a.input, a.seq_scratch, a.nblocks);
-            }
+            if (!a.nblocks) return 0;
+            k_fse<<<cdiv(a.nblocks, FSE_BLOCKS_PER_CTA), 32, kFseSmem, s>>>(a.descs, a.aux, a.input, a.seq_scratch, a.nblocks, a.fse_order);
             break;
         case 3:
             // frames whose blocks are assembled in shared memory: persistent CTAs, one per SM, frames from a ticket counter
-            if (a.nframes && a.n_cta_frames)
-                k_exec_cta<<<a.n_cta_frames < num_sms() ? a.n_cta_frames : num_sms(), XC_THREADS, XC_SMEM_BYTES, s>>>(
-                    a.descs, a.aux, a.frames, a.states, a.input, a.lit_scratch, a.seq_scratch, a.output, a.output_cap, a.cta_frames, a.n_cta_frames, a.resume,
-                    a.ticket);
+            if (!a.nframes || !a.n_cta_frames) return 0;
+            k_exec_cta<<<a.n_cta_frames < num_sms() ? a.n_cta_frames : num_sms(), XC_THREADS, XC_SMEM_BYTES, s>>>(
+                a.descs, a.aux, a.frames, a.states, a.input, a.lit_scratch, a.seq_scratch, a.output, a.output_cap, a.cta_frames, a.n_cta_frames, a.resume,
+                a.ticket);
             break;
-        case 4:
-            // every other frame, and whatever k_exec_cta left (resume[]): one warp per frame
-            if (a.nframes) {
-                // optional waves (B200Z_EXEC_WAVE frames per launch): fewer live windows, so match sources stay in L2
-                static const uint32_t wave = [] { const char *e = getenv("B200Z_EXEC_WAVE"); return e ? (uint32_t)strtoul(e, nullptr, 10) : 0u; }();
-                const uint32_t step = wave ? wave : a.nframes;
-                for (uint32_t base = 0; base < a.nframes; base += step) {
-                    const uint32_t n = a.nframes - base < step ? a.nframes - base : step;
-                    k_exec<<<cdiv(n, EXEC_WARPS), EXEC_WARPS * 32, 0, s>>>(a.descs, a.aux, a.frames, a.states, a.input, a.lit_scratch, a.seq_scratch,
-                                                                 a.output, a.output_cap, base + n, a.resume, base);
-                }
-            }
-            break;
-        default: break;
+        case 4: return launch_exec(a, s, false, launched);
+        default: return 0;
     }
-    return (int)cudaGetLastError();
+    return launched_one(launched);
 }
 
 int launch_walk(const uint8_t *d_input, uint64_t input_len, const uint64_t *d_src_off, const uint64_t *d_src_size, uint32_t nframes, WalkFrame *d_wf,
-                const uint32_t *d_first_block, WalkBlock *d_wb, int fill, cudaStream_t s) {
-    if (nframes) k_walk<<<cdiv(nframes, 128), 128, 0, s>>>(d_input, input_len, d_src_off, d_src_size, nframes, d_wf, d_first_block, d_wb, fill);
-    return (int)cudaGetLastError();
+                const uint32_t *d_first_block, WalkBlock *d_wb, int fill, cudaStream_t s, uint64_t *launched) {
+    if (!nframes) return 0;
+    k_walk<<<cdiv(nframes, 128), 128, 0, s>>>(d_input, input_len, d_src_off, d_src_size, nframes, d_wf, d_first_block, d_wb, fill);
+    return launched_one(launched);
 }
 
-int launch_checksum(const PipelineArgs &a, cudaStream_t s) {
-    if (a.nframes) k_xxh64<<<cdiv(a.nframes * 4, 128), 128, 0, s>>>(a.frames, a.states, a.output, a.nframes);
-    return (int)cudaGetLastError();
+int launch_checksum(const PipelineArgs &a, cudaStream_t s, uint64_t *launched) {
+    if (!a.nframes) return 0;
+    k_xxh64<<<cdiv(a.nframes * 4, 128), 128, 0, s>>>(a.frames, a.states, a.output, a.nframes);
+    return launched_one(launched);
 }
 
 // resume[] and the ticket counter start from their initial image for every pass
@@ -1577,22 +1583,10 @@ int reset_sched(const PipelineArgs &a, cudaStream_t s) {
     return (int)cudaMemcpyAsync(a.ticket, a.sched_init, a.sched_bytes, cudaMemcpyDeviceToDevice, s);
 }
 
-int launch_pipeline(const PipelineArgs &a, cudaStream_t s) {
+int launch_pipeline(const PipelineArgs &a, cudaStream_t s, uint64_t *launched) {
     if (int e = reset_sched(a, s)) return e;
-    for (int st = 0; st < kNumStages; st++) { int e = launch_stage(a, st, s); if (e) return e; }
+    for (int st = 0; st < kNumStages; st++) { int e = launch_stage(a, st, s, launched); if (e) return e; }
     return 0;
-}
-
-static int launch_exec_warp(const PipelineArgs &a, cudaStream_t s, bool dependent_of_fse) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(cdiv(a.nframes, EXEC_WARPS)); cfg.blockDim = dim3(EXEC_WARPS * 32); cfg.dynamicSmemBytes = 0; cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    static const bool no_pdl = [] { const char *e = getenv("B200Z_EXEC_PDL"); return e && e[0] == '0'; }();   // A/B knob: k_exec strictly after k_fse
-    cfg.attrs = attr; cfg.numAttrs = dependent_of_fse && !no_pdl ? 1 : 0;
-    return (int)cudaLaunchKernelEx(&cfg, k_exec, a.descs, (const BlockAux *)a.aux, a.frames, a.states, a.input, (const uint8_t *)a.lit_scratch,
-                                   (const uint32_t *)a.seq_scratch, a.output, a.output_cap, a.nframes, a.resume, 0u);
 }
 
 // The shipped launch order.  k_exec (one warp per frame) runs BESIDE k_fse: it is launched in the same stream as k_fse's
@@ -1601,16 +1595,16 @@ static int launch_exec_warp(const PipelineArgs &a, cudaStream_t s, bool dependen
 // block's sequence stage is over (BlockAux::ready).  k_fse is a latency-bound chain that leaves most issue slots idle; k_exec is
 // issue-bound.  Frames of k_exec_cta follow when k_fse is complete, then k_exec once more for whatever k_exec_cta handed back.
 // (k_huf beside k_fse on a second stream was measured: no gain -- both want the shared memory of every SM.)
-int launch_pipeline_overlapped(const PipelineArgs &a, const PipelineStreams &ps) {
+int launch_pipeline_overlapped(const PipelineArgs &a, const PipelineStreams &ps, uint64_t *launched) {
     int e;
     if ((e = reset_sched(a, ps.main))) return e;
-    if ((e = launch_tables_literals(a, ps))) return e;
-    if ((e = launch_fse_exec(a, ps.main))) return e;
-    return launch_cta_rest(a, ps.main);
+    if ((e = launch_tables_literals(a, ps, launched))) return e;
+    if ((e = launch_fse_exec(a, ps.main, launched))) return e;
+    return launch_cta_rest(a, ps.main, launched);
 }
 
 // k_setup (both sides) and k_huf
-int launch_tables_literals(const PipelineArgs &a, const PipelineStreams &ps) {
+int launch_tables_literals(const PipelineArgs &a, const PipelineStreams &ps, uint64_t *launched) {
     int e;
     if (a.nblocks && ps.side && ps.fork && ps.join) {
         // literals side (Huffman tables, then k_huf) on the side stream, beside the FSE table builds on the main stream; both are
@@ -1618,37 +1612,32 @@ int launch_tables_literals(const PipelineArgs &a, const PipelineStreams &ps) {
         if ((e = (int)cudaEventRecord(ps.fork, ps.main))) return e;
         if ((e = (int)cudaStreamWaitEvent(ps.side, ps.fork, 0))) return e;
         k_setup<<<cdiv(a.nblocks, SETUP_WARPS), SETUP_WARPS * 32, 0, ps.side>>>(a.descs, a.aux, a.input, a.nblocks, 1u);
-        if ((e = (int)cudaGetLastError())) return e;
-        if ((e = launch_stage(a, 1, ps.side))) return e;
+        if ((e = launched_one(launched))) return e;
+        if ((e = launch_stage(a, 1, ps.side, launched))) return e;
         if ((e = (int)cudaEventRecord(ps.join, ps.side))) return e;
         k_setup<<<cdiv(a.nblocks, SETUP_WARPS), SETUP_WARPS * 32, 0, ps.main>>>(a.descs, a.aux, a.input, a.nblocks, 2u);
-        if ((e = (int)cudaGetLastError())) return e;
+        if ((e = launched_one(launched))) return e;
         if ((e = (int)cudaStreamWaitEvent(ps.main, ps.join, 0))) return e;
     } else {
-        if ((e = launch_stage(a, 0, ps.main))) return e;
-        if ((e = launch_stage(a, 1, ps.main))) return e;
+        if ((e = launch_stage(a, 0, ps.main, launched))) return e;
+        if ((e = launch_stage(a, 1, ps.main, launched))) return e;
     }
     return 0;
 }
 
 // k_fse and, beside it, k_exec for the frames of the warp kernel
-int launch_fse_exec(const PipelineArgs &a, cudaStream_t s) {
+int launch_fse_exec(const PipelineArgs &a, cudaStream_t s, uint64_t *launched) {
     int e;
-    if ((e = launch_stage(a, 2, s))) return e;
-    if (!a.nframes || a.n_cta_frames >= a.nframes) return 0;
-    return launch_exec_warp(a, s, a.nblocks != 0);
+    if ((e = launch_stage(a, 2, s, launched))) return e;
+    if (a.n_cta_frames >= a.nframes) return 0;
+    return launch_exec(a, s, a.nblocks != 0, launched);
 }
 
 // k_exec_cta for its frames, then k_exec for what it handed back
-int launch_cta_rest(const PipelineArgs &a, cudaStream_t s) {
+int launch_cta_rest(const PipelineArgs &a, cudaStream_t s, uint64_t *launched) {
     if (!a.nframes || !a.n_cta_frames) return 0;
-    if (int e = launch_stage(a, 3, s)) return e;
-    return launch_exec_warp(a, s, false);
-}
-
-// launches of launch_pipeline_overlapped
-uint32_t pipeline_launch_count(const PipelineArgs &a) {
-    return (a.nblocks ? 4u : 0u) + (a.nframes && a.n_cta_frames < a.nframes ? 1u : 0u) + (a.nframes && a.n_cta_frames ? 2u : 0u);
+    if (int e = launch_stage(a, 3, s, launched)) return e;
+    return launch_exec(a, s, false, launched);
 }
 
 }  // namespace b200z

@@ -32,23 +32,23 @@ struct PipelineArgs {
                                   // next block of EVERY frame ready instead of whole frames one after the other
 };
 
+// Every launcher adds the kernels it enqueued to *launched and returns 0 or the cudaError_t of the first failing call.
 int init_kernels();  // per-device function attributes (dynamic shared memory); call once per context
-int launch_predefined(FseSlot *predef, cudaStream_t s);
+int launch_predefined(FseSlot *predef, cudaStream_t s, uint64_t *launched);
 constexpr int kNumStages = 5;
 extern const char *const kStageNames[kNumStages];
-int launch_stage(const PipelineArgs &a, int stage, cudaStream_t s);
+int launch_stage(const PipelineArgs &a, int stage, cudaStream_t s, uint64_t *launched);
 int reset_sched(const PipelineArgs &a, cudaStream_t s);      // ticket / resume[] back to their initial image (start of every pass)
-int launch_pipeline(const PipelineArgs &a, cudaStream_t s);   // the stages one after the other (profiling, streaming decoder)
+int launch_pipeline(const PipelineArgs &a, cudaStream_t s, uint64_t *launched);   // the stages one after the other (streaming decoder)
 // device-side header walk for device-resident input (k_walk): fill = 0 counts the blocks of every frame, fill = 1 writes the digests
 int launch_walk(const uint8_t *d_input, uint64_t input_len, const uint64_t *d_src_off, const uint64_t *d_src_size, uint32_t nframes, WalkFrame *d_wf,
-                const uint32_t *d_first_block, WalkBlock *d_wb, int fill, cudaStream_t s);
+                const uint32_t *d_first_block, WalkBlock *d_wb, int fill, cudaStream_t s, uint64_t *launched);
 uint32_t num_sms();   // of the current device (132 on H100 SXM)
-int launch_checksum(const PipelineArgs &a, cudaStream_t s);   // optional 5th stage: XXH64 of every frame's plaintext
+int launch_checksum(const PipelineArgs &a, cudaStream_t s, uint64_t *launched);   // optional 5th stage: XXH64 of every frame's plaintext
 struct PipelineStreams { cudaStream_t main, side; cudaEvent_t fork, join; };
-int launch_pipeline_overlapped(const PipelineArgs &a, const PipelineStreams &ps);   // the shipped order: k_exec beside k_fse (programmatic dependent launch)
-int launch_tables_literals(const PipelineArgs &a, const PipelineStreams &ps);   // k_setup (literals side + k_huf on `side`, sequences side on `main`)
-int launch_fse_exec(const PipelineArgs &a, cudaStream_t s);    // k_fse + (beside it) k_exec for the warp kernel's frames
-int launch_cta_rest(const PipelineArgs &a, cudaStream_t s);    // k_exec_cta + k_exec for what it handed back
-uint32_t pipeline_launch_count(const PipelineArgs &a);
+int launch_pipeline_overlapped(const PipelineArgs &a, const PipelineStreams &ps, uint64_t *launched);   // the shipped order: k_exec beside k_fse (programmatic dependent launch)
+int launch_tables_literals(const PipelineArgs &a, const PipelineStreams &ps, uint64_t *launched);   // k_setup (literals side + k_huf on `side`, sequences side on `main`)
+int launch_fse_exec(const PipelineArgs &a, cudaStream_t s, uint64_t *launched);    // k_fse + (beside it) k_exec for the warp kernel's frames
+int launch_cta_rest(const PipelineArgs &a, cudaStream_t s, uint64_t *launched);    // k_exec_cta + k_exec for what it handed back
 
 }  // namespace b200z
