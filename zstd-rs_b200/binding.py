@@ -15,8 +15,7 @@ import subprocess
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# B200Z_LIB: development knob to load an experimental build of the same library (profiles/variants.sh); never a fallback
-_SO = os.environ.get("B200Z_LIB") or os.path.join(_HERE, "libb200zstd.so")
+_SO = os.path.join(_HERE, "libb200zstd.so")
 _HEADER = os.path.join(_HERE, "..", "include", "b200zstd.h")
 
 READ_FN = C.CFUNCTYPE(C.c_long, C.c_void_p, C.POINTER(C.c_uint8), C.c_size_t)

@@ -7,7 +7,6 @@
 #include <string.h>
 
 #include <algorithm>
-#include <chrono>
 #include <map>
 #include <memory>
 #include <string>
@@ -354,20 +353,17 @@ struct Submission {
             }
             if (!force_warp && !force_cta) route_exec_frames(work.data(), eligible.data(), frames.size(), num_sms(), cta_frames);
         }
-        // the order in which k_fse takes the blocks (build_fse_order, plan.cpp).  B200Z_FSE_ORDER=0 keeps the descriptor order.
+        // the order in which k_fse takes the blocks (build_fse_order, plan.cpp)
         fse_order.clear();
-        {
-            const char *eo = getenv("B200Z_FSE_ORDER");
-            if (!(eo && eo[0] == '0') && !frames.empty()) {
-                std::vector<uint8_t> on_cta(frames.size(), 0);
-                for (uint32_t f : cta_frames) on_cta[f] = 1;
-                std::vector<uint32_t> fb(frames.size()), nb(frames.size()), nseq(descs.size());
-                for (size_t f = 0; f < frames.size(); f++) { fb[f] = frames[f].first_block; nb[f] = frames[f].nblocks; }
-                for (size_t i = 0; i < descs.size(); i++) nseq[i] = descs[i].nseq;
-                build_fse_order(fb.data(), nb.data(), on_cta.data(), frames.size(), nseq.data(), descs.size(), fse_order);
-            }
-            if (!fse_order.empty() && (e = d_order.ensure(4 * fse_order.size()))) return e;
+        if (!frames.empty()) {
+            std::vector<uint8_t> on_cta(frames.size(), 0);
+            for (uint32_t f : cta_frames) on_cta[f] = 1;
+            std::vector<uint32_t> fb(frames.size()), nb(frames.size()), nseq(descs.size());
+            for (size_t f = 0; f < frames.size(); f++) { fb[f] = frames[f].first_block; nb[f] = frames[f].nblocks; }
+            for (size_t i = 0; i < descs.size(); i++) nseq[i] = descs[i].nseq;
+            build_fse_order(fb.data(), nb.data(), on_cta.data(), frames.size(), nseq.data(), descs.size(), fse_order);
         }
+        if (!fse_order.empty() && (e = d_order.ensure(4 * fse_order.size()))) return e;
         // scheduling buffer: [ticket + 3 counters][resume[nframes]][cta frame list][initial image of the first two parts]
         if ((e = d_sched.ensure(2 * (16 + 4 * frames.size()) + 4 * cta_frames.size() + 32))) return e;
         HufSlot *hs = d_huf.as<HufSlot>();
@@ -563,26 +559,17 @@ extern "C" int b200z_batch_prepare(b200z_ctx *c, const uint8_t *input, size_t in
     if (int e = c->use()) return e;
     std::unique_ptr<b200z_batch> b(new b200z_batch());
     b->ctx = c; b->input_len = input_len;
-    const uint8_t *hin = input;
+    const bool on_device = input_mem == B200Z_MEM_DEVICE;
     WalkHost walk;
-    std::vector<uint8_t> host_copy;
-    if (input_mem == B200Z_MEM_DEVICE) {
+    if (on_device) {
         // The input stays on the device: k_walk follows the frame / block / section headers there and brings back the ~16 bytes per
-        // block the planner parses (SURVEY.md 8(f).3) -- not the compressed data (B200Z_WALK=host copies it back and walks on the host,
-        // for A/B tests).
+        // block the planner parses (SURVEY.md 8(f).3) -- not the compressed data.
         b->d_input = input;
-        const char *wm = getenv("B200Z_WALK");
-        if (wm && !strcmp(wm, "host")) {
-            host_copy.resize(input_len);
-            if (input_len) CU(c, cudaMemcpy(host_copy.data(), input, input_len, cudaMemcpyDeviceToHost));
-            hin = host_copy.data();
-        } else {
-            hin = nullptr;
-            if (int e = device_walk(c, input, input_len, frames, nframes, walk)) return e;
-        }
+        if (int e = device_walk(c, input, input_len, frames, nframes, walk)) return e;
     }
-    if (int e = plan_batch(b.get(), hin, input_len, frames, nframes, dicts, ndicts, forced, max_window, hin ? nullptr : (input_mem == B200Z_MEM_DEVICE ? &walk : nullptr))) return e;
-    if (input_mem != B200Z_MEM_DEVICE) {
+    if (int e = plan_batch(b.get(), on_device ? nullptr : input, input_len, frames, nframes, dicts, ndicts, forced, max_window, on_device ? &walk : nullptr))
+        return e;
+    if (!on_device) {
         if (int e = b->d_input_own.ensure(input_len + 16, false)) return e;
         if (input_len) CU(c, cudaMemcpyAsync(b->d_input_own.p, input, input_len, cudaMemcpyHostToDevice, c->stream));
         b->d_input = b->d_input_own.as<uint8_t>();
@@ -896,9 +883,6 @@ static int decode_frames_pipelined(b200z_ctx *c, const uint8_t *input, size_t in
         }
         cut.push_back(nframes);
     }
-    const bool trace = getenv("B200Z_TRACE") != nullptr;
-    auto t_start = std::chrono::steady_clock::now();
-    auto now_ms = [&]() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count(); };
     struct Pending { size_t f0 = 0, f1 = 0; bool live = false; } pend[2];
     auto retire = [&](int s) -> int {   // results of the chunk that used set s
         if (!pend[s].live) return 0;
@@ -914,12 +898,9 @@ static int decode_frames_pipelined(b200z_ctx *c, const uint8_t *input, size_t in
     for (size_t ci = 0; ci + 1 < cut.size(); ci++) {
         const int s = (int)(ci & 1);
         const size_t f0 = cut[ci], f1 = cut[ci + 1];
-        double t0 = now_ms();
         if (int e = retire(s)) return e;
-        double t1 = now_ms();
         b200z_batch *b = p->set[s];
         if (int e = plan_batch(b, input, input_len, frames + f0, f1 - f0, dicts, ndicts, forced, max_window)) return e;
-        double t2 = now_ms();
         // input byte range and output byte range of this chunk
         uint64_t ilo = UINT64_MAX, ihi = 0, olo = UINT64_MAX, ohi = 0;
         for (size_t i = f0; i < f1; i++) {
@@ -951,11 +932,9 @@ static int decode_frames_pipelined(b200z_ctx *c, const uint8_t *input, size_t in
         if (ohi > olo) CU(c, cudaMemcpyAsync(output + olo, d_out + olo, ohi - olo, cudaMemcpyDeviceToHost, p->s_d2h));
         CU(c, cudaEventRecord(p->ev_done[s], p->s_d2h));
         pend[s].f0 = f0; pend[s].f1 = f1; pend[s].live = true;
-        if (trace) fprintf(stderr, "[b200z] chunk %zu frames %zu..%zu: start %.2f retire-wait %.2f plan %.2f enqueue %.2f ms\n", ci, f0, f1, t0, t1 - t0, t2 - t1, now_ms() - t2);
     }
     if (int e = retire(0)) return e;
     if (int e = retire(1)) return e;
-    if (trace) fprintf(stderr, "[b200z] pipelined one-shot done at %.2f ms\n", now_ms());
     return 0;
 }
 
@@ -1011,7 +990,7 @@ extern "C" int b200z_decode_blocks_batch(b200z_ctx *c, const b200z_block_desc *b
     if (int e = c->use()) return e;
     std::vector<uint8_t> host_copy;
     const uint8_t *hin = compressed;
-    if (compressed_mem == B200Z_MEM_DEVICE) {   // the section headers are walked on the host (as in b200z_batch_prepare)
+    if (compressed_mem == B200Z_MEM_DEVICE) {   // the section headers are walked on the host
         host_copy.resize(compressed_len);
         if (compressed_len) CU(c, cudaMemcpy(host_copy.data(), compressed, compressed_len, cudaMemcpyDeviceToHost));
         hin = host_copy.data();

@@ -464,19 +464,9 @@ __global__ void __launch_bounds__(32) k_huf(const BlockDesc *__restrict__ descs,
 // written four at a time as three 16-byte vectors.  A warp alone on its scheduler is bound by the 16-lane integer
 // pipe (2 cycles per warp instruction), not by dependencies: the step is written for instruction count.
 // ------------------------------------------------------------------------------------------------------------
-#ifndef B200Z_FSE_CHAINS
-#define B200Z_FSE_CHAINS 1
-#endif
-constexpr uint32_t FSE_CHAINS = B200Z_FSE_CHAINS;            // blocks per lane, decoded interleaved
-#ifndef B200Z_FSE_LANES
-#define B200Z_FSE_LANES 16
-#endif
-constexpr uint32_t FSE_LANES = B200Z_FSE_LANES;              // lanes of the warp that carry blocks
-constexpr uint32_t FSE_BLOCKS_PER_CTA = FSE_LANES * FSE_CHAINS;
+constexpr uint32_t FSE_LANES = 16;                  // lanes of the warp that carry blocks (= blocks per CTA)
 constexpr uint32_t FSE_TAB_U16 = 512 + 512 + 256;   // LL, ML, OF entries per block
-#ifndef B200Z_FSE_PUBLISH
-#define B200Z_FSE_PUBLISH 128u   // sequences between two progress publications (power of two, multiple of 4)
-#endif
+constexpr uint32_t FSE_PUBLISH = 128;               // sequences between two progress publications (power of two, multiple of 4)
 
 __constant__ uint32_t c_ll_base[36] = {0,1,2,3,4,5,6,7,8,9,10,11,12,13,14,15,16,18,20,22,24,28,32,40,48,64,128,256,512,1024,2048,4096,8192,16384,32768,65536};
 __constant__ uint8_t c_ll_bits[36] = {0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,0,1,1,1,1,2,2,3,3,4,6,7,8,9,10,11,12,13,14,15,16};
@@ -522,9 +512,7 @@ struct FseState {
     }
 };
 
-// One block's sequence decode on the fast path: everything a chain carries between steps.  A lane runs FSE_CHAINS of
-// them interleaved -- the chains are independent, so the second one's instructions fill the dependency stalls of the
-// first (one warp per scheduler: there is nobody else to issue).
+// One block's sequence decode on the fast path: everything a lane carries between steps.
 struct FseChain {
     // per block
     uint32_t b; const BlockDesc *d; bool active, run, bad; uint32_t st_seq;
@@ -674,45 +662,30 @@ __device__ __noinline__ void fse_exact_block(const BlockDesc *d, BlockAux *aux, 
     aux[b].out_size = (ovf >> 31) ? 0xffffffffu : out_end - lit_end + d->regen_size;   // sum of ml + regenerated literals
 }
 
-#ifdef B200Z_PROBE
-// Development probe (profiles/variants.sh probe "-DB200Z_PROBE", profiles/probe_overlap.py): device timestamps of the k_fse / k_exec pair.
-// [0] first k_fse CTA start, [1] last k_fse CTA end, [2] first k_exec warp start, [3] last k_exec warp end, [4] last k_exec warp start,
-// [5] first k_exec warp end (globaltimer, ns).  Not part of the shipped library.
-__device__ unsigned long long g_probe[8];
-__device__ __forceinline__ unsigned long long probe_now() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
-extern "C" int b200z_probe_read(unsigned long long *out, int reset) {
-    if (out && cudaMemcpyFromSymbol(out, g_probe, sizeof(unsigned long long) * 8) != cudaSuccess) return 1;
-    if (reset) {
-        const unsigned long long init[8] = {~0ull, 0, ~0ull, 0, 0, ~0ull, 0, 0};
-        if (cudaMemcpyToSymbol(g_probe, init, sizeof init) != cudaSuccess) return 1;
-    }
-    return 0;
-}
-#endif
 __global__ void __launch_bounds__(32) k_fse(const BlockDesc *__restrict__ descs, BlockAux *__restrict__ aux, const uint8_t *__restrict__ input,
                                           uint32_t *__restrict__ seq_scratch, uint32_t nblocks, const uint32_t *__restrict__ order) {
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // this CTA is resident: k_exec may follow (launch_pipeline_overlapped)
-#ifdef B200Z_PROBE
-    if (threadIdx.x == 0) atomicMin(&g_probe[0], probe_now());
-#endif
     extern __shared__ __align__(16) uint8_t smem_fse[];
     uint16_t *tabs = reinterpret_cast<uint16_t *>(smem_fse);
-    uint32_t *s_ll_base = reinterpret_cast<uint32_t *>(smem_fse + FSE_BLOCKS_PER_CTA * FSE_TAB_U16 * 2);
+    uint32_t *s_ll_base = reinterpret_cast<uint32_t *>(smem_fse + FSE_LANES * FSE_TAB_U16 * 2);
     uint32_t *s_ml_base = s_ll_base + 36;
     uint8_t *s_ll_bits = reinterpret_cast<uint8_t *>(s_ml_base + 53);
     uint8_t *s_ml_bits = s_ll_bits + 36;
-    uint32_t *s_ll = reinterpret_cast<uint32_t *>(smem_fse + FSE_BLOCKS_PER_CTA * FSE_TAB_U16 * 2 + 512);   // base | bits << 24
+    uint32_t *s_ll = reinterpret_cast<uint32_t *>(smem_fse + FSE_LANES * FSE_TAB_U16 * 2 + 512);   // base | bits << 24
     uint32_t *s_ml = s_ll + 36;
-    uint8_t *s_ring = smem_fse + FSE_BLOCKS_PER_CTA * FSE_TAB_U16 * 2 + 1024;                                // FSE_BLOCKS_PER_CTA x RING_STRIDE
+    uint8_t *s_ring = smem_fse + FSE_LANES * FSE_TAB_U16 * 2 + 1024;                                // FSE_LANES x RING_STRIDE
     const uint32_t lane = threadIdx.x;
     for (uint32_t i = lane; i < 36; i += 32) { s_ll_base[i] = c_ll_base[i]; s_ll_bits[i] = c_ll_bits[i]; s_ll[i] = c_ll_base[i] | ((uint32_t)c_ll_bits[i] << 24); }
     for (uint32_t i = lane; i < 53; i += 32) { s_ml_base[i] = c_ml_base[i]; s_ml_bits[i] = c_ml_bits[i]; s_ml[i] = c_ml_base[i] | ((uint32_t)c_ml_bits[i] << 24); }
 
-    FseChain ch[FSE_CHAINS];
-#pragma unroll
-    for (int k = 0; k < (int)FSE_CHAINS; k++) {
+    // The lane's block.  Its state is a one-element array walked by a one-trip loop on purpose: addressed through the
+    // loop index, it is promoted to registers only after the loop is unrolled, and ptxas schedules the fast path as it
+    // was tuned.  As a plain local it is promoted at once and the schedule changes: k_fse alone took 1.270 ms instead
+    // of 1.254 ms on C2b (H100 80GB HBM3, 700 W power limit).
+    FseChain ch[1];
+    for (int k = 0; k < 1; k++) {
         FseChain &c = ch[k];
-        c.b = blockIdx.x * FSE_BLOCKS_PER_CTA + FSE_CHAINS * lane + k;   // neighbouring blocks share a lane: similar lengths
+        c.b = blockIdx.x * FSE_LANES + lane;
         c.active = lane < FSE_LANES && c.b < nblocks;
         if (c.active && order) c.b = order[c.b];   // PipelineArgs::fse_order
         c.d = c.active ? &descs[c.b] : nullptr;
@@ -724,16 +697,13 @@ __global__ void __launch_bounds__(32) k_fse(const BlockDesc *__restrict__ descs,
             c.run = c.d->btype == BT_COMPRESSED && !c.d->host_status && c.d->nseq != 0 && c.st_seq == 0;
         }
         c.tl = c.run ? c.d->ll : nullptr; c.to = c.run ? c.d->of : nullptr; c.tm = c.run ? c.d->ml : nullptr;
-    }
-    // ---- stage the tables of the CTA's blocks (warp-cooperative, 16-byte vectors); slot = FSE_CHAINS * lane + chain
-    for (uint32_t j = 0; j < FSE_LANES; j++) {
-#pragma unroll
-        for (int k = 0; k < (int)FSE_CHAINS; k++) {
+        // ---- stage the tables of the CTA's blocks (warp-cooperative, 16-byte vectors); lane j's block goes to slot j
+        for (uint32_t j = 0; j < FSE_LANES; j++) {
             const FseTab *pj[3];
-            pj[0] = (const FseTab *)(uintptr_t)__shfl_sync(0xffffffffu, (unsigned long long)(uintptr_t)ch[k].tl, j);
-            pj[1] = (const FseTab *)(uintptr_t)__shfl_sync(0xffffffffu, (unsigned long long)(uintptr_t)ch[k].tm, j);
-            pj[2] = (const FseTab *)(uintptr_t)__shfl_sync(0xffffffffu, (unsigned long long)(uintptr_t)ch[k].to, j);
-            uint16_t *dstj = tabs + (FSE_CHAINS * j + k) * FSE_TAB_U16;
+            pj[0] = (const FseTab *)(uintptr_t)__shfl_sync(0xffffffffu, (unsigned long long)(uintptr_t)c.tl, j);
+            pj[1] = (const FseTab *)(uintptr_t)__shfl_sync(0xffffffffu, (unsigned long long)(uintptr_t)c.tm, j);
+            pj[2] = (const FseTab *)(uintptr_t)__shfl_sync(0xffffffffu, (unsigned long long)(uintptr_t)c.to, j);
+            uint16_t *dstj = tabs + j * FSE_TAB_U16;
             const uint32_t offs[3] = {0, 512, 1024};
 #pragma unroll
             for (int t = 0; t < 3; t++) {
@@ -746,120 +716,76 @@ __global__ void __launch_bounds__(32) k_fse(const BlockDesc *__restrict__ descs,
                 for (uint32_t i = lane; i < n16; i += 32) d4[i] = s4[i];
             }
         }
-    }
-    __syncwarp();
-    uint32_t qLL = (uint32_t)__cvta_generic_to_shared(s_ll), qML = (uint32_t)__cvta_generic_to_shared(s_ml);
-    asm volatile("" : "+r"(qLL), "+r"(qML));
+        __syncwarp();
+        uint32_t qLL = (uint32_t)__cvta_generic_to_shared(s_ll), qML = (uint32_t)__cvta_generic_to_shared(s_ml);
+        asm volatile("" : "+r"(qLL), "+r"(qML));
 
-    // ---------------- fast path: branch-free steps; anything unusual (bad code, > 32 extra bits in one sequence,
-    // under/over-run, uninitialised table) sets `bad` and the block is decoded again by the exact path below.
-#pragma unroll
-    for (int k = 0; k < (int)FSE_CHAINS; k++) {
-        FseChain &c = ch[k];
-        if (!c.run) { c.bad = false; continue; }
-        const uint32_t slot = FSE_CHAINS * lane + k;
-        const uint8_t *src = input + c.d->src_off + aux[c.b].seq_bits_off;
-        const uint32_t len = c.d->src_size - aux[c.b].seq_bits_off;
-        const uint16_t *TL = tabs + slot * FSE_TAB_U16;
-        const uint32_t ring_addr = (uint32_t)__cvta_generic_to_shared(s_ring + slot * RING_STRIDE) + 16u;   // slot 0; the mirror slot sits below
-        c.bad = !c.br.init(src, len, ring_addr) || !c.tl || !c.tl->valid || !c.to || !c.to->valid || !c.tm || !c.tm->valid;
-        if (!c.bad) c.bad = c.tl->log > 9u || c.tm->log > 9u || c.to->log > 8u;   // never true for a built table: the staged copies are sized for these
-        c.flags = 0; c.max_of = 0; c.max_x = 0; c.i = 0; c.out_end = 0; c.lit_end = 0; c.ovf = 0;
-        c.nseq = c.d->nseq;
-        c.h0 = 1u << SEQ_SYM_SHIFT; c.h1 = 2u << SEQ_SYM_SHIFT; c.h2 = 3u << SEQ_SYM_SHIFT;   // "slot k at the block's start"
-        c.out = seq_scratch + c.d->seq_buf_off * 3;
-        if (!c.bad) {
-            c.logL = c.tl->log; c.logM = c.tm->log; c.logO = c.to->log;
-            const uint32_t aTL = (uint32_t)__cvta_generic_to_shared(TL), aTM = aTL + 1024u, aTO = aTL + 2048u;
-            c.qTL = aTL - (2u << c.logL); c.qTM = aTM - (2u << c.logM); c.qTO = aTO - (2u << c.logO);
-            // initial states LL, OF, ML (sequence_section_decoder.rs:164-166)
-            uint32_t hi, lo;
-            c.br.window(hi, lo);
-            const uint32_t t1 = shl_c(hi, c.logL), t2 = shl_c(t1, c.logO);
-            c.eL = fse_lds16(aTL + (shr_c(hi, 32u - c.logL) << 1));
-            c.eO = fse_lds16(aTO + (shr_c(t1, 32u - c.logO) << 1));
-            c.eM = fse_lds16(aTM + (shr_c(t2, 32u - c.logM) << 1));
-            c.br.P -= (int32_t)(c.logL + c.logO + c.logM);
+        // ---------------- fast path: branch-free steps; anything unusual (bad code, > 32 extra bits in one sequence,
+        // under/over-run, uninitialised table) sets `bad` and the block is decoded again by the exact path below.
+        const uint16_t *TL = tabs + lane * FSE_TAB_U16;
+        if (c.run) {
+            const uint8_t *src = input + c.d->src_off + aux[c.b].seq_bits_off;
+            const uint32_t len = c.d->src_size - aux[c.b].seq_bits_off;
+            const uint32_t ring_addr = (uint32_t)__cvta_generic_to_shared(s_ring + lane * RING_STRIDE) + 16u;   // slot 0; the mirror slot sits below
+            c.bad = !c.br.init(src, len, ring_addr) || !c.tl || !c.tl->valid || !c.to || !c.to->valid || !c.tm || !c.tm->valid;
+            if (!c.bad) c.bad = c.tl->log > 9u || c.tm->log > 9u || c.to->log > 8u;   // never true for a built table: the staged copies are sized for these
+            c.flags = 0; c.max_of = 0; c.max_x = 0; c.i = 0; c.out_end = 0; c.lit_end = 0; c.ovf = 0;
+            c.nseq = c.d->nseq;
+            c.h0 = 1u << SEQ_SYM_SHIFT; c.h1 = 2u << SEQ_SYM_SHIFT; c.h2 = 3u << SEQ_SYM_SHIFT;   // "slot k at the block's start"
+            c.out = seq_scratch + c.d->seq_buf_off * 3;
+            if (!c.bad) {
+                c.logL = c.tl->log; c.logM = c.tm->log; c.logO = c.to->log;
+                const uint32_t aTL = (uint32_t)__cvta_generic_to_shared(TL), aTM = aTL + 1024u, aTO = aTL + 2048u;
+                c.qTL = aTL - (2u << c.logL); c.qTM = aTM - (2u << c.logM); c.qTO = aTO - (2u << c.logO);
+                // initial states LL, OF, ML (sequence_section_decoder.rs:164-166)
+                uint32_t hi, lo;
+                c.br.window(hi, lo);
+                const uint32_t t1 = shl_c(hi, c.logL), t2 = shl_c(t1, c.logO);
+                c.eL = fse_lds16(aTL + (shr_c(hi, 32u - c.logL) << 1));
+                c.eO = fse_lds16(aTO + (shr_c(t1, 32u - c.logO) << 1));
+                c.eM = fse_lds16(aTM + (shr_c(t2, 32u - c.logM) << 1));
+                c.br.P -= (int32_t)(c.logL + c.logO + c.logM);
+            }
         }
-    }
-    // joint loop: groups of four sequences of every chain, step by step in turn
-    {
-        bool joint = true;
-        uint32_t nmin = 0xFFFFFFFFu;
+        // groups of four sequences, then the last ones one at a time
+        if (c.run && !c.bad) {
+            if (!c.flags) {
+                uint32_t stage[12];
+                for (; c.i + 4 < c.nseq; c.i += 4) {
 #pragma unroll
-        for (int k = 0; k < (int)FSE_CHAINS; k++) { joint = joint && ch[k].run && !ch[k].bad; nmin = min(nmin, ch[k].run ? ch[k].nseq : 0u); }
-        if (FSE_CHAINS > 1 && joint) {
-            uint32_t stage[FSE_CHAINS][12];
-            uint32_t i = 0, anyflag = 0;
-            for (; i + 4 < nmin; i += 4) {
-#pragma unroll
-                for (int q = 0; q < 4; q++) {
-#pragma unroll
-                    for (int k = 0; k < (int)FSE_CHAINS; k++) fse_step(ch[k], qLL, qML, stage[k][3 * q], stage[k][3 * q + 1], stage[k][3 * q + 2], true);
-                    if (q & 1) {
-#pragma unroll
-                        for (int k = 0; k < (int)FSE_CHAINS; k++) ch[k].br.service();
-                    }
+                    for (int q = 0; q < 4; q++) { fse_step(c, qLL, qML, stage[3 * q], stage[3 * q + 1], stage[3 * q + 2], true); if (q & 1) c.br.service(); }
+                    fse_group_end(c, stage);
+                    if (c.flags) break;
+                    if (((c.i + 4) & (FSE_PUBLISH - 1u)) == 0) fse_publish_progress(aux, c.b, c.i + 4);   // the fence costs ~1 us
                 }
-#pragma unroll
-                for (int k = 0; k < (int)FSE_CHAINS; k++) { ch[k].i = i; fse_group_end(ch[k], stage[k]); anyflag |= ch[k].flags; }
-                if (anyflag) { i += 4; break; }
             }
-#pragma unroll
-            for (int k = 0; k < (int)FSE_CHAINS; k++) ch[k].i = i;
-        }
-    }
-    // each chain on its own: the rest of its groups, then its last sequences one at a time
-#pragma unroll
-    for (int k = 0; k < (int)FSE_CHAINS; k++) {
-        FseChain &c = ch[k];
-        if (!c.run || c.bad) continue;
-        if (!c.flags) {
-            uint32_t stage[12];
-            for (; c.i + 4 < c.nseq; c.i += 4) {
-#pragma unroll
-                for (int q = 0; q < 4; q++) { fse_step(c, qLL, qML, stage[3 * q], stage[3 * q + 1], stage[3 * q + 2], true); if (q & 1) c.br.service(); }
-                fse_group_end(c, stage);
-                if (c.flags) break;
-                if (((c.i + 4) & (B200Z_FSE_PUBLISH - 1u)) == 0) fse_publish_progress(aux, c.b, c.i + 4);   // the fence costs ~1 us
+            if (!c.flags) {
+                for (; c.i < c.nseq; c.i++) {
+                    uint32_t ll, ml, of;
+                    fse_step(c, qLL, qML, ll, ml, of, c.i + 1 < c.nseq);
+                    c.br.service();
+                    c.flags |= (uint32_t)(c.br.P < 0) | (uint32_t)(c.max_x > 38u) | ((c.max_of + 2u) >> 5);
+                    c.out[3 * c.i] = ll; c.out[3 * c.i + 1] = ml; c.out[3 * c.i + 2] = of;
+                }
+            }
+            c.bad = c.flags != 0 || c.br.P != 0;
+            if (!c.bad) {
+                aux[c.b].pad = 0;
+                aux[c.b].hist_after[0] = c.h0; aux[c.b].hist_after[1] = c.h1; aux[c.b].hist_after[2] = c.h2;
+                aux[c.b].sum_ll = c.lit_end;
+                aux[c.b].flags = (c.ovf >> 31) ? AUX_WIDE : 0u;
+                aux[c.b].out_size = (c.ovf >> 31) ? 0xffffffffu : c.out_end - c.lit_end + c.d->regen_size;   // sum of ml + regenerated literals
             }
         }
-        if (!c.flags) {
-            for (; c.i < c.nseq; c.i++) {
-                uint32_t ll, ml, of;
-                fse_step(c, qLL, qML, ll, ml, of, c.i + 1 < c.nseq);
-                c.br.service();
-                c.flags |= (uint32_t)(c.br.P < 0) | (uint32_t)(c.max_x > 38u) | ((c.max_of + 2u) >> 5);
-                c.out[3 * c.i] = ll; c.out[3 * c.i + 1] = ml; c.out[3 * c.i + 2] = of;
-            }
+        asm volatile("cp.async.wait_group 0;" ::: "memory");
+        // verdict; a block the fast path gave up on is decoded again by the exact path
+        if (c.active) {
+            if (!c.run) aux[c.b].pad = c.st_seq;
+            else if (c.bad) fse_exact_block(c.d, aux, c.b, input, seq_scratch, TL, TL + 512, TL + 1024, c.tl, c.to, c.tm, s_ll_base, s_ml_base, s_ll_bits, s_ml_bits, c.st_seq);
         }
-        c.bad = c.flags != 0 || c.br.P != 0;
-        if (!c.bad) {
-            aux[c.b].pad = 0;
-            aux[c.b].hist_after[0] = c.h0; aux[c.b].hist_after[1] = c.h1; aux[c.b].hist_after[2] = c.h2;
-            aux[c.b].sum_ll = c.lit_end;
-            aux[c.b].flags = (c.ovf >> 31) ? AUX_WIDE : 0u;
-            aux[c.b].out_size = (c.ovf >> 31) ? 0xffffffffu : c.out_end - c.lit_end + c.d->regen_size;   // sum of ml + regenerated literals
-        }
+        // hand-off: the block's records, verdict and sizes are in memory
+        if (c.active) fse_publish_ready(aux, c.b);
     }
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-    // verdicts; blocks the fast path gave up on are decoded again by the exact path
-#pragma unroll
-    for (int k = 0; k < (int)FSE_CHAINS; k++) {
-        FseChain &c = ch[k];
-        if (!c.active) continue;
-        if (!c.run) { aux[c.b].pad = c.st_seq; continue; }
-        if (!c.bad) continue;
-        const uint16_t *TL = tabs + (FSE_CHAINS * lane + k) * FSE_TAB_U16;
-        fse_exact_block(c.d, aux, c.b, input, seq_scratch, TL, TL + 512, TL + 1024, c.tl, c.to, c.tm, s_ll_base, s_ml_base, s_ll_bits, s_ml_bits, c.st_seq);
-    }
-    // hand-off: the block's records, verdict and sizes are in memory
-#pragma unroll
-    for (int k = 0; k < (int)FSE_CHAINS; k++)
-        if (ch[k].active) fse_publish_ready(aux, ch[k].b);
-#ifdef B200Z_PROBE
-    if (threadIdx.x == 0) atomicMax(&g_probe[1], probe_now());
-#endif
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -896,10 +822,7 @@ struct LitSrc { const uint8_t *p; uint32_t rle; uint8_t byte; uint32_t regen; };
 
 // exact sequential execution of up to 32 sequences held one per lane (my_ll/my_ml/my_of); `resolved` = offsets
 // already went through do_offset_history.  Returns 0 or an error code.
-#ifndef B200Z_EXEC_PER_LANE
-#define B200Z_EXEC_PER_LANE 2
-#endif
-constexpr uint32_t EXEC_PER_LANE = B200Z_EXEC_PER_LANE;      // consecutive sequences a lane holds (even)
+constexpr uint32_t EXEC_PER_LANE = 2;                       // consecutive sequences a lane holds (even)
 constexpr uint32_t EXEC_BATCH = 32 * EXEC_PER_LANE;         // sequences per batch
 // Sequence j of the batch lives in lane j / EXEC_PER_LANE, slot j % EXEC_PER_LANE.
 __device__ __forceinline__ uint32_t exec_pick(const uint32_t (&v)[EXEC_PER_LANE], uint32_t slot) {
@@ -992,42 +915,25 @@ __device__ __forceinline__ bool exec_wait_ready(const BlockAux *aux, uint32_t b,
     return __shfl_sync(0xffffffffu, ok, 0) != 0;
 }
 
-#ifndef B200Z_EXEC_WARPS
-#define B200Z_EXEC_WARPS 4
-#endif
-constexpr uint32_t EXEC_WARPS = B200Z_EXEC_WARPS;
-#ifndef B200Z_EXEC_TMAX
-#define B200Z_EXEC_TMAX 8128
-#endif
-constexpr uint32_t EXEC_TMAX = B200Z_EXEC_TMAX;             // most bytes one batch may produce on the fast path (sizes the end-bit mask)
-#ifndef B200Z_EXEC_CHUNK_ROWS
-#define B200Z_EXEC_CHUNK_ROWS 4
-#endif
-#ifndef B200Z_EXEC_PREFETCH
-#define B200Z_EXEC_PREFETCH 1
-#endif
-constexpr uint32_t EXEC_CHUNK_ROWS = B200Z_EXEC_CHUNK_ROWS;                    // rows (of 32 bytes) whose loads are in flight together
+constexpr uint32_t EXEC_WARPS = 4;
+constexpr uint32_t EXEC_TMAX = 8128;         // most bytes one batch may produce on the fast path (sizes the end-bit mask)
+constexpr uint32_t EXEC_CHUNK_ROWS = 4;      // rows (of 32 bytes) whose loads are in flight together
 constexpr uint32_t EXEC_MASK_WORDS = (EXEC_TMAX + 31) / 32 + EXEC_CHUNK_ROWS;
 // CTAs per SM the register budget must allow: 6 gives 80 registers (few spills).  On an H100 this runs k_exec ~19 % faster
 // than 8 (64 registers, ~190 bytes of spills per thread); 4 and 5 measure the same as 6.
-#ifndef B200Z_EXEC_MINB
-#define B200Z_EXEC_MINB 6
-#endif
+constexpr int EXEC_MINB = 6;
 
-__global__ void __launch_bounds__(EXEC_WARPS * 32, B200Z_EXEC_MINB) k_exec(const BlockDesc *__restrict__ descs, const BlockAux *__restrict__ aux,
+__global__ void __launch_bounds__(EXEC_WARPS * 32, EXEC_MINB) k_exec(const BlockDesc *__restrict__ descs, const BlockAux *__restrict__ aux,
                                                         const FrameDesc *__restrict__ frames, FrameState *__restrict__ states,
                                                         const uint8_t *__restrict__ input, const uint8_t *__restrict__ lit_scratch,
                                                         const uint32_t *__restrict__ seq_scratch, uint8_t *__restrict__ output, uint64_t output_cap,
-                                                        uint32_t nframes, uint32_t *__restrict__ resume, uint32_t frame_base) {
+                                                        uint32_t nframes, uint32_t *__restrict__ resume) {
     __shared__ uint32_t s_mask[EXEC_WARPS][EXEC_MASK_WORDS];
     __shared__ __align__(16) uint2 s_recs[EXEC_WARPS][EXEC_BATCH];
     __shared__ ExecState s_saved[EXEC_WARPS];   // the state at the current block's start (kept out of the registers: read only on a rollback)
-    const uint32_t f = frame_base + ((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    const uint32_t f = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const uint32_t lane = threadIdx.x & 31, lt = lanemask_lt();
     if (f >= nframes) return;
-#ifdef B200Z_PROBE
-    if (lane == 0) { const unsigned long long t = probe_now(); atomicMin(&g_probe[2], t); atomicMax(&g_probe[4], t); }
-#endif
     uint32_t a_mask = (uint32_t)__cvta_generic_to_shared(s_mask[threadIdx.x >> 5]);   // this warp's bitmask of sequence ends
     uint32_t a_recs = (uint32_t)__cvta_generic_to_shared(s_recs[threadIdx.x >> 5]);   // this warp's per-sequence records
     asm volatile("" : "+r"(a_mask), "+r"(a_recs));   // keep both addresses in registers (ptxas would recompute them from %tid per chunk)
@@ -1212,19 +1118,17 @@ __global__ void __launch_bounds__(EXEC_WARPS * 32, B200Z_EXEC_MINB) k_exec(const
                 const uint32_t nrows = (T + 31) >> 5;
                 // The batch's match sources are scattered over the frame's window, and with thousands of frames in flight the
                 // windows do not stay in L2: ask for the sectors now, a few hundred instructions before the rows need them.
-                if (B200Z_EXEC_PREFETCH) {
 #pragma unroll
-                    for (uint32_t k = 0; k < K; k++) {
-                        if (on[k]) {
-                            const uint8_t *src = out + st.produced + mstart[k] - offs[k];
-                            prefetch_l2(src);
-                            if ((((uint32_t)(uintptr_t)src) & 31u) + mls[k] > 32u) prefetch_l2(src + mls[k] - 1);
-                        }
+                for (uint32_t k = 0; k < K; k++) {
+                    if (on[k]) {
+                        const uint8_t *src = out + st.produced + mstart[k] - offs[k];
+                        prefetch_l2(src);
+                        if ((((uint32_t)(uintptr_t)src) & 31u) + mls[k] > 32u) prefetch_l2(src + mls[k] - 1);
                     }
-                    if (lane == 31 && lit.regen) {
-                        const uint32_t ahead = st.litpos + L + 256u;   // the literal stream is sequential: stay two lines ahead
-                        prefetch_l2(lit.p + (ahead < lit.regen ? ahead : lit.regen - 1));
-                    }
+                }
+                if (lane == 31 && lit.regen) {
+                    const uint32_t ahead = st.litpos + L + 256u;   // the literal stream is sequential: stay two lines ahead
+                    prefetch_l2(lit.p + (ahead < lit.regen ? ahead : lit.regen - 1));
                 }
                 sts32(a_mask + (lane << 2), 0u);
                 if (nrows > 32u - EXEC_CHUNK_ROWS)
@@ -1347,9 +1251,6 @@ __global__ void __launch_bounds__(EXEC_WARPS * 32, B200Z_EXEC_MINB) k_exec(const
         o.hist[0] = st.h0; o.hist[1] = st.h1; o.hist[2] = st.h2;
         o.status = status; o.produced = st.produced; o.counter = st.counter; o.error_block = err_block; o.blocks_done = blocks_done;
         if (resume) resume[f] = RESUME_SKIP;   // a later launch of this kernel in the same pass has nothing to do here
-#ifdef B200Z_PROBE
-        { const unsigned long long t = probe_now(); atomicMax(&g_probe[3], t); atomicMin(&g_probe[5], t); }
-#endif
     }
 }
 
@@ -1488,7 +1389,7 @@ int launch_predefined(FseSlot *predef, cudaStream_t s, uint64_t *launched) {
 }
 
 constexpr uint32_t kHufSmem = HUF_BLOCKS_PER_CTA * HUF_SMEM_PER_BLOCK + 32 * RING_STRIDE;
-constexpr uint32_t kFseSmem = FSE_BLOCKS_PER_CTA * FSE_TAB_U16 * 2 + 1024 + FSE_BLOCKS_PER_CTA * RING_STRIDE;
+constexpr uint32_t kFseSmem = FSE_LANES * FSE_TAB_U16 * 2 + 1024 + FSE_LANES * RING_STRIDE;
 
 static int g_num_sms[64];   // per device ordinal, filled by init_kernels
 
@@ -1528,10 +1429,9 @@ static int launch_exec(const PipelineArgs &a, cudaStream_t s, bool dependent_of_
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
-    static const bool no_pdl = [] { const char *e = getenv("B200Z_EXEC_PDL"); return e && e[0] == '0'; }();   // A/B knob: k_exec strictly after k_fse
-    cfg.attrs = attr; cfg.numAttrs = dependent_of_fse && !no_pdl ? 1 : 0;
+    cfg.attrs = attr; cfg.numAttrs = dependent_of_fse ? 1 : 0;
     const int e = (int)cudaLaunchKernelEx(&cfg, k_exec, a.descs, (const BlockAux *)a.aux, a.frames, a.states, a.input, (const uint8_t *)a.lit_scratch,
-                                          (const uint32_t *)a.seq_scratch, a.output, a.output_cap, a.nframes, a.resume, 0u);
+                                          (const uint32_t *)a.seq_scratch, a.output, a.output_cap, a.nframes, a.resume);
     if (!e) ++*launched;
     return e;
 }
@@ -1549,7 +1449,7 @@ int launch_stage(const PipelineArgs &a, int stage, cudaStream_t s, uint64_t *lau
             break;
         case 2:
             if (!a.nblocks) return 0;
-            k_fse<<<cdiv(a.nblocks, FSE_BLOCKS_PER_CTA), 32, kFseSmem, s>>>(a.descs, a.aux, a.input, a.seq_scratch, a.nblocks, a.fse_order);
+            k_fse<<<cdiv(a.nblocks, FSE_LANES), 32, kFseSmem, s>>>(a.descs, a.aux, a.input, a.seq_scratch, a.nblocks, a.fse_order);
             break;
         case 3:
             // frames whose blocks are assembled in shared memory: persistent CTAs, one per SM, frames from a ticket counter
