@@ -212,3 +212,41 @@ def symbolic_offsets(ll, of_raw):
             h[2] = h[1]; h[1] = h[0]; h[0] = actual
         out.append(actual)
     return np.array(out, dtype=np.uint64), h
+
+
+def run_frame(oracle, data, max_blocks=None, base=0x1005, strict=False):
+    """Runs the Compressed blocks of a frame through the model: the oracle's per-block traces ({ll, ml, offset_value},
+    literals) are turned into what k_fse hands over -- prefix-form records with symbolic offsets -- and each block's output
+    must be the reference's.  base: global address of the frame's first byte.  A block the model bails out of is skipped,
+    or fails the check when `strict`.  Returns (blocks run, sequences run)."""
+    d = oracle.FrameDecoder(); d.trace_enable()
+    r = d.reset(data); d.decode_blocks(r); out = d.collect()
+    blocks, lits, seqs = d.trace()
+    hist = [1, 4, 8]
+    pos = 0
+    nblk = nseq = 0
+    for tb in blocks:
+        size = tb["out_size"]
+        if tb["block_type"] == 2:
+            n = tb["num_sequences"]
+            s = seqs[tb["seq_offset"]:tb["seq_offset"] + n]
+            lit = lits[tb["lit_offset"]:tb["lit_offset"] + tb["regenerated_size"]]
+            sym, h_after = symbolic_offsets(s[:, 0], s[:, 2])
+            # symbols resolve to the reference's actual offsets, and the history carries over symbolically
+            got_actual = np.array([sym_resolve(int(v), hist) for v in sym], dtype=np.uint64)
+            assert np.array_equal(got_actual, s[:, 3].astype(np.uint64))
+            if max_blocks is None or nblk < max_blocks:
+                rec = to_prefix(s[:, 0], s[:, 1], sym)
+                try:
+                    got = exec_block(rec, hist, lit, out[:pos], base + pos)
+                    assert got == out[pos:pos + size], (nblk, size)
+                except Bail:
+                    if strict:
+                        raise
+                nblk += 1; nseq += n
+            if n:
+                hist = [sym_resolve(int(v), hist) for v in h_after]
+                assert hist == list(tb["offset_hist_after"])
+        pos += size
+    assert pos == len(out)
+    return nblk, nseq

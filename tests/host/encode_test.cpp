@@ -1,11 +1,14 @@
-// Host-side driver of zstd-rs_b200/csrc/encode.cuh (the block encoder k_cenc runs on the GPU), for tests/test_compress_host.py.
-//   encode_test IN OUT   IN = u32 nlit, nlit literal bytes, u32 nseq, nseq x {u32 ll, ml, of}
-//                        OUT = the content of a Compressed block for them
+// Host-side driver of zstd-rs_b200/csrc/encode.cuh (the block encoder k_cenc runs on the GPU), for tests/seqcraft.py.
+//   encode_test [--ov] IN OUT   IN = u32 nlit, nlit literal bytes, u32 nseq, nseq x {u32 ll, ml, of}
+//                               OUT = the content of a Compressed block for them
+// With --ov the third field is the zstd Offset_Value itself (1-3 are repeat codes): the encoder writes of + 3 with code
+// flog2(of + 3), so passing ov - 3 (mod 2^32) emits exactly ov.
 // It checks what the format needs of the tables -- Huffman lengths <= 11 with a complete code, FSE counts summing to 2^log --
 // and prints "ok <content size> <huffman literals 0/1> <LL mode> <OF mode> <ML mode>".
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
+#include <cstring>
 #include <vector>
 #include "../../zstd-rs_b200/csrc/encode.cuh"
 using namespace b200z;
@@ -13,7 +16,9 @@ using namespace b200z;
 #define CHECK(c) do { if (!(c)) { printf("FAIL %s:%d %s\n", __FILE__, __LINE__, #c); return 1; } } while (0)
 
 int main(int argc, char **argv) {
-    if (argc != 3) return 2;
+    const bool ov = argc == 4 && !strcmp(argv[1], "--ov");
+    if (argc != 3 && !ov) return 2;
+    argv += ov ? 1 : 0;
     FILE *f = fopen(argv[1], "rb");
     if (!f) return 2;
     uint32_t nlit = 0, nseq = 0;
@@ -23,6 +28,8 @@ int main(int argc, char **argv) {
     std::vector<SeqRec> seqs(nseq + 1);
     if (fread(seqs.data(), sizeof(SeqRec), nseq, f) != nseq) return 2;
     fclose(f);
+    if (ov)
+        for (uint32_t i = 0; i < nseq; i++) seqs[i].of -= 3;
     static EncScratch s;
     const uint32_t cap = 4 * ENC_BLOCK;
     std::vector<uint8_t> out(cap);

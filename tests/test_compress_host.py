@@ -1,21 +1,18 @@
 """CPU checks of the compressor's format layer: zstd-rs_b200/csrc/encode.cuh (the code k_cenc runs on the GPU) compiled for the
-host encodes crafted literal and sequence sets into Compressed blocks; each is wrapped in a frame here and must decode to the
+host encodes crafted literal and sequence sets into Compressed blocks (tests/seqcraft.py); each is wrapped in a frame and must decode to the
 expected bytes with the oracle (ruzstd's decode semantics) and with libzstd.  Also: compress_bound and the layout of the new
 C-ABI structs."""
 import os
 import random
-import shutil
-import struct
 import subprocess
 
 import pytest
 
 import datagen
+import seqcraft
 from conftest import ROOT
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-pytestmark = pytest.mark.skipif(not os.path.exists(NVCC), reason="nvcc not available")
+pytestmark = pytest.mark.skipif(not os.path.exists(seqcraft.NVCC), reason="nvcc not available")
 
 LL_BASE = [*range(16), 16, 18, 20, 22, 24, 28, 32, 40, 48, 64, *[1 << k for k in range(7, 17)]]
 LL_BITS = [0] * 16 + [1, 1, 1, 1, 2, 2, 3, 3, 4, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16]
@@ -23,58 +20,12 @@ ML_BASE = [*range(3, 35), 35, 37, 39, 41, 43, 47, 51, 59, 67, 83, 99, 131, 259, 
 ML_BITS = [0] * 32 + [1, 1, 1, 1, 2, 2, 3, 3, 4, 4, 5, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16]
 
 
-@pytest.fixture(scope="module")
-def encoder(tmp_path_factory):
-    exe = str(tmp_path_factory.mktemp("enc") / "encode_test")
-    subprocess.check_call([NVCC, "-x", "cu", "-std=c++17", "-O2", "-w", "-o", exe, os.path.join(HERE, "host", "encode_test.cpp")])
-    return exe
-
-
-def encode(exe, tmp_path, lits, seqs):
-    src, dst = tmp_path / "in.bin", tmp_path / "out.bin"
-    src.write_bytes(struct.pack("<I", len(lits)) + bytes(lits) + struct.pack("<I", len(seqs)) + b"".join(struct.pack("<3I", *q) for q in seqs))
-    out = subprocess.run([exe, str(src), str(dst)], capture_output=True, text=True, timeout=120)
-    assert out.returncode == 0 and out.stdout.startswith("ok"), out.stdout + out.stderr
-    f = out.stdout.split()
-    return dst.read_bytes(), int(f[2]), [int(x) for x in f[3:6]]
-
-
-def execute(history, lits, seqs):
-    out = bytearray(history)
-    li = 0
-    for ll, ml, of in seqs:
-        out += lits[li:li + ll]
-        li += ll
-        assert 1 <= of <= len(out)
-        start = len(out) - of
-        while ml > 0:   # overlapping copies repeat the last `of` bytes
-            chunk = out[start:start + min(ml, of)]
-            out += chunk
-            start += len(chunk)
-            ml -= len(chunk)
-    out += lits[li:]
-    return bytes(out[len(history):])
-
-
-def frame(history, content, plain_len):
-    total = len(history) + plain_len
-    hdr = struct.pack("<IBBI", 0xFD2FB528, 2 << 6, (17 - 10) << 3, total)
-    blocks = b""
-    for i in range(0, len(history), 131072):
-        piece = history[i:i + 131072]
-        blocks += struct.pack("<I", (len(piece) << 3))[:3] + piece
-    assert len(content) <= 131072
-    blocks += struct.pack("<I", 1 | (2 << 1) | (len(content) << 3))[:3] + content
-    return hdr + blocks
-
-
-def roundtrip(exe, tmp_path, oracle, lits, seqs, history=b""):
+def roundtrip(oracle, lits, seqs, history=b""):
     lits = bytes(lits)
-    content, huf, modes = encode(exe, tmp_path, lits, seqs)
-    plain = execute(history, lits, seqs)
-    assert len(plain) <= 131072
-    fr = frame(history, content, len(plain))
-    expect = history + plain
+    blocks = [("raw", history[i:i + 131072]) for i in range(0, len(history), 131072)] + [("cmp", lits, seqs)]
+    expect = seqcraft.execute(blocks)
+    assert expect is not seqcraft.ERROR and len(expect) - len(history) <= 131072
+    fr, [(huf, modes)] = seqcraft.frame(blocks)
     assert oracle.decode_frame(fr)[0] == expect
     assert datagen.decompress(fr, len(expect)) == expect
     return huf, modes
@@ -84,18 +35,18 @@ def skewed(rng, n, alphabet):
     return bytes(rng.choice(alphabet) for _ in range(n))
 
 
-def test_literals_distinct_counts(encoder, tmp_path, oracle):
+def test_literals_distinct_counts(oracle):
     rng = random.Random(1)
-    assert roundtrip(encoder, tmp_path, oracle, b"a" * 3000, [])[0] == 0          # one symbol: no Huffman table exists
-    assert roundtrip(encoder, tmp_path, oracle, b"a" * 700, [])[0] == 0           # <= 1024 literals: Raw
-    assert roundtrip(encoder, tmp_path, oracle, skewed(rng, 5000, b"ab"), [])[0] == 1
+    assert roundtrip(oracle, b"a" * 3000, [])[0] == 0          # one symbol: no Huffman table exists
+    assert roundtrip(oracle, b"a" * 700, [])[0] == 0           # <= 1024 literals: Raw
+    assert roundtrip(oracle, skewed(rng, 5000, b"ab"), [])[0] == 1
     lits = bytes(rng.choice(range(256)) if rng.random() < 0.3 else rng.choice(b"etaoin ") for _ in range(30000))
     assert len(set(lits)) == 256
-    assert roundtrip(encoder, tmp_path, oracle, lits, [])[0] == 1
-    assert roundtrip(encoder, tmp_path, oracle, os.urandom(20000), [])[0] == 0   # Huffman does not pay
+    assert roundtrip(oracle, lits, [])[0] == 1
+    assert roundtrip(oracle, os.urandom(20000), [])[0] == 0   # Huffman does not pay
 
 
-def test_literals_rare_symbol_and_length_limit(encoder, tmp_path, oracle):
+def test_literals_rare_symbol_and_length_limit(oracle):
     fib = [1, 1]
     while len(fib) < 21:
         fib.append(fib[-1] + fib[-2])
@@ -103,26 +54,26 @@ def test_literals_rare_symbol_and_length_limit(encoder, tmp_path, oracle):
     for s, c in enumerate(fib):   # Fibonacci counts: an unlimited Huffman code would be 20 bits deep
         lits += bytes([65 + s]) * c
     random.Random(2).shuffle(lits)
-    assert roundtrip(encoder, tmp_path, oracle, lits, [])[0] == 1
+    assert roundtrip(oracle, lits, [])[0] == 1
     lits = bytearray(b"e" * 50000 + b"t" * 30000 + b"\x07")
     random.Random(3).shuffle(lits)
-    assert roundtrip(encoder, tmp_path, oracle, lits, [])[0] == 1
+    assert roundtrip(oracle, lits, [])[0] == 1
 
 
-def test_literals_fse_compressed_weights(encoder, tmp_path, oracle):
+def test_literals_fse_compressed_weights(oracle):
     rng = random.Random(4)
     lits = bytes(min(255, int(rng.expovariate(1 / 40))) for _ in range(60000))   # symbols up to 255: > 128 weights
     assert max(lits) > 128
-    assert roundtrip(encoder, tmp_path, oracle, lits, [])[0] == 1
+    assert roundtrip(oracle, lits, [])[0] == 1
 
 
 @pytest.mark.parametrize("nseq", [1, 127, 128, 0x7EFF, 0x7F00, 0x7FFF, 0x8000, 40000])
-def test_sequence_counts(encoder, tmp_path, oracle, nseq):
+def test_sequence_counts(oracle, nseq):
     rng = random.Random(nseq)
     history = skewed(rng, 1000, b"abcdefgh")
     seqs = [(rng.choice([0, 0, 1]) if nseq < 40000 else 0, 3, rng.randint(1, 1000)) for _ in range(nseq)]
     lits = skewed(rng, sum(q[0] for q in seqs) + 5, b"xyz")
-    roundtrip(encoder, tmp_path, oracle, lits, seqs, history)
+    roundtrip(oracle, lits, seqs, history)
 
 
 def _values(bases, bits):
@@ -132,7 +83,7 @@ def _values(bases, bits):
     return sorted(set(vals))
 
 
-def test_every_ll_code_boundary(encoder, tmp_path, oracle):
+def test_every_ll_code_boundary(oracle):
     rng = random.Random(5)
     vals = _values(LL_BASE, LL_BITS)
     groups, cur = [], []
@@ -147,10 +98,10 @@ def test_every_ll_code_boundary(encoder, tmp_path, oracle):
             g = [131072 - 4]
         seqs = [(v, 4, rng.randint(1, 50)) for v in g]
         lits = skewed(rng, sum(g), b"0123456789")
-        roundtrip(encoder, tmp_path, oracle, lits, seqs, history=b"h" * 64)
+        roundtrip(oracle, lits, seqs, history=b"h" * 64)
 
 
-def test_every_ml_code_boundary(encoder, tmp_path, oracle):
+def test_every_ml_code_boundary(oracle):
     rng = random.Random(6)
     vals = _values(ML_BASE, ML_BITS)
     groups, cur = [], []
@@ -163,24 +114,24 @@ def test_every_ml_code_boundary(encoder, tmp_path, oracle):
     for g in groups:
         g = [min(v, 131072 - 1) for v in g]
         seqs = [(1, v, rng.randint(1, 64)) for v in g]
-        roundtrip(encoder, tmp_path, oracle, skewed(rng, len(g), b"xy"), seqs, history=bytes(range(64)))
+        roundtrip(oracle, skewed(rng, len(g), b"xy"), seqs, history=bytes(range(64)))
 
 
-def test_offsets_up_to_window(encoder, tmp_path, oracle):
+def test_offsets_up_to_window(oracle):
     rng = random.Random(7)
     history = os.urandom(131072)
     offs = [131072, 131071, 131000, 100000, 65536, 65535, 1 << 15, 4096, 5, 1]
     seqs = [(1, 6, o) for o in offs] + [(2, 5, rng.randint(1, 131072)) for _ in range(500)]
-    roundtrip(encoder, tmp_path, oracle, skewed(rng, 1600, b"pq"), seqs, history)
+    roundtrip(oracle, skewed(rng, 1600, b"pq"), seqs, history)
 
 
-def test_single_code_tables_are_rle(encoder, tmp_path, oracle):
+def test_single_code_tables_are_rle(oracle):
     seqs = [(0, 4, 5)] * 300
-    huf, modes = roundtrip(encoder, tmp_path, oracle, b"abcdefgh", seqs, history=b"12345678")
+    huf, modes = roundtrip(oracle, b"abcdefgh", seqs, history=b"12345678")
     assert modes == [1, 1, 1]
     seqs = [(0, 4, 5), (3, 40, 900)] * 200
     rng = random.Random(8)
-    huf, modes = roundtrip(encoder, tmp_path, oracle, skewed(rng, 600, b"abc"), seqs, history=bytes(1000))
+    huf, modes = roundtrip(oracle, skewed(rng, 600, b"abc"), seqs, history=bytes(1000))
     assert modes == [2, 2, 2]
 
 

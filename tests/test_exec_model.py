@@ -2,43 +2,9 @@
 the oracle's per-block traces ({ll, ml, offset_value}, literals) are turned into what k_fse hands over -- prefix-form
 records with symbolic offsets -- and executed by the model; the result must be the reference's output of that block."""
 import numpy as np
-import pytest
 
 from conftest import read_golden
 import emul_exec_cta as E
-
-
-def _run_frame(oracle, data, max_blocks=None, dict_bytes=None):
-    d = oracle.FrameDecoder(); d.trace_enable()
-    r = d.reset(data); d.decode_blocks(r); out = d.collect()
-    blocks, lits, seqs = d.trace()
-    hist = [1, 4, 8]
-    pos = 0
-    nblk = nseq = 0
-    for tb in blocks:
-        size = tb["out_size"]
-        if tb["block_type"] == 2:
-            n = tb["num_sequences"]
-            s = seqs[tb["seq_offset"]:tb["seq_offset"] + n]
-            lit = lits[tb["lit_offset"]:tb["lit_offset"] + tb["regenerated_size"]]
-            sym, h_after = E.symbolic_offsets(s[:, 0], s[:, 2])
-            # symbols resolve to the reference's actual offsets, and the history carries over symbolically
-            got_actual = np.array([E.sym_resolve(int(v), hist) for v in sym], dtype=np.uint64)
-            assert np.array_equal(got_actual, s[:, 3].astype(np.uint64))
-            if max_blocks is None or nblk < max_blocks:
-                rec = E.to_prefix(s[:, 0], s[:, 1], sym)
-                try:
-                    got = E.exec_block(rec, hist, lit, out[:pos], 0x1000 + pos + 5)
-                    assert got == out[pos:pos + size], (nblk, size)
-                except E.Bail:
-                    pass
-                nblk += 1; nseq += n
-            if n:
-                hist = [E.sym_resolve(int(v), hist) for v in h_after]
-                assert hist == list(tb["offset_hist_after"])
-        pos += size
-    assert pos == len(out)
-    return nblk, nseq
 
 
 def test_model_on_corpus_frames(oracle, manifest):
@@ -47,7 +13,7 @@ def test_model_on_corpus_frames(oracle, manifest):
     picked = [n for n in names if manifest["corpus"][n]["size"] < 40000][:14] + ["z000003.zst"]   # z000003: 137 small blocks, far sources into row 0
     nb = ns = 0
     for n in picked:
-        b, s = _run_frame(oracle, read_golden("decodecorpus", n))
+        b, s = E.run_frame(oracle, read_golden("decodecorpus", n))
         nb += b; ns += s
     assert nb > 20 and ns > 2000
 
@@ -64,7 +30,7 @@ def test_model_on_synthetic(oracle):
     lowent = bytes(rng.choice(np.arange(40, 56, dtype=np.uint8), 126000, p=np.arange(1, 17) / 136.0)) + text[:4000]
     for plain, mb in ((text, None), (runs, None), (chained, None), (lowent, None)):
         frame = G.compress(np.frombuffer(plain, dtype=np.uint8), level=3)
-        nb, ns = _run_frame(oracle, frame, mb)
+        nb, ns = E.run_frame(oracle, frame, mb)
         assert nb >= 1
 
 
