@@ -28,7 +28,7 @@ XC_BATCH = 1024          # k_exec_cta: sequences per batch
 FSE_FAST_XBITS = 38      # k_fse: most extra bits (LL + ML + OF) one sequence may carry on the fast path
 OVERLAP_LENGTHS = [3, 4, 31, 32, 33, 127, 128, 129, 300]
 
-# k_exec_cta's reasons for handing a frame back to k_exec (b200z_batch_debug_sched, api.cpp)
+# k_exec_cta's reasons for handing a frame back to k_exec, as b200z_batch_debug_sched reports them (XC_WHY_* in exec_cta.cuh)
 WHY_SEQ_RECORDS = 4      # raw offsets that cannot be resolved in place (values >= 2^30)
 WHY_BLOCK_SIZE = 8       # block sizes / literal counts it does not take
 WHY_SEQ_CHECK = 32       # sequence validation failed (offset 0, offset beyond the output)

@@ -705,7 +705,7 @@ static void fill_result(const b200z_batch *b, size_t i, const FrameState *st, b2
         if (b->checksummed) { r.has_calculated_checksum = 1; r.calculated_checksum = (uint32_t)st->xxh64; }
         return;
     }
-    r.status = (int32_t)(st->status & 0xffffu); r.stage = (int32_t)((st->status >> 16) & 0xffu); r.error_block = st->error_block;
+    r.status = (int32_t)status_code(st->status); r.stage = (int32_t)status_stage(st->status); r.error_block = st->error_block;
     // bytes_read_from_source at the point the reference returns the error (frame_decoder.rs:325-341)
     uint32_t j = st->blocks_done;
     uint64_t before = j > 0 ? b->block_end_bytes[fi.first_block_end + j - 1] : fi.hdr.header_size;
@@ -782,8 +782,7 @@ extern "C" int b200z_batch_debug_block_flags(b200z_batch *b, uint32_t block, uin
     return 0;
 }
 // execution scheduling counters of the LAST run: [0] frames given to k_exec_cta, [1] frames it handed back to k_exec,
-// [2] OR of the reasons (1 error status, 2 capacity, 4 raw/wide sequence records, 8 block size, 16 RLE literals that do not
-// fit, 32 sequence validation (dictionary reach, invalid offsets), 64 internal wait timed out, 128 frame state), [3] blocks left to k_exec
+// [2] OR of the reasons (XC_WHY_* in exec_cta.cuh), [3] blocks left to k_exec
 extern "C" int b200z_batch_debug_sched(b200z_batch *b, uint32_t out[4]) {
     if (!b || !out) return B200Z_ERR_INVALID_ARGUMENT;
     b200z_ctx *c = b->ctx;
@@ -1012,8 +1011,8 @@ extern "C" int b200z_decode_blocks_batch(b200z_ctx *c, const b200z_block_desc *b
             const BlockDesc &d = s.add_block(bd.src_off, bh, (uint32_t)f, k, hin + bd.src_off, nullptr, cur);
             if (bd.block_type == BT_COMPRESSED) {
                 // the descriptor says what the caller's parsers found: it must be what the content says
-                const bool lit_seen = !(d.host_status && (d.host_status >> 24) == 1 && d.lit_type == 0 && d.regen_size == 0 && d.lit_off == 0);
-                if (lit_seen && (d.lit_type != bd.literals_type || d.regen_size != bd.regenerated_size)) return B200Z_ERR_INVALID_ARGUMENT;
+                // the planner sets lit_off (>= 1) once it has parsed the literals header; an error before that leaves it 0
+                if (d.lit_off != 0 && (d.lit_type != bd.literals_type || d.regen_size != bd.regenerated_size)) return B200Z_ERR_INVALID_ARGUMENT;
                 if (!d.host_status && (d.nseq != bd.num_sequences || (d.nseq && d.modes != bd.modes))) return B200Z_ERR_INVALID_ARGUMENT;
             }
             if (d.host_status) break;   // decompress_block would have returned here: later blocks of the frame are never reached
@@ -1053,7 +1052,7 @@ extern "C" int b200z_decode_blocks_batch(b200z_ctx *c, const b200z_block_desc *b
             const int64_t si = sub_of[bf.first_block + k];
             const bool failed_here = fs.status && k == fs.error_block;
             if (si < 0 || (fs.status && k > fs.error_block)) { o.status = B200Z_BLOCK_NOT_REACHED; continue; }
-            if (failed_here) { o.status = (int32_t)(fs.status & 0xffffu); o.stage = (int32_t)((fs.status >> 16) & 0xffu); continue; }
+            if (failed_here) { o.status = (int32_t)status_code(fs.status); o.stage = (int32_t)status_stage(fs.status); continue; }
             const BlockDesc &d = s.descs[(size_t)si];
             o.out_size = d.btype == BT_COMPRESSED ? aux[(size_t)si].out_size : d.raw_size;
         }
@@ -1288,7 +1287,7 @@ static int fd_submit(b200z_frame_decoder *d, const TableCursor &cur, uint32_t *f
     CU(c, cudaStreamSynchronize(c->stream));
     uint64_t extra = 0;
     for (size_t i = 0; i < aux.size(); i++) {   // blocks after the first failing one are never executed (nor looked at by the reference)
-        if (s.descs[i].host_status || aux[i].status || aux[i].pad) break;
+        if (block_first_error(s.descs[i].host_status, aux[i].status, aux[i].seq_status)) break;
         extra += aux[i].out_size;
     }
     if ((e = fd_reserve_out(d, extra))) return e;
@@ -1324,7 +1323,7 @@ static int fd_submit(b200z_frame_decoder *d, const TableCursor &cur, uint32_t *f
     d->state = st;
     d->produced = st.produced;
     *done_blocks = st.blocks_done;
-    if (st.status) { *failed_block = st.blocks_done; d->last_stage = (int)((st.status >> 16) & 0xff); return (int)(st.status & 0xffff); }
+    if (st.status) { *failed_block = st.blocks_done; d->last_stage = (int)status_stage(st.status); return (int)status_code(st.status); }
     return 0;
 }
 
@@ -1344,7 +1343,7 @@ long slice_read(void *user, uint8_t *buf, size_t n) {  // impl Read for &[u8]
 static int fd_decode_blocks_impl(b200z_frame_decoder *d, b200z_read_fn rd, void *user, int strategy, size_t n, int *finished, SliceReader *slice) {
     if (!d || !rd) return B200Z_ERR_INVALID_ARGUMENT;
     if (!d->has_state) return fd_fail(d, B200Z_ERR_NOT_YET_INITIALIZED, 0);
-    if (d->state.status) return fd_fail(d, (int)(d->state.status & 0xffff), (int)((d->state.status >> 16) & 0xff));
+    if (d->state.status) return fd_fail(d, (int)status_code(d->state.status), (int)status_stage(d->state.status));
     const size_t buffer_size_before = fd_buffer_len(d);
     const size_t block_counter_before = d->block_counter;
     bool stop = false;

@@ -104,7 +104,7 @@ struct alignas(16) BlockDesc {
     uint32_t seq_off;        // offset of the sequences payload (after the 1-4 byte header) inside the block content
     uint32_t nseq;           // number of sequences
     uint32_t modes;          // compression modes byte
-    uint32_t host_status;    // error the planner found for this block (stage in bits 16..23), 0 = none
+    uint32_t host_status;    // error the planner found for this block (host_status()), 0 = none
     uint32_t block_in_frame; // ordinal of the block inside its frame
     uint32_t last;           // last block of the frame
     uint32_t pad0[5];
@@ -116,12 +116,12 @@ struct alignas(16) BlockDesc {
 
 // Per-block results written by the kernels
 struct alignas(16) BlockAux {
-    uint32_t status;         // first error of this block: code | stage << 16, 0 = ok
+    uint32_t status;         // literals-stage status (mk_status), 0 = ok
     uint32_t out_size;       // decompressed size of the block (known after sequence decode)
     uint32_t lit_streams_off;// offset inside the block content where the jump table / single stream starts
     uint32_t seq_bits_off;   // offset inside the block content where the sequence bitstream starts
     uint32_t sum_ll;         // sum of literal lengths over the block's sequences (mod 2^32)
-    uint32_t pad;            // sequence-stage status (code | stage << 16); literals-stage status is `status`
+    uint32_t seq_status;     // sequence-stage status (mk_status), 0 = ok; valid once `ready` is set
     uint32_t hist_after[3];  // offset history after the block (symbolic, seq_sym_*), unless AUX_RAW_OFFSETS
     uint32_t flags;          // AUX_*
     uint32_t ready;          // 1 once the block's sequence stage is over (k_fse): k_exec, launched as k_fse's programmatic
@@ -181,6 +181,23 @@ struct WalkBlock {
     uint8_t pad[6];
 };
 
+// ---- status words: code | stage << 16 (b200z_error, B200Z_STAGE_*), 0 = ok
 __host__ __device__ inline uint32_t mk_status(uint32_t code, uint32_t stage) { return code | (stage << 16); }
+__host__ __device__ inline uint32_t status_code(uint32_t s) { return s & 0xffffu; }
+__host__ __device__ inline uint32_t status_stage(uint32_t s) { return (s >> 16) & 0xffu; }
+// BlockDesc::host_status adds where the planner's error lies relative to the literals stage (bits 24..31), so that the device can
+// report a block's first error in the reference's order (block_first_error)
+constexpr uint32_t HS_BEFORE_LITERALS = 1, HS_AFTER_LITERALS = 2;
+__host__ __device__ inline uint32_t host_status(uint32_t code, uint32_t stage, uint32_t pos) { return mk_status(code, stage) | (pos << 24); }
+__host__ __device__ inline uint32_t host_status_pos(uint32_t hs) { return hs >> 24; }
+__host__ __device__ inline uint32_t host_status_word(uint32_t hs) { return hs & 0x00ffffffu; }
+// The first error of a block in the reference's order: a planner error before the literals stage, the literals stage
+// (BlockAux::status), any other planner error (sequences header), the sequence stage (BlockAux::seq_status).  0 = none.
+__host__ __device__ inline uint32_t block_first_error(uint32_t host_st, uint32_t lit_st, uint32_t seq_st) {
+    if (host_status_pos(host_st) == HS_BEFORE_LITERALS) return host_status_word(host_st);
+    if (lit_st) return lit_st;
+    if (host_st) return host_status_word(host_st);
+    return seq_st;
+}
 
 }  // namespace b200z

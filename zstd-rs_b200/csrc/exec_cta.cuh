@@ -51,6 +51,18 @@ static_assert(XC_SMEM_BYTES <= 232448, "k_exec_cta: more than 227 KiB of shared 
 static_assert(XC_MASK_BYTES >= XC_ROWS_MAX * 16 && XC_FIRST_BYTES >= XC_ROWS_MAX * 8, "k_exec_cta tables");
 constexpr uint32_t XC_SPIN_LIMIT = 1u << 18;               // bounded waits: a stuck wait turns into a bail-out, never a hang
 
+// Why a frame was handed back to k_exec: bits OR-ed into ticket[2], read by b200z_batch_debug_sched
+enum : uint32_t {
+    XC_WHY_ERROR = 1u,          // an error status (planner, literals or sequence stage)
+    XC_WHY_CAPACITY = 2u,       // the output does not fit
+    XC_WHY_SEQ_RECORDS = 4u,    // wide records, or raw offsets that cannot be resolved in place (values >= 2^30)
+    XC_WHY_BLOCK_SIZE = 8u,     // block sizes / literal counts it does not take
+    XC_WHY_RLE_LITERALS = 16u,  // RLE literals that do not fit beside the window
+    XC_WHY_SEQ_CHECK = 32u,     // sequence validation failed (dictionary reach, invalid offsets)
+    XC_WHY_TIMEOUT = 64u,       // an internal wait timed out
+    XC_WHY_FRAME_STATE = 128u,  // the frame arrived failed or with a dictionary
+};
+
 struct XcMisc {               // at XC_OFF_MISC
     unsigned long long mbar;  // literals bulk-copy barrier
     uint32_t ticket;
@@ -79,7 +91,6 @@ __device__ __forceinline__ void xc_bulk_wait0() { asm volatile("cp.async.bulk.wa
 __device__ __forceinline__ void xc_fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void xc_fence_cta() { asm volatile("fence.acq_rel.cta;" ::: "memory"); }
 __device__ __forceinline__ uint32_t xc_ld_acquire_shared(uint32_t a) { uint32_t v; asm volatile("ld.acquire.cta.shared::cta.u32 %0, [%1];" : "=r"(v) : "r"(a) : "memory"); return v; }
-__device__ __forceinline__ uint32_t xc_ld_cg_u32(const uint32_t *p) { uint32_t v; asm volatile("ld.global.cg.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
 __device__ __forceinline__ uint32_t xc_ldg_cg_u8(const uint8_t *p) { uint32_t v; asm volatile("ld.global.cg.u8 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
 
 // 8-byte ring record: lo = match start (window position, 18 bits) | literal delta << 18 (low 14 bits),
@@ -236,12 +247,12 @@ __device__ __forceinline__ XcLoad xc_load(const XcBlk &B, uint32_t k, uint32_t t
         const uint32_t i = i0 + q;
         L.out[q] = 0; L.lit[q] = 0; L.of[q] = 0;
         // (past the read-only data path: a raw-offset block's records were rewritten by this kernel a moment ago)
-        if (i < B.nseq) { const uint32_t *p = B.seqs + (uint64_t)i * 3; L.out[q] = xc_ld_cg_u32(p); L.lit[q] = xc_ld_cg_u32(p + 1); L.of[q] = xc_ld_cg_u32(p + 2); }
+        if (i < B.nseq) { const uint32_t *p = B.seqs + (uint64_t)i * 3; L.out[q] = ld_cg_u32(p); L.lit[q] = ld_cg_u32(p + 1); L.of[q] = ld_cg_u32(p + 2); }
         else if (i < B.ntot) { L.out[q] = B.out_size; L.lit[q] = B.regen; }   // trailing literals (sequence_execution.rs:40-44)
     }
     L.p_out = 0; L.p_lit = 0;
     // (no shuffle here: the loads stay in flight while the rows of the previous batch are produced)
-    if (lane == 0 && i0 != 0 && i0 <= B.nseq) { const uint32_t *p = B.seqs + (uint64_t)(i0 - 1) * 3; L.p_out = xc_ld_cg_u32(p); L.p_lit = xc_ld_cg_u32(p + 1); }
+    if (lane == 0 && i0 != 0 && i0 <= B.nseq) { const uint32_t *p = B.seqs + (uint64_t)(i0 - 1) * 3; L.p_out = ld_cg_u32(p); L.p_lit = ld_cg_u32(p + 1); }
     return L;
 }
 
@@ -335,18 +346,18 @@ __global__ void __launch_bounds__(XC_THREADS, 1) k_exec_cta(const BlockDesc *__r
         uint32_t blocks_done = fs.blocks_done;
         const uint32_t nblocks = fd.nblocks;
         bool bailed = fs.status != 0 || fd.dict != nullptr;
-        uint32_t why = bailed ? 128u : 0u;   // debug: why the frame was handed to k_exec (ticket[2] collects the OR, ticket[1] the count)
+        uint32_t why = bailed ? XC_WHY_FRAME_STATE : 0u;   // debug: why the frame was handed to k_exec (ticket[2] collects the OR, ticket[1] the count)
         bool fresh = true;   // no block of this frame has been stored by this CTA yet
         uint32_t bi = 0;
         for (; bi < nblocks && !bailed; bi++) {
             const uint32_t b = fd.first_block + bi;
             const BlockDesc &d = descs[b];
             const BlockAux &ax = aux[b];
-            if (d.host_status || ax.status) { bailed = true; why |= 1u; break; }
+            if (d.host_status || ax.status) { bailed = true; why |= XC_WHY_ERROR; break; }
             const uint32_t btype = d.btype;
             if (btype != BT_COMPRESSED) {
                 const uint32_t n = d.raw_size;
-                if (produced + n > cap) { bailed = true; why |= 2u; break; }
+                if (produced + n > cap) { bailed = true; why |= XC_WHY_CAPACITY; break; }
                 uint8_t *dst = out + produced;
                 if (btype == BT_RAW) { const uint8_t *srcp = input + d.src_off; for (uint32_t j = tid; j < n; j += XC_THREADS) dst[j] = srcp[j]; }
                 else { const uint8_t v = input[d.src_off]; for (uint32_t j = tid; j < n; j += XC_THREADS) dst[j] = v; }
@@ -357,7 +368,7 @@ __global__ void __launch_bounds__(XC_THREADS, 1) k_exec_cta(const BlockDesc *__r
                 continue;
             }
             const uint32_t nseq = d.nseq;
-            if (nseq && (ax.pad || (ax.flags & AUX_WIDE))) { bailed = true; why |= ax.pad ? 1u : 4u; break; }
+            if (nseq && (ax.seq_status || (ax.flags & AUX_WIDE))) { bailed = true; why |= ax.seq_status ? XC_WHY_ERROR : XC_WHY_SEQ_RECORDS; break; }
             if (nseq && (ax.flags & AUX_RAW_OFFSETS)) {
                 // k_fse's exact path left raw offset_values (a sequence with more extra bits than its fast path takes, an offset
                 // code >= 30, ...).  do_offset_history (sequence_execution.rs:59-118) is a serial walk: warp 0 runs it over the block's
@@ -366,7 +377,7 @@ __global__ void __launch_bounds__(XC_THREADS, 1) k_exec_cta(const BlockDesc *__r
                 uint32_t *sq = const_cast<uint32_t *>(seq_scratch) + d.seq_buf_off * 3;
                 uint32_t big = (h0 | h1 | h2) >> SEQ_SYM_SHIFT;   // values >= 2^30 cannot be told from symbols afterwards
                 for (uint32_t i = tid; i < nseq; i += XC_THREADS) big |= sq[3 * i + 2] >> SEQ_SYM_SHIFT;
-                if (__syncthreads_or((int)big)) { bailed = true; why |= 4u; break; }
+                if (__syncthreads_or((int)big)) { bailed = true; why |= XC_WHY_SEQ_RECORDS; break; }
                 if (warp == 0) {
                     uint32_t a0 = h0, a1 = h1, a2 = h2, prev_lit = 0;
                     for (uint32_t base = 0; base < nseq; base += 32) {
@@ -394,7 +405,7 @@ __global__ void __launch_bounds__(XC_THREADS, 1) k_exec_cta(const BlockDesc *__r
             }
             const uint32_t out_size = ax.out_size, regen = d.regen_size;
             const uint32_t sum_ll = nseq ? ax.sum_ll : 0u;
-            if (out_size > XC_WIN_MAX || produced + out_size > cap || sum_ll > regen || regen > out_size) { bailed = true; why |= produced + out_size > cap ? 2u : 8u; break; }
+            if (out_size > XC_WIN_MAX || produced + out_size > cap || sum_ll > regen || regen > out_size) { bailed = true; why |= produced + out_size > cap ? XC_WHY_CAPACITY : XC_WHY_BLOCK_SIZE; break; }
             if (out_size == 0) { blocks_done++; continue; }
             XcBlk B;
             B.S = S;
@@ -417,7 +428,7 @@ __global__ void __launch_bounds__(XC_THREADS, 1) k_exec_cta(const BlockDesc *__r
             const uint32_t lit_bytes = (loff + regen + 15u) & ~15u;
             // literals that do not fit beside the window are read from global memory byte by byte (a block that is nearly all literals)
             const bool litg = wbytes + lit_bytes > XC_DATA_BYTES;
-            if (litg && lt == LT_RLE) { bailed = true; why |= 16u; break; }
+            if (litg && lt == LT_RLE) { bailed = true; why |= XC_WHY_RLE_LITERALS; break; }
             B.lit_gp = litg ? lit_g + loff : nullptr;
             B.lit_s = wbytes + loff;
             const bool has_far = B.reach != 0;
@@ -502,7 +513,7 @@ __global__ void __launch_bounds__(XC_THREADS, 1) k_exec_cta(const BlockDesc *__r
                 }
                 blk_bail = misc->bail != 0;
             }
-            if (blk_bail) { bailed = true; why |= misc->bail == 2u ? 64u : 32u; break; }
+            if (blk_bail) { bailed = true; why |= misc->bail == 2u ? XC_WHY_TIMEOUT : XC_WHY_SEQ_CHECK; break; }
             // ---- head / tail bytes around the 16-byte aligned part
             {
                 const uint32_t head_end = min((B.woff + 15u) & ~15u, B.a_end);
@@ -511,7 +522,7 @@ __global__ void __launch_bounds__(XC_THREADS, 1) k_exec_cta(const BlockDesc *__r
                 else if (tid < 32) { const uint32_t a = tail_beg + (tid - 16u); if (a < B.a_end) B.gout[a - B.woff] = (uint8_t)lds8(S + a); }
             }
             if (nseq) {   // the history after the block, in terms of the history at its start (k_fse, symbolic)
-                const uint32_t a0 = xc_ld_cg_u32(&ax.hist_after[0]), a1 = xc_ld_cg_u32(&ax.hist_after[1]), a2 = xc_ld_cg_u32(&ax.hist_after[2]);
+                const uint32_t a0 = ld_cg_u32(&ax.hist_after[0]), a1 = ld_cg_u32(&ax.hist_after[1]), a2 = ld_cg_u32(&ax.hist_after[2]);
                 const uint32_t n0 = seq_sym_resolve(a0, h0, h1, h2), n1 = seq_sym_resolve(a1, h0, h1, h2), n2 = seq_sym_resolve(a2, h0, h1, h2);
                 h0 = n0; h1 = n1; h2 = n2;
             }

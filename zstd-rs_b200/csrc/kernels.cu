@@ -71,7 +71,7 @@ __global__ void __launch_bounds__(SETUP_WARPS * 32) k_setup(const BlockDesc *__r
     SetupScratch &sc = scratch[warp];
     const BlockDesc &d = descs[b];
     uint32_t st_lit = 0, st_seq = 0, lit_streams_off = 0, seq_bits_off = 0;
-    if (d.btype == BT_COMPRESSED && !(d.host_status && (d.host_status >> 24) == 1)) {
+    if (d.btype == BT_COMPRESSED && host_status_pos(d.host_status) != HS_BEFORE_LITERALS) {
         const uint8_t *content = input + d.src_off;
         if (!(parts & 1u)) {
         } else if (d.lit_type == LT_COMPRESSED) {
@@ -104,9 +104,9 @@ __global__ void __launch_bounds__(SETUP_WARPS * 32) k_setup(const BlockDesc *__r
     }
     if (lane == 0) {
         BlockAux &a = aux[b];
-        if (parts & 1u) { a.status = st_lit; a.lit_streams_off = lit_streams_off; }   // literals-stage status; the sequence-stage status travels in `pad` until k_exec orders them
+        if (parts & 1u) { a.status = st_lit; a.lit_streams_off = lit_streams_off; }
         if (parts & 2u) {
-            a.out_size = 0; a.seq_bits_off = seq_bits_off; a.sum_ll = 0; a.pad = st_seq;
+            a.out_size = 0; a.seq_bits_off = seq_bits_off; a.sum_ll = 0; a.seq_status = st_seq;
             a.hist_after[0] = a.hist_after[1] = a.hist_after[2] = 0; a.flags = 0; a.ready = 0; a.progress = 0;
         }
     }
@@ -383,7 +383,7 @@ __global__ void __launch_bounds__(32) k_huf(const BlockDesc *__restrict__ descs,
     if (active) {
         d = &descs[b];
         work = d->btype == BT_COMPRESSED && (d->lit_type == LT_COMPRESSED || d->lit_type == LT_TREELESS) &&
-               !(d->host_status && (d->host_status >> 24) == 1) && aux[b].status == 0;
+               host_status_pos(d->host_status) != HS_BEFORE_LITERALS && aux[b].status == 0;
         if (work) {
             slot = d->huf;
             if (slot == nullptr || slot->max_bits == 0) { err = B200Z_ERR_LIT_UNINITIALIZED_HUFFMAN_TABLE; work = false; }
@@ -656,7 +656,7 @@ __device__ __noinline__ void fse_exact_block(const BlockDesc *d, BlockAux *aux, 
         if (!err && br.p > 0) err = B200Z_ERR_SEQ_EXTRA_BITS;
         if (err) st_seq = mk_status(err, B200Z_STAGE_SEQUENCES);
     }
-    aux[b].pad = st_seq;
+    aux[b].seq_status = st_seq;
     aux[b].sum_ll = lit_end;
     aux[b].flags = AUX_RAW_OFFSETS | ((ovf >> 31) ? AUX_WIDE : 0u);
     aux[b].out_size = (ovf >> 31) ? 0xffffffffu : out_end - lit_end + d->regen_size;   // sum of ml + regenerated literals
@@ -691,7 +691,7 @@ __global__ void __launch_bounds__(32) k_fse(const BlockDesc *__restrict__ descs,
         c.d = c.active ? &descs[c.b] : nullptr;
         c.st_seq = 0; c.run = false; c.bad = false;
         if (c.active) {
-            c.st_seq = aux[c.b].pad;
+            c.st_seq = aux[c.b].seq_status;
             if (c.d->btype != BT_COMPRESSED) aux[c.b].out_size = c.d->raw_size;
             else if (!c.d->host_status && c.d->nseq == 0) aux[c.b].out_size = c.d->regen_size;
             c.run = c.d->btype == BT_COMPRESSED && !c.d->host_status && c.d->nseq != 0 && c.st_seq == 0;
@@ -770,7 +770,7 @@ __global__ void __launch_bounds__(32) k_fse(const BlockDesc *__restrict__ descs,
             }
             c.bad = c.flags != 0 || c.br.P != 0;
             if (!c.bad) {
-                aux[c.b].pad = 0;
+                aux[c.b].seq_status = 0;
                 aux[c.b].hist_after[0] = c.h0; aux[c.b].hist_after[1] = c.h1; aux[c.b].hist_after[2] = c.h2;
                 aux[c.b].sum_ll = c.lit_end;
                 aux[c.b].flags = (c.ovf >> 31) ? AUX_WIDE : 0u;
@@ -780,7 +780,7 @@ __global__ void __launch_bounds__(32) k_fse(const BlockDesc *__restrict__ descs,
         asm volatile("cp.async.wait_group 0;" ::: "memory");
         // verdict; a block the fast path gave up on is decoded again by the exact path
         if (c.active) {
-            if (!c.run) aux[c.b].pad = c.st_seq;
+            if (!c.run) aux[c.b].seq_status = c.st_seq;
             else if (c.bad) fse_exact_block(c.d, aux, c.b, input, seq_scratch, TL, TL + 512, TL + 1024, c.tl, c.to, c.tm, s_ll_base, s_ml_base, s_ll_bits, s_ml_bits, c.st_seq);
         }
         // hand-off: the block's records, verdict and sizes are in memory
@@ -893,26 +893,37 @@ __device__ __forceinline__ uint32_t ld_cg_u32(const uint32_t *p) {
     asm volatile("ld.global.cg.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
     return v;
 }
-// Block-granular hand-off from k_fse (fse_publish_ready): k_exec may be launched as k_fse's programmatic dependent and then
-// runs beside it; a frame's block is executed as soon as its sequence stage is over.  Bounded by wall clock (globaltimer),
-// generously: the producer always shows up (all of k_fse's CTAs are resident before k_exec's first one, programmatic
-// dependent launch), a timeout means the device is shared or being debugged -- it is reported as B200Z_ERR_CUDA for the
-// frame instead of hanging the GPU.  Warp-uniform result.
-__device__ __forceinline__ bool exec_wait_ready(const BlockAux *aux, uint32_t b, uint32_t lane) {
-    uint32_t ok = 1;
+// Hand-off from k_fse (fse_publish_progress / fse_publish_ready): k_exec may be launched as k_fse's programmatic dependent and
+// then runs beside it, consuming a block's records as they are published.  Lane 0 waits until `need` records of the block are
+// published or its sequence stage is over; the result is warp-uniform.  Bounded by wall clock (globaltimer), generously: the
+// producer always shows up (all of k_fse's CTAs are resident before k_exec's first one, programmatic dependent launch), a timeout
+// means the device is shared or being debugged -- it is reported as B200Z_ERR_CUDA for the frame instead of hanging the GPU.
+enum : uint32_t { WAIT_PROGRESS = 0, WAIT_READY = 1, WAIT_TIMEOUT = 2 };
+__device__ __forceinline__ uint32_t exec_wait(const BlockAux &a, uint32_t need, uint32_t lane, uint32_t &published) {
+    uint32_t fin = WAIT_PROGRESS, got = 0;
     if (lane == 0) {
-        if (ld_acquire_u32(&aux[b].ready) == 0u) {
-            unsigned long long t0, t1;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-            for (;;) {
-                __nanosleep(500);
-                if (ld_acquire_u32(&aux[b].ready) != 0u) break;
+        unsigned long long t0 = 0, t1;
+        for (uint32_t spins = 0;; spins++) {
+            if (ld_acquire_u32(&a.ready)) { fin = WAIT_READY; break; }
+            got = ld_acquire_u32(&a.progress);
+            if (got >= need) break;
+            __nanosleep(200);
+            if ((spins & 1023u) == 0) {
                 asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-                if (t1 - t0 > 20000000000ull) { ok = 0; break; }   // 20 s
+                if (t0 == 0) t0 = t1; else if (t1 - t0 > 20000000000ull) { fin = WAIT_TIMEOUT; break; }   // 20 s
             }
         }
     }
-    return __shfl_sync(0xffffffffu, ok, 0) != 0;
+    fin = __shfl_sync(0xffffffffu, fin, 0);
+    published = __shfl_sync(0xffffffffu, got, 0);
+    return fin;
+}
+// The sequence stage's verdict on a block whose BlockAux::ready is set: go on, failed (seq_status), or replay -- the exact path
+// rewrote the records with raw offsets (AUX_RAW_OFFSETS), so records consumed before the verdict were the wrong ones.
+enum : uint32_t { SEQ_GO = 0, SEQ_FAILED = 1, SEQ_REPLAY = 2 };
+__device__ __forceinline__ uint32_t exec_seq_verdict(const BlockAux &a, uint32_t &seq_status, uint32_t &flags) {
+    seq_status = ld_cg_u32(&a.seq_status); flags = ld_cg_u32(&a.flags);
+    return seq_status ? SEQ_FAILED : ((flags & AUX_RAW_OFFSETS) ? SEQ_REPLAY : SEQ_GO);
 }
 
 constexpr uint32_t EXEC_WARPS = 4;
@@ -953,24 +964,17 @@ __global__ void __launch_bounds__(EXEC_WARPS * 32, EXEC_MINB) k_exec(const Block
     for (uint32_t bi = first_bi; bi < fd.nblocks && !status; bi++) {
         const uint32_t b = fd.first_block + bi;
         const BlockDesc &d = descs[b];
-        // first error in the reference's order: header-level planner errors, literals, sequence header (planner),
-        // sequence tables + decode, then execution
-        uint32_t hs = d.host_status, hpos = hs >> 24;
-        hs &= 0x00ffffffu;
         // k_fse may still be running (this kernel is its programmatic dependent).  The literals stage is complete (stream order);
         // the sequence stage of this block is over once BlockAux::ready is set -- until then its records are consumed as the
         // fast path of k_fse publishes them (BlockAux::progress).  Results of k_fse are read past the L1.
-        const bool seq_block = d.btype == BT_COMPRESSED && d.nseq != 0 && !hs;
+        const bool seq_block = d.btype == BT_COMPRESSED && d.nseq != 0 && !d.host_status;
         bool known = !seq_block || __shfl_sync(0xffffffffu, lane == 0 ? ld_acquire_u32(&aux[b].ready) : 0u, 0) != 0u;   // the sequence stage's verdict is in
-        const uint32_t ax_status = ld_cg_u32(&aux[b].status);
-        uint32_t ax_pad = seq_block && known ? ld_cg_u32(&aux[b].pad) : 0u, ax_flags = seq_block && known ? ld_cg_u32(&aux[b].flags) : 0u;
-        uint32_t bs = 0;
-        if (hs && hpos == 1) bs = hs;
-        else if (ax_status) bs = ax_status;
-        else if (hs) bs = hs;
-        else if (ax_pad) bs = ax_pad;
+        uint32_t seq_st = 0, ax_flags = 0;
+        // (a replay verdict needs no replay here: nothing is consumed yet, the block runs on the raw offsets from the start)
+        if (seq_block && known) exec_seq_verdict(aux[b], seq_st, ax_flags);
         // a block whose sequence stage failed executes nothing: in the reference decode_sequences completes before
         // execute_sequences starts (block_decoder.rs:176-183)
+        const uint32_t bs = block_first_error(d.host_status, ld_cg_u32(&aux[b].status), seq_st);
         if (bs) { status = bs; err_block = d.block_in_frame; break; }
 
         if (d.btype == BT_RAW) {
@@ -990,254 +994,237 @@ __global__ void __launch_bounds__(EXEC_WARPS * 32, EXEC_MINB) k_exec(const Block
             // the block's start: where a sequence-stage error / a replay by the exact path rolls back to
             if (lane == 0) s_saved[threadIdx.x >> 5] = st;
             __syncwarp();
-            uint32_t redo = 0;            // 1: sequence-stage error after records were consumed, 2: the records were rewritten with raw offsets
-          exec_block_again:
-            st = s_saved[threadIdx.x >> 5];
-            st.litpos = 0;
-            uint32_t e = 0;
-            uint32_t avail = known ? 0xFFFFFFFFu : 0u;   // records that may be read
-            // block-level descriptor fields used inside the batch loop are consumed here once: a first use inside the loop
-            // would wait on a scoreboard shared with the record prefetch issued just before it (a full memory latency per batch)
-            uint32_t resolved_u = (ax_flags & AUX_RAW_OFFSETS) ? 0u : 1u, nseq_u = d.nseq;
-            const uint32_t *seqs = seq_scratch + d.seq_buf_off * 3;
-            asm volatile("" : "+r"(resolved_u), "+r"(nseq_u), "+l"(seqs));
-            const bool resolved = resolved_u != 0;
-            __syncwarp();
-            // A batch is EXEC_BATCH sequences, EXEC_PER_LANE consecutive ones per lane (contiguous 12-byte records in prefix
-            // form {out_end, lit_end, of}: ll and ml are differences of neighbouring records); the next batch's records are
-            // requested into L2 one batch ahead.
-            constexpr uint32_t K = EXEC_PER_LANE;
-            uint32_t carry_out = 0, carry_lit = 0;   // prefix sums at the end of the previous batch
-            const uint32_t bh0 = st.h0, bh1 = st.h1, bh2 = st.h2;   // history at the block's start: what the symbols refer to
-            for (uint32_t base = 0; base < nseq_u && !e; base += EXEC_BATCH) {
-                const uint32_t nb = nseq_u - base < EXEC_BATCH ? nseq_u - base : EXEC_BATCH;
-                if (avail < base + nb) {   // wait for k_fse: either these records, or the end of the block's sequence stage
-                    uint32_t got = 0, fin = 0;
-                    if (lane == 0) {
-                        unsigned long long t0 = 0, t1;
-                        for (uint32_t spins = 0;; spins++) {
-                            fin = ld_acquire_u32(&aux[b].ready);
-                            if (fin) break;
-                            got = ld_acquire_u32(&aux[b].progress);
-                            if (got >= base + nb) break;
-                            __nanosleep(200);
-                            if ((spins & 1023u) == 0) {
-                                asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-                                if (t0 == 0) t0 = t1; else if (t1 - t0 > 20000000000ull) { fin = 2; break; }   // 20 s: see exec_wait_ready
-                            }
+            uint32_t e, verdict, resolved_u, bh0, bh1, bh2;
+            do {   // once more when the exact path of k_fse rewrote the records the first run consumed
+                st = s_saved[threadIdx.x >> 5];
+                st.litpos = 0;
+                e = 0; verdict = SEQ_GO;
+                uint32_t avail = known ? 0xFFFFFFFFu : 0u;   // records that may be read
+                // block-level descriptor fields used inside the batch loop are consumed here once: a first use inside the loop
+                // would wait on a scoreboard shared with the record prefetch issued just before it (a full memory latency per batch)
+                resolved_u = (ax_flags & AUX_RAW_OFFSETS) ? 0u : 1u;
+                uint32_t nseq_u = d.nseq;
+                const uint32_t *seqs = seq_scratch + d.seq_buf_off * 3;
+                asm volatile("" : "+r"(resolved_u), "+r"(nseq_u), "+l"(seqs));
+                const bool resolved = resolved_u != 0;
+                __syncwarp();
+                // A batch is EXEC_BATCH sequences, EXEC_PER_LANE consecutive ones per lane (contiguous 12-byte records in prefix
+                // form {out_end, lit_end, of}: ll and ml are differences of neighbouring records); the next batch's records are
+                // requested into L2 one batch ahead.
+                constexpr uint32_t K = EXEC_PER_LANE;
+                uint32_t carry_out = 0, carry_lit = 0;   // prefix sums at the end of the previous batch
+                bh0 = st.h0; bh1 = st.h1; bh2 = st.h2;   // history at the block's start: what the symbols refer to
+                for (uint32_t base = 0; base < nseq_u && !e; base += EXEC_BATCH) {
+                    const uint32_t nb = nseq_u - base < EXEC_BATCH ? nseq_u - base : EXEC_BATCH;
+                    if (avail < base + nb) {   // wait for k_fse: either these records, or the end of the block's sequence stage
+                        const uint32_t w = exec_wait(aux[b], base + nb, lane, avail);
+                        if (w == WAIT_TIMEOUT) { e = B200Z_ERR_CUDA; break; }
+                        if (w == WAIT_READY) {
+                            known = true; avail = 0xFFFFFFFFu;
+                            verdict = exec_seq_verdict(aux[b], seq_st, ax_flags);
+                            if (verdict != SEQ_GO) break;
                         }
                     }
-                    fin = __shfl_sync(0xffffffffu, fin, 0); got = __shfl_sync(0xffffffffu, got, 0);
-                    if (fin == 2) { e = B200Z_ERR_CUDA; break; }
-                    if (fin) {
-                        known = true; avail = 0xFFFFFFFFu;
-                        ax_pad = ld_cg_u32(&aux[b].pad); ax_flags = ld_cg_u32(&aux[b].flags);
-                        if (ax_pad) { redo = 1; break; }
-                        if (ax_flags & AUX_RAW_OFFSETS) { redo = 2; break; }   // (the records consumed so far were symbolic: run the block again)
-                    } else avail = got;
-                }
-                uint32_t lls[K], mls[K], ofs[K], pe_out[K], pe_lit[K];
-                bool on[K];
-                const uint32_t old_out = carry_out, old_lit = carry_lit;
-                {
-                    const uint32_t *sp = seqs + (uint64_t)(base + K * lane) * 3;
-                    uint32_t raw[3 * K];
-                    if (K * lane + K <= nb) {   // all my records exist: K * 12 contiguous bytes, 8-byte aligned
-#pragma unroll
-                        for (uint32_t k = 0; k < 3 * K; k += 2) { const uint2 r = ld_cg_u32x2(sp + k); raw[k] = r.x; raw[k + 1] = r.y; }
-                    } else {
-#pragma unroll
+                    uint32_t lls[K], mls[K], ofs[K], pe_out[K], pe_lit[K];
+                    bool on[K];
+                    const uint32_t old_out = carry_out, old_lit = carry_lit;
+                    {
+                        const uint32_t *sp = seqs + (uint64_t)(base + K * lane) * 3;
+                        uint32_t raw[3 * K];
+                        if (K * lane + K <= nb) {   // all my records exist: K * 12 contiguous bytes, 8-byte aligned
+    #pragma unroll
+                            for (uint32_t k = 0; k < 3 * K; k += 2) { const uint2 r = ld_cg_u32x2(sp + k); raw[k] = r.x; raw[k + 1] = r.y; }
+                        } else {
+    #pragma unroll
+                            for (uint32_t k = 0; k < K; k++) {
+                                const bool have = K * lane + k < nb;
+                                raw[3 * k] = have ? ld_cg_u32(sp + 3 * k) : 0u; raw[3 * k + 1] = have ? ld_cg_u32(sp + 3 * k + 1) : 0u; raw[3 * k + 2] = have ? ld_cg_u32(sp + 3 * k + 2) : 1u;
+                            }
+                        }
+                        // prefix form -> lengths: my first record's predecessor is the last record of the lane below (or the carry)
+                        uint32_t p_out = __shfl_up_sync(0xffffffffu, raw[3 * (K - 1)], 1), p_lit = __shfl_up_sync(0xffffffffu, raw[3 * (K - 1) + 1], 1);
+                        if (lane == 0) { p_out = carry_out; p_lit = carry_lit; }
+    #pragma unroll
                         for (uint32_t k = 0; k < K; k++) {
-                            const bool have = K * lane + k < nb;
-                            raw[3 * k] = have ? ld_cg_u32(sp + 3 * k) : 0u; raw[3 * k + 1] = have ? ld_cg_u32(sp + 3 * k + 1) : 0u; raw[3 * k + 2] = have ? ld_cg_u32(sp + 3 * k + 2) : 1u;
+                            on[k] = K * lane + k < nb;
+                            const uint32_t ll = raw[3 * k + 1] - p_lit, ml = raw[3 * k] - p_out - ll;
+                            lls[k] = on[k] ? ll : 0u; mls[k] = on[k] ? ml : 0u; ofs[k] = raw[3 * k + 2];
+                            p_out = raw[3 * k]; p_lit = raw[3 * k + 1];
+                            pe_out[k] = p_out; pe_lit[k] = p_lit;
                         }
-                    }
-                    // prefix form -> lengths: my first record's predecessor is the last record of the lane below (or the carry)
-                    uint32_t p_out = __shfl_up_sync(0xffffffffu, raw[3 * (K - 1)], 1), p_lit = __shfl_up_sync(0xffffffffu, raw[3 * (K - 1) + 1], 1);
-                    if (lane == 0) { p_out = carry_out; p_lit = carry_lit; }
-#pragma unroll
-                    for (uint32_t k = 0; k < K; k++) {
-                        on[k] = K * lane + k < nb;
-                        const uint32_t ll = raw[3 * k + 1] - p_lit, ml = raw[3 * k] - p_out - ll;
-                        lls[k] = on[k] ? ll : 0u; mls[k] = on[k] ? ml : 0u; ofs[k] = raw[3 * k + 2];
-                        p_out = raw[3 * k]; p_lit = raw[3 * k + 1];
-                        pe_out[k] = p_out; pe_lit[k] = p_lit;
-                    }
-                    {   // carry: the batch's last record
-                        const uint32_t lastl = (nb - 1) / K, lasts = (nb - 1) % K;
-                        uint32_t co = raw[0], cl = raw[1];
-#pragma unroll
-                        for (uint32_t k = 1; k < K; k++) { co = lasts == k ? raw[3 * k] : co; cl = lasts == k ? raw[3 * k + 1] : cl; }
-                        carry_out = __shfl_sync(0xffffffffu, co, lastl); carry_lit = __shfl_sync(0xffffffffu, cl, lastl);
-                    }
-                    if (base + EXEC_BATCH < nseq_u && lane * 128u < (nseq_u - base - EXEC_BATCH) * 12u && lane * 128u < EXEC_BATCH * 12u)
-                        prefetch_l2(reinterpret_cast<const uint8_t *>(seqs + (uint64_t)(base + EXEC_BATCH) * 3) + lane * 128u);
-                }
-                // the records are prefix sums already (k_fse): batch totals and batch-relative positions are differences
-                const uint32_t T = carry_out - old_out, L = carry_lit - old_lit;
-                // per sequence: inclusive end of its bytes, start of its match, inclusive end of its literals (all batch-relative)
-                uint32_t oend[K], mstart[K], lend[K];
-#pragma unroll
-                for (uint32_t k = 0; k < K; k++) { oend[k] = on[k] ? pe_out[k] - old_out : T; lend[k] = on[k] ? pe_lit[k] - old_lit : L; mstart[k] = oend[k] - mls[k]; }
-                // actual offsets: symbols resolve against the history at the block's start; a block flagged AUX_RAW_OFFSETS
-                // (exact path of k_fse) runs do_offset_history here, sequence by sequence
-                uint32_t offs[K];
-#pragma unroll
-                for (uint32_t k = 0; k < K; k++) offs[k] = resolved ? seq_sym_resolve(ofs[k], bh0, bh1, bh2) : ofs[k];
-                uint32_t h0 = st.h0, h1 = st.h1, h2 = st.h2;
-                if (!resolved) {
-                    // cheap scalar steps (sequence_execution.rs:59-118); committed only if the fast path is taken (the exact path
-                    // redoes the steps itself)
-                    for (uint32_t j = 0; j < nb; j++) {
-                        const uint32_t slot = j % K, src_lane = j / K;
-                        uint32_t ll = __shfl_sync(0xffffffffu, exec_pick(lls, slot), src_lane), of = __shfl_sync(0xffffffffu, exec_pick(ofs, slot), src_lane);
-                        uint32_t actual = offset_history_step(of, ll, h0, h1, h2);
-                        if (lane == src_lane) {
-#pragma unroll
-                            for (uint32_t k = 0; k < K; k++) offs[k] = slot == k ? actual : offs[k];
+                        {   // carry: the batch's last record
+                            const uint32_t lastl = (nb - 1) / K, lasts = (nb - 1) % K;
+                            uint32_t co = raw[0], cl = raw[1];
+    #pragma unroll
+                            for (uint32_t k = 1; k < K; k++) { co = lasts == k ? raw[3 * k] : co; cl = lasts == k ? raw[3 * k + 1] : cl; }
+                            carry_out = __shfl_sync(0xffffffffu, co, lastl); carry_lit = __shfl_sync(0xffffffffu, cl, lastl);
                         }
+                        if (base + EXEC_BATCH < nseq_u && lane * 128u < (nseq_u - base - EXEC_BATCH) * 12u && lane * 128u < EXEC_BATCH * 12u)
+                            prefetch_l2(reinterpret_cast<const uint8_t *>(seqs + (uint64_t)(base + EXEC_BATCH) * 3) + lane * 128u);
                     }
-                }
-                const uint64_t reach = st.produced - st.drained;   // bytes of earlier output a match may reach back into
-                bool ok = true, ovl = false;
-#pragma unroll
-                for (uint32_t k = 0; k < K; k++) {
-                    ok = ok && (!on[k] || (offs[k] != 0 && (uint64_t)offs[k] <= reach + mstart[k]));
-                    ovl = ovl || offs[k] < mls[k];
-                }
-                const bool fast = __all_sync(0xffffffffu, ok) && T <= EXEC_TMAX && (uint64_t)st.litpos + L <= lit.regen && st.produced + T <= st.cap && !lit.rle;
-                if (!fast) {
-                    e = exec_batch_exact(st, lit, fd, out, nb, lls, mls, resolved ? offs : ofs, resolved, lane);
-                    continue;
-                }
-                if (!resolved) { st.h0 = h0; st.h1 = h1; st.h2 = h2; }
-                // ---------------- fast path
-                // Sequence j owns the bytes [lit_begin_j, out_end_j): its literal run, then its match.  A bit is set at
-                // the last byte of every sequence, so the owner of output byte q is the number of set bits below q;
-                // one 8-byte shared-memory record per sequence then tells the byte where it comes from.
-                const uint32_t nrows = (T + 31) >> 5;
-                // The batch's match sources are scattered over the frame's window, and with thousands of frames in flight the
-                // windows do not stay in L2: ask for the sectors now, a few hundred instructions before the rows need them.
-#pragma unroll
-                for (uint32_t k = 0; k < K; k++) {
-                    if (on[k]) {
-                        const uint8_t *src = out + st.produced + mstart[k] - offs[k];
-                        prefetch_l2(src);
-                        if ((((uint32_t)(uintptr_t)src) & 31u) + mls[k] > 32u) prefetch_l2(src + mls[k] - 1);
-                    }
-                }
-                if (lane == 31 && lit.regen) {
-                    const uint32_t ahead = st.litpos + L + 256u;   // the literal stream is sequential: stay two lines ahead
-                    prefetch_l2(lit.p + (ahead < lit.regen ? ahead : lit.regen - 1));
-                }
-                sts32(a_mask + (lane << 2), 0u);
-                if (nrows > 32u - EXEC_CHUNK_ROWS)
-                    for (uint32_t w = lane + 32; w < ((nrows + EXEC_CHUNK_ROWS - 1u) & ~(EXEC_CHUNK_ROWS - 1u)); w += 32) sts32(a_mask + (w << 2), 0u);
-                // 8-byte record: literal byte q of the sequence is literal number (q - m_before) of the batch (m_before = match bytes
-                // of the earlier sequences = match start - literal end), match byte q comes from output position q - offset
-                // (m_start, m_before <= EXEC_TMAX: 16 bits each)
-#pragma unroll
-                for (uint32_t k = 0; k < K; k += 2)
-                    sts128(a_recs + ((K * lane + k) << 3), mstart[k] | ((mstart[k] - lend[k]) << 16), offs[k], mstart[k + 1] | ((mstart[k + 1] - lend[k + 1]) << 16), offs[k + 1]);
-                const bool has_ovl = __any_sync(0xffffffffu, ovl);   // some match overlaps its own output (rare)
-                __syncwarp();
-#pragma unroll
-                for (uint32_t k = 0; k < K; k++)
-                    if (on[k]) red_or_shared(a_mask + (((oend[k] - 1) >> 5) << 2), 1u << ((oend[k] - 1) & 31u));
-                __syncwarp();
-                uint8_t *bout = out + st.produced;
-                const uint8_t *litq = lit.p + st.litpos;
-                asm volatile("" : "+l"(bout), "+l"(litq));   // keep both bases as single 64-bit registers (one add per access)
-                uint32_t before = 0;   // sequences ended in earlier rows
-                // Rows are produced EXEC_CHUNK_ROWS at a time: every byte whose source lies before the chunk (literals, and
-                // matches reaching back past the chunk start) is loaded first -- EXEC_CHUNK_ROWS independent loads per lane in
-                // flight -- then stored; the few bytes whose source lies inside the chunk follow, row by row.  (Issuing the
-                // next chunk's loads before this chunk's stores was measured slower: more bytes turn dependent.)
-                // The per-byte work is branch-free: one select between the literal and the match source.
-                // tag: TAG_NONE = nothing to do, TAG_STORE = value loaded, otherwise the (batch-relative, >= floor) source
-                // position of a match byte that had to wait.
-                constexpr int32_t TAG_NONE = INT32_MIN, TAG_STORE = INT32_MIN + 1;
-                constexpr int R = (int)EXEC_CHUNK_ROWS;
-                auto load_chunk = [&](uint32_t r0, int32_t floor, uint32_t (&val)[R], int32_t (&tag)[R]) {
-#pragma unroll
-                    for (int i = 0; i < R; i++) {
-                        const uint32_t q = ((r0 + i) << 5) + lane;
-                        const uint32_t word = lds32(a_mask + ((r0 + i) << 2));
-                        const uint32_t owner = before + __popc(word & lt);   // sequences that ended below q
-                        before += __popc(word);
-                        const uint2 rc = lds64(a_recs + ((owner & (EXEC_BATCH - 1u)) << 3));
-                        const uint32_t mst = rc.x & 0xffffu;
-                        const bool is_match = q >= mst;
-                        int32_t sp = (int32_t)q - (int32_t)rc.y;                  // batch-relative source of a match byte
-                        if (has_ovl) {                                            // overlapping match: byte k comes from k mod offset
-                            const uint32_t kk = q - mst;
-                            if (is_match && kk >= rc.y) sp = (int32_t)mst - (int32_t)rc.y + (int32_t)(kk % rc.y);
-                        }
-                        const bool valid = q < T;
-                        const bool dep = is_match && sp >= floor;
-                        const int32_t idx = is_match ? sp : (int32_t)(q - (rc.x >> 16));
-                        const uint8_t *bp = is_match ? (const uint8_t *)bout : litq;
-                        tag[i] = valid ? (dep ? sp : TAG_STORE) : TAG_NONE;
-                        val[i] = 0;
-                        if (valid && !dep) val[i] = bp[idx];
-                    }
-                };
-                auto store_chunk = [&](uint32_t r0, int32_t floor, const uint32_t (&val)[R], const int32_t (&tag)[R]) {
-#pragma unroll
-                    for (int i = 0; i < R; i++)
-                        if (tag[i] == TAG_STORE) bout[((r0 + i) << 5) + lane] = (uint8_t)val[i];
-                    // dependent bytes, rows in order (sources in earlier rows are final, inside the row the lowest pending byte is ready)
-                    bool anydep = false;
-#pragma unroll
-                    for (int i = 0; i < R; i++) anydep |= tag[i] >= floor;
-                    if (__any_sync(0xffffffffu, anydep)) {
-#pragma unroll
-                        for (int i = 0; i < R; i++) {
-                            bool mine = tag[i] >= floor;
-                            uint32_t pending = __ballot_sync(0xffffffffu, mine);
-                            const int32_t row0 = (int32_t)((r0 + i) << 5);
-                            while (pending) {
-                                __syncwarp();
-                                bool ready = mine && (tag[i] < row0 || !((pending >> (tag[i] - row0)) & 1u));
-                                if (ready) { bout[row0 + (int32_t)lane] = bout[tag[i]]; mine = false; }
-                                pending &= ~__ballot_sync(0xffffffffu, ready);
+                    // the records are prefix sums already (k_fse): batch totals and batch-relative positions are differences
+                    const uint32_t T = carry_out - old_out, L = carry_lit - old_lit;
+                    // per sequence: inclusive end of its bytes, start of its match, inclusive end of its literals (all batch-relative)
+                    uint32_t oend[K], mstart[K], lend[K];
+    #pragma unroll
+                    for (uint32_t k = 0; k < K; k++) { oend[k] = on[k] ? pe_out[k] - old_out : T; lend[k] = on[k] ? pe_lit[k] - old_lit : L; mstart[k] = oend[k] - mls[k]; }
+                    // actual offsets: symbols resolve against the history at the block's start; a block flagged AUX_RAW_OFFSETS
+                    // (exact path of k_fse) runs do_offset_history here, sequence by sequence
+                    uint32_t offs[K];
+    #pragma unroll
+                    for (uint32_t k = 0; k < K; k++) offs[k] = resolved ? seq_sym_resolve(ofs[k], bh0, bh1, bh2) : ofs[k];
+                    uint32_t h0 = st.h0, h1 = st.h1, h2 = st.h2;
+                    if (!resolved) {
+                        // cheap scalar steps (sequence_execution.rs:59-118); committed only if the fast path is taken (the exact path
+                        // redoes the steps itself)
+                        for (uint32_t j = 0; j < nb; j++) {
+                            const uint32_t slot = j % K, src_lane = j / K;
+                            uint32_t ll = __shfl_sync(0xffffffffu, exec_pick(lls, slot), src_lane), of = __shfl_sync(0xffffffffu, exec_pick(ofs, slot), src_lane);
+                            uint32_t actual = offset_history_step(of, ll, h0, h1, h2);
+                            if (lane == src_lane) {
+    #pragma unroll
+                                for (uint32_t k = 0; k < K; k++) offs[k] = slot == k ? actual : offs[k];
                             }
                         }
+                    }
+                    const uint64_t reach = st.produced - st.drained;   // bytes of earlier output a match may reach back into
+                    bool ok = true, ovl = false;
+    #pragma unroll
+                    for (uint32_t k = 0; k < K; k++) {
+                        ok = ok && (!on[k] || (offs[k] != 0 && (uint64_t)offs[k] <= reach + mstart[k]));
+                        ovl = ovl || offs[k] < mls[k];
+                    }
+                    const bool fast = __all_sync(0xffffffffu, ok) && T <= EXEC_TMAX && (uint64_t)st.litpos + L <= lit.regen && st.produced + T <= st.cap && !lit.rle;
+                    if (!fast) {
+                        e = exec_batch_exact(st, lit, fd, out, nb, lls, mls, resolved ? offs : ofs, resolved, lane);
+                        continue;
+                    }
+                    if (!resolved) { st.h0 = h0; st.h1 = h1; st.h2 = h2; }
+                    // ---------------- fast path
+                    // Sequence j owns the bytes [lit_begin_j, out_end_j): its literal run, then its match.  A bit is set at
+                    // the last byte of every sequence, so the owner of output byte q is the number of set bits below q;
+                    // one 8-byte shared-memory record per sequence then tells the byte where it comes from.
+                    const uint32_t nrows = (T + 31) >> 5;
+                    // The batch's match sources are scattered over the frame's window, and with thousands of frames in flight the
+                    // windows do not stay in L2: ask for the sectors now, a few hundred instructions before the rows need them.
+    #pragma unroll
+                    for (uint32_t k = 0; k < K; k++) {
+                        if (on[k]) {
+                            const uint8_t *src = out + st.produced + mstart[k] - offs[k];
+                            prefetch_l2(src);
+                            if ((((uint32_t)(uintptr_t)src) & 31u) + mls[k] > 32u) prefetch_l2(src + mls[k] - 1);
+                        }
+                    }
+                    if (lane == 31 && lit.regen) {
+                        const uint32_t ahead = st.litpos + L + 256u;   // the literal stream is sequential: stay two lines ahead
+                        prefetch_l2(lit.p + (ahead < lit.regen ? ahead : lit.regen - 1));
+                    }
+                    sts32(a_mask + (lane << 2), 0u);
+                    if (nrows > 32u - EXEC_CHUNK_ROWS)
+                        for (uint32_t w = lane + 32; w < ((nrows + EXEC_CHUNK_ROWS - 1u) & ~(EXEC_CHUNK_ROWS - 1u)); w += 32) sts32(a_mask + (w << 2), 0u);
+                    // 8-byte record: literal byte q of the sequence is literal number (q - m_before) of the batch (m_before = match bytes
+                    // of the earlier sequences = match start - literal end), match byte q comes from output position q - offset
+                    // (m_start, m_before <= EXEC_TMAX: 16 bits each)
+    #pragma unroll
+                    for (uint32_t k = 0; k < K; k += 2)
+                        sts128(a_recs + ((K * lane + k) << 3), mstart[k] | ((mstart[k] - lend[k]) << 16), offs[k], mstart[k + 1] | ((mstart[k + 1] - lend[k + 1]) << 16), offs[k + 1]);
+                    const bool has_ovl = __any_sync(0xffffffffu, ovl);   // some match overlaps its own output (rare)
+                    __syncwarp();
+    #pragma unroll
+                    for (uint32_t k = 0; k < K; k++)
+                        if (on[k]) red_or_shared(a_mask + (((oend[k] - 1) >> 5) << 2), 1u << ((oend[k] - 1) & 31u));
+                    __syncwarp();
+                    uint8_t *bout = out + st.produced;
+                    const uint8_t *litq = lit.p + st.litpos;
+                    asm volatile("" : "+l"(bout), "+l"(litq));   // keep both bases as single 64-bit registers (one add per access)
+                    uint32_t before = 0;   // sequences ended in earlier rows
+                    // Rows are produced EXEC_CHUNK_ROWS at a time: every byte whose source lies before the chunk (literals, and
+                    // matches reaching back past the chunk start) is loaded first -- EXEC_CHUNK_ROWS independent loads per lane in
+                    // flight -- then stored; the few bytes whose source lies inside the chunk follow, row by row.  (Issuing the
+                    // next chunk's loads before this chunk's stores was measured slower: more bytes turn dependent.)
+                    // The per-byte work is branch-free: one select between the literal and the match source.
+                    // tag: TAG_NONE = nothing to do, TAG_STORE = value loaded, otherwise the (batch-relative, >= floor) source
+                    // position of a match byte that had to wait.
+                    constexpr int32_t TAG_NONE = INT32_MIN, TAG_STORE = INT32_MIN + 1;
+                    constexpr int R = (int)EXEC_CHUNK_ROWS;
+                    auto load_chunk = [&](uint32_t r0, int32_t floor, uint32_t (&val)[R], int32_t (&tag)[R]) {
+    #pragma unroll
+                        for (int i = 0; i < R; i++) {
+                            const uint32_t q = ((r0 + i) << 5) + lane;
+                            const uint32_t word = lds32(a_mask + ((r0 + i) << 2));
+                            const uint32_t owner = before + __popc(word & lt);   // sequences that ended below q
+                            before += __popc(word);
+                            const uint2 rc = lds64(a_recs + ((owner & (EXEC_BATCH - 1u)) << 3));
+                            const uint32_t mst = rc.x & 0xffffu;
+                            const bool is_match = q >= mst;
+                            int32_t sp = (int32_t)q - (int32_t)rc.y;                  // batch-relative source of a match byte
+                            if (has_ovl) {                                            // overlapping match: byte k comes from k mod offset
+                                const uint32_t kk = q - mst;
+                                if (is_match && kk >= rc.y) sp = (int32_t)mst - (int32_t)rc.y + (int32_t)(kk % rc.y);
+                            }
+                            const bool valid = q < T;
+                            const bool dep = is_match && sp >= floor;
+                            const int32_t idx = is_match ? sp : (int32_t)(q - (rc.x >> 16));
+                            const uint8_t *bp = is_match ? (const uint8_t *)bout : litq;
+                            tag[i] = valid ? (dep ? sp : TAG_STORE) : TAG_NONE;
+                            val[i] = 0;
+                            if (valid && !dep) val[i] = bp[idx];
+                        }
+                    };
+                    auto store_chunk = [&](uint32_t r0, int32_t floor, const uint32_t (&val)[R], const int32_t (&tag)[R]) {
+    #pragma unroll
+                        for (int i = 0; i < R; i++)
+                            if (tag[i] == TAG_STORE) bout[((r0 + i) << 5) + lane] = (uint8_t)val[i];
+                        // dependent bytes, rows in order (sources in earlier rows are final, inside the row the lowest pending byte is ready)
+                        bool anydep = false;
+    #pragma unroll
+                        for (int i = 0; i < R; i++) anydep |= tag[i] >= floor;
+                        if (__any_sync(0xffffffffu, anydep)) {
+    #pragma unroll
+                            for (int i = 0; i < R; i++) {
+                                bool mine = tag[i] >= floor;
+                                uint32_t pending = __ballot_sync(0xffffffffu, mine);
+                                const int32_t row0 = (int32_t)((r0 + i) << 5);
+                                while (pending) {
+                                    __syncwarp();
+                                    bool ready = mine && (tag[i] < row0 || !((pending >> (tag[i] - row0)) & 1u));
+                                    if (ready) { bout[row0 + (int32_t)lane] = bout[tag[i]]; mine = false; }
+                                    pending &= ~__ballot_sync(0xffffffffu, ready);
+                                }
+                            }
+                        }
+                        __syncwarp();
+                    };
+                    for (uint32_t r0 = 0; r0 < nrows; r0 += R) {
+                        uint32_t va[R]; int32_t ta[R];
+                        load_chunk(r0, (int32_t)(r0 << 5), va, ta);
+                        store_chunk(r0, (int32_t)(r0 << 5), va, ta);
                     }
                     __syncwarp();
-                };
-                for (uint32_t r0 = 0; r0 < nrows; r0 += R) {
-                    uint32_t va[R]; int32_t ta[R];
-                    load_chunk(r0, (int32_t)(r0 << 5), va, ta);
-                    store_chunk(r0, (int32_t)(r0 << 5), va, ta);
+                    st.produced += T; st.counter += T; st.litpos += L;
                 }
-                __syncwarp();
-                st.produced += T; st.counter += T; st.litpos += L;
-            }
-            if (!e && st.litpos < lit.regen) {
-                uint32_t rest = lit.regen - st.litpos;
-                if (st.produced + rest > st.cap) e = B200Z_ERR_TARGET_TOO_SMALL;
-                else {
-                    if (lit.rle) warp_fill(out + st.produced, lit.byte, rest, lane); else warp_copy(out + st.produced, lit.p + st.litpos, rest, lane);
-                    st.produced += rest; st.counter += rest;
+                if (!e && st.litpos < lit.regen) {
+                    uint32_t rest = lit.regen - st.litpos;
+                    if (st.produced + rest > st.cap) e = B200Z_ERR_TARGET_TOO_SMALL;
+                    else {
+                        if (lit.rle) warp_fill(out + st.produced, lit.byte, rest, lane); else warp_copy(out + st.produced, lit.p + st.litpos, rest, lane);
+                        st.produced += rest; st.counter += rest;
+                    }
                 }
-            }
-            if (!known && !redo && e != B200Z_ERR_CUDA) {
-                // everything was consumed (or an execution error came up) before the sequence stage's verdict: it decides
-                if (!exec_wait_ready(aux, b, lane)) e = B200Z_ERR_CUDA;
-                else {
-                    known = true;
-                    ax_pad = ld_cg_u32(&aux[b].pad); ax_flags = ld_cg_u32(&aux[b].flags);
-                    if (ax_pad) redo = 1; else if (ax_flags & AUX_RAW_OFFSETS) redo = 2;
+                if (!known && e != B200Z_ERR_CUDA) {
+                    // everything was consumed (or an execution error came up) before the sequence stage's verdict: it decides
+                    // (progress never reaches ~0: only `ready` or the clock ends this wait)
+                    uint32_t published;
+                    if (exec_wait(aux[b], 0xFFFFFFFFu, lane, published) == WAIT_TIMEOUT) e = B200Z_ERR_CUDA;
+                    else { known = true; verdict = exec_seq_verdict(aux[b], seq_st, ax_flags); }
                 }
-            }
-            if (redo == 2) { redo = 0; goto exec_block_again; }
-            if (redo == 1) {   // decode_sequences failed: the reference executes nothing of this block (block_decoder.rs:176-183)
+            } while (verdict == SEQ_REPLAY);
+            if (verdict == SEQ_FAILED) {   // decode_sequences failed: the reference executes nothing of this block (block_decoder.rs:176-183)
                 st = s_saved[threadIdx.x >> 5];
-                status = ax_pad; err_block = d.block_in_frame; break;
+                status = seq_st; err_block = d.block_in_frame; break;
             }
             if (e) { status = mk_status(e, e == B200Z_ERR_CUDA ? B200Z_STAGE_SEQUENCES : (e == B200Z_ERR_TARGET_TOO_SMALL ? B200Z_STAGE_DRAIN : B200Z_STAGE_EXECUTE)); err_block = d.block_in_frame; break; }
-            if (resolved && d.nseq) {   // the history after the block, in terms of the history at its start
+            if (resolved_u && d.nseq) {   // the history after the block, in terms of the history at its start
                 const uint32_t a0 = ld_cg_u32(&aux[b].hist_after[0]), a1 = ld_cg_u32(&aux[b].hist_after[1]), a2 = ld_cg_u32(&aux[b].hist_after[2]);
                 st.h0 = seq_sym_resolve(a0, bh0, bh1, bh2); st.h1 = seq_sym_resolve(a1, bh0, bh1, bh2); st.h2 = seq_sym_resolve(a2, bh0, bh1, bh2);
             }
@@ -1245,7 +1232,7 @@ __global__ void __launch_bounds__(EXEC_WARPS * 32, EXEC_MINB) k_exec(const Block
         __syncwarp();
         blocks_done++;
     }
-    if (!status && fd.host_status) { status = fd.host_status & 0x00ffffffu; err_block = blocks_done; }
+    if (!status && fd.host_status) { status = fd.host_status; err_block = blocks_done; }
     if (lane == 0) {
         FrameState &o = states[f];
         o.hist[0] = st.h0; o.hist[1] = st.h1; o.hist[2] = st.h2;

@@ -100,11 +100,11 @@ void plan_compressed_block(const uint8_t *c, uint32_t size, BlockDesc &d, BlockR
 void plan_compressed_block_view(const uint8_t *c, const uint8_t *seq, uint32_t size, BlockDesc &d, BlockRefs &r, TableCursor &cur,
                                 uint32_t &n_huf_slots, uint32_t &n_fse_slots, uint64_t &lit_bytes, uint64_t &nseq_total) {
     // ---- literals section header (literals_section.rs:117-223)
-    if (size == 0) { d.host_status = host_status(B200Z_ERR_LITSEC_GET_BITS, B200Z_STAGE_BLOCK_BODY, 1); return; }
+    if (size == 0) { d.host_status = host_status(B200Z_ERR_LITSEC_GET_BITS, B200Z_STAGE_BLOCK_BODY, HS_BEFORE_LITERALS); return; }
     uint32_t lt = c[0] & 3, sf = (c[0] >> 2) & 3, need;
     if (lt == LT_RAW || lt == LT_RLE) need = (sf == 0 || sf == 2) ? 1 : (sf == 1 ? 2 : 3);
     else need = sf <= 1 ? 3 : (sf == 2 ? 4 : 5);
-    if (size < need) { d.host_status = host_status(B200Z_ERR_LITSEC_NOT_ENOUGH_BYTES, B200Z_STAGE_BLOCK_BODY, 1); return; }
+    if (size < need) { d.host_status = host_status(B200Z_ERR_LITSEC_NOT_ENOUGH_BYTES, B200Z_STAGE_BLOCK_BODY, HS_BEFORE_LITERALS); return; }
     uint32_t regen = 0, comp = 0, nstreams = 0;
     if (lt == LT_RAW || lt == LT_RLE) {
         if (sf == 0 || sf == 2) regen = c[0] >> 3;
@@ -119,7 +119,7 @@ void plan_compressed_block_view(const uint8_t *c, const uint8_t *seq, uint32_t s
     d.lit_type = lt; d.nstreams = nstreams; d.regen_size = regen; d.lit_comp_size = comp; d.lit_off = need;
     // block_decoder.rs:120-134
     uint32_t upper = (lt == LT_COMPRESSED || lt == LT_TREELESS) ? comp : (lt == LT_RLE ? 1 : regen);
-    if (size - need < upper) { d.host_status = host_status(B200Z_ERR_MALFORMED_SECTION_HEADER, B200Z_STAGE_BLOCK_BODY, 1); return; }
+    if (size - need < upper) { d.host_status = host_status(B200Z_ERR_MALFORMED_SECTION_HEADER, B200Z_STAGE_BLOCK_BODY, HS_BEFORE_LITERALS); return; }
     if (lt == LT_COMPRESSED) {
         r.build_huf = (int32_t)n_huf_slots++;
         cur.huf.kind = TabRef::SLOT; cur.huf.idx = (uint32_t)r.build_huf;
@@ -143,11 +143,11 @@ void plan_compressed_block_view(const uint8_t *c, const uint8_t *seq, uint32_t s
             if (nseq != 0) { if (rem < 3) bad = true; else { modes = s[2]; hdr = 3; } }
         }
     } else { if (rem < 4) bad = true; else { nseq = (uint32_t)s[1] + ((uint32_t)s[2] << 8) + 0x7F00; modes = s[3]; hdr = 4; } }
-    if (bad) { d.host_status = host_status(B200Z_ERR_SEQHDR_NOT_ENOUGH_BYTES, B200Z_STAGE_BLOCK_BODY, 2); return; }
+    if (bad) { d.host_status = host_status(B200Z_ERR_SEQHDR_NOT_ENOUGH_BYTES, B200Z_STAGE_BLOCK_BODY, HS_AFTER_LITERALS); return; }
     d.nseq = nseq; d.modes = modes; d.seq_off = need + upper + hdr;
     if (nseq == 0) {
         // block_decoder.rs:185-191: bytes after an empty sequences section
-        if (rem - hdr != 0) d.host_status = host_status(B200Z_ERR_SEQ_EXTRA_BITS, B200Z_STAGE_SEQUENCES, 2);
+        if (rem - hdr != 0) d.host_status = host_status(B200Z_ERR_SEQ_EXTRA_BITS, B200Z_STAGE_SEQUENCES, HS_AFTER_LITERALS);
         return;
     }
     uint32_t ml_ = (modes >> 6) & 3, mo = (modes >> 4) & 3, mm = (modes >> 2) & 3;

@@ -49,7 +49,7 @@ struct TableCursor {
 
 // Fills the section-level fields of `d` for a Compressed block whose content is content[0..size).
 // Errors the reference raises from header parsing are recorded in d.host_status with their position
-// (1 = before the literals stage, 2 = after it) so the device can report the first error in reference order.
+// (HS_BEFORE_LITERALS / HS_AFTER_LITERALS) so the device can report the first error in reference order.
 void plan_compressed_block(const uint8_t *content, uint32_t size, BlockDesc &d, BlockRefs &r, TableCursor &cur,
                            uint32_t &n_huf_slots, uint32_t &n_fse_slots, uint64_t &lit_bytes, uint64_t &nseq_total);
 
@@ -66,8 +66,6 @@ void route_exec_frames(const uint64_t *work, const uint8_t *eligible, size_t nfr
 // empty (= descriptor order) when no frame of the warp kernel has two blocks or the frames do not cover the blocks exactly.
 void build_fse_order(const uint32_t *first_block, const uint32_t *nblocks, const uint8_t *on_cta, size_t nframes, const uint32_t *nseq,
                      size_t nblocks_total, std::vector<uint32_t> &order);
-
-inline uint32_t host_status(uint32_t code, uint32_t stage, uint32_t pos) { return code | (stage << 16) | (pos << 24); }
 
 // XXH64 (seed 0) streaming -- the hash the reference feeds on drain (decode_buffer.rs:42,225,290,301)
 struct XXH64State {
