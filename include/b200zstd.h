@@ -258,6 +258,14 @@ int b200z_batch_debug_sequences(b200z_batch *b, uint32_t block, uint32_t *host_o
  * (sequence_execution.rs:59-118), symbolic where they depend on the repeat-offset history at the block's start:
  * tag << 30 | decrements, tag 1..3 = history slot + 1 */
 int b200z_batch_debug_block_flags(b200z_batch *b, uint32_t block, uint32_t *flags);
+/* the entropy tables block `block` decodes with, as the planner resolved them (the defining block's table for Treeless
+ * literals and Repeat modes, the predefined tables, a dictionary's tables), copied raw: the huff0 table into huf_out
+ * (B200Z_DEBUG_HUF_BYTES: u32 max_bits, u32 status, 8 bytes padding, u8 symbol[2048], 4-bit code length nb4[1024]) and the
+ * LL, OF and ML tables into fse_out (3 x B200Z_DEBUG_FSE_BYTES: u32 log, u32 valid, u32 is_rle, u32 padding, u16 entry[512],
+ * entry = (1 << (log - nb) | base >> nb) | symbol << 10).  present[0..3] (huf, ll, of, ml) = 0 where the block has no table. */
+#define B200Z_DEBUG_HUF_BYTES 3088
+#define B200Z_DEBUG_FSE_BYTES 1040
+int b200z_batch_debug_tables(b200z_batch *b, uint32_t block, uint8_t *huf_out, uint8_t *fse_out, uint32_t present[4]);
 /* execution scheduling counters of the last run (tests / profiling): [0] frames given to k_exec_cta (block assembled in
  * shared memory), [1] frames it handed back to k_exec (one warp per frame), [2] OR of the reasons, [3] blocks handed back */
 int b200z_batch_debug_sched(b200z_batch *b, uint32_t out[4]);

@@ -26,6 +26,7 @@ MEM_HOST, MEM_DEVICE = 0, 1
 ERR_SKIP_FRAME = 8
 FLAG_CHECKSUM = 1
 FLAG_PROFILE = 2
+HUF_DEBUG_BYTES, FSE_DEBUG_BYTES = 3088, 1040   # B200Z_DEBUG_HUF_BYTES / B200Z_DEBUG_FSE_BYTES: one raw huff0 / FSE table
 UNCOMPRESSED, FASTEST = 0, 1   # CompressionLevel (ruzstd encoding/mod.rs:24-67); Default / Better / Best are not implemented there
 
 
@@ -112,6 +113,7 @@ def lib():
         "b200z_batch_debug_sequences": (C.c_int, [vp, C.c_uint32, vp, sz, C.POINTER(sz)]),
         "b200z_batch_debug_block_flags": (C.c_int, [vp, C.c_uint32, C.POINTER(C.c_uint32)]),
         "b200z_batch_debug_sched": (C.c_int, [vp, C.POINTER(C.c_uint32)]),
+        "b200z_batch_debug_tables": (C.c_int, [vp, C.c_uint32, vp, vp, C.POINTER(C.c_uint32)]),
         "b200z_debug_route_frames": (C.c_int, [vp, vp, sz, C.c_uint32, vp, C.POINTER(sz)]),
         "b200z_debug_fse_order": (C.c_int, [vp, vp, vp, sz, vp, sz, vp, C.POINTER(sz)]),
         "b200z_batch_destroy": (None, [vp]),
@@ -459,6 +461,32 @@ class Batch:
         v = C.c_uint32()
         self.ctx._chk(self.ctx.L.b200z_batch_debug_block_flags(self.h, block, C.byref(v)))
         return v.value
+
+    def debug_tables(self, block):
+        """{"huf", "ll", "of", "ml"} tables block `block` decodes with (None = absent).  huf: {"max_bits", "entries": 2^max_bits
+        (symbol, nb)}; ll/of/ml: {"log", "valid", "is_rle", "entries": 2^log (symbol, nb, baseline)} unpacked from fse_pack16."""
+        huf = np.zeros(HUF_DEBUG_BYTES, dtype=np.uint8)
+        fse = np.zeros(3 * FSE_DEBUG_BYTES, dtype=np.uint8)
+        present = (C.c_uint32 * 4)()
+        self.ctx._chk(self.ctx.L.b200z_batch_debug_tables(self.h, block, huf.ctypes.data, fse.ctypes.data, present))
+        out = {"huf": None, "ll": None, "of": None, "ml": None}
+        if present[0]:
+            mb = int(huf[:4].view(np.uint32)[0])
+            sym, nb4 = huf[16:16 + 2048], huf[16 + 2048:]
+            n = 1 << mb if mb else 0
+            out["huf"] = {"max_bits": mb, "entries": [(int(sym[i]), int(nb4[i >> 1] >> (4 * (i & 1))) & 15) for i in range(n)]}
+        for k, name in enumerate(("ll", "of", "ml")):
+            if not present[1 + k]:
+                continue
+            t = fse[k * FSE_DEBUG_BYTES:(k + 1) * FSE_DEBUG_BYTES]
+            log, valid, is_rle = (int(x) for x in t[:12].view(np.uint32))
+            ents = []
+            for e in t[16:].view(np.uint16)[:1 << log] if log <= 9 else []:
+                f, s = int(e) & 0x3FF, int(e) >> 10
+                nb = log - (f.bit_length() - 1) if f else 0
+                ents.append((s, nb, (f - (1 << (f.bit_length() - 1))) << nb if f else 0))
+            out[name] = {"log": log, "valid": valid, "is_rle": is_rle, "entries": ents}
+        return out
 
     def close(self):
         if getattr(self, "h", None) and self.ctx.h:

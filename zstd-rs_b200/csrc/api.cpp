@@ -770,6 +770,23 @@ extern "C" int b200z_batch_debug_sequences(b200z_batch *b, uint32_t block, uint3
     *nseq = d.nseq;
     return 0;
 }
+// the tables a block decodes with, as the planner resolved them into its descriptor (the defining slot for Treeless / Repeat,
+// the predefined tables, a dictionary's or the streaming carry's tables), copied raw; a null table is reported absent
+extern "C" int b200z_batch_debug_tables(b200z_batch *b, uint32_t block, uint8_t *huf_out, uint8_t *fse_out, uint32_t present[4]) {
+    if (!b || block >= b->sub.descs.size() || !huf_out || !fse_out || !present) return B200Z_ERR_INVALID_ARGUMENT;
+    static_assert(sizeof(HufSlot) == B200Z_DEBUG_HUF_BYTES && sizeof(FseTab) == B200Z_DEBUG_FSE_BYTES, "b200zstd.h table sizes");
+    b200z_ctx *c = b->ctx;
+    const BlockDesc &d = b->sub.descs[block];
+    CU(c, cudaStreamSynchronize(c->stream));
+    present[0] = d.huf != nullptr;
+    if (d.huf) CU(c, cudaMemcpy(huf_out, d.huf, sizeof(HufSlot), cudaMemcpyDeviceToHost));
+    const FseTab *t[3] = {d.ll, d.of, d.ml};
+    for (int k = 0; k < 3; k++) {
+        present[1 + k] = t[k] != nullptr;
+        if (t[k]) CU(c, cudaMemcpy(fse_out + k * sizeof(FseTab), t[k], sizeof(FseTab), cudaMemcpyDeviceToHost));
+    }
+    return 0;
+}
 // flags of a block's sequence stage: bit 0 = `of` values are raw offset_values (otherwise offsets after do_offset_history,
 // symbolic where they depend on the history at the block's start: tag << 30 | decrements, tag 1..3 = history slot + 1)
 extern "C" int b200z_batch_debug_block_flags(b200z_batch *b, uint32_t block, uint32_t *flags) {
