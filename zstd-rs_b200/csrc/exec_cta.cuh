@@ -235,6 +235,17 @@ __device__ __forceinline__ bool xc_rows(const XcBlk &B, uint32_t r0, uint32_t lo
     return true;
 }
 
+// xc_rows for a block's variant (bit 0: FAR, bit 1: LITG); `lo` = first row of the sub-phase
+template <int NR>
+__device__ __forceinline__ bool xc_rows_of(uint32_t variant, const XcBlk &B, uint32_t r0, uint32_t lo, bool has_ovl, uint32_t lane) {
+    switch (variant) {
+        case 0: return xc_rows<false, false, NR>(B, r0, lo << 7, has_ovl, lane);
+        case 1: return xc_rows<true, false, NR>(B, r0, lo << 7, has_ovl, lane);
+        case 2: return xc_rows<false, true, NR>(B, r0, lo << 7, has_ovl, lane);
+        default: return xc_rows<true, true, NR>(B, r0, lo << 7, has_ovl, lane);
+    }
+}
+
 // registers a thread carries from the record loads of a batch to its build step: XC_PER_THREAD consecutive records,
 // and (lane 0 only) the record before the warp's first
 struct XcLoad { uint32_t out[XC_PER_THREAD], lit[XC_PER_THREAD], of[XC_PER_THREAD], p_out, p_lit; };
@@ -340,8 +351,7 @@ __global__ void __launch_bounds__(XC_THREADS, 1) k_exec_cta(const BlockDesc *__r
         uint32_t h0 = fs.hist[0], h1 = fs.hist[1], h2 = fs.hist[2];
         uint64_t produced = fs.produced, counter = fs.counter;
         const uint64_t drained = fs.drained;
-        uint64_t cap = fd.out_cap;
-        if (fd.out_off > output_cap) cap = 0; else if (cap > output_cap - fd.out_off) cap = output_cap - fd.out_off;
+        const uint64_t cap = frame_out_room(fd, output_cap);
         uint8_t *out = output + fd.out_off;
         uint32_t blocks_done = fs.blocks_done;
         const uint32_t nblocks = fd.nblocks;
@@ -354,13 +364,10 @@ __global__ void __launch_bounds__(XC_THREADS, 1) k_exec_cta(const BlockDesc *__r
             const BlockDesc &d = descs[b];
             const BlockAux &ax = aux[b];
             if (d.host_status || ax.status) { bailed = true; why |= XC_WHY_ERROR; break; }
-            const uint32_t btype = d.btype;
-            if (btype != BT_COMPRESSED) {
+            if (d.btype != BT_COMPRESSED) {
                 const uint32_t n = d.raw_size;
                 if (produced + n > cap) { bailed = true; why |= XC_WHY_CAPACITY; break; }
-                uint8_t *dst = out + produced;
-                if (btype == BT_RAW) { const uint8_t *srcp = input + d.src_off; for (uint32_t j = tid; j < n; j += XC_THREADS) dst[j] = srcp[j]; }
-                else { const uint8_t v = input[d.src_off]; for (uint32_t j = tid; j < n; j += XC_THREADS) dst[j] = v; }
+                raw_rle_block(out + produced, d, input, tid, XC_THREADS);
                 produced += n;   // extend_from_reader: total_output_counter untouched (decode_buffer.rs:66-72)
                 blocks_done++;
                 fresh = false;
@@ -476,22 +483,8 @@ __global__ void __launch_bounds__(XC_THREADS, 1) k_exec_cta(const BlockDesc *__r
                     if (lo != row_lo) { __syncthreads(); xc_planes_reset(S, tid); __syncthreads(); }
                     uint32_t r = lo + warp;
                     const uint32_t variant = (has_far ? 1u : 0u) | (litg ? 2u : 0u);
-                    for (; r + XC_WARPS < hi && ok; r += 2 * XC_WARPS) {
-                        switch (variant) {
-                            case 0: ok = xc_rows<false, false, 2>(B, r, lo << 7, has_ovl, lane); break;
-                            case 1: ok = xc_rows<true, false, 2>(B, r, lo << 7, has_ovl, lane); break;
-                            case 2: ok = xc_rows<false, true, 2>(B, r, lo << 7, has_ovl, lane); break;
-                            default: ok = xc_rows<true, true, 2>(B, r, lo << 7, has_ovl, lane); break;
-                        }
-                    }
-                    if (r < hi && ok) {
-                        switch (variant) {
-                            case 0: ok = xc_rows<false, false, 1>(B, r, lo << 7, has_ovl, lane); break;
-                            case 1: ok = xc_rows<true, false, 1>(B, r, lo << 7, has_ovl, lane); break;
-                            case 2: ok = xc_rows<false, true, 1>(B, r, lo << 7, has_ovl, lane); break;
-                            default: ok = xc_rows<true, true, 1>(B, r, lo << 7, has_ovl, lane); break;
-                        }
-                    }
+                    for (; r + XC_WARPS < hi && ok; r += 2 * XC_WARPS) ok = xc_rows_of<2>(variant, B, r, lo, has_ovl, lane);
+                    if (r < hi && ok) ok = xc_rows_of<1>(variant, B, r, lo, has_ovl, lane);
                 }
                 if (!ok && lane == 0) misc->bail = 2u;
                 xc_fence_proxy_async();
@@ -521,11 +514,7 @@ __global__ void __launch_bounds__(XC_THREADS, 1) k_exec_cta(const BlockDesc *__r
                 if (tid < 16) { const uint32_t a = B.woff + tid; if (a < head_end) B.gout[a - B.woff] = (uint8_t)lds8(S + a); }
                 else if (tid < 32) { const uint32_t a = tail_beg + (tid - 16u); if (a < B.a_end) B.gout[a - B.woff] = (uint8_t)lds8(S + a); }
             }
-            if (nseq) {   // the history after the block, in terms of the history at its start (k_fse, symbolic)
-                const uint32_t a0 = ld_cg_u32(&ax.hist_after[0]), a1 = ld_cg_u32(&ax.hist_after[1]), a2 = ld_cg_u32(&ax.hist_after[2]);
-                const uint32_t n0 = seq_sym_resolve(a0, h0, h1, h2), n1 = seq_sym_resolve(a1, h0, h1, h2), n2 = seq_sym_resolve(a2, h0, h1, h2);
-                h0 = n0; h1 = n1; h2 = n2;
-            }
+            if (nseq) block_hist_after(ax, h0, h1, h2, h0, h1, h2);
             produced += out_size; counter += out_size;
             blocks_done++;
             fresh = false;

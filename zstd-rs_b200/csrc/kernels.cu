@@ -789,7 +789,9 @@ __global__ void __launch_bounds__(32) k_fse(const BlockDesc *__restrict__ descs,
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// k_exec: LZ77 execution.  One warp per frame, blocks in order, 64 sequences per step.
+// k_exec: LZ77 execution.  One warp per frame, blocks in order, 64 sequences per step.  The kernel body walks a frame's
+// blocks; exec_compressed_block runs a Compressed block batch by batch: exec_load_batch (records -> lengths and positions),
+// exec_batch_offsets (actual offsets), then exec_batch_fast or exec_batch_exact.
 //
 // Fast path (per batch of 64 sequences, lane j = sequences 2j and 2j + 1): one warp scan gives every sequence its
 // literal and match positions; a bitmask of sequence ends in shared memory lets each OUTPUT byte find its owner
@@ -820,8 +822,6 @@ struct ExecState {
 };
 struct LitSrc { const uint8_t *p; uint32_t rle; uint8_t byte; uint32_t regen; };
 
-// exact sequential execution of up to 32 sequences held one per lane (my_ll/my_ml/my_of); `resolved` = offsets
-// already went through do_offset_history.  Returns 0 or an error code.
 constexpr uint32_t EXEC_PER_LANE = 2;                       // consecutive sequences a lane holds (even)
 constexpr uint32_t EXEC_BATCH = 32 * EXEC_PER_LANE;         // sequences per batch
 // Sequence j of the batch lives in lane j / EXEC_PER_LANE, slot j % EXEC_PER_LANE.
@@ -831,6 +831,9 @@ __device__ __forceinline__ uint32_t exec_pick(const uint32_t (&v)[EXEC_PER_LANE]
     for (uint32_t k = 1; k < EXEC_PER_LANE; k++) r = slot == k ? v[k] : r;
     return r;
 }
+// Exact sequential execution of the first nb sequences of a batch (up to EXEC_BATCH, EXEC_PER_LANE consecutive ones per lane
+// in lls / mls / ofs), one after the other; `resolved` = offsets already went through do_offset_history.  Returns 0 or an
+// error code.
 __device__ uint32_t exec_batch_exact(ExecState &st, const LitSrc &lit, const FrameDesc &fd, uint8_t *out, uint32_t nb, const uint32_t (&lls)[EXEC_PER_LANE],
                                      const uint32_t (&mls)[EXEC_PER_LANE], const uint32_t (&ofs)[EXEC_PER_LANE], bool resolved, uint32_t lane) {
     for (uint32_t j = 0; j < nb; j++) {
@@ -926,6 +929,26 @@ __device__ __forceinline__ uint32_t exec_seq_verdict(const BlockAux &a, uint32_t
     return seq_status ? SEQ_FAILED : ((flags & AUX_RAW_OFFSETS) ? SEQ_REPLAY : SEQ_GO);
 }
 
+// ---- what both execution kernels do (k_exec_cta, exec_cta.cuh, is included further down)
+// Bytes a frame may write at its out_off: its out_cap, as far as the output buffer reaches
+__device__ __forceinline__ uint64_t frame_out_room(const FrameDesc &fd, uint64_t output_cap) {
+    uint64_t cap = fd.out_cap;
+    if (fd.out_off > output_cap) cap = 0; else if (cap > output_cap - fd.out_off) cap = output_cap - fd.out_off;
+    return cap;
+}
+// The bytes of a Raw or RLE block at dst, written by threads first, first + stride, ...; the caller has checked the room
+__device__ __forceinline__ void raw_rle_block(uint8_t *dst, const BlockDesc &d, const uint8_t *input, uint32_t first, uint32_t stride) {
+    const uint32_t n = d.raw_size;
+    if (d.btype == BT_RAW) { const uint8_t *src = input + d.src_off; for (uint32_t j = first; j < n; j += stride) dst[j] = src[j]; }
+    else { const uint8_t v = input[d.src_off]; for (uint32_t j = first; j < n; j += stride) dst[j] = v; }
+}
+// The offset history after a Compressed block with sequences: k_fse's three symbols (BlockAux::hist_after) resolved against
+// the history at the block's start (b0, b1, b2)
+__device__ __forceinline__ void block_hist_after(const BlockAux &a, uint32_t b0, uint32_t b1, uint32_t b2, uint32_t &h0, uint32_t &h1, uint32_t &h2) {
+    const uint32_t a0 = ld_cg_u32(&a.hist_after[0]), a1 = ld_cg_u32(&a.hist_after[1]), a2 = ld_cg_u32(&a.hist_after[2]);
+    h0 = seq_sym_resolve(a0, b0, b1, b2); h1 = seq_sym_resolve(a1, b0, b1, b2); h2 = seq_sym_resolve(a2, b0, b1, b2);
+}
+
 constexpr uint32_t EXEC_WARPS = 4;
 constexpr uint32_t EXEC_TMAX = 8128;         // most bytes one batch may produce on the fast path (sizes the end-bit mask)
 constexpr uint32_t EXEC_CHUNK_ROWS = 4;      // rows (of 32 bytes) whose loads are in flight together
@@ -933,6 +956,283 @@ constexpr uint32_t EXEC_MASK_WORDS = (EXEC_TMAX + 31) / 32 + EXEC_CHUNK_ROWS;
 // CTAs per SM the register budget must allow: 6 gives 80 registers (few spills).  On an H100 this runs k_exec ~19 % faster
 // than 8 (64 registers, ~190 bytes of spills per thread); 4 and 5 measure the same as 6.
 constexpr int EXEC_MINB = 6;
+
+// ---- the stages of k_exec
+// A batch: EXEC_BATCH sequences, EXEC_PER_LANE consecutive ones per lane (exec_pick), positions relative to the batch's start
+struct ExecBatch {
+    uint32_t ll[EXEC_PER_LANE], ml[EXEC_PER_LANE], of[EXEC_PER_LANE];   // of: as k_fse left it (a symbol, or a raw offset_value)
+    uint32_t oend[EXEC_PER_LANE], mstart[EXEC_PER_LANE], lend[EXEC_PER_LANE];   // inclusive end of its bytes, start of its match, inclusive end of its literals
+    bool on[EXEC_PER_LANE];   // the slot holds one of the batch's nb sequences
+    uint32_t T, L;            // bytes and literals of the batch
+};
+// Loads the batch at `base`: contiguous 12-byte records in prefix form {out_end, lit_end, of}, so ll and ml are differences of
+// neighbouring records; carry_out / carry_lit = the prefix sums at the end of the previous batch, advanced to this one's end.
+// The next batch's records are requested into L2 one batch ahead.
+__device__ __forceinline__ ExecBatch exec_load_batch(const uint32_t *seqs, uint32_t base, uint32_t nb, uint32_t nseq, uint32_t lane, uint32_t &carry_out,
+                                                     uint32_t &carry_lit) {
+    constexpr uint32_t K = EXEC_PER_LANE;
+    ExecBatch B;
+    uint32_t pe_out[K], pe_lit[K];
+    const uint32_t old_out = carry_out, old_lit = carry_lit;
+    const uint32_t *sp = seqs + (uint64_t)(base + K * lane) * 3;
+    uint32_t raw[3 * K];
+    if (K * lane + K <= nb) {   // all my records exist: K * 12 contiguous bytes, 8-byte aligned
+#pragma unroll
+        for (uint32_t k = 0; k < 3 * K; k += 2) { const uint2 r = ld_cg_u32x2(sp + k); raw[k] = r.x; raw[k + 1] = r.y; }
+    } else {
+#pragma unroll
+        for (uint32_t k = 0; k < K; k++) {
+            const bool have = K * lane + k < nb;
+            raw[3 * k] = have ? ld_cg_u32(sp + 3 * k) : 0u; raw[3 * k + 1] = have ? ld_cg_u32(sp + 3 * k + 1) : 0u; raw[3 * k + 2] = have ? ld_cg_u32(sp + 3 * k + 2) : 1u;
+        }
+    }
+    // prefix form -> lengths: my first record's predecessor is the last record of the lane below (or the carry)
+    uint32_t p_out = __shfl_up_sync(0xffffffffu, raw[3 * (K - 1)], 1), p_lit = __shfl_up_sync(0xffffffffu, raw[3 * (K - 1) + 1], 1);
+    if (lane == 0) { p_out = carry_out; p_lit = carry_lit; }
+#pragma unroll
+    for (uint32_t k = 0; k < K; k++) {
+        B.on[k] = K * lane + k < nb;
+        const uint32_t ll = raw[3 * k + 1] - p_lit, ml = raw[3 * k] - p_out - ll;
+        B.ll[k] = B.on[k] ? ll : 0u; B.ml[k] = B.on[k] ? ml : 0u; B.of[k] = raw[3 * k + 2];
+        p_out = raw[3 * k]; p_lit = raw[3 * k + 1];
+        pe_out[k] = p_out; pe_lit[k] = p_lit;
+    }
+    {   // carry: the batch's last record
+        const uint32_t lastl = (nb - 1) / K, lasts = (nb - 1) % K;
+        uint32_t co = raw[0], cl = raw[1];
+#pragma unroll
+        for (uint32_t k = 1; k < K; k++) { co = lasts == k ? raw[3 * k] : co; cl = lasts == k ? raw[3 * k + 1] : cl; }
+        carry_out = __shfl_sync(0xffffffffu, co, lastl); carry_lit = __shfl_sync(0xffffffffu, cl, lastl);
+    }
+    if (base + EXEC_BATCH < nseq && lane * 128u < (nseq - base - EXEC_BATCH) * 12u && lane * 128u < EXEC_BATCH * 12u)
+        prefetch_l2(reinterpret_cast<const uint8_t *>(seqs + (uint64_t)(base + EXEC_BATCH) * 3) + lane * 128u);
+    // the records are prefix sums already (k_fse): batch totals and batch-relative positions are differences
+    B.T = carry_out - old_out; B.L = carry_lit - old_lit;
+#pragma unroll
+    for (uint32_t k = 0; k < K; k++) { B.oend[k] = B.on[k] ? pe_out[k] - old_out : B.T; B.lend[k] = B.on[k] ? pe_lit[k] - old_lit : B.L; B.mstart[k] = B.oend[k] - B.ml[k]; }
+    return B;
+}
+
+// The actual offsets of a batch: symbols resolve against the history at the block's start (b0, b1, b2); a block flagged
+// AUX_RAW_OFFSETS (exact path of k_fse) runs do_offset_history here instead, sequence by sequence, on h0, h1, h2.
+__device__ __forceinline__ void exec_batch_offsets(const ExecBatch &B, uint32_t nb, bool resolved, uint32_t b0, uint32_t b1, uint32_t b2, uint32_t lane,
+                                                   uint32_t (&offs)[EXEC_PER_LANE], uint32_t &h0, uint32_t &h1, uint32_t &h2) {
+    constexpr uint32_t K = EXEC_PER_LANE;
+#pragma unroll
+    for (uint32_t k = 0; k < K; k++) offs[k] = resolved ? seq_sym_resolve(B.of[k], b0, b1, b2) : B.of[k];
+    if (!resolved) {
+        // cheap scalar steps (sequence_execution.rs:59-118); the caller commits the history only if the fast path is taken (the
+        // exact path redoes the steps itself)
+        for (uint32_t j = 0; j < nb; j++) {
+            const uint32_t slot = j % K, src_lane = j / K;
+            uint32_t ll = __shfl_sync(0xffffffffu, exec_pick(B.ll, slot), src_lane), of = __shfl_sync(0xffffffffu, exec_pick(B.of, slot), src_lane);
+            uint32_t actual = offset_history_step(of, ll, h0, h1, h2);
+            if (lane == src_lane) {
+#pragma unroll
+                for (uint32_t k = 0; k < K; k++) offs[k] = slot == k ? actual : offs[k];
+            }
+        }
+    }
+}
+
+// Rows are produced EXEC_CHUNK_ROWS at a time: every byte whose source lies before the chunk (literals, and matches reaching
+// back past the chunk start, `floor`) is loaded first -- EXEC_CHUNK_ROWS independent loads per lane in flight -- then stored;
+// the few bytes whose source lies inside the chunk follow, row by row.  (Issuing the next chunk's loads before this chunk's
+// stores was measured slower: more bytes turn dependent.)  The per-byte work is branch-free: one select between the literal
+// and the match source.
+// tag: TAG_NONE = nothing to do, TAG_STORE = value loaded, otherwise the (batch-relative, >= floor) source position of a match
+// byte that had to wait.
+constexpr int32_t TAG_NONE = INT32_MIN, TAG_STORE = INT32_MIN + 1;
+// `before` = sequences ended in earlier rows (advanced past the chunk)
+__device__ __forceinline__ void exec_load_chunk(uint32_t r0, int32_t floor, uint32_t &before, uint32_t T, bool has_ovl, const uint8_t *bout, const uint8_t *litq,
+                                                uint32_t a_mask, uint32_t a_recs, uint32_t lane, uint32_t lt, uint32_t (&val)[EXEC_CHUNK_ROWS],
+                                                int32_t (&tag)[EXEC_CHUNK_ROWS]) {
+#pragma unroll
+    for (int i = 0; i < (int)EXEC_CHUNK_ROWS; i++) {
+        const uint32_t q = ((r0 + i) << 5) + lane;
+        const uint32_t word = lds32(a_mask + ((r0 + i) << 2));
+        const uint32_t owner = before + __popc(word & lt);   // sequences that ended below q
+        before += __popc(word);
+        const uint2 rc = lds64(a_recs + ((owner & (EXEC_BATCH - 1u)) << 3));
+        const uint32_t mst = rc.x & 0xffffu;
+        const bool is_match = q >= mst;
+        int32_t sp = (int32_t)q - (int32_t)rc.y;                  // batch-relative source of a match byte
+        if (has_ovl) {                                            // overlapping match: byte k comes from k mod offset
+            const uint32_t kk = q - mst;
+            if (is_match && kk >= rc.y) sp = (int32_t)mst - (int32_t)rc.y + (int32_t)(kk % rc.y);
+        }
+        const bool valid = q < T;
+        const bool dep = is_match && sp >= floor;
+        const int32_t idx = is_match ? sp : (int32_t)(q - (rc.x >> 16));
+        const uint8_t *bp = is_match ? bout : litq;
+        tag[i] = valid ? (dep ? sp : TAG_STORE) : TAG_NONE;
+        val[i] = 0;
+        if (valid && !dep) val[i] = bp[idx];
+    }
+}
+__device__ __forceinline__ void exec_store_chunk(uint8_t *bout, uint32_t r0, int32_t floor, const uint32_t (&val)[EXEC_CHUNK_ROWS], const int32_t (&tag)[EXEC_CHUNK_ROWS],
+                                                 uint32_t lane) {
+#pragma unroll
+    for (int i = 0; i < (int)EXEC_CHUNK_ROWS; i++)
+        if (tag[i] == TAG_STORE) bout[((r0 + i) << 5) + lane] = (uint8_t)val[i];
+    // dependent bytes, rows in order (sources in earlier rows are final, inside the row the lowest pending byte is ready)
+    bool anydep = false;
+#pragma unroll
+    for (int i = 0; i < (int)EXEC_CHUNK_ROWS; i++) anydep |= tag[i] >= floor;
+    if (__any_sync(0xffffffffu, anydep)) {
+#pragma unroll
+        for (int i = 0; i < (int)EXEC_CHUNK_ROWS; i++) {
+            bool mine = tag[i] >= floor;
+            uint32_t pending = __ballot_sync(0xffffffffu, mine);
+            const int32_t row0 = (int32_t)((r0 + i) << 5);
+            while (pending) {
+                __syncwarp();
+                bool ready = mine && (tag[i] < row0 || !((pending >> (tag[i] - row0)) & 1u));
+                if (ready) { bout[row0 + (int32_t)lane] = bout[tag[i]]; mine = false; }
+                pending &= ~__ballot_sync(0xffffffffu, ready);
+            }
+        }
+    }
+    __syncwarp();
+}
+
+// The fast path of a batch whose offsets are valid (offs) and whose bytes fit.  Sequence j owns the bytes [lit_begin_j,
+// out_end_j): its literal run, then its match.  A bit is set at the last byte of every sequence, so the owner of output byte q
+// is the number of set bits below q; one 8-byte shared-memory record per sequence then tells the byte where it comes from.
+__device__ __forceinline__ void exec_batch_fast(ExecState &st, const LitSrc &lit, uint8_t *out, const ExecBatch &B, const uint32_t (&offs)[EXEC_PER_LANE],
+                                                bool ovl, uint32_t a_mask, uint32_t a_recs, uint32_t lane, uint32_t lt) {
+    constexpr uint32_t K = EXEC_PER_LANE;
+    const uint32_t nrows = (B.T + 31) >> 5;
+    // The batch's match sources are scattered over the frame's window, and with thousands of frames in flight the windows do
+    // not stay in L2: ask for the sectors now, a few hundred instructions before the rows need them.
+#pragma unroll
+    for (uint32_t k = 0; k < K; k++) {
+        if (B.on[k]) {
+            const uint8_t *src = out + st.produced + B.mstart[k] - offs[k];
+            prefetch_l2(src);
+            if ((((uint32_t)(uintptr_t)src) & 31u) + B.ml[k] > 32u) prefetch_l2(src + B.ml[k] - 1);
+        }
+    }
+    if (lane == 31 && lit.regen) {
+        const uint32_t ahead = st.litpos + B.L + 256u;   // the literal stream is sequential: stay two lines ahead
+        prefetch_l2(lit.p + (ahead < lit.regen ? ahead : lit.regen - 1));
+    }
+    sts32(a_mask + (lane << 2), 0u);
+    if (nrows > 32u - EXEC_CHUNK_ROWS)
+        for (uint32_t w = lane + 32; w < ((nrows + EXEC_CHUNK_ROWS - 1u) & ~(EXEC_CHUNK_ROWS - 1u)); w += 32) sts32(a_mask + (w << 2), 0u);
+    // 8-byte record: literal byte q of the sequence is literal number (q - m_before) of the batch (m_before = match bytes of the
+    // earlier sequences = match start - literal end), match byte q comes from output position q - offset (m_start, m_before <=
+    // EXEC_TMAX: 16 bits each)
+#pragma unroll
+    for (uint32_t k = 0; k < K; k += 2)
+        sts128(a_recs + ((K * lane + k) << 3), B.mstart[k] | ((B.mstart[k] - B.lend[k]) << 16), offs[k], B.mstart[k + 1] | ((B.mstart[k + 1] - B.lend[k + 1]) << 16),
+               offs[k + 1]);
+    const bool has_ovl = __any_sync(0xffffffffu, ovl);   // some match overlaps its own output (rare)
+    __syncwarp();
+#pragma unroll
+    for (uint32_t k = 0; k < K; k++)
+        if (B.on[k]) red_or_shared(a_mask + (((B.oend[k] - 1) >> 5) << 2), 1u << ((B.oend[k] - 1) & 31u));
+    __syncwarp();
+    uint8_t *bout = out + st.produced;
+    const uint8_t *litq = lit.p + st.litpos;
+    asm volatile("" : "+l"(bout), "+l"(litq));   // keep both bases as single 64-bit registers (one add per access)
+    uint32_t before = 0;   // sequences ended in earlier rows
+    for (uint32_t r0 = 0; r0 < nrows; r0 += EXEC_CHUNK_ROWS) {
+        uint32_t va[EXEC_CHUNK_ROWS]; int32_t ta[EXEC_CHUNK_ROWS];
+        exec_load_chunk(r0, (int32_t)(r0 << 5), before, B.T, has_ovl, bout, litq, a_mask, a_recs, lane, lt, va, ta);
+        exec_store_chunk(bout, r0, (int32_t)(r0 << 5), va, ta, lane);
+    }
+    __syncwarp();
+    st.produced += B.T; st.counter += B.T; st.litpos += B.L;
+}
+
+// One Compressed block: its sequences batch by batch (fast path, or the exact path for a batch with anything unusual), then
+// the trailing literals and the sequence stage's verdict.  `known`, seq_st and ax_flags: the verdict, if it is in already.
+// Returns the block's status word (0 = executed: st and its history are the frame's state after the block); a block whose
+// sequence stage failed is rolled back to its start, which `saved` (shared memory) holds meanwhile.
+__device__ __forceinline__ uint32_t exec_compressed_block(ExecState &st, ExecState &saved, const BlockDesc &d, const BlockAux &ax, const FrameDesc &fd, uint8_t *out,
+                                                          const uint8_t *input, const uint8_t *lit_scratch, const uint32_t *seq_scratch, bool known, uint32_t seq_st,
+                                                          uint32_t ax_flags, uint32_t a_mask, uint32_t a_recs, uint32_t lane, uint32_t lt) {
+    LitSrc lit;
+    lit.rle = 0; lit.byte = 0; lit.regen = d.regen_size;
+    if (d.lit_type == LT_RAW) lit.p = input + d.src_off + d.lit_off;
+    else if (d.lit_type == LT_RLE) { lit.p = nullptr; lit.rle = 1; lit.byte = input[d.src_off + d.lit_off]; }
+    else lit.p = lit_scratch + d.lit_buf_off;
+    // the block's start: where a sequence-stage error / a replay by the exact path rolls back to
+    if (lane == 0) saved = st;
+    __syncwarp();
+    uint32_t e, verdict, resolved_u, bh0, bh1, bh2;
+    do {   // once more when the exact path of k_fse rewrote the records the first run consumed
+        st = saved;
+        st.litpos = 0;
+        e = 0; verdict = SEQ_GO;
+        uint32_t avail = known ? 0xFFFFFFFFu : 0u;   // records that may be read
+        // block-level descriptor fields used inside the batch loop are consumed here once: a first use inside the loop would wait
+        // on a scoreboard shared with the record prefetch issued just before it (a full memory latency per batch)
+        resolved_u = (ax_flags & AUX_RAW_OFFSETS) ? 0u : 1u;
+        uint32_t nseq_u = d.nseq;
+        const uint32_t *seqs = seq_scratch + d.seq_buf_off * 3;
+        asm volatile("" : "+r"(resolved_u), "+r"(nseq_u), "+l"(seqs));
+        const bool resolved = resolved_u != 0;
+        __syncwarp();
+        uint32_t carry_out = 0, carry_lit = 0;   // prefix sums at the end of the previous batch
+        bh0 = st.h0; bh1 = st.h1; bh2 = st.h2;   // history at the block's start: what the symbols refer to
+        for (uint32_t base = 0; base < nseq_u && !e; base += EXEC_BATCH) {
+            const uint32_t nb = nseq_u - base < EXEC_BATCH ? nseq_u - base : EXEC_BATCH;
+            if (avail < base + nb) {   // wait for k_fse: either these records, or the end of the block's sequence stage
+                const uint32_t w = exec_wait(ax, base + nb, lane, avail);
+                if (w == WAIT_TIMEOUT) { e = B200Z_ERR_CUDA; break; }
+                if (w == WAIT_READY) {
+                    known = true; avail = 0xFFFFFFFFu;
+                    verdict = exec_seq_verdict(ax, seq_st, ax_flags);
+                    if (verdict != SEQ_GO) break;
+                }
+            }
+            const ExecBatch B = exec_load_batch(seqs, base, nb, nseq_u, lane, carry_out, carry_lit);
+            uint32_t offs[EXEC_PER_LANE], h0 = st.h0, h1 = st.h1, h2 = st.h2;
+            exec_batch_offsets(B, nb, resolved, bh0, bh1, bh2, lane, offs, h0, h1, h2);
+            const uint64_t reach = st.produced - st.drained;   // bytes of earlier output a match may reach back into
+            bool ok = true, ovl = false;
+#pragma unroll
+            for (uint32_t k = 0; k < EXEC_PER_LANE; k++) {
+                ok = ok && (!B.on[k] || (offs[k] != 0 && (uint64_t)offs[k] <= reach + B.mstart[k]));
+                ovl = ovl || offs[k] < B.ml[k];
+            }
+            const bool fast = __all_sync(0xffffffffu, ok) && B.T <= EXEC_TMAX && (uint64_t)st.litpos + B.L <= lit.regen && st.produced + B.T <= st.cap && !lit.rle;
+            if (!fast) {
+                uint32_t xof[EXEC_PER_LANE];   // actual offsets, or the raw values the exact path runs do_offset_history on
+#pragma unroll
+                for (uint32_t k = 0; k < EXEC_PER_LANE; k++) xof[k] = resolved ? offs[k] : B.of[k];
+                e = exec_batch_exact(st, lit, fd, out, nb, B.ll, B.ml, xof, resolved, lane);
+                continue;
+            }
+            if (!resolved) { st.h0 = h0; st.h1 = h1; st.h2 = h2; }
+            exec_batch_fast(st, lit, out, B, offs, ovl, a_mask, a_recs, lane, lt);
+        }
+        if (!e && st.litpos < lit.regen) {
+            uint32_t rest = lit.regen - st.litpos;
+            if (st.produced + rest > st.cap) e = B200Z_ERR_TARGET_TOO_SMALL;
+            else {
+                if (lit.rle) warp_fill(out + st.produced, lit.byte, rest, lane); else warp_copy(out + st.produced, lit.p + st.litpos, rest, lane);
+                st.produced += rest; st.counter += rest;
+            }
+        }
+        if (!known && e != B200Z_ERR_CUDA) {
+            // everything was consumed (or an execution error came up) before the sequence stage's verdict: it decides
+            // (progress never reaches ~0: only `ready` or the clock ends this wait)
+            uint32_t published;
+            if (exec_wait(ax, 0xFFFFFFFFu, lane, published) == WAIT_TIMEOUT) e = B200Z_ERR_CUDA;
+            else { known = true; verdict = exec_seq_verdict(ax, seq_st, ax_flags); }
+        }
+    } while (verdict == SEQ_REPLAY);
+    if (verdict == SEQ_FAILED) {   // decode_sequences failed: the reference executes nothing of this block (block_decoder.rs:176-183)
+        st = saved;
+        return seq_st;
+    }
+    if (e) return mk_status(e, e == B200Z_ERR_CUDA ? B200Z_STAGE_SEQUENCES : (e == B200Z_ERR_TARGET_TOO_SMALL ? B200Z_STAGE_DRAIN : B200Z_STAGE_EXECUTE));
+    if (resolved_u && d.nseq) block_hist_after(ax, bh0, bh1, bh2, st.h0, st.h1, st.h2);
+    return 0;
+}
 
 __global__ void __launch_bounds__(EXEC_WARPS * 32, EXEC_MINB) k_exec(const BlockDesc *__restrict__ descs, const BlockAux *__restrict__ aux,
                                                         const FrameDesc *__restrict__ frames, FrameState *__restrict__ states,
@@ -956,8 +1256,7 @@ __global__ void __launch_bounds__(EXEC_WARPS * 32, EXEC_MINB) k_exec(const Block
     ExecState st;
     st.h0 = fs.hist[0]; st.h1 = fs.hist[1]; st.h2 = fs.hist[2];
     st.produced = fs.produced; st.counter = fs.counter; st.drained = fs.drained;
-    st.cap = fd.out_cap;
-    if (fd.out_off > output_cap) st.cap = 0; else if (st.cap > output_cap - fd.out_off) st.cap = output_cap - fd.out_off;
+    st.cap = frame_out_room(fd, output_cap);
     uint8_t *out = output + fd.out_off;
     uint32_t status = fs.status, err_block = fs.error_block, blocks_done = fs.blocks_done;
 
@@ -977,257 +1276,14 @@ __global__ void __launch_bounds__(EXEC_WARPS * 32, EXEC_MINB) k_exec(const Block
         const uint32_t bs = block_first_error(d.host_status, ld_cg_u32(&aux[b].status), seq_st);
         if (bs) { status = bs; err_block = d.block_in_frame; break; }
 
-        if (d.btype == BT_RAW) {
+        if (d.btype != BT_COMPRESSED) {
             if (st.produced + d.raw_size > st.cap) { status = mk_status(B200Z_ERR_TARGET_TOO_SMALL, B200Z_STAGE_DRAIN); err_block = d.block_in_frame; break; }
-            warp_copy(out + st.produced, input + d.src_off, d.raw_size, lane);
+            raw_rle_block(out + st.produced, d, input, lane, 32);
             st.produced += d.raw_size;   // extend_from_reader: total_output_counter untouched (decode_buffer.rs:66-72)
-        } else if (d.btype == BT_RLE) {
-            if (st.produced + d.raw_size > st.cap) { status = mk_status(B200Z_ERR_TARGET_TOO_SMALL, B200Z_STAGE_DRAIN); err_block = d.block_in_frame; break; }
-            warp_fill(out + st.produced, input[d.src_off], d.raw_size, lane);
-            st.produced += d.raw_size;
         } else {
-            LitSrc lit;
-            lit.rle = 0; lit.byte = 0; lit.regen = d.regen_size;
-            if (d.lit_type == LT_RAW) lit.p = input + d.src_off + d.lit_off;
-            else if (d.lit_type == LT_RLE) { lit.p = nullptr; lit.rle = 1; lit.byte = input[d.src_off + d.lit_off]; }
-            else lit.p = lit_scratch + d.lit_buf_off;
-            // the block's start: where a sequence-stage error / a replay by the exact path rolls back to
-            if (lane == 0) s_saved[threadIdx.x >> 5] = st;
-            __syncwarp();
-            uint32_t e, verdict, resolved_u, bh0, bh1, bh2;
-            do {   // once more when the exact path of k_fse rewrote the records the first run consumed
-                st = s_saved[threadIdx.x >> 5];
-                st.litpos = 0;
-                e = 0; verdict = SEQ_GO;
-                uint32_t avail = known ? 0xFFFFFFFFu : 0u;   // records that may be read
-                // block-level descriptor fields used inside the batch loop are consumed here once: a first use inside the loop
-                // would wait on a scoreboard shared with the record prefetch issued just before it (a full memory latency per batch)
-                resolved_u = (ax_flags & AUX_RAW_OFFSETS) ? 0u : 1u;
-                uint32_t nseq_u = d.nseq;
-                const uint32_t *seqs = seq_scratch + d.seq_buf_off * 3;
-                asm volatile("" : "+r"(resolved_u), "+r"(nseq_u), "+l"(seqs));
-                const bool resolved = resolved_u != 0;
-                __syncwarp();
-                // A batch is EXEC_BATCH sequences, EXEC_PER_LANE consecutive ones per lane (contiguous 12-byte records in prefix
-                // form {out_end, lit_end, of}: ll and ml are differences of neighbouring records); the next batch's records are
-                // requested into L2 one batch ahead.
-                constexpr uint32_t K = EXEC_PER_LANE;
-                uint32_t carry_out = 0, carry_lit = 0;   // prefix sums at the end of the previous batch
-                bh0 = st.h0; bh1 = st.h1; bh2 = st.h2;   // history at the block's start: what the symbols refer to
-                for (uint32_t base = 0; base < nseq_u && !e; base += EXEC_BATCH) {
-                    const uint32_t nb = nseq_u - base < EXEC_BATCH ? nseq_u - base : EXEC_BATCH;
-                    if (avail < base + nb) {   // wait for k_fse: either these records, or the end of the block's sequence stage
-                        const uint32_t w = exec_wait(aux[b], base + nb, lane, avail);
-                        if (w == WAIT_TIMEOUT) { e = B200Z_ERR_CUDA; break; }
-                        if (w == WAIT_READY) {
-                            known = true; avail = 0xFFFFFFFFu;
-                            verdict = exec_seq_verdict(aux[b], seq_st, ax_flags);
-                            if (verdict != SEQ_GO) break;
-                        }
-                    }
-                    uint32_t lls[K], mls[K], ofs[K], pe_out[K], pe_lit[K];
-                    bool on[K];
-                    const uint32_t old_out = carry_out, old_lit = carry_lit;
-                    {
-                        const uint32_t *sp = seqs + (uint64_t)(base + K * lane) * 3;
-                        uint32_t raw[3 * K];
-                        if (K * lane + K <= nb) {   // all my records exist: K * 12 contiguous bytes, 8-byte aligned
-    #pragma unroll
-                            for (uint32_t k = 0; k < 3 * K; k += 2) { const uint2 r = ld_cg_u32x2(sp + k); raw[k] = r.x; raw[k + 1] = r.y; }
-                        } else {
-    #pragma unroll
-                            for (uint32_t k = 0; k < K; k++) {
-                                const bool have = K * lane + k < nb;
-                                raw[3 * k] = have ? ld_cg_u32(sp + 3 * k) : 0u; raw[3 * k + 1] = have ? ld_cg_u32(sp + 3 * k + 1) : 0u; raw[3 * k + 2] = have ? ld_cg_u32(sp + 3 * k + 2) : 1u;
-                            }
-                        }
-                        // prefix form -> lengths: my first record's predecessor is the last record of the lane below (or the carry)
-                        uint32_t p_out = __shfl_up_sync(0xffffffffu, raw[3 * (K - 1)], 1), p_lit = __shfl_up_sync(0xffffffffu, raw[3 * (K - 1) + 1], 1);
-                        if (lane == 0) { p_out = carry_out; p_lit = carry_lit; }
-    #pragma unroll
-                        for (uint32_t k = 0; k < K; k++) {
-                            on[k] = K * lane + k < nb;
-                            const uint32_t ll = raw[3 * k + 1] - p_lit, ml = raw[3 * k] - p_out - ll;
-                            lls[k] = on[k] ? ll : 0u; mls[k] = on[k] ? ml : 0u; ofs[k] = raw[3 * k + 2];
-                            p_out = raw[3 * k]; p_lit = raw[3 * k + 1];
-                            pe_out[k] = p_out; pe_lit[k] = p_lit;
-                        }
-                        {   // carry: the batch's last record
-                            const uint32_t lastl = (nb - 1) / K, lasts = (nb - 1) % K;
-                            uint32_t co = raw[0], cl = raw[1];
-    #pragma unroll
-                            for (uint32_t k = 1; k < K; k++) { co = lasts == k ? raw[3 * k] : co; cl = lasts == k ? raw[3 * k + 1] : cl; }
-                            carry_out = __shfl_sync(0xffffffffu, co, lastl); carry_lit = __shfl_sync(0xffffffffu, cl, lastl);
-                        }
-                        if (base + EXEC_BATCH < nseq_u && lane * 128u < (nseq_u - base - EXEC_BATCH) * 12u && lane * 128u < EXEC_BATCH * 12u)
-                            prefetch_l2(reinterpret_cast<const uint8_t *>(seqs + (uint64_t)(base + EXEC_BATCH) * 3) + lane * 128u);
-                    }
-                    // the records are prefix sums already (k_fse): batch totals and batch-relative positions are differences
-                    const uint32_t T = carry_out - old_out, L = carry_lit - old_lit;
-                    // per sequence: inclusive end of its bytes, start of its match, inclusive end of its literals (all batch-relative)
-                    uint32_t oend[K], mstart[K], lend[K];
-    #pragma unroll
-                    for (uint32_t k = 0; k < K; k++) { oend[k] = on[k] ? pe_out[k] - old_out : T; lend[k] = on[k] ? pe_lit[k] - old_lit : L; mstart[k] = oend[k] - mls[k]; }
-                    // actual offsets: symbols resolve against the history at the block's start; a block flagged AUX_RAW_OFFSETS
-                    // (exact path of k_fse) runs do_offset_history here, sequence by sequence
-                    uint32_t offs[K];
-    #pragma unroll
-                    for (uint32_t k = 0; k < K; k++) offs[k] = resolved ? seq_sym_resolve(ofs[k], bh0, bh1, bh2) : ofs[k];
-                    uint32_t h0 = st.h0, h1 = st.h1, h2 = st.h2;
-                    if (!resolved) {
-                        // cheap scalar steps (sequence_execution.rs:59-118); committed only if the fast path is taken (the exact path
-                        // redoes the steps itself)
-                        for (uint32_t j = 0; j < nb; j++) {
-                            const uint32_t slot = j % K, src_lane = j / K;
-                            uint32_t ll = __shfl_sync(0xffffffffu, exec_pick(lls, slot), src_lane), of = __shfl_sync(0xffffffffu, exec_pick(ofs, slot), src_lane);
-                            uint32_t actual = offset_history_step(of, ll, h0, h1, h2);
-                            if (lane == src_lane) {
-    #pragma unroll
-                                for (uint32_t k = 0; k < K; k++) offs[k] = slot == k ? actual : offs[k];
-                            }
-                        }
-                    }
-                    const uint64_t reach = st.produced - st.drained;   // bytes of earlier output a match may reach back into
-                    bool ok = true, ovl = false;
-    #pragma unroll
-                    for (uint32_t k = 0; k < K; k++) {
-                        ok = ok && (!on[k] || (offs[k] != 0 && (uint64_t)offs[k] <= reach + mstart[k]));
-                        ovl = ovl || offs[k] < mls[k];
-                    }
-                    const bool fast = __all_sync(0xffffffffu, ok) && T <= EXEC_TMAX && (uint64_t)st.litpos + L <= lit.regen && st.produced + T <= st.cap && !lit.rle;
-                    if (!fast) {
-                        e = exec_batch_exact(st, lit, fd, out, nb, lls, mls, resolved ? offs : ofs, resolved, lane);
-                        continue;
-                    }
-                    if (!resolved) { st.h0 = h0; st.h1 = h1; st.h2 = h2; }
-                    // ---------------- fast path
-                    // Sequence j owns the bytes [lit_begin_j, out_end_j): its literal run, then its match.  A bit is set at
-                    // the last byte of every sequence, so the owner of output byte q is the number of set bits below q;
-                    // one 8-byte shared-memory record per sequence then tells the byte where it comes from.
-                    const uint32_t nrows = (T + 31) >> 5;
-                    // The batch's match sources are scattered over the frame's window, and with thousands of frames in flight the
-                    // windows do not stay in L2: ask for the sectors now, a few hundred instructions before the rows need them.
-    #pragma unroll
-                    for (uint32_t k = 0; k < K; k++) {
-                        if (on[k]) {
-                            const uint8_t *src = out + st.produced + mstart[k] - offs[k];
-                            prefetch_l2(src);
-                            if ((((uint32_t)(uintptr_t)src) & 31u) + mls[k] > 32u) prefetch_l2(src + mls[k] - 1);
-                        }
-                    }
-                    if (lane == 31 && lit.regen) {
-                        const uint32_t ahead = st.litpos + L + 256u;   // the literal stream is sequential: stay two lines ahead
-                        prefetch_l2(lit.p + (ahead < lit.regen ? ahead : lit.regen - 1));
-                    }
-                    sts32(a_mask + (lane << 2), 0u);
-                    if (nrows > 32u - EXEC_CHUNK_ROWS)
-                        for (uint32_t w = lane + 32; w < ((nrows + EXEC_CHUNK_ROWS - 1u) & ~(EXEC_CHUNK_ROWS - 1u)); w += 32) sts32(a_mask + (w << 2), 0u);
-                    // 8-byte record: literal byte q of the sequence is literal number (q - m_before) of the batch (m_before = match bytes
-                    // of the earlier sequences = match start - literal end), match byte q comes from output position q - offset
-                    // (m_start, m_before <= EXEC_TMAX: 16 bits each)
-    #pragma unroll
-                    for (uint32_t k = 0; k < K; k += 2)
-                        sts128(a_recs + ((K * lane + k) << 3), mstart[k] | ((mstart[k] - lend[k]) << 16), offs[k], mstart[k + 1] | ((mstart[k + 1] - lend[k + 1]) << 16), offs[k + 1]);
-                    const bool has_ovl = __any_sync(0xffffffffu, ovl);   // some match overlaps its own output (rare)
-                    __syncwarp();
-    #pragma unroll
-                    for (uint32_t k = 0; k < K; k++)
-                        if (on[k]) red_or_shared(a_mask + (((oend[k] - 1) >> 5) << 2), 1u << ((oend[k] - 1) & 31u));
-                    __syncwarp();
-                    uint8_t *bout = out + st.produced;
-                    const uint8_t *litq = lit.p + st.litpos;
-                    asm volatile("" : "+l"(bout), "+l"(litq));   // keep both bases as single 64-bit registers (one add per access)
-                    uint32_t before = 0;   // sequences ended in earlier rows
-                    // Rows are produced EXEC_CHUNK_ROWS at a time: every byte whose source lies before the chunk (literals, and
-                    // matches reaching back past the chunk start) is loaded first -- EXEC_CHUNK_ROWS independent loads per lane in
-                    // flight -- then stored; the few bytes whose source lies inside the chunk follow, row by row.  (Issuing the
-                    // next chunk's loads before this chunk's stores was measured slower: more bytes turn dependent.)
-                    // The per-byte work is branch-free: one select between the literal and the match source.
-                    // tag: TAG_NONE = nothing to do, TAG_STORE = value loaded, otherwise the (batch-relative, >= floor) source
-                    // position of a match byte that had to wait.
-                    constexpr int32_t TAG_NONE = INT32_MIN, TAG_STORE = INT32_MIN + 1;
-                    constexpr int R = (int)EXEC_CHUNK_ROWS;
-                    auto load_chunk = [&](uint32_t r0, int32_t floor, uint32_t (&val)[R], int32_t (&tag)[R]) {
-    #pragma unroll
-                        for (int i = 0; i < R; i++) {
-                            const uint32_t q = ((r0 + i) << 5) + lane;
-                            const uint32_t word = lds32(a_mask + ((r0 + i) << 2));
-                            const uint32_t owner = before + __popc(word & lt);   // sequences that ended below q
-                            before += __popc(word);
-                            const uint2 rc = lds64(a_recs + ((owner & (EXEC_BATCH - 1u)) << 3));
-                            const uint32_t mst = rc.x & 0xffffu;
-                            const bool is_match = q >= mst;
-                            int32_t sp = (int32_t)q - (int32_t)rc.y;                  // batch-relative source of a match byte
-                            if (has_ovl) {                                            // overlapping match: byte k comes from k mod offset
-                                const uint32_t kk = q - mst;
-                                if (is_match && kk >= rc.y) sp = (int32_t)mst - (int32_t)rc.y + (int32_t)(kk % rc.y);
-                            }
-                            const bool valid = q < T;
-                            const bool dep = is_match && sp >= floor;
-                            const int32_t idx = is_match ? sp : (int32_t)(q - (rc.x >> 16));
-                            const uint8_t *bp = is_match ? (const uint8_t *)bout : litq;
-                            tag[i] = valid ? (dep ? sp : TAG_STORE) : TAG_NONE;
-                            val[i] = 0;
-                            if (valid && !dep) val[i] = bp[idx];
-                        }
-                    };
-                    auto store_chunk = [&](uint32_t r0, int32_t floor, const uint32_t (&val)[R], const int32_t (&tag)[R]) {
-    #pragma unroll
-                        for (int i = 0; i < R; i++)
-                            if (tag[i] == TAG_STORE) bout[((r0 + i) << 5) + lane] = (uint8_t)val[i];
-                        // dependent bytes, rows in order (sources in earlier rows are final, inside the row the lowest pending byte is ready)
-                        bool anydep = false;
-    #pragma unroll
-                        for (int i = 0; i < R; i++) anydep |= tag[i] >= floor;
-                        if (__any_sync(0xffffffffu, anydep)) {
-    #pragma unroll
-                            for (int i = 0; i < R; i++) {
-                                bool mine = tag[i] >= floor;
-                                uint32_t pending = __ballot_sync(0xffffffffu, mine);
-                                const int32_t row0 = (int32_t)((r0 + i) << 5);
-                                while (pending) {
-                                    __syncwarp();
-                                    bool ready = mine && (tag[i] < row0 || !((pending >> (tag[i] - row0)) & 1u));
-                                    if (ready) { bout[row0 + (int32_t)lane] = bout[tag[i]]; mine = false; }
-                                    pending &= ~__ballot_sync(0xffffffffu, ready);
-                                }
-                            }
-                        }
-                        __syncwarp();
-                    };
-                    for (uint32_t r0 = 0; r0 < nrows; r0 += R) {
-                        uint32_t va[R]; int32_t ta[R];
-                        load_chunk(r0, (int32_t)(r0 << 5), va, ta);
-                        store_chunk(r0, (int32_t)(r0 << 5), va, ta);
-                    }
-                    __syncwarp();
-                    st.produced += T; st.counter += T; st.litpos += L;
-                }
-                if (!e && st.litpos < lit.regen) {
-                    uint32_t rest = lit.regen - st.litpos;
-                    if (st.produced + rest > st.cap) e = B200Z_ERR_TARGET_TOO_SMALL;
-                    else {
-                        if (lit.rle) warp_fill(out + st.produced, lit.byte, rest, lane); else warp_copy(out + st.produced, lit.p + st.litpos, rest, lane);
-                        st.produced += rest; st.counter += rest;
-                    }
-                }
-                if (!known && e != B200Z_ERR_CUDA) {
-                    // everything was consumed (or an execution error came up) before the sequence stage's verdict: it decides
-                    // (progress never reaches ~0: only `ready` or the clock ends this wait)
-                    uint32_t published;
-                    if (exec_wait(aux[b], 0xFFFFFFFFu, lane, published) == WAIT_TIMEOUT) e = B200Z_ERR_CUDA;
-                    else { known = true; verdict = exec_seq_verdict(aux[b], seq_st, ax_flags); }
-                }
-            } while (verdict == SEQ_REPLAY);
-            if (verdict == SEQ_FAILED) {   // decode_sequences failed: the reference executes nothing of this block (block_decoder.rs:176-183)
-                st = s_saved[threadIdx.x >> 5];
-                status = seq_st; err_block = d.block_in_frame; break;
-            }
-            if (e) { status = mk_status(e, e == B200Z_ERR_CUDA ? B200Z_STAGE_SEQUENCES : (e == B200Z_ERR_TARGET_TOO_SMALL ? B200Z_STAGE_DRAIN : B200Z_STAGE_EXECUTE)); err_block = d.block_in_frame; break; }
-            if (resolved_u && d.nseq) {   // the history after the block, in terms of the history at its start
-                const uint32_t a0 = ld_cg_u32(&aux[b].hist_after[0]), a1 = ld_cg_u32(&aux[b].hist_after[1]), a2 = ld_cg_u32(&aux[b].hist_after[2]);
-                st.h0 = seq_sym_resolve(a0, bh0, bh1, bh2); st.h1 = seq_sym_resolve(a1, bh0, bh1, bh2); st.h2 = seq_sym_resolve(a2, bh0, bh1, bh2);
-            }
+            status = exec_compressed_block(st, s_saved[threadIdx.x >> 5], d, aux[b], fd, out, input, lit_scratch, seq_scratch, known, seq_st, ax_flags, a_mask,
+                                           a_recs, lane, lt);
+            if (status) { err_block = d.block_in_frame; break; }
         }
         __syncwarp();
         blocks_done++;
