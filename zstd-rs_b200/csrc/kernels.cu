@@ -796,8 +796,8 @@ __global__ void __launch_bounds__(32) k_fse(const BlockDesc *__restrict__ descs,
 // Fast path (per batch of 64 sequences, lane j = sequences 2j and 2j + 1): one warp scan gives every sequence its
 // literal and match positions; a bitmask of sequence ends in shared memory lets each OUTPUT byte find its owner
 // with one popc, an 8-byte record per sequence tells it where it comes from; the batch's bytes are then produced
-// row by row (32 consecutive bytes = one coalesced store), four rows' loads in flight: literal bytes and match
-// bytes whose source is final first, then the few match bytes whose source lies inside the same four rows,
+// row by row (32 consecutive bytes = one coalesced store), eight rows' loads in flight: literal bytes and match
+// bytes whose source is final first, then the few match bytes whose source lies inside the same eight rows,
 // looping inside a row until it is complete (sources always precede destinations, so the lowest pending byte is
 // always ready).  Overlapping matches use source = start + (k mod offset), the byte-order-preserving form of
 // repeat_in_chunks (decode_buffer.rs:113-141).  Anything unusual in a batch (dictionary reach, zero offsets,
@@ -951,7 +951,9 @@ __device__ __forceinline__ void block_hist_after(const BlockAux &a, uint32_t b0,
 
 constexpr uint32_t EXEC_WARPS = 4;
 constexpr uint32_t EXEC_TMAX = 8128;         // most bytes one batch may produce on the fast path (sizes the end-bit mask)
-constexpr uint32_t EXEC_CHUNK_ROWS = 4;      // rows (of 32 bytes) whose loads are in flight together
+// rows (of 32 bytes) whose loads are in flight together.  8 instead of 4: k_exec alone 6 % faster on C2b (H100 80GB HBM3, 400 W
+// power limit), with 66 / 88 bytes of spill stores / loads per thread instead of 48 / 48; 16 spills ~200 bytes per thread.
+constexpr uint32_t EXEC_CHUNK_ROWS = 8;
 constexpr uint32_t EXEC_MASK_WORDS = (EXEC_TMAX + 31) / 32 + EXEC_CHUNK_ROWS;
 // CTAs per SM the register budget must allow: 6 gives 80 registers (few spills).  On an H100 this runs k_exec ~19 % faster
 // than 8 (64 registers, ~190 bytes of spills per thread); 4 and 5 measure the same as 6.
@@ -1100,14 +1102,16 @@ __device__ __forceinline__ void exec_store_chunk(uint8_t *bout, uint32_t r0, int
 // out_end_j): its literal run, then its match.  A bit is set at the last byte of every sequence, so the owner of output byte q
 // is the number of set bits below q; one 8-byte shared-memory record per sequence then tells the byte where it comes from.
 __device__ __forceinline__ void exec_batch_fast(ExecState &st, const LitSrc &lit, uint8_t *out, const ExecBatch &B, const uint32_t (&offs)[EXEC_PER_LANE],
-                                                bool ovl, uint32_t a_mask, uint32_t a_recs, uint32_t lane, uint32_t lt) {
+                                                bool ovl, bool far_sources, uint32_t a_mask, uint32_t a_recs, uint32_t lane, uint32_t lt) {
     constexpr uint32_t K = EXEC_PER_LANE;
     const uint32_t nrows = (B.T + 31) >> 5;
-    // The batch's match sources are scattered over the frame's window, and with thousands of frames in flight the windows do
-    // not stay in L2: ask for the sectors now, a few hundred instructions before the rows need them.
+    // In a block that follows earlier output of its frame (far_sources), match sources may lie in earlier blocks, written long
+    // before and no longer in L2 with thousands of frames in flight: ask for the sectors now, a few hundred instructions before
+    // the rows need them.  In a frame's first block every source was written by this warp a moment ago; there the prefetches
+    // only cost issue slots (C2b, single-block frames: 3.7 % faster passes without them, DESIGN.md section 6).
 #pragma unroll
     for (uint32_t k = 0; k < K; k++) {
-        if (B.on[k]) {
+        if (far_sources && B.on[k]) {
             const uint8_t *src = out + st.produced + B.mstart[k] - offs[k];
             prefetch_l2(src);
             if ((((uint32_t)(uintptr_t)src) & 31u) + B.ml[k] > 32u) prefetch_l2(src + B.ml[k] - 1);
@@ -1207,7 +1211,9 @@ __device__ __forceinline__ uint32_t exec_compressed_block(ExecState &st, ExecSta
                 continue;
             }
             if (!resolved) { st.h0 = h0; st.h1 = h1; st.h2 = h2; }
-            exec_batch_fast(st, lit, out, B, offs, ovl, a_mask, a_recs, lane, lt);
+            // (the block's start is read back from shared memory: a flag kept in a register across the loop costs spills)
+            const bool far_sources = saved.produced != saved.drained;   // the frame has output before this block that matches may reach
+            exec_batch_fast(st, lit, out, B, offs, ovl, far_sources, a_mask, a_recs, lane, lt);
         }
         if (!e && st.litpos < lit.regen) {
             uint32_t rest = lit.regen - st.litpos;
