@@ -189,7 +189,7 @@ extern "C" int b200z_dict_create(b200z_ctx *c, const uint8_t *raw, size_t len, b
     if (memcmp(raw, magic, 4) != 0) return B200Z_ERR_DICT_BAD_MAGIC_NUM;
     std::unique_ptr<b200z_dict, void (*)(b200z_dict *)> d(new b200z_dict(), dict_free);
     d->ctx = c;
-    d->id = (uint32_t)raw[4] | ((uint32_t)raw[5] << 8) | ((uint32_t)raw[6] << 16) | ((uint32_t)raw[7] << 24);
+    d->id = rd32le(raw + 4);
     const uint8_t *t = raw + 8;
     size_t tl = len - 8;
     std::unique_ptr<HufSlot> huf(new HufSlot());
@@ -209,7 +209,7 @@ extern "C" int b200z_dict_create(b200z_ctx *c, const uint8_t *raw, size_t len, b
         t += used; tl -= used;
     }
     if (tl < 12) return B200Z_ERR_DICT_NOT_ENOUGH_BYTES;
-    for (int i = 0; i < 3; i++) d->hist[i] = (uint32_t)t[4 * i] | ((uint32_t)t[4 * i + 1] << 8) | ((uint32_t)t[4 * i + 2] << 16) | ((uint32_t)t[4 * i + 3] << 24);
+    for (int i = 0; i < 3; i++) d->hist[i] = rd32le(t + 4 * i);
     d->has_tables = true;
     CU(c, cudaMalloc((void **)&d->d_huf, sizeof(HufSlot)));
     CU(c, cudaMalloc((void **)&d->d_fse, sizeof(FseSlot)));
@@ -303,21 +303,23 @@ struct Submission {
         if (ci >= 0) cursor_from_carry(cur, carries[ci], (uint32_t)ci);
         return cur;
     }
-    // Appends a block.  A Compressed block is planned from its content, or from the section headers k_walk brought back (`view`);
+    // Appends a block.  A Compressed block is planned from its section headers, as parsed here from its content or by k_walk (`sec`);
     // `cur` moves on to the tables it leaves current.
-    const BlockDesc &add_block(uint64_t src_off, const BlockHeader &bh, uint32_t frame, uint32_t block_in_frame, const uint8_t *content,
-                               const WalkBlock *view, TableCursor &cur) {
+    const BlockDesc &add_block(uint64_t src_off, const BlockHeader &bh, uint32_t frame, uint32_t block_in_frame, const SectionHeaders &sec,
+                               TableCursor &cur) {
         BlockDesc d;
         memset(&d, 0, sizeof d);
         BlockRefs r;
         d.src_off = src_off; d.src_size = bh.content_size; d.frame = frame; d.btype = bh.type; d.raw_size = bh.decompressed_size;
         d.block_in_frame = block_in_frame; d.last = bh.last;
-        if (bh.type == BT_COMPRESSED) {
-            if (view) plan_compressed_block_view(view->lit, view->seq, bh.content_size, d, r, cur, n_huf, n_fse, lit_bytes, nseq);
-            else plan_compressed_block(content, bh.content_size, d, r, cur, n_huf, n_fse, lit_bytes, nseq);
-        }
+        if (bh.type == BT_COMPRESSED) plan_compressed_block(sec, d, r, cur, n_huf, n_fse, lit_bytes, nseq);
         descs.push_back(d); refs.push_back(r);
         return descs.back();
+    }
+    const BlockDesc &add_block(uint64_t src_off, const BlockHeader &bh, uint32_t frame, uint32_t block_in_frame, const uint8_t *content,
+                               TableCursor &cur) {
+        const SectionHeaders sec = bh.type == BT_COMPRESSED ? parse_section_headers(content, bh.content_size) : SectionHeaders();
+        return add_block(src_off, bh, frame, block_in_frame, sec, cur);
     }
     // resolve table references to device pointers and upload descriptors
     int upload(b200z_ctx *c, cudaStream_t stream = nullptr) {
@@ -498,7 +500,8 @@ static int plan_batch(b200z_batch *b, const uint8_t *in, size_t in_len, const b2
                 fd.host_status = mk_status(bh.type == BT_COMPRESSED ? B200Z_ERR_BLOCK_CONTENT_READ : B200Z_ERR_BLOCK_BODY_READ, B200Z_STAGE_BLOCK_BODY);
                 break;
             }
-            const BlockDesc &d = s.add_block(io.src_off + pos, bh, (uint32_t)fi.sub_frame, bif++, wbk ? nullptr : p + pos, wbk, cur);
+            const BlockDesc &d = wbk ? s.add_block(io.src_off + pos, bh, (uint32_t)fi.sub_frame, bif++, wbk->sec, cur)
+                                     : s.add_block(io.src_off + pos, bh, (uint32_t)fi.sub_frame, bif++, p + pos, cur);
             pos += bh.content_size;
             bytes_read += 3 + bh.content_size;
             b->block_end_bytes.push_back(bytes_read);
@@ -508,8 +511,7 @@ static int plan_batch(b200z_batch *b, const uint8_t *in, size_t in_len, const b2
                     if (len - pos < 4) { fd.host_status = mk_status(B200Z_ERR_FAILED_TO_READ_CHECKSUM, B200Z_STAGE_CHECKSUM); break; }
                     fi.has_checksum = true;
                     if (walk && (walk->wf[i].end_pos != pos || walk->wf[i].tail_avail < 4)) return B200Z_ERR_INVALID_ARGUMENT;
-                    const uint8_t *q = walk ? walk->wf[i].tail : p + pos;
-                    fi.checksum = (uint32_t)q[0] | ((uint32_t)q[1] << 8) | ((uint32_t)q[2] << 16) | ((uint32_t)q[3] << 24);
+                    fi.checksum = rd32le(walk ? walk->wf[i].tail : p + pos);
                     bytes_read += 4;
                 }
                 break;
@@ -521,7 +523,7 @@ static int plan_batch(b200z_batch *b, const uint8_t *in, size_t in_len, const b2
     return 0;
 }
 
-// k_walk twice (count, fill) with a host prefix sum in between; ~16 bytes per block and 48 per frame come back
+// k_walk twice (count, fill) with a host prefix sum in between; 40 bytes per block and 48 per frame come back
 static int device_walk(b200z_ctx *c, const uint8_t *d_input, size_t input_len, const b200z_frame_io *frames, size_t nframes, WalkHost &w) {
     w.wf.assign(nframes, WalkFrame()); w.first.assign(nframes, 0); w.wb.clear();
     if (!nframes) return 0;
@@ -562,8 +564,8 @@ extern "C" int b200z_batch_prepare(b200z_ctx *c, const uint8_t *input, size_t in
     const bool on_device = input_mem == B200Z_MEM_DEVICE;
     WalkHost walk;
     if (on_device) {
-        // The input stays on the device: k_walk follows the frame / block / section headers there and brings back the ~16 bytes per
-        // block the planner parses (SURVEY.md 8(f).3) -- not the compressed data.
+        // The input stays on the device: k_walk parses the frame / block / section headers there and brings back what the planner
+        // needs of each block (SURVEY.md 8(f).3) -- not the compressed data.
         b->d_input = input;
         if (int e = device_walk(c, input, input_len, frames, nframes, walk)) return e;
     }
@@ -1025,13 +1027,14 @@ extern "C" int b200z_decode_blocks_batch(b200z_ctx *c, const b200z_block_desc *b
             BlockHeader bh;
             bh.last = bd.last_block; bh.type = bd.block_type; bh.decompressed_size = bd.decompressed_size; bh.content_size = bd.content_size;
             sub_of[bf.first_block + k] = (int64_t)s.descs.size();
-            const BlockDesc &d = s.add_block(bd.src_off, bh, (uint32_t)f, k, hin + bd.src_off, nullptr, cur);
-            if (bd.block_type == BT_COMPRESSED) {
-                // the descriptor says what the caller's parsers found: it must be what the content says
-                // the planner sets lit_off (>= 1) once it has parsed the literals header; an error before that leaves it 0
-                if (d.lit_off != 0 && (d.lit_type != bd.literals_type || d.regen_size != bd.regenerated_size)) return B200Z_ERR_INVALID_ARGUMENT;
-                if (!d.host_status && (d.nseq != bd.num_sequences || (d.nseq && d.modes != bd.modes))) return B200Z_ERR_INVALID_ARGUMENT;
+            SectionHeaders sec = {};
+            if (bh.type == BT_COMPRESSED) {
+                // the descriptor says what the caller's parsers found: it must be what the content says, as far as its headers parse
+                sec = parse_section_headers(hin + bd.src_off, bh.content_size);
+                if (sec.lit_off != 0 && (sec.lit_type != bd.literals_type || sec.regen_size != bd.regenerated_size)) return B200Z_ERR_INVALID_ARGUMENT;
+                if (!sec.status && (sec.nseq != bd.num_sequences || (sec.nseq && sec.modes != bd.modes))) return B200Z_ERR_INVALID_ARGUMENT;
             }
+            const BlockDesc &d = s.add_block(bd.src_off, bh, (uint32_t)f, k, sec, cur);
             if (d.host_status) break;   // decompress_block would have returned here: later blocks of the frame are never reached
         }
         s.frames.back().nblocks = (uint32_t)s.descs.size() - s.frames.back().first_block;
@@ -1153,11 +1156,12 @@ extern "C" uint32_t b200z_frame_decoder_skip_frame_length(const b200z_frame_deco
 extern "C" int b200z_frame_decoder_last_stage(const b200z_frame_decoder *d) { return d->last_stage; }
 extern "C" const char *b200z_frame_decoder_last_error_message(const b200z_frame_decoder *d) { return d->err.c_str(); }
 
-static bool read_exact(b200z_read_fn rd, void *user, uint8_t *buf, size_t n) {
+static size_t read_upto(b200z_read_fn rd, void *user, uint8_t *buf, size_t n) {   // stops at the end of the source; returns the bytes read
     size_t got = 0;
-    while (got < n) { long r = rd(user, buf + got, n - got); if (r <= 0) return false; got += (size_t)r; }
-    return true;
+    while (got < n) { long r = rd(user, buf + got, n - got); if (r <= 0) break; got += (size_t)r; }
+    return got;
 }
+static bool read_exact(b200z_read_fn rd, void *user, uint8_t *buf, size_t n) { return read_upto(rd, user, buf, n) == n; }
 
 static void fd_apply_dict(b200z_frame_decoder *d, const b200z_dict *dict) {  // DecoderScratch::init_from_dict, scratch.rs:70-78
     d->carry = carry_of_dict(dict);
@@ -1165,35 +1169,19 @@ static void fd_apply_dict(b200z_frame_decoder *d, const b200z_dict *dict) {  // 
     d->using_dict = dict;
 }
 
-// reset (frame_decoder.rs:200-221): read the header through the callback exactly like read_frame_header does
+// reset (frame_decoder.rs:200-221): read the header through the callback as read_frame_header does -- the magic number, then the
+// descriptor byte (or a skippable frame's length), then the rest of the header -- and never a byte past it
 extern "C" int b200z_frame_decoder_reset(b200z_frame_decoder *d, b200z_read_fn rd, void *user) {
     if (!d || !rd) return B200Z_ERR_INVALID_ARGUMENT;
     uint8_t buf[32];
-    // pull the header piecewise so that no byte beyond it is consumed (frame.rs:6-85)
     size_t have = 0;
-    auto need = [&](size_t n) { if (have >= n) return true; if (!read_exact(rd, user, buf + have, n - have)) return false; have = n; return true; };
-    FrameHeader h; uint32_t skip = 0; size_t consumed = 0;
-    if (!need(4)) return fd_fail(d, B200Z_ERR_MAGIC_NUMBER_READ, B200Z_STAGE_FRAME_HEADER);
-    uint32_t magic = (uint32_t)buf[0] | ((uint32_t)buf[1] << 8) | ((uint32_t)buf[2] << 16) | ((uint32_t)buf[3] << 24);
-    if (magic >= 0x184D2A50u && magic <= 0x184D2A5Fu) {
-        if (!need(8)) return fd_fail(d, B200Z_ERR_FRAME_DESCRIPTOR_READ, B200Z_STAGE_FRAME_HEADER);
-        parse_frame_header(buf, 8, h, skip, consumed);
-        d->skip_len = skip;
-        return fd_fail(d, B200Z_ERR_SKIP_FRAME, B200Z_STAGE_FRAME_HEADER);
+    for (size_t want; (want = frame_header_want(buf, have)) > have;) {
+        have += read_upto(rd, user, buf + have, want - have);
+        if (have < want) break;   // parse_frame_header names the field that could not be read
     }
-    if (magic != 0xFD2FB528u) return fd_fail(d, B200Z_ERR_BAD_MAGIC_NUMBER, B200Z_STAGE_FRAME_HEADER);
-    if (!need(5)) return fd_fail(d, B200Z_ERR_FRAME_DESCRIPTOR_READ, B200Z_STAGE_FRAME_HEADER);
-    uint8_t desc = buf[4];
-    size_t pos = 5;
-    bool single = (desc >> 5) & 1;
-    if (!single) { if (!need(pos + 1)) return fd_fail(d, B200Z_ERR_WINDOW_DESCRIPTOR_READ, B200Z_STAGE_FRAME_HEADER); pos += 1; }
-    static const uint8_t did_len[4] = {0, 1, 2, 4};
-    size_t dl = did_len[desc & 3];
-    if (dl) { if (!need(pos + dl)) return fd_fail(d, B200Z_ERR_DICTIONARY_ID_READ, B200Z_STAGE_FRAME_HEADER); pos += dl; }
-    uint32_t flag = desc >> 6;
-    size_t fl = flag == 0 ? (single ? 1 : 0) : (flag == 1 ? 2 : (flag == 2 ? 4 : 8));
-    if (fl) { if (!need(pos + fl)) return fd_fail(d, B200Z_ERR_FRAME_CONTENT_SIZE_READ, B200Z_STAGE_FRAME_HEADER); pos += fl; }
-    int e = parse_frame_header(buf, pos, h, skip, consumed);
+    FrameHeader h; uint32_t skip = 0; size_t consumed = 0;
+    int e = parse_frame_header(buf, have, h, skip, consumed);
+    if (e == B200Z_ERR_SKIP_FRAME) d->skip_len = skip;
     if (e) return fd_fail(d, e, B200Z_STAGE_FRAME_HEADER);
     uint64_t window = 0;
     if ((e = frame_window_size(h, window))) return fd_fail(d, e, B200Z_STAGE_FRAME_HEADER);
@@ -1392,7 +1380,7 @@ static int fd_decode_blocks_impl(b200z_frame_decoder *d, b200z_read_fn rd, void 
                 pending_err = bh.type == BT_COMPRESSED ? B200Z_ERR_BLOCK_CONTENT_READ : B200Z_ERR_BLOCK_BODY_READ; pending_stage = B200Z_STAGE_BLOCK_BODY;
                 break;
             }
-            const BlockDesc &bd = s.add_block(off, bh, 0, (uint32_t)(d->block_counter + s.descs.size()), d->staging.data() + off, nullptr, cur);
+            const BlockDesc &bd = s.add_block(off, bh, 0, (uint32_t)(d->block_counter + s.descs.size()), d->staging.data() + off, cur);
             brc += bh.content_size;
             bytes_after.push_back(brc);
             if (bd.host_status) break;
@@ -1419,7 +1407,7 @@ static int fd_decode_blocks_impl(b200z_frame_decoder *d, b200z_read_fn rd, void 
                 uint8_t cs[4];
                 if (!read_exact(rd, user, cs, 4)) return fd_fail(d, B200Z_ERR_FAILED_TO_READ_CHECKSUM, B200Z_STAGE_CHECKSUM);
                 d->bytes_read_counter += 4;
-                d->check_sum = (uint32_t)cs[0] | ((uint32_t)cs[1] << 8) | ((uint32_t)cs[2] << 16) | ((uint32_t)cs[3] << 24);
+                d->check_sum = rd32le(cs);
                 d->has_check_sum = true;
             }
             break;
@@ -1500,7 +1488,7 @@ extern "C" int b200z_frame_decoder_decode_from_to(b200z_frame_decoder *d, const 
         if (d->hdr.content_checksum() && d->frame_finished && !d->has_check_sum) {  // :465-477
             if (mt.len >= 4) {
                 d->bytes_read_counter += 4;
-                d->check_sum = (uint32_t)mt.p[0] | ((uint32_t)mt.p[1] << 8) | ((uint32_t)mt.p[2] << 16) | ((uint32_t)mt.p[3] << 24);
+                d->check_sum = rd32le(mt.p);
                 d->has_check_sum = true;
             }
             *read = 4; *written = 0;

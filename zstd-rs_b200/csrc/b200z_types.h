@@ -15,6 +15,15 @@
 #pragma once
 #include <stdint.h>
 
+// functions compiled for both the device and the host (tables.cuh, framing.cuh)
+#ifdef __CUDACC__
+#define B200Z_HD __host__ __device__ __forceinline__
+#define B200Z_HDN __host__ __device__
+#else
+#define B200Z_HD inline
+#define B200Z_HDN
+#endif
+
 namespace b200z {
 
 // ---- block types / literal types as on the wire (block_decoder.rs:259-268, literals_section.rs:226-235)
@@ -156,29 +165,6 @@ struct alignas(16) FrameDesc {
     uint32_t nblocks;
     uint32_t host_status;     // planner error that ends the frame after `nblocks` blocks (code | stage << 16)
     uint32_t pad;
-};
-
-// ---- device-side header walk (k_walk): what the host planner needs of a frame that lives in device memory -- the frame header,
-// every block's 3-byte header, the first bytes of its literals section and sequences section headers, the checksum -- instead of
-// copying the compressed input back to the host (frame.rs:6-85, block_decoder.rs:201-283, literals_section.rs:117-223,
-// sequence_section.rs:108-167 locate these bytes; the planner re-parses them with the same code it uses on host input)
-struct WalkFrame {
-    uint8_t hdr[20];      // the frame's first bytes (magic .. frame header), zero padded
-    uint32_t hdr_avail;   // how many of them exist
-    uint32_t nblocks;     // block digests of this frame
-    uint32_t stop;        // 0 last block seen, 1 block header truncated, 2 reserved type / size too large, 3 content truncated, 4 no walk (frame header)
-    uint32_t tail_avail;  // bytes available after the last block (up to 4: the content checksum)
-    uint8_t tail[4];
-    uint32_t pad;
-    uint64_t end_pos;     // frame-relative position after the last walked block
-};
-struct WalkBlock {
-    uint64_t pos;         // frame-relative position of the 3-byte block header
-    uint32_t seq_off;     // offset of the sequences section header inside the block content (0 = not reachable)
-    uint8_t bh[3], lit_avail;
-    uint8_t lit[5], seq_avail;
-    uint8_t seq[4];
-    uint8_t pad[6];
 };
 
 // ---- status words: code | stage << 16 (b200z_error, B200Z_STAGE_*), 0 = ok

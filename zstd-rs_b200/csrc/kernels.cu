@@ -1323,95 +1323,56 @@ __global__ void k_xxh64(const FrameDesc *__restrict__ frames, FrameState *__rest
 
 // ------------------------------------------------------------------------------------------------------------
 // k_walk: the frame / block / section header walk on the device, for input that lives in device memory (SURVEY 8(f) rank 3,
-// first step).  One thread per frame follows the chain of 3-byte block headers (read_block_header, block_decoder.rs:201-283),
-// locates the literals and sequences section headers (literals_section.rs:117-223 gives the sizes that locate
-// sequence_section.rs:108-167) and hands the host planner exactly the bytes it parses: ~16 bytes per block instead of the whole
-// compressed input.  fill == 0: count the blocks; fill == 1: write the digests at first_block[frame].
+// first step).  One thread per frame runs the planner's own header parsers (framing.cuh) along the chain of blocks and hands it
+// their results, with the frame header bytes and the checksum: 40 bytes per block instead of the whole compressed input.
+// fill == 0: count the blocks; fill == 1: write the digests at first_block[frame].  The digests are assembled in global memory,
+// so that no byte array of the thread needs local memory.
 // ------------------------------------------------------------------------------------------------------------
 __global__ void k_walk(const uint8_t *__restrict__ input, uint64_t input_len, const uint64_t *__restrict__ src_off, const uint64_t *__restrict__ src_size,
                        uint32_t nframes, WalkFrame *__restrict__ wf, const uint32_t *__restrict__ first_block, WalkBlock *__restrict__ wb, int fill) {
     const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= nframes) return;
-    WalkFrame F;
-    for (int i = 0; i < 20; i++) F.hdr[i] = 0;
-    F.hdr_avail = 0; F.nblocks = 0; F.stop = 4; F.tail_avail = 0; F.pad = 0; F.end_pos = 0;
-    for (int i = 0; i < 4; i++) F.tail[i] = 0;
-    const uint64_t so = src_off[f], len = src_size[f];
-    if (so <= input_len && len <= input_len - so) {
-        const uint8_t *p = input + so;
-        F.hdr_avail = (uint32_t)(len < 20 ? len : 20);
-        for (uint32_t i = 0; i < F.hdr_avail; i++) F.hdr[i] = p[i];
-        // frame header size (frame.rs:6-85); anything wrong with it is the planner's to report
-        uint64_t pos = 0;
-        bool ok = len >= 5 && (uint32_t)(F.hdr[0] | (F.hdr[1] << 8) | (F.hdr[2] << 16) | ((uint32_t)F.hdr[3] << 24)) == 0xFD2FB528u;
-        if (ok) {
-            const uint32_t desc = F.hdr[4], single = (desc >> 5) & 1u, flag = desc >> 6;
-            const uint32_t dl = (desc & 3u) == 3u ? 4u : (desc & 3u);
-            const uint32_t fl = flag == 0 ? single : (flag == 1 ? 2u : (flag == 2 ? 4u : 8u));
-            pos = 5u + (single ? 0u : 1u) + dl + fl;
-            ok = len >= pos;
-        }
-        if (ok) {
-            uint32_t nb = 0;
-            const uint32_t base = fill ? first_block[f] : 0u;
-            for (;;) {
-                if (len - pos < 3) { F.stop = 1; break; }
-                const uint32_t b0 = p[pos], b1 = p[pos + 1], b2 = p[pos + 2];
-                const uint32_t t = (b0 >> 1) & 3u, size = (b0 >> 3) | (b1 << 5) | (b2 << 13);
-                WalkBlock B;
-                B.pos = pos; B.seq_off = 0; B.bh[0] = (uint8_t)b0; B.bh[1] = (uint8_t)b1; B.bh[2] = (uint8_t)b2; B.lit_avail = 0; B.seq_avail = 0;
-                for (int i = 0; i < 5; i++) B.lit[i] = 0;
-                for (int i = 0; i < 4; i++) B.seq[i] = 0;
-                for (int i = 0; i < 6; i++) B.pad[i] = 0;
-                if (t == 3 || size > 128u * 1024u) {   // the planner reports FoundReservedBlock / BlockSizeTooLarge from these 3 bytes
-                    if (fill) wb[base + nb] = B;
-                    nb++; F.stop = 2; break;
-                }
-                const uint32_t content = t == BT_RLE ? 1u : size;
-                pos += 3;
-                if (len - pos < content) {
-                    if (fill) wb[base + nb] = B;
-                    nb++; F.stop = 3; break;
-                }
-                if (t == BT_COMPRESSED && size) {
-                    const uint8_t *c = p + pos;
-                    B.lit_avail = (uint8_t)(size < 5 ? size : 5);
-                    for (uint32_t i = 0; i < B.lit_avail; i++) B.lit[i] = c[i];
-                    const uint32_t lt = c[0] & 3u, sf = (c[0] >> 2) & 3u;
-                    const uint32_t need = (lt == LT_RAW || lt == LT_RLE) ? ((sf == 0 || sf == 2) ? 1u : (sf == 1 ? 2u : 3u)) : (sf <= 1 ? 3u : (sf == 2 ? 4u : 5u));
-                    if (size >= need) {
-                        uint32_t regen, comp = 0;
-                        if (lt == LT_RAW || lt == LT_RLE) {
-                            if (sf == 0 || sf == 2) regen = c[0] >> 3;
-                            else if (sf == 1) regen = (c[0] >> 4) + ((uint32_t)c[1] << 4);
-                            else regen = (c[0] >> 4) + ((uint32_t)c[1] << 4) + ((uint32_t)c[2] << 12);
-                        } else if (sf <= 1) { regen = (c[0] >> 4) + (((uint32_t)c[1] & 0x3f) << 4); comp = (c[1] >> 6) + ((uint32_t)c[2] << 2); }
-                        else if (sf == 2) { regen = (c[0] >> 4) + ((uint32_t)c[1] << 4) + (((uint32_t)c[2] & 3) << 12); comp = (c[2] >> 2) + ((uint32_t)c[3] << 6); }
-                        else { regen = (c[0] >> 4) + ((uint32_t)c[1] << 4) + (((uint32_t)c[2] & 0x3f) << 12); comp = (c[2] >> 6) + ((uint32_t)c[3] << 2) + ((uint32_t)c[4] << 10); }
-                        const uint32_t upper = (lt == LT_COMPRESSED || lt == LT_TREELESS) ? comp : (lt == LT_RLE ? 1u : regen);
-                        if (size - need >= upper) {
-                            const uint32_t rem = size - need - upper;
-                            B.seq_off = need + upper;
-                            B.seq_avail = (uint8_t)(rem < 4 ? rem : 4);
-                            for (uint32_t i = 0; i < B.seq_avail; i++) B.seq[i] = c[need + upper + i];
-                        }
-                    }
-                }
+    const uint64_t so = src_off[f];
+    const uint64_t len = so <= input_len && src_size[f] <= input_len - so ? src_size[f] : 0;   // (out of range: nothing to walk)
+    const uint8_t *p = input + so;
+    WalkFrame &F = wf[f];
+    const uint32_t hdr_avail = (uint32_t)(len < 20 ? len : 20);
+    for (uint32_t i = 0; i < 20; i++) F.hdr[i] = i < hdr_avail ? p[i] : 0;
+    uint32_t nb = 0, stop = 4, tail_avail = 0;
+    uint64_t end_pos = 0;
+    FrameHeader fh;
+    uint32_t skip_len;
+    size_t pos;
+    if (parse_frame_header(p, len, fh, skip_len, pos) == 0) {   // anything wrong with the frame header is the planner's to report
+        const uint32_t base = fill ? first_block[f] : 0u;
+        for (;;) {
+            if (len - pos < 3) { stop = 1; break; }
+            WalkBlock B = {};
+            B.pos = pos; B.bh[0] = p[pos]; B.bh[1] = p[pos + 1]; B.bh[2] = p[pos + 2];
+            BlockHeader bh;
+            if (parse_block_header(p + pos, bh)) {   // the planner reports FoundReservedBlock / BlockSizeTooLarge from these 3 bytes
                 if (fill) wb[base + nb] = B;
-                nb++;
-                pos += content;
-                if (b0 & 1u) {   // last block: the content checksum may follow
-                    F.stop = 0;
-                    const uint64_t left = len - pos;
-                    F.tail_avail = (uint32_t)(left < 4 ? left : 4);
-                    for (uint32_t i = 0; i < F.tail_avail; i++) F.tail[i] = p[pos + i];
-                    break;
-                }
+                nb++; stop = 2; break;
             }
-            F.nblocks = nb; F.end_pos = pos;
+            pos += 3;
+            if (len - pos < bh.content_size) {
+                if (fill) wb[base + nb] = B;
+                nb++; stop = 3; break;
+            }
+            if (bh.type == BT_COMPRESSED) B.sec = parse_section_headers(p + pos, bh.content_size);
+            if (fill) wb[base + nb] = B;
+            nb++;
+            pos += bh.content_size;
+            if (bh.last) {   // the content checksum may follow
+                stop = 0;
+                tail_avail = (uint32_t)(len - pos < 4 ? len - pos : 4);
+                break;
+            }
         }
+        end_pos = pos;
     }
-    wf[f] = F;
+    for (uint32_t i = 0; i < 4; i++) F.tail[i] = i < tail_avail ? p[end_pos + i] : 0;
+    F.hdr_avail = hdr_avail; F.nblocks = nb; F.stop = stop; F.tail_avail = tail_avail; F.pad = 0; F.end_pos = end_pos;
 }
 
 }  // namespace b200z

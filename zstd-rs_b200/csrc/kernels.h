@@ -4,6 +4,7 @@
 #include <stdint.h>
 
 #include "b200z_types.h"
+#include "framing.cuh"
 
 namespace b200z {
 

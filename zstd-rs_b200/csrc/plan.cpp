@@ -1,4 +1,4 @@
-// plan.cpp -- host-side framing (see plan.h for the reference functions each piece mirrors).
+// plan.cpp -- host-side planning of a submission (plan.h).
 #include "plan.h"
 
 #include <string.h>
@@ -8,76 +8,7 @@
 
 namespace b200z {
 
-static inline uint32_t rd32le(const uint8_t *p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
 static inline uint64_t rd64le(const uint8_t *p) { return (uint64_t)rd32le(p) | ((uint64_t)rd32le(p + 4) << 32); }
-
-// frame.rs:6-85.  Each read_exact that would fail maps to the matching *ReadError leaf.
-int parse_frame_header(const uint8_t *p, size_t len, FrameHeader &h, uint32_t &skip_len, size_t &consumed) {
-    consumed = 0;
-    if (len < 4) { consumed = len; return B200Z_ERR_MAGIC_NUMBER_READ; }
-    uint32_t magic = rd32le(p);
-    size_t pos = 4;
-    if (magic >= 0x184D2A50u && magic <= 0x184D2A5Fu) {
-        if (len < 8) { consumed = len; return B200Z_ERR_FRAME_DESCRIPTOR_READ; }
-        skip_len = rd32le(p + 4);
-        consumed = 8;
-        return B200Z_ERR_SKIP_FRAME;
-    }
-    if (magic != 0xFD2FB528u) { consumed = 4; return B200Z_ERR_BAD_MAGIC_NUMBER; }
-    if (len < pos + 1) { consumed = len; return B200Z_ERR_FRAME_DESCRIPTOR_READ; }
-    h = FrameHeader();
-    h.descriptor = p[pos++];
-    if (!h.single_segment()) {
-        if (len < pos + 1) { consumed = len; return B200Z_ERR_WINDOW_DESCRIPTOR_READ; }
-        h.window_descriptor = p[pos++];
-    }
-    static const uint8_t did_len[4] = {0, 1, 2, 4};
-    uint32_t dl = did_len[h.descriptor & 3];
-    if (dl) {
-        if (len < pos + dl) { consumed = len; return B200Z_ERR_DICTIONARY_ID_READ; }
-        uint32_t id = 0;
-        for (uint32_t i = 0; i < dl; i++) id += (uint32_t)p[pos + i] << (8 * i);
-        pos += dl;
-        if (id != 0) { h.has_dict_id = true; h.dict_id = id; }
-    }
-    uint32_t flag = h.descriptor >> 6;
-    uint32_t fl = flag == 0 ? (h.single_segment() ? 1 : 0) : (flag == 1 ? 2 : (flag == 2 ? 4 : 8));
-    if (fl) {
-        if (len < pos + fl) { consumed = len; return B200Z_ERR_FRAME_CONTENT_SIZE_READ; }
-        uint64_t fcs = 0;
-        for (uint32_t i = 0; i < fl; i++) fcs += (uint64_t)p[pos + i] << (8 * i);
-        if (fl == 2) fcs += 256;
-        h.frame_content_size = fcs;
-        pos += fl;
-    }
-    h.header_size = (uint8_t)pos;
-    consumed = pos;
-    return 0;
-}
-
-// frame.rs:116-139
-int frame_window_size(const FrameHeader &h, uint64_t &out) {
-    if (h.single_segment()) { out = h.frame_content_size; return 0; }
-    uint64_t exp = h.window_descriptor >> 3, mant = h.window_descriptor & 7;
-    uint64_t base = 1ull << (10 + exp);
-    uint64_t w = base + (base / 8) * mant;
-    const uint64_t MAXW = (1ull << 41) + 7 * (1ull << 38);
-    if (w >= 1024) { if (w < MAXW) { out = w; return 0; } return B200Z_ERR_WINDOW_TOO_BIG; }
-    return B200Z_ERR_WINDOW_TOO_SMALL;
-}
-
-// block_decoder.rs:201-283
-int parse_block_header(const uint8_t b[3], BlockHeader &h) {
-    uint32_t t = (b[0] >> 1) & 3;
-    if (t == 3) return B200Z_ERR_FOUND_RESERVED_BLOCK;
-    uint32_t size = (uint32_t)(b[0] >> 3) | ((uint32_t)b[1] << 5) | ((uint32_t)b[2] << 13);
-    if (size > 128u * 1024u) return B200Z_ERR_BLOCK_SIZE_TOO_LARGE;
-    h.type = t;
-    h.decompressed_size = (t == BT_RAW || t == BT_RLE) ? size : 0;
-    h.content_size = t == BT_RLE ? 1 : size;
-    h.last = b[0] & 1;
-    return 0;
-}
 
 static TabRef one_mode(uint32_t mode, TabRef cur, int32_t slot_idx) {
     TabRef r;
@@ -89,37 +20,12 @@ static TabRef one_mode(uint32_t mode, TabRef cur, int32_t slot_idx) {
     }
 }
 
-void plan_compressed_block(const uint8_t *c, uint32_t size, BlockDesc &d, BlockRefs &r, TableCursor &cur,
-                           uint32_t &n_huf_slots, uint32_t &n_fse_slots, uint64_t &lit_bytes, uint64_t &nseq_total) {
-    plan_compressed_block_view(c, nullptr, size, d, r, cur, n_huf_slots, n_fse_slots, lit_bytes, nseq_total);
-}
-
-// `c`: the first bytes of the block content (the literals section header: at most 5 are read); `seq`: the first bytes of the sequences
-// section header (at most 4 are read), or null when `c` is the whole content.  The device-side header walk (k_walk) hands over
-// exactly these bytes per block.
-void plan_compressed_block_view(const uint8_t *c, const uint8_t *seq, uint32_t size, BlockDesc &d, BlockRefs &r, TableCursor &cur,
-                                uint32_t &n_huf_slots, uint32_t &n_fse_slots, uint64_t &lit_bytes, uint64_t &nseq_total) {
-    // ---- literals section header (literals_section.rs:117-223)
-    if (size == 0) { d.host_status = host_status(B200Z_ERR_LITSEC_GET_BITS, B200Z_STAGE_BLOCK_BODY, HS_BEFORE_LITERALS); return; }
-    uint32_t lt = c[0] & 3, sf = (c[0] >> 2) & 3, need;
-    if (lt == LT_RAW || lt == LT_RLE) need = (sf == 0 || sf == 2) ? 1 : (sf == 1 ? 2 : 3);
-    else need = sf <= 1 ? 3 : (sf == 2 ? 4 : 5);
-    if (size < need) { d.host_status = host_status(B200Z_ERR_LITSEC_NOT_ENOUGH_BYTES, B200Z_STAGE_BLOCK_BODY, HS_BEFORE_LITERALS); return; }
-    uint32_t regen = 0, comp = 0, nstreams = 0;
-    if (lt == LT_RAW || lt == LT_RLE) {
-        if (sf == 0 || sf == 2) regen = c[0] >> 3;
-        else if (sf == 1) regen = (c[0] >> 4) + ((uint32_t)c[1] << 4);
-        else regen = (c[0] >> 4) + ((uint32_t)c[1] << 4) + ((uint32_t)c[2] << 12);
-    } else {
-        nstreams = sf == 0 ? 1 : 4;
-        if (sf <= 1) { regen = (c[0] >> 4) + (((uint32_t)c[1] & 0x3f) << 4); comp = (c[1] >> 6) + ((uint32_t)c[2] << 2); }
-        else if (sf == 2) { regen = (c[0] >> 4) + ((uint32_t)c[1] << 4) + (((uint32_t)c[2] & 3) << 12); comp = (c[2] >> 2) + ((uint32_t)c[3] << 6); }
-        else { regen = (c[0] >> 4) + ((uint32_t)c[1] << 4) + (((uint32_t)c[2] & 0x3f) << 12); comp = (c[2] >> 6) + ((uint32_t)c[3] << 2) + ((uint32_t)c[4] << 10); }
-    }
-    d.lit_type = lt; d.nstreams = nstreams; d.regen_size = regen; d.lit_comp_size = comp; d.lit_off = need;
-    // block_decoder.rs:120-134
-    uint32_t upper = (lt == LT_COMPRESSED || lt == LT_TREELESS) ? comp : (lt == LT_RLE ? 1 : regen);
-    if (size - need < upper) { d.host_status = host_status(B200Z_ERR_MALFORMED_SECTION_HEADER, B200Z_STAGE_BLOCK_BODY, HS_BEFORE_LITERALS); return; }
+void plan_compressed_block(const SectionHeaders &sec, BlockDesc &d, BlockRefs &r, TableCursor &cur, uint32_t &n_huf_slots, uint32_t &n_fse_slots,
+                           uint64_t &lit_bytes, uint64_t &nseq_total) {
+    d.lit_type = sec.lit_type; d.nstreams = sec.nstreams; d.regen_size = sec.regen_size; d.lit_comp_size = sec.lit_comp_size; d.lit_off = sec.lit_off;
+    d.nseq = sec.nseq; d.modes = sec.modes; d.seq_off = sec.seq_off; d.host_status = sec.status;
+    if (host_status_pos(sec.status) == HS_BEFORE_LITERALS) return;
+    const uint32_t lt = sec.lit_type, nseq = sec.nseq, modes = sec.modes;
     if (lt == LT_COMPRESSED) {
         r.build_huf = (int32_t)n_huf_slots++;
         cur.huf.kind = TabRef::SLOT; cur.huf.idx = (uint32_t)r.build_huf;
@@ -127,29 +33,9 @@ void plan_compressed_block_view(const uint8_t *c, const uint8_t *seq, uint32_t s
     } else if (lt == LT_TREELESS) r.huf = cur.huf;
     if (lt == LT_COMPRESSED || lt == LT_TREELESS) {
         d.lit_buf_off = lit_bytes;
-        lit_bytes += ((uint64_t)regen + 31) & ~15ull;  // 16-byte aligned, >= 16 bytes of slack for vector stores
+        lit_bytes += ((uint64_t)sec.regen_size + 31) & ~15ull;  // 16-byte aligned, >= 16 bytes of slack for vector stores
     }
-    // ---- sequences section header (sequence_section.rs:108-167)
-    const uint8_t *s = seq ? seq : c + need + upper;
-    uint32_t rem = size - need - upper, hdr = 0, nseq = 0, modes = 0;
-    bool bad = false;
-    if (rem == 0) bad = true;
-    else if (s[0] == 0) { hdr = 1; }
-    else if (s[0] < 128) { if (rem < 2) bad = true; else { nseq = s[0]; modes = s[1]; hdr = 2; } }
-    else if (s[0] < 255) {
-        if (rem < 2) bad = true;
-        else {
-            nseq = (((uint32_t)s[0] - 128) << 8) + s[1]; hdr = 2;
-            if (nseq != 0) { if (rem < 3) bad = true; else { modes = s[2]; hdr = 3; } }
-        }
-    } else { if (rem < 4) bad = true; else { nseq = (uint32_t)s[1] + ((uint32_t)s[2] << 8) + 0x7F00; modes = s[3]; hdr = 4; } }
-    if (bad) { d.host_status = host_status(B200Z_ERR_SEQHDR_NOT_ENOUGH_BYTES, B200Z_STAGE_BLOCK_BODY, HS_AFTER_LITERALS); return; }
-    d.nseq = nseq; d.modes = modes; d.seq_off = need + upper + hdr;
-    if (nseq == 0) {
-        // block_decoder.rs:185-191: bytes after an empty sequences section
-        if (rem - hdr != 0) d.host_status = host_status(B200Z_ERR_SEQ_EXTRA_BITS, B200Z_STAGE_SEQUENCES, HS_AFTER_LITERALS);
-        return;
-    }
+    if (nseq == 0) return;   // (also when the sequences header failed)
     uint32_t ml_ = (modes >> 6) & 3, mo = (modes >> 4) & 3, mm = (modes >> 2) & 3;
     bool needs_slot = ml_ == MODE_RLE || ml_ == MODE_FSE || mo == MODE_RLE || mo == MODE_FSE || mm == MODE_RLE || mm == MODE_FSE;
     if (needs_slot) r.build_fse = (int32_t)n_fse_slots++;

@@ -15,14 +15,6 @@
 #include "../../include/b200zstd.h"
 #include "b200z_types.h"
 
-#ifdef __CUDACC__
-#define B200Z_HD __host__ __device__ __forceinline__
-#define B200Z_HDN __host__ __device__
-#else
-#define B200Z_HD inline
-#define B200Z_HDN
-#endif
-
 namespace b200z {
 
 B200Z_HD uint32_t hbs(uint32_t x) {  // "highest_bit_set": 32 - clz, x > 0  (fse_decoder.rs:326-329)
