@@ -428,6 +428,20 @@ size_t b200z_compress_bound(size_t src_size);
 int b200z_compress_frames_batch(b200z_ctx *ctx, const uint8_t *input, size_t input_len, int input_mem,
                                 const b200z_compress_io *frames, size_t nframes, int level, int checksum,
                                 uint8_t *output, size_t output_cap, int output_mem, b200z_compress_result *results);
+/* EXTENSION (ruzstd's FrameCompressor writes no dictionary ID and matches against no dictionary): compression against one
+ * dictionary per submission.  The first 128 KiB of every frame may also match the last 128 KiB of the dictionary's content
+ * (offsets stay within the 128 KiB window); the content checksum covers the frame's own plaintext.  A formatted dictionary's ID
+ * goes into every frame header in the smallest field that holds it; a raw-content dictionary writes no ID (libzstd's
+ * convention), so such frames are decoded with it forced (`forced_dict`, force_dict).  The encoder does not use a formatted
+ * dictionary's entropy tables or repeat offsets.  The dictionary's match table is built on the ctx stream by its first use here
+ * (one more kernel launch) and kept until b200z_dict_destroy.  dict == NULL writes exactly what b200z_compress_frames_batch
+ * writes.  Besides that entry's checks: B200Z_ERR_INVALID_ARGUMENT for a dictionary created on another ctx and for
+ * dst_cap < b200z_compress_bound_dict(src_size, dict), before any launch. */
+int b200z_compress_frames_batch_dict(b200z_ctx *ctx, const uint8_t *input, size_t input_len, int input_mem,
+                                     const b200z_compress_io *frames, size_t nframes, int level, int checksum, const b200z_dict *dict,
+                                     uint8_t *output, size_t output_cap, int output_mem, b200z_compress_result *results);
+/* b200z_compress_bound(src_size) + the size of the dictionary ID field the frame carries with `dict` (0, 1, 2 or 4 bytes) */
+size_t b200z_compress_bound_dict(size_t src_size, const b200z_dict *dict);
 int b200z_compress_num_stages(void);
 const char *b200z_compress_stage_name(int stage);
 /* each kernel's device milliseconds in the last b200z_compress_frames_batch run with B200Z_FLAG_PROFILE set */

@@ -151,6 +151,8 @@ def lib():
         "b200z_xxh64": (C.c_uint64, [vp, sz]),
         "b200z_compress_bound": (sz, [sz]),
         "b200z_compress_frames_batch": (C.c_int, [vp, vp, sz, C.c_int, vp, sz, C.c_int, C.c_int, vp, sz, C.c_int, vp]),
+        "b200z_compress_frames_batch_dict": (C.c_int, [vp, vp, sz, C.c_int, vp, sz, C.c_int, C.c_int, vp, vp, sz, C.c_int, vp]),
+        "b200z_compress_bound_dict": (sz, [sz, vp]),
         "b200z_compress_num_stages": (C.c_int, []),
         "b200z_compress_stage_name": (C.c_char_p, [C.c_int]),
         "b200z_compress_last_profile": (C.c_int, [vp, C.POINTER(C.c_float), sz]),
@@ -357,31 +359,34 @@ def decode_frames(ctx, input, frames, output, dicts=None, forced_dict=None, max_
     return res
 
 
-def compress_bound(n):
-    """b200z_compress_bound: the largest frame compress_frames can write for n input bytes."""
-    return lib().b200z_compress_bound(n)
+def compress_bound(n, dict=None):
+    """b200z_compress_bound (b200z_compress_bound_dict with a Dictionary): the largest frame compress_frames can write for n input
+    bytes."""
+    return lib().b200z_compress_bound(n) if dict is None else lib().b200z_compress_bound_dict(n, dict.h)
 
 
-def compress_frames(ctx, input, io, output, level=FASTEST, checksum=True):
-    """b200z_compress_frames_batch: one zstd frame per COMPRESS_IO_DTYPE row (src_off, src_size, dst_off, dst_cap), every block of
-    every frame compressed at once.  input/output: bytes, numpy or torch (host or cuda).  Returns COMPRESS_RESULT_DTYPE rows."""
+def compress_frames(ctx, input, io, output, level=FASTEST, checksum=True, dict=None):
+    """b200z_compress_frames_batch_dict: one zstd frame per COMPRESS_IO_DTYPE row (src_off, src_size, dst_off, dst_cap), every block
+    of every frame compressed at once, against `dict` (a Dictionary of this context) when given.  input/output: bytes, numpy or
+    torch (host or cuda).  Returns COMPRESS_RESULT_DTYPE rows."""
     fr = np.ascontiguousarray(io, dtype=COMPRESS_IO_DTYPE)
     res = np.zeros(len(fr), dtype=COMPRESS_RESULT_DTYPE)
     ip, il, _k1 = _ptr(input)
     op, ol, _k2 = _ptr(output)
-    e = ctx.L.b200z_compress_frames_batch(ctx.h, ip, il, MEM_DEVICE if _is_device(input) else MEM_HOST, fr.ctypes.data, len(fr), level,
-                                          1 if checksum else 0, op, ol, MEM_DEVICE if _is_device(output) else MEM_HOST, res.ctypes.data)
+    e = ctx.L.b200z_compress_frames_batch_dict(ctx.h, ip, il, MEM_DEVICE if _is_device(input) else MEM_HOST, fr.ctypes.data, len(fr), level,
+                                               1 if checksum else 0, dict.h if dict is not None else None, op, ol,
+                                               MEM_DEVICE if _is_device(output) else MEM_HOST, res.ctypes.data)
     ctx._chk(e)
     return res
 
 
-def compress_to_vec(ctx, data, level=FASTEST, checksum=True):
-    """Mirror of ruzstd::encoding::compress_to_vec (encoding/mod.rs): one frame holding `data`, as bytes."""
+def compress_to_vec(ctx, data, level=FASTEST, checksum=True, dict=None):
+    """Mirror of ruzstd::encoding::compress_to_vec (encoding/mod.rs): one frame holding `data`, as bytes (against `dict` when given)."""
     src = bytes(data)
-    cap = compress_bound(len(src))
+    cap = compress_bound(len(src), dict)
     out = np.zeros(cap, dtype=np.uint8)
     io = np.array([(0, len(src), 0, cap)], dtype=COMPRESS_IO_DTYPE)
-    res = compress_frames(ctx, src, io, out, level, checksum)
+    res = compress_frames(ctx, src, io, out, level, checksum, dict)
     return out[:int(res[0]["dst_size"])].tobytes()
 
 

@@ -159,6 +159,7 @@ struct b200z_dict {
     FseSlot *d_fse = nullptr;
     uint8_t *d_content = nullptr;
     size_t content_len = 0;
+    uint32_t *d_ctab = nullptr;   // the compressor's match table of the content (k_cdict), built by its first compression
 };
 
 static void dict_free(b200z_dict *d) {
@@ -167,6 +168,7 @@ static void dict_free(b200z_dict *d) {
     if (d->d_huf) cudaFree(d->d_huf);
     if (d->d_fse) cudaFree(d->d_fse);
     if (d->d_content) cudaFree(d->d_content);
+    if (d->d_ctab) cudaFree(d->d_ctab);
     delete d;
 }
 
@@ -1619,6 +1621,10 @@ extern "C" size_t b200z_compress_bound(size_t n) {
     const size_t blocks = std::max<size_t>(1, (n + ENC_BLOCK - 1) / ENC_BLOCK);
     return n + 14 + 3 * blocks + 4;
 }
+// the ID a frame compressed against `d` carries: a formatted dictionary's own, none for raw content (libzstd's convention: it
+// rejects a frame whose ID does not match a raw-content dictionary; the decoder selects one with forced_dict)
+static uint32_t compress_dict_id(const b200z_dict *d) { return d && d->has_tables ? d->id : 0; }
+extern "C" size_t b200z_compress_bound_dict(size_t n, const b200z_dict *d) { return b200z_compress_bound(n) + dict_id_field_size(compress_dict_id(d)); }
 extern "C" int b200z_compress_num_stages(void) { return kCompressStages; }
 extern "C" const char *b200z_compress_stage_name(int stage) { return stage >= 0 && stage < kCompressStages ? kCompressStageNames[stage] : ""; }
 
@@ -1643,9 +1649,17 @@ extern "C" int b200z_compress_last_profile(const b200z_ctx *c, float *stage_ms, 
 extern "C" int b200z_compress_frames_batch(b200z_ctx *c, const uint8_t *input, size_t input_len, int input_mem, const b200z_compress_io *frames,
                                            size_t nframes, int level, int checksum, uint8_t *output, size_t output_cap, int output_mem,
                                            b200z_compress_result *results) {
+    return b200z_compress_frames_batch_dict(c, input, input_len, input_mem, frames, nframes, level, checksum, nullptr, output, output_cap,
+                                            output_mem, results);
+}
+
+extern "C" int b200z_compress_frames_batch_dict(b200z_ctx *c, const uint8_t *input, size_t input_len, int input_mem, const b200z_compress_io *frames,
+                                                size_t nframes, int level, int checksum, const b200z_dict *dict, uint8_t *output,
+                                                size_t output_cap, int output_mem, b200z_compress_result *results) {
     // ---- everything is checked before any device work
     if (level >= 2 && level <= 4) return B200Z_ERR_REFERENCE_WOULD_PANIC;   // Default / Better / Best: unimplemented!() in the reference
     if (!c || (level != B200Z_LEVEL_UNCOMPRESSED && level != B200Z_LEVEL_FASTEST)) return B200Z_ERR_INVALID_ARGUMENT;
+    if (dict && dict->ctx != c) { c->err = "dictionary created on another context"; return B200Z_ERR_INVALID_ARGUMENT; }
     if ((nframes && (!frames || !results)) || (input_mem != B200Z_MEM_HOST && input_mem != B200Z_MEM_DEVICE) ||
         (output_mem != B200Z_MEM_HOST && output_mem != B200Z_MEM_DEVICE) || (input_len && !input) || (output_cap && !output) || nframes > 0xffffffffu) {
         c->err = "invalid argument";
@@ -1656,8 +1670,8 @@ extern "C" int b200z_compress_frames_batch(b200z_ctx *c, const uint8_t *input, s
     for (size_t i = 0; i < nframes; i++) {
         const b200z_compress_io &f = frames[i];
         if (f.src_off > input_len || f.src_size > input_len - f.src_off || f.dst_off > output_cap || f.dst_cap > output_cap - f.dst_off ||
-            f.dst_cap < b200z_compress_bound(f.src_size)) {
-            c->err = "frame " + std::to_string(i) + ": range outside input/output or dst_cap < b200z_compress_bound(src_size)";
+            f.dst_cap < b200z_compress_bound_dict(f.src_size, dict)) {
+            c->err = "frame " + std::to_string(i) + ": range outside input/output or dst_cap < b200z_compress_bound_dict(src_size, dict)";
             return B200Z_ERR_INVALID_ARGUMENT;
         }
         dst.push_back({f.dst_off, f.dst_cap});
@@ -1713,12 +1727,28 @@ extern "C" int b200z_compress_frames_batch(b200z_ctx *c, const uint8_t *input, s
     }
     CU(c, cudaMemcpyAsync(r.frames.p, hf.data(), nframes * sizeof(CFrame), cudaMemcpyHostToDevice, s));
     CU(c, cudaMemcpyAsync(r.blocks.p, hb.data(), nblocks * sizeof(CBlock), cudaMemcpyHostToDevice, s));
+    // the dictionary's match table, built once and kept with the dictionary (not one of the timed stages).  Offsets stay within
+    // the 128 KiB window, so the kernels see the content's last ENC_WINDOW bytes only.
+    const bool match_dict = fast && dict && dict->content_len >= ENC_MIN_MATCH;
+    const uint32_t dict_tail = dict ? (uint32_t)std::min<size_t>(dict->content_len, ENC_WINDOW) : 0;
+    const uint8_t *dict_at = dict ? dict->d_content + (dict->content_len - dict_tail) : nullptr;
+    b200z_dict *md = const_cast<b200z_dict *>(dict);
+    if (match_dict && !md->d_ctab) {
+        CU(c, cudaMalloc((void **)&md->d_ctab, sizeof(uint32_t) << CD_LOG));
+        if (int le = launch_dict_table(dict_at, dict_tail, md->d_ctab, s, &c->launches)) {
+            cudaFree(md->d_ctab);
+            md->d_ctab = nullptr;
+            return c->set_cuda_err((cudaError_t)le, "k_cdict");
+        }
+    }
     CompressArgs a{};
     a.frames = r.frames.as<CFrame>(); a.blocks = r.blocks.as<CBlock>(); a.input = d_in; a.output = d_out;
     a.lit_stage = r.lit_stage.as<uint8_t>(); a.seq_stage = r.seq_stage.as<SeqRec>(); a.lits = r.lits.as<uint8_t>(); a.seqs = r.seqs.as<SeqRec>();
     a.enc = a.lit_stage; a.info = r.info.as<CBlockInfo>(); a.res = r.res.as<CBlockInfo>(); a.csum = r.csum.as<uint64_t>();
     a.results = r.results.as<b200z_compress_result>(); a.nframes = (uint32_t)nframes; a.nblocks = (uint32_t)nblocks; a.level = level;
     a.checksum = checksum ? 1 : 0;
+    a.dict_id = compress_dict_id(dict);
+    if (match_dict) { a.dict = dict_at; a.dtab = dict->d_ctab; a.dict_len = dict_tail; }
     const bool prof = (c->flags & B200Z_FLAG_PROFILE) != 0;
     if (prof) CU(c, cudaEventRecord(r.ev[0], s));
     for (int st = 0; st < kCompressStages; st++) {

@@ -4,10 +4,12 @@
 //   k_cenc      : one warp per block: Huffman literals, FSE sequences, the Raw / RLE / Compressed decision (encode.cuh)
 //   k_cxxh64    : content checksum of every frame's input (xxh64.cuh; four serial chains per frame)
 //   k_cassemble : one CTA per block: frame header, the block at its prefix-summed offset, the checksum, per-frame results
+//   k_cdict     : not a stage: the match table of a dictionary, built once the first time the dictionary is used (EXTENSION)
 //
 // Every block is encoded from its own literals and sequences only (no Repeat / Treeless modes, no repeat offsets), so all
 // blocks of all frames -- including the blocks of one huge frame -- run at the same time.  Matches may still reach back into
-// the previous block: the input is all there from the start.
+// the previous block: the input is all there from the start.  With a dictionary (an extension: ruzstd's encoder has none), the
+// first ENC_WINDOW bytes of every frame may also match the dictionary's content, which lies before the frame's first byte.
 #include <cuda_runtime.h>
 #include <limits.h>
 #include <stdint.h>
@@ -43,12 +45,17 @@ __device__ __forceinline__ uint32_t match_len(const uint8_t *a, const uint8_t *b
 // its position up in the first-occurrence table and in the warp's private most-recent table (seeded with the CM_SEED bytes
 // before the segment, which may lie in the previous block), keeps the longer verified candidate (candidate < position, offset
 // <= 128 KiB, inside the frame), and the first lane with a match of >= 5 bytes wins.  A match never crosses its segment's end.
+// With DICT, a lane whose position is fewer than ENC_WINDOW bytes into the frame also looks up the dictionary's table (k_cdict)
+// when that source is within the window, and verifies it against the dictionary's content; the longest candidate wins, the
+// smaller offset on a tie.  A dictionary match stops at the dictionary's end.  Without DICT the code is the plain parse.
 // Sequences and literals go to per-segment staging; the CTA then packs them, the trailing literals of a segment joining the
 // first sequence after them.
 // ------------------------------------------------------------------------------------------------------------
+template <bool DICT>
 __global__ void __launch_bounds__(CM_THREADS, 1)
 k_cmatch(const CBlock *__restrict__ blocks, const uint8_t *__restrict__ input, uint8_t *__restrict__ lit_stage, SeqRec *__restrict__ seq_stage,
-         uint8_t *__restrict__ lits, SeqRec *__restrict__ seqs, CBlockInfo *__restrict__ info) {
+         uint8_t *__restrict__ lits, SeqRec *__restrict__ seqs, CBlockInfo *__restrict__ info, const uint8_t *__restrict__ dict,
+         const uint32_t *__restrict__ dtab, uint32_t dict_len) {
     extern __shared__ __align__(16) uint8_t smem_cm[];
     uint32_t *t1 = reinterpret_cast<uint32_t *>(smem_cm);
     int32_t *tp_all = reinterpret_cast<int32_t *>(smem_cm + (4u << CM_T1_LOG));
@@ -81,7 +88,7 @@ k_cmatch(const CBlock *__restrict__ blocks, const uint8_t *__restrict__ input, u
     while (p + ENC_MIN_MATCH <= e) {
         const uint32_t q = p + lane;
         const bool valid = q + ENC_MIN_MATCH <= e;
-        uint32_t len = 0, cand = 0, h2 = 0;
+        uint32_t len = 0, cand = 0, h2 = 0, xlim = e - q;   // xlim: how far the match may be extended
         if (valid) {
             const uint32_t lim = min(CM_CAP, e - q);
             const uint32_t c1 = t1[hash5(src + q, CM_T1_LOG)];
@@ -92,6 +99,16 @@ k_cmatch(const CBlock *__restrict__ blocks, const uint8_t *__restrict__ input, u
                 const uint32_t l2 = match_len(src + q, src + c2, lim);
                 if (l2 > len || (l2 == len && (uint32_t)((int32_t)q - c2) < cand)) { len = l2; cand = (uint32_t)((int32_t)q - c2); }
             }
+            const uint32_t fpos = blk.back + q;   // back < ENC_WINDOW means it is the block's position in the frame
+            if (DICT && fpos < ENC_WINDOW) {
+                const uint32_t c3 = __ldg(dtab + hash5(src + q, CD_LOG));
+                const uint32_t off3 = fpos + dict_len - (c3 - 1);
+                if (c3 && off3 <= ENC_WINDOW) {
+                    const uint32_t rest = dict_len - (c3 - 1);   // dictionary bytes from the source to the dictionary's end
+                    const uint32_t l3 = match_len(src + q, dict + (c3 - 1), min(lim, rest));
+                    if (l3 > len || (l3 == len && off3 < cand)) { len = l3; cand = off3; xlim = min(xlim, rest); }
+                }
+            }
         }
         __syncwarp();
         if (valid) atomicMax(&tp[h2], (int32_t)q);
@@ -101,10 +118,12 @@ k_cmatch(const CBlock *__restrict__ blocks, const uint8_t *__restrict__ input, u
         const uint32_t qj = p + j, off = __shfl_sync(0xffffffffu, cand, j);
         uint32_t ml = __shfl_sync(0xffffffffu, len, j);
         if (ml == CM_CAP) {   // extend the chosen match 32 bytes at a time
-            const uint32_t lim = e - qj;
+            const uint32_t lim = DICT ? __shfl_sync(0xffffffffu, xlim, j) : e - qj;
+            const uint32_t fpos = blk.back + qj;   // an offset beyond the frame's start points into the dictionary
+            const uint8_t *ref = DICT && off > fpos ? dict + dict_len - (off - fpos) : src + qj - off;
             while (ml < lim) {
                 const uint32_t i = ml + lane;
-                const bool stop = i >= lim || __ldg(src + qj + i) != __ldg(src + qj + i - off);
+                const bool stop = i >= lim || __ldg(src + qj + i) != __ldg(ref + i);
                 const uint32_t sm = __ballot_sync(0xffffffffu, stop);
                 if (sm) { ml += __ffs(sm) - 1; break; }
                 ml += 32;
@@ -179,7 +198,7 @@ __global__ void k_cxxh64(const CFrame *__restrict__ frames, const uint8_t *__res
 __global__ void __launch_bounds__(256)
 k_cassemble(const CFrame *__restrict__ frames, const CBlock *__restrict__ blocks, const CBlockInfo *__restrict__ res, const uint8_t *__restrict__ enc,
             const uint8_t *__restrict__ input, const uint64_t *__restrict__ csum, uint8_t *__restrict__ output, b200z_compress_result *__restrict__ results,
-            int level, int checksum) {
+            int level, int checksum, uint32_t dict_id) {
     __shared__ uint64_t s_red[3][8];
     const uint32_t b = blockIdx.x, tid = threadIdx.x;
     const CBlock blk = blocks[b];
@@ -202,7 +221,7 @@ k_cassemble(const CFrame *__restrict__ frames, const CBlock *__restrict__ blocks
     __syncthreads();
     before = nraw = nrle = 0;
     for (int i = 0; i < 8; i++) { before += s_red[0][i]; nraw += s_red[1][i]; nrle += s_red[2][i]; }
-    const uint32_t hdr = frame_header_size(fr.src_size);
+    const uint32_t hdr = frame_header_size(fr.src_size, dict_id);
     uint8_t *dst = output + fr.dst_off + hdr + before;
     const uint32_t type = level == 0 ? 0u : res[b].type;
     const uint32_t csize = type == 0 ? blk.size : type == 1 ? 1u : res[b].csize;
@@ -210,7 +229,7 @@ k_cassemble(const CFrame *__restrict__ frames, const CBlock *__restrict__ blocks
     if (tid == 0) {
         const uint32_t bh = (last ? 1u : 0u) | (type << 1) | ((type == 1 ? blk.size : csize) << 3);
         dst[0] = (uint8_t)bh; dst[1] = (uint8_t)(bh >> 8); dst[2] = (uint8_t)(bh >> 16);
-        if (b == fr.first_block) write_frame_header(output + fr.dst_off, fr.src_size, checksum != 0);
+        if (b == fr.first_block) write_frame_header(output + fr.dst_off, fr.src_size, checksum != 0, dict_id);
     }
     for (uint32_t i = tid; i < csize; i += 256) dst[3 + i] = from[i];
     if (last && tid == 0) {
@@ -224,20 +243,46 @@ k_cassemble(const CFrame *__restrict__ frames, const CBlock *__restrict__ blocks
     }
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// k_cdict: the dictionary's match table.  The host hands it the dictionary's last ENC_WINDOW bytes (nothing further back can be
+// referenced); every position with 5 bytes before their end goes under its 5-byte hash, the most recent position winning
+// (atomicMax, so the table does not depend on the schedule).  Entries hold position + 1 over a zeroed table.
+// ------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_cdict(const uint8_t *__restrict__ dict, uint32_t end, uint32_t *__restrict__ dtab) {
+    const uint32_t d = blockIdx.x * 256 + threadIdx.x;
+    if (d < end) atomicMax(&dtab[hash5(dict + d, CD_LOG)], d + 1);
+}
+
 static uint32_t cdiv_u(uint64_t a, uint32_t b) { return (uint32_t)((a + b - 1) / b); }
 
 int init_compress_kernels() {
-    return (int)cudaFuncSetAttribute(k_cmatch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CM_SMEM);
+    cudaError_t e = cudaFuncSetAttribute(k_cmatch<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CM_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cmatch<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CM_SMEM);
+    return (int)e;
+}
+
+int launch_dict_table(const uint8_t *dict, uint32_t len, uint32_t *dtab, cudaStream_t s, uint64_t *launched) {
+    int e = (int)cudaMemsetAsync(dtab, 0, sizeof(uint32_t) << CD_LOG, s);
+    if (e || len < ENC_MIN_MATCH) return e;
+    const uint32_t end = len - ENC_MIN_MATCH + 1;
+    k_cdict<<<cdiv_u(end, 256), 256, 0, s>>>(dict, end, dtab);
+    e = (int)cudaGetLastError();
+    if (!e) ++*launched;
+    return e;
 }
 
 const char *const kCompressStageNames[kCompressStages] = {"k_cmatch", "k_cenc", "k_cxxh64", "k_cassemble"};
 
 int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s, uint64_t *launched) {
     switch (stage) {
-    case 0: if (!a.level || !a.nblocks) return 0; k_cmatch<<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info); break;
+    case 0:
+        if (!a.level || !a.nblocks) return 0;
+        if (a.dtab) k_cmatch<true><<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, a.dict, a.dtab, a.dict_len);
+        else k_cmatch<false><<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, nullptr, nullptr, 0);
+        break;
     case 1: if (!a.level || !a.nblocks) return 0; k_cenc<<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res); break;
     case 2: if (!a.checksum || !a.nframes) return 0; k_cxxh64<<<cdiv_u((uint64_t)a.nframes * 4, 128), 128, 0, s>>>(a.frames, a.input, a.csum, a.nframes); break;
-    case 3: if (!a.nblocks) return 0; k_cassemble<<<a.nblocks, 256, 0, s>>>(a.frames, a.blocks, a.res, a.enc, a.input, a.csum, a.output, a.results, a.level, a.checksum); break;
+    case 3: if (!a.nblocks) return 0; k_cassemble<<<a.nblocks, 256, 0, s>>>(a.frames, a.blocks, a.res, a.enc, a.input, a.csum, a.output, a.results, a.level, a.checksum, a.dict_id); break;
     default: return (int)cudaErrorInvalidValue;
     }
     const int e = (int)cudaGetLastError();

@@ -42,9 +42,20 @@ struct CompressArgs {
     b200z_compress_result *results;
     uint32_t nframes, nblocks;
     int level, checksum;
+    // the submission's dictionary (EXTENSION: ruzstd's FrameCompressor writes no dictionary ID and uses none).  dict_id goes into
+    // every frame header (0: no field); dict / dtab are null when there is nothing to match against
+    const uint8_t *dict;    // the last dict_len <= ENC_WINDOW bytes of its content (device): all a match can reach
+    const uint32_t *dtab;   // [1 << CD_LOG] from k_cdict
+    uint32_t dict_len, dict_id;
 };
 
+// the dictionary match table: 5-byte hash of a position in the dictionary's last ENC_WINDOW bytes -> that position + 1 (0 = none)
+constexpr uint32_t CD_LOG = 17;
+
 int init_compress_kernels();
+// fills dtab[1 << CD_LOG] for the device content dict[len], len <= ENC_WINDOW (a memset and k_cdict, on stream s); adds the kernels
+// it enqueued to *launched
+int launch_dict_table(const uint8_t *dict, uint32_t len, uint32_t *dtab, cudaStream_t s, uint64_t *launched);
 constexpr int kCompressStages = 4;
 extern const char *const kCompressStageNames[kCompressStages];
 int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s, uint64_t *launched);   // adds the kernels it enqueued to *launched

@@ -444,17 +444,22 @@ B200Z_HDN inline uint32_t encode_block(EncScratch &s, const uint8_t *lits, uint3
     return s.total;
 }
 
-// frame header for a frame of `n` bytes: Single_Segment = 0, 128 KiB window, Frame_Content_Size in the smallest legal field
-B200Z_HD uint32_t frame_header_size(uint64_t n) { return 6 + ((n >= 256 && n <= 65791) ? 2 : (n >> 32) ? 8 : 4); }
-B200Z_HD uint32_t write_frame_header(uint8_t *dst, uint64_t n, bool checksum) {
-    const uint32_t fcs = frame_header_size(n) - 6;
+// frame header for a frame of `n` bytes: Single_Segment = 0, 128 KiB window, the dictionary ID in the smallest field that holds
+// it (none for ID 0, as ruzstd's minify_val sizes it, encoding/frame_header.rs), Frame_Content_Size in the smallest legal field
+B200Z_HD uint32_t dict_id_field_size(uint32_t dict_id) { return dict_id == 0 ? 0 : dict_id <= 0xffu ? 1 : dict_id <= 0xffffu ? 2 : 4; }
+B200Z_HD uint32_t frame_header_size(uint64_t n, uint32_t dict_id) {
+    return 6 + dict_id_field_size(dict_id) + ((n >= 256 && n <= 65791) ? 2 : (n >> 32) ? 8 : 4);
+}
+B200Z_HD uint32_t write_frame_header(uint8_t *dst, uint64_t n, bool checksum, uint32_t dict_id) {
+    const uint32_t did = dict_id_field_size(dict_id), fcs = frame_header_size(n, dict_id) - 6 - did;
     const uint32_t flag = fcs == 2 ? 1 : fcs == 4 ? 2 : 3;
     put_le(dst, 4, 0, 0xFD2FB528u, 4);
-    dst[4] = (uint8_t)((flag << 6) | (checksum ? 4u : 0u));
+    dst[4] = (uint8_t)((flag << 6) | (checksum ? 4u : 0u) | (did == 4 ? 3u : did));
     dst[5] = (uint8_t)((17 - 10) << 3);
+    for (uint32_t i = 0; i < did; i++) dst[6 + i] = (uint8_t)(dict_id >> (8 * i));
     const uint64_t v = fcs == 2 ? n - 256 : n;
-    for (uint32_t i = 0; i < fcs; i++) dst[6 + i] = (uint8_t)(v >> (8 * i));
-    return 6 + fcs;
+    for (uint32_t i = 0; i < fcs; i++) dst[6 + did + i] = (uint8_t)(v >> (8 * i));
+    return 6 + did + fcs;
 }
 
 }  // namespace b200z
