@@ -280,6 +280,55 @@ int b200z_debug_fse_order(const uint32_t *first_block, const uint32_t *nblocks, 
 void b200z_batch_destroy(b200z_batch *b);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Tier 1c -- decode_all on the batch path: one buffer of frames back to back (zstd and skippable frames, as in multi-frame .zst
+ * files), decoded in one GPU submission.  Does what FrameDecoder::decode_all / decode_all_to_vec (frame_decoder.rs:541-610) does,
+ * without the caller knowing where a frame starts or where its plaintext goes:
+ *   prepare: finds the frames -- from offset 0, each frame's header walk says where the next one starts; on device input every
+ *            byte offset is tested for a magic number on the GPU first (k_find_frames) and only the candidates' header digests
+ *            come back -- and plans them as one submission.  b200z_batch_info[0] = the zstd frames found.
+ *   run:     b200z_batch_run on such a batch decodes every frame and places the plaintexts back to back in `d_output` by the size
+ *            each frame decodes to (never by Frame_Content_Size, which the reference does not check either), clamped to output_cap.
+ *            b200z_batch_run_profile / _timeline return B200Z_ERR_INVALID_ARGUMENT for it.
+ *   finish:  the outcome, with the first error in stream order as decode_all raises it (frame header, FailedToSkipFrame, block,
+ *            literals, sequences, execution, checksum read or TargetTooSmall).
+ * The chain of frames ends at the end of the input, at a break in it (no magic number: BadMagicNumber, or MagicNumberRead with
+ * fewer than 4 bytes left), at a skippable frame that runs past the input (FailedToSkipFrame) or at a frame whose walk stopped
+ * (frame header error, truncated block, missing checksum), which is reported as the planner reports it.
+ * Differences from the reference: frames after the failing one may have been decoded too (they are not counted); on an error,
+ * `written` still says how many bytes the frames before the failing one wrote, and output past them is unspecified.  When a
+ * frame does not fit, the reference's UptoBytes(1 MiB) loop is replayed from the frame's block sizes to tell TargetTooSmall from
+ * a later error of the same frame; an execution error in a block that no longer fits is not seen (that block is not executed).
+ * ---------------------------------------------------------------------------------------------------------- */
+typedef struct b200z_all_result {
+    uint64_t written;          /* plaintext bytes of the frames before the failing one (all of them without an error)        */
+    uint64_t frames;           /* zstd frames decoded before the failing one                                                  */
+    uint64_t skippable_frames; /* skippable frames passed before the failing one                                              */
+    uint64_t error_offset;     /* input offset of the failing frame (input_len without an error)                              */
+    int32_t status;            /* 0 or the b200z_error decode_all returns                                                    */
+    int32_t stage;             /* b200z_stage of the error (0 for TargetTooSmall, as the reference reports them)               */
+    int32_t error_frame;       /* index of the failing zstd frame in `results`, -1 when the failure is not a zstd frame's     */
+    uint32_t reserved;
+} b200z_all_result;
+
+/* `dicts` and `max_window_size` as for b200z_decode_frames_batch.  `forced_dict` is an EXTENSION: decode_all calls init per frame
+ * and never forces a dictionary; a non-NULL forced_dict is applied to every zstd frame (raw-content dictionary frames, which
+ * carry no dictionary id).  NULL gives the reference's behaviour. */
+int b200z_decode_all_prepare(b200z_ctx *ctx, const uint8_t *input, size_t input_len, int input_mem, const b200z_dict *const *dicts,
+                             size_t ndicts, const b200z_dict *forced_dict, uint64_t max_window_size, b200z_batch **out);
+/* synchronises; `results` is NULL or has room for b200z_batch_info[0] entries, one per zstd frame of the chain in stream order */
+int b200z_decode_all_finish(b200z_batch *b, b200z_all_result *summary, b200z_frame_result *results);
+/* one-shot form: prepare, run, finish; with host output the `written` bytes are copied back */
+int b200z_decode_all_batch(b200z_ctx *ctx, const uint8_t *input, size_t input_len, int input_mem, const b200z_dict *const *dicts,
+                           size_t ndicts, const b200z_dict *forced_dict, uint64_t max_window_size, uint8_t *output, size_t output_cap,
+                           int output_mem, b200z_all_result *summary);
+/* Host-only view of how prepare finds the frames (no context, no device; for CPU tests): the input offsets of the frames of the
+ * chain, the one where it ends included.  by_candidates = 0: the host-input walk, frame to frame.  by_candidates = 1: the
+ * device-input selection -- every byte offset tested for a magic number, every candidate walked with the bytes left from it, the
+ * chain followed through the sorted candidates -- with the scan and the walks done on the host.  `at` has room for `cap` offsets;
+ * *n = the chain's length. */
+int b200z_debug_decode_all_chain(const uint8_t *input, size_t input_len, int by_candidates, uint64_t *at, size_t cap, size_t *n);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Tier 1b -- block-level batch entry: the thin FFI for a host that keeps the reference's OWN frame / block /
  * section header parsing (frame.rs:6-85, block_decoder.rs:201-247, literals_section.rs:117-223,
  * sequence_section.rs:108-167) and ships compressed blocks.  It replaces the one call site of the hot path,

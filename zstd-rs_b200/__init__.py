@@ -9,7 +9,8 @@ There is no CPU decode path: every decode call needs a CUDA device and fails lou
 Import name: ``zstd_rs_b200`` (the directory name has a hyphen; see ``_pkg.py`` at the repo root).
 """
 from .binding import (  # noqa: F401
-    ALL, FASTEST, UNCOMPRESSED, UPTO_BLOCKS, UPTO_BYTES, B200ZError, Batch, Context, Dictionary, FrameDecoder, StreamingDecoder,
-    build, compress_bound, compress_frames, compress_profile, compress_to_vec, decode_blocks, decode_frames, error_names, lib, lib_path, xxh64,
+    ALL, FASTEST, UNCOMPRESSED, UPTO_BLOCKS, UPTO_BYTES, AllBatch, B200ZError, Batch, Context, Dictionary, FrameDecoder, StreamingDecoder,
+    build, compress_bound, compress_frames, compress_profile, compress_to_vec, decode_all, decode_all_batch, decode_blocks, decode_frames,
+    error_names, lib, lib_path, xxh64,
 )
 from . import binding  # noqa: F401

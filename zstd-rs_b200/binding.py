@@ -52,6 +52,8 @@ FRAME_RESULT_DTYPE = np.dtype([("out_size", "<u8"), ("bytes_read", "<u8"), ("con
                                ("status", "<i4"), ("stage", "<i4"), ("blocks_decoded", "<u4"), ("error_block", "<u4"),
                                ("has_checksum", "<u4"), ("checksum_from_data", "<u4"), ("has_dict_id", "<u4"), ("dict_id", "<u4"),
                                ("has_calculated_checksum", "<u4"), ("calculated_checksum", "<u4")])
+ALL_RESULT_DTYPE = np.dtype([("written", "<u8"), ("frames", "<u8"), ("skippable_frames", "<u8"), ("error_offset", "<u8"), ("status", "<i4"),
+                             ("stage", "<i4"), ("error_frame", "<i4"), ("reserved", "<u4")])
 COMPRESS_IO_DTYPE = np.dtype([("src_off", "<u8"), ("src_size", "<u8"), ("dst_off", "<u8"), ("dst_cap", "<u8")])
 COMPRESS_RESULT_DTYPE = np.dtype([("dst_size", "<u8"), ("status", "<i4"), ("blocks", "<u4"), ("raw_blocks", "<u4"), ("rle_blocks", "<u4"),
                                   ("has_checksum", "<u4"), ("checksum", "<u4")])
@@ -117,6 +119,10 @@ def lib():
         "b200z_debug_route_frames": (C.c_int, [vp, vp, sz, C.c_uint32, vp, C.POINTER(sz)]),
         "b200z_debug_fse_order": (C.c_int, [vp, vp, vp, sz, vp, sz, vp, C.POINTER(sz)]),
         "b200z_batch_destroy": (None, [vp]),
+        "b200z_decode_all_prepare": (C.c_int, [vp, vp, sz, C.c_int, pp, sz, vp, C.c_uint64, pp]),
+        "b200z_decode_all_finish": (C.c_int, [vp, vp, vp]),
+        "b200z_decode_all_batch": (C.c_int, [vp, vp, sz, C.c_int, pp, sz, vp, C.c_uint64, vp, sz, C.c_int, vp]),
+        "b200z_debug_decode_all_chain": (C.c_int, [vp, sz, C.c_int, vp, sz, C.POINTER(sz)]),
         "b200z_frame_decoder_new": (C.c_int, [vp, pp]),
         "b200z_frame_decoder_free": (None, [vp]),
         "b200z_frame_decoder_set_max_window_size": (None, [vp, C.c_uint64]),
@@ -357,6 +363,103 @@ def decode_frames(ctx, input, frames, output, dicts=None, forced_dict=None, max_
                                         res.ctypes.data)
     ctx._chk(e)
     return res
+
+
+def _summary(a):
+    return {k: int(a[0][k]) for k in ALL_RESULT_DTYPE.names if k != "reserved"}
+
+
+def decode_all(ctx, input, output, dicts=None, forced_dict=None, max_window_size=0):
+    """b200z_decode_all_prepare / b200z_batch_run / b200z_decode_all_finish: FrameDecoder::decode_all (frame_decoder.rs:541-577) of a
+    buffer of concatenated zstd and skippable frames in one GPU submission, the plaintexts back to back at the start of `output`.
+    input/output: bytes, numpy or torch (host or cuda).  `forced_dict` (a Dictionary) is an extension: it is applied to every frame.
+    Returns (summary dict: written, frames, skippable_frames, error_offset, status, stage, error_frame; FRAME_RESULT_DTYPE rows, one
+    per zstd frame of the chain).  Errors are reported in the summary, not raised."""
+    b = AllBatch(ctx, input, dicts, forced_dict, max_window_size)
+    try:
+        if _is_device(output):
+            b.run(output)
+        else:
+            import torch
+            op, ol, _k = _ptr(output)
+            dev = torch.empty(ol + 16, dtype=torch.uint8, device=f"cuda:{ctx.device}")
+            b.run(dev[:ol])
+            summary, res = b.finish()
+            if summary["written"]:
+                host = dev[:summary["written"]].cpu().numpy()   # kept alive until the copy is done
+                C.memmove(op, host.ctypes.data, summary["written"])
+            return summary, res
+        return b.finish()
+    finally:
+        b.close()
+
+
+class AllBatch:
+    """Prepared decode_all submission (b200z_decode_all_prepare): the frames of `input` found and planned; run() decodes them into a
+    device buffer, back to back by decoded size; finish() gives (summary dict, FRAME_RESULT_DTYPE rows).  Mirrors Batch."""
+
+    def __init__(self, ctx, input, dicts=None, forced_dict=None, max_window_size=0):
+        self.ctx = ctx
+        ip, il, self._k = _ptr(input)
+        darr, nd, forced = _dict_args(dicts, forced_dict)
+        self._dicts = (dicts, forced_dict)
+        h = C.c_void_p()
+        ctx._chk(ctx.L.b200z_decode_all_prepare(ctx.h, ip, il, MEM_DEVICE if _is_device(input) else MEM_HOST, darr, nd, forced, max_window_size,
+                                                C.byref(h)))
+        self.h = h
+
+    def run(self, d_output):
+        op, ol, _k = _ptr(d_output)
+        assert _is_device(d_output), "AllBatch.run writes into device memory"
+        self.ctx._chk(self.ctx.L.b200z_batch_run(self.h, op, ol))
+
+    def finish(self):
+        res = np.zeros(self.info()["frames"], dtype=FRAME_RESULT_DTYPE)
+        s = np.zeros(1, dtype=ALL_RESULT_DTYPE)
+        self.ctx._chk(self.ctx.L.b200z_decode_all_finish(self.h, s.ctypes.data, res.ctypes.data))
+        return _summary(s), res
+
+    def info(self):
+        """As Batch.info; "frames" is the number of zstd frames found."""
+        a = (C.c_uint64 * 8)()
+        self.ctx.L.b200z_batch_info(self.h, a)
+        k = ["frames", "blocks", "compressed_blocks", "planned_bytes", "literal_scratch_bytes", "sequences", "launches_per_run"]
+        return dict(zip(k, list(a)))
+
+    def close(self):
+        if getattr(self, "h", None) and self.ctx.h:
+            self.ctx.L.b200z_batch_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def decode_all_batch(ctx, input, output, dicts=None, forced_dict=None, max_window_size=0):
+    """b200z_decode_all_batch, the one-shot form of decode_all: returns the summary dict only."""
+    ip, il, _k1 = _ptr(input)
+    op, ol, _k2 = _ptr(output)
+    darr, nd, forced = _dict_args(dicts, forced_dict)
+    s = np.zeros(1, dtype=ALL_RESULT_DTYPE)
+    ctx._chk(ctx.L.b200z_decode_all_batch(ctx.h, ip, il, MEM_DEVICE if _is_device(input) else MEM_HOST, darr, nd, forced, max_window_size, op, ol,
+                                          MEM_DEVICE if _is_device(output) else MEM_HOST, s.ctypes.data))
+    return _summary(s)
+
+
+def decode_all_chain(data, by_candidates=False):
+    """Host-only: the input offsets of the frames decode_all visits -- the host-input walk, or (by_candidates) the device-input
+    selection through every magic-number candidate, with the scan and the walks done on the host."""
+    b = np.frombuffer(bytes(data), dtype=np.uint8)
+    n = C.c_size_t()
+    cap = len(b) // 4 + 2
+    out = np.zeros(cap, dtype=np.uint64)
+    rc = lib().b200z_debug_decode_all_chain(b.ctypes.data if len(b) else None, len(b), 1 if by_candidates else 0, out.ctypes.data, cap, C.byref(n))
+    if rc:
+        raise B200ZError(rc, 0, "b200z_debug_decode_all_chain")
+    return [int(x) for x in out[:n.value]]
 
 
 def compress_bound(n, dict=None):

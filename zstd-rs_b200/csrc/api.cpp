@@ -448,6 +448,13 @@ struct b200z_batch {
     bool ran = false;
     bool checksummed = false;
     uint64_t run_launches = 0;               // kernels the most recent b200z_batch_run launched
+    // decode_all batches (b200z_decode_all_prepare): `info` holds one entry per frame of the chain, in stream order, and k_place
+    // places the frames of the submission back to back on every run
+    bool decode_all = false;
+    std::vector<uint64_t> chain;             // input offset of every frame of the chain
+    std::vector<uint8_t> chain_zstd;         // 1 where the chain holds a zstd frame (one b200z_frame_result each)
+    uint64_t zstd_frames = 0;
+    uint64_t ran_output_cap = 0;             // output_cap of the most recent b200z_batch_run
 };
 
 // what k_walk brought back for a batch whose input lives in device memory (the planner then never sees the compressed bytes)
@@ -525,9 +532,12 @@ static int plan_batch(b200z_batch *b, const uint8_t *in, size_t in_len, const b2
     return 0;
 }
 
-// k_walk twice (count, fill) with a host prefix sum in between; 40 bytes per block and 48 per frame come back
-static int device_walk(b200z_ctx *c, const uint8_t *d_input, size_t input_len, const b200z_frame_io *frames, size_t nframes, WalkHost &w) {
-    w.wf.assign(nframes, WalkFrame()); w.first.assign(nframes, 0); w.wb.clear();
+// k_walk twice (count, fill) with a host prefix sum in between; 40 bytes per block and 48 per frame come back.  `counted`: w.wf already
+// holds the count pass's frame digests (decode_all's candidate walk), so only the fill pass runs.
+static int device_walk(b200z_ctx *c, const uint8_t *d_input, size_t input_len, const b200z_frame_io *frames, size_t nframes, WalkHost &w,
+                       bool counted = false) {
+    if (!counted) w.wf.assign(nframes, WalkFrame());
+    w.first.assign(nframes, 0); w.wb.clear();
     if (!nframes) return 0;
     std::vector<uint64_t> so(2 * nframes);
     for (size_t i = 0; i < nframes; i++) { so[i] = frames[i].src_off; so[nframes + i] = frames[i].src_size; }
@@ -537,10 +547,13 @@ static int device_walk(b200z_ctx *c, const uint8_t *d_input, size_t input_len, c
     if (int e = d_first.ensure(nframes * 4, false)) return e;
     CU(c, cudaMemcpyAsync(d_io.p, so.data(), so.size() * 8, cudaMemcpyHostToDevice, c->stream));
     const uint64_t *d_off = d_io.as<uint64_t>(), *d_sz = d_off + nframes;
-    int le = launch_walk(d_input, input_len, d_off, d_sz, (uint32_t)nframes, d_wf.as<WalkFrame>(), nullptr, nullptr, 0, c->stream, &c->launches);
-    if (le) return c->set_cuda_err((cudaError_t)le, "k_walk");
-    CU(c, cudaMemcpyAsync(w.wf.data(), d_wf.p, nframes * sizeof(WalkFrame), cudaMemcpyDeviceToHost, c->stream));
-    CU(c, cudaStreamSynchronize(c->stream));
+    int le = 0;
+    if (!counted) {
+        le = launch_walk(d_input, input_len, d_off, d_sz, (uint32_t)nframes, d_wf.as<WalkFrame>(), nullptr, nullptr, 0, c->stream, &c->launches);
+        if (le) return c->set_cuda_err((cudaError_t)le, "k_walk");
+        CU(c, cudaMemcpyAsync(w.wf.data(), d_wf.p, nframes * sizeof(WalkFrame), cudaMemcpyDeviceToHost, c->stream));
+        CU(c, cudaStreamSynchronize(c->stream));
+    }
     uint64_t total = 0;
     for (size_t i = 0; i < nframes; i++) { w.first[i] = (uint32_t)total; total += w.wf[i].nblocks; }
     if (total > 0xFFFFFFF0ull) return B200Z_ERR_INVALID_ARGUMENT;
@@ -554,6 +567,8 @@ static int device_walk(b200z_ctx *c, const uint8_t *d_input, size_t input_len, c
     CU(c, cudaStreamSynchronize(c->stream));
     return 0;
 }
+
+static int batch_upload(b200z_batch *b, const uint8_t *input, size_t input_len, bool on_device);
 
 extern "C" int b200z_batch_prepare(b200z_ctx *c, const uint8_t *input, size_t input_len, int input_mem, const b200z_frame_io *frames,
                                    size_t nframes, const b200z_dict *const *dicts, size_t ndicts, const b200z_dict *forced,
@@ -573,6 +588,14 @@ extern "C" int b200z_batch_prepare(b200z_ctx *c, const uint8_t *input, size_t in
     }
     if (int e = plan_batch(b.get(), on_device ? nullptr : input, input_len, frames, nframes, dicts, ndicts, forced, max_window, on_device ? &walk : nullptr))
         return e;
+    if (int e = batch_upload(b.get(), input, input_len, on_device)) return e;
+    *out = b.release();
+    return 0;
+}
+
+// the device side of a planned batch: the input (copied in when it lives in host memory), descriptors, tables and frame states
+static int batch_upload(b200z_batch *b, const uint8_t *input, size_t input_len, bool on_device) {
+    b200z_ctx *c = b->ctx;
     if (!on_device) {
         if (int e = b->d_input_own.ensure(input_len + 16, false)) return e;
         if (input_len) CU(c, cudaMemcpyAsync(b->d_input_own.p, input, input_len, cudaMemcpyHostToDevice, c->stream));
@@ -583,7 +606,6 @@ extern "C" int b200z_batch_prepare(b200z_ctx *c, const uint8_t *input, size_t in
     if (!b->sub.states.empty())
         CU(c, cudaMemcpyAsync(b->d_states_init.p, b->sub.states.data(), b->sub.states.size() * sizeof(FrameState), cudaMemcpyHostToDevice, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
-    *out = b.release();
     return 0;
 }
 
@@ -607,6 +629,24 @@ static int restore_states(b200z_batch *b) {
     return 0;
 }
 
+// A decode_all pass: the frames go back to back by the size they decode to, which is known on the device after k_fse.  So the pass
+// runs in two stages, as the frame decoder's submissions do: tables, literals and sequences of every block (k_setup, k_huf, k_fse);
+// k_place, which writes every frame's out_off / out_cap; then execution (k_exec_cta, k_exec) and, with B200Z_FLAG_CHECKSUM, k_xxh64.
+// There is no host round trip in between; what is given up is k_exec running beside k_fse.
+static int enqueue_decode_all_pass(b200z_ctx *c, const PipelineArgs &a, const PipelineStreams &ps, bool *checksummed, uint64_t *launched) {
+    PipelineArgs a_dec = a;
+    a_dec.nframes = 0;
+    if (int e = launch_pipeline_overlapped(a_dec, ps, launched)) return c->set_cuda_err((cudaError_t)e, "launch_pipeline (decode)");
+    if (int e = launch_place(a, ps.main, launched)) return c->set_cuda_err((cudaError_t)e, "k_place");
+    PipelineArgs a_ex = a;
+    a_ex.nblocks = 0;
+    if (int e = launch_pipeline_overlapped(a_ex, ps, launched)) return c->set_cuda_err((cudaError_t)e, "launch_pipeline (execute)");
+    *checksummed = (c->flags & B200Z_FLAG_CHECKSUM) && a.nframes;
+    if (*checksummed)
+        if (int e = launch_checksum(a, ps.main, launched)) return c->set_cuda_err((cudaError_t)e, "launch_checksum");
+    return 0;
+}
+
 extern "C" int b200z_batch_run(b200z_batch *b, uint8_t *d_output, size_t output_cap) {
     if (!b) return B200Z_ERR_INVALID_ARGUMENT;
     b200z_ctx *c = b->ctx;
@@ -614,7 +654,10 @@ extern "C" int b200z_batch_run(b200z_batch *b, uint8_t *d_output, size_t output_
     if (int e = restore_states(b)) return e;
     PipelineArgs a = b->sub.args(b->d_input, d_output, output_cap);
     b->run_launches = 0;
-    int e = enqueue_pass(c, a, PipelineStreams{c->stream, c->side, c->ev_fork, c->ev_join}, &b->checksummed, &b->run_launches);
+    b->ran_output_cap = output_cap;
+    const PipelineStreams ps{c->stream, c->side, c->ev_fork, c->ev_join};
+    int e = b->decode_all ? enqueue_decode_all_pass(c, a, ps, &b->checksummed, &b->run_launches)
+                          : enqueue_pass(c, a, ps, &b->checksummed, &b->run_launches);
     c->launches += b->run_launches;
     if (e) return e;
     b->ran = true;
@@ -623,7 +666,7 @@ extern "C" int b200z_batch_run(b200z_batch *b, uint8_t *d_output, size_t output_
 
 // Same as b200z_batch_run but with a CUDA event between stages; synchronises and reports per-kernel milliseconds.
 extern "C" int b200z_batch_run_profile(b200z_batch *b, uint8_t *d_output, size_t output_cap, float *stage_ms, size_t nstages) {
-    if (!b || !stage_ms) return B200Z_ERR_INVALID_ARGUMENT;
+    if (!b || !stage_ms || b->decode_all) return B200Z_ERR_INVALID_ARGUMENT;
     b200z_ctx *c = b->ctx;
     if (int e = c->use()) return e;
     if (int e = restore_states(b)) return e;
@@ -647,7 +690,7 @@ extern "C" int b200z_batch_run_profile(b200z_batch *b, uint8_t *d_output, size_t
 // the start of the pass, of the table builds + k_huf (two streams), of the pair k_fse + k_exec (k_exec runs beside k_fse as its programmatic dependent: an event
 // between the two would serialise them) and of k_exec_cta + the k_exec launch that takes what it handed back.
 extern "C" int b200z_batch_run_timeline(b200z_batch *b, uint8_t *d_output, size_t output_cap, float *out_ms, size_t n) {
-    if (!b || !out_ms || n < 4) return B200Z_ERR_INVALID_ARGUMENT;
+    if (!b || !out_ms || n < 4 || b->decode_all) return B200Z_ERR_INVALID_ARGUMENT;
     b200z_ctx *c = b->ctx;
     if (int e = c->use()) return e;
     if (int e = restore_states(b)) return e;
@@ -719,7 +762,7 @@ static void fill_result(const b200z_batch *b, size_t i, const FrameState *st, b2
 }
 
 extern "C" int b200z_batch_finish(b200z_batch *b, b200z_frame_result *results) {
-    if (!b || !results) return B200Z_ERR_INVALID_ARGUMENT;
+    if (!b || !results || b->decode_all) return B200Z_ERR_INVALID_ARGUMENT;
     b200z_ctx *c = b->ctx;
     if (int e = c->use()) return e;
     Submission &s = b->sub;
@@ -738,7 +781,7 @@ extern "C" int b200z_batch_info(const b200z_batch *b, uint64_t out[8]) {
     const Submission &s = b->sub;
     uint64_t ncomp = 0, planned = 0;
     for (auto &d : s.descs) { ncomp += d.btype == BT_COMPRESSED; planned += d.src_size + 3; }
-    out[0] = s.frames.size(); out[1] = s.descs.size(); out[2] = ncomp; out[3] = planned; out[4] = s.lit_bytes; out[5] = s.nseq;
+    out[0] = b->decode_all ? b->zstd_frames : s.frames.size(); out[1] = s.descs.size(); out[2] = ncomp; out[3] = planned; out[4] = s.lit_bytes; out[5] = s.nseq;
     out[6] = b->run_launches; out[7] = 0;
     return 0;
 }
@@ -995,6 +1038,267 @@ extern "C" int b200z_decode_frames_batch(b200z_ctx *c, const uint8_t *input, siz
             CU(c, cudaMemcpyAsync(output + lo, dout + lo, hi - lo, cudaMemcpyDeviceToHost, c->stream));
             CU(c, cudaStreamSynchronize(c->stream));
         }
+    }
+    return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// tier 1c: decode_all on the batch path (FrameDecoder::decode_all, frame_decoder.rs:541-577) -- find the frames of a buffer of
+// concatenated frames, decode them in one submission, place them back to back by decoded size on the device (k_place)
+// ---------------------------------------------------------------------------------------------------------------
+namespace {
+
+struct Chain {
+    std::vector<uint64_t> at;    // input offset of every frame visited, the one where the chain ends included
+    std::vector<WalkFrame> wf;   // its header walk (a zeroed digest where no frame starts: it parses as BadMagicNumber / MagicNumberRead)
+};
+
+// decode_all's way from one frame to the next, from offset 0 (frame_chain_next, framing.cuh): it ends at the end of the input, at a
+// break in the chain, or at a skippable frame that runs past the input.  walk_at(pos) gives the walk of the frame at pos, or null when
+// no frame starts there.
+template <class WalkAt>
+void follow_chain(uint64_t input_len, WalkAt walk_at, Chain &ch) {
+    ch.at.clear(); ch.wf.clear();
+    for (uint64_t pos = 0; pos < input_len;) {
+        WalkFrame none;
+        const WalkFrame *F = walk_at(pos);
+        if (!F) {
+            memset(&none, 0, sizeof none);
+            none.hdr_avail = (uint32_t)std::min<uint64_t>(input_len - pos, 20);
+            none.stop = 4;
+            F = &none;
+        }
+        ch.at.push_back(pos); ch.wf.push_back(*F);
+        const uint64_t next = frame_chain_next(pos, *F);
+        if (next == pos || next > input_len) break;
+        pos = next;
+    }
+}
+
+// host input: the same walk as k_walk, on the host
+void host_chain(const uint8_t *in, uint64_t input_len, Chain &ch) {
+    WalkFrame F;
+    follow_chain(input_len, [&](uint64_t pos) -> const WalkFrame * { walk_frame(in + pos, input_len - pos, F, nullptr, nullptr, 0, 0); return &F; }, ch);
+}
+
+// device input: the chain through the candidate frame starts (any order) and their walks with the bytes left from each
+void chain_from_candidates(uint64_t input_len, const std::vector<uint64_t> &cand, const std::vector<WalkFrame> &cand_wf, Chain &ch) {
+    std::vector<uint32_t> order(cand.size());
+    for (uint32_t i = 0; i < order.size(); i++) order[i] = i;
+    std::sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) { return cand[x] < cand[y]; });
+    std::vector<uint64_t> sorted(cand.size());
+    for (size_t i = 0; i < order.size(); i++) sorted[i] = cand[order[i]];
+    follow_chain(input_len, [&](uint64_t pos) -> const WalkFrame * {
+        auto it = std::lower_bound(sorted.begin(), sorted.end(), pos);
+        return it != sorted.end() && *it == pos ? &cand_wf[order[it - sorted.begin()]] : nullptr;
+    }, ch);
+}
+
+bool is_frame_magic(const uint8_t *p) { const uint32_t m = rd32le(p); return m == ZSTD_MAGIC || skippable_magic(m); }
+
+}  // namespace
+
+// k_find_frames, then k_walk in count mode once per candidate; the candidates' offsets and frame digests come back, not the input
+static int device_chain(b200z_ctx *c, const uint8_t *d_input, uint64_t input_len, Chain &ch) {
+    std::vector<uint64_t> cand;
+    std::vector<WalkFrame> cand_wf;
+    uint64_t n = 0;
+    if (input_len >= 4) {
+        uint64_t cap = 4096 + input_len / 16384;
+        DevBuf d_cand, d_count, d_wf;
+        for (;;) {
+            if (cap > 0xFFFFFFF0ull) return B200Z_ERR_INVALID_ARGUMENT;
+            if (int e = d_cand.ensure(2 * cap * 8, false)) return e;
+            if (int e = d_count.ensure(8, false)) return e;
+            CU(c, cudaMemsetAsync(d_count.p, 0, 8, c->stream));
+            uint64_t *d_off = d_cand.as<uint64_t>(), *d_size = d_off + cap;
+            if (int le = launch_find_frames(d_input, input_len, d_off, d_size, (uint32_t)cap, d_count.as<unsigned long long>(), c->stream, &c->launches))
+                return c->set_cuda_err((cudaError_t)le, "k_find_frames");
+            CU(c, cudaMemcpyAsync(&n, d_count.p, 8, cudaMemcpyDeviceToHost, c->stream));
+            CU(c, cudaStreamSynchronize(c->stream));
+            if (n <= cap) break;
+            cap = n;   // more candidates than room (false candidates are ordinary input): grow and scan again
+        }
+        if (n) {
+            uint64_t *d_off = d_cand.as<uint64_t>(), *d_size = d_off + cap;
+            if (int e = d_wf.ensure(n * sizeof(WalkFrame), false)) return e;
+            if (int le = launch_walk(d_input, input_len, d_off, d_size, (uint32_t)n, d_wf.as<WalkFrame>(), nullptr, nullptr, 0, c->stream, &c->launches))
+                return c->set_cuda_err((cudaError_t)le, "k_walk");
+            cand.resize(n); cand_wf.resize(n);
+            CU(c, cudaMemcpyAsync(cand.data(), d_off, n * 8, cudaMemcpyDeviceToHost, c->stream));
+            CU(c, cudaMemcpyAsync(cand_wf.data(), d_wf.p, n * sizeof(WalkFrame), cudaMemcpyDeviceToHost, c->stream));
+            CU(c, cudaStreamSynchronize(c->stream));
+        }
+    }
+    chain_from_candidates(input_len, cand, cand_wf, ch);
+    return 0;
+}
+
+extern "C" int b200z_debug_decode_all_chain(const uint8_t *input, size_t input_len, int by_candidates, uint64_t *at, size_t cap, size_t *n) {
+    if (!n || (!input && input_len) || (!at && cap)) return B200Z_ERR_INVALID_ARGUMENT;
+    Chain ch;
+    if (!by_candidates) host_chain(input, input_len, ch);
+    else {
+        std::vector<uint64_t> cand;
+        std::vector<WalkFrame> cand_wf;
+        for (uint64_t p = 0; p + 4 <= input_len; p++) {
+            if (!is_frame_magic(input + p)) continue;
+            cand.push_back(p);
+            cand_wf.emplace_back();
+            walk_frame(input + p, input_len - p, cand_wf.back(), nullptr, nullptr, 0, 0);
+        }
+        std::reverse(cand.begin(), cand.end());   // the device's candidates come in no particular order
+        std::reverse(cand_wf.begin(), cand_wf.end());
+        chain_from_candidates(input_len, cand, cand_wf, ch);
+    }
+    for (size_t i = 0; i < ch.at.size() && i < cap; i++) at[i] = ch.at[i];
+    *n = ch.at.size();
+    return 0;
+}
+
+extern "C" int b200z_decode_all_prepare(b200z_ctx *c, const uint8_t *input, size_t input_len, int input_mem, const b200z_dict *const *dicts,
+                                        size_t ndicts, const b200z_dict *forced, uint64_t max_window, b200z_batch **out) {
+    if (!c || !out || (!input && input_len) || (!dicts && ndicts)) return B200Z_ERR_INVALID_ARGUMENT;
+    *out = nullptr;
+    if (int e = c->use()) return e;
+    std::unique_ptr<b200z_batch> b(new b200z_batch());
+    b->ctx = c; b->input_len = input_len; b->decode_all = true;
+    const bool on_device = input_mem == B200Z_MEM_DEVICE;
+    Chain ch;
+    if (on_device) {
+        b->d_input = input;
+        if (int e = device_chain(c, input, input_len, ch)) return e;
+    } else {
+        host_chain(input, input_len, ch);
+    }
+    // every frame of the chain is planned with the rest of the input; the plaintexts are placed by k_place on every run
+    std::vector<b200z_frame_io> io(ch.at.size());
+    b->chain = ch.at;
+    b->chain_zstd.assign(ch.at.size(), 0);
+    for (size_t i = 0; i < io.size(); i++) {
+        io[i] = b200z_frame_io{ch.at[i], input_len - ch.at[i], 0, 0};
+        b->chain_zstd[i] = ch.wf[i].hdr_avail >= 4 && rd32le(ch.wf[i].hdr) == ZSTD_MAGIC;
+        b->zstd_frames += b->chain_zstd[i];
+    }
+    WalkHost walk;
+    if (on_device) {
+        walk.wf = ch.wf;   // the candidates' count pass: only the fill pass runs again
+        if (int e = device_walk(c, input, input_len, io.data(), io.size(), walk, true)) return e;
+    }
+    if (int e = plan_batch(b.get(), on_device ? nullptr : input, input_len, io.data(), io.size(), dicts, ndicts, forced, max_window, on_device ? &walk : nullptr))
+        return e;
+    if (int e = batch_upload(b.get(), input, input_len, on_device)) return e;
+    *out = b.release();
+    return 0;
+}
+
+// decode_all's loop over the frame that runs out of output (frame_decoder.rs:556-572): decode_blocks(UptoBytes(1 MiB)), read what the
+// output still holds, TargetTooSmall while the decode buffer keeps collectable bytes (the window is kept until the frame is finished).
+// size[0..n) are the bytes of the blocks that decode.  fails: the frame's error comes next -- block n fails, or, when
+// `last_is_final` (block n - 1 is the frame's last block), the content checksum cannot be read.  Returns true when the reference
+// raises TargetTooSmall before that error (or before the end of the frame).
+static bool decode_all_runs_out_first(const uint64_t *size, uint32_t n, bool fails, bool last_is_final, uint64_t window, uint64_t room) {
+    uint64_t buf = 0;
+    uint32_t i = 0;
+    for (;;) {
+        uint64_t grown = 0;
+        bool finished = false;
+        for (;;) {
+            if (i == n) return false;   // block n fails before anything more is read
+            buf += size[i]; grown += size[i]; i++;
+            if (i == n && last_is_final) {
+                if (fails) return false;   // FailedToReadChecksum, in the same decode_blocks call
+                finished = true;
+                break;
+            }
+            if (grown >= (1u << 20)) break;
+        }
+        const uint64_t drainable = finished ? buf : (buf > window ? buf - window : 0);
+        const uint64_t amount = std::min(room, drainable);
+        room -= amount; buf -= amount;
+        if (finished ? buf : (buf > window ? buf - window : 0)) return true;
+        if (finished) return false;
+    }
+}
+
+extern "C" int b200z_decode_all_finish(b200z_batch *b, b200z_all_result *sum, b200z_frame_result *results) {
+    if (!b || !sum || !b->decode_all) return B200Z_ERR_INVALID_ARGUMENT;
+    b200z_ctx *c = b->ctx;
+    if (int e = c->use()) return e;
+    const Submission &s = b->sub;
+    std::vector<FrameState> st(s.states.size());
+    if (!st.empty()) CU(c, cudaMemcpyAsync(st.data(), s.d_states.p, st.size() * sizeof(FrameState), cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    memset(sum, 0, sizeof *sum);
+    sum->error_offset = b->input_len;
+    sum->error_frame = -1;
+    bool failed = false;
+    auto fail = [&](uint32_t word, size_t i, int32_t zi) {
+        failed = true;
+        sum->status = (int32_t)status_code(word); sum->stage = (int32_t)status_stage(word);
+        sum->error_offset = b->chain[i]; sum->error_frame = zi;
+    };
+    int32_t zi = -1;
+    for (size_t i = 0; i < b->chain.size(); i++) {
+        const FramePlanInfo &fi = b->info[i];
+        const FrameState *fs = fi.sub_frame >= 0 ? &st[fi.sub_frame] : nullptr;
+        if (b->chain_zstd[i]) { zi++; if (results) fill_result(b, i, fs, results[zi]); }
+        if (failed) continue;
+        if (fi.pre_status == B200Z_ERR_SKIP_FRAME) {   // `input.get(length..)`: the skipped bytes must be there
+            if (b->chain[i] + 8 + fi.skip_len > b->input_len) fail(mk_status(B200Z_ERR_FAILED_TO_SKIP_FRAME, B200Z_STAGE_FRAME_HEADER), i, -1);
+            else sum->skippable_frames++;
+            continue;
+        }
+        if (fi.pre_status) { fail(mk_status((uint32_t)fi.pre_status, (uint32_t)fi.pre_stage), i, b->chain_zstd[i] ? zi : -1); continue; }
+        if (fs->status == 0) { sum->written += fs->produced; sum->frames++; continue; }
+        // The first failing frame.  What the device found first is the reference's error unless the output ran out before it: replay
+        // decode_all's loop over the frame's block sizes.  With TargetTooSmall from the device (the frame did not fit), the error that
+        // may come before it is the first one stage A or the planner found.
+        const FrameDesc &fd = s.frames[fi.sub_frame];
+        std::vector<BlockAux> aux(fd.nblocks);
+        if (fd.nblocks) {
+            CU(c, cudaMemcpyAsync(aux.data(), s.d_aux.as<BlockAux>() + fd.first_block, fd.nblocks * sizeof(BlockAux), cudaMemcpyDeviceToHost, c->stream));
+            CU(c, cudaStreamSynchronize(c->stream));
+        }
+        uint32_t word = fs->status, n = fs->blocks_done;
+        bool fails = true;
+        if (status_code(word) == B200Z_ERR_TARGET_TOO_SMALL) {
+            word = fd.host_status; n = fd.nblocks;
+            for (uint32_t k = 0; k < fd.nblocks; k++) {
+                const BlockAux &x = aux[k];
+                if (uint32_t w = block_first_error(s.descs[fd.first_block + k].host_status, x.status, x.seq_status)) { word = w; n = k; break; }
+            }
+            fails = word != 0;
+        }
+        std::vector<uint64_t> size(n);
+        for (uint32_t k = 0; k < n; k++) size[k] = aux[k].out_size;
+        const bool last_is_final = n > 0 && s.descs[fd.first_block + n - 1].last;
+        if (decode_all_runs_out_first(size.data(), n, fails, last_is_final, fi.window, b->ran_output_cap - sum->written))
+            word = mk_status(B200Z_ERR_TARGET_TOO_SMALL, 0);
+        fail(word, i, zi);
+    }
+    return 0;
+}
+
+extern "C" int b200z_decode_all_batch(b200z_ctx *c, const uint8_t *input, size_t input_len, int input_mem, const b200z_dict *const *dicts,
+                                      size_t ndicts, const b200z_dict *forced, uint64_t max_window, uint8_t *output, size_t output_cap,
+                                      int output_mem, b200z_all_result *summary) {
+    if (!c || !summary || (!output && output_cap)) return B200Z_ERR_INVALID_ARGUMENT;
+    b200z_batch *b = nullptr;
+    int e = b200z_decode_all_prepare(c, input, input_len, input_mem, dicts, ndicts, forced, max_window, &b);
+    if (e) return e;
+    std::unique_ptr<b200z_batch, void (*)(b200z_batch *)> guard(b, b200z_batch_destroy);
+    DevBuf d_out;
+    uint8_t *dout = output;
+    if (output_mem != B200Z_MEM_DEVICE) {
+        if ((e = d_out.ensure(output_cap + 16, false))) return e;
+        dout = d_out.as<uint8_t>();
+    }
+    if ((e = b200z_batch_run(b, dout, output_cap))) return e;
+    if ((e = b200z_decode_all_finish(b, summary, nullptr))) return e;
+    if (output_mem != B200Z_MEM_DEVICE && summary->written) {
+        CU(c, cudaMemcpyAsync(output, dout, summary->written, cudaMemcpyDeviceToHost, c->stream));
+        CU(c, cudaStreamSynchronize(c->stream));
     }
     return 0;
 }

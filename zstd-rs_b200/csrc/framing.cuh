@@ -184,4 +184,59 @@ struct WalkBlock {
     uint8_t pad[5];
 };
 
+// The header walk of the frame at p[0..len): the planner's parsers along the chain of blocks, run by k_walk on device input and by
+// the host on host input.  F gets the frame digest.  fill == 0 only counts the blocks; fill == 1 writes their digests at
+// wb[first[idx]].  Anything wrong with the frame header is the planner's to report (stop = 4, no blocks).
+B200Z_HD void walk_frame(const uint8_t *p, uint64_t len, WalkFrame &F, WalkBlock *wb, const uint32_t *first, uint32_t idx, int fill) {
+    const uint32_t hdr_avail = (uint32_t)(len < 20 ? len : 20);
+    for (uint32_t i = 0; i < 20; i++) F.hdr[i] = i < hdr_avail ? p[i] : 0;
+    uint32_t nb = 0, stop = 4, tail_avail = 0;
+    uint64_t end_pos = 0;
+    FrameHeader fh;
+    uint32_t skip_len;
+    size_t pos;
+    if (parse_frame_header(p, len, fh, skip_len, pos) == 0) {
+        const uint32_t base = fill ? first[idx] : 0u;
+        for (;;) {
+            if (len - pos < 3) { stop = 1; break; }
+            WalkBlock B = {};
+            B.pos = pos; B.bh[0] = p[pos]; B.bh[1] = p[pos + 1]; B.bh[2] = p[pos + 2];
+            BlockHeader bh;
+            if (parse_block_header(p + pos, bh)) {   // the planner reports FoundReservedBlock / BlockSizeTooLarge from these 3 bytes
+                if (fill) wb[base + nb] = B;
+                nb++; stop = 2; break;
+            }
+            pos += 3;
+            if (len - pos < bh.content_size) {
+                if (fill) wb[base + nb] = B;
+                nb++; stop = 3; break;
+            }
+            if (bh.type == BT_COMPRESSED) B.sec = parse_section_headers(p + pos, bh.content_size);
+            if (fill) wb[base + nb] = B;
+            nb++;
+            pos += bh.content_size;
+            if (bh.last) {   // the content checksum may follow
+                stop = 0;
+                tail_avail = (uint32_t)(len - pos < 4 ? len - pos : 4);
+                break;
+            }
+        }
+        end_pos = pos;
+    }
+    for (uint32_t i = 0; i < 4; i++) F.tail[i] = i < tail_avail ? p[end_pos + i] : 0;
+    F.hdr_avail = hdr_avail; F.nblocks = nb; F.stop = stop; F.tail_avail = tail_avail; F.pad = 0; F.end_pos = end_pos;
+}
+
+// Where a buffer of concatenated frames goes on after the frame at offset `at` whose walk is F (decode_all, frame_decoder.rs:541-577):
+// behind the content checksum, if the descriptor announces one, for a zstd frame whose walk reached its last block; behind the
+// skipped bytes for a skippable frame; `at` itself -- the chain ends there -- for anything else.  The caller checks the result
+// against the input's length (a skippable frame that runs past it is FailedToSkipFrame).
+B200Z_HD uint64_t frame_chain_next(uint64_t at, const WalkFrame &F) {
+    if (F.hdr_avail < 4) return at;
+    const uint32_t magic = rd32le(F.hdr);
+    if (skippable_magic(magic)) return F.hdr_avail < 8 ? at : at + 8 + rd32le(F.hdr + 4);
+    if (magic != ZSTD_MAGIC || F.stop != 0) return at;
+    return at + F.end_pos + (((F.hdr[4] >> 2) & 1u) ? 4 : 0);
+}
+
 }  // namespace b200z

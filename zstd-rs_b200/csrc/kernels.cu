@@ -10,6 +10,7 @@
 //   k_exec       : LZ77 execution into the frame's output (execute_sequences sequence_execution.rs:5-118,
 //                  DecodeBuffer::{push,repeat,repeat_from_dict} decode_buffer.rs:74-179), one warp per frame,
 //                  blocks of a frame in order
+//   k_find_frames, k_place : decode_all's frame discovery on device input and back-to-back placement by decoded size
 //
 // Integer/byte work only; the roofline is HBM bandwidth (DESIGN.md section 4).
 #include <cuda_runtime.h>
@@ -1323,7 +1324,7 @@ __global__ void k_xxh64(const FrameDesc *__restrict__ frames, FrameState *__rest
 
 // ------------------------------------------------------------------------------------------------------------
 // k_walk: the frame / block / section header walk on the device, for input that lives in device memory (SURVEY 8(f) rank 3,
-// first step).  One thread per frame runs the planner's own header parsers (framing.cuh) along the chain of blocks and hands it
+// first step).  One thread per frame runs the planner's own header parsers (walk_frame, framing.cuh) along the chain of blocks and hands it
 // their results, with the frame header bytes and the checksum: 40 bytes per block instead of the whole compressed input.
 // fill == 0: count the blocks; fill == 1: write the digests at first_block[frame].  The digests are assembled in global memory,
 // so that no byte array of the thread needs local memory.
@@ -1334,45 +1335,138 @@ __global__ void k_walk(const uint8_t *__restrict__ input, uint64_t input_len, co
     if (f >= nframes) return;
     const uint64_t so = src_off[f];
     const uint64_t len = so <= input_len && src_size[f] <= input_len - so ? src_size[f] : 0;   // (out of range: nothing to walk)
-    const uint8_t *p = input + so;
-    WalkFrame &F = wf[f];
-    const uint32_t hdr_avail = (uint32_t)(len < 20 ? len : 20);
-    for (uint32_t i = 0; i < 20; i++) F.hdr[i] = i < hdr_avail ? p[i] : 0;
-    uint32_t nb = 0, stop = 4, tail_avail = 0;
-    uint64_t end_pos = 0;
-    FrameHeader fh;
-    uint32_t skip_len;
-    size_t pos;
-    if (parse_frame_header(p, len, fh, skip_len, pos) == 0) {   // anything wrong with the frame header is the planner's to report
-        const uint32_t base = fill ? first_block[f] : 0u;
-        for (;;) {
-            if (len - pos < 3) { stop = 1; break; }
-            WalkBlock B = {};
-            B.pos = pos; B.bh[0] = p[pos]; B.bh[1] = p[pos + 1]; B.bh[2] = p[pos + 2];
-            BlockHeader bh;
-            if (parse_block_header(p + pos, bh)) {   // the planner reports FoundReservedBlock / BlockSizeTooLarge from these 3 bytes
-                if (fill) wb[base + nb] = B;
-                nb++; stop = 2; break;
-            }
-            pos += 3;
-            if (len - pos < bh.content_size) {
-                if (fill) wb[base + nb] = B;
-                nb++; stop = 3; break;
-            }
-            if (bh.type == BT_COMPRESSED) B.sec = parse_section_headers(p + pos, bh.content_size);
-            if (fill) wb[base + nb] = B;
-            nb++;
-            pos += bh.content_size;
-            if (bh.last) {   // the content checksum may follow
-                stop = 0;
-                tail_avail = (uint32_t)(len - pos < 4 ? len - pos : 4);
-                break;
+    walk_frame(input + so, len, wf[f], wb, first_block, f, fill);
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// k_find_frames: the candidate frame starts of a buffer of concatenated frames (decode_all) -- every byte offset whose 4 bytes
+// read a zstd magic number (0xFD2FB528) or a skippable one (0x184D2A50..5F).  The walk from one frame to the next is serial; this
+// scan is not.  One lane per 16-byte-aligned chunk of the buffer: it loads its chunk and the next one as 16-byte vectors, never a
+// chunk that holds no input byte (the caller's buffer is not padded), and tests the 16 offsets of its chunk.  A warp compacts its
+// candidates with a ballot, a shuffle scan and one atomic: off[] gets the offsets and size[] the bytes left from each (the
+// src_size k_walk walks it with), up to `cap`; *count gets the number found, which may exceed cap (the caller grows and relaunches).
+// ------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t frame_magic_hits(uint4 a, uint4 b) {
+    const uint32_t w[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+    uint32_t hits = 0;
+#pragma unroll
+    for (uint32_t j = 0; j < 16; j++) {
+        const uint32_t k = j >> 2, s = (j & 3) * 8;
+        const uint32_t v = s ? __funnelshift_r(w[k], w[k + 1], s) : w[k];
+        if (v == ZSTD_MAGIC || (v & 0xFFFFFFF0u) == 0x184D2A50u) hits |= 1u << j;
+    }
+    return hits;
+}
+
+__global__ void __launch_bounds__(256) k_find_frames(const uint8_t *__restrict__ input, uint64_t input_len, uint64_t *__restrict__ off,
+                                                     uint64_t *__restrict__ size, uint32_t cap, unsigned long long *__restrict__ count) {
+    const uint64_t a0 = (uint64_t)(uintptr_t)input & ~15ull, end = (uint64_t)(uintptr_t)input + input_len;
+    const uint64_t nchunks = (end - a0 + 15) >> 4;
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t warps = (uint64_t)gridDim.x * (blockDim.x >> 5);
+    for (uint64_t c0 = ((uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * 32; c0 < nchunks; c0 += warps * 32) {
+        const uint64_t c = c0 + lane;
+        uint32_t hits = 0;
+        if (c < nchunks) {
+            const uint64_t at = a0 + 16 * c;
+            const uint4 v = __ldg((const uint4 *)at);
+            const uint4 nx = at + 16 < end ? __ldg((const uint4 *)(at + 16)) : make_uint4(0, 0, 0, 0);
+            hits = frame_magic_hits(v, nx);
+            // offsets before the buffer, and those with fewer than 4 bytes left in it, are no candidates
+            const uint64_t first = (uint64_t)(uintptr_t)input;
+            if (at < first) hits &= 0xFFFFu << (first - at);
+            if (at + 20 > end) {
+                const int64_t last = (int64_t)end - 4 - (int64_t)at;   // the last offset of the chunk with 4 bytes left
+                hits &= last < 0 ? 0u : (1u << (last + 1)) - 1u;
             }
         }
-        end_pos = pos;
+        const uint32_t n = __popc(hits);
+        if (!__ballot_sync(0xffffffffu, n != 0)) continue;
+        uint32_t incl = n;
+#pragma unroll
+        for (uint32_t d = 1; d < 32; d <<= 1) {
+            const uint32_t t = __shfl_up_sync(0xffffffffu, incl, d);
+            if (lane >= d) incl += t;
+        }
+        unsigned long long base = 0;
+        if (lane == 31) base = atomicAdd(count, (unsigned long long)incl);
+        base = __shfl_sync(0xffffffffu, base, 31);
+        uint64_t slot = base + incl - n;
+        for (; hits; hits &= hits - 1, slot++) {
+            if (slot >= cap) break;
+            const uint64_t o = a0 + 16 * c + __ffs(hits) - 1 - (uint64_t)(uintptr_t)input;
+            off[slot] = o; size[slot] = input_len - o;
+        }
     }
-    for (uint32_t i = 0; i < 4; i++) F.tail[i] = i < tail_avail ? p[end_pos + i] : 0;
-    F.hdr_avail = hdr_avail; F.nblocks = nb; F.stop = stop; F.tail_avail = tail_avail; F.pad = 0; F.end_pos = end_pos;
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// k_place: where each frame of a decode_all submission writes, by what it decodes to (never by Frame_Content_Size; the reference
+// does not compare the two): a frame's size is the sum of its blocks' out_size (Raw and RLE included) up to its first error
+// (block_first_error); an exclusive scan over the frames in submission order places them back to back.  out_off / out_cap of
+// every frame are written into the frame descriptors, clamped to output_cap.  Runs between k_fse and the execution kernels.
+// One CTA: tiles of PLACE_THREADS * PLACE_PER_THREAD frames, a thread takes consecutive frames, a shuffle + shared-memory scan
+// across the CTA, and a running carry from one tile to the next.
+// ------------------------------------------------------------------------------------------------------------
+constexpr uint32_t PLACE_THREADS = 1024, PLACE_PER_THREAD = 4;
+
+__global__ void __launch_bounds__(PLACE_THREADS) k_place(const BlockDesc *__restrict__ descs, const BlockAux *__restrict__ aux,
+                                                         FrameDesc *__restrict__ frames, uint32_t nframes, uint64_t output_cap) {
+    __shared__ uint64_t warp_sum[PLACE_THREADS / 32];
+    __shared__ uint64_t carry_s;
+    const uint32_t t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    if (t == 0) carry_s = 0;
+    __syncthreads();
+    for (uint32_t tile = 0; tile < nframes; tile += PLACE_THREADS * PLACE_PER_THREAD) {
+        uint64_t sz[PLACE_PER_THREAD], mine = 0;
+#pragma unroll
+        for (uint32_t k = 0; k < PLACE_PER_THREAD; k++) {
+            const uint32_t f = tile + t * PLACE_PER_THREAD + k;
+            uint64_t s = 0;
+            if (f < nframes) {
+                const uint32_t b0 = frames[f].first_block, nb = frames[f].nblocks;
+                for (uint32_t b = b0; b < b0 + nb; b++) {
+                    const BlockAux &x = aux[b];
+                    if (block_first_error(descs[b].host_status, x.status, x.seq_status)) break;
+                    s += x.out_size;
+                }
+            }
+            sz[k] = s; mine += s;
+        }
+        // exclusive scan of `mine` across the CTA
+        uint64_t incl = mine;
+#pragma unroll
+        for (uint32_t d = 1; d < 32; d <<= 1) {
+            const uint64_t v = __shfl_up_sync(0xffffffffu, incl, d);
+            if (lane >= d) incl += v;
+        }
+        if (lane == 31) warp_sum[warp] = incl;
+        __syncthreads();
+        if (warp == 0) {
+            uint64_t w = warp_sum[lane], wi = w;
+#pragma unroll
+            for (uint32_t d = 1; d < 32; d <<= 1) {
+                const uint64_t v = __shfl_up_sync(0xffffffffu, wi, d);
+                if (lane >= d) wi += v;
+            }
+            warp_sum[lane] = wi - w;   // exclusive prefix of the warps
+        }
+        __syncthreads();
+        uint64_t at = carry_s + warp_sum[warp] + incl - mine;
+#pragma unroll
+        for (uint32_t k = 0; k < PLACE_PER_THREAD; k++) {
+            const uint32_t f = tile + t * PLACE_PER_THREAD + k;
+            if (f < nframes) {
+                const uint64_t o = at < output_cap ? at : output_cap;
+                frames[f].out_off = o;
+                frames[f].out_cap = sz[k] < output_cap - o ? sz[k] : output_cap - o;
+            }
+            at += sz[k];
+        }
+        __syncthreads();
+        if (t == PLACE_THREADS - 1) carry_s = at;
+        __syncthreads();
+    }
 }
 
 }  // namespace b200z
@@ -1478,6 +1572,21 @@ int launch_walk(const uint8_t *d_input, uint64_t input_len, const uint64_t *d_sr
                 const uint32_t *d_first_block, WalkBlock *d_wb, int fill, cudaStream_t s, uint64_t *launched) {
     if (!nframes) return 0;
     k_walk<<<cdiv(nframes, 128), 128, 0, s>>>(d_input, input_len, d_src_off, d_src_size, nframes, d_wf, d_first_block, d_wb, fill);
+    return launched_one(launched);
+}
+
+int launch_find_frames(const uint8_t *d_input, uint64_t input_len, uint64_t *d_off, uint64_t *d_size, uint32_t cap, unsigned long long *d_count,
+                       cudaStream_t s, uint64_t *launched) {
+    if (input_len < 4) return 0;
+    const uint64_t nchunks = ((uint64_t)(uintptr_t)d_input + input_len - ((uint64_t)(uintptr_t)d_input & ~15ull) + 15) >> 4;
+    const uint64_t want = (nchunks + 255) / 256, most = (uint64_t)num_sms() * 16;
+    k_find_frames<<<(uint32_t)(want < most ? want : most), 256, 0, s>>>(d_input, input_len, d_off, d_size, cap, d_count);
+    return launched_one(launched);
+}
+
+int launch_place(const PipelineArgs &a, cudaStream_t s, uint64_t *launched) {
+    if (!a.nframes) return 0;
+    k_place<<<1, PLACE_THREADS, 0, s>>>(a.descs, a.aux, const_cast<FrameDesc *>(a.frames), a.nframes, a.output_cap);
     return launched_one(launched);
 }
 

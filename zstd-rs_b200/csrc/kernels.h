@@ -44,6 +44,12 @@ int launch_pipeline(const PipelineArgs &a, cudaStream_t s, uint64_t *launched); 
 // device-side header walk for device-resident input (k_walk): fill = 0 counts the blocks of every frame, fill = 1 writes the digests
 int launch_walk(const uint8_t *d_input, uint64_t input_len, const uint64_t *d_src_off, const uint64_t *d_src_size, uint32_t nframes, WalkFrame *d_wf,
                 const uint32_t *d_first_block, WalkBlock *d_wb, int fill, cudaStream_t s, uint64_t *launched);
+// candidate frame starts of a buffer of concatenated frames (k_find_frames): offsets and bytes left from them into d_off / d_size (room for
+// cap), the number found into *d_count (zeroed by the caller; it may exceed cap)
+int launch_find_frames(const uint8_t *d_input, uint64_t input_len, uint64_t *d_off, uint64_t *d_size, uint32_t cap, unsigned long long *d_count,
+                       cudaStream_t s, uint64_t *launched);
+// k_place: out_off / out_cap of every frame of a.frames, back to back by decoded size (after k_fse, before execution)
+int launch_place(const PipelineArgs &a, cudaStream_t s, uint64_t *launched);
 uint32_t num_sms();   // of the current device (132 on H100 SXM)
 int launch_checksum(const PipelineArgs &a, cudaStream_t s, uint64_t *launched);   // optional 5th stage: XXH64 of every frame's plaintext
 struct PipelineStreams { cudaStream_t main, side; cudaEvent_t fork, join; };
