@@ -496,6 +496,36 @@ const char *b200z_compress_stage_name(int stage);
 /* each kernel's device milliseconds in the last b200z_compress_frames_batch run with B200Z_FLAG_PROFILE set */
 int b200z_compress_last_profile(const b200z_ctx *ctx, float *stage_ms, size_t n);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Raw-content dictionary trainer -- EXTENSION in place of ruzstd::dictionary::create_raw_dict_from_source /
+ * create_raw_dict_from_dir (dictionary/mod.rs:76,127, feature dict_builder).  The reference cannot serve as the model: its
+ * reservoir sample reads the whole source to EOF (reservoir.rs:83-104), so its epoch loop (mod.rs:171-188) reads nothing and
+ * every source of 16 bytes or more gives an empty dictionary; pick_best_segment (cover.rs:71-95) also ignores its epoch.  This
+ * entry implements what the reference's comments describe, exactly (DESIGN.md section 4.5): the local-maximum-coverage
+ * method over 16-byte k-mers with every k-mer of the collection counted (2^22 hashed slots), epochs as compute_epoch_info with
+ * the collection's byte count, the best segment of every epoch scored by the distinct k-mers it holds (a k-mer that leaves its
+ * sample counts nothing), the counts of a chosen segment's k-mers zeroed for later epochs, and the segments concatenated by
+ * ascending score (ties by epoch), the last dict_size bytes kept.  n < 16 returns the input itself; dict_size == 0 returns
+ * nothing.  The result does not depend on the schedule.
+ * ---------------------------------------------------------------------------------------------------------- */
+typedef struct b200z_dict_segment {
+    uint64_t src_off;   /* the segment's first byte in `samples`                                  */
+    uint64_t score;     /* sum of the counts of its distinct k-mers when it was chosen            */
+    uint32_t epoch;
+    uint32_t size;      /* bytes: min(segment_size, samples_len, the epoch's length)              */
+} b200z_dict_segment;
+
+/* Trains on `samples` (host or device memory, B200Z_MEM_*), cut into nsamples samples of sample_sizes[] bytes (NULL: one
+ * sample; nsamples is then ignored), and writes the dictionary to the host buffer `dict` (*dict_len bytes) and, when `segments`
+ * is not NULL, one record per epoch in epoch order (*nsegments).  segment_size 0 means 2048, the reference's default.  Checked
+ * before any launch, B200Z_ERR_INVALID_ARGUMENT: segment_size outside [16, 65536], sample sizes that do not sum to samples_len,
+ * samples_len >= 2^32, dict_cap below what will be written (samples_len when it is below 16, else min(dict_size, the sum of the
+ * epochs' segment sizes)), or segments_cap below the number of epochs.  Kernels: k_dtcount, k_dtprev, then one k_dtepoch per
+ * epoch, all on the ctx stream and counted in b200z_ctx_kernel_launches. */
+int b200z_dict_train_raw(b200z_ctx *ctx, const uint8_t *samples, size_t samples_len, int samples_mem, const size_t *sample_sizes,
+                         size_t nsamples, size_t dict_size, size_t segment_size, uint8_t *dict, size_t dict_cap, size_t *dict_len,
+                         b200z_dict_segment *segments, size_t segments_cap, size_t *nsegments);
+
 /* XXH64(seed 0) of a host buffer -- the content-checksum hash the reference feeds on drain
  * (decode_buffer.rs:42,225,290,301); exposed so bindings can verify checksums like tests/decode_corpus.rs:61-74 */
 uint64_t b200z_xxh64(const uint8_t *data, size_t len);

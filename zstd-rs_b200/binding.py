@@ -57,6 +57,7 @@ ALL_RESULT_DTYPE = np.dtype([("written", "<u8"), ("frames", "<u8"), ("skippable_
 COMPRESS_IO_DTYPE = np.dtype([("src_off", "<u8"), ("src_size", "<u8"), ("dst_off", "<u8"), ("dst_cap", "<u8")])
 COMPRESS_RESULT_DTYPE = np.dtype([("dst_size", "<u8"), ("status", "<i4"), ("blocks", "<u4"), ("raw_blocks", "<u4"), ("rle_blocks", "<u4"),
                                   ("has_checksum", "<u4"), ("checksum", "<u4")])
+DICT_SEGMENT_DTYPE = np.dtype([("src_off", "<u8"), ("score", "<u8"), ("epoch", "<u4"), ("size", "<u4")])
 assert FRAME_IO_DTYPE.itemsize == C.sizeof(FrameIO) and FRAME_RESULT_DTYPE.itemsize == C.sizeof(FrameResult)
 
 
@@ -162,6 +163,7 @@ def lib():
         "b200z_compress_num_stages": (C.c_int, []),
         "b200z_compress_stage_name": (C.c_char_p, [C.c_int]),
         "b200z_compress_last_profile": (C.c_int, [vp, C.POINTER(C.c_float), sz]),
+        "b200z_dict_train_raw": (C.c_int, [vp, vp, sz, C.c_int, vp, sz, sz, sz, vp, sz, C.POINTER(sz), vp, sz, C.POINTER(sz)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)          # AttributeError here == a symbol the header declares is not exported
@@ -500,6 +502,59 @@ def compress_profile(ctx):
     ms = (C.c_float * n)()
     ctx._chk(L.b200z_compress_last_profile(ctx.h, ms, n))
     return {L.b200z_compress_stage_name(i).decode(): ms[i] for i in range(n)}
+
+
+def raw_dict_bounds(n, dict_size):
+    """(dictionary bytes, segment records) that always hold what b200z_dict_train_raw writes for n sample bytes: n itself below
+    16 bytes, else min(dict_size, n), because the segments lie in disjoint epochs; and max(1, n // 10000) records, because every
+    epoch but a lone one is at least 10,000 bytes long (tests/test_dict_train_model.py checks both against the epoch rule)."""
+    return (n if n < 16 else min(dict_size, n)), max(1, n // 10000)
+
+
+def create_raw_dict(ctx, samples, dict_size, sample_sizes=None, segment_size=2048, segments=False):
+    """b200z_dict_train_raw: a raw-content dictionary of at most `dict_size` bytes trained on the GPU (an extension in place of
+    ruzstd::dictionary; DESIGN.md section 4.5).  samples: bytes, numpy or torch (host or cuda), cut into samples by
+    `sample_sizes` (None: one sample), or a list of bytes-likes, one sample each.  Returns the dictionary as bytes, or (bytes,
+    DICT_SEGMENT_DTYPE rows in epoch order) with segments=True."""
+    if isinstance(samples, (list, tuple)):
+        parts = [bytes(x) for x in samples]
+        if sample_sizes is None:
+            sample_sizes = [len(x) for x in parts]
+        samples = b"".join(parts)
+    ip, n, _k = _ptr(samples)
+    sizes = None if sample_sizes is None else np.ascontiguousarray(sample_sizes, dtype=np.uint64)
+    cap, nseg_cap = raw_dict_bounds(n, dict_size)
+    out = np.zeros(max(cap, 1), dtype=np.uint8)
+    segs = np.zeros(nseg_cap, dtype=DICT_SEGMENT_DTYPE)
+    dlen, nseg = C.c_size_t(), C.c_size_t()
+    ctx._chk(ctx.L.b200z_dict_train_raw(ctx.h, ip, n, MEM_DEVICE if _is_device(samples) else MEM_HOST,
+                                        None if sizes is None else sizes.ctypes.data, 0 if sizes is None else len(sizes), dict_size,
+                                        segment_size, out.ctypes.data, cap, C.byref(dlen), segs.ctypes.data if segments else None,
+                                        len(segs), C.byref(nseg)))
+    d = out[:dlen.value].tobytes()
+    return (d, segs[:nseg.value].copy()) if segments else d
+
+
+def create_raw_dict_from_source(ctx, source, source_size, output, dict_size):
+    """ruzstd::dictionary::create_raw_dict_from_source (dictionary/mod.rs:127): reads `source` (a reader or bytes) to its end and
+    writes a raw-content dictionary of at most `dict_size` bytes to `output` (anything with write()).  The training runs on the
+    bytes read, so `source_size`, the reference's estimate of them, is not used."""
+    data = bytes(source) if isinstance(source, (bytes, bytearray, memoryview)) else source.read()
+    output.write(create_raw_dict(ctx, data, dict_size))
+
+
+def create_raw_dict_from_dir(ctx, path, output, dict_size):
+    """ruzstd::dictionary::create_raw_dict_from_dir (dictionary/mod.rs:76): every file under `path`, subdirectories included, is
+    one sample.  Deviation: the files are taken in sorted path order, where the reference chains them in read_dir order (which
+    the file system decides), so the dictionary does not depend on the file system."""
+    files = []
+    for dirpath, _, names in os.walk(path):
+        files += [os.path.join(dirpath, f) for f in names]
+    parts = []
+    for f in sorted(files):
+        with open(f, "rb") as fh:
+            parts.append(fh.read())
+    output.write(create_raw_dict(ctx, parts, dict_size))
 
 
 class Batch:

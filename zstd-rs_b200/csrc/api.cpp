@@ -14,6 +14,7 @@
 
 #include "../../include/b200zstd.h"
 #include "compress.h"
+#include "dict_train.h"
 #include "kernels.h"
 #include "plan.h"
 #include "tables.cuh"
@@ -84,6 +85,7 @@ struct b200z_ctx {
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     struct PipeResources *pipe = nullptr;  // lazily created by the pipelined one-shot path
     struct CompressResources *comp = nullptr;   // lazily created by the first compression
+    struct DictTrainResources *dtrain = nullptr;   // lazily created by the first dictionary training
     FseSlot *d_predef = nullptr;
     std::string err;
     uint64_t launches = 0;
@@ -128,11 +130,13 @@ extern "C" int b200z_ctx_create(int device, b200z_ctx **out) {
 }
 static void pipe_free(b200z_ctx *c);
 static void compress_free(b200z_ctx *c);
+static void dtrain_free(b200z_ctx *c);
 extern "C" void b200z_ctx_destroy(b200z_ctx *c) {
     if (!c) return;
     cudaSetDevice(c->device);
     pipe_free(c);
     compress_free(c);
+    dtrain_free(c);
     if (c->d_predef) cudaFree(c->d_predef);
     if (c->ev_fork) cudaEventDestroy(c->ev_fork);
     if (c->ev_join) cudaEventDestroy(c->ev_join);
@@ -2067,5 +2071,138 @@ extern "C" int b200z_compress_frames_batch_dict(b200z_ctx *c, const uint8_t *inp
     r.profiled = prof;
     if (prof)
         for (int st = 0; st < kCompressStages; st++) CU(c, cudaEventElapsedTime(&r.stage_ms[st], r.ev[st], r.ev[st + 1]));
+    return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// raw-content dictionary trainer (EXTENSION in place of ruzstd::dictionary, DESIGN.md section 4.5): host checks and the epoch
+// plan, then k_dtcount -> k_dtprev -> one k_dtepoch per epoch on the ctx stream; the chosen segments' bytes are then gathered
+// into the host dictionary by ascending score
+// ---------------------------------------------------------------------------------------------------------------
+struct DictTrainResources {
+    DevBuf input, starts, slots, dist, freq, best, done, segs;
+};
+static void dtrain_free(b200z_ctx *c) {
+    delete c->dtrain;
+    c->dtrain = nullptr;
+}
+
+struct DtEpoch { uint32_t e0, e1, le; };
+
+// compute_epoch_info (cover.rs:117-132) with the collection's n bytes in place of its k-mer count; the last epoch runs to n
+static std::vector<DtEpoch> dt_epochs(uint64_t n, uint64_t dict_size, uint64_t seg) {
+    const uint64_t L = std::min(seg, n);
+    uint64_t E = std::max<uint64_t>(1, dict_size / L), es = n / E;
+    if (es < 10000) {
+        es = std::min<uint64_t>(10000, n);
+        E = n / es;
+    }
+    std::vector<DtEpoch> out(E);
+    for (uint64_t e = 0; e < E; e++) {
+        const uint64_t e0 = e * es, e1 = e + 1 == E ? n : e0 + es;
+        out[e] = DtEpoch{(uint32_t)e0, (uint32_t)e1, (uint32_t)std::min(L, e1 - e0)};
+    }
+    return out;
+}
+
+extern "C" int b200z_dict_train_raw(b200z_ctx *c, const uint8_t *samples, size_t samples_len, int samples_mem, const size_t *sample_sizes,
+                                    size_t nsamples, size_t dict_size, size_t segment_size, uint8_t *dict, size_t dict_cap, size_t *dict_len,
+                                    b200z_dict_segment *segments, size_t segments_cap, size_t *nsegments) {
+    // ---- everything is checked before any device work
+    if (!c) return B200Z_ERR_INVALID_ARGUMENT;
+    auto reject = [c](const char *why) { c->err = why; return B200Z_ERR_INVALID_ARGUMENT; };
+    const size_t seg = segment_size ? segment_size : 2048;
+    if ((samples_len && !samples) || (samples_mem != B200Z_MEM_HOST && samples_mem != B200Z_MEM_DEVICE) || !dict_len) return reject("invalid argument");
+    if (seg < DT_K || seg > 65536) return reject("segment_size outside [16, 65536]");
+    if (samples_len >= (1ull << 32)) return reject("samples_len >= 2^32");
+    std::vector<uint32_t> starts;
+    if (sample_sizes) {
+        if (nsamples >= (1ull << 32)) return reject("more than 2^32 - 1 samples");
+        uint64_t sum = 0;
+        for (size_t i = 0; i < nsamples; i++) {
+            if (sample_sizes[i] > samples_len - sum) return reject("sample sizes do not sum to samples_len");
+            starts.push_back((uint32_t)sum);
+            sum += sample_sizes[i];
+        }
+        if (sum != samples_len) return reject("sample sizes do not sum to samples_len");
+    } else {
+        starts.push_back(0);
+    }
+    starts.push_back((uint32_t)samples_len);
+    const uint64_t n = samples_len;
+    std::vector<DtEpoch> ep;
+    uint64_t total = 0, need = n;
+    if (n >= DT_K) {
+        if (dict_size) ep = dt_epochs(n, dict_size, seg);
+        for (const DtEpoch &x : ep) total += x.le;
+        need = std::min<uint64_t>(dict_size, total);
+    }
+    if (dict_cap < need || (need && !dict)) return reject("dict_cap is smaller than the dictionary");
+    if (segments && segments_cap < ep.size()) return reject("segments_cap is smaller than the number of epochs");
+    *dict_len = 0;
+    if (nsegments) *nsegments = 0;
+    if (n < DT_K) {   // the reference's rule: a source this short is its own dictionary
+        if (n && samples_mem == B200Z_MEM_DEVICE) {
+            if (int e = c->use()) return e;
+            CU(c, cudaMemcpy(dict, samples, n, cudaMemcpyDeviceToHost));
+        } else if (n) {
+            memcpy(dict, samples, n);
+        }
+        *dict_len = n;
+        return 0;
+    }
+    if (ep.empty()) return 0;
+    if (int e = c->use()) return e;
+    // ---- device passes
+    if (!c->dtrain) c->dtrain = new DictTrainResources();
+    DictTrainResources &r = *c->dtrain;
+    const uint32_t E = (uint32_t)ep.size(), ns = (uint32_t)(starts.size() - 1);
+    int e = 0;
+    if ((e = r.starts.ensure(starts.size() * 4)) || (e = r.slots.ensure(n * 4)) || (e = r.dist.ensure(n * 2)) ||
+        (e = r.freq.ensure(sizeof(uint32_t) << DT_F)) || (e = r.best.ensure((size_t)E * 8)) || (e = r.done.ensure((size_t)E * 4)) ||
+        (e = r.segs.ensure((size_t)E * sizeof(b200z_dict_segment))))
+        return e;
+    cudaStream_t s = c->stream;
+    const uint8_t *d_in = samples;
+    if (samples_mem == B200Z_MEM_HOST) {
+        if ((e = r.input.ensure(n + 16))) return e;
+        CU(c, cudaMemcpyAsync(r.input.p, samples, n, cudaMemcpyHostToDevice, s));
+        d_in = r.input.as<uint8_t>();
+    }
+    CU(c, cudaMemcpyAsync(r.starts.p, starts.data(), starts.size() * 4, cudaMemcpyHostToDevice, s));
+    CU(c, cudaMemsetAsync(r.freq.p, 0, sizeof(uint32_t) << DT_F, s));
+    CU(c, cudaMemsetAsync(r.best.p, 0, (size_t)E * 8, s));
+    CU(c, cudaMemsetAsync(r.done.p, 0, (size_t)E * 4, s));
+    uint32_t *slots = r.slots.as<uint32_t>(), *freq = r.freq.as<uint32_t>();
+    uint16_t *dist = r.dist.as<uint16_t>();
+    if (int le = launch_dt_count(d_in, (uint32_t)n, r.starts.as<uint32_t>(), ns, slots, freq, s, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_dtcount");
+    const uint32_t w = (uint32_t)std::min<uint64_t>(seg, n) - (DT_K - 1);
+    if (int le = launch_dt_prev(slots, (uint32_t)n, w, dist, s, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_dtprev");
+    for (uint32_t i = 0; i < E; i++)
+        if (int le = launch_dt_epoch(slots, dist, freq, i, ep[i].e0, ep[i].e1, ep[i].le, r.best.as<unsigned long long>() + i, r.done.as<uint32_t>() + i,
+                                     r.segs.as<b200z_dict_segment>() + i, s, &c->launches))
+            return c->set_cuda_err((cudaError_t)le, "k_dtepoch");
+    std::vector<b200z_dict_segment> hs(E);
+    CU(c, cudaMemcpyAsync(hs.data(), r.segs.p, (size_t)E * sizeof(b200z_dict_segment), cudaMemcpyDeviceToHost, s));
+    CU(c, cudaStreamSynchronize(s));
+    // ---- the dictionary: segments by ascending score (ties by epoch), the highest score last, nearest the data; the last `need`
+    // bytes of their concatenation
+    std::vector<uint32_t> order(E);
+    for (uint32_t i = 0; i < E; i++) order[i] = i;
+    std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return hs[a].score < hs[b].score; });
+    uint64_t skip = total - need, at = 0;
+    for (uint32_t i : order) {
+        const b200z_dict_segment &g = hs[i];
+        const uint64_t drop = std::min<uint64_t>(skip, g.size), len = g.size - drop;
+        skip -= drop;
+        if (!len) continue;
+        if (samples_mem == B200Z_MEM_HOST) memcpy(dict + at, samples + g.src_off + drop, len);
+        else CU(c, cudaMemcpyAsync(dict + at, samples + g.src_off + drop, len, cudaMemcpyDeviceToHost, s));
+        at += len;
+    }
+    if (samples_mem == B200Z_MEM_DEVICE) CU(c, cudaStreamSynchronize(s));
+    *dict_len = at;
+    if (segments) memcpy(segments, hs.data(), (size_t)E * sizeof(b200z_dict_segment));
+    if (nsegments) *nsegments = E;
     return 0;
 }
