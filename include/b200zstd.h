@@ -467,6 +467,13 @@ typedef struct b200z_compress_result {
 /* context flag: b200z_compress_frames_batch records a CUDA event between its kernels and keeps each kernel's milliseconds
  * for b200z_compress_last_profile (profiling aid for bench.py; it synchronises anyway) */
 #define B200Z_FLAG_PROFILE 2u
+/* context flag: b200z_compress_frames_batch_dict with a formatted dictionary uses the dictionary's entropy tables in every frame's
+ * first block: Treeless literals with its Huffman codes and Repeat for each of the LL / OF / ML tables, each only where it is
+ * smaller (estimated, for the sequence tables) than the block's own tables.  Later blocks keep their own tables, so no block
+ * depends on another's encoding.  Without the flag, or with a raw-content dictionary, the output is what it is without it.  The
+ * encoder's view of the tables is built on the host by the dictionary's first use with the flag (no kernel launch) and kept
+ * until b200z_dict_destroy. */
+#define B200Z_FLAG_DICT_TABLES 4u
 
 /* the largest frame b200z_compress_frames_batch can write for src_size bytes: src_size + 14 + 3 * max(1, ceil(src_size / 131072)) + 4 */
 size_t b200z_compress_bound(size_t src_size);
@@ -481,8 +488,8 @@ int b200z_compress_frames_batch(b200z_ctx *ctx, const uint8_t *input, size_t inp
  * dictionary per submission.  The first 128 KiB of every frame may also match the last 128 KiB of the dictionary's content
  * (offsets stay within the 128 KiB window); the content checksum covers the frame's own plaintext.  A formatted dictionary's ID
  * goes into every frame header in the smallest field that holds it; a raw-content dictionary writes no ID (libzstd's
- * convention), so such frames are decoded with it forced (`forced_dict`, force_dict).  The encoder does not use a formatted
- * dictionary's entropy tables or repeat offsets.  The dictionary's match table is built on the ctx stream by its first use here
+ * convention), so such frames are decoded with it forced (`forced_dict`, force_dict).  The encoder uses a formatted dictionary's
+ * entropy tables only with B200Z_FLAG_DICT_TABLES, and never its repeat offsets.  The dictionary's match table is built on the ctx stream by its first use here
  * (one more kernel launch) and kept until b200z_dict_destroy.  dict == NULL writes exactly what b200z_compress_frames_batch
  * writes.  Besides that entry's checks: B200Z_ERR_INVALID_ARGUMENT for a dictionary created on another ctx and for
  * dst_cap < b200z_compress_bound_dict(src_size, dict), before any launch. */
@@ -525,6 +532,37 @@ typedef struct b200z_dict_segment {
 int b200z_dict_train_raw(b200z_ctx *ctx, const uint8_t *samples, size_t samples_len, int samples_mem, const size_t *sample_sizes,
                          size_t nsamples, size_t dict_size, size_t segment_size, uint8_t *dict, size_t dict_cap, size_t *dict_len,
                          b200z_dict_segment *segments, size_t segments_cap, size_t *nsegments);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * Dictionary finalizer -- EXTENSION, the counterpart of libzstd's ZDICT_finalizeDictionary (ruzstd has none): turns dictionary
+ * content (for instance b200z_dict_train_raw's) into a zstd-format dictionary that carries an ID and entropy tables, which
+ * Dictionary::decode_dict (b200z_dict_create), ruzstd and libzstd load.  The statistics come from the GPU: the first block (at
+ * most 128 KiB) of every sample is parsed against the content by the compressor's own parse (k_cmatch, with the content's match
+ * table from k_cdict), and k_dstats counts the literal bytes and the LL / ML / OF codes of every block that is not RLE (u64
+ * totals, integer atomics: the result does not depend on the schedule).  The samples go through in submissions of a bounded
+ * number of blocks.  On the host, every symbol gets a count of at least 1 (literals 0-255, LL 0-35, ML 0-52, OF 0 up to
+ * floor(log2(content_len + 131072))), and the tables are written at accuracy logs OF 8, ML 9, LL 9 with Huffman codes of at
+ * most 11 bits.  Layout: magic 0xEC30A437, ID, Huffman description, OF, ML, LL descriptions, repeat offsets 1, 4, 8, content.
+ * When the header and the content exceed dict_cap, the content's LAST bytes are kept (the trainer puts its best segments
+ * last).  dict_id 0 derives the ID as libzstd does: (XXH64(content written, seed 0) mod (2^31 - 32768)) + 32768.
+ * ---------------------------------------------------------------------------------------------------------- */
+/* an upper bound on the header (everything before the content) b200z_dict_finalize writes */
+#define B200Z_DICT_HEADER_MAX 328
+/* Finalizes `content` (host memory) on `samples` (host or device memory, B200Z_MEM_*) cut into nsamples samples of
+ * sample_sizes[] bytes; nsamples == 0 is legal and gives the tables of flat counts.  Writes the dictionary to the host buffer
+ * `dict` (*dict_len bytes).  Checked before any launch, B200Z_ERR_INVALID_ARGUMENT: content_len below 8 or >= 2^31, dict_cap below
+ * B200Z_DICT_HEADER_MAX + 8, sample sizes that do not sum to samples_len, dict_id >= 2^31 (the format reserves those IDs; libzstd
+ * and ruzstd accept them, so this library does not write them).  Kernels: k_cdict once, then k_cmatch and k_dstats per
+ * submission, all on the ctx stream and counted in b200z_ctx_kernel_launches.  Device memory: the compressor's per-block staging
+ * for min(nsamples, 2048) blocks (about 0.9 MB per block whatever the samples' sizes, so up to about 1.8 GB), a copy of host samples,
+ * and 0.5 MB for the content's match table; all of it stays with the ctx (reused by later compressions) until b200z_ctx_destroy. */
+int b200z_dict_finalize(b200z_ctx *ctx, const uint8_t *content, size_t content_len,
+                        const uint8_t *samples, size_t samples_len, int samples_mem, const size_t *sample_sizes, size_t nsamples,
+                        uint32_t dict_id, uint8_t *dict, size_t dict_cap, size_t *dict_len);
+/* Host only: what b200z_dict_finalize writes for the statistics counts[377] (literal bytes 0-255, LL codes 0-35, ML codes 0-52,
+ * OF codes 0-31, in that order), with the same argument checks */
+int b200z_debug_dict_from_counts(const uint64_t counts[377], const uint8_t *content, size_t content_len, uint32_t dict_id,
+                                 uint8_t *dict, size_t dict_cap, size_t *dict_len);
 
 /* XXH64(seed 0) of a host buffer -- the content-checksum hash the reference feeds on drain
  * (decode_buffer.rs:42,225,290,301); exposed so bindings can verify checksums like tests/decode_corpus.rs:61-74 */

@@ -1,6 +1,7 @@
 """zstd-rs_b200 -- GPU-native (H100, sm_90a) zstd block decompressor behind ruzstd's FrameDecoder / StreamingDecoder API,
 a batch compressor at ruzstd's Uncompressed and Fastest levels (compress_frames / compress_to_vec), and a raw-content
-dictionary trainer in place of ruzstd::dictionary (create_raw_dict, create_raw_dict_from_source, create_raw_dict_from_dir).
+dictionary trainer in place of ruzstd::dictionary (create_raw_dict, create_raw_dict_from_source, create_raw_dict_from_dir)
+and a finalizer that turns its content into a zstd-format dictionary (finalize_dict, create_dict).
 
 The product is the C-ABI library ``libb200zstd.so`` (include/b200zstd.h, sources in csrc/).  This package is the
 Python host-side mirror of the reference interface (same names, argument meaning and error behaviour as
@@ -11,8 +12,8 @@ Import name: ``zstd_rs_b200`` (the directory name has a hyphen; see ``_pkg.py`` 
 """
 from .binding import (  # noqa: F401
     ALL, FASTEST, UNCOMPRESSED, UPTO_BLOCKS, UPTO_BYTES, AllBatch, B200ZError, Batch, Context, Dictionary, FrameDecoder, StreamingDecoder,
-    build, compress_bound, compress_frames, compress_profile, compress_to_vec, create_raw_dict, create_raw_dict_from_dir,
+    build, compress_bound, compress_frames, compress_profile, compress_to_vec, create_dict, create_raw_dict, create_raw_dict_from_dir,
     create_raw_dict_from_source, decode_all, decode_all_batch, decode_blocks, decode_frames,
-    error_names, lib, lib_path, xxh64,
+    dict_from_counts, error_names, finalize_dict, lib, lib_path, xxh64,
 )
 from . import binding  # noqa: F401

@@ -26,6 +26,7 @@ MEM_HOST, MEM_DEVICE = 0, 1
 ERR_SKIP_FRAME = 8
 FLAG_CHECKSUM = 1
 FLAG_PROFILE = 2
+FLAG_DICT_TABLES = 4
 HUF_DEBUG_BYTES, FSE_DEBUG_BYTES = 3088, 1040   # B200Z_DEBUG_HUF_BYTES / B200Z_DEBUG_FSE_BYTES: one raw huff0 / FSE table
 UNCOMPRESSED, FASTEST = 0, 1   # CompressionLevel (ruzstd encoding/mod.rs:24-67); Default / Better / Best are not implemented there
 
@@ -164,6 +165,8 @@ def lib():
         "b200z_compress_stage_name": (C.c_char_p, [C.c_int]),
         "b200z_compress_last_profile": (C.c_int, [vp, C.POINTER(C.c_float), sz]),
         "b200z_dict_train_raw": (C.c_int, [vp, vp, sz, C.c_int, vp, sz, sz, sz, vp, sz, C.POINTER(sz), vp, sz, C.POINTER(sz)]),
+        "b200z_dict_finalize": (C.c_int, [vp, vp, sz, vp, sz, C.c_int, vp, sz, C.c_uint32, vp, sz, C.POINTER(sz)]),
+        "b200z_debug_dict_from_counts": (C.c_int, [vp, vp, sz, C.c_uint32, vp, sz, C.POINTER(sz)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)          # AttributeError here == a symbol the header declares is not exported
@@ -470,28 +473,36 @@ def compress_bound(n, dict=None):
     return lib().b200z_compress_bound(n) if dict is None else lib().b200z_compress_bound_dict(n, dict.h)
 
 
-def compress_frames(ctx, input, io, output, level=FASTEST, checksum=True, dict=None):
+def compress_frames(ctx, input, io, output, level=FASTEST, checksum=True, dict=None, dict_tables=False):
     """b200z_compress_frames_batch_dict: one zstd frame per COMPRESS_IO_DTYPE row (src_off, src_size, dst_off, dst_cap), every block
-    of every frame compressed at once, against `dict` (a Dictionary of this context) when given.  input/output: bytes, numpy or
-    torch (host or cuda).  Returns COMPRESS_RESULT_DTYPE rows."""
+    of every frame compressed at once, against `dict` (a Dictionary of this context) when given.  dict_tables=True sets
+    FLAG_DICT_TABLES for the call: a formatted dictionary's entropy tables may then code each frame's first block.  input/output:
+    bytes, numpy or torch (host or cuda).  Returns COMPRESS_RESULT_DTYPE rows."""
     fr = np.ascontiguousarray(io, dtype=COMPRESS_IO_DTYPE)
     res = np.zeros(len(fr), dtype=COMPRESS_RESULT_DTYPE)
     ip, il, _k1 = _ptr(input)
     op, ol, _k2 = _ptr(output)
-    e = ctx.L.b200z_compress_frames_batch_dict(ctx.h, ip, il, MEM_DEVICE if _is_device(input) else MEM_HOST, fr.ctypes.data, len(fr), level,
-                                               1 if checksum else 0, dict.h if dict is not None else None, op, ol,
-                                               MEM_DEVICE if _is_device(output) else MEM_HOST, res.ctypes.data)
+    flags = ctx.L.b200z_ctx_flags(ctx.h)
+    if dict_tables:
+        ctx.L.b200z_ctx_set_flags(ctx.h, flags | FLAG_DICT_TABLES)
+    try:
+        e = ctx.L.b200z_compress_frames_batch_dict(ctx.h, ip, il, MEM_DEVICE if _is_device(input) else MEM_HOST, fr.ctypes.data, len(fr),
+                                                   level, 1 if checksum else 0, dict.h if dict is not None else None, op, ol,
+                                                   MEM_DEVICE if _is_device(output) else MEM_HOST, res.ctypes.data)
+    finally:
+        ctx.L.b200z_ctx_set_flags(ctx.h, flags)
     ctx._chk(e)
     return res
 
 
-def compress_to_vec(ctx, data, level=FASTEST, checksum=True, dict=None):
-    """Mirror of ruzstd::encoding::compress_to_vec (encoding/mod.rs): one frame holding `data`, as bytes (against `dict` when given)."""
+def compress_to_vec(ctx, data, level=FASTEST, checksum=True, dict=None, dict_tables=False):
+    """Mirror of ruzstd::encoding::compress_to_vec (encoding/mod.rs): one frame holding `data`, as bytes (against `dict` when given,
+    with its entropy tables when dict_tables=True)."""
     src = bytes(data)
     cap = compress_bound(len(src), dict)
     out = np.zeros(cap, dtype=np.uint8)
     io = np.array([(0, len(src), 0, cap)], dtype=COMPRESS_IO_DTYPE)
-    res = compress_frames(ctx, src, io, out, level, checksum, dict)
+    res = compress_frames(ctx, src, io, out, level, checksum, dict, dict_tables)
     return out[:int(res[0]["dst_size"])].tobytes()
 
 
@@ -555,6 +566,61 @@ def create_raw_dict_from_dir(ctx, path, output, dict_size):
         with open(f, "rb") as fh:
             parts.append(fh.read())
     output.write(create_raw_dict(ctx, parts, dict_size))
+
+
+DICT_HEADER_MAX = 328   # B200Z_DICT_HEADER_MAX: an upper bound on a finalized dictionary's header
+
+
+def _samples_arg(samples, sample_sizes):
+    """(samples buffer, sample sizes as u64 or None): a list of bytes-likes is one sample each; a buffer without sizes is one sample."""
+    if isinstance(samples, (list, tuple)):
+        parts = [bytes(x) for x in samples]
+        if sample_sizes is None:
+            sample_sizes = [len(x) for x in parts]
+        samples = b"".join(parts)
+    return samples, None if sample_sizes is None else np.ascontiguousarray(sample_sizes, dtype=np.uint64)
+
+
+def finalize_dict(ctx, content, samples, sample_sizes=None, dict_id=0, dict_cap=None):
+    """b200z_dict_finalize: `content` (bytes) as a zstd-format dictionary whose entropy tables come from the statistics of
+    `samples` on the GPU (an extension, the counterpart of ZDICT_finalizeDictionary; DESIGN.md section 4.6).  samples: bytes,
+    numpy or torch (host or cuda), cut by `sample_sizes` (None: one sample), or a list of bytes-likes, one sample each; an empty
+    list gives the tables of flat counts.  dict_id 0 derives libzstd's ID from the content.  dict_cap: the largest dictionary
+    wanted (None: room for all of the content); the content's last bytes are kept when it does not fit.  Returns bytes."""
+    c = bytes(content)
+    samples, sizes = _samples_arg(samples, sample_sizes)
+    ip, n, _k = _ptr(samples)
+    if sizes is None:
+        sizes = np.array([n], dtype=np.uint64)
+    cap = DICT_HEADER_MAX + len(c) if dict_cap is None else dict_cap
+    out = np.zeros(max(cap, 1), dtype=np.uint8)
+    dlen = C.c_size_t()
+    ctx._chk(ctx.L.b200z_dict_finalize(ctx.h, c, len(c), ip, n, MEM_DEVICE if _is_device(samples) else MEM_HOST, sizes.ctypes.data, len(sizes),
+                                       dict_id, out.ctypes.data, cap, C.byref(dlen)))
+    return out[:dlen.value].tobytes()
+
+
+def create_dict(ctx, samples, dict_size, sample_sizes=None, segment_size=2048, dict_id=0):
+    """A zstd-format dictionary of at most `dict_size` bytes: create_raw_dict's content, finalized on the same samples
+    (finalize_dict), its first bytes giving way to the header."""
+    samples, sizes = _samples_arg(samples, sample_sizes)
+    content = create_raw_dict(ctx, samples, dict_size, sample_sizes=sizes, segment_size=segment_size)
+    return finalize_dict(ctx, content, samples, sizes, dict_id=dict_id, dict_cap=dict_size)
+
+
+def dict_from_counts(counts, content, dict_id=0, dict_cap=None):
+    """Host-only: what finalize_dict writes for the statistics counts[377] (literal bytes, LL, ML, OF codes) -- dict_from_counts,
+    csrc/dict_format.cpp."""
+    cnt = np.ascontiguousarray(counts, dtype=np.uint64)
+    assert cnt.shape == (377,)
+    c = bytes(content)
+    cap = DICT_HEADER_MAX + len(c) if dict_cap is None else dict_cap
+    out = np.zeros(max(cap, 1), dtype=np.uint8)
+    dlen = C.c_size_t()
+    rc = lib().b200z_debug_dict_from_counts(cnt.ctypes.data, c, len(c), dict_id, out.ctypes.data, cap, C.byref(dlen))
+    if rc:
+        raise B200ZError(rc, 0, "b200z_debug_dict_from_counts")
+    return out[:dlen.value].tobytes()
 
 
 class Batch:

@@ -164,6 +164,13 @@ struct b200z_dict {
     uint8_t *d_content = nullptr;
     size_t content_len = 0;
     uint32_t *d_ctab = nullptr;   // the compressor's match table of the content (k_cdict), built by its first compression
+    // a formatted dictionary's tables as parsed (Huffman weights; OF / ML / LL normalized counts by ENC_LL / ENC_OF / ENC_ML), and
+    // the encoder's view of them, built on the host by the first compression with B200Z_FLAG_DICT_TABLES
+    uint8_t huf_weights[260] = {};
+    uint32_t huf_nweights = 0;
+    int16_t norm[3][64] = {};
+    uint32_t nnorm[3] = {}, log[3] = {};
+    EncDict *d_enc = nullptr;
 };
 
 static void dict_free(b200z_dict *d) {
@@ -173,6 +180,7 @@ static void dict_free(b200z_dict *d) {
     if (d->d_fse) cudaFree(d->d_fse);
     if (d->d_content) cudaFree(d->d_content);
     if (d->d_ctab) cudaFree(d->d_ctab);
+    if (d->d_enc) cudaFree(d->d_enc);
     delete d;
 }
 
@@ -185,7 +193,8 @@ static int dict_upload_content(b200z_dict *d, const uint8_t *content, size_t len
 }
 
 // Dictionary::decode_dict (dictionary.rs:45-126).  The table descriptions are parsed and expanded with the same
-// code the GPU runs per block (tables.cuh, compiled for the host here) and uploaded once.
+// code the GPU runs per block (tables.cuh, compiled for the host here) and uploaded once.  The parsed weights and normalized
+// counts are kept for the encoder (B200Z_FLAG_DICT_TABLES): each description is read once, then expanded for the decoder.
 extern "C" int b200z_dict_create(b200z_ctx *c, const uint8_t *raw, size_t len, b200z_dict **out) {
     if (!c || !out || (!raw && len)) return B200Z_ERR_INVALID_ARGUMENT;
     *out = nullptr;
@@ -202,15 +211,26 @@ extern "C" int b200z_dict_create(b200z_ctx *c, const uint8_t *raw, size_t len, b
     std::unique_ptr<FseSlot> fse(new FseSlot());
     memset(huf.get(), 0, sizeof(HufSlot));
     memset(fse.get(), 0, sizeof(FseSlot));
-    uint32_t used = 0;
-    int e = huf_build_decoder(t, (uint32_t)std::min<size_t>(tl, 0x7fffffff), huf.get(), used);
-    if (e) return e;
+    uint32_t used = 0, mb = 0;
+    // huf_build_decoder's two steps (tables.cuh)
+    int e = huf_read_weights(t, (uint32_t)std::min<size_t>(tl, 0x7fffffff), d->huf_weights, d->huf_nweights, used);
+    if (e || (e = huf_build_table(d->huf_weights, d->huf_nweights, huf.get(), mb))) return e;
+    huf->max_bits = mb;
     if (tl < used) return B200Z_ERR_DICT_NOT_ENOUGH_BYTES;
     t += used; tl -= used;
-    struct { FseTab *tab; uint32_t max_log, max_sym; } order[3] = {{&fse->of, 8, 31}, {&fse->ml, 9, 52}, {&fse->ll, 9, 35}};  // OF, ML, LL
-    for (auto &o : order) {
-        e = fse_build_decoder(t, (uint32_t)std::min<size_t>(tl, 0x7fffffff), o.max_log, o.max_sym, o.tab, used);
+    struct { FseTab *tab; uint32_t max_log, max_sym, enc; } order[3] = {{&fse->of, 8, 31, ENC_OF}, {&fse->ml, 9, 52, ENC_ML}, {&fse->ll, 9, 35, ENC_LL}};
+    for (auto &o : order) {   // OF, ML, LL: fse_build_decoder's steps (tables.cuh)
+        int16_t probs[256];
+        uint32_t nprobs = 0, acc_log = 0;
+        e = fse_read_probabilities(t, (uint32_t)std::min<size_t>(tl, 0x7fffffff), o.max_log, o.max_sym, probs, nprobs, acc_log, used);
         if (e) return e;
+        std::vector<uint32_t> wide(FSE_MAX_ENTRIES);
+        uint16_t counter[256];
+        if ((e = fse_build_table(probs, nprobs, acc_log, o.max_sym, wide.data(), counter))) return e;
+        fse_compact(wide.data(), acc_log, o.tab);
+        memcpy(d->norm[o.enc], probs, nprobs * sizeof(int16_t));
+        d->nnorm[o.enc] = nprobs;
+        d->log[o.enc] = acc_log;
         if (tl < used) return B200Z_ERR_DICT_NOT_ENOUGH_BYTES;
         t += used; tl -= used;
     }
@@ -1938,6 +1958,7 @@ extern "C" const char *b200z_compress_stage_name(int stage) { return stage >= 0 
 
 struct CompressResources {
     DevBuf frames, blocks, lit_stage, seq_stage, lits, seqs, info, res, csum, results, input, output;
+    DevBuf dcontent, dtab, dcounts;   // b200z_dict_finalize: the content's tail, its match table and the statistics
     cudaEvent_t ev[kCompressStages + 1] = {};
     float stage_ms[kCompressStages] = {};
     bool profiled = false;
@@ -2049,8 +2070,18 @@ extern "C" int b200z_compress_frames_batch_dict(b200z_ctx *c, const uint8_t *inp
             return c->set_cuda_err((cudaError_t)le, "k_cdict");
         }
     }
+    // the encoder's view of a formatted dictionary's tables, built on the host once and kept with the dictionary (no launch)
+    const bool use_tables = fast && dict && dict->has_tables && (c->flags & B200Z_FLAG_DICT_TABLES);
+    if (use_tables && !md->d_enc) {
+        std::unique_ptr<EncDict> ed(new EncDict());
+        const int16_t *probs[3] = {md->norm[0], md->norm[1], md->norm[2]};
+        enc_dict_build(md->huf_weights, md->huf_nweights, probs, md->nnorm, md->log, *ed);
+        CU(c, cudaMalloc((void **)&md->d_enc, sizeof(EncDict)));
+        CU(c, cudaMemcpy(md->d_enc, ed.get(), sizeof(EncDict), cudaMemcpyHostToDevice));
+    }
     CompressArgs a{};
     a.frames = r.frames.as<CFrame>(); a.blocks = r.blocks.as<CBlock>(); a.input = d_in; a.output = d_out;
+    a.etab = use_tables ? dict->d_enc : nullptr;
     a.lit_stage = r.lit_stage.as<uint8_t>(); a.seq_stage = r.seq_stage.as<SeqRec>(); a.lits = r.lits.as<uint8_t>(); a.seqs = r.seqs.as<SeqRec>();
     a.enc = a.lit_stage; a.info = r.info.as<CBlockInfo>(); a.res = r.res.as<CBlockInfo>(); a.csum = r.csum.as<uint64_t>();
     a.results = r.results.as<b200z_compress_result>(); a.nframes = (uint32_t)nframes; a.nblocks = (uint32_t)nblocks; a.level = level;
@@ -2205,4 +2236,78 @@ extern "C" int b200z_dict_train_raw(b200z_ctx *c, const uint8_t *samples, size_t
     if (segments) memcpy(segments, hs.data(), (size_t)E * sizeof(b200z_dict_segment));
     if (nsegments) *nsegments = E;
     return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// dictionary finalizer (EXTENSION, ZDICT_finalizeDictionary's counterpart, DESIGN.md section 4.6): host checks, then k_cdict on the
+// content's tail and, per submission of at most DS_BLOCKS samples, k_cmatch<true> -> k_dstats on the compressor's staging; the
+// counts come back and dict_from_counts (dict_format.cpp) writes the dictionary
+// ---------------------------------------------------------------------------------------------------------------
+extern "C" int b200z_debug_dict_from_counts(const uint64_t counts[377], const uint8_t *content, size_t content_len, uint32_t dict_id,
+                                            uint8_t *dict, size_t dict_cap, size_t *dict_len) {
+    return dict_from_counts(counts, content, content_len, dict_id, dict, dict_cap, dict_len);
+}
+
+extern "C" int b200z_dict_finalize(b200z_ctx *c, const uint8_t *content, size_t content_len, const uint8_t *samples, size_t samples_len,
+                                   int samples_mem, const size_t *sample_sizes, size_t nsamples, uint32_t dict_id, uint8_t *dict,
+                                   size_t dict_cap, size_t *dict_len) {
+    // ---- everything is checked before any device work
+    if (!c) return B200Z_ERR_INVALID_ARGUMENT;
+    auto reject = [c](const char *why) { c->err = why; return B200Z_ERR_INVALID_ARGUMENT; };
+    if (!content || (samples_len && !samples) || (nsamples && !sample_sizes) || (samples_mem != B200Z_MEM_HOST && samples_mem != B200Z_MEM_DEVICE) ||
+        !dict || !dict_len)
+        return reject("invalid argument");
+    if (dict_check_args(content_len, dict_id, dict_cap))
+        return reject("content_len outside [8, 2^31), dict_id >= 2^31 or dict_cap < B200Z_DICT_HEADER_MAX + 8");
+    if (nsamples > 0xffffffffu) return reject("more than 2^32 - 1 samples");
+    std::vector<CBlock> hb(nsamples);
+    uint64_t sum = 0;
+    for (size_t i = 0; i < nsamples; i++) {
+        if (sample_sizes[i] > samples_len - sum) return reject("sample sizes do not sum to samples_len");
+        hb[i] = CBlock{sum, (uint32_t)std::min<size_t>(sample_sizes[i], ENC_BLOCK), 0, (uint32_t)i, 0};
+        sum += sample_sizes[i];
+    }
+    if (sum != samples_len) return reject("sample sizes do not sum to samples_len");
+    std::vector<uint64_t> counts(DS_BINS, 0);
+    if (nsamples) {
+        if (int e = c->use()) return e;
+        if (!c->comp) {
+            c->comp = new CompressResources();
+            for (cudaEvent_t &e : c->comp->ev) CU(c, cudaEventCreate(&e));
+        }
+        CompressResources &r = *c->comp;
+        const uint64_t per = std::min<uint64_t>(nsamples, DS_BLOCKS);
+        const uint32_t tail = (uint32_t)std::min<size_t>(content_len, ENC_WINDOW);   // all a match can reach
+        int e = 0;
+        if ((e = r.blocks.ensure(nsamples * sizeof(CBlock))) || (e = r.lit_stage.ensure(per * ENC_BLOCK)) ||
+            (e = r.seq_stage.ensure(per * CBLOCK_SEQS * sizeof(SeqRec))) || (e = r.lits.ensure(per * ENC_BLOCK)) ||
+            (e = r.seqs.ensure(per * CBLOCK_SEQS * sizeof(SeqRec))) || (e = r.info.ensure(per * sizeof(CBlockInfo))) ||
+            (e = r.dcontent.ensure(tail + 16)) || (e = r.dtab.ensure(sizeof(uint32_t) << CD_LOG)) || (e = r.dcounts.ensure(DS_BINS * 8)))
+            return e;
+        cudaStream_t s = c->stream;
+        const uint8_t *d_in = samples;
+        if (samples_mem == B200Z_MEM_HOST) {
+            if ((e = r.input.ensure(samples_len + 16))) return e;
+            CU(c, cudaMemcpyAsync(r.input.p, samples, samples_len, cudaMemcpyHostToDevice, s));
+            d_in = r.input.as<uint8_t>();
+        }
+        CU(c, cudaMemcpyAsync(r.dcontent.p, content + (content_len - tail), tail, cudaMemcpyHostToDevice, s));
+        CU(c, cudaMemcpyAsync(r.blocks.p, hb.data(), nsamples * sizeof(CBlock), cudaMemcpyHostToDevice, s));
+        CU(c, cudaMemsetAsync(r.dcounts.p, 0, DS_BINS * 8, s));
+        if (int le = launch_dict_table(r.dcontent.as<uint8_t>(), tail, r.dtab.as<uint32_t>(), s, &c->launches))
+            return c->set_cuda_err((cudaError_t)le, "k_cdict");
+        CompressArgs a{};
+        a.input = d_in;
+        a.lit_stage = r.lit_stage.as<uint8_t>(); a.seq_stage = r.seq_stage.as<SeqRec>(); a.lits = r.lits.as<uint8_t>();
+        a.seqs = r.seqs.as<SeqRec>(); a.info = r.info.as<CBlockInfo>();
+        a.dict = r.dcontent.as<uint8_t>(); a.dtab = r.dtab.as<uint32_t>(); a.dict_len = tail;
+        for (uint64_t b0 = 0; b0 < nsamples; b0 += per) {
+            a.blocks = r.blocks.as<CBlock>() + b0;
+            a.nblocks = (uint32_t)std::min<uint64_t>(per, nsamples - b0);
+            if (int le = launch_dict_stats(a, r.dcounts.as<unsigned long long>(), s, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_dstats");
+        }
+        CU(c, cudaMemcpyAsync(counts.data(), r.dcounts.p, DS_BINS * 8, cudaMemcpyDeviceToHost, s));
+        CU(c, cudaStreamSynchronize(s));
+    }
+    return dict_from_counts(counts.data(), content, content_len, dict_id, dict, dict_cap, dict_len);
 }

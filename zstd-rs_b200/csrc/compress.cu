@@ -5,8 +5,10 @@
 //   k_cxxh64    : content checksum of every frame's input (xxh64.cuh; four serial chains per frame)
 //   k_cassemble : one CTA per block: frame header, the block at its prefix-summed offset, the checksum, per-frame results
 //   k_cdict     : not a stage: the match table of a dictionary, built once the first time the dictionary is used (EXTENSION)
+//   k_dstats    : not a stage: literal and sequence-code histograms of k_cmatch's parse, for b200z_dict_finalize (EXTENSION)
 //
-// Every block is encoded from its own literals and sequences only (no Repeat / Treeless modes, no repeat offsets), so all
+// Every block is encoded from its own literals and sequences only (no repeat offsets; Repeat / Treeless modes only in a frame's
+// first block with a formatted dictionary's tables, which the format makes that block's previous tables), so all
 // blocks of all frames -- including the blocks of one huge frame -- run at the same time.  Matches may still reach back into
 // the previous block: the input is all there from the start.  With a dictionary (an extension: ruzstd's encoder has none), the
 // first ENC_WINDOW bytes of every frame may also match the dictionary's content, which lies before the frame's first byte.
@@ -163,21 +165,25 @@ k_cmatch(const CBlock *__restrict__ blocks, const uint8_t *__restrict__ input, u
 
 // ------------------------------------------------------------------------------------------------------------
 // k_cenc: one warp per block encodes its literals and sequences (encode_block) into the block's staging slot and decides the
-// block type: RLE when all bytes are equal, Compressed when smaller than the input block, else Raw.
+// block type: RLE when all bytes are equal, Compressed when smaller than the input block, else Raw.  A formatted dictionary's
+// tables (dt, B200Z_FLAG_DICT_TABLES) go to a frame's first block only (back == 0); without them (TABLES = false) encode_block gets
+// a constant nullptr, so the plain path carries none of that code.
 // ------------------------------------------------------------------------------------------------------------
+template <bool TABLES>
 __global__ void __launch_bounds__(CE_WARPS * 32)
 k_cenc(const CBlock *__restrict__ blocks, uint32_t nblocks, const CBlockInfo *__restrict__ info, const uint8_t *__restrict__ lits,
-       const SeqRec *__restrict__ seqs, uint8_t *__restrict__ enc, CBlockInfo *__restrict__ res) {
+       const SeqRec *__restrict__ seqs, uint8_t *__restrict__ enc, CBlockInfo *__restrict__ res, const EncDict *__restrict__ dt) {
     __shared__ EncScratch scratch[CE_WARPS];
     const uint32_t w = threadIdx.x >> 5, lane = threadIdx.x & 31, b = blockIdx.x * CE_WARPS + w;
     if (b >= nblocks) return;
     const CBlockInfo in = info[b];
     const uint32_t n = blocks[b].size;
+    const EncDict *bdt = TABLES && blocks[b].back == 0 ? dt : nullptr;
     uint32_t type = 0, csize = n;
     if (in.type == 1) { type = 1; csize = 1; }
     else if (n) {
         const uint32_t size = encode_block(scratch[w], lits + (size_t)b * ENC_BLOCK, in.nlit, seqs + (size_t)b * CBLOCK_SEQS, in.nseq,
-                                           enc + (size_t)b * ENC_BLOCK, ENC_BLOCK, lane, 32);
+                                           enc + (size_t)b * ENC_BLOCK, ENC_BLOCK, lane, 32, TABLES ? bdt : nullptr);
         if (size < n) { type = 2; csize = size; }
     }
     if (lane == 0) res[b] = CBlockInfo{in.nlit, in.nseq, type, csize};
@@ -253,7 +259,48 @@ __global__ void __launch_bounds__(256) k_cdict(const uint8_t *__restrict__ dict,
     if (d < end) atomicMax(&dtab[hash5(dict + d, CD_LOG)], d + 1);
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// k_dstats: the entropy statistics of a dictionary's training samples (b200z_dict_finalize).  One CTA per parsed block (k_cmatch
+// against the dictionary's content): the histograms of its literal bytes and of its sequences' LL / ML / OF codes, as the
+// encoder codes them (offsets raw as offset + 3), in shared memory, then added to the u64 totals.  RLE blocks are left out:
+// the encoder writes no literals or sequences for them.  Integer atomics only, so the totals do not depend on the schedule.
+// ------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(DS_THREADS)
+k_dstats(const CBlockInfo *__restrict__ info, const uint8_t *__restrict__ lits, const SeqRec *__restrict__ seqs,
+         unsigned long long *__restrict__ counts) {
+    __shared__ uint32_t h[DS_BINS];
+    const uint32_t b = blockIdx.x, tid = threadIdx.x;
+    const CBlockInfo in = info[b];
+    if (in.type == 1) return;
+    for (uint32_t i = tid; i < DS_BINS; i += DS_THREADS) h[i] = 0;
+    __syncthreads();
+    const uint8_t *l = lits + (size_t)b * ENC_BLOCK;
+    for (uint32_t i = tid; i < in.nlit; i += DS_THREADS) atomicAdd(&h[DS_LIT + __ldg(l + i)], 1u);
+    const SeqRec *q = seqs + (size_t)b * CBLOCK_SEQS;
+    for (uint32_t i = tid; i < in.nseq; i += DS_THREADS) {
+        const SeqRec r = q[i];
+        atomicAdd(&h[DS_LL + ll_code(r.ll)], 1u);
+        atomicAdd(&h[DS_ML + ml_code(r.ml)], 1u);
+        atomicAdd(&h[DS_OF + of_code(r.of)], 1u);
+    }
+    __syncthreads();
+    for (uint32_t i = tid; i < DS_BINS; i += DS_THREADS)
+        if (h[i]) atomicAdd(&counts[i], (unsigned long long)h[i]);
+}
+
 static uint32_t cdiv_u(uint64_t a, uint32_t b) { return (uint32_t)((a + b - 1) / b); }
+
+int launch_dict_stats(const CompressArgs &a, unsigned long long *counts, cudaStream_t s, uint64_t *launched) {
+    if (!a.nblocks) return 0;
+    k_cmatch<true><<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, a.dict, a.dtab, a.dict_len);
+    int e = (int)cudaGetLastError();
+    if (e) return e;
+    ++*launched;
+    k_dstats<<<a.nblocks, DS_THREADS, 0, s>>>(a.info, a.lits, a.seqs, counts);
+    e = (int)cudaGetLastError();
+    if (!e) ++*launched;
+    return e;
+}
 
 int init_compress_kernels() {
     cudaError_t e = cudaFuncSetAttribute(k_cmatch<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CM_SMEM);
@@ -280,7 +327,11 @@ int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s, uint
         if (a.dtab) k_cmatch<true><<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, a.dict, a.dtab, a.dict_len);
         else k_cmatch<false><<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, nullptr, nullptr, 0);
         break;
-    case 1: if (!a.level || !a.nblocks) return 0; k_cenc<<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res); break;
+    case 1:
+        if (!a.level || !a.nblocks) return 0;
+        if (a.etab) k_cenc<true><<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res, a.etab);
+        else k_cenc<false><<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res, nullptr);
+        break;
     case 2: if (!a.checksum || !a.nframes) return 0; k_cxxh64<<<cdiv_u((uint64_t)a.nframes * 4, 128), 128, 0, s>>>(a.frames, a.input, a.csum, a.nframes); break;
     case 3: if (!a.nblocks) return 0; k_cassemble<<<a.nblocks, 256, 0, s>>>(a.frames, a.blocks, a.res, a.enc, a.input, a.csum, a.output, a.results, a.level, a.checksum, a.dict_id); break;
     default: return (int)cudaErrorInvalidValue;

@@ -47,6 +47,7 @@ struct CompressArgs {
     const uint8_t *dict;    // the last dict_len <= ENC_WINDOW bytes of its content (device): all a match can reach
     const uint32_t *dtab;   // [1 << CD_LOG] from k_cdict
     uint32_t dict_len, dict_id;
+    const EncDict *etab;    // a formatted dictionary's tables for the frames' first blocks (B200Z_FLAG_DICT_TABLES), else null
 };
 
 // the dictionary match table: 5-byte hash of a position in the dictionary's last ENC_WINDOW bytes -> that position + 1 (0 = none)
@@ -56,6 +57,17 @@ int init_compress_kernels();
 // fills dtab[1 << CD_LOG] for the device content dict[len], len <= ENC_WINDOW (a memset and k_cdict, on stream s); adds the kernels
 // it enqueued to *launched
 int launch_dict_table(const uint8_t *dict, uint32_t len, uint32_t *dtab, cudaStream_t s, uint64_t *launched);
+// dictionary statistics (b200z_dict_finalize): literal bytes, LL, ML and OF code counts, in that order, in one u64 array
+constexpr uint32_t DS_LIT = 0, DS_LL = 256, DS_ML = DS_LL + 36, DS_OF = DS_ML + 53, DS_BINS = DS_OF + 32;   // 377 bins
+constexpr uint32_t DS_THREADS = 256;
+constexpr uint32_t DS_BLOCKS = 2048;   // blocks per statistics submission: the compressor's staging of that many blocks (~1.8 GB)
+// k_cmatch<true> over a.blocks[a.nblocks] against a.dict / a.dtab, then k_dstats, which adds every non-RLE block's histograms to
+// counts[DS_BINS]; adds the kernels it enqueued to *launched
+int launch_dict_stats(const CompressArgs &a, unsigned long long *counts, cudaStream_t s, uint64_t *launched);
+// dict_format.cpp (host): the argument rule of b200z_dict_finalize that needs no counts, and the dictionary from counts[DS_BINS]
+int dict_check_args(size_t content_len, uint32_t dict_id, size_t dict_cap);
+int dict_from_counts(const uint64_t *counts, const uint8_t *content, size_t content_len, uint32_t dict_id, uint8_t *dict, size_t dict_cap,
+                     size_t *dict_len);
 constexpr int kCompressStages = 4;
 extern const char *const kCompressStageNames[kCompressStages];
 int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s, uint64_t *launched);   // adds the kernels it enqueued to *launched

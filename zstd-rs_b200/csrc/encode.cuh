@@ -8,6 +8,9 @@
 //              accuracy log <= 9 / 8 / 9 for LL / OF / ML (compressed.rs:55-72), RLE when the block has a single code;
 //              never Repeat
 // No block depends on another block's encoding, which is what lets every block of every frame be encoded at once.
+// With a formatted dictionary's tables (EncDict, B200Z_FLAG_DICT_TABLES; k_cenc passes them for a frame's first block only, the
+// one block where the format makes them the "previous" tables) encode_block may also choose Treeless literals with the
+// dictionary's Huffman codes and, per sequence table, Repeat with the dictionary's FSE table; without them it writes the above.
 #pragma once
 #include <stdint.h>
 
@@ -300,6 +303,52 @@ B200Z_HDN inline uint32_t huf_write_weights(const uint8_t *len, uint32_t maxb, u
     return 1 + size;
 }
 
+// ---- a formatted dictionary's tables, as the encoder uses them -------------------------------------------------------
+struct EncDict {
+    uint16_t huf_code[256];
+    uint8_t huf_len[256];      // 0: the byte has no code in the dictionary's table
+    FseCT ct[3];               // by ENC_LL / ENC_OF / ENC_ML
+    int16_t norm[3][64];       // normalized counts, 0 past the table's last symbol
+};
+// From the dictionary's Huffman weights (nweights explicit ones; the last symbol's weight is implied) and its three FSE tables'
+// normalized counts (nprobs[t] of them at accuracy log logs[t]), as Dictionary::decode_dict parsed them, so both are valid.
+B200Z_HDN inline void enc_dict_build(const uint8_t *weights, uint32_t nweights, const int16_t *const probs[3], const uint32_t nprobs[3],
+                                     const uint32_t logs[3], EncDict &d) {
+    uint32_t sum = 0;
+    for (uint32_t i = 0; i < nweights; i++) sum += weights[i] ? 1u << (weights[i] - 1) : 0u;
+    const uint32_t maxb = hbs(sum), last = hbs((1u << maxb) - sum);
+    for (uint32_t i = 0; i < 256; i++) {
+        const uint32_t w = i < nweights ? weights[i] : i == nweights ? last : 0u;
+        d.huf_len[i] = (uint8_t)(w ? maxb + 1 - w : 0);
+    }
+    huf_codes(d.huf_len, maxb, d.huf_code);
+    for (uint32_t t = 0; t < 3; t++) {
+        for (uint32_t c = 0; c < 64; c++) d.norm[t][c] = c < nprobs[t] ? probs[t][c] : 0;
+        fse_build_ctable(d.norm[t], nprobs[t] - 1, logs[t], d.ct[t]);
+    }
+}
+
+// log2(p) in 8-bit fixed point, p >= 1, in integers only (so the host and the GPU agree): the integer part from the highest set
+// bit, the fraction bit by bit by squaring the mantissa
+B200Z_HD uint32_t log2_q8(uint32_t p) {
+    const uint32_t hb = flog2(p);
+    uint64_t x = ((uint64_t)p << 16) >> hb;   // mantissa in [1, 2), 16 fraction bits
+    uint32_t r = hb << 8;
+    for (int i = 7; i >= 0; i--) {
+        x = (x * x) >> 16;
+        if (x >= (2u << 16)) { x >>= 1; r |= 1u << i; }
+    }
+    return r;
+}
+// estimated bits (8-bit fixed point) of coding cnt[0..maxsym] with normalized counts norm at accuracy log `log`: log - log2(p) per
+// symbol (a "less than 1" count costs as 1)
+B200Z_HD uint64_t fse_cost_q8(const uint32_t *cnt, uint32_t maxsym, const int16_t *norm, uint32_t log) {
+    uint64_t c = 0;
+    for (uint32_t s = 0; s <= maxsym; s++)
+        if (cnt[s]) c += (uint64_t)cnt[s] * ((log << 8) - log2_q8(norm[s] > 0 ? (uint32_t)norm[s] : 1u));
+    return c;
+}
+
 // ---- block ----------------------------------------------------------------------------------------------------
 struct EncScratch {   // per warp (shared memory on the GPU)
     uint32_t lit_cnt[256];
@@ -311,8 +360,10 @@ struct EncScratch {   // per warp (shared memory on the GPU)
     uint32_t mode[3], maxsym[3];
     uint32_t stream_bits[4], stream_off[4];
     uint32_t use_huf, lit_end, total;
+    uint32_t use_dict, dict_bits[4];   // Treeless literals with the dictionary's codes
 };
 
+B200Z_HD uint32_t raw_literals_header_size(uint32_t n) { return n < 32 ? 1 : n < 4096 ? 2 : 3; }
 B200Z_HD uint32_t raw_literals_header(uint8_t *dst, uint32_t cap, uint32_t n) {
     if (n < 32) { put_byte(dst, cap, 0, n << 3); return 1; }
     if (n < 4096) { put_le(dst, cap, 0, (1u << 2) | (n << 4), 2); return 2; }
@@ -323,11 +374,17 @@ B200Z_HD uint32_t raw_literals_header(uint8_t *dst, uint32_t cap, uint32_t n) {
 // Encodes one block's literals and sequences as the content of a Compressed block into dst[0, cap) and returns its size
 // (which may exceed cap: then only the first cap bytes were stored).  Every lane of the group calls it; nlanes = 32 on the
 // GPU, 1 on the host.  The trailing literals after the last sequence are the literals not consumed by any sequence.
+// dt: a formatted dictionary's tables when the block is a frame's first block, else nullptr (then the output is exactly what it
+// is without this argument).  With them:
+//   literals   Treeless (the dictionary's codes; 1 stream below 1024 literals, else 4) when every literal byte has a code and it
+//              is strictly smaller than what the rule above chooses (own Huffman or Raw)
+//   sequences  per table, Repeat when the block has more than one code, every code has a nonzero count in the dictionary's
+//              table, and its estimated cost is at most the table's own description plus its own estimated cost (fse_cost_q8)
 B200Z_HDN inline uint32_t encode_block(EncScratch &s, const uint8_t *lits, uint32_t nlit, const SeqRec *seqs, uint32_t nseq,
-                                      uint8_t *dst, uint32_t cap, uint32_t lane, uint32_t nlanes) {
+                                      uint8_t *dst, uint32_t cap, uint32_t lane, uint32_t nlanes, const EncDict *dt = nullptr) {
     for (uint32_t i = lane; i < 256; i += nlanes) s.lit_cnt[i] = 0;
     for (uint32_t i = lane; i < 3 * 64; i += nlanes) s.cnt[i / 64][i % 64] = 0;
-    for (uint32_t i = lane; i < 4; i += nlanes) s.stream_bits[i] = 0;
+    for (uint32_t i = lane; i < 4; i += nlanes) { s.stream_bits[i] = 0; if (dt) s.dict_bits[i] = 0; }
     B200Z_ENC_SYNC();
     for (uint32_t i = lane; i < nlit; i += nlanes) B200Z_ENC_ADD(&s.lit_cnt[lits[i]], 1u);
     for (uint32_t i = lane; i < nseq; i += nlanes) {
@@ -350,20 +407,49 @@ B200Z_HDN inline uint32_t encode_block(EncScratch &s, const uint8_t *lits, uint3
             const uint32_t tree = huf_write_weights(s.huf_len, maxb, dst + 5, cap > 5 ? cap - 5 : 0);
             if (tree) { s.use_huf = 1; s.lit_end = tree; }
         }
+        if (dt) {
+            s.use_dict = nlit >= 2;
+            for (uint32_t i = 0; i < 256; i++) if (s.lit_cnt[i] && !dt->huf_len[i]) s.use_dict = 0;
+        }
     }
     B200Z_ENC_SYNC();
-    if (s.use_huf) {
-        uint32_t b[4] = {0, 0, 0, 0};
-        for (uint32_t i = lane; i < nlit; i += nlanes) b[i / seg] += s.huf_len[lits[i]];
+    const uint32_t dstreams = nlit < 1024 ? 1 : 4;   // streams of Treeless literals
+    const bool try_dict = dt && s.use_dict;           // (dt is a constant nullptr in the plain path: all of this folds away)
+    if (s.use_huf || try_dict) {
+        uint32_t b[4] = {0, 0, 0, 0}, db[4] = {0, 0, 0, 0};
+        if (s.use_huf) for (uint32_t i = lane; i < nlit; i += nlanes) b[i / seg] += s.huf_len[lits[i]];
+        if (try_dict) for (uint32_t i = lane; i < nlit; i += nlanes) db[dstreams == 1 ? 0 : i / seg] += dt->huf_len[lits[i]];
         for (uint32_t k = 0; k < 4; k++) if (b[k]) B200Z_ENC_ADD(&s.stream_bits[k], b[k]);
+        for (uint32_t k = 0; k < 4; k++) if (db[k]) B200Z_ENC_ADD(&s.dict_bits[k], db[k]);
         B200Z_ENC_SYNC();
         if (lane == 0) {
             const uint32_t tree = s.lit_end;
             uint32_t csize = tree + 6;
             for (uint32_t k = 0; k < 4; k++) csize += (s.stream_bits[k] + 8) / 8;   // + the end marker bit
             const uint32_t hsize = (nlit < 16384 && csize < 16384) ? 4 : 5;
-            if (hsize + csize >= nlit + 3) s.use_huf = 0;   // Huffman does not pay (compressed.rs:367-371)
-            else {
+            if (s.use_huf && hsize + csize >= nlit + 3) s.use_huf = 0;   // Huffman does not pay (compressed.rs:367-371)
+            if (try_dict) {   // Treeless only when strictly smaller than the choice above
+                uint32_t dsize = dstreams == 1 ? 0 : 6;
+                for (uint32_t k = 0; k < dstreams; k++) dsize += (s.dict_bits[k] + 8) / 8;
+                const uint32_t dh = dstreams == 1 ? 3 : (nlit < 16384 && dsize < 16384) ? 4 : 5;
+                const uint32_t today = s.use_huf ? hsize + csize : raw_literals_header_size(nlit) + nlit;
+                if ((dstreams == 1 && dsize >= 1024) || dh + dsize >= today) s.use_dict = 0;
+                else {
+                    s.use_huf = 0;
+                    if (dh == 3) put_le(dst, cap, 0, 3u | (nlit << 4) | (dsize << 14), 3);
+                    else if (dh == 4) put_le(dst, cap, 0, 3u | (2u << 2) | (nlit << 4) | ((uint64_t)dsize << 18), 4);
+                    else put_le(dst, cap, 0, 3u | (3u << 2) | ((uint64_t)nlit << 4) | ((uint64_t)dsize << 22), 5);
+                    uint32_t off = dh + (dstreams == 1 ? 0 : 6);
+                    for (uint32_t k = 0; k < dstreams; k++) {
+                        const uint32_t sz = (s.dict_bits[k] + 8) / 8;
+                        if (dstreams == 4 && k < 3) put_le(dst, cap, dh + 2 * k, sz, 2);
+                        s.stream_off[k] = off;
+                        off += sz;
+                    }
+                    s.lit_end = off;
+                }
+            }
+            if (s.use_huf) {
                 if (hsize == 4) for (uint32_t i = 0; i < tree; i++) put_byte(dst, cap, 4 + i, 5 + i < cap ? dst[5 + i] : 0u);
                 if (hsize == 4) put_le(dst, cap, 0, 2u | (2u << 2) | (nlit << 4) | ((uint64_t)csize << 18), 4);
                 else put_le(dst, cap, 0, 2u | (3u << 2) | ((uint64_t)nlit << 4) | ((uint64_t)csize << 22), 5);
@@ -379,11 +465,15 @@ B200Z_HDN inline uint32_t encode_block(EncScratch &s, const uint8_t *lits, uint3
         }
         B200Z_ENC_SYNC();
     }
-    if (s.use_huf) {
-        for (uint32_t k = lane; k < 4; k += nlanes) {   // each stream is written backwards: the decoder reads it from the end
-            const uint32_t lo = k * seg, hi = k == 3 ? nlit : lo + seg, off = s.stream_off[k];
+    const bool dict_lits = dt && s.use_dict;
+    if (s.use_huf || dict_lits) {
+        const uint16_t *code = dict_lits ? dt->huf_code : s.huf_code;
+        const uint8_t *len = dict_lits ? dt->huf_len : s.huf_len;
+        const uint32_t ns = dict_lits ? dstreams : 4;
+        for (uint32_t k = lane; k < ns; k += nlanes) {   // each stream is written backwards: the decoder reads it from the end
+            const uint32_t lo = ns == 1 ? 0 : k * seg, hi = k == ns - 1 ? nlit : lo + seg, off = s.stream_off[k];
             BitW w{dst + off, cap > off ? cap - off : 0, 0, 0, 0};
-            for (uint32_t i = hi; i > lo; i--) w.put(s.huf_code[lits[i - 1]], s.huf_len[lits[i - 1]]);
+            for (uint32_t i = hi; i > lo; i--) w.put(code[lits[i - 1]], len[lits[i - 1]]);
             w.close();
         }
     } else {
@@ -401,6 +491,7 @@ B200Z_HDN inline uint32_t encode_block(EncScratch &s, const uint8_t *lits, uint3
         if (nseq) {
             const uint32_t pmodes = p++;
             uint32_t modes = 0;
+            const FseCT *ct[3] = {&s.ct[0], &s.ct[1], &s.ct[2]};
             for (uint32_t t = 0; t < 3; t++) {
                 uint32_t distinct = 0, maxsym = 0;
                 for (uint32_t c = 0; c <= enc_max_sym(t); c++) if (s.cnt[t][c]) { distinct++; maxsym = c; }
@@ -411,7 +502,16 @@ B200Z_HDN inline uint32_t encode_block(EncScratch &s, const uint8_t *lits, uint3
                     const uint32_t log = fse_pick_log(nseq, maxsym, distinct, enc_max_log(t));
                     fse_normalize(s.cnt[t], maxsym, nseq, log, s.norm[t]);
                     fse_build_ctable(s.norm[t], maxsym, log, s.ct[t]);
-                    p += fse_write_ncount(s.norm[t], maxsym, log, dst + p, cap > p ? cap - p : 0);
+                    const uint32_t desc = fse_write_ncount(s.norm[t], maxsym, log, dst + p, cap > p ? cap - p : 0);
+                    bool rep = dt != nullptr;
+                    for (uint32_t c = 0; rep && c <= maxsym; c++) if (s.cnt[t][c] && !dt->norm[t][c]) rep = false;
+                    if (rep && fse_cost_q8(s.cnt[t], maxsym, dt->norm[t], dt->ct[t].log) <=
+                                   ((uint64_t)desc << 11) + fse_cost_q8(s.cnt[t], maxsym, s.norm[t], log)) {
+                        s.mode[t] = 3;   // Repeat: the dictionary's table, no description
+                        ct[t] = &dt->ct[t];
+                    } else {
+                        p += desc;
+                    }
                 }
             }
             modes = (s.mode[ENC_LL] << 6) | (s.mode[ENC_OF] << 4) | (s.mode[ENC_ML] << 2);
@@ -422,19 +522,19 @@ B200Z_HDN inline uint32_t encode_block(EncScratch &s, const uint8_t *lits, uint3
             uint32_t st[3] = {0, 0, 0};
             const SeqRec q = seqs[nseq - 1];
             const uint32_t c0[3] = {ll_code(q.ll), of_code(q.of), ml_code(q.ml)};
-            for (uint32_t t = 0; t < 3; t++) if (s.mode[t] == 2) st[t] = fse_init_state(s.ct[t], c0[t]);   // no bits: order is free
+            for (uint32_t t = 0; t < 3; t++) if (s.mode[t] >= 2) st[t] = fse_init_state(*ct[t], c0[t]);   // no bits: order is free
             w.put(q.ll, ll_bits(c0[ENC_LL]));
             w.put(q.ml - 3, ml_bits(c0[ENC_ML]));
             w.put(q.of + 3, c0[ENC_OF]);
             for (uint32_t n = nseq - 1; n-- > 0;) {
                 const SeqRec r = seqs[n];
                 const uint32_t c[3] = {ll_code(r.ll), of_code(r.of), ml_code(r.ml)};
-                for (uint32_t t : kEncOrder) if (s.mode[t] == 2) fse_encode(w, s.ct[t], st[t], c[t]);
+                for (uint32_t t : kEncOrder) if (s.mode[t] >= 2) fse_encode(w, *ct[t], st[t], c[t]);
                 w.put(r.ll, ll_bits(c[ENC_LL]));
                 w.put(r.ml - 3, ml_bits(c[ENC_ML]));
                 w.put(r.of + 3, c[ENC_OF]);
             }
-            for (uint32_t t : kFlushOrder) if (s.mode[t] == 2) w.put(st[t], s.ct[t].log);
+            for (uint32_t t : kFlushOrder) if (s.mode[t] >= 2) w.put(st[t], ct[t]->log);
             w.close();
             p += w.pos;
         }
