@@ -51,7 +51,7 @@ __device__ __forceinline__ uint32_t match_len(const uint8_t *a, const uint8_t *b
 // when that source is within the window, and verifies it against the dictionary's content; the longest candidate wins, the
 // smaller offset on a tie.  A dictionary match stops at the dictionary's end.  Without DICT the code is the plain parse.
 // Sequences and literals go to per-segment staging; the CTA then packs them, the trailing literals of a segment joining the
-// first sequence after them.
+// first sequence after them.  tests/cparse.py states this parse rule by rule; the GPU must produce exactly its sequences.
 // ------------------------------------------------------------------------------------------------------------
 template <bool DICT>
 __global__ void __launch_bounds__(CM_THREADS, 1)
@@ -97,6 +97,8 @@ k_cmatch(const CBlock *__restrict__ blocks, const uint8_t *__restrict__ input, u
             h2 = hash5(src + q, CM_TP_LOG);
             const int32_t c2 = tp[h2];
             if (c1 < q) { len = match_len(src + q, src + c1, lim); cand = q - c1; }
+            // the window check cannot fail: c2 >= s - CM_SEED and q < s + seglen <= s + CM_SEED, so a tp offset is below 32 KiB
+            // (offsets up to 128 KiB come from t1 only)
             if (c2 != INT_MIN && c2 < (int32_t)q && (int32_t)q - c2 <= (int32_t)ENC_WINDOW) {
                 const uint32_t l2 = match_len(src + q, src + c2, lim);
                 if (l2 > len || (l2 == len && (uint32_t)((int32_t)q - c2) < cand)) { len = l2; cand = (uint32_t)((int32_t)q - c2); }
