@@ -504,6 +504,38 @@ const char *b200z_compress_stage_name(int stage);
 int b200z_compress_last_profile(const b200z_ctx *ctx, float *stage_ms, size_t n);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Stream compressor -- mirror of ruzstd's FrameCompressor (encoding/frame_compressor.rs:75-276): one frame from a source of
+ * unknown length (`read_cb`, io::Read::read semantics) to a drain (`write_cb`, io::Write::write_all over it), in bounded memory.
+ * The frame is the reference's framing: magic, FHD 0x04 with the checksum or 0x00 without, Window_Descriptor 0x38 (128 KiB), no
+ * Frame_Content_Size, 128 KiB blocks; a block is last only when a read returned 0 before it filled, so a source whose length is
+ * a multiple of 128 KiB (0 included) ends with an empty last Raw block (01 00 00); then the low 32 bits of XXH64 (seed 0) of the
+ * plaintext when the checksum is on.  Level Uncompressed writes Raw blocks, byte for byte the reference's frame, on the host
+ * only (no kernel, no device copy).  Level Fastest writes every block's type and body as b200z_compress_frames_batch does for the
+ * same block of the same input compressed as one frame.
+ * The source is read into chunks of whole blocks: B200Z_PIPELINE_CHUNK_BYTES (read by _new) rounded down to a multiple of
+ * 131072, at least 131072; 64 MiB by default.  At Fastest each non-empty chunk is uploaded and compressed by three kernels
+ * (k_cmatch, k_cenc, k_cassemble) on the ctx stream, counted in b200z_ctx_kernel_launches, while the host reads and hashes the
+ * next chunk and writes the previous one: one write_cb pass per chunk (header in the first, trailer in the last), not per block.
+ * Memory, allocated by the first Fastest compress and kept until _free, depends on the chunk C only.  Device: 2 * (C + 131072)
+ * input, 2 * (C + 3 * C / 131072) output, and the compressor's staging for C / 131072 blocks (about 0.9 MB per block); about
+ * 0.7 GB at 64 MiB.  Pinned host: 2 * C input and 2 * (C + 3 * C / 131072) output.
+ * Errors: a read returning < 0 (or more than asked for), or a write returning <= 0, is an unwrap() panic in the reference; here
+ * compress returns B200Z_ERR_REFERENCE_WOULD_PANIC (message in b200z_ctx_last_error_message), bytes already written stay
+ * written, and the compressor stays usable.  Hashing and matching state reset with every compress.
+ * ---------------------------------------------------------------------------------------------------------- */
+typedef struct b200z_frame_compressor b200z_frame_compressor;
+/* FrameCompressor::new :77.  B200Z_ERR_INVALID_ARGUMENT for a level outside 0-4 */
+int b200z_frame_compressor_new(b200z_ctx *ctx, int level, int checksum, b200z_frame_compressor **out);
+void b200z_frame_compressor_free(b200z_frame_compressor *fc);
+int b200z_frame_compressor_set_compression_level(b200z_frame_compressor *fc, int level);   /* :263; 0-4, else INVALID_ARGUMENT */
+int b200z_frame_compressor_compression_level(const b200z_frame_compressor *fc);            /* :273 */
+/* compress :131-224: one frame from read_cb to write_cb.  B200Z_ERR_REFERENCE_WOULD_PANIC for levels 2-4 before any read, write
+ * or launch.  result (may be NULL): dst_size = bytes written, blocks (the trailing empty block included), raw / RLE blocks
+ * (the empty block is Raw), has_checksum, checksum */
+int b200z_frame_compressor_compress(b200z_frame_compressor *fc, b200z_read_fn read_cb, void *read_user, b200z_write_fn write_cb,
+                                    void *write_user, b200z_compress_result *result);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Raw-content dictionary trainer -- EXTENSION in place of ruzstd::dictionary::create_raw_dict_from_source /
  * create_raw_dict_from_dir (dictionary/mod.rs:76,127, feature dict_builder).  The reference cannot serve as the model: its
  * reservoir sample reads the whole source to EOF (reservoir.rs:83-104), so its epoch loop (mod.rs:171-188) reads nothing and

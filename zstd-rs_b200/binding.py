@@ -164,6 +164,11 @@ def lib():
         "b200z_compress_num_stages": (C.c_int, []),
         "b200z_compress_stage_name": (C.c_char_p, [C.c_int]),
         "b200z_compress_last_profile": (C.c_int, [vp, C.POINTER(C.c_float), sz]),
+        "b200z_frame_compressor_new": (C.c_int, [vp, C.c_int, C.c_int, pp]),
+        "b200z_frame_compressor_free": (None, [vp]),
+        "b200z_frame_compressor_set_compression_level": (C.c_int, [vp, C.c_int]),
+        "b200z_frame_compressor_compression_level": (C.c_int, [vp]),
+        "b200z_frame_compressor_compress": (C.c_int, [vp, READ_FN, vp, WRITE_FN, vp, vp]),
         "b200z_dict_train_raw": (C.c_int, [vp, vp, sz, C.c_int, vp, sz, sz, sz, vp, sz, C.POINTER(sz), vp, sz, C.POINTER(sz)]),
         "b200z_dict_finalize": (C.c_int, [vp, vp, sz, vp, sz, C.c_int, vp, sz, C.c_uint32, vp, sz, C.POINTER(sz)]),
         "b200z_debug_dict_from_counts": (C.c_int, [vp, vp, sz, C.c_uint32, vp, sz, C.POINTER(sz)]),
@@ -504,6 +509,104 @@ def compress_to_vec(ctx, data, level=FASTEST, checksum=True, dict=None, dict_tab
     io = np.array([(0, len(src), 0, cap)], dtype=COMPRESS_IO_DTYPE)
     res = compress_frames(ctx, src, io, out, level, checksum, dict, dict_tables)
     return out[:int(res[0]["dst_size"])].tobytes()
+
+
+class FrameCompressor:
+    """GPU-backed mirror of ruzstd::encoding::FrameCompressor (frame_compressor.rs:75-276): compress() reads the source to its end
+    and writes one frame to the drain, chunk by chunk, in memory bounded by the chunk size (b200z_frame_compressor, see
+    include/b200zstd.h).  Sources: bytes or file-likes with read(); drains: file-likes with write(), or a bytearray, which the
+    frame is appended to.  An exception raised by the source or the drain fails the call as the reference's unwrap() would,
+    with B200ZError(REFERENCE_WOULD_PANIC) raised from it."""
+
+    def __init__(self, ctx, level=FASTEST, checksum=True):
+        self.ctx, self.L = ctx, ctx.L
+        self.h = None
+        h = C.c_void_p()
+        ctx._chk(self.L.b200z_frame_compressor_new(ctx.h, level, 1 if checksum else 0, C.byref(h)))
+        self.h = h
+        self._source = self._drain = None
+
+    def __del__(self):
+        try:
+            if self.h and self.ctx.h:
+                self.L.b200z_frame_compressor_free(self.h)
+        except Exception:
+            pass
+
+    def set_source(self, source):
+        old, self._source = self._source, source
+        return old
+
+    def set_drain(self, drain):
+        old, self._drain = self._drain, drain
+        return old
+
+    def source(self): return self._source
+    def drain(self): return self._drain
+
+    def take_source(self):
+        s, self._source = self._source, None
+        return s
+
+    def take_drain(self):
+        d, self._drain = self._drain, None
+        return d
+
+    def set_compression_level(self, level):
+        """Returns the previous level, as the reference does."""
+        old = self.compression_level()
+        self.ctx._chk(self.L.b200z_frame_compressor_set_compression_level(self.h, level))
+        return old
+
+    def compression_level(self): return self.L.b200z_frame_compressor_compression_level(self.h)
+
+    def compress(self):
+        """One frame from the source to the drain.  Returns the COMPRESS_RESULT_DTYPE row: dst_size = bytes written, blocks,
+        raw / RLE blocks, checksum."""
+        panic = [k for k, v in error_names().items() if v == "B200Z_ERR_REFERENCE_WOULD_PANIC"][0]
+        if self._source is None or self._drain is None:
+            raise B200ZError(panic, 0, "FrameCompressor::compress: no source or no drain set")
+        src = _Reader(self._source).src
+        drain = self._drain
+        failure = []
+
+        def _read(_user, buf, n):
+            try:
+                b = src.read(n)
+                if b:
+                    C.memmove(buf, b, len(b))
+                return len(b)
+            except Exception as e:
+                failure.append(e)
+                return -1
+
+        def _write(_user, buf, n):
+            try:
+                if isinstance(drain, bytearray):
+                    drain.extend(C.string_at(buf, n))
+                    return n
+                r = drain.write(C.string_at(buf, n))
+                return n if r is None else r
+            except Exception as e:
+                failure.append(e)
+                return -1
+
+        rd, wr = READ_FN(_read), WRITE_FN(_write)
+        res = np.zeros(1, dtype=COMPRESS_RESULT_DTYPE)
+        e = self.L.b200z_frame_compressor_compress(self.h, rd, None, wr, None, res.ctypes.data)
+        if e:
+            err = B200ZError(e, 0, self.L.b200z_ctx_last_error_message(self.ctx.h).decode())
+            raise err from (failure[0] if failure else None)
+        return res[0]
+
+
+def compress(ctx, source, target, level=FASTEST, checksum=True):
+    """Mirror of ruzstd::encoding::compress (encoding/mod.rs): one frame from `source` (bytes or a reader) to `target` (a writer
+    or a bytearray) through a FrameCompressor.  Returns its result row."""
+    fc = FrameCompressor(ctx, level, checksum)
+    fc.set_source(source)
+    fc.set_drain(target)
+    return fc.compress()
 
 
 def compress_profile(ctx):

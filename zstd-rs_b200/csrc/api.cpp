@@ -2106,6 +2106,286 @@ extern "C" int b200z_compress_frames_batch_dict(b200z_ctx *c, const uint8_t *inp
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// stream compressor (FrameCompressor, frame_compressor.rs:75-276): the source is read into chunks of whole 128 KiB blocks and
+// the frame is written chunk by chunk.  Uncompressed frames the blocks on the host.  Fastest runs k_cmatch -> k_cenc ->
+// k_cassemble<true> on each chunk on the ctx stream, uploads on one copy stream and downloads on another, while the calling
+// thread reads and hashes the next chunk and writes the previous one (the pattern of decode_frames_pipelined).
+// ---------------------------------------------------------------------------------------------------------------
+namespace {
+struct PinnedBuf {
+    uint8_t *p = nullptr;
+    PinnedBuf() = default;
+    PinnedBuf(const PinnedBuf &) = delete;
+    PinnedBuf &operator=(const PinnedBuf &) = delete;
+    ~PinnedBuf() { if (p) cudaFreeHost(p); }
+    int alloc(size_t n) {   // once: the size never changes for its owner
+        if (p) return 0;
+        if (cudaMallocHost((void **)&p, n) != cudaSuccess) { p = nullptr; cudaGetLastError(); return B200Z_ERR_OUT_OF_MEMORY; }
+        return 0;
+    }
+};
+constexpr size_t FC_HEADER = 6;       // magic, FHD, Window_Descriptor
+constexpr size_t FC_HDR_ROOM = 16;    // in front of a chunk's blocks in its output buffer: the first chunk's header goes there
+constexpr size_t FC_TRAILER = 3 + 4;  // after them in the last chunk: the empty last block and the checksum
+}  // namespace
+
+struct b200z_frame_compressor {
+    b200z_ctx *ctx = nullptr;
+    int device = 0;
+    int level = B200Z_LEVEL_FASTEST;
+    bool checksum = true;
+    uint64_t chunk = 64ull << 20;   // bytes per chunk, a multiple of ENC_BLOCK
+    std::vector<uint8_t> raw;       // Uncompressed: one chunk's part of the frame
+    // Fastest, allocated by its first compress; slot s serves chunks k with k & 1 == s
+    cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
+    cudaEvent_t ev_h2d[2] = {}, ev_k[2] = {}, ev_d2h[2] = {};
+    PinnedBuf h_in[2], h_out[2], h_desc[2];   // desc: the chunk's CFrame, its CBlocks, then its b200z_compress_result
+    DevBuf d_in[2], d_out[2], d_desc[2];      // d_in: the previous chunk's last ENC_WINDOW bytes, then the chunk
+    DevBuf lit_stage, seq_stage, lits, seqs, info, res;   // k_cmatch / k_cenc staging, shared: the kernels run in order on one stream
+    bool ready = false;
+    ~b200z_frame_compressor() {
+        for (int i = 0; i < 2; i++)
+            for (cudaEvent_t e : {ev_h2d[i], ev_k[i], ev_d2h[i]}) if (e) cudaEventDestroy(e);
+        if (s_h2d) cudaStreamDestroy(s_h2d);
+        if (s_d2h) cudaStreamDestroy(s_d2h);
+    }
+    uint32_t chunk_blocks() const { return (uint32_t)(chunk / ENC_BLOCK); }
+    size_t chunk_bound() const { return chunk + 3ull * chunk_blocks(); }   // the chunk's blocks, packed, at most
+    size_t res_off() const { return sizeof(CFrame) + (size_t)chunk_blocks() * sizeof(CBlock); }
+    size_t desc_bytes() const { return res_off() + sizeof(b200z_compress_result); }
+};
+
+static int fc_valid_level(int level) { return level >= 0 && level <= 4; }   // CompressionLevel: Uncompressed .. Best
+static int fc_panic(b200z_ctx *c, const char *what) { c->err = what; return B200Z_ERR_REFERENCE_WOULD_PANIC; }
+
+extern "C" int b200z_frame_compressor_new(b200z_ctx *c, int level, int checksum, b200z_frame_compressor **out) {
+    if (!out) return B200Z_ERR_INVALID_ARGUMENT;
+    *out = nullptr;
+    if (!c || !fc_valid_level(level)) return B200Z_ERR_INVALID_ARGUMENT;
+    std::unique_ptr<b200z_frame_compressor> fc(new b200z_frame_compressor());
+    fc->ctx = c;
+    fc->device = c->device;
+    fc->level = level;
+    fc->checksum = checksum != 0;
+    if (const char *ev = getenv("B200Z_PIPELINE_CHUNK_BYTES"))
+        fc->chunk = std::max<uint64_t>(ENC_BLOCK, strtoull(ev, nullptr, 10) / ENC_BLOCK * ENC_BLOCK);
+    *out = fc.release();
+    return 0;
+}
+extern "C" void b200z_frame_compressor_free(b200z_frame_compressor *fc) {
+    if (!fc) return;
+    if (fc->ready) {
+        cudaSetDevice(fc->device);
+        cudaStreamSynchronize(fc->s_h2d);
+        cudaStreamSynchronize(fc->s_d2h);
+    }
+    delete fc;
+}
+extern "C" int b200z_frame_compressor_set_compression_level(b200z_frame_compressor *fc, int level) {
+    if (!fc || !fc_valid_level(level)) return B200Z_ERR_INVALID_ARGUMENT;
+    fc->level = level;
+    return 0;
+}
+extern "C" int b200z_frame_compressor_compression_level(const b200z_frame_compressor *fc) { return fc ? fc->level : B200Z_LEVEL_FASTEST; }
+
+// reads up to `cap` bytes, stopping at the first read that returns 0 (*eof; the reference stops there too); false on a read
+// error (< 0, or more than was asked for)
+static bool fc_read(b200z_read_fn rd, void *ru, uint8_t *buf, size_t cap, size_t *n, bool *eof) {
+    size_t got = 0;
+    *eof = false;
+    while (got < cap) {
+        const long r = rd(ru, buf + got, cap - got);
+        if (r < 0 || (size_t)r > cap - got) return false;
+        if (r == 0) { *eof = true; break; }
+        got += (size_t)r;
+    }
+    *n = got;
+    return true;
+}
+static bool fc_write(b200z_write_fn wr, void *wu, const uint8_t *p, size_t n) {   // write_all
+    while (n) {
+        const long w = wr(wu, p, n);
+        if (w <= 0 || (size_t)w > n) return false;
+        p += w;
+        n -= (size_t)w;
+    }
+    return true;
+}
+static void fc_le(uint8_t *p, uint64_t v, int n) { for (int i = 0; i < n; i++) p[i] = (uint8_t)(v >> (8 * i)); }
+// the frame header (frame_compressor.rs:144-151): no Frame_Content_Size, Single_Segment 0, a 128 KiB window
+static void fc_header(uint8_t *dst, bool checksum) {
+    fc_le(dst, 0xFD2FB528u, 4);
+    dst[4] = checksum ? 0x04 : 0x00;
+    dst[5] = 0x38;
+}
+// the end of the frame after its last chunk: the empty last Raw block when the source ended on a block boundary (the reference's
+// uncompressed_data.is_empty() branch, :175-186), then the checksum (:215-223).  Returns the bytes written at dst.
+static size_t fc_trailer(uint8_t *dst, bool empty_block, bool checksum, const XXH64State &h, b200z_compress_result &r) {
+    size_t len = 0;
+    if (empty_block) { fc_le(dst, 1, 3); len = 3; r.blocks++; r.raw_blocks++; }
+    if (checksum) {
+        r.has_checksum = 1;
+        r.checksum = (uint32_t)h.digest();
+        fc_le(dst + len, r.checksum, 4);
+        len += 4;
+    }
+    return len;
+}
+
+// Uncompressed: Raw blocks read straight into place behind their headers, one chunk of them per write
+static int fc_compress_raw(b200z_frame_compressor *fc, b200z_read_fn rd, void *ru, b200z_write_fn wr, void *wu, XXH64State &h,
+                           b200z_compress_result &r) {
+    b200z_ctx *c = fc->ctx;
+    const uint32_t nb = fc->chunk_blocks();
+    fc->raw.resize(FC_HDR_ROOM + (size_t)nb * (3 + ENC_BLOCK) + FC_TRAILER);
+    uint8_t *const body = fc->raw.data() + FC_HDR_ROOM;
+    for (uint64_t k = 0;; k++) {
+        size_t len = 0, n = 0;
+        bool eof = false;
+        for (uint32_t i = 0; i < nb && !eof; i++) {
+            if (!fc_read(rd, ru, body + len + 3, ENC_BLOCK, &n, &eof)) return fc_panic(c, "FrameCompressor::compress: the source's read failed");
+            if (n == 0) break;   // the source ended on a block boundary: the trailer's empty block is the last
+            h.update(body + len + 3, n);
+            fc_le(body + len, (eof ? 1u : 0u) | ((uint32_t)n << 3), 3);
+            len += 3 + n;
+            r.blocks++;
+            r.raw_blocks++;
+        }
+        uint8_t *start = body;
+        if (k == 0) { start -= FC_HEADER; fc_header(start, fc->checksum); }
+        if (eof) len += fc_trailer(body + len, n == 0, fc->checksum, h, r);
+        const size_t w = (size_t)(body + len - start);
+        if (!fc_write(wr, wu, start, w)) return fc_panic(c, "FrameCompressor::compress: the drain's write failed");
+        r.dst_size += w;
+        if (eof) return 0;
+    }
+}
+
+static int fc_prepare(b200z_frame_compressor *fc) {
+    if (fc->ready) return 0;
+    b200z_ctx *c = fc->ctx;
+    const size_t C = fc->chunk, nb = fc->chunk_blocks(), bound = fc->chunk_bound();
+    if (!fc->s_h2d) CU(c, cudaStreamCreateWithFlags(&fc->s_h2d, cudaStreamNonBlocking));
+    if (!fc->s_d2h) CU(c, cudaStreamCreateWithFlags(&fc->s_d2h, cudaStreamNonBlocking));
+    for (int i = 0; i < 2; i++)
+        for (cudaEvent_t *e : {&fc->ev_h2d[i], &fc->ev_k[i], &fc->ev_d2h[i]})
+            if (!*e) CU(c, cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    int e = 0;
+    for (int i = 0; i < 2 && !e; i++)
+        if ((e = fc->d_in[i].ensure(ENC_WINDOW + C + 16, false)) || (e = fc->d_out[i].ensure(bound + 16, false)) ||
+            (e = fc->d_desc[i].ensure(fc->desc_bytes(), false)) || (e = fc->h_in[i].alloc(C)) ||
+            (e = fc->h_out[i].alloc(FC_HDR_ROOM + bound + FC_TRAILER)) || (e = fc->h_desc[i].alloc(fc->desc_bytes())))
+            break;
+    if (!e) e = fc->lit_stage.ensure(nb * ENC_BLOCK, false) || fc->seq_stage.ensure(nb * CBLOCK_SEQS * sizeof(SeqRec), false) ||
+                fc->lits.ensure(nb * ENC_BLOCK, false) || fc->seqs.ensure(nb * CBLOCK_SEQS * sizeof(SeqRec), false) ||
+                fc->info.ensure(nb * sizeof(CBlockInfo), false) || fc->res.ensure(nb * sizeof(CBlockInfo), false) ? B200Z_ERR_OUT_OF_MEMORY : 0;
+    if (e) { c->err = "FrameCompressor: out of memory for chunks of " + std::to_string(C) + " bytes"; return e; }
+    fc->ready = true;
+    return 0;
+}
+
+// Fastest: chunk k (slot s = k & 1) is read into h_in[s] and hashed, uploaded behind the previous chunk's last 128 KiB
+// (for matches that reach back), compressed, downloaded to h_out[s] and written.  While chunk k uploads and compresses, the
+// host reads chunk k + 1 and writes chunk k - 1.  A slot's buffers are reused only after the event of the last work that read
+// them: ev_k (kernels: d_in, d_desc), ev_h2d (upload: h_in, h_desc), ev_d2h (download: d_out, the result, h_out).
+static int fc_compress_fast(b200z_frame_compressor *fc, b200z_read_fn rd, void *ru, b200z_write_fn wr, void *wu, XXH64State &h,
+                            b200z_compress_result &r) {
+    b200z_ctx *c = fc->ctx;
+    if (int e = fc_prepare(fc)) return e;
+    const uint64_t C = fc->chunk;
+    cudaStream_t ks = c->stream;
+    size_t n[2] = {0, 0};               // the chunk read into h_in[s]
+    bool eof[2] = {false, false};
+    size_t out_n[2] = {0, 0};           // the chunk whose output is in slot s
+    auto enqueue = [&](uint64_t k, int s) -> int {
+        const uint32_t m = (uint32_t)((n[s] + ENC_BLOCK - 1) / ENC_BLOCK);
+        CFrame *hf = reinterpret_cast<CFrame *>(fc->h_desc[s].p);
+        CBlock *hb = reinterpret_cast<CBlock *>(hf + 1);
+        *hf = CFrame{ENC_WINDOW, n[s], 0, 0, m};
+        for (uint32_t i = 0; i < m; i++) {
+            const uint64_t at = (uint64_t)i * ENC_BLOCK;
+            hb[i] = CBlock{ENC_WINDOW + at, (uint32_t)std::min<uint64_t>(ENC_BLOCK, n[s] - at), (uint32_t)std::min<uint64_t>(k * C + at, ENC_WINDOW), 0, 0};
+        }
+        uint8_t *din = fc->d_in[s].as<uint8_t>();
+        CU(c, cudaStreamWaitEvent(fc->s_h2d, fc->ev_k[s], 0));   // chunk k - 2's kernels are done with d_in[s] and d_desc[s]
+        if (k) CU(c, cudaMemcpyAsync(din, fc->d_in[s ^ 1].as<uint8_t>() + C, ENC_WINDOW, cudaMemcpyDeviceToDevice, fc->s_h2d));
+        CU(c, cudaMemcpyAsync(din + ENC_WINDOW, fc->h_in[s].p, n[s], cudaMemcpyHostToDevice, fc->s_h2d));
+        CU(c, cudaMemcpyAsync(fc->d_desc[s].p, hf, sizeof(CFrame) + m * sizeof(CBlock), cudaMemcpyHostToDevice, fc->s_h2d));
+        CU(c, cudaEventRecord(fc->ev_h2d[s], fc->s_h2d));
+        CU(c, cudaStreamWaitEvent(ks, fc->ev_h2d[s], 0));
+        CompressArgs a{};
+        a.frames = fc->d_desc[s].as<CFrame>();
+        a.blocks = reinterpret_cast<const CBlock *>(a.frames + 1);
+        a.results = reinterpret_cast<b200z_compress_result *>(fc->d_desc[s].as<uint8_t>() + fc->res_off());
+        a.input = din; a.output = fc->d_out[s].as<uint8_t>();
+        a.lit_stage = fc->lit_stage.as<uint8_t>(); a.seq_stage = fc->seq_stage.as<SeqRec>(); a.lits = fc->lits.as<uint8_t>();
+        a.seqs = fc->seqs.as<SeqRec>(); a.enc = a.lit_stage; a.info = fc->info.as<CBlockInfo>(); a.res = fc->res.as<CBlockInfo>();
+        a.nframes = 1; a.nblocks = m; a.level = B200Z_LEVEL_FASTEST;
+        if (int le = launch_compress_chunk(a, ks, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_cmatch / k_cenc / k_cassemble<true>");
+        CU(c, cudaEventRecord(fc->ev_k[s], ks));
+        CU(c, cudaStreamWaitEvent(fc->s_d2h, fc->ev_k[s], 0));
+        CU(c, cudaMemcpyAsync(fc->h_desc[s].p + fc->res_off(), a.results, sizeof(b200z_compress_result), cudaMemcpyDeviceToHost, fc->s_d2h));
+        CU(c, cudaMemcpyAsync(fc->h_out[s].p + FC_HDR_ROOM, a.output, n[s] + 3ull * m, cudaMemcpyDeviceToHost, fc->s_d2h));
+        CU(c, cudaEventRecord(fc->ev_d2h[s], fc->s_d2h));
+        return 0;
+    };
+    auto write_chunk = [&](uint64_t k, int s, bool final) -> int {
+        uint8_t *const body = fc->h_out[s].p + FC_HDR_ROOM;
+        size_t len = 0;
+        if (out_n[s]) {
+            CU(c, cudaEventSynchronize(fc->ev_d2h[s]));
+            const b200z_compress_result &cr = *reinterpret_cast<const b200z_compress_result *>(fc->h_desc[s].p + fc->res_off());
+            len = cr.dst_size;
+            r.blocks += cr.blocks; r.raw_blocks += cr.raw_blocks; r.rle_blocks += cr.rle_blocks;
+        }
+        uint8_t *start = body;
+        if (k == 0) { start -= FC_HEADER; fc_header(start, fc->checksum); }
+        if (final) len += fc_trailer(body + len, out_n[s] % ENC_BLOCK == 0, fc->checksum, h, r);
+        const size_t w = (size_t)(body + len - start);
+        if (!fc_write(wr, wu, start, w)) return fc_panic(c, "FrameCompressor::compress: the drain's write failed");
+        r.dst_size += w;
+        return 0;
+    };
+    int e = 0;
+    if (!fc_read(rd, ru, fc->h_in[0].p, C, &n[0], &eof[0])) e = fc_panic(c, "FrameCompressor::compress: the source's read failed");
+    else h.update(fc->h_in[0].p, n[0]);
+    for (uint64_t k = 0; !e; k++) {
+        const int s = (int)(k & 1);
+        out_n[s] = n[s];
+        if (n[s] && (e = enqueue(k, s))) break;
+        if (!eof[s]) {   // read chunk k + 1 into the other slot once chunk k - 1's upload is done with it
+            if (k && cudaEventSynchronize(fc->ev_h2d[s ^ 1]) != cudaSuccess) { e = c->set_cuda_err(cudaGetLastError(), "upload"); break; }
+            if (!fc_read(rd, ru, fc->h_in[s ^ 1].p, C, &n[s ^ 1], &eof[s ^ 1])) { e = fc_panic(c, "FrameCompressor::compress: the source's read failed"); break; }
+            h.update(fc->h_in[s ^ 1].p, n[s ^ 1]);
+        }
+        if (k && (e = write_chunk(k - 1, s ^ 1, false))) break;
+        if (eof[s]) { e = write_chunk(k, s, true); break; }
+    }
+    if (e) {   // leave nothing in flight: the buffers are reused by the next compress
+        cudaStreamSynchronize(fc->s_h2d);
+        cudaStreamSynchronize(ks);
+        cudaStreamSynchronize(fc->s_d2h);
+    }
+    return e;
+}
+
+extern "C" int b200z_frame_compressor_compress(b200z_frame_compressor *fc, b200z_read_fn rd, void *ru, b200z_write_fn wr, void *wu,
+                                               b200z_compress_result *result) {
+    if (!fc || !rd || !wr) return B200Z_ERR_INVALID_ARGUMENT;
+    b200z_ctx *c = fc->ctx;
+    if (fc->level >= 2) return fc_panic(c, "FrameCompressor::compress: compression levels above Fastest are unimplemented!() in the reference");
+    b200z_compress_result r{};
+    XXH64State h;
+    h.reset();
+    int e = 0;
+    if (fc->level == B200Z_LEVEL_UNCOMPRESSED) e = fc_compress_raw(fc, rd, ru, wr, wu, h, r);
+    else if (!(e = c->use())) e = fc_compress_fast(fc, rd, ru, wr, wu, h, r);
+    r.status = e;
+    if (result) *result = r;
+    return e;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // raw-content dictionary trainer (EXTENSION in place of ruzstd::dictionary, DESIGN.md section 4.5): host checks and the epoch
 // plan, then k_dtcount -> k_dtprev -> one k_dtepoch per epoch on the ctx stream; the chosen segments' bytes are then gathered
 // into the host dictionary by ascending score

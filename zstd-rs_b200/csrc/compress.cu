@@ -4,6 +4,7 @@
 //   k_cenc      : one warp per block: Huffman literals, FSE sequences, the Raw / RLE / Compressed decision (encode.cuh)
 //   k_cxxh64    : content checksum of every frame's input (xxh64.cuh; four serial chains per frame)
 //   k_cassemble : one CTA per block: frame header, the block at its prefix-summed offset, the checksum, per-frame results
+//                 (<true>: one chunk of a streamed frame, blocks only; the host writes header, trailer and checksum)
 //   k_cdict     : not a stage: the match table of a dictionary, built once the first time the dictionary is used (EXTENSION)
 //   k_dstats    : not a stage: literal and sequence-code histograms of k_cmatch's parse, for b200z_dict_finalize (EXTENSION)
 //
@@ -202,7 +203,11 @@ __global__ void k_cxxh64(const CFrame *__restrict__ frames, const uint8_t *__res
 // ------------------------------------------------------------------------------------------------------------
 // k_cassemble: one CTA per block.  Its offset inside the frame is the sum of the sizes of the blocks before it (read by the
 // whole CTA); the first block also writes the frame header, the last one the checksum and the frame's result.
+// With STREAM (b200z_frame_compressor) a CFrame is one chunk of a frame whose header, trailing empty block and checksum the host
+// writes: the blocks are packed from the chunk's dst_off, and only a chunk that ends inside a block (the source ended there)
+// sets the last-block bit on its last block.  Its result holds the chunk's packed size and block counts.
 // ------------------------------------------------------------------------------------------------------------
+template <bool STREAM>
 __global__ void __launch_bounds__(256)
 k_cassemble(const CFrame *__restrict__ frames, const CBlock *__restrict__ blocks, const CBlockInfo *__restrict__ res, const uint8_t *__restrict__ enc,
             const uint8_t *__restrict__ input, const uint64_t *__restrict__ csum, uint8_t *__restrict__ output, b200z_compress_result *__restrict__ results,
@@ -211,9 +216,10 @@ k_cassemble(const CFrame *__restrict__ frames, const CBlock *__restrict__ blocks
     const uint32_t b = blockIdx.x, tid = threadIdx.x;
     const CBlock blk = blocks[b];
     const CFrame fr = frames[blk.frame];
-    const bool last = b == fr.first_block + fr.nblocks - 1;
+    const bool end = b == fr.first_block + fr.nblocks - 1;   // the CFrame's last block
+    const bool last = end && (!STREAM || fr.src_size % ENC_BLOCK != 0);
     uint64_t before = 0, nraw = 0, nrle = 0;
-    for (uint32_t i = fr.first_block + tid; i < b + (last ? 1u : 0u); i += 256) {
+    for (uint32_t i = fr.first_block + tid; i < b + (end ? 1u : 0u); i += 256) {
         const uint32_t t = level == 0 ? 0u : res[i].type;
         const uint32_t sz = 3 + (t == 0 ? blocks[i].size : t == 1 ? 1u : res[i].csize);
         if (i < b) before += sz;
@@ -229,7 +235,7 @@ k_cassemble(const CFrame *__restrict__ frames, const CBlock *__restrict__ blocks
     __syncthreads();
     before = nraw = nrle = 0;
     for (int i = 0; i < 8; i++) { before += s_red[0][i]; nraw += s_red[1][i]; nrle += s_red[2][i]; }
-    const uint32_t hdr = frame_header_size(fr.src_size, dict_id);
+    const uint32_t hdr = STREAM ? 0u : frame_header_size(fr.src_size, dict_id);
     uint8_t *dst = output + fr.dst_off + hdr + before;
     const uint32_t type = level == 0 ? 0u : res[b].type;
     const uint32_t csize = type == 0 ? blk.size : type == 1 ? 1u : res[b].csize;
@@ -237,16 +243,17 @@ k_cassemble(const CFrame *__restrict__ frames, const CBlock *__restrict__ blocks
     if (tid == 0) {
         const uint32_t bh = (last ? 1u : 0u) | (type << 1) | ((type == 1 ? blk.size : csize) << 3);
         dst[0] = (uint8_t)bh; dst[1] = (uint8_t)(bh >> 8); dst[2] = (uint8_t)(bh >> 16);
-        if (b == fr.first_block) write_frame_header(output + fr.dst_off, fr.src_size, checksum != 0, dict_id);
+        if (!STREAM && b == fr.first_block) write_frame_header(output + fr.dst_off, fr.src_size, checksum != 0, dict_id);
     }
     for (uint32_t i = tid; i < csize; i += 256) dst[3 + i] = from[i];
-    if (last && tid == 0) {
-        const uint32_t c = checksum ? (uint32_t)csum[blk.frame] : 0u;
+    if (end && tid == 0) {
+        const bool sum = !STREAM && checksum;
+        const uint32_t c = sum ? (uint32_t)csum[blk.frame] : 0u;
         uint64_t size = hdr + before + 3 + csize;
-        if (checksum) { for (int i = 0; i < 4; i++) dst[3 + csize + i] = (uint8_t)(c >> (8 * i)); size += 4; }
+        if (sum) { for (int i = 0; i < 4; i++) dst[3 + csize + i] = (uint8_t)(c >> (8 * i)); size += 4; }
         b200z_compress_result r;
         r.dst_size = size; r.status = 0; r.blocks = fr.nblocks; r.raw_blocks = (uint32_t)nraw; r.rle_blocks = (uint32_t)nrle;
-        r.has_checksum = checksum ? 1u : 0u; r.checksum = c;
+        r.has_checksum = sum ? 1u : 0u; r.checksum = c;
         results[blk.frame] = r;
     }
 }
@@ -335,9 +342,19 @@ int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s, uint
         else k_cenc<false><<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res, nullptr);
         break;
     case 2: if (!a.checksum || !a.nframes) return 0; k_cxxh64<<<cdiv_u((uint64_t)a.nframes * 4, 128), 128, 0, s>>>(a.frames, a.input, a.csum, a.nframes); break;
-    case 3: if (!a.nblocks) return 0; k_cassemble<<<a.nblocks, 256, 0, s>>>(a.frames, a.blocks, a.res, a.enc, a.input, a.csum, a.output, a.results, a.level, a.checksum, a.dict_id); break;
+    case 3: if (!a.nblocks) return 0; k_cassemble<false><<<a.nblocks, 256, 0, s>>>(a.frames, a.blocks, a.res, a.enc, a.input, a.csum, a.output, a.results, a.level, a.checksum, a.dict_id); break;
     default: return (int)cudaErrorInvalidValue;
     }
+    const int e = (int)cudaGetLastError();
+    if (!e) ++*launched;
+    return e;
+}
+
+int launch_compress_chunk(const CompressArgs &a, cudaStream_t s, uint64_t *launched) {
+    if (!a.nblocks) return 0;
+    for (int st = 0; st < 2; st++)
+        if (int e = launch_compress_stage(a, st, s, launched)) return e;
+    k_cassemble<true><<<a.nblocks, 256, 0, s>>>(a.frames, a.blocks, a.res, a.enc, a.input, nullptr, a.output, a.results, a.level, 0, 0);
     const int e = (int)cudaGetLastError();
     if (!e) ++*launched;
     return e;

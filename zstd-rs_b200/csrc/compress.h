@@ -71,5 +71,8 @@ int dict_from_counts(const uint64_t *counts, const uint8_t *content, size_t cont
 constexpr int kCompressStages = 4;
 extern const char *const kCompressStageNames[kCompressStages];
 int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s, uint64_t *launched);   // adds the kernels it enqueued to *launched
+// one chunk of a streamed frame (b200z_frame_compressor, Fastest): k_cmatch, k_cenc, k_cassemble<true> over a.blocks[a.nblocks],
+// which all belong to a.frames[0] (the chunk); no dictionary, no checksum kernel.  Adds the kernels it enqueued to *launched
+int launch_compress_chunk(const CompressArgs &a, cudaStream_t s, uint64_t *launched);
 
 }  // namespace b200z
