@@ -118,19 +118,36 @@ def nominal_size(blocks):
     return n
 
 
-def frame(blocks, window_log=17, content_size=True, checksum=False, ov=False):
+def frame(blocks, window_log=17, content_size=True, checksum=False, ov=False, plain=None, dict_id=None, dict_id_bytes=4,
+          single_segment=False, window_desc=None):
     """The frame's bytes, and (huffman literals 0/1, [LL, OF, ML] modes) of each Compressed block.  content_size: True = the
     reference's content size (omitted for an error case), None = no Frame_Content_Size field, or a number.  checksum: append
-    the content checksum (XXH64 of the reference's content)."""
-    plain = execute(blocks, ov)
+    the content checksum (XXH64 of the reference's content).  plain: the content, when `execute` cannot tell it (a frame that
+    reaches into a dictionary).  dict_id: a Dictionary_ID field of dict_id_bytes (1, 2 or 4) bytes.  single_segment: no
+    Window_Descriptor, the window is the content size.  window_desc: the Window_Descriptor byte (exponent and mantissa)."""
+    if plain is None:
+        plain = execute(blocks, ov)
     if content_size is True:
         content_size = None if plain is ERROR else len(plain)
     fhd = (4 if checksum else 0)
     fcs = b""
     if content_size is not None:
-        fcs = struct.pack("<I", content_size) if content_size < 1 << 32 else struct.pack("<Q", content_size)
-        fhd |= (2 if len(fcs) == 4 else 3) << 6
-    out = struct.pack("<IBB", 0xFD2FB528, fhd, (window_log - 10) << 3) + fcs
+        if single_segment and content_size < 256:
+            fcs = struct.pack("<B", content_size)
+        else:
+            fcs = struct.pack("<I", content_size) if content_size < 1 << 32 else struct.pack("<Q", content_size)
+            fhd |= (2 if len(fcs) == 4 else 3) << 6
+    did = b""
+    if dict_id is not None:
+        did = struct.pack("<Q", dict_id)[:dict_id_bytes]
+        assert int.from_bytes(did, "little") == dict_id
+        fhd |= {1: 1, 2: 2, 4: 3}[dict_id_bytes]
+    if single_segment:
+        assert content_size is not None
+        out = struct.pack("<IB", 0xFD2FB528, fhd | 0x20) + did + fcs
+    else:
+        wd = (window_log - 10) << 3 if window_desc is None else window_desc
+        out = struct.pack("<IBB", 0xFD2FB528, fhd, wd) + did + fcs
     encs = []
     for i, b in enumerate(blocks):
         last = 1 if i + 1 == len(blocks) else 0
