@@ -401,6 +401,7 @@ int b200z_frame_decoder_init(b200z_frame_decoder *d, b200z_read_fn read_cb, void
 int b200z_frame_decoder_reset(b200z_frame_decoder *d, b200z_read_fn read_cb, void *user);  /* reset :200 */
 /* on B200Z_ERR_SKIP_FRAME from init/reset: the SkipFrame{length} payload (frame.rs:15-23) */
 uint32_t b200z_frame_decoder_skip_frame_length(const b200z_frame_decoder *d);
+/* a dictionary replaces the one of its ID for the frames reset after the call: the frame in progress keeps the one it started with */
 int b200z_frame_decoder_add_dict(b200z_frame_decoder *d, const uint8_t *raw, size_t len);  /* decode_dict + add_dict :224 */
 int b200z_frame_decoder_add_raw_content_dict(b200z_frame_decoder *d, uint32_t id, const uint8_t *content, size_t len); /* EXTENSION */
 int b200z_frame_decoder_force_dict(b200z_frame_decoder *d, uint32_t dict_id);              /* :229 */

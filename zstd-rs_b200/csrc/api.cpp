@@ -21,6 +21,8 @@
 
 using namespace b200z;
 
+static int ctx_cuda_err(b200z_ctx *c, cudaError_t e, const char *what);   // b200z_ctx::set_cuda_err
+
 // ---------------------------------------------------------------------------------------------------------------
 // small helpers
 // ---------------------------------------------------------------------------------------------------------------
@@ -52,25 +54,63 @@ const ErrName kErrNames[] = {
 };
 #undef EN
 
-struct DevBuf {
+// The owners of the library's CUDA resources: each frees what it holds when it is destroyed, so no path, an error path
+// included, frees by hand.  Buf is device memory (DevBuf) or pinned host memory (PinnedBuf).
+template <bool Pinned> struct Buf {
     void *p = nullptr;
     size_t cap = 0;
-    DevBuf() = default;
-    DevBuf(const DevBuf &) = delete;
-    DevBuf &operator=(const DevBuf &) = delete;
-    ~DevBuf() { release(); }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
-    // contents are NOT preserved
+    Buf() = default;
+    Buf(Buf &&o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    Buf &operator=(Buf &&o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }
+    ~Buf() { release(); }
+    void release() {
+        if (p) Pinned ? cudaFreeHost(p) : cudaFree(p);
+        p = nullptr; cap = 0;
+    }
+    // exactly n bytes in place of what it held; returns CUDA's error, cleared
+    cudaError_t alloc(size_t n) {
+        release();
+        const cudaError_t e = Pinned ? cudaMallocHost(&p, n) : cudaMalloc(&p, n);
+        if (e != cudaSuccess) { p = nullptr; cudaGetLastError(); return e; }
+        cap = n;
+        return cudaSuccess;
+    }
+    // at least n bytes, and at least 1.5 times the old capacity with `grow`; contents are NOT preserved
     int ensure(size_t n, bool grow = true) {
         if (n <= cap) return 0;
-        size_t want = n;
-        if (grow && cap) want = std::max(n, cap + cap / 2);
-        release();
-        if (cudaMalloc(&p, want ? want : 16) != cudaSuccess) { p = nullptr; cudaGetLastError(); return B200Z_ERR_OUT_OF_MEMORY; }
-        cap = want ? want : 16;
-        return 0;
+        return alloc(grow && cap ? std::max(n, cap + cap / 2) : n) == cudaSuccess ? 0 : B200Z_ERR_OUT_OF_MEMORY;
     }
     template <class T> T *as() const { return (T *)p; }
+};
+using DevBuf = Buf<false>;
+using PinnedBuf = Buf<true>;
+
+// A non-blocking stream and an event.  create() returns 0 or B200Z_ERR_CUDA, with the context's error message set.
+struct Stream {
+    cudaStream_t s = nullptr;
+    Stream() = default;
+    Stream(const Stream &) = delete;
+    Stream &operator=(const Stream &) = delete;
+    ~Stream() { if (s) cudaStreamDestroy(s); }
+    int create(b200z_ctx *c, int priority = 0) {   // 0: the default priority
+        const cudaError_t e = cudaStreamCreateWithPriority(&s, cudaStreamNonBlocking, priority);
+        if (e != cudaSuccess) { s = nullptr; return ctx_cuda_err(c, e, "cudaStreamCreateWithPriority"); }
+        return 0;
+    }
+    operator cudaStream_t() const { return s; }
+};
+struct Event {
+    cudaEvent_t e = nullptr;
+    Event() = default;
+    Event(const Event &) = delete;
+    Event &operator=(const Event &) = delete;
+    ~Event() { if (e) cudaEventDestroy(e); }
+    int create(b200z_ctx *c, unsigned flags = cudaEventDisableTiming) {
+        const cudaError_t r = cudaEventCreateWithFlags(&e, flags);
+        if (r != cudaSuccess) { e = nullptr; return ctx_cuda_err(c, r, "cudaEventCreateWithFlags"); }
+        return 0;
+    }
+    operator cudaEvent_t() const { return e; }
 };
 
 }  // namespace
@@ -78,18 +118,23 @@ struct DevBuf {
 // ---------------------------------------------------------------------------------------------------------------
 // context
 // ---------------------------------------------------------------------------------------------------------------
+struct PipeResources;
+struct CompressResources;
+struct DictTrainResources;
+
 struct b200z_ctx {
     int device = 0;
-    cudaStream_t stream = nullptr;
-    cudaStream_t side = nullptr;          // k_huf runs here, beside k_fse
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-    struct PipeResources *pipe = nullptr;  // lazily created by the pipelined one-shot path
-    struct CompressResources *comp = nullptr;   // lazily created by the first compression
-    struct DictTrainResources *dtrain = nullptr;   // lazily created by the first dictionary training
-    FseSlot *d_predef = nullptr;
+    Stream stream;
+    Stream side;                           // k_huf runs here, beside k_fse
+    Event ev_fork, ev_join;
+    DevBuf d_predef;                       // FseSlot: the predefined tables
+    std::unique_ptr<PipeResources> pipe;         // lazily created by the pipelined one-shot path
+    std::unique_ptr<CompressResources> comp;     // lazily created by the first compression
+    std::unique_ptr<DictTrainResources> dtrain;  // lazily created by the first dictionary training
     std::string err;
     uint64_t launches = 0;
     uint32_t flags = 0;
+    ~b200z_ctx();                          // at the end of the file, where the lazily created resources are complete
     int set_cuda_err(cudaError_t e, const char *what) {
         char buf[256];
         snprintf(buf, sizeof buf, "CUDA error in %s: %s", what, cudaGetErrorString(e));
@@ -99,6 +144,7 @@ struct b200z_ctx {
     }
     int use() { cudaError_t e = cudaSetDevice(device); return e == cudaSuccess ? 0 : set_cuda_err(e, "cudaSetDevice"); }
 };
+static int ctx_cuda_err(b200z_ctx *c, cudaError_t e, const char *what) { return c->set_cuda_err(e, what); }
 
 #define CU(ctx, call) do { cudaError_t _e = (call); if (_e != cudaSuccess) return (ctx)->set_cuda_err(_e, #call); } while (0)
 
@@ -118,34 +164,22 @@ extern "C" int b200z_ctx_create(int device, b200z_ctx **out) {
     if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return B200Z_ERR_NO_DEVICE; }
     int prio_lo = 0, prio_hi = 0;
     cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
-    if (cudaStreamCreateWithPriority(&c->stream, cudaStreamNonBlocking, prio_hi) != cudaSuccess) { cudaGetLastError(); return B200Z_ERR_NO_DEVICE; }
-    if (cudaStreamCreateWithPriority(&c->side, cudaStreamNonBlocking, prio_lo) != cudaSuccess || cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming) != cudaSuccess) { cudaGetLastError(); return B200Z_ERR_CUDA; }
-    if (cudaMalloc((void **)&c->d_predef, sizeof(FseSlot)) != cudaSuccess) { cudaGetLastError(); return B200Z_ERR_OUT_OF_MEMORY; }
+    if (c->stream.create(c.get(), prio_hi)) return B200Z_ERR_NO_DEVICE;
+    if (c->side.create(c.get(), prio_lo) || c->ev_fork.create(c.get()) || c->ev_join.create(c.get())) return B200Z_ERR_CUDA;
+    if (int e = c->d_predef.ensure(sizeof(FseSlot), false)) return e;
     if (init_kernels() || init_compress_kernels()) { cudaGetLastError(); return B200Z_ERR_CUDA; }
-    int e = launch_predefined(c->d_predef, c->stream, &c->launches);
+    int e = launch_predefined(c->d_predef.as<FseSlot>(), c->stream, &c->launches);
     if (e || cudaStreamSynchronize(c->stream) != cudaSuccess) { cudaGetLastError(); return B200Z_ERR_CUDA; }
     *out = c.release();
     return 0;
 }
-static void pipe_free(b200z_ctx *c);
-static void compress_free(b200z_ctx *c);
-static void dtrain_free(b200z_ctx *c);
 extern "C" void b200z_ctx_destroy(b200z_ctx *c) {
     if (!c) return;
     cudaSetDevice(c->device);
-    pipe_free(c);
-    compress_free(c);
-    dtrain_free(c);
-    if (c->d_predef) cudaFree(c->d_predef);
-    if (c->ev_fork) cudaEventDestroy(c->ev_fork);
-    if (c->ev_join) cudaEventDestroy(c->ev_join);
-    if (c->side) cudaStreamDestroy(c->side);
-    if (c->stream) cudaStreamDestroy(c->stream);
     delete c;
 }
 extern "C" const char *b200z_ctx_last_error_message(const b200z_ctx *c) { return c ? c->err.c_str() : ""; }
-extern "C" void *b200z_ctx_stream(const b200z_ctx *c) { return c ? (void *)c->stream : nullptr; }
+extern "C" void *b200z_ctx_stream(const b200z_ctx *c) { return c ? (void *)c->stream.s : nullptr; }
 extern "C" uint64_t b200z_ctx_kernel_launches(const b200z_ctx *c) { return c ? c->launches : 0; }
 extern "C" void b200z_ctx_set_flags(b200z_ctx *c, uint32_t flags) { if (c) c->flags = flags; }
 extern "C" uint32_t b200z_ctx_flags(const b200z_ctx *c) { return c ? c->flags : 0; }
@@ -159,36 +193,25 @@ struct b200z_dict {
     uint32_t id = 0;
     uint32_t hist[3] = {1, 4, 8};
     bool has_tables = false;
-    HufSlot *d_huf = nullptr;
-    FseSlot *d_fse = nullptr;
-    uint8_t *d_content = nullptr;
+    DevBuf d_huf, d_fse;          // HufSlot, FseSlot
+    DevBuf d_content;             // content_len bytes
     size_t content_len = 0;
-    uint32_t *d_ctab = nullptr;   // the compressor's match table of the content (k_cdict), built by its first compression
-    // a formatted dictionary's tables as parsed (Huffman weights; OF / ML / LL normalized counts by ENC_LL / ENC_OF / ENC_ML), and
-    // the encoder's view of them, built on the host by the first compression with B200Z_FLAG_DICT_TABLES
+    // Built by the first compression that needs them, and stored only once complete.  The compressor's match table of the
+    // content (k_cdict); a formatted dictionary's tables as parsed (Huffman weights; OF / ML / LL normalized counts by ENC_LL /
+    // ENC_OF / ENC_ML), and the encoder's view of them (EncDict), built on the host for B200Z_FLAG_DICT_TABLES
+    mutable DevBuf d_ctab;
     uint8_t huf_weights[260] = {};
     uint32_t huf_nweights = 0;
     int16_t norm[3][64] = {};
     uint32_t nnorm[3] = {}, log[3] = {};
-    EncDict *d_enc = nullptr;
+    mutable DevBuf d_enc;
 };
-
-static void dict_free(b200z_dict *d) {
-    if (!d) return;
-    cudaSetDevice(d->ctx->device);
-    if (d->d_huf) cudaFree(d->d_huf);
-    if (d->d_fse) cudaFree(d->d_fse);
-    if (d->d_content) cudaFree(d->d_content);
-    if (d->d_ctab) cudaFree(d->d_ctab);
-    if (d->d_enc) cudaFree(d->d_enc);
-    delete d;
-}
 
 static int dict_upload_content(b200z_dict *d, const uint8_t *content, size_t len) {
     b200z_ctx *c = d->ctx;
     d->content_len = len;
-    CU(c, cudaMalloc((void **)&d->d_content, len + 16));
-    if (len) CU(c, cudaMemcpy(d->d_content, content, len, cudaMemcpyHostToDevice));
+    CU(c, d->d_content.alloc(len + 16));
+    if (len) CU(c, cudaMemcpy(d->d_content.p, content, len, cudaMemcpyHostToDevice));
     return 0;
 }
 
@@ -202,7 +225,7 @@ extern "C" int b200z_dict_create(b200z_ctx *c, const uint8_t *raw, size_t len, b
     if (len < 8) return B200Z_ERR_DICT_NOT_ENOUGH_BYTES;
     static const uint8_t magic[4] = {0x37, 0xA4, 0x30, 0xEC};
     if (memcmp(raw, magic, 4) != 0) return B200Z_ERR_DICT_BAD_MAGIC_NUM;
-    std::unique_ptr<b200z_dict, void (*)(b200z_dict *)> d(new b200z_dict(), dict_free);
+    std::unique_ptr<b200z_dict> d(new b200z_dict());
     d->ctx = c;
     d->id = rd32le(raw + 4);
     const uint8_t *t = raw + 8;
@@ -237,10 +260,10 @@ extern "C" int b200z_dict_create(b200z_ctx *c, const uint8_t *raw, size_t len, b
     if (tl < 12) return B200Z_ERR_DICT_NOT_ENOUGH_BYTES;
     for (int i = 0; i < 3; i++) d->hist[i] = rd32le(t + 4 * i);
     d->has_tables = true;
-    CU(c, cudaMalloc((void **)&d->d_huf, sizeof(HufSlot)));
-    CU(c, cudaMalloc((void **)&d->d_fse, sizeof(FseSlot)));
-    CU(c, cudaMemcpy(d->d_huf, huf.get(), sizeof(HufSlot), cudaMemcpyHostToDevice));
-    CU(c, cudaMemcpy(d->d_fse, fse.get(), sizeof(FseSlot), cudaMemcpyHostToDevice));
+    CU(c, d->d_huf.alloc(sizeof(HufSlot)));
+    CU(c, d->d_fse.alloc(sizeof(FseSlot)));
+    CU(c, cudaMemcpy(d->d_huf.p, huf.get(), sizeof(HufSlot), cudaMemcpyHostToDevice));
+    CU(c, cudaMemcpy(d->d_fse.p, fse.get(), sizeof(FseSlot), cudaMemcpyHostToDevice));
     if ((e = dict_upload_content(d.get(), t + 12, tl - 12))) return e;
     *out = d.release();
     return 0;
@@ -249,7 +272,7 @@ extern "C" int b200z_dict_create_raw_content(b200z_ctx *c, uint32_t id, const ui
     if (!c || !out || (!content && len)) return B200Z_ERR_INVALID_ARGUMENT;
     *out = nullptr;
     if (int e = c->use()) return e;
-    std::unique_ptr<b200z_dict, void (*)(b200z_dict *)> d(new b200z_dict(), dict_free);
+    std::unique_ptr<b200z_dict> d(new b200z_dict());
     d->ctx = c; d->id = id;
     if (int e = dict_upload_content(d.get(), content, len)) return e;
     *out = d.release();
@@ -258,7 +281,11 @@ extern "C" int b200z_dict_create_raw_content(b200z_ctx *c, uint32_t id, const ui
 extern "C" uint32_t b200z_dict_id(const b200z_dict *d) { return d ? d->id : 0; }
 extern "C" int b200z_dict_offset_history(const b200z_dict *d, uint32_t out[3]) { if (!d) return B200Z_ERR_INVALID_ARGUMENT; memcpy(out, d->hist, 12); return 0; }
 extern "C" size_t b200z_dict_content_size(const b200z_dict *d) { return d ? d->content_len : 0; }
-extern "C" void b200z_dict_destroy(b200z_dict *d) { dict_free(d); }
+extern "C" void b200z_dict_destroy(b200z_dict *d) {
+    if (!d) return;
+    cudaSetDevice(d->ctx->device);
+    delete d;
+}
 
 // ---------------------------------------------------------------------------------------------------------------
 // A "submission": host-side plan + its device mirror.  Used by the batch entry (many frames, fresh state) and
@@ -283,7 +310,10 @@ void cursor_from_carry(TableCursor &cur, const CarrySet &cs, uint32_t carry_idx)
 CarrySet carry_of_dict(const b200z_dict *d) {
     CarrySet cs;
     cs.dict = d;
-    if (d && d->has_tables) { cs.huf = d->d_huf; cs.ll = &d->d_fse->ll; cs.of = &d->d_fse->of; cs.ml = &d->d_fse->ml; }
+    if (d && d->has_tables) {
+        const FseSlot *f = d->d_fse.as<FseSlot>();
+        cs.huf = d->d_huf.as<HufSlot>(); cs.ll = &f->ll; cs.of = &f->of; cs.ml = &f->ml;
+    }
     return cs;
 }
 
@@ -318,7 +348,7 @@ struct Submission {
         FrameDesc fd;
         memset(&fd, 0, sizeof fd);
         fd.out_off = out_off; fd.out_cap = out_cap; fd.window_size = window;
-        fd.dict = dict ? dict->d_content : nullptr; fd.dict_len = dict ? dict->content_len : 0;
+        fd.dict = dict ? dict->d_content.as<uint8_t>() : nullptr; fd.dict_len = dict ? dict->content_len : 0;
         fd.first_block = (uint32_t)descs.size();
         FrameState st;
         memset(&st, 0, sizeof st);
@@ -396,7 +426,7 @@ struct Submission {
         if ((e = d_sched.ensure(2 * (16 + 4 * frames.size()) + 4 * cta_frames.size() + 32))) return e;
         HufSlot *hs = d_huf.as<HufSlot>();
         FseSlot *fs = d_fse.as<FseSlot>();
-        const FseSlot *pd = c->d_predef;
+        const FseSlot *pd = c->d_predef.as<FseSlot>();
         for (size_t i = 0; i < descs.size(); i++) {
             BlockDesc &d = descs[i];
             const BlockRefs &r = refs[i];
@@ -695,8 +725,8 @@ extern "C" int b200z_batch_run_profile(b200z_batch *b, uint8_t *d_output, size_t
     if (int e = c->use()) return e;
     if (int e = restore_states(b)) return e;
     PipelineArgs a = b->sub.args(b->d_input, d_output, output_cap);
-    cudaEvent_t ev[kNumStages + 1];
-    for (auto &e : ev) CU(c, cudaEventCreate(&e));
+    Event ev[kNumStages + 1];
+    for (Event &e : ev) if (e.create(c, cudaEventDefault)) return B200Z_ERR_CUDA;
     if (int e = reset_sched(a, c->stream)) return c->set_cuda_err((cudaError_t)e, "reset_sched");
     CU(c, cudaEventRecord(ev[0], c->stream));
     for (int st = 0; st < kNumStages; st++) {
@@ -706,7 +736,6 @@ extern "C" int b200z_batch_run_profile(b200z_batch *b, uint8_t *d_output, size_t
     }
     CU(c, cudaStreamSynchronize(c->stream));
     for (int st = 0; st < kNumStages && (size_t)st < nstages; st++) CU(c, cudaEventElapsedTime(&stage_ms[st], ev[st], ev[st + 1]));
-    for (auto &e : ev) cudaEventDestroy(e);
     b->ran = true;
     return 0;
 }
@@ -720,8 +749,8 @@ extern "C" int b200z_batch_run_timeline(b200z_batch *b, uint8_t *d_output, size_
     if (int e = restore_states(b)) return e;
     PipelineArgs a = b->sub.args(b->d_input, d_output, output_cap);
     if (int e = reset_sched(a, c->stream)) return c->set_cuda_err((cudaError_t)e, "reset_sched");
-    cudaEvent_t ev[5];
-    for (auto &e : ev) CU(c, cudaEventCreate(&e));
+    Event ev[5];
+    for (Event &e : ev) if (e.create(c, cudaEventDefault)) return B200Z_ERR_CUDA;
     CU(c, cudaStreamSynchronize(c->stream));
     CU(c, cudaEventRecord(ev[0], c->stream));
     PipelineStreams ps{c->stream, c->side, c->ev_fork, c->ev_join};
@@ -735,7 +764,6 @@ extern "C" int b200z_batch_run_timeline(b200z_batch *b, uint8_t *d_output, size_
     if (le) return c->set_cuda_err((cudaError_t)le, "launch_stage");
     CU(c, cudaStreamSynchronize(c->stream));
     for (int i = 0; i < 4; i++) CU(c, cudaEventElapsedTime(&out_ms[i], ev[0], ev[i + 1]));
-    for (auto &e : ev) cudaEventDestroy(e);
     return 0;
 }
 // host-only views of the scheduling decisions (plan.cpp), for CPU tests: no context, no device
@@ -895,59 +923,33 @@ extern "C" void b200z_batch_destroy(b200z_batch *b) {
 // reused across calls.
 // ---------------------------------------------------------------------------------------------------------------
 struct PipeResources {
-    cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
+    Stream s_h2d, s_d2h;
     // chunk i's kernels run on stream pair i & 1, so the (latency-bound) kernels of neighbouring chunks overlap
-    cudaStream_t k_main[2] = {nullptr, nullptr}, k_side[2] = {nullptr, nullptr};
-    cudaEvent_t k_fork[2] = {nullptr, nullptr}, k_join[2] = {nullptr, nullptr};
-    b200z_batch *set[2] = {nullptr, nullptr};
-    cudaEvent_t ev_h2d[2] = {nullptr, nullptr}, ev_k[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr};
-    FrameState *h_states[2] = {nullptr, nullptr};   // pinned
-    size_t h_states_cap[2] = {0, 0};
+    Stream k_main[2], k_side[2];
+    Event k_fork[2], k_join[2];
+    std::unique_ptr<b200z_batch> set[2];
+    Event ev_h2d[2], ev_k[2], ev_done[2];
+    PinnedBuf h_states[2];   // FrameState
     DevBuf d_in[2];
     DevBuf d_out;
 };
 
-static void pipe_free(b200z_ctx *c) {
-    PipeResources *p = c->pipe;
-    if (!p) return;
-    for (int i = 0; i < 2; i++) {
-        if (p->set[i]) delete p->set[i];
-        if (p->ev_h2d[i]) cudaEventDestroy(p->ev_h2d[i]);
-        if (p->ev_k[i]) cudaEventDestroy(p->ev_k[i]);
-        if (p->ev_done[i]) cudaEventDestroy(p->ev_done[i]);
-        if (p->k_fork[i]) cudaEventDestroy(p->k_fork[i]);
-        if (p->k_join[i]) cudaEventDestroy(p->k_join[i]);
-        if (p->k_main[i]) cudaStreamDestroy(p->k_main[i]);
-        if (p->k_side[i]) cudaStreamDestroy(p->k_side[i]);
-        if (p->h_states[i]) cudaFreeHost(p->h_states[i]);
-    }
-    if (p->s_h2d) cudaStreamDestroy(p->s_h2d);
-    if (p->s_d2h) cudaStreamDestroy(p->s_d2h);
-    delete p;
-    c->pipe = nullptr;
-}
-
 static int pipe_get(b200z_ctx *c, PipeResources **out) {
     if (!c->pipe) {
         std::unique_ptr<PipeResources> p(new PipeResources());
-        CU(c, cudaStreamCreateWithFlags(&p->s_h2d, cudaStreamNonBlocking));
-        CU(c, cudaStreamCreateWithFlags(&p->s_d2h, cudaStreamNonBlocking));
+        if (p->s_h2d.create(c) || p->s_d2h.create(c)) return B200Z_ERR_CUDA;
         int prio_lo = 0, prio_hi = 0;
         cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
         for (int i = 0; i < 2; i++) {
-            CU(c, cudaStreamCreateWithPriority(&p->k_main[i], cudaStreamNonBlocking, prio_hi));
-            CU(c, cudaStreamCreateWithPriority(&p->k_side[i], cudaStreamNonBlocking, prio_lo));
-            CU(c, cudaEventCreateWithFlags(&p->k_fork[i], cudaEventDisableTiming));
-            CU(c, cudaEventCreateWithFlags(&p->k_join[i], cudaEventDisableTiming));
-            p->set[i] = new b200z_batch();
+            if (p->k_main[i].create(c, prio_hi) || p->k_side[i].create(c, prio_lo) || p->k_fork[i].create(c) || p->k_join[i].create(c) ||
+                p->ev_h2d[i].create(c) || p->ev_k[i].create(c) || p->ev_done[i].create(c))
+                return B200Z_ERR_CUDA;
+            p->set[i].reset(new b200z_batch());
             p->set[i]->ctx = c;
-            CU(c, cudaEventCreateWithFlags(&p->ev_h2d[i], cudaEventDisableTiming));
-            CU(c, cudaEventCreateWithFlags(&p->ev_k[i], cudaEventDisableTiming));
-            CU(c, cudaEventCreateWithFlags(&p->ev_done[i], cudaEventDisableTiming));
         }
-        c->pipe = p.release();
+        c->pipe = std::move(p);
     }
-    *out = c->pipe;
+    *out = c->pipe.get();
     return 0;
 }
 
@@ -974,10 +976,10 @@ static int decode_frames_pipelined(b200z_ctx *c, const uint8_t *input, size_t in
     auto retire = [&](int s) -> int {   // results of the chunk that used set s
         if (!pend[s].live) return 0;
         CU(c, cudaEventSynchronize(p->ev_done[s]));
-        b200z_batch *b = p->set[s];
+        const b200z_batch *b = p->set[s].get();
         for (size_t i = pend[s].f0; i < pend[s].f1; i++) {
             int32_t sf = b->info[i - pend[s].f0].sub_frame;
-            fill_result(b, i - pend[s].f0, sf >= 0 ? &p->h_states[s][sf] : nullptr, results[i]);
+            fill_result(b, i - pend[s].f0, sf >= 0 ? p->h_states[s].as<FrameState>() + sf : nullptr, results[i]);
         }
         pend[s].live = false;
         return 0;
@@ -986,7 +988,7 @@ static int decode_frames_pipelined(b200z_ctx *c, const uint8_t *input, size_t in
         const int s = (int)(ci & 1);
         const size_t f0 = cut[ci], f1 = cut[ci + 1];
         if (int e = retire(s)) return e;
-        b200z_batch *b = p->set[s];
+        b200z_batch *b = p->set[s].get();
         if (int e = plan_batch(b, input, input_len, frames + f0, f1 - f0, dicts, ndicts, forced, max_window)) return e;
         // input byte range and output byte range of this chunk
         uint64_t ilo = UINT64_MAX, ihi = 0, olo = UINT64_MAX, ohi = 0;
@@ -1009,13 +1011,8 @@ static int decode_frames_pipelined(b200z_ctx *c, const uint8_t *input, size_t in
         CU(c, cudaEventRecord(p->ev_k[s], km));
         CU(c, cudaStreamWaitEvent(p->s_d2h, p->ev_k[s], 0));
         size_t nst = b->sub.states.size();
-        if (nst > p->h_states_cap[s]) {
-            if (p->h_states[s]) cudaFreeHost(p->h_states[s]);
-            p->h_states[s] = nullptr; p->h_states_cap[s] = 0;
-            CU(c, cudaMallocHost((void **)&p->h_states[s], (nst + nst / 2 + 16) * sizeof(FrameState)));
-            p->h_states_cap[s] = nst + nst / 2 + 16;
-        }
-        if (nst) CU(c, cudaMemcpyAsync(p->h_states[s], b->sub.d_states.p, nst * sizeof(FrameState), cudaMemcpyDeviceToHost, p->s_d2h));
+        if (int e = p->h_states[s].ensure(nst * sizeof(FrameState))) return e;
+        if (nst) CU(c, cudaMemcpyAsync(p->h_states[s].p, b->sub.d_states.p, nst * sizeof(FrameState), cudaMemcpyDeviceToHost, p->s_d2h));
         if (ohi > olo) CU(c, cudaMemcpyAsync(output + olo, d_out + olo, ohi - olo, cudaMemcpyDeviceToHost, p->s_d2h));
         CU(c, cudaEventRecord(p->ev_done[s], p->s_d2h));
         pend[s].f0 = f0; pend[s].f1 = f1; pend[s].live = true;
@@ -1420,7 +1417,7 @@ extern "C" int b200z_decode_blocks_batch(b200z_ctx *c, const b200z_block_desc *b
 struct b200z_frame_decoder {
     b200z_ctx *ctx = nullptr;
     uint64_t max_window = B200Z_DEFAULT_MAX_WINDOW_SIZE;
-    std::map<uint32_t, b200z_dict *> dicts;           // FrameDecoder.dicts (BTreeMap<u32, Dictionary>), owned
+    std::map<uint32_t, std::shared_ptr<b200z_dict>> dicts;   // FrameDecoder.dicts (BTreeMap<u32, Dictionary>)
     // FrameDecoderState (frame_decoder.rs:86-94)
     bool has_state = false;
     FrameHeader hdr;
@@ -1430,7 +1427,9 @@ struct b200z_frame_decoder {
     uint64_t bytes_read_counter = 0;
     bool has_check_sum = false;
     uint32_t check_sum = 0;
-    const b200z_dict *using_dict = nullptr;
+    // the dictionary the frame started with, kept until the next reset even when add_dict replaces it (the reference copies it
+    // into the frame's scratch, DecoderScratch::init_from_dict)
+    std::shared_ptr<const b200z_dict> using_dict;
     uint32_t skip_len = 0;
     int last_stage = 0;
     std::string err;
@@ -1441,8 +1440,7 @@ struct b200z_frame_decoder {
     FrameState state;                                  // host mirror of the device-side frame state
     XXH64State hash;                                   // decode_buffer.rs:16, fed on drain
     // "current tables" (DecoderScratch.huf/.fse): which kinds exist + persistent device copies
-    HufSlot *d_carry_huf = nullptr;
-    FseSlot *d_carry_fse = nullptr;
+    DevBuf d_carry_huf, d_carry_fse;                   // HufSlot, FseSlot
     CarrySet carry;                                    // what the next submission starts from
     Submission sub;
     DevBuf d_input;
@@ -1465,17 +1463,14 @@ extern "C" int b200z_frame_decoder_new(b200z_ctx *c, b200z_frame_decoder **out) 
     d->ctx = c;
     memset(&d->state, 0, sizeof d->state);
     d->hash.reset();
-    CU(c, cudaMalloc((void **)&d->d_carry_huf, sizeof(HufSlot)));
-    CU(c, cudaMalloc((void **)&d->d_carry_fse, sizeof(FseSlot)));
+    CU(c, d->d_carry_huf.alloc(sizeof(HufSlot)));
+    CU(c, d->d_carry_fse.alloc(sizeof(FseSlot)));
     *out = d.release();
     return 0;
 }
 extern "C" void b200z_frame_decoder_free(b200z_frame_decoder *d) {
     if (!d) return;
     cudaSetDevice(d->ctx->device);
-    for (auto &kv : d->dicts) dict_free(kv.second);
-    if (d->d_carry_huf) cudaFree(d->d_carry_huf);
-    if (d->d_carry_fse) cudaFree(d->d_carry_fse);
     delete d;
 }
 extern "C" void b200z_frame_decoder_set_max_window_size(b200z_frame_decoder *d, uint64_t n) {
@@ -1493,10 +1488,10 @@ static size_t read_upto(b200z_read_fn rd, void *user, uint8_t *buf, size_t n) { 
 }
 static bool read_exact(b200z_read_fn rd, void *user, uint8_t *buf, size_t n) { return read_upto(rd, user, buf, n) == n; }
 
-static void fd_apply_dict(b200z_frame_decoder *d, const b200z_dict *dict) {  // DecoderScratch::init_from_dict, scratch.rs:70-78
-    d->carry = carry_of_dict(dict);
+static void fd_apply_dict(b200z_frame_decoder *d, std::shared_ptr<const b200z_dict> dict) {  // DecoderScratch::init_from_dict, scratch.rs:70-78
+    d->carry = carry_of_dict(dict.get());
     d->state.hist[0] = dict->hist[0]; d->state.hist[1] = dict->hist[1]; d->state.hist[2] = dict->hist[2];
-    d->using_dict = dict;
+    d->using_dict = std::move(dict);
 }
 
 // reset (frame_decoder.rs:200-221): read the header through the callback as read_frame_header does -- the magic number, then the
@@ -1535,23 +1530,24 @@ extern "C" int b200z_frame_decoder_reset(b200z_frame_decoder *d, b200z_read_fn r
 }
 extern "C" int b200z_frame_decoder_init(b200z_frame_decoder *d, b200z_read_fn rd, void *user) { return b200z_frame_decoder_reset(d, rd, user); }
 
+// add_dict / add_raw_content_dict: `x` (created with error e) replaces a dictionary of the same ID for the frames that start
+// after this call; the frame in progress keeps the one it started with
+static int fd_add_dict(b200z_frame_decoder *d, int e, b200z_dict *x) {
+    if (e) return fd_fail(d, e, B200Z_STAGE_DICTIONARY);
+    d->dicts[x->id] = std::shared_ptr<b200z_dict>(x, b200z_dict_destroy);
+    return 0;
+}
 extern "C" int b200z_frame_decoder_add_dict(b200z_frame_decoder *d, const uint8_t *raw, size_t len) {
     if (!d) return B200Z_ERR_INVALID_ARGUMENT;
     b200z_dict *x = nullptr;
-    int e = b200z_dict_create(d->ctx, raw, len, &x);
-    if (e) return fd_fail(d, e, B200Z_STAGE_DICTIONARY);
-    auto it = d->dicts.find(x->id);
-    if (it != d->dicts.end()) { if (d->using_dict == it->second) d->using_dict = nullptr; dict_free(it->second); it->second = x; } else d->dicts[x->id] = x;
-    return 0;
+    const int e = b200z_dict_create(d->ctx, raw, len, &x);
+    return fd_add_dict(d, e, x);
 }
 extern "C" int b200z_frame_decoder_add_raw_content_dict(b200z_frame_decoder *d, uint32_t id, const uint8_t *content, size_t len) {
     if (!d) return B200Z_ERR_INVALID_ARGUMENT;
     b200z_dict *x = nullptr;
-    int e = b200z_dict_create_raw_content(d->ctx, id, content, len, &x);
-    if (e) return fd_fail(d, e, B200Z_STAGE_DICTIONARY);
-    auto it = d->dicts.find(id);
-    if (it != d->dicts.end()) { if (d->using_dict == it->second) d->using_dict = nullptr; dict_free(it->second); it->second = x; } else d->dicts[id] = x;
-    return 0;
+    const int e = b200z_dict_create_raw_content(d->ctx, id, content, len, &x);
+    return fd_add_dict(d, e, x);
 }
 extern "C" int b200z_frame_decoder_force_dict(b200z_frame_decoder *d, uint32_t dict_id) {  // :229-243
     if (!d) return B200Z_ERR_INVALID_ARGUMENT;
@@ -1581,15 +1577,14 @@ static int fd_reserve_out(b200z_frame_decoder *d, uint64_t extra) {
     if (need <= d->d_out.cap) return 0;
     uint64_t want = std::max<uint64_t>(live + extra + 64, (uint64_t)d->d_out.cap + d->d_out.cap / 2);
     want = std::max<uint64_t>(want, 1u << 20);
-    void *np = nullptr;
-    if (cudaMalloc(&np, want) != cudaSuccess) { cudaGetLastError(); return B200Z_ERR_OUT_OF_MEMORY; }
+    DevBuf grown;
+    if (int e = grown.ensure(want, false)) return e;
     if (live) {
-        cudaError_t ce = cudaMemcpyAsync(np, d->d_out.as<uint8_t>() + (d->drained - d->base), live, cudaMemcpyDeviceToDevice, c->stream);
+        cudaError_t ce = cudaMemcpyAsync(grown.p, d->d_out.as<uint8_t>() + (d->drained - d->base), live, cudaMemcpyDeviceToDevice, c->stream);
         if (ce == cudaSuccess) ce = cudaStreamSynchronize(c->stream);
-        if (ce != cudaSuccess) { cudaFree(np); return c->set_cuda_err(ce, "grow output"); }
+        if (ce != cudaSuccess) return c->set_cuda_err(ce, "grow output");
     }
-    d->d_out.release();
-    d->d_out.p = np; d->d_out.cap = want;
+    d->d_out = std::move(grown);
     d->base = d->drained;
     return 0;
 }
@@ -1606,7 +1601,7 @@ static int fd_submit(b200z_frame_decoder *d, const TableCursor &cur, uint32_t *f
     FrameDesc fd;
     memset(&fd, 0, sizeof fd);
     fd.out_off = 0; fd.window_size = d->window;
-    fd.dict = d->using_dict ? d->using_dict->d_content : nullptr; fd.dict_len = d->using_dict ? d->using_dict->content_len : 0;
+    fd.dict = d->using_dict ? d->using_dict->d_content.as<uint8_t>() : nullptr; fd.dict_len = d->using_dict ? d->using_dict->content_len : 0;
     fd.first_block = 0; fd.nblocks = (uint32_t)s.descs.size();
     d->state.produced = d->produced; d->state.drained = d->drained; d->state.blocks_done = 0; d->state.status = 0;
     s.frames.assign(1, fd); s.states.assign(1, d->state);
@@ -1636,21 +1631,22 @@ static int fd_submit(b200z_frame_decoder *d, const TableCursor &cur, uint32_t *f
     // carry the current tables over to the next submission (device-to-device, tables never visit the host)
     CarrySet next;
     if (cur.huf.kind == TabRef::SLOT) {
-        CU(c, cudaMemcpyAsync(d->d_carry_huf, s.d_huf.as<HufSlot>() + cur.huf.idx, sizeof(HufSlot), cudaMemcpyDeviceToDevice, c->stream));
-        next.huf = d->d_carry_huf;
+        CU(c, cudaMemcpyAsync(d->d_carry_huf.p, s.d_huf.as<HufSlot>() + cur.huf.idx, sizeof(HufSlot), cudaMemcpyDeviceToDevice, c->stream));
+        next.huf = d->d_carry_huf.as<HufSlot>();
     } else if (cur.huf.kind == TabRef::CARRY) next.huf = d->carry.huf;
     auto carry_fse = [&](const TabRef &t, int which, FseTab *dst, const FseTab *old) -> const FseTab * {
         const FseTab *src = nullptr;
         if (t.kind == TabRef::SLOT) { const FseSlot *sl = s.d_fse.as<FseSlot>() + t.idx; src = which == 0 ? &sl->ll : (which == 1 ? &sl->of : &sl->ml); }
-        else if (t.kind == TabRef::PREDEF) { const FseSlot *sl = c->d_predef; return which == 0 ? &sl->ll : (which == 1 ? &sl->of : &sl->ml); }
+        else if (t.kind == TabRef::PREDEF) { const FseSlot *sl = c->d_predef.as<FseSlot>(); return which == 0 ? &sl->ll : (which == 1 ? &sl->of : &sl->ml); }
         else if (t.kind == TabRef::CARRY) return old;
         else return nullptr;
         if (cudaMemcpyAsync(dst, src, sizeof(FseTab), cudaMemcpyDeviceToDevice, c->stream) != cudaSuccess) return nullptr;
         return dst;
     };
-    next.ll = carry_fse(cur.ll, 0, &d->d_carry_fse->ll, d->carry.ll);
-    next.of = carry_fse(cur.of, 1, &d->d_carry_fse->of, d->carry.of);
-    next.ml = carry_fse(cur.ml, 2, &d->d_carry_fse->ml, d->carry.ml);
+    FseSlot *cf = d->d_carry_fse.as<FseSlot>();
+    next.ll = carry_fse(cur.ll, 0, &cf->ll, d->carry.ll);
+    next.of = carry_fse(cur.of, 1, &cf->of, d->carry.of);
+    next.ml = carry_fse(cur.ml, 2, &cf->ml, d->carry.ml);
     FrameState st;
     CU(c, cudaMemcpyAsync(&st, s.d_states.p, sizeof(FrameState), cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
@@ -1956,18 +1952,40 @@ extern "C" size_t b200z_compress_bound_dict(size_t n, const b200z_dict *d) { ret
 extern "C" int b200z_compress_num_stages(void) { return kCompressStages; }
 extern "C" const char *b200z_compress_stage_name(int stage) { return stage >= 0 && stage < kCompressStages ? kCompressStageNames[stage] : ""; }
 
+// k_cmatch / k_cenc staging for nblocks blocks (CompressArgs)
+struct CompressStaging {
+    DevBuf lit_stage, seq_stage, lits, seqs, info, res;
+    int ensure(uint64_t nblocks, bool grow) {
+        int e = 0;
+        if ((e = lit_stage.ensure(nblocks * ENC_BLOCK, grow)) || (e = seq_stage.ensure(nblocks * CBLOCK_SEQS * sizeof(SeqRec), grow)) ||
+            (e = lits.ensure(nblocks * ENC_BLOCK, grow)) || (e = seqs.ensure(nblocks * CBLOCK_SEQS * sizeof(SeqRec), grow)) ||
+            (e = info.ensure(nblocks * sizeof(CBlockInfo), grow)) || (e = res.ensure(nblocks * sizeof(CBlockInfo), grow)))
+            return e;
+        return 0;
+    }
+    void bind(CompressArgs &a) const {
+        a.lit_stage = lit_stage.as<uint8_t>(); a.seq_stage = seq_stage.as<SeqRec>(); a.lits = lits.as<uint8_t>(); a.seqs = seqs.as<SeqRec>();
+        a.enc = a.lit_stage; a.info = info.as<CBlockInfo>(); a.res = res.as<CBlockInfo>();
+    }
+};
+
 struct CompressResources {
-    DevBuf frames, blocks, lit_stage, seq_stage, lits, seqs, info, res, csum, results, input, output;
+    DevBuf frames, blocks, csum, results, input, output;
+    CompressStaging stage;
     DevBuf dcontent, dtab, dcounts;   // b200z_dict_finalize: the content's tail, its match table and the statistics
-    cudaEvent_t ev[kCompressStages + 1] = {};
+    Event ev[kCompressStages + 1];
     float stage_ms[kCompressStages] = {};
     bool profiled = false;
 };
-static void compress_free(b200z_ctx *c) {
-    if (!c->comp) return;
-    for (cudaEvent_t e : c->comp->ev) if (e) cudaEventDestroy(e);
-    delete c->comp;
-    c->comp = nullptr;
+// the context's, created by its first compression or dictionary finalization
+static int compress_get(b200z_ctx *c, CompressResources **out) {
+    if (!c->comp) {
+        std::unique_ptr<CompressResources> r(new CompressResources());
+        for (Event &e : r->ev) if (e.create(c, cudaEventDefault)) return B200Z_ERR_CUDA;
+        c->comp = std::move(r);
+    }
+    *out = c->comp.get();
+    return 0;
 }
 extern "C" int b200z_compress_last_profile(const b200z_ctx *c, float *stage_ms, size_t n) {
     if (!c || !stage_ms || !c->comp || !c->comp->profiled) return B200Z_ERR_INVALID_ARGUMENT;
@@ -2027,20 +2045,15 @@ extern "C" int b200z_compress_frames_batch_dict(b200z_ctx *c, const uint8_t *inp
         } while (pos < f.src_size);
         hf[i].nblocks = (uint32_t)hb.size() - hf[i].first_block;
     }
-    if (!c->comp) {
-        c->comp = new CompressResources();
-        for (cudaEvent_t &e : c->comp->ev) CU(c, cudaEventCreate(&e));
-    }
-    CompressResources &r = *c->comp;
+    CompressResources *rp = nullptr;
+    if (int e = compress_get(c, &rp)) return e;
+    CompressResources &r = *rp;
     const bool fast = level == B200Z_LEVEL_FASTEST;
     int e = 0;
+    // Uncompressed takes the blocks' results only, not the match and entropy staging
     if ((e = r.frames.ensure(nframes * sizeof(CFrame))) || (e = r.blocks.ensure(nblocks * sizeof(CBlock))) ||
-        (e = r.res.ensure(nblocks * sizeof(CBlockInfo))) || (e = r.csum.ensure(nframes * 8)) ||
+        (e = fast ? r.stage.ensure(nblocks, true) : r.stage.res.ensure(nblocks * sizeof(CBlockInfo))) || (e = r.csum.ensure(nframes * 8)) ||
         (e = r.results.ensure(nframes * sizeof(b200z_compress_result))))
-        return e;
-    if (fast && ((e = r.lit_stage.ensure(nblocks * ENC_BLOCK)) || (e = r.seq_stage.ensure(nblocks * CBLOCK_SEQS * sizeof(SeqRec))) ||
-                 (e = r.lits.ensure(nblocks * ENC_BLOCK)) || (e = r.seqs.ensure(nblocks * CBLOCK_SEQS * sizeof(SeqRec))) ||
-                 (e = r.info.ensure(nblocks * sizeof(CBlockInfo)))))
         return e;
     const uint8_t *d_in = input;
     uint8_t *d_out = output;
@@ -2060,34 +2073,33 @@ extern "C" int b200z_compress_frames_batch_dict(b200z_ctx *c, const uint8_t *inp
     // the 128 KiB window, so the kernels see the content's last ENC_WINDOW bytes only.
     const bool match_dict = fast && dict && dict->content_len >= ENC_MIN_MATCH;
     const uint32_t dict_tail = dict ? (uint32_t)std::min<size_t>(dict->content_len, ENC_WINDOW) : 0;
-    const uint8_t *dict_at = dict ? dict->d_content + (dict->content_len - dict_tail) : nullptr;
-    b200z_dict *md = const_cast<b200z_dict *>(dict);
-    if (match_dict && !md->d_ctab) {
-        CU(c, cudaMalloc((void **)&md->d_ctab, sizeof(uint32_t) << CD_LOG));
-        if (int le = launch_dict_table(dict_at, dict_tail, md->d_ctab, s, &c->launches)) {
-            cudaFree(md->d_ctab);
-            md->d_ctab = nullptr;
-            return c->set_cuda_err((cudaError_t)le, "k_cdict");
-        }
+    const uint8_t *dict_at = dict ? dict->d_content.as<uint8_t>() + (dict->content_len - dict_tail) : nullptr;
+    if (match_dict && !dict->d_ctab.p) {
+        DevBuf tab;
+        CU(c, tab.alloc(sizeof(uint32_t) << CD_LOG));
+        if (int le = launch_dict_table(dict_at, dict_tail, tab.as<uint32_t>(), s, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_cdict");
+        dict->d_ctab = std::move(tab);
     }
     // the encoder's view of a formatted dictionary's tables, built on the host once and kept with the dictionary (no launch)
     const bool use_tables = fast && dict && dict->has_tables && (c->flags & B200Z_FLAG_DICT_TABLES);
-    if (use_tables && !md->d_enc) {
+    if (use_tables && !dict->d_enc.p) {
         std::unique_ptr<EncDict> ed(new EncDict());
-        const int16_t *probs[3] = {md->norm[0], md->norm[1], md->norm[2]};
-        enc_dict_build(md->huf_weights, md->huf_nweights, probs, md->nnorm, md->log, *ed);
-        CU(c, cudaMalloc((void **)&md->d_enc, sizeof(EncDict)));
-        CU(c, cudaMemcpy(md->d_enc, ed.get(), sizeof(EncDict), cudaMemcpyHostToDevice));
+        const int16_t *probs[3] = {dict->norm[0], dict->norm[1], dict->norm[2]};
+        enc_dict_build(dict->huf_weights, dict->huf_nweights, probs, dict->nnorm, dict->log, *ed);
+        DevBuf enc;
+        CU(c, enc.alloc(sizeof(EncDict)));
+        CU(c, cudaMemcpy(enc.p, ed.get(), sizeof(EncDict), cudaMemcpyHostToDevice));
+        dict->d_enc = std::move(enc);
     }
     CompressArgs a{};
     a.frames = r.frames.as<CFrame>(); a.blocks = r.blocks.as<CBlock>(); a.input = d_in; a.output = d_out;
-    a.etab = use_tables ? dict->d_enc : nullptr;
-    a.lit_stage = r.lit_stage.as<uint8_t>(); a.seq_stage = r.seq_stage.as<SeqRec>(); a.lits = r.lits.as<uint8_t>(); a.seqs = r.seqs.as<SeqRec>();
-    a.enc = a.lit_stage; a.info = r.info.as<CBlockInfo>(); a.res = r.res.as<CBlockInfo>(); a.csum = r.csum.as<uint64_t>();
+    a.etab = use_tables ? dict->d_enc.as<EncDict>() : nullptr;
+    r.stage.bind(a);
+    a.csum = r.csum.as<uint64_t>();
     a.results = r.results.as<b200z_compress_result>(); a.nframes = (uint32_t)nframes; a.nblocks = (uint32_t)nblocks; a.level = level;
     a.checksum = checksum ? 1 : 0;
     a.dict_id = compress_dict_id(dict);
-    if (match_dict) { a.dict = dict_at; a.dtab = dict->d_ctab; a.dict_len = dict_tail; }
+    if (match_dict) { a.dict = dict_at; a.dtab = dict->d_ctab.as<uint32_t>(); a.dict_len = dict_tail; }
     const bool prof = (c->flags & B200Z_FLAG_PROFILE) != 0;
     if (prof) CU(c, cudaEventRecord(r.ev[0], s));
     for (int st = 0; st < kCompressStages; st++) {
@@ -2112,18 +2124,6 @@ extern "C" int b200z_compress_frames_batch_dict(b200z_ctx *c, const uint8_t *inp
 // thread reads and hashes the next chunk and writes the previous one (the pattern of decode_frames_pipelined).
 // ---------------------------------------------------------------------------------------------------------------
 namespace {
-struct PinnedBuf {
-    uint8_t *p = nullptr;
-    PinnedBuf() = default;
-    PinnedBuf(const PinnedBuf &) = delete;
-    PinnedBuf &operator=(const PinnedBuf &) = delete;
-    ~PinnedBuf() { if (p) cudaFreeHost(p); }
-    int alloc(size_t n) {   // once: the size never changes for its owner
-        if (p) return 0;
-        if (cudaMallocHost((void **)&p, n) != cudaSuccess) { p = nullptr; cudaGetLastError(); return B200Z_ERR_OUT_OF_MEMORY; }
-        return 0;
-    }
-};
 constexpr size_t FC_HEADER = 6;       // magic, FHD, Window_Descriptor
 constexpr size_t FC_HDR_ROOM = 16;    // in front of a chunk's blocks in its output buffer: the first chunk's header goes there
 constexpr size_t FC_TRAILER = 3 + 4;  // after them in the last chunk: the empty last block and the checksum
@@ -2137,18 +2137,13 @@ struct b200z_frame_compressor {
     uint64_t chunk = 64ull << 20;   // bytes per chunk, a multiple of ENC_BLOCK
     std::vector<uint8_t> raw;       // Uncompressed: one chunk's part of the frame
     // Fastest, allocated by its first compress; slot s serves chunks k with k & 1 == s
-    cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
-    cudaEvent_t ev_h2d[2] = {}, ev_k[2] = {}, ev_d2h[2] = {};
+    // (b200z_frame_compressor_free synchronises the copy streams before any of these is released)
+    Stream s_h2d, s_d2h;
+    Event ev_h2d[2], ev_k[2], ev_d2h[2];
     PinnedBuf h_in[2], h_out[2], h_desc[2];   // desc: the chunk's CFrame, its CBlocks, then its b200z_compress_result
     DevBuf d_in[2], d_out[2], d_desc[2];      // d_in: the previous chunk's last ENC_WINDOW bytes, then the chunk
-    DevBuf lit_stage, seq_stage, lits, seqs, info, res;   // k_cmatch / k_cenc staging, shared: the kernels run in order on one stream
+    CompressStaging stage;                    // shared: the kernels run in order on one stream
     bool ready = false;
-    ~b200z_frame_compressor() {
-        for (int i = 0; i < 2; i++)
-            for (cudaEvent_t e : {ev_h2d[i], ev_k[i], ev_d2h[i]}) if (e) cudaEventDestroy(e);
-        if (s_h2d) cudaStreamDestroy(s_h2d);
-        if (s_d2h) cudaStreamDestroy(s_d2h);
-    }
     uint32_t chunk_blocks() const { return (uint32_t)(chunk / ENC_BLOCK); }
     size_t chunk_bound() const { return chunk + 3ull * chunk_blocks(); }   // the chunk's blocks, packed, at most
     size_t res_off() const { return sizeof(CFrame) + (size_t)chunk_blocks() * sizeof(CBlock); }
@@ -2265,20 +2260,18 @@ static int fc_prepare(b200z_frame_compressor *fc) {
     if (fc->ready) return 0;
     b200z_ctx *c = fc->ctx;
     const size_t C = fc->chunk, nb = fc->chunk_blocks(), bound = fc->chunk_bound();
-    if (!fc->s_h2d) CU(c, cudaStreamCreateWithFlags(&fc->s_h2d, cudaStreamNonBlocking));
-    if (!fc->s_d2h) CU(c, cudaStreamCreateWithFlags(&fc->s_d2h, cudaStreamNonBlocking));
+    if (!fc->s_h2d && fc->s_h2d.create(c)) return B200Z_ERR_CUDA;
+    if (!fc->s_d2h && fc->s_d2h.create(c)) return B200Z_ERR_CUDA;
     for (int i = 0; i < 2; i++)
-        for (cudaEvent_t *e : {&fc->ev_h2d[i], &fc->ev_k[i], &fc->ev_d2h[i]})
-            if (!*e) CU(c, cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+        for (Event *e : {&fc->ev_h2d[i], &fc->ev_k[i], &fc->ev_d2h[i]})
+            if (!*e && e->create(c)) return B200Z_ERR_CUDA;
     int e = 0;
     for (int i = 0; i < 2 && !e; i++)
         if ((e = fc->d_in[i].ensure(ENC_WINDOW + C + 16, false)) || (e = fc->d_out[i].ensure(bound + 16, false)) ||
-            (e = fc->d_desc[i].ensure(fc->desc_bytes(), false)) || (e = fc->h_in[i].alloc(C)) ||
-            (e = fc->h_out[i].alloc(FC_HDR_ROOM + bound + FC_TRAILER)) || (e = fc->h_desc[i].alloc(fc->desc_bytes())))
+            (e = fc->d_desc[i].ensure(fc->desc_bytes(), false)) || (e = fc->h_in[i].ensure(C, false)) ||
+            (e = fc->h_out[i].ensure(FC_HDR_ROOM + bound + FC_TRAILER, false)) || (e = fc->h_desc[i].ensure(fc->desc_bytes(), false)))
             break;
-    if (!e) e = fc->lit_stage.ensure(nb * ENC_BLOCK, false) || fc->seq_stage.ensure(nb * CBLOCK_SEQS * sizeof(SeqRec), false) ||
-                fc->lits.ensure(nb * ENC_BLOCK, false) || fc->seqs.ensure(nb * CBLOCK_SEQS * sizeof(SeqRec), false) ||
-                fc->info.ensure(nb * sizeof(CBlockInfo), false) || fc->res.ensure(nb * sizeof(CBlockInfo), false) ? B200Z_ERR_OUT_OF_MEMORY : 0;
+    if (!e) e = fc->stage.ensure(nb, false);
     if (e) { c->err = "FrameCompressor: out of memory for chunks of " + std::to_string(C) + " bytes"; return e; }
     fc->ready = true;
     return 0;
@@ -2299,7 +2292,7 @@ static int fc_compress_fast(b200z_frame_compressor *fc, b200z_read_fn rd, void *
     size_t out_n[2] = {0, 0};           // the chunk whose output is in slot s
     auto enqueue = [&](uint64_t k, int s) -> int {
         const uint32_t m = (uint32_t)((n[s] + ENC_BLOCK - 1) / ENC_BLOCK);
-        CFrame *hf = reinterpret_cast<CFrame *>(fc->h_desc[s].p);
+        CFrame *hf = fc->h_desc[s].as<CFrame>();
         CBlock *hb = reinterpret_cast<CBlock *>(hf + 1);
         *hf = CFrame{ENC_WINDOW, n[s], 0, 0, m};
         for (uint32_t i = 0; i < m; i++) {
@@ -2318,23 +2311,22 @@ static int fc_compress_fast(b200z_frame_compressor *fc, b200z_read_fn rd, void *
         a.blocks = reinterpret_cast<const CBlock *>(a.frames + 1);
         a.results = reinterpret_cast<b200z_compress_result *>(fc->d_desc[s].as<uint8_t>() + fc->res_off());
         a.input = din; a.output = fc->d_out[s].as<uint8_t>();
-        a.lit_stage = fc->lit_stage.as<uint8_t>(); a.seq_stage = fc->seq_stage.as<SeqRec>(); a.lits = fc->lits.as<uint8_t>();
-        a.seqs = fc->seqs.as<SeqRec>(); a.enc = a.lit_stage; a.info = fc->info.as<CBlockInfo>(); a.res = fc->res.as<CBlockInfo>();
+        fc->stage.bind(a);
         a.nframes = 1; a.nblocks = m; a.level = B200Z_LEVEL_FASTEST;
         if (int le = launch_compress_chunk(a, ks, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_cmatch / k_cenc / k_cassemble<true>");
         CU(c, cudaEventRecord(fc->ev_k[s], ks));
         CU(c, cudaStreamWaitEvent(fc->s_d2h, fc->ev_k[s], 0));
-        CU(c, cudaMemcpyAsync(fc->h_desc[s].p + fc->res_off(), a.results, sizeof(b200z_compress_result), cudaMemcpyDeviceToHost, fc->s_d2h));
-        CU(c, cudaMemcpyAsync(fc->h_out[s].p + FC_HDR_ROOM, a.output, n[s] + 3ull * m, cudaMemcpyDeviceToHost, fc->s_d2h));
+        CU(c, cudaMemcpyAsync(fc->h_desc[s].as<uint8_t>() + fc->res_off(), a.results, sizeof(b200z_compress_result), cudaMemcpyDeviceToHost, fc->s_d2h));
+        CU(c, cudaMemcpyAsync(fc->h_out[s].as<uint8_t>() + FC_HDR_ROOM, a.output, n[s] + 3ull * m, cudaMemcpyDeviceToHost, fc->s_d2h));
         CU(c, cudaEventRecord(fc->ev_d2h[s], fc->s_d2h));
         return 0;
     };
     auto write_chunk = [&](uint64_t k, int s, bool final) -> int {
-        uint8_t *const body = fc->h_out[s].p + FC_HDR_ROOM;
+        uint8_t *const body = fc->h_out[s].as<uint8_t>() + FC_HDR_ROOM;
         size_t len = 0;
         if (out_n[s]) {
             CU(c, cudaEventSynchronize(fc->ev_d2h[s]));
-            const b200z_compress_result &cr = *reinterpret_cast<const b200z_compress_result *>(fc->h_desc[s].p + fc->res_off());
+            const b200z_compress_result &cr = *reinterpret_cast<const b200z_compress_result *>(fc->h_desc[s].as<uint8_t>() + fc->res_off());
             len = cr.dst_size;
             r.blocks += cr.blocks; r.raw_blocks += cr.raw_blocks; r.rle_blocks += cr.rle_blocks;
         }
@@ -2347,16 +2339,16 @@ static int fc_compress_fast(b200z_frame_compressor *fc, b200z_read_fn rd, void *
         return 0;
     };
     int e = 0;
-    if (!fc_read(rd, ru, fc->h_in[0].p, C, &n[0], &eof[0])) e = fc_panic(c, "FrameCompressor::compress: the source's read failed");
-    else h.update(fc->h_in[0].p, n[0]);
+    if (!fc_read(rd, ru, fc->h_in[0].as<uint8_t>(), C, &n[0], &eof[0])) e = fc_panic(c, "FrameCompressor::compress: the source's read failed");
+    else h.update(fc->h_in[0].as<uint8_t>(), n[0]);
     for (uint64_t k = 0; !e; k++) {
         const int s = (int)(k & 1);
         out_n[s] = n[s];
         if (n[s] && (e = enqueue(k, s))) break;
         if (!eof[s]) {   // read chunk k + 1 into the other slot once chunk k - 1's upload is done with it
             if (k && cudaEventSynchronize(fc->ev_h2d[s ^ 1]) != cudaSuccess) { e = c->set_cuda_err(cudaGetLastError(), "upload"); break; }
-            if (!fc_read(rd, ru, fc->h_in[s ^ 1].p, C, &n[s ^ 1], &eof[s ^ 1])) { e = fc_panic(c, "FrameCompressor::compress: the source's read failed"); break; }
-            h.update(fc->h_in[s ^ 1].p, n[s ^ 1]);
+            if (!fc_read(rd, ru, fc->h_in[s ^ 1].as<uint8_t>(), C, &n[s ^ 1], &eof[s ^ 1])) { e = fc_panic(c, "FrameCompressor::compress: the source's read failed"); break; }
+            h.update(fc->h_in[s ^ 1].as<uint8_t>(), n[s ^ 1]);
         }
         if (k && (e = write_chunk(k - 1, s ^ 1, false))) break;
         if (eof[s]) { e = write_chunk(k, s, true); break; }
@@ -2393,10 +2385,8 @@ extern "C" int b200z_frame_compressor_compress(b200z_frame_compressor *fc, b200z
 struct DictTrainResources {
     DevBuf input, starts, slots, dist, freq, best, done, segs;
 };
-static void dtrain_free(b200z_ctx *c) {
-    delete c->dtrain;
-    c->dtrain = nullptr;
-}
+
+b200z_ctx::~b200z_ctx() = default;
 
 struct DtEpoch { uint32_t e0, e1, le; };
 
@@ -2465,7 +2455,7 @@ extern "C" int b200z_dict_train_raw(b200z_ctx *c, const uint8_t *samples, size_t
     if (ep.empty()) return 0;
     if (int e = c->use()) return e;
     // ---- device passes
-    if (!c->dtrain) c->dtrain = new DictTrainResources();
+    if (!c->dtrain) c->dtrain.reset(new DictTrainResources());
     DictTrainResources &r = *c->dtrain;
     const uint32_t E = (uint32_t)ep.size(), ns = (uint32_t)(starts.size() - 1);
     int e = 0;
@@ -2551,18 +2541,14 @@ extern "C" int b200z_dict_finalize(b200z_ctx *c, const uint8_t *content, size_t 
     std::vector<uint64_t> counts(DS_BINS, 0);
     if (nsamples) {
         if (int e = c->use()) return e;
-        if (!c->comp) {
-            c->comp = new CompressResources();
-            for (cudaEvent_t &e : c->comp->ev) CU(c, cudaEventCreate(&e));
-        }
-        CompressResources &r = *c->comp;
+        CompressResources *rp = nullptr;
+        if (int e = compress_get(c, &rp)) return e;
+        CompressResources &r = *rp;
         const uint64_t per = std::min<uint64_t>(nsamples, DS_BLOCKS);
         const uint32_t tail = (uint32_t)std::min<size_t>(content_len, ENC_WINDOW);   // all a match can reach
         int e = 0;
-        if ((e = r.blocks.ensure(nsamples * sizeof(CBlock))) || (e = r.lit_stage.ensure(per * ENC_BLOCK)) ||
-            (e = r.seq_stage.ensure(per * CBLOCK_SEQS * sizeof(SeqRec))) || (e = r.lits.ensure(per * ENC_BLOCK)) ||
-            (e = r.seqs.ensure(per * CBLOCK_SEQS * sizeof(SeqRec))) || (e = r.info.ensure(per * sizeof(CBlockInfo))) ||
-            (e = r.dcontent.ensure(tail + 16)) || (e = r.dtab.ensure(sizeof(uint32_t) << CD_LOG)) || (e = r.dcounts.ensure(DS_BINS * 8)))
+        if ((e = r.blocks.ensure(nsamples * sizeof(CBlock))) || (e = r.stage.ensure(per, true)) || (e = r.dcontent.ensure(tail + 16)) ||
+            (e = r.dtab.ensure(sizeof(uint32_t) << CD_LOG)) || (e = r.dcounts.ensure(DS_BINS * 8)))
             return e;
         cudaStream_t s = c->stream;
         const uint8_t *d_in = samples;
@@ -2578,8 +2564,7 @@ extern "C" int b200z_dict_finalize(b200z_ctx *c, const uint8_t *content, size_t 
             return c->set_cuda_err((cudaError_t)le, "k_cdict");
         CompressArgs a{};
         a.input = d_in;
-        a.lit_stage = r.lit_stage.as<uint8_t>(); a.seq_stage = r.seq_stage.as<SeqRec>(); a.lits = r.lits.as<uint8_t>();
-        a.seqs = r.seqs.as<SeqRec>(); a.info = r.info.as<CBlockInfo>();
+        r.stage.bind(a);
         a.dict = r.dcontent.as<uint8_t>(); a.dtab = r.dtab.as<uint32_t>(); a.dict_len = tail;
         for (uint64_t b0 = 0; b0 < nsamples; b0 += per) {
             a.blocks = r.blocks.as<CBlock>() + b0;
