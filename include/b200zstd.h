@@ -328,6 +328,83 @@ int b200z_decode_all_batch(b200z_ctx *ctx, const uint8_t *input, size_t input_le
  * *n = the chain's length. */
 int b200z_debug_decode_all_chain(const uint8_t *input, size_t input_len, int by_candidates, uint64_t *at, size_t cap, size_t *n);
 
+/* Reader and writer callbacks (io::Read::read / io::Write::write semantics), for tiers 1d and 2 and the stream compressor */
+typedef long (*b200z_read_fn)(void *user, uint8_t *buf, size_t len);        /* bytes read, 0 = EOF, <0 = error */
+typedef long (*b200z_write_fn)(void *user, const uint8_t *buf, size_t len); /* bytes written, 0 = full, <0 = error */
+
+/* ------------------------------------------------------------------------------------------------------------
+ * Tier 1d -- decode_all from a reader to a writer, chunk by chunk, in bounded memory.  Decodes a source of any length (a .zst
+ * file of concatenated zstd and skippable frames, pzstd output, the stream compressor's single frame of unknown size) at GPU
+ * speed without holding the whole input or output anywhere.  Rules:
+ *   Output:    the drain receives what FrameDecoder::decode_all (frame_decoder.rs:541-577) writes for the source's bytes with
+ *              unlimited output: the zstd frames' plaintexts back to back, skippable frames skipped -- decode_all's rule, not
+ *              StreamingDecoder's single frame -- whatever the chunk size and however the source splits its reads.
+ *   Errors:    `all` is what b200z_decode_all_batch reports for the same bytes with enough output room; TargetTooSmall cannot occur.
+ *              After an error nothing more is written: the drain ends with the failing frame's output up to its first failing block
+ *              (`delivered`).  The source may have been read up to one chunk past the failing frame.
+ *   Read / write failures: a read returning < 0 (or more than asked for) ends the source, as the tier-2 reader treats it, and the
+ *              frame in progress fails with the reference's read leaf (BLOCK_HEADER_READ, BLOCK_CONTENT_READ, ...).  A write returning
+ *              <= 0 is B200Z_ERR_FAILED_TO_DRAIN_DECODEBUFFER at B200Z_STAGE_DRAIN (collect_to_writer's leaf).  Nothing is left in
+ *              flight either way, and the context stays usable.
+ *   Checksums: EXTENSION, with B200Z_FLAG_CHECKSUM: every frame's XXH64 is computed on the GPU, frames that span submissions
+ *              included, and compared with the checksum the frame carries.  As in the reference (frame_decoder.rs:253-270) it is
+ *              reported, never enforced.
+ *   Dictionaries: as decode_all: `dicts` selected by frame dictionary ID; `forced_dict` the tier-1c extension for raw-content frames.
+ *   History:   documented deviation, for frames RFC 8878 does not allow.  A frame that continues into a submission reaches back
+ *              window_size bytes (at least 32) before the submission's first byte of that frame; inside a submission it reaches all of
+ *              the frame's earlier output.  An offset past the window, which the reference accepts only when its undrained buffer
+ *              happens to hold more, may therefore fail or not depending on where a chunk boundary falls.  Likewise a submission's
+ *              output room is the sum of its blocks' bounds, min(128 KiB, window) for a Compressed block: a Compressed block that
+ *              decodes to more may overrun it, depending on the other blocks of its submission and so on the chunk size.  Its frame
+ *              then fails with B200Z_ERR_BLOCK_OUTPUT_LIMIT (B200Z_STAGE_EXECUTE) where decode_all_batch may decode it.  Spec-valid
+ *              frames never depend on either.
+ * Chunking: the source is read into a pinned buffer and cut at block ends into submissions.  With C = B200Z_PIPELINE_CHUNK_BYTES
+ * (read by each call; 64 MiB by default) a submission holds whole blocks and at most C bytes of input (frame headers, blocks,
+ * checksums and the skippable frames between its frames), a decoded size bound of 4 * C (a Raw or RLE block counts its size, a
+ * Compressed block min(128 KiB, window)), C / 16384 blocks and C / 4 sequences -- or exactly one block, whatever C is.  Skippable
+ * frames in front of a submission are read and dropped, never buffered.  While submission k decodes, the calling thread reads and
+ * cuts k + 1 and writes k - 1; a frame that runs past a cut continues from its state, tables and window tail, carried device to
+ * device (k_carry); the host reads back only each submission's frame states and then exactly the plaintext it writes.
+ * Memory, allocated by the first call (again when C changes) and kept by the context, depends on C and on the largest window W
+ * seen only.  Device, per each of two slots: C + 2 * 131097 input, max(W, 32) + max(4 * C, 131072) output, 4 * C + 32 * C / 16384
+ * literals, 12 * (C / 4 + C / 4096) sequence scratch and 6.2 KB of tables per block (C / 16384 blocks): in all about
+ * 2 * (12.4 * C + W), 1.7 GB at 64 MiB.  Pinned host: 2 * (C + 2 * 131097) input and max(4 * C, 131072) output.
+ * Returns 0 when the call ran to an outcome, which `result` reports (an error in the stream, a failed drain); otherwise a b200z_error
+ * (B200Z_ERR_INVALID_ARGUMENT, B200Z_ERR_OUT_OF_MEMORY, B200Z_ERR_CUDA) and `result` says what was delivered before it.
+ * ---------------------------------------------------------------------------------------------------------- */
+typedef struct b200z_stream_result {
+    b200z_all_result all;          /* what b200z_decode_all_batch reports for the same bytes with unlimited output           */
+    uint64_t delivered;            /* bytes handed to write_cb: all.written, plus on an error the failing frame's output of
+                                      every block before its first failing block                                             */
+    uint64_t submissions;          /* GPU submissions (chunks) the call ran                                                    */
+    uint64_t checksum_frames;      /* B200Z_FLAG_CHECKSUM: frames that carry a checksum and were compared                      */
+    uint64_t checksum_mismatches;
+    int64_t first_mismatch_frame;  /* index among the zstd frames, -1 when none                                               */
+} b200z_stream_result;
+
+int b200z_decode_all_stream(b200z_ctx *ctx, b200z_read_fn read_cb, void *read_user, b200z_write_fn write_cb, void *write_user,
+                            const b200z_dict *const *dicts, size_t ndicts, const b200z_dict *forced_dict, uint64_t max_window_size,
+                            b200z_stream_result *result);
+
+/* Host-only view of how b200z_decode_all_stream cuts a byte string into submissions at chunk size `chunk` (no context, no device;
+ * for CPU tests).  One record per submission that holds a frame: [start, end) its stream bytes (skippable frames dropped in front
+ * of it excluded), in_bytes = end - start, the decoded size bound, blocks, sequences and frames it holds; flags bit 0: its first
+ * frame continues from the one before, bit 1: its last frame continues into the next.  `end`: where the cutter stopped -- the error
+ * it can see from the headers it reads (frame header, skipped bytes, block header, truncated block or checksum), at which frame
+ * (error_offset = the frame's stream offset, the source's length without an error), the skippable frames passed and the most
+ * bytes it held in its buffer.  `cuts` has room for `cap` records; *n = the number of records. */
+typedef struct b200z_stream_cut {
+    uint64_t start, end, in_bytes, out_bound, nblocks, nseq;
+    uint32_t nframes, flags;
+} b200z_stream_cut;
+typedef struct b200z_stream_cut_end {
+    uint64_t error_offset, skippable_frames, peak_buffered;
+    int32_t status, stage, error_frame;
+    uint32_t reserved;
+} b200z_stream_cut_end;
+int b200z_debug_stream_cut(const uint8_t *input, size_t input_len, uint64_t chunk, b200z_stream_cut *cuts, size_t cap, size_t *n,
+                           b200z_stream_cut_end *end);
+
 /* ------------------------------------------------------------------------------------------------------------
  * Tier 1b -- block-level batch entry: the thin FFI for a host that keeps the reference's OWN frame / block /
  * section header parsing (frame.rs:6-85, block_decoder.rs:201-247, literals_section.rs:117-223,
@@ -383,8 +460,6 @@ int b200z_decode_blocks_batch(b200z_ctx *ctx, const b200z_block_desc *blocks, si
  * Tier 2 -- mirror of ruzstd's FrameDecoder (decoding/frame_decoder.rs:154-627), GPU-backed.
  * Same names, argument meaning and error behaviour; `read_cb` has io::Read::read semantics.
  * ---------------------------------------------------------------------------------------------------------- */
-typedef long (*b200z_read_fn)(void *user, uint8_t *buf, size_t len);        /* bytes read, 0 = EOF, <0 = error */
-typedef long (*b200z_write_fn)(void *user, const uint8_t *buf, size_t len); /* bytes written, 0 = full, <0 = error */
 
 /* BlockDecodingStrategy (frame_decoder.rs:96-100) */
 #define B200Z_STRATEGY_ALL 0

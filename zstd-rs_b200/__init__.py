@@ -2,7 +2,8 @@
 a batch compressor at ruzstd's Uncompressed and Fastest levels (compress_frames / compress_to_vec), a stream compressor behind
 ruzstd's FrameCompressor / encoding::compress API (FrameCompressor, compress), and a raw-content
 dictionary trainer in place of ruzstd::dictionary (create_raw_dict, create_raw_dict_from_source, create_raw_dict_from_dir)
-and a finalizer that turns its content into a zstd-format dictionary (finalize_dict, create_dict).
+and a finalizer that turns its content into a zstd-format dictionary (finalize_dict, create_dict).  decode_all_stream decodes a
+source of concatenated frames to a drain chunk by chunk through the GPU, in bounded memory.
 
 The product is the C-ABI library ``libb200zstd.so`` (include/b200zstd.h, sources in csrc/).  This package is the
 Python host-side mirror of the reference interface (same names, argument meaning and error behaviour as
@@ -15,7 +16,7 @@ from .binding import (  # noqa: F401
     ALL, FASTEST, UNCOMPRESSED, UPTO_BLOCKS, UPTO_BYTES, AllBatch, B200ZError, Batch, Context, Dictionary, FrameCompressor, FrameDecoder,
     StreamingDecoder, build, compress, compress_bound, compress_frames, compress_profile, compress_to_vec, create_dict, create_raw_dict,
     create_raw_dict_from_dir,
-    create_raw_dict_from_source, decode_all, decode_all_batch, decode_blocks, decode_frames,
+    create_raw_dict_from_source, decode_all, decode_all_batch, decode_all_stream, decode_blocks, decode_frames,
     dict_from_counts, error_names, finalize_dict, lib, lib_path, xxh64,
 )
 from . import binding  # noqa: F401

@@ -125,6 +125,8 @@ def lib():
         "b200z_decode_all_finish": (C.c_int, [vp, vp, vp]),
         "b200z_decode_all_batch": (C.c_int, [vp, vp, sz, C.c_int, pp, sz, vp, C.c_uint64, vp, sz, C.c_int, vp]),
         "b200z_debug_decode_all_chain": (C.c_int, [vp, sz, C.c_int, vp, sz, C.POINTER(sz)]),
+        "b200z_decode_all_stream": (C.c_int, [vp, READ_FN, vp, WRITE_FN, vp, pp, sz, vp, C.c_uint64, vp]),
+        "b200z_debug_stream_cut": (C.c_int, [vp, sz, C.c_uint64, vp, sz, C.POINTER(sz), vp]),
         "b200z_frame_decoder_new": (C.c_int, [vp, pp]),
         "b200z_frame_decoder_free": (None, [vp]),
         "b200z_frame_decoder_set_max_window_size": (None, [vp, C.c_uint64]),
@@ -470,6 +472,68 @@ def decode_all_chain(data, by_candidates=False):
     if rc:
         raise B200ZError(rc, 0, "b200z_debug_decode_all_chain")
     return [int(x) for x in out[:n.value]]
+
+
+STREAM_RESULT_DTYPE = np.dtype([("all", ALL_RESULT_DTYPE), ("delivered", "<u8"), ("submissions", "<u8"), ("checksum_frames", "<u8"),
+                                ("checksum_mismatches", "<u8"), ("first_mismatch_frame", "<i8")])
+STREAM_CUT_DTYPE = np.dtype([("start", "<u8"), ("end", "<u8"), ("in_bytes", "<u8"), ("out_bound", "<u8"), ("nblocks", "<u8"), ("nseq", "<u8"),
+                             ("nframes", "<u4"), ("flags", "<u4")])
+STREAM_CUT_END_DTYPE = np.dtype([("error_offset", "<u8"), ("skippable_frames", "<u8"), ("peak_buffered", "<u8"), ("status", "<i4"), ("stage", "<i4"),
+                                 ("error_frame", "<i4"), ("reserved", "<u4")])
+
+
+def decode_all_stream(ctx, source, drain, dicts=None, forced_dict=None, max_window_size=0):
+    """b200z_decode_all_stream: FrameDecoder::decode_all of everything `source` holds (bytes, or an object with read(n)) to `drain` (an
+    object with write(b), or a bytearray, which the plaintext is appended to), chunk by chunk through the GPU in bounded memory
+    (B200Z_PIPELINE_CHUNK_BYTES per chunk).  Returns a dict: the decode_all summary (written, frames, skippable_frames, error_offset,
+    status, stage, error_frame) and delivered, submissions, checksum_frames, checksum_mismatches, first_mismatch_frame.  Errors in the
+    stream, a source that raises (it ends the source) and a drain that raises or returns 0 (FAILED_TO_DRAIN_DECODEBUFFER) are reported
+    in the dict, not raised."""
+    src = _Reader(source).src
+
+    def _read(_user, buf, n):
+        try:
+            b = src.read(n)
+            if b:
+                C.memmove(buf, b, len(b))
+            return len(b)
+        except Exception:
+            return -1
+
+    def _write(_user, buf, n):
+        try:
+            if isinstance(drain, bytearray):
+                drain.extend(C.string_at(buf, n))
+                return n
+            r = drain.write(C.string_at(buf, n))
+            return n if r is None else r
+        except Exception:
+            return -1
+
+    rd, wr = READ_FN(_read), WRITE_FN(_write)
+    darr, nd, forced = _dict_args(dicts, forced_dict)
+    res = np.zeros(1, dtype=STREAM_RESULT_DTYPE)
+    ctx._chk(ctx.L.b200z_decode_all_stream(ctx.h, rd, None, wr, None, darr, nd, forced, max_window_size, res.ctypes.data))
+    out = _summary(res["all"])
+    out.update({k: int(res[0][k]) for k in STREAM_RESULT_DTYPE.names if k != "all"})
+    return out
+
+
+def stream_cut(data, chunk):
+    """Host-only: how decode_all_stream cuts `data` at chunk size `chunk` -- (STREAM_CUT_DTYPE rows, one per submission; the end
+    record as a dict: error_offset, skippable_frames, peak_buffered, status, stage, error_frame)."""
+    b = np.frombuffer(bytes(data), dtype=np.uint8)
+    n = C.c_size_t()
+    end = np.zeros(1, dtype=STREAM_CUT_END_DTYPE)
+    cap = 64
+    while True:
+        cuts = np.zeros(cap, dtype=STREAM_CUT_DTYPE)
+        rc = lib().b200z_debug_stream_cut(b.ctypes.data if len(b) else None, len(b), chunk, cuts.ctypes.data, cap, C.byref(n), end.ctypes.data)
+        if rc:
+            raise B200ZError(rc, 0, "b200z_debug_stream_cut")
+        if n.value <= cap:
+            return cuts[:n.value], {k: int(end[0][k]) for k in STREAM_CUT_END_DTYPE.names if k != "reserved"}
+        cap = n.value
 
 
 def compress_bound(n, dict=None):

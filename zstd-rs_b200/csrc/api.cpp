@@ -121,6 +121,7 @@ struct Event {
 struct PipeResources;
 struct CompressResources;
 struct DictTrainResources;
+struct StreamDecodeResources;
 
 struct b200z_ctx {
     int device = 0;
@@ -131,6 +132,7 @@ struct b200z_ctx {
     std::unique_ptr<PipeResources> pipe;         // lazily created by the pipelined one-shot path
     std::unique_ptr<CompressResources> comp;     // lazily created by the first compression
     std::unique_ptr<DictTrainResources> dtrain;  // lazily created by the first dictionary training
+    std::unique_ptr<StreamDecodeResources> sdec; // lazily created by the first b200z_decode_all_stream
     std::string err;
     uint64_t launches = 0;
     uint32_t flags = 0;
@@ -687,14 +689,19 @@ static int restore_states(b200z_batch *b) {
 // runs in two stages, as the frame decoder's submissions do: tables, literals and sequences of every block (k_setup, k_huf, k_fse);
 // k_place, which writes every frame's out_off / out_cap; then execution (k_exec_cta, k_exec) and, with B200Z_FLAG_CHECKSUM, k_xxh64.
 // There is no host round trip in between; what is given up is k_exec running beside k_fse.
-static int enqueue_decode_all_pass(b200z_ctx *c, const PipelineArgs &a, const PipelineStreams &ps, bool *checksummed, uint64_t *launched) {
+// `resume`: the first frame continues from the stream decoder's previous submission (k_place_resume places it behind its carried tail)
+static int enqueue_decode_all_stages(b200z_ctx *c, const PipelineArgs &a, const PipelineStreams &ps, bool resume, uint64_t *launched) {
     PipelineArgs a_dec = a;
     a_dec.nframes = 0;
     if (int e = launch_pipeline_overlapped(a_dec, ps, launched)) return c->set_cuda_err((cudaError_t)e, "launch_pipeline (decode)");
-    if (int e = launch_place(a, ps.main, launched)) return c->set_cuda_err((cudaError_t)e, "k_place");
+    if (int e = resume ? launch_place_resume(a, ps.main, launched) : launch_place(a, ps.main, launched)) return c->set_cuda_err((cudaError_t)e, "k_place");
     PipelineArgs a_ex = a;
     a_ex.nblocks = 0;
     if (int e = launch_pipeline_overlapped(a_ex, ps, launched)) return c->set_cuda_err((cudaError_t)e, "launch_pipeline (execute)");
+    return 0;
+}
+static int enqueue_decode_all_pass(b200z_ctx *c, const PipelineArgs &a, const PipelineStreams &ps, bool *checksummed, uint64_t *launched) {
+    if (int e = enqueue_decode_all_stages(c, a, ps, false, launched)) return e;
     *checksummed = (c->flags & B200Z_FLAG_CHECKSUM) && a.nframes;
     if (*checksummed)
         if (int e = launch_checksum(a, ps.main, launched)) return c->set_cuda_err((cudaError_t)e, "launch_checksum");
@@ -1321,6 +1328,558 @@ extern "C" int b200z_decode_all_batch(b200z_ctx *c, const uint8_t *input, size_t
         CU(c, cudaMemcpyAsync(output, dout, summary->written, cudaMemcpyDeviceToHost, c->stream));
         CU(c, cudaStreamSynchronize(c->stream));
     }
+    return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// tier 1d: decode_all from a reader to a writer (b200z_decode_all_stream).  The source is cut at block ends into submissions of
+// bounded input and output; each is a decode_all pass (enqueue_decode_all_stages).  A frame that runs past a cut continues in the
+// next submission from its state, tables and window tail, carried device to device (k_carry, the table copies below).
+// ---------------------------------------------------------------------------------------------------------------
+namespace {
+
+constexpr uint64_t SD_BLOCK_ROOM = 18 + 3 + 131072 + 4;   // a frame header, one block and a checksum: a submission always takes one block
+
+// The cut rules' bounds for a chunk of C bytes (DESIGN.md 4.9).  A submission with one block may exceed any of them.
+struct SdBounds {
+    uint64_t chunk, out, blocks, seqs;
+    explicit SdBounds(uint64_t C) : chunk(C), out(4 * C), blocks(std::max<uint64_t>(1, C / 16384)), seqs(C / 4) {}
+    uint64_t buffer() const { return chunk + 2 * SD_BLOCK_ROOM; }   // host input per slot: no cut is ever forced by it
+    uint64_t out_room() const { return std::max<uint64_t>(out, 131072); }
+};
+
+// the source, read into the buffer of the submission being planned: buf[0, have) holds stream bytes from offset `off` on
+struct SdSource {
+    b200z_read_fn rd = nullptr;
+    void *user = nullptr;
+    uint8_t *buf = nullptr;
+    size_t have = 0, cap = 0, peak = 0;
+    uint64_t off = 0;
+    bool eof = false;
+    std::vector<uint8_t> scratch;
+    // buf[0, n) available, unless the source ends first (a read that fails or returns more than asked for ends it, as the frame
+    // decoder's reader treats them); n <= cap
+    bool fill(size_t n) {
+        while (have < n && !eof) {
+            const long r = rd(user, buf + have, cap - have);
+            if (r <= 0 || (size_t)r > cap - have) { eof = true; break; }
+            have += (size_t)r;
+        }
+        peak = std::max(peak, have);
+        return have >= n;
+    }
+    // drops the n bytes at the front, reading and discarding those past the buffer (a skippable frame is never buffered); false when
+    // the source ends first
+    bool drop(uint64_t n) {
+        if (n <= have) { memmove(buf, buf + n, have - n); have -= (size_t)n; off += n; return true; }
+        n -= have; off += have; have = 0;
+        scratch.resize(1 << 16);
+        while (n) {
+            const long r = eof ? 0 : rd(user, scratch.data(), (size_t)std::min<uint64_t>(n, scratch.size()));
+            if (r <= 0 || (uint64_t)r > n) { eof = true; return false; }
+            n -= (uint64_t)r; off += (uint64_t)r;
+        }
+        return true;
+    }
+    // the bytes after a cut at `cut` become the front of `next`, the buffer of the next submission
+    void advance(size_t cut, uint8_t *next) {
+        if (have > cut) memmove(next, buf + cut, have - cut);
+        have -= cut; off += cut; buf = next;
+    }
+};
+
+struct SdFrame {                  // a frame of a planned submission
+    uint64_t at = 0;              // stream offset of its magic number
+    int32_t zi = 0;               // its index among the zstd frames
+    uint32_t skips_before = 0;    // skippable frames passed between the previous frame and this one
+    bool has_checksum = false;    // the checksum it carries was read in this submission
+    uint32_t checksum = 0;
+};
+
+// the frame that continues past the submission planned last
+struct SdCont {
+    bool on = false;
+    SdFrame frame;
+    const b200z_dict *dict = nullptr;
+    uint64_t window = 0;
+    bool checksum = false;
+    uint32_t next_block = 0;
+    CarrySet tables;              // what its next block starts from
+};
+
+struct SdPlan {
+    std::vector<SdFrame> frames;
+    bool resumed = false, continues = false, ends = false;   // ends: nothing comes after it (end of the source, or an error)
+    size_t cut = 0;               // buffer bytes the submission takes
+    uint64_t start = 0, in_bytes = 0, out_bound = 0, nblocks = 0, nseq = 0;
+    uint32_t skips_after = 0;
+    uint32_t end_word = 0;        // an error the cutter found past the submission's frames (status word), 0 = none
+    uint64_t end_at = 0;
+    int32_t end_zi = -1;
+    uint64_t resume_window = 0;   // window of the resumed frame
+    TableCursor cur_end;          // the continuing frame's tables after its last block here (what the next submission copies)
+};
+
+struct SdPlanner {
+    SdBounds bnd;
+    const b200z_dict *const *dicts;
+    size_t ndicts;
+    const b200z_dict *forced;
+    uint64_t max_window;
+    const HufSlot *carry_huf = nullptr;     // where the continuing frame's tables are carried (device)
+    const FseSlot *carry_fse = nullptr;
+    const FseSlot *predef = nullptr;
+    SdCont cont;
+    int32_t zi = -1;
+    uint64_t max_window_seen = 0;
+    SdPlanner(uint64_t C, const b200z_dict *const *d, size_t nd, const b200z_dict *f, uint64_t mw) : bnd(C), dicts(d), ndicts(nd), forced(f) {
+        max_window = std::min<uint64_t>(mw ? mw : B200Z_DEFAULT_MAX_WINDOW_SIZE, (1ull << 41) + 7 * (1ull << 38));
+    }
+
+    // the most a block adds to the output: a Raw / RLE block's size, min(128 KiB, window) for a Compressed block
+    static uint64_t out_of(const BlockHeader &bh, uint64_t window) { return bh.type == BT_COMPRESSED ? std::min<uint64_t>(131072, window) : bh.decompressed_size; }
+    static uint64_t seqs_of(const BlockHeader &bh, const uint8_t *content) {
+        if (bh.type != BT_COMPRESSED) return 0;
+        const SectionHeaders sec = parse_section_headers(content, bh.content_size);
+        return ((uint64_t)sec.nseq + 3) & ~3ull;
+    }
+    bool fits(const SdPlan &p, uint64_t in, uint64_t out, uint64_t seqs) const {
+        return p.nblocks == 0 || (p.in_bytes + in <= bnd.chunk && p.out_bound + out <= bnd.out && p.nblocks + 1 <= bnd.blocks && p.nseq + seqs <= bnd.seqs);
+    }
+    void fail_at(SdPlan &p, uint32_t word, uint64_t at, int32_t z) { p.end_word = word; p.end_at = at; p.end_zi = z; p.ends = true; }
+
+    // Plans the next submission into s / p from the source (its buffer starts with the bytes carried over from the last cut).
+    void plan(SdSource &src, Submission &s, SdPlan &p) {
+        s.clear();
+        p = SdPlan();
+        size_t pos = 0;
+        bool active = false;   // inside a frame: a block header comes next
+        TableCursor cur;
+        uint64_t window = 0;
+        bool checksum = false;
+        uint32_t bif = 0, skips = 0;
+        const b200z_dict *fdict = nullptr;
+        auto start_frame = [&](const SdFrame &f, const b200z_dict *dict, uint64_t w) {
+            p.frames.push_back(f);
+            p.frames.back().skips_before = skips;
+            skips = 0;
+            window = w;
+            fdict = dict;
+        };
+        if (cont.on) {
+            // the frame continues from its carried state, tables and tail (k_carry writes its state and placement)
+            start_frame(cont.frame, cont.dict, cont.window);
+            FrameDesc fd;
+            memset(&fd, 0, sizeof fd);
+            fd.window_size = cont.window;
+            fd.dict = cont.dict ? cont.dict->d_content.as<uint8_t>() : nullptr; fd.dict_len = cont.dict ? cont.dict->content_len : 0;
+            FrameState st;
+            memset(&st, 0, sizeof st);
+            s.frames.push_back(fd); s.states.push_back(st);
+            s.carries.push_back(cont.tables);
+            cursor_from_carry(cur, cont.tables, (uint32_t)s.carries.size() - 1);
+            checksum = cont.checksum; bif = cont.next_block;
+            p.resumed = true; p.resume_window = cont.window;
+            active = true;
+            cont.on = false;
+        }
+        p.start = src.off;
+        for (;;) {
+            if (!active) {
+                if (!src.fill(pos + 1)) { p.ends = true; break; }   // the end of the source, between frames
+                size_t want;
+                while ((want = frame_header_want(src.buf + pos, src.have - pos)) > src.have - pos && src.fill(pos + want)) {}
+                FrameHeader h;
+                uint32_t skip = 0;
+                size_t hs = 0;
+                const uint64_t at = src.off + pos;
+                int e = parse_frame_header(src.buf + pos, src.have - pos, h, skip, hs);
+                if (e == B200Z_ERR_SKIP_FRAME) {
+                    const uint64_t n = 8ull + skip;
+                    if (p.frames.empty()) {   // in front of the submission: dropped, never buffered
+                        if (!src.drop(n)) { fail_at(p, mk_status(B200Z_ERR_FAILED_TO_SKIP_FRAME, B200Z_STAGE_FRAME_HEADER), at, -1); break; }
+                        p.start = src.off;
+                        skips++;
+                        continue;
+                    }
+                    if (p.in_bytes + n > bnd.chunk) break;   // cut in front of it: the next submission drops it
+                    if (!src.fill(pos + n)) { fail_at(p, mk_status(B200Z_ERR_FAILED_TO_SKIP_FRAME, B200Z_STAGE_FRAME_HEADER), at, -1); break; }
+                    pos += n; p.in_bytes += n;
+                    skips++;
+                    continue;
+                }
+                const bool zstd = src.have - pos >= 4 && rd32le(src.buf + pos) == ZSTD_MAGIC;
+                if (zstd) zi++;
+                const int32_t z = zstd ? zi : -1;
+                uint64_t w = 0;
+                if (!e) e = frame_window_size(h, w);
+                if (!e && w > max_window) e = B200Z_ERR_WINDOW_SIZE_TOO_BIG;
+                const b200z_dict *dict = nullptr;
+                if (!e && h.has_dict_id) {
+                    for (size_t k = 0; k < ndicts; k++) if (dicts[k]->id == h.dict_id) dict = dicts[k];
+                    if (!dict) e = B200Z_ERR_DICT_NOT_PROVIDED;
+                }
+                if (e) { fail_at(p, mk_status((uint32_t)e, B200Z_STAGE_FRAME_HEADER), at, z); break; }
+                if (forced) dict = forced;
+                // the frame header goes with the frame's first block: cut in front of it when that block does not fit
+                BlockHeader bh;
+                bool have_bh = src.fill(pos + hs + 3), bh_ok = have_bh && !parse_block_header(src.buf + pos + hs, bh);
+                if (bh_ok && src.fill(pos + hs + 3 + bh.content_size)) {
+                    const uint64_t in = hs + 3 + bh.content_size + (bh.last && h.content_checksum() ? 4 : 0);
+                    if (!fits(p, in, out_of(bh, w), seqs_of(bh, src.buf + pos + hs + 3))) { zi--; break; }
+                }
+                max_window_seen = std::max(max_window_seen, w);
+                SdFrame f;
+                f.at = at; f.zi = z;
+                start_frame(f, dict, w);
+                cur = s.add_frame(dict, 0, 0, w);
+                checksum = h.content_checksum(); bif = 0;
+                pos += hs; p.in_bytes += hs;
+                active = true;
+            }
+            // a block of the active frame
+            FrameDesc &fd = s.frames.back();
+            if (!src.fill(pos + 3)) { fd.host_status = mk_status(B200Z_ERR_BLOCK_HEADER_READ, B200Z_STAGE_BLOCK_HEADER); p.ends = true; break; }
+            BlockHeader bh;
+            if (int e = parse_block_header(src.buf + pos, bh)) { fd.host_status = mk_status((uint32_t)e, B200Z_STAGE_BLOCK_HEADER); p.ends = true; break; }
+            if (!src.fill(pos + 3 + bh.content_size)) {
+                fd.host_status = mk_status(bh.type == BT_COMPRESSED ? B200Z_ERR_BLOCK_CONTENT_READ : B200Z_ERR_BLOCK_BODY_READ, B200Z_STAGE_BLOCK_BODY);
+                p.ends = true;
+                break;
+            }
+            const uint64_t in = 3 + bh.content_size + (bh.last && checksum ? 4 : 0), out = out_of(bh, window);
+            const uint64_t seqs = seqs_of(bh, src.buf + pos + 3);
+            if (!fits(p, in, out, seqs)) break;   // cut at this block end: the frame continues in the next submission
+            const BlockDesc &d = s.add_block(pos + 3, bh, (uint32_t)s.frames.size() - 1, bif++, src.buf + pos + 3, cur);
+            s.frames.back().nblocks++;
+            pos += 3 + bh.content_size;
+            p.in_bytes += 3 + bh.content_size; p.out_bound += out; p.nblocks++; p.nseq += seqs;
+            if (d.host_status) { p.ends = true; break; }   // the frame fails at this block; nothing after it is looked at
+            if (bh.last) {
+                active = false;
+                if (checksum) {
+                    if (!src.fill(pos + 4)) { s.frames.back().host_status = mk_status(B200Z_ERR_FAILED_TO_READ_CHECKSUM, B200Z_STAGE_CHECKSUM); p.ends = true; break; }
+                    p.frames.back().has_checksum = true;
+                    p.frames.back().checksum = rd32le(src.buf + pos);
+                    pos += 4; p.in_bytes += 4;
+                }
+            }
+        }
+        p.cut = pos;
+        p.skips_after = skips;
+        if (active && !p.ends) {   // the active frame continues: its state, tables and tail are carried
+            p.continues = true;
+            p.cur_end = cur;
+            cont.on = true;
+            cont.frame = p.frames.back();
+            cont.frame.skips_before = 0;
+            cont.window = window;
+            cont.checksum = checksum;
+            cont.next_block = bif;
+            cont.dict = fdict;
+            // the tables its next block starts from: a table built here is copied to the carry slots after the pass
+            auto fse_of = [](const FseSlot *sl, int which) -> const FseTab * { return which == 0 ? &sl->ll : (which == 1 ? &sl->of : &sl->ml); };
+            auto next_fse = [&](const TabRef &t, int which) -> const FseTab * {
+                if (t.kind == TabRef::SLOT) return fse_of(carry_fse, which);
+                if (t.kind == TabRef::PREDEF) return fse_of(predef, which);
+                if (t.kind == TabRef::CARRY) { const CarrySet &cs = s.carries[t.idx]; return which == 0 ? cs.ll : (which == 1 ? cs.of : cs.ml); }
+                return nullptr;
+            };
+            CarrySet next;
+            next.huf = cur.huf.kind == TabRef::SLOT ? carry_huf : (cur.huf.kind == TabRef::CARRY ? s.carries[cur.huf.idx].huf : nullptr);
+            next.ll = next_fse(cur.ll, 0); next.of = next_fse(cur.of, 1); next.ml = next_fse(cur.ml, 2);
+            cont.tables = next;
+        }
+    }
+};
+
+struct SdSlice { const uint8_t *p; size_t len; };
+long sd_slice_read(void *user, uint8_t *buf, size_t n) {
+    SdSlice *s = (SdSlice *)user;
+    const size_t k = std::min(n, s->len);
+    if (k) memcpy(buf, s->p, k);
+    s->p += k; s->len -= k;
+    return (long)k;
+}
+
+}  // namespace
+
+struct StreamDecodeResources {
+    uint64_t chunk = 0;
+    // s_d2h brings back each submission's frame states behind its pass; s_out the plaintext (and a failing frame's block sizes) of a
+    // submission whose states are back.  On one stream the plaintext of k - 1 would queue behind the wait for k's pass.
+    Stream s_h2d, s_d2h, s_out;
+    // ev_read[s]: recorded on the kernel stream once the next submission's k_carry has read slot s (its frame states, placement and
+    // tail), so that an upload into slot s waits for it, not only for slot s's own pass
+    Event ev_h2d[2], ev_k[2], ev_d2h[2], ev_read[2];
+    PinnedBuf h_in[2], h_out, h_states[2];
+    DevBuf d_in[2], d_out[2];
+    DevBuf d_tab_huf, d_tab_fse;   // the continuing frame's tables built in the previous submission (HufSlot, FseSlot)
+    DevBuf d_carry;                // StreamCarry[2]: what flows into the submission of slot s
+    Submission sub[2];
+    uint64_t window = 0;           // d_out[] holds a tail of max(window, 32) bytes
+};
+
+static uint64_t sd_chunk_bytes() {
+    uint64_t C = 64ull << 20;
+    if (const char *ev = getenv("B200Z_PIPELINE_CHUNK_BYTES")) { const uint64_t v = strtoull(ev, nullptr, 10); if (v) C = v; }
+    return C;
+}
+
+// every buffer sized for the chunk once, so that the memory held depends on the chunk and the largest window only
+static int sd_get(b200z_ctx *c, uint64_t C, StreamDecodeResources **out) {
+    if (!c->sdec || c->sdec->chunk != C) {
+        c->sdec.reset();
+        std::unique_ptr<StreamDecodeResources> r(new StreamDecodeResources());
+        r->chunk = C;
+        if (r->s_h2d.create(c) || r->s_d2h.create(c) || r->s_out.create(c)) return B200Z_ERR_CUDA;
+        for (int i = 0; i < 2; i++)
+            if (r->ev_h2d[i].create(c) || r->ev_k[i].create(c) || r->ev_d2h[i].create(c) || r->ev_read[i].create(c)) return B200Z_ERR_CUDA;
+        const SdBounds b(C);
+        const uint64_t nb = b.blocks, nf = nb + 1, room = b.out_room();
+        int e = 0;
+        for (int i = 0; i < 2 && !e; i++) {
+            Submission &s = r->sub[i];
+            if ((e = r->h_in[i].ensure(b.buffer(), false)) || (e = r->h_states[i].ensure(nf * sizeof(FrameState), false)) ||
+                (e = r->d_in[i].ensure(b.buffer() + 32, false)) || (e = s.d_descs.ensure(nb * sizeof(BlockDesc), false)) ||
+                (e = s.d_aux.ensure(nb * sizeof(BlockAux), false)) || (e = s.d_frames.ensure(nf * sizeof(FrameDesc), false)) ||
+                (e = s.d_states.ensure(nf * sizeof(FrameState), false)) || (e = s.d_huf.ensure(nb * sizeof(HufSlot), false)) ||
+                (e = s.d_fse.ensure(nb * sizeof(FseSlot), false)) || (e = s.d_lit.ensure(room + 32 * nb + 64, false)) ||
+                (e = s.d_seq.ensure((b.seqs + 4 * nb + 4) * 12, false)) || (e = s.d_order.ensure(4 * nb, false)) ||
+                (e = s.d_sched.ensure(2 * (16 + 4 * nf) + 4 * nf + 32, false)))
+                break;
+        }
+        if (!e && !(e = r->h_out.ensure(room + 64, false)) && !(e = r->d_tab_huf.ensure(sizeof(HufSlot), false)) && !(e = r->d_tab_fse.ensure(sizeof(FseSlot), false)))
+            e = r->d_carry.ensure(2 * sizeof(StreamCarry), false);
+        if (e) { c->err = "decode_all_stream: out of memory for chunks of " + std::to_string(C) + " bytes"; return e; }
+        c->sdec = std::move(r);
+    }
+    *out = c->sdec.get();
+    return 0;
+}
+
+static int sd_write(b200z_write_fn wr, void *wu, const uint8_t *p, size_t n, uint64_t *delivered) {   // write_all; false on a write <= 0
+    while (n) {
+        const long w = wr(wu, p, n);
+        if (w <= 0 || (size_t)w > n) return 0;
+        p += w; n -= (size_t)w; *delivered += (uint64_t)w;
+    }
+    return 1;
+}
+
+extern "C" int b200z_decode_all_stream(b200z_ctx *c, b200z_read_fn rd, void *ru, b200z_write_fn wr, void *wu, const b200z_dict *const *dicts, size_t ndicts,
+                                       const b200z_dict *forced, uint64_t max_window, b200z_stream_result *result) {
+    if (!c || !rd || !wr || !result || (!dicts && ndicts)) return B200Z_ERR_INVALID_ARGUMENT;
+    if (int e = c->use()) return e;
+    const uint64_t C = sd_chunk_bytes();
+    StreamDecodeResources *R = nullptr;
+    if (int e = sd_get(c, C, &R)) return e;
+    b200z_stream_result res;
+    memset(&res, 0, sizeof res);
+    res.first_mismatch_frame = -1;
+    res.all.error_frame = -1;
+    SdPlanner pl(C, dicts, ndicts, forced, max_window);
+    pl.carry_huf = R->d_tab_huf.as<HufSlot>(); pl.carry_fse = R->d_tab_fse.as<FseSlot>(); pl.predef = c->d_predef.as<FseSlot>();
+    SdSource src;
+    src.rd = rd; src.user = ru; src.cap = (size_t)SdBounds(C).buffer();
+    src.buf = R->h_in[0].as<uint8_t>();
+    SdPlan plan[2];
+    const bool hash = (c->flags & B200Z_FLAG_CHECKSUM) != 0;
+    const PipelineStreams ps{c->stream, c->side, c->ev_fork, c->ev_join};
+    StreamCarry *d_carry = R->d_carry.as<StreamCarry>();
+    const uint64_t room = SdBounds(C).out_room();
+    uint64_t cont_total = 0;     // plaintext of the continuing frame before the submission being retired
+    bool stopped = false;
+    auto out_cap_of = [&](const SdPlan &p) { return (p.resumed ? std::max<uint64_t>(p.resume_window, 32) : 0) + p.out_bound; };
+    auto enqueue = [&](int s) -> int {
+        const SdPlan &p = plan[s];
+        Submission &sub = R->sub[s];
+        if (p.frames.empty()) return 0;
+        // the tail room grows with the largest window seen; only this slot's buffer: the other holds the previous submission's
+        // plaintext, not yet written, and the tail k_carry reads
+        R->window = std::max(R->window, pl.max_window_seen);
+        const uint64_t out_need = std::max<uint64_t>(R->window, 32) + room + 64;
+        if (out_need > R->d_out[s].cap) {
+            CU(c, cudaEventSynchronize(R->ev_read[s]));   // the previous submission's k_carry may still read the tail there
+            if (int e = R->d_out[s].ensure(out_need, false)) return e;
+        }
+        CU(c, cudaStreamWaitEvent(R->s_h2d, R->ev_k[s], 0));      // the submission two back is done with slot s
+        CU(c, cudaStreamWaitEvent(R->s_h2d, R->ev_read[s], 0));   // and the previous one's k_carry has read it
+        if (p.cut) CU(c, cudaMemcpyAsync(R->d_in[s].p, R->h_in[s].p, p.cut, cudaMemcpyHostToDevice, R->s_h2d));
+        if (int e = sub.upload(c, R->s_h2d)) return e;
+        CU(c, cudaEventRecord(R->ev_h2d[s], R->s_h2d));
+        CU(c, cudaStreamWaitEvent(c->stream, R->ev_h2d[s], 0));
+        PipelineArgs a = sub.args(R->d_in[s].as<uint8_t>(), R->d_out[s].as<uint8_t>(), out_cap_of(p));
+        if (p.resumed) {
+            const Submission &ps_ = R->sub[s ^ 1];
+            PipelineArgs prev = ps_.args(nullptr, R->d_out[s ^ 1].as<uint8_t>(), 0);
+            if (int le = launch_carry(prev, (uint32_t)ps_.frames.size() - 1, a, d_carry + (s ^ 1), d_carry + s, plan[s ^ 1].resumed && plan[s ^ 1].frames.size() == 1,
+                                      std::max<uint64_t>(p.resume_window, 32), c->stream, &c->launches))
+                return c->set_cuda_err((cudaError_t)le, "k_carry");
+        }
+        CU(c, cudaEventRecord(R->ev_read[s ^ 1], c->stream));
+        if (int e = enqueue_decode_all_stages(c, a, ps, p.resumed, &c->launches)) return e;
+        if (hash)
+            if (int le = launch_checksum_stream(a, d_carry + s, d_carry + (s ^ 1), p.resumed, p.continues, c->stream, &c->launches))
+                return c->set_cuda_err((cudaError_t)le, "k_xxh64_stream");
+        if (p.continues) {   // the continuing frame's tables built here, for the next submission (the host knows which: no wait)
+            const TableCursor &t = p.cur_end;
+            if (t.huf.kind == TabRef::SLOT)
+                CU(c, cudaMemcpyAsync(R->d_tab_huf.p, sub.d_huf.as<HufSlot>() + t.huf.idx, sizeof(HufSlot), cudaMemcpyDeviceToDevice, c->stream));
+            FseSlot *dst = R->d_tab_fse.as<FseSlot>();
+            const FseSlot *src_slots = sub.d_fse.as<FseSlot>();
+            if (t.ll.kind == TabRef::SLOT) CU(c, cudaMemcpyAsync(&dst->ll, &src_slots[t.ll.idx].ll, sizeof(FseTab), cudaMemcpyDeviceToDevice, c->stream));
+            if (t.of.kind == TabRef::SLOT) CU(c, cudaMemcpyAsync(&dst->of, &src_slots[t.of.idx].of, sizeof(FseTab), cudaMemcpyDeviceToDevice, c->stream));
+            if (t.ml.kind == TabRef::SLOT) CU(c, cudaMemcpyAsync(&dst->ml, &src_slots[t.ml.idx].ml, sizeof(FseTab), cudaMemcpyDeviceToDevice, c->stream));
+        }
+        CU(c, cudaEventRecord(R->ev_k[s], c->stream));
+        CU(c, cudaStreamWaitEvent(R->s_d2h, R->ev_k[s], 0));
+        CU(c, cudaMemcpyAsync(R->h_states[s].p, sub.d_states.p, sub.frames.size() * sizeof(FrameState), cudaMemcpyDeviceToHost, R->s_d2h));
+        CU(c, cudaEventRecord(R->ev_d2h[s], R->s_d2h));
+        res.submissions++;
+        return 0;
+    };
+    // the outcome of the submission in slot s, in stream order: its plaintext up to the first failing block goes to the drain
+    auto retire = [&](int s) -> int {
+        const SdPlan &p = plan[s];
+        const Submission &sub = R->sub[s];
+        b200z_all_result all = res.all;
+        uint64_t ck = res.checksum_frames, mism = res.checksum_mismatches;
+        int64_t first_mism = res.first_mismatch_frame;
+        uint64_t T0 = 0, len = 0, total = cont_total;
+        bool failed = false;
+        if (!p.frames.empty()) {
+            CU(c, cudaEventSynchronize(R->ev_d2h[s]));
+            const FrameState *st = R->h_states[s].as<FrameState>();
+            if (p.resumed) T0 = std::min<uint64_t>(cont_total, std::max<uint64_t>(p.resume_window, 32));
+            for (size_t f = 0; f < p.frames.size(); f++) {
+                const SdFrame &F = p.frames[f];
+                all.skippable_frames += F.skips_before;
+                const uint64_t before = f == 0 && p.resumed ? cont_total : 0, tail = f == 0 ? T0 : 0;
+                if (st[f].status) {
+                    // the frame's output before its first failing block (blocks_done counts this submission's blocks)
+                    const FrameDesc &fd = sub.frames[f];
+                    const uint32_t n = std::min(st[f].blocks_done, fd.nblocks);
+                    if (n) {
+                        std::vector<BlockAux> aux(n);
+                        CU(c, cudaMemcpyAsync(aux.data(), sub.d_aux.as<BlockAux>() + fd.first_block, n * sizeof(BlockAux), cudaMemcpyDeviceToHost, R->s_out));
+                        CU(c, cudaStreamSynchronize(R->s_out));
+                        for (uint32_t k = 0; k < n; k++) len += aux[k].out_size;
+                    }
+                    uint32_t word = st[f].status;
+                    // a block that decodes to more than its bound (RFC 8878 forbids it) ran out of the submission's output room
+                    if (status_code(word) == B200Z_ERR_TARGET_TOO_SMALL) word = mk_status(B200Z_ERR_BLOCK_OUTPUT_LIMIT, B200Z_STAGE_EXECUTE);
+                    all.status = (int32_t)status_code(word); all.stage = (int32_t)status_stage(word);
+                    all.error_offset = F.at; all.error_frame = F.zi;
+                    failed = true;
+                    break;
+                }
+                const uint64_t fresh = st[f].produced - tail;
+                len += fresh;
+                if (f + 1 == p.frames.size() && p.continues) { total = before + fresh; continue; }
+                all.frames++; all.written += before + fresh;
+                if (hash && F.has_checksum) {
+                    ck++;
+                    if ((uint32_t)st[f].xxh64 != F.checksum) { mism++; if (first_mism < 0) first_mism = F.zi; }
+                }
+            }
+        }
+        if (!failed) {
+            all.skippable_frames += p.skips_after;
+            if (p.end_word) {
+                all.status = (int32_t)status_code(p.end_word); all.stage = (int32_t)status_stage(p.end_word);
+                all.error_offset = p.end_at; all.error_frame = p.end_zi;
+                failed = true;
+            }
+        }
+        if (len) {
+            // the states are back, so this submission's pass is over; the next one keeps running meanwhile
+            CU(c, cudaMemcpyAsync(R->h_out.p, R->d_out[s].as<uint8_t>() + T0, len, cudaMemcpyDeviceToHost, R->s_out));
+            CU(c, cudaStreamSynchronize(R->s_out));
+            if (!sd_write(wr, wu, R->h_out.as<uint8_t>(), len, &res.delivered)) {
+                res.all.status = B200Z_ERR_FAILED_TO_DRAIN_DECODEBUFFER; res.all.stage = B200Z_STAGE_DRAIN;
+                res.all.error_offset = p.frames.front().at; res.all.error_frame = p.frames.front().zi;
+                stopped = true;
+                return 0;
+            }
+        }
+        res.all = all;
+        res.checksum_frames = ck; res.checksum_mismatches = mism; res.first_mismatch_frame = first_mism;
+        cont_total = total;
+        if (failed) stopped = true;
+        return 0;
+    };
+    int e = 0;
+    pl.plan(src, R->sub[0], plan[0]);
+    for (int k = 0; !e; k++) {
+        const int s = k & 1;
+        if ((e = enqueue(s))) break;
+        if (k && (e = retire(s ^ 1))) break;
+        if (stopped) break;
+        if (plan[s].ends) { e = retire(s); break; }
+        // the next submission: its buffer (slot s ^ 1) is free once the upload of the submission two back is done
+        if (k && cudaEventSynchronize(R->ev_h2d[s ^ 1]) != cudaSuccess) { e = c->set_cuda_err(cudaGetLastError(), "upload"); break; }
+        src.advance(plan[s].cut, R->h_in[s ^ 1].as<uint8_t>());
+        pl.plan(src, R->sub[s ^ 1], plan[s ^ 1]);
+    }
+    // leave nothing in flight: the buffers are reused by the next call
+    cudaStreamSynchronize(R->s_h2d);
+    cudaStreamSynchronize(c->stream);
+    cudaStreamSynchronize(R->s_d2h);
+    cudaStreamSynchronize(R->s_out);
+    // now both slots take the largest window's tail, so that what the context holds does not depend on how many submissions ran
+    for (DevBuf &d : R->d_out)
+        if (!e) e = d.ensure(std::max<uint64_t>(R->window, 32) + room + 64, false);
+    if (!res.all.status) res.all.error_offset = src.off + src.have;
+    *result = res;
+    return e;
+}
+
+// b200z_debug_stream_cut: the planner alone over a byte string, with host buffers (no context, no device)
+extern "C" int b200z_debug_stream_cut(const uint8_t *input, size_t input_len, uint64_t chunk, b200z_stream_cut *cuts, size_t cap, size_t *n,
+                                      b200z_stream_cut_end *end) {
+    if (!n || !end || (!input && input_len) || (!cuts && cap) || !chunk) return B200Z_ERR_INVALID_ARGUMENT;
+    SdSlice sr{input, input_len};
+    SdPlanner pl(chunk, nullptr, 0, nullptr, 0);
+    static const FseSlot *const fake = reinterpret_cast<const FseSlot *>(16);   // table pointers are never dereferenced here
+    pl.carry_huf = reinterpret_cast<const HufSlot *>(16); pl.carry_fse = fake; pl.predef = fake;
+    SdSource src;
+    src.rd = sd_slice_read; src.user = &sr; src.cap = (size_t)pl.bnd.buffer();
+    std::vector<uint8_t> buf[2] = {std::vector<uint8_t>(src.cap), std::vector<uint8_t>(src.cap)};
+    src.buf = buf[0].data();
+    Submission sub;
+    SdPlan p;
+    size_t k = 0;
+    memset(end, 0, sizeof *end);
+    end->error_frame = -1;
+    for (;; k++) {
+        pl.plan(src, sub, p);
+        if (!p.frames.empty()) {
+            if (k < cap) {
+                b200z_stream_cut &o = cuts[k];
+                o.start = p.start; o.end = p.start + p.cut; o.in_bytes = p.in_bytes; o.out_bound = p.out_bound; o.nblocks = p.nblocks;
+                o.nseq = p.nseq; o.nframes = (uint32_t)p.frames.size(); o.flags = (p.resumed ? 1u : 0u) | (p.continues ? 2u : 0u);
+            }
+        } else k--;
+        end->skippable_frames += p.skips_after;
+        for (const SdFrame &f : p.frames) end->skippable_frames += f.skips_before;
+        if (p.ends) {
+            end->status = (int32_t)status_code(p.end_word); end->stage = (int32_t)status_stage(p.end_word);
+            if (!p.end_word && !sub.frames.empty()) {   // a frame that fails on a header the planner read (block header, truncation)
+                const uint32_t hs = sub.frames.back().host_status;
+                if (hs) { end->status = (int32_t)status_code(hs); end->stage = (int32_t)status_stage(hs); }
+                else for (const BlockDesc &d : sub.descs) if (d.host_status) { end->status = (int32_t)status_code(host_status_word(d.host_status)); end->stage = (int32_t)status_stage(host_status_word(d.host_status)); }
+                if (end->status) { end->error_offset = p.frames.back().at; end->error_frame = p.frames.back().zi; }
+            }
+            if (p.end_word) { end->error_offset = p.end_at; end->error_frame = p.end_zi; }
+            if (!end->status) end->error_offset = src.off + p.cut;
+            k++;
+            break;
+        }
+        src.advance(p.cut, buf[(k + 1) & 1].data());
+    }
+    end->peak_buffered = src.peak;
+    *n = k;
     return 0;
 }
 

@@ -155,6 +155,15 @@ struct alignas(16) FrameState {
     uint64_t pad;
 };
 
+// What the stream decoder (tier 1d) carries on the device into a submission whose first frame continues from the one before:
+// the frame's plaintext bytes before the submission (k_carry), and, with the checksum, its XXH64 accumulators after `stripes`
+// whole 32-byte stripes (k_xxh64_stream).  The carried tail of the frame's output holds the bytes hashed after those stripes.
+struct alignas(16) StreamCarry {
+    uint64_t v[4];
+    uint64_t stripes;
+    uint64_t total;
+};
+
 struct alignas(16) FrameDesc {
     uint64_t out_off;         // where the frame's byte 0 lives in the output buffer
     uint64_t out_cap;         // room at out_off

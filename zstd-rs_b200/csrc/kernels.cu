@@ -1410,8 +1410,11 @@ __global__ void __launch_bounds__(256) k_find_frames(const uint8_t *__restrict__
 // ------------------------------------------------------------------------------------------------------------
 constexpr uint32_t PLACE_THREADS = 1024, PLACE_PER_THREAD = 4;
 
-__global__ void __launch_bounds__(PLACE_THREADS) k_place(const BlockDesc *__restrict__ descs, const BlockAux *__restrict__ aux,
-                                                         FrameDesc *__restrict__ frames, uint32_t nframes, uint64_t output_cap) {
+// RESUME (k_place_resume): the first frame continues from the stream decoder's previous submission; its carried tail of
+// states[0].produced bytes sits at the front of the output (k_carry), so it is placed at 0 with the tail counted in its size.
+template <bool RESUME>
+__device__ __forceinline__ void place_frames(const BlockDesc *__restrict__ descs, const BlockAux *__restrict__ aux, FrameDesc *__restrict__ frames,
+                                             uint32_t nframes, uint64_t output_cap, const FrameState *__restrict__ states) {
     __shared__ uint64_t warp_sum[PLACE_THREADS / 32];
     __shared__ uint64_t carry_s;
     const uint32_t t = threadIdx.x, lane = t & 31, warp = t >> 5;
@@ -1422,7 +1425,7 @@ __global__ void __launch_bounds__(PLACE_THREADS) k_place(const BlockDesc *__rest
 #pragma unroll
         for (uint32_t k = 0; k < PLACE_PER_THREAD; k++) {
             const uint32_t f = tile + t * PLACE_PER_THREAD + k;
-            uint64_t s = 0;
+            uint64_t s = RESUME && f == 0 ? states[0].produced : 0;
             if (f < nframes) {
                 const uint32_t b0 = frames[f].first_block, nb = frames[f].nblocks;
                 for (uint32_t b = b0; b < b0 + nb; b++) {
@@ -1466,6 +1469,104 @@ __global__ void __launch_bounds__(PLACE_THREADS) k_place(const BlockDesc *__rest
         __syncthreads();
         if (t == PLACE_THREADS - 1) carry_s = at;
         __syncthreads();
+    }
+}
+
+__global__ void __launch_bounds__(PLACE_THREADS) k_place(const BlockDesc *__restrict__ descs, const BlockAux *__restrict__ aux,
+                                                         FrameDesc *__restrict__ frames, uint32_t nframes, uint64_t output_cap) {
+    place_frames<false>(descs, aux, frames, nframes, output_cap, nullptr);
+}
+__global__ void __launch_bounds__(PLACE_THREADS) k_place_resume(const BlockDesc *__restrict__ descs, const BlockAux *__restrict__ aux,
+                                                                FrameDesc *__restrict__ frames, uint32_t nframes, uint64_t output_cap,
+                                                                const FrameState *__restrict__ states) {
+    place_frames<true>(descs, aux, frames, nframes, output_cap, states);
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// k_carry (stream decoder, tier 1d): hands the frame that continues past a submission (frame `plast` of the previous one: pframes /
+// pstates / pout) to the next submission (frame 0: nframes_ / nstates / nout), device to device.  When the frame failed, the next
+// frame state only takes its status.  The frame's last T = min(produced, max(window, 32)) bytes go to the front of the next output, so that offsets reach
+// back into them (and the checksum finds the bytes after its last whole stripe there); the next frame state continues the offset
+// history and total_output_counter with produced = T, drained = 0; the frame is placed at 0 with T bytes so far.  StreamCarry::total:
+// the frame's plaintext bytes before the previous submission (carry_prev, when `resumed`: the frame continued into it) and before the
+// next one (carry_next).  Every thread copies 16-byte pieces of the tail, grid-stride; thread 0 writes the state.
+// ------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_carry(const FrameDesc *__restrict__ pframes, const FrameState *__restrict__ pstates, uint32_t plast,
+                                               const uint8_t *__restrict__ pout, FrameDesc *__restrict__ nframes_, FrameState *__restrict__ nstates,
+                                               uint8_t *__restrict__ nout, const StreamCarry *__restrict__ carry_prev,
+                                               StreamCarry *__restrict__ carry_next, uint32_t resumed) {
+    const FrameState &ps = pstates[plast];
+    if (ps.status) {
+        // the frame failed: the host stops at it and discards the next submission, which is already in flight.  Its first frame
+        // starts failed, so that the execution kernels and the hash pass over it at once.
+        if (blockIdx.x == 0 && threadIdx.x == 0) {
+            FrameState n = {};
+            n.status = ps.status;
+            nstates[0] = n;
+        }
+        return;
+    }
+    const uint64_t window = pframes[plast].window_size, keep = window > 32 ? window : 32;
+    const uint64_t produced = ps.produced, T = produced < keep ? produced : keep;
+    const uint8_t *src = pout + pframes[plast].out_off + (produced - T);
+    // 16 bytes per piece: two aligned 16-byte loads of the source, shifted into place, one aligned store
+    const uintptr_t sa = (uintptr_t)src, base = sa & ~(uintptr_t)15;
+    const uint32_t sh = (uint32_t)(sa & 15);
+    const uint64_t pieces = (T + 15) >> 4;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < pieces; i += (uint64_t)gridDim.x * blockDim.x) {
+        const ulonglong2 a = reinterpret_cast<const ulonglong2 *>(base)[i];
+        ulonglong2 o = a;
+        if (sh) {
+            const ulonglong2 b = reinterpret_cast<const ulonglong2 *>(base)[i + 1];
+            const uint32_t s8 = (sh & 7) * 8;
+            const uint64_t w0 = sh < 8 ? a.x : a.y, w1 = sh < 8 ? a.y : b.x, w2 = sh < 8 ? b.x : b.y;
+            o.x = s8 ? (w0 >> s8) | (w1 << (64 - s8)) : w0;
+            o.y = s8 ? (w1 >> s8) | (w2 << (64 - s8)) : w1;
+        }
+        reinterpret_cast<ulonglong2 *>(nout)[i] = o;
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        const uint64_t before = resumed ? carry_prev->total : 0, tail_before = before < keep ? before : keep;
+        carry_next->total = before + (produced - tail_before);
+        FrameState n;
+        n.hist[0] = ps.hist[0]; n.hist[1] = ps.hist[1]; n.hist[2] = ps.hist[2];
+        n.status = 0; n.produced = T; n.drained = 0; n.counter = ps.counter; n.error_block = 0; n.blocks_done = 0; n.xxh64 = 0; n.pad = 0;
+        nstates[0] = n;
+        nframes_[0].out_off = 0;
+        nframes_[0].out_cap = T;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// k_xxh64_stream: k_xxh64 for a stream decoder submission.  Frame 0 may resume (`resumed`): its accumulators and stripe count come
+// from carry_in, and its bytes after those stripes start in the carried tail at the front of the output.  The last frame may stop
+// mid-frame (`continues`): its whole stripes are folded in and the accumulators go to carry_out for the next submission.
+// ------------------------------------------------------------------------------------------------------------
+__global__ void k_xxh64_stream(const FrameDesc *__restrict__ frames, FrameState *__restrict__ states, const uint8_t *__restrict__ output,
+                               uint32_t nframes, const StreamCarry *__restrict__ carry_in, StreamCarry *__restrict__ carry_out, uint32_t resumed,
+                               uint32_t continues) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t f = t >> 2, k = t & 3;
+    if (f >= nframes) return;
+    const FrameState &st = states[f];
+    const FrameDesc &fd = frames[f];
+    const uint8_t *p = output + fd.out_off;
+    uint64_t len = st.status ? 0 : st.produced, done = 0, v = xxh64_init_lane(k);
+    if (f == 0 && resumed && !st.status) {
+        const uint64_t keep = fd.window_size > 32 ? fd.window_size : 32, total = carry_in->total, T = total < keep ? total : keep;
+        done = 32 * carry_in->stripes;
+        const uint64_t skip = T - (total - done);   // the tail's bytes before the first one not hashed yet
+        v = carry_in->v[k];
+        p += skip;
+        len = len > skip ? len - skip : 0;
+    }
+    const bool finish = !(continues && f == nframes - 1);
+    const uint64_t h = xxh64_group_resume(p, len, k, v, done, finish);
+    if (finish) {
+        if (k == 0) states[f].xxh64 = h;
+    } else if (!st.status) {
+        carry_out->v[k] = v;
+        if (k == 0) carry_out->stripes = done / 32 + (len >> 5);
     }
 }
 
@@ -1590,9 +1691,31 @@ int launch_place(const PipelineArgs &a, cudaStream_t s, uint64_t *launched) {
     return launched_one(launched);
 }
 
+int launch_place_resume(const PipelineArgs &a, cudaStream_t s, uint64_t *launched) {
+    if (!a.nframes) return 0;
+    k_place_resume<<<1, PLACE_THREADS, 0, s>>>(a.descs, a.aux, const_cast<FrameDesc *>(a.frames), a.nframes, a.output_cap, a.states);
+    return launched_one(launched);
+}
+
 int launch_checksum(const PipelineArgs &a, cudaStream_t s, uint64_t *launched) {
     if (!a.nframes) return 0;
     k_xxh64<<<cdiv(a.nframes * 4, 128), 128, 0, s>>>(a.frames, a.states, a.output, a.nframes);
+    return launched_one(launched);
+}
+
+int launch_checksum_stream(const PipelineArgs &a, const StreamCarry *carry_in, StreamCarry *carry_out, bool resumed, bool continues, cudaStream_t s,
+                           uint64_t *launched) {
+    if (!a.nframes) return 0;
+    k_xxh64_stream<<<cdiv(a.nframes * 4, 128), 128, 0, s>>>(a.frames, a.states, a.output, a.nframes, carry_in, carry_out, resumed, continues);
+    return launched_one(launched);
+}
+
+int launch_carry(const PipelineArgs &prev, uint32_t plast, const PipelineArgs &next, const StreamCarry *carry_prev, StreamCarry *carry_next, bool resumed,
+                 uint64_t max_tail, cudaStream_t s, uint64_t *launched) {
+    const uint64_t pieces = (max_tail + 15) / 16, most = (uint64_t)num_sms() * 8;
+    const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((pieces + 255) / 256, most));
+    k_carry<<<grid, 256, 0, s>>>(prev.frames, prev.states, plast, prev.output, const_cast<FrameDesc *>(next.frames), next.states, next.output, carry_prev,
+                                 carry_next, resumed);
     return launched_one(launched);
 }
 

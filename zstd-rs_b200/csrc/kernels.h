@@ -52,6 +52,14 @@ int launch_find_frames(const uint8_t *d_input, uint64_t input_len, uint64_t *d_o
 int launch_place(const PipelineArgs &a, cudaStream_t s, uint64_t *launched);
 uint32_t num_sms();   // of the current device (132 on H100 SXM)
 int launch_checksum(const PipelineArgs &a, cudaStream_t s, uint64_t *launched);   // optional 5th stage: XXH64 of every frame's plaintext
+// the stream decoder (tier 1d): k_place_resume places a submission whose first frame continues behind its carried tail; k_carry hands
+// frame `plast` of `prev` to frame 0 of `next` (max_tail: the most bytes it may carry, max(window, 32)); k_xxh64_stream hashes frames
+// that may resume from carry_in and stop mid-frame into carry_out
+int launch_place_resume(const PipelineArgs &a, cudaStream_t s, uint64_t *launched);
+int launch_carry(const PipelineArgs &prev, uint32_t plast, const PipelineArgs &next, const StreamCarry *carry_prev, StreamCarry *carry_next, bool resumed,
+                 uint64_t max_tail, cudaStream_t s, uint64_t *launched);
+int launch_checksum_stream(const PipelineArgs &a, const StreamCarry *carry_in, StreamCarry *carry_out, bool resumed, bool continues, cudaStream_t s,
+                           uint64_t *launched);
 struct PipelineStreams { cudaStream_t main, side; cudaEvent_t fork, join; };
 int launch_pipeline_overlapped(const PipelineArgs &a, const PipelineStreams &ps, uint64_t *launched);   // the shipped order: k_exec beside k_fse (programmatic dependent launch)
 int launch_tables_literals(const PipelineArgs &a, const PipelineStreams &ps, uint64_t *launched);   // k_setup (literals side + k_huf on `side`, sequences side on `main`)
