@@ -269,6 +269,9 @@ int b200z_batch_debug_tables(b200z_batch *b, uint32_t block, uint8_t *huf_out, u
 /* execution scheduling counters of the last run (tests / profiling): [0] frames given to k_exec_cta (block assembled in
  * shared memory), [1] frames it handed back to k_exec (one warp per frame), [2] OR of the reasons, [3] blocks handed back */
 int b200z_batch_debug_sched(b200z_batch *b, uint32_t out[4]);
+/* waves the literal and sequence kernels take for this batch's blocks on its device (a wave = every CTA resident at once):
+ * [0] k_huf, [1] k_fse, [2] k_huf's resident CTAs per SM with the bit-reader ring it takes for this batch, [3] k_fse's */
+int b200z_batch_debug_waves(b200z_batch *b, uint32_t out[4]);
 /* Host-only views of a submission's scheduling decisions (no context, no device; for CPU tests of the host logic).
  * b200z_debug_route_frames: which frames k_exec_cta would take (largest first) given each frame's work (sequences + compressed
  * bytes / 16) and whether it is eligible (>= 2 blocks, >= 4096 compressed bytes, no dictionary); cta_frames has room for nframes.

@@ -117,6 +117,7 @@ def lib():
         "b200z_batch_debug_sequences": (C.c_int, [vp, C.c_uint32, vp, sz, C.POINTER(sz)]),
         "b200z_batch_debug_block_flags": (C.c_int, [vp, C.c_uint32, C.POINTER(C.c_uint32)]),
         "b200z_batch_debug_sched": (C.c_int, [vp, C.POINTER(C.c_uint32)]),
+        "b200z_batch_debug_waves": (C.c_int, [vp, C.POINTER(C.c_uint32)]),
         "b200z_batch_debug_tables": (C.c_int, [vp, C.c_uint32, vp, vp, C.POINTER(C.c_uint32)]),
         "b200z_debug_route_frames": (C.c_int, [vp, vp, sz, C.c_uint32, vp, C.POINTER(sz)]),
         "b200z_debug_fse_order": (C.c_int, [vp, vp, vp, sz, vp, sz, vp, C.POINTER(sz)]),
@@ -852,6 +853,11 @@ class Batch:
         a = (C.c_uint32 * 4)()
         self.ctx._chk(self.ctx.L.b200z_batch_debug_sched(self.h, a))
         return {"cta_frames": a[0], "handed_back_frames": a[1], "reasons": a[2], "handed_back_blocks": a[3]}
+
+    def debug_waves(self):
+        a = (C.c_uint32 * 4)()
+        self.ctx._chk(self.ctx.L.b200z_batch_debug_waves(self.h, a))
+        return {"k_huf": a[0], "k_fse": a[1], "k_huf_ctas_per_sm": a[2], "k_fse_ctas_per_sm": a[3]}
 
     def debug_block_flags(self, block):
         v = C.c_uint32()

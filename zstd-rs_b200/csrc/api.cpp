@@ -917,6 +917,13 @@ extern "C" int b200z_batch_debug_sched(b200z_batch *b, uint32_t out[4]) {
     out[1] = h[1]; out[2] = h[2]; out[3] = h[3];
     return 0;
 }
+// waves of the literal and sequence kernels for this batch's blocks: [0] k_huf, [1] k_fse, [2] / [3] their resident CTAs per SM
+extern "C" int b200z_batch_debug_waves(b200z_batch *b, uint32_t out[4]) {
+    if (!b || !out) return B200Z_ERR_INVALID_ARGUMENT;
+    if (cudaSetDevice(b->ctx->device) != cudaSuccess) { cudaGetLastError(); return B200Z_ERR_CUDA; }
+    entropy_waves((uint32_t)b->sub.descs.size(), out);
+    return 0;
+}
 extern "C" void b200z_batch_destroy(b200z_batch *b) {
     if (!b) return;
     cudaSetDevice(b->ctx->device);

@@ -17,6 +17,7 @@
 #include <limits.h>
 #include <stdlib.h>
 #include <stdint.h>
+#include <type_traits>
 
 #include "kernels.h"
 #include "setup.cuh"
@@ -127,8 +128,6 @@ __device__ __forceinline__ uint32_t shl_c(uint32_t a, uint32_t n) { uint32_t r; 
 __device__ __forceinline__ uint32_t fsl_c(uint32_t lo, uint32_t hi, uint32_t n) { return __funnelshift_lc(lo, hi, n); }
 __device__ __forceinline__ uint32_t bfind32(uint32_t a) { uint32_t r; asm("bfind.u32 %0, %1;" : "=r"(r) : "r"(a)); return r; }   // floor(log2 a)
 
-constexpr uint32_t RING_STRIDE = 144;   // bytes of shared memory per bitstream: a mirror group + 8 groups of 16 bytes (PosRing)
-
 // ---- shared-memory accessors by 32-bit shared address
 __device__ __forceinline__ uint32_t lds32(uint32_t a) { uint32_t v; asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(a) : "memory"); return v; }
 __device__ __forceinline__ uint2 lds64(uint32_t a) { uint2 v; asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(a) : "memory"); return v; }
@@ -143,28 +142,47 @@ __device__ __forceinline__ void red_or_shared(uint32_t a, uint32_t v) { asm vola
 
 // Position-based reversed bit reader for the fast paths of k_fse and k_huf.  The only state is P = bits_remaining()
 // (bit_reader_reverse.rs:27-29); every read assembles the 64 bits below position P from three words of a per-lane
-// shared-memory ring (8 groups of 16 bytes + a mirror of the top group below slot 0, so that the three words are
-// always at a0, a0 - 4, a0 - 8) that cp.async keeps filled 7 groups ahead of consumption.  No window registers,
-// no refill / skip bookkeeping: a step costs 3 LDS + 2 funnel shifts.  Bits below the stream start are NOT
-// zeroed here: reading them makes P negative, which the caller checks (the block is then replayed by the exact
+// shared-memory ring (kSlots groups of kGroupBytes + a mirror of the top group below slot 0, so that the three words
+// are always at a0, a0 - 4, a0 - 8) that cp.async keeps filled kSlots - 1 groups ahead of consumption.  No window
+// registers, no refill / skip bookkeeping: a step costs 3 LDS + 2 funnel shifts.  Bits below the stream start are
+// NOT zeroed here: reading them makes P negative, which the caller checks (the block is then replayed by the exact
 // path, whose reader zero-fills like BitReaderReversed, bit_reader_reverse.rs:57-83).
+//
+// The geometry is the caller's: kWait, the cp.async.wait_group depth of service(), follows from how often it calls
+// service() (see FseRing and HufRing below).
+template <uint32_t kGroupBytes, uint32_t kSlots, uint32_t kWait>
 struct PosRing {
-    const uint4 *base;   // 16-byte aligned address at or below the stream start
-    uint32_t ring;       // shared-memory byte address of slot 0 (the mirror slot is at ring - 16)
+    static_assert((kGroupBytes == 8 || kGroupBytes == 16) && kSlots >= 4 && (kSlots & (kSlots - 1)) == 0, "PosRing geometry");
+    static constexpr uint32_t kStride = (kSlots + 1) * kGroupBytes;   // bytes of shared memory per bitstream: the mirror + the slots
+    static constexpr uint32_t kSlot0 = kGroupBytes;                   // offset of slot 0 in those bytes (the mirror slot comes first)
+    static constexpr uint32_t kGroupShift = kGroupBytes == 16 ? 7 : 6;   // log2 of the bits per group
+    static constexpr uint32_t kGroupBits = kGroupBytes * 8, kRingSlots = kSlots, kWaitDepth = kWait;
+    using Group = typename std::conditional<kGroupBytes == 16, uint4, uint2>::type;
+
+    const Group *base;   // kGroupBytes-aligned address at or below the stream start
+    uint32_t ring;       // shared-memory byte address of slot 0 (the mirror slot is at ring - kGroupBytes)
     int32_t gm1;         // bit offset of the stream's first byte inside group 0, minus 1
     int32_t next_g;      // next group to request (descending)
     int32_t P;           // bits_remaining()
 
     __device__ __forceinline__ uint32_t lds(uint32_t addr) const { uint32_t w; asm volatile("ld.shared.u32 %0, [%1];" : "=r"(w) : "r"(addr) : "memory"); return w; }
-    // request group g when `on` (predicated, no branch): slot g & 7, plus the mirror below slot 0 for slot 7
+    // request group g when `on` (predicated, no branch): slot g % kSlots, plus the mirror below slot 0 for the top slot.
+    // 16-byte copies bypass L1 (.cg); cp.async takes .cg for 16 bytes only, so 8-byte copies are .ca, and they ask L2 for
+    // the whole 128-byte line, which the next 15 requests of the lane read (k_huf alone on C2b: 0.71 -> 0.68 ms,
+    // H100 80GB HBM3 at a 700 W power limit).
     __device__ __forceinline__ void request(int32_t g, bool on) {
-        const uint32_t slot = (uint32_t)g & 7u;
-        const uint32_t dst = ring + (slot << 4);
-        const uint4 *src = base + g;
-        const uint32_t p1 = on ? 1u : 0u, p2 = (on && slot == 7u) ? 1u : 0u;
-        asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.u32 p, %3, 0;\n\tsetp.ne.u32 q, %4, 0;\n\t"
-                     "@p cp.async.cg.shared.global [%0], [%2], 16;\n\t@q cp.async.cg.shared.global [%1], [%2], 16;\n\t"
-                     "cp.async.commit_group;\n\t}" ::"r"(dst), "r"(ring - 16u), "l"(src), "r"(p1), "r"(p2) : "memory");
+        const uint32_t slot = (uint32_t)g & (kSlots - 1u);
+        const uint32_t dst = ring + slot * kGroupBytes;
+        const Group *src = base + g;
+        const uint32_t p1 = on ? 1u : 0u, p2 = (on && slot == kSlots - 1u) ? 1u : 0u;
+        if constexpr (kGroupBytes == 16)
+            asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.u32 p, %3, 0;\n\tsetp.ne.u32 q, %4, 0;\n\t"
+                         "@p cp.async.cg.shared.global [%0], [%2], 16;\n\t@q cp.async.cg.shared.global [%1], [%2], 16;\n\t"
+                         "cp.async.commit_group;\n\t}" ::"r"(dst), "r"(ring - 16u), "l"(src), "r"(p1), "r"(p2) : "memory");
+        else
+            asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.u32 p, %3, 0;\n\tsetp.ne.u32 q, %4, 0;\n\t"
+                         "@p cp.async.ca.shared.global.L2::128B [%0], [%2], 8;\n\t@q cp.async.ca.shared.global.L2::128B [%1], [%2], 8;\n\t"
+                         "cp.async.commit_group;\n\t}" ::"r"(dst), "r"(ring - 8u), "l"(src), "r"(p1), "r"(p2) : "memory");
     }
     __device__ __forceinline__ bool init(const uint8_t *src, uint32_t len, uint32_t ring_slot0) {
         ring = ring_slot0; base = nullptr; gm1 = -1; next_g = -1; P = 0;
@@ -172,35 +190,50 @@ struct PosRing {
         const uint32_t last = src[len - 1];
         if (last == 0) return false;
         const uintptr_t a = (uintptr_t)src;
-        base = (const uint4 *)(a & ~(uintptr_t)15);
-        gm1 = (int32_t)((uint32_t)(a & 15) * 8u) - 1;
+        base = (const Group *)(a & ~(uintptr_t)(kGroupBytes - 1));
+        gm1 = (int32_t)((uint32_t)(a & (kGroupBytes - 1)) * 8u) - 1;
         P = (int32_t)((len - 1) * 8u + (31u - (uint32_t)__clz((int)last)));
-        const int32_t gt = (gm1 + P) >> 7;    // group of the first data bit (-1 only for an empty stream at offset 0)
-        for (int32_t g = gt; g > gt - 8; g--) request(g, g >= 0);
-        next_g = gt - 8;
+        const int32_t gt = (gm1 + P) >> kGroupShift;   // group of the first data bit (-1 only for an empty stream at offset 0)
+        for (int32_t g = gt; g > gt - (int32_t)kSlots; g--) request(g, g >= 0);
+        next_g = gt - (int32_t)kSlots;
         asm volatile("cp.async.wait_group 0;" ::: "memory");
         return true;
     }
-    // the 64 bits below position P, left aligned in hi:lo (garbage once P < 64 bits from the stream start: unused)
+    // the 64 bits below position P, left aligned in hi:lo (garbage once P < 64 bits from the stream start: unused).
+    // The three words lie in the group of the next unread bit and the one below it.
     __device__ __forceinline__ void window(uint32_t &hi, uint32_t &lo) const {
-        const int32_t G = gm1 + P;                               // bit index (from `base`) of the next unread bit
-        const uint32_t a0 = ring + (((uint32_t)G >> 3) & 0x7cu);  // word (G >> 5) & 31 of the ring
+        const int32_t G = gm1 + P;                                                      // bit index (from `base`) of the next unread bit
+        const uint32_t a0 = ring + (((uint32_t)G >> 3) & ((kSlots * kGroupBytes - 1u) & ~3u));   // word G >> 5 of the ring, modulo its size
         const uint32_t A = lds(a0), B = lds(a0 - 4u), C = lds(a0 - 8u);
-        const uint32_t sh = ~(uint32_t)G;                         // 31 - (G & 31), the funnel shift uses the low 5 bits
+        const uint32_t sh = ~(uint32_t)G;                                                // 31 - (G & 31), the funnel shift uses the low 5 bits
         hi = __funnelshift_l(B, A, sh);
         lo = __funnelshift_l(C, B, sh);
     }
-    // Keeps the ring 7 groups ahead.  Call at least once per 116 consumed bits (every second sequence): consumption
-    // then leaves at most one group per call, so one request per call keeps up; the groups a step can touch before
-    // the next call (down to 2 below the current one) are complete after wait_group 5.
+    // Keeps the ring kSlots - 1 groups ahead with at most one request per call, which keeps up when the caller consumes
+    // at most one group between two calls.  Afterwards next_g <= gh - kSlots, and the requests are consecutive groups
+    // above next_g, one commit group per call: the kWait newest commit groups, which may still be in flight, hold
+    // groups at or below gh - kSlots + kWait, and every group above that is complete.
     __device__ __forceinline__ void service() {
-        const int32_t gh = (gm1 + P) >> 7;
-        const bool need = next_g >= gh - 7;
+        const int32_t gh = (gm1 + P) >> kGroupShift;
+        const bool need = next_g >= gh - (int32_t)(kSlots - 1);
         request(next_g, need && next_g >= 0);
         next_g -= need ? 1 : 0;
-        asm volatile("cp.async.wait_group 5;" ::: "memory");
+        asm volatile("cp.async.wait_group %0;" ::"n"(kWait) : "memory");
     }
 };
+
+// k_fse: 8 groups of 16 bytes, 7 groups (896 bits) ahead.  Call service() at least once per 116 consumed bits (every
+// second sequence); the groups a step can touch before the next call (down to 2 below the current one) are complete
+// after wait_group 5.
+using FseRing = PosRing<16, 8, 5>;
+// k_huf takes one of two rings (k_huf_narrow_ring picks).  Wide: FseRing's geometry, 144 bytes per lane, 7 CTAs per SM; service()
+// after every second window (<= 88 bits), wait_group 5 as above.  Narrow: 8 groups of 8 bytes, 7 groups (448 bits, ten windows
+// of four 11-bit codes) ahead, 72 bytes per lane, 8 CTAs per SM; service() after every window (<= 44 bits, less than a group):
+// the one window read before the next call touches the current group and the one below it, complete after wait_group 6.  The
+// narrow ring's chains are slower (C3, two waves with either ring: k_huf alone 1.76 ms wide, 2.30 ms narrow, on an H100 80GB
+// HBM3 at a 700 W power limit), so it only pays where it saves the second wave.
+using HufRingWide = PosRing<16, 8, 5>;
+using HufRingNarrow = PosRing<8, 8, 6>;
 
 // Reversed bit reader for the decode kernels: 64-bit window hi:lo (left aligned) fed by ALIGNED 128-bit loads,
 // double buffered (`nxt` is requested a whole 16-byte group before it is needed, so L2/HBM latency overlaps
@@ -276,10 +309,16 @@ struct HufBits {
 // checks); the stream was "regular" iff it is then exhausted exactly (every code consumes >= 1 bit, so ending on
 // bits_remaining == 0 after `cap` symbols is equivalent to the reference's loop stopping there,
 // literals_section_decoder.rs:112-121).  Returns true when regular; otherwise the caller replays with huf_stream2.
+template <class Ring>
 __device__ __forceinline__ bool huf_stream_fast(const uint8_t *__restrict__ tsym, const uint8_t *__restrict__ tnb, uint32_t mb,
                                                 const uint8_t *src, uint32_t len, uint8_t *dst, uint32_t cap, uint32_t ring_addr) {
-    PosRing br;
-    if (!br.init(src, len, ring_addr + 16u)) return false;   // slot 0 of the ring; the mirror slot sits below it
+    // Windows of four symbols (<= 44 bits each) between two service() calls: two when they stay under one group, else one, so that
+    // one request per call keeps up.  The windows read between two calls touch groups down to gh - kWindows (the first one gh and
+    // gh - 1, the second at most one lower), which have to be complete after wait_group kWaitDepth (PosRing::service).
+    constexpr uint32_t kWindows = 2 * 44 < Ring::kGroupBits ? 2 : 1;
+    static_assert(kWindows * 44 < Ring::kGroupBits && Ring::kWaitDepth + 1 + kWindows <= Ring::kRingSlots, "k_huf: ring serviced too rarely");
+    Ring br;
+    if (!br.init(src, len, ring_addr + Ring::kSlot0)) return false;
     const uint32_t sh = 32u - mb;
     uint32_t a_sym = (uint32_t)__cvta_generic_to_shared(tsym), a_nb = (uint32_t)__cvta_generic_to_shared(tnb);
     asm volatile("" : "+r"(a_sym), "+r"(a_nb));
@@ -308,7 +347,7 @@ __device__ __forceinline__ bool huf_stream_fast(const uint8_t *__restrict__ tsym
             br.window(hi, lo);
             const uint32_t s0 = sym1(hi, lo, used), s1 = sym1(hi, lo, used), s2 = sym1(hi, lo, used), s3 = sym1(hi, lo, used);
             br.P -= (int32_t)used;
-            if (q & 1) br.service();                  // every 8 symbols (<= 88 bits)
+            if ((q + 1) % kWindows == 0) br.service();
             w[q] = s0 | (s1 << 8) | (s2 << 16) | (s3 << 24);
         }
         *reinterpret_cast<uint4 *>(dst + n) = make_uint4(w[0], w[1], w[2], w[3]);
@@ -369,6 +408,7 @@ __device__ __forceinline__ int huf_stream2(const uint8_t *__restrict__ tsym, con
     return br.p == 0 ? 0 : 1;
 }
 
+template <class Ring>
 __global__ void __launch_bounds__(32) k_huf(const BlockDesc *__restrict__ descs, BlockAux *__restrict__ aux, const uint8_t *__restrict__ input,
                                           uint8_t *__restrict__ lit_scratch, uint32_t nblocks) {
     extern __shared__ __align__(16) uint8_t smem_huf[];
@@ -429,8 +469,8 @@ __global__ void __launch_bounds__(32) k_huf(const BlockDesc *__restrict__ descs,
                 // fast path: the standard split -- streams 0..2 regenerate S bytes, stream 3 the rest
                 if (regen >= 3 * S) {
                     uint32_t cap = k < 3 ? S : regen - 3 * S;
-                    uint32_t ring_addr = (uint32_t)__cvta_generic_to_shared(smem_huf + HUF_BLOCKS_PER_CTA * HUF_SMEM_PER_BLOCK + lane * RING_STRIDE);
-                    irregular = !huf_stream_fast(tsym, tnb, mb, s0 + off[k], off[k + 1] - off[k], dst + k * S, cap, ring_addr);
+                    uint32_t ring_addr = (uint32_t)__cvta_generic_to_shared(smem_huf + HUF_BLOCKS_PER_CTA * HUF_SMEM_PER_BLOCK + lane * Ring::kStride);
+                    irregular = !huf_stream_fast<Ring>(tsym, tnb, mb, s0 + off[k], off[k + 1] - off[k], dst + k * S, cap, ring_addr);
                 } else irregular = true;
                 // any anomaly in the group -> lane 0 of the group replays the block with the reference's exact semantics
                 uint32_t gmask = 0xFu << (lane & 28u);
@@ -521,7 +561,7 @@ struct FseChain {
     uint32_t logL, logM, logO, qTL, qTM, qTO;   // accuracy logs; shared-memory table addresses biased by -2^log entries
     uint32_t *out; uint32_t nseq;
     // running
-    PosRing br;
+    FseRing br;
     uint32_t eL, eM, eO, h0, h1, h2;   // h*: repeat-offset history, symbolic (b200z_types.h seq_sym_*)
     uint32_t out_end, lit_end, ovf;    // prefix sums of ll + ml and of ll; OR of all their values (bit 31 = reached 2^31)
     uint32_t flags, max_of, max_x, i;
@@ -674,7 +714,7 @@ __global__ void __launch_bounds__(32) k_fse(const BlockDesc *__restrict__ descs,
     uint8_t *s_ml_bits = s_ll_bits + 36;
     uint32_t *s_ll = reinterpret_cast<uint32_t *>(smem_fse + FSE_LANES * FSE_TAB_U16 * 2 + 512);   // base | bits << 24
     uint32_t *s_ml = s_ll + 36;
-    uint8_t *s_ring = smem_fse + FSE_LANES * FSE_TAB_U16 * 2 + 1024;                                // FSE_LANES x RING_STRIDE
+    uint8_t *s_ring = smem_fse + FSE_LANES * FSE_TAB_U16 * 2 + 1024;                                // FSE_LANES x FseRing::kStride
     const uint32_t lane = threadIdx.x;
     for (uint32_t i = lane; i < 36; i += 32) { s_ll_base[i] = c_ll_base[i]; s_ll_bits[i] = c_ll_bits[i]; s_ll[i] = c_ll_base[i] | ((uint32_t)c_ll_bits[i] << 24); }
     for (uint32_t i = lane; i < 53; i += 32) { s_ml_base[i] = c_ml_base[i]; s_ml_bits[i] = c_ml_bits[i]; s_ml[i] = c_ml_base[i] | ((uint32_t)c_ml_bits[i] << 24); }
@@ -727,7 +767,7 @@ __global__ void __launch_bounds__(32) k_fse(const BlockDesc *__restrict__ descs,
         if (c.run) {
             const uint8_t *src = input + c.d->src_off + aux[c.b].seq_bits_off;
             const uint32_t len = c.d->src_size - aux[c.b].seq_bits_off;
-            const uint32_t ring_addr = (uint32_t)__cvta_generic_to_shared(s_ring + lane * RING_STRIDE) + 16u;   // slot 0; the mirror slot sits below
+            const uint32_t ring_addr = (uint32_t)__cvta_generic_to_shared(s_ring + lane * FseRing::kStride) + FseRing::kSlot0;
             c.bad = !c.br.init(src, len, ring_addr) || !c.tl || !c.tl->valid || !c.to || !c.to->valid || !c.tm || !c.tm->valid;
             if (!c.bad) c.bad = c.tl->log > 9u || c.tm->log > 9u || c.to->log > 8u;   // never true for a built table: the staged copies are sized for these
             c.flags = 0; c.max_of = 0; c.max_x = 0; c.i = 0; c.out_end = 0; c.lit_end = 0; c.ovf = 0;
@@ -1593,27 +1633,42 @@ int launch_predefined(FseSlot *predef, cudaStream_t s, uint64_t *launched) {
     return launched_one(launched);
 }
 
-constexpr uint32_t kHufSmem = HUF_BLOCKS_PER_CTA * HUF_SMEM_PER_BLOCK + 32 * RING_STRIDE;
-constexpr uint32_t kFseSmem = FSE_LANES * FSE_TAB_U16 * 2 + 1024 + FSE_LANES * RING_STRIDE;
+template <class Ring> constexpr uint32_t huf_smem() { return HUF_BLOCKS_PER_CTA * HUF_SMEM_PER_BLOCK + 32 * Ring::kStride; }
+constexpr uint32_t kFseSmem = FSE_LANES * FSE_TAB_U16 * 2 + 1024 + FSE_LANES * FseRing::kStride;
+// Every lane of k_huf is one serial Huffman chain, so a grid that needs a second wave takes twice as long as one that
+// does not.  With 1 KiB of shared memory reserved per CTA, 8 CTAs of k_huf with the narrow ring (64 blocks) fit in an SM's
+// 228 KiB: on 132 SMs that is 8,448 blocks at once, more than the 8,192 of a 1 GiB submission of 128 KiB blocks; with the
+// wide ring 7 CTAs fit (7,392 blocks).
+static_assert(8 * (huf_smem<HufRingNarrow>() + 1024) <= 228 * 1024, "k_huf: 8 CTAs per SM with the narrow ring");
 
 static int g_num_sms[64];   // per device ordinal, filled by init_kernels
+// per device ordinal, filled by init_kernels: resident CTAs per SM of k_huf with the wide ring, with the narrow ring, of k_fse
+static int g_ctas_per_sm[64][3];
+
+template <class Ring> static cudaError_t huf_attributes(int *ctas_per_sm) {
+    cudaError_t e = cudaFuncSetAttribute(k_huf<Ring>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)huf_smem<Ring>());
+    if (e != cudaSuccess) return e;
+    // k_fse and k_huf run side by side: ask for the largest shared-memory carve-out so that both fit
+    e = cudaFuncSetAttribute(k_huf<Ring>, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
+    if (e != cudaSuccess) return e;
+    return cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, k_huf<Ring>, 32, huf_smem<Ring>());
+}
 
 int init_kernels() {
     cudaError_t e = cudaFuncSetAttribute(k_fse, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFseSmem);
     if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(k_huf, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHufSmem);
-    if (e != cudaSuccess) return (int)e;
     e = cudaFuncSetAttribute(k_exec_cta, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)XC_SMEM_BYTES);
     if (e != cudaSuccess) return (int)e;
-    // k_fse and k_huf run side by side: ask for the largest shared-memory carve-out so that both fit
     e = cudaFuncSetAttribute(k_fse, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
     if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(k_huf, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
-    if (e != cudaSuccess) return (int)e;
+    int wide = 0, narrow = 0, fse = 0;
+    if ((e = huf_attributes<HufRingWide>(&wide)) != cudaSuccess) return (int)e;
+    if ((e = huf_attributes<HufRingNarrow>(&narrow)) != cudaSuccess) return (int)e;
+    if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fse, k_fse, 32, kFseSmem)) != cudaSuccess) return (int)e;
     int dev = 0, sms = 0;
     if ((e = cudaGetDevice(&dev)) != cudaSuccess) return (int)e;
     if ((e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return (int)e;
-    if (dev >= 0 && dev < 64) g_num_sms[dev] = sms;
+    if (dev >= 0 && dev < 64) { g_num_sms[dev] = sms; g_ctas_per_sm[dev][0] = wide; g_ctas_per_sm[dev][1] = narrow; g_ctas_per_sm[dev][2] = fse; }
     return 0;
 }
 
@@ -1621,6 +1676,27 @@ uint32_t num_sms() {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64 || g_num_sms[dev] <= 0) return 132;
     return (uint32_t)g_num_sms[dev];
+}
+
+// resident CTAs per SM on the current device: 0 = k_huf wide, 1 = k_huf narrow, 2 = k_fse (0 before init_kernels)
+static uint32_t ctas_per_sm(int which) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 0;
+    return (uint32_t)g_ctas_per_sm[dev][which];
+}
+
+// k_huf reads its streams through the narrow ring only where that saves the second wave: the grid fits in one wave of the narrow
+// ring and not in one of the wide ring (7,393-8,448 blocks on 132 SMs).  Everywhere else the wide ring's faster chains win.
+static bool k_huf_narrow_ring(uint32_t nblocks) {
+    const uint32_t ctas = cdiv(nblocks, HUF_BLOCKS_PER_CTA), sms = num_sms();
+    return ctas > ctas_per_sm(0) * sms && ctas <= ctas_per_sm(1) * sms;
+}
+
+void entropy_waves(uint32_t nblocks, uint32_t out[4]) {
+    const uint32_t huf = ctas_per_sm(k_huf_narrow_ring(nblocks) ? 1 : 0), fse = ctas_per_sm(2), sms = num_sms();
+    out[0] = huf ? cdiv(cdiv(nblocks, HUF_BLOCKS_PER_CTA), huf * sms) : 0;
+    out[1] = fse ? cdiv(cdiv(nblocks, FSE_LANES), fse * sms) : 0;
+    out[2] = huf; out[3] = fse;
 }
 
 const char *const kStageNames[kNumStages] = {"k_setup", "k_huf", "k_fse", "k_exec_cta", "k_exec"};
@@ -1650,7 +1726,10 @@ int launch_stage(const PipelineArgs &a, int stage, cudaStream_t s, uint64_t *lau
             break;
         case 1:
             if (!a.nblocks) return 0;
-            k_huf<<<cdiv(a.nblocks, HUF_BLOCKS_PER_CTA), 32, kHufSmem, s>>>(a.descs, a.aux, a.input, a.lit_scratch, a.nblocks);
+            if (k_huf_narrow_ring(a.nblocks))
+                k_huf<HufRingNarrow><<<cdiv(a.nblocks, HUF_BLOCKS_PER_CTA), 32, huf_smem<HufRingNarrow>(), s>>>(a.descs, a.aux, a.input, a.lit_scratch, a.nblocks);
+            else
+                k_huf<HufRingWide><<<cdiv(a.nblocks, HUF_BLOCKS_PER_CTA), 32, huf_smem<HufRingWide>(), s>>>(a.descs, a.aux, a.input, a.lit_scratch, a.nblocks);
             break;
         case 2:
             if (!a.nblocks) return 0;

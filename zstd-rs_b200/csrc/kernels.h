@@ -51,6 +51,9 @@ int launch_find_frames(const uint8_t *d_input, uint64_t input_len, uint64_t *d_o
 // k_place: out_off / out_cap of every frame of a.frames, back to back by decoded size (after k_fse, before execution)
 int launch_place(const PipelineArgs &a, cudaStream_t s, uint64_t *launched);
 uint32_t num_sms();   // of the current device (132 on H100 SXM)
+// on the current device, for a submission of nblocks blocks: out[0] / out[1] the waves k_huf / k_fse take, out[2] / out[3] their
+// resident CTAs per SM, k_huf's with the bit-reader ring it takes for nblocks (0 = unknown: init_kernels has not run on this device)
+void entropy_waves(uint32_t nblocks, uint32_t out[4]);
 int launch_checksum(const PipelineArgs &a, cudaStream_t s, uint64_t *launched);   // optional 5th stage: XXH64 of every frame's plaintext
 // the stream decoder (tier 1d): k_place_resume places a submission whose first frame continues behind its carried tail; k_carry hands
 // frame `plast` of `prev` to frame 0 of `next` (max_tail: the most bytes it may carry, max(window, 32)); k_xxh64_stream hashes frames
