@@ -1,13 +1,14 @@
 #!/usr/bin/env python3
 """bench_compress.py -- input GB/s of the batch compressor (b200z_compress_frames_batch, ruzstd's Fastest level, checksum on).
 
-    python bench_compress.py [--steps K] [--warmup W] [--skip-cpu]
+    python bench_compress.py [--steps K] [--warmup W] [--skip-cpu] [--level fastest|lazy]
 
 The workload is the C2b plaintext (1 GiB of enwik9-shaped text, datagen.c2_text_plain), device-resident, in two shapes:
 8192 frames of 128 KiB and one 1 GiB frame (C2a's plaintext shape, where the content checksum is four serial chains).
 Prints one JSON line: per shape the input GB/s (CUDA events around the call, median of the steps), the ratio, each kernel's
 milliseconds, (input + output bytes) / t against the HBM peak, the card's name and power limit, and `cpu_baseline`:
-libzstd 1.5.5 level 1 on the same 128 KiB pieces, one thread and all host threads.  Nothing is written to the tree.
+libzstd 1.5.5 level 1 on the same 128 KiB pieces, one thread and all host threads.  --level lazy measures the LAZY extension
+level instead, and adds libzstd level 3 to the baseline.  Nothing is written to the tree.
 """
 import argparse
 import json
@@ -43,26 +44,26 @@ def card_info():
     return info
 
 
-def libzstd_compress_baseline(datas):
-    """libzstd 1.5.5 level 1 (one frame per piece): one thread on the first 64 pieces, and all host threads on all of them."""
+def libzstd_compress_baseline(datas, level=1):
+    """libzstd 1.5.5 at `level` (one frame per piece): one thread on the first 64 pieces, and all host threads on all of them."""
     import datagen as G
     from concurrent.futures import ThreadPoolExecutor
     sub = datas[:64]
     t0 = time.perf_counter()
-    n1 = sum(len(G.compress(d, level=1)) for d in sub)
+    n1 = sum(len(G.compress(d, level=level)) for d in sub)
     one = sum(len(d) for d in sub) / (time.perf_counter() - t0) / GB
     threads = bench.host_threads()
     with ThreadPoolExecutor(max_workers=threads) as ex:
         t0 = time.perf_counter()
-        sizes = list(ex.map(lambda d: len(G.compress(d, level=1)), datas))
+        sizes = list(ex.map(lambda d: len(G.compress(d, level=level)), datas))
         dt = time.perf_counter() - t0
     total = sum(len(d) for d in datas)
-    return {"kind": "libzstd 1.5.5 level 1", "one_core_GBps": one, "one_core_ratio": sum(len(d) for d in sub) / n1,
+    return {"kind": f"libzstd 1.5.5 level {level}", "one_core_GBps": one, "one_core_ratio": sum(len(d) for d in sub) / n1,
             "all_cores_GBps": total / dt / GB, "cores": threads, "ratio": total / sum(sizes)}
 
 
 def run_compress(args):
-    """b200z_compress_frames_batch at the Fastest level on the 1 GiB C2b plaintext, device-resident, in two shapes:
+    """b200z_compress_frames_batch at the Fastest (or LAZY) level on the 1 GiB C2b plaintext, device-resident, in two shapes:
     8192 frames of 128 KiB (C2b) and one 1 GiB frame (C2a's plaintext shape).  Each output is first decoded on the GPU and must
     equal the input; then the call is timed with CUDA events after warm-up, and one more run with a CUDA event between kernels
     gives each kernel's time."""
@@ -77,7 +78,8 @@ def run_compress(args):
     plain = datagen.c2_text_plain(total)
     d_in = torch.from_numpy(plain).cuda()
     peak, peak_src = bench.measured_peak()
-    line = {"metric": "compress_GBps", "unit": "GB/s", "level": "Fastest", "checksum": True, "card": card_info(), "input_bytes": total, "shapes": {}}
+    level = pkg.LAZY if args.level == "lazy" else pkg.FASTEST
+    line = {"metric": "compress_GBps", "unit": "GB/s", "level": "LAZY" if args.level == "lazy" else "Fastest", "checksum": True, "card": card_info(), "input_bytes": total, "shapes": {}}
     for shape, frame_bytes in (("c2b", args.frame_bytes), ("c2a", total)):
         nfr = total // frame_bytes
         io = np.zeros(nfr, dtype=pkg.binding.COMPRESS_IO_DTYPE)
@@ -85,7 +87,7 @@ def run_compress(args):
         for i in range(nfr):
             io[i] = (i * frame_bytes, frame_bytes, i * cap, cap)
         d_out = torch.empty(nfr * cap, dtype=torch.uint8, device="cuda")
-        res = pkg.compress_frames(ctx, d_in, io, d_out)
+        res = pkg.compress_frames(ctx, d_in, io, d_out, level)
         assert (res["status"] == 0).all()
         dio = np.zeros(nfr, dtype=pkg.binding.FRAME_IO_DTYPE)
         dio["src_off"], dio["src_size"], dio["out_off"], dio["out_cap"] = io["dst_off"], res["dst_size"], io["src_off"], frame_bytes
@@ -94,18 +96,18 @@ def run_compress(args):
         assert (dres["status"] == 0).all() and torch.equal(back[:total], d_in), f"{shape}: GPU decode of the compressed frames differs from the input"
         del back
         for _ in range(args.warmup):
-            pkg.compress_frames(ctx, d_in, io, d_out)
+            pkg.compress_frames(ctx, d_in, io, d_out, level)
         stream = torch.cuda.ExternalStream(ctx.stream())
         times = []
         for _ in range(args.steps):
             a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             a.record(stream)
-            pkg.compress_frames(ctx, d_in, io, d_out)
+            pkg.compress_frames(ctx, d_in, io, d_out, level)
             b.record(stream)
             b.synchronize()
             times.append(a.elapsed_time(b) / 1e3)
         ctx.set_flags(pkg.binding.FLAG_PROFILE)
-        pkg.compress_frames(ctx, d_in, io, d_out)
+        pkg.compress_frames(ctx, d_in, io, d_out, level)
         prof = pkg.compress_profile(ctx)
         ctx.set_flags(0)
         t = float(np.median(times))
@@ -118,7 +120,10 @@ def run_compress(args):
         del d_out
     line["value"], line["ratio"] = line["shapes"]["c2b"]["value"], line["shapes"]["c2b"]["ratio"]
     if not args.skip_cpu:
-        line["cpu_baseline"] = libzstd_compress_baseline([plain[i:i + args.frame_bytes] for i in range(0, total, args.frame_bytes)])
+        pieces = [plain[i:i + args.frame_bytes] for i in range(0, total, args.frame_bytes)]
+        line["cpu_baseline"] = libzstd_compress_baseline(pieces)
+        if args.level == "lazy":
+            line["cpu_baseline_level3"] = libzstd_compress_baseline(pieces, 3)
     ctx.close()
     print(json.dumps(line))
 
@@ -130,6 +135,7 @@ def main():
     ap.add_argument("--frame-bytes", type=int, default=131072)
     ap.add_argument("--c2a-bytes", type=int, default=1 << 30, help="total plaintext bytes (both shapes)")
     ap.add_argument("--skip-cpu", action="store_true")
+    ap.add_argument("--level", choices=("fastest", "lazy"), default="fastest")
     run_compress(ap.parse_args())
     return 0
 

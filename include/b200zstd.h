@@ -543,6 +543,17 @@ typedef struct b200z_compress_result {
 /* CompressionLevel (encoding/mod.rs:24-67): Default = 2, Better = 3, Best = 4 are unimplemented!() in the reference */
 #define B200Z_LEVEL_UNCOMPRESSED 0
 #define B200Z_LEVEL_FASTEST 1
+/* EXTENSION (not a ruzstd level; its output is not ruzstd's): the value after the reference's Best = 4.  Same framing, window,
+ * blocks, compress bound and kernels as Fastest; a deeper parse and repeat offsets.  The parse keeps Fastest's blocks, 8 segments
+ * per block, rounds of 32 positions and 5-byte minimum match, and adds per segment a table of the 6 most recent positions per
+ * hash (seeded from 32 KiB before the segment), the segment's three most recent distinct offsets as candidates at every
+ * position, and a lazy choice: the first position with a match competes with the next four, each candidate scored
+ * 4 * length - floor(log2 offset) (a repeat scores 4 * length) less 3 per byte it starts later.  Each Compressed block codes an
+ * offset as a repeat code where the decoder's offset history, tracked from the block's start with all three slots unknown,
+ * names it; so no block depends on another block's encoding.  DESIGN.md section 4.4 states the rules and tests/clazy.py models
+ * them byte for byte.  Accepted by the batch entries (with or without a dictionary and B200Z_FLAG_DICT_TABLES) and the stream
+ * compressor; b200z_dict_finalize keeps the Fastest parse. */
+#define B200Z_LEVEL_LAZY 5
 /* context flag: b200z_compress_frames_batch records a CUDA event between its kernels and keeps each kernel's milliseconds
  * for b200z_compress_last_profile (profiling aid for bench.py; it synchronises anyway) */
 #define B200Z_FLAG_PROFILE 2u
@@ -559,7 +570,8 @@ size_t b200z_compress_bound(size_t src_size);
 /* Compresses `nframes` frames.  `input` / `output` are host or device memory (B200Z_MEM_*); `checksum` != 0 appends the
  * content checksum.  Returns 0 when the submission ran (results[nframes] filled).  Checked before any launch:
  * B200Z_ERR_INVALID_ARGUMENT for a range outside `input` / `output`, dst_cap < b200z_compress_bound(src_size), overlapping
- * destination ranges or an unknown level; B200Z_ERR_REFERENCE_WOULD_PANIC for the levels the reference does not implement. */
+ * destination ranges or an unknown level; B200Z_ERR_REFERENCE_WOULD_PANIC for the levels the reference does not implement.
+ * Levels: Uncompressed, Fastest and the extension B200Z_LEVEL_LAZY. */
 int b200z_compress_frames_batch(b200z_ctx *ctx, const uint8_t *input, size_t input_len, int input_mem,
                                 const b200z_compress_io *frames, size_t nframes, int level, int checksum,
                                 uint8_t *output, size_t output_cap, int output_mem, b200z_compress_result *results);
@@ -590,9 +602,9 @@ int b200z_compress_last_profile(const b200z_ctx *ctx, float *stage_ms, size_t n)
  * a multiple of 128 KiB (0 included) ends with an empty last Raw block (01 00 00); then the low 32 bits of XXH64 (seed 0) of the
  * plaintext when the checksum is on.  Level Uncompressed writes Raw blocks, byte for byte the reference's frame, on the host
  * only (no kernel, no device copy).  Level Fastest writes every block's type and body as b200z_compress_frames_batch does for the
- * same block of the same input compressed as one frame.
+ * same block of the same input compressed as one frame, and so does level LAZY (EXTENSION) at LAZY.
  * The source is read into chunks of whole blocks: B200Z_PIPELINE_CHUNK_BYTES (read by _new) rounded down to a multiple of
- * 131072, at least 131072; 64 MiB by default.  At Fastest each non-empty chunk is uploaded and compressed by three kernels
+ * 131072, at least 131072; 64 MiB by default.  At Fastest (and LAZY) each non-empty chunk is uploaded and compressed by three kernels
  * (k_cmatch, k_cenc, k_cassemble) on the ctx stream, counted in b200z_ctx_kernel_launches, while the host reads and hashes the
  * next chunk and writes the previous one: one write_cb pass per chunk (header in the first, trailer in the last), not per block.
  * Memory, allocated by the first Fastest compress and kept until _free, depends on the chunk C only.  Device: 2 * (C + 131072)
@@ -603,10 +615,10 @@ int b200z_compress_last_profile(const b200z_ctx *ctx, float *stage_ms, size_t n)
  * written, and the compressor stays usable.  Hashing and matching state reset with every compress.
  * ---------------------------------------------------------------------------------------------------------- */
 typedef struct b200z_frame_compressor b200z_frame_compressor;
-/* FrameCompressor::new :77.  B200Z_ERR_INVALID_ARGUMENT for a level outside 0-4 */
+/* FrameCompressor::new :77.  B200Z_ERR_INVALID_ARGUMENT for a level outside 0-4 and B200Z_LEVEL_LAZY */
 int b200z_frame_compressor_new(b200z_ctx *ctx, int level, int checksum, b200z_frame_compressor **out);
 void b200z_frame_compressor_free(b200z_frame_compressor *fc);
-int b200z_frame_compressor_set_compression_level(b200z_frame_compressor *fc, int level);   /* :263; 0-4, else INVALID_ARGUMENT */
+int b200z_frame_compressor_set_compression_level(b200z_frame_compressor *fc, int level);   /* :263; 0-4 or LAZY, else INVALID_ARGUMENT */
 int b200z_frame_compressor_compression_level(const b200z_frame_compressor *fc);            /* :273 */
 /* compress :131-224: one frame from read_cb to write_cb.  B200Z_ERR_REFERENCE_WOULD_PANIC for levels 2-4 before any read, write
  * or launch.  result (may be NULL): dst_size = bytes written, blocks (the trailing empty block included), raw / RLE blocks

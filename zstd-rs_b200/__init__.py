@@ -1,5 +1,5 @@
 """zstd-rs_b200 -- GPU-native (H100, sm_90a) zstd block decompressor behind ruzstd's FrameDecoder / StreamingDecoder API,
-a batch compressor at ruzstd's Uncompressed and Fastest levels (compress_frames / compress_to_vec), a stream compressor behind
+a batch compressor at ruzstd's Uncompressed and Fastest levels and an extension level LAZY (compress_frames / compress_to_vec), a stream compressor behind
 ruzstd's FrameCompressor / encoding::compress API (FrameCompressor, compress), and a raw-content
 dictionary trainer in place of ruzstd::dictionary (create_raw_dict, create_raw_dict_from_source, create_raw_dict_from_dir)
 and a finalizer that turns its content into a zstd-format dictionary (finalize_dict, create_dict).  decode_all_stream decodes a
@@ -13,7 +13,7 @@ There is no CPU decode path: every decode call needs a CUDA device and fails lou
 Import name: ``zstd_rs_b200`` (the directory name has a hyphen; see ``_pkg.py`` at the repo root).
 """
 from .binding import (  # noqa: F401
-    ALL, FASTEST, UNCOMPRESSED, UPTO_BLOCKS, UPTO_BYTES, AllBatch, B200ZError, Batch, Context, Dictionary, FrameCompressor, FrameDecoder,
+    ALL, FASTEST, LAZY, UNCOMPRESSED, UPTO_BLOCKS, UPTO_BYTES, AllBatch, B200ZError, Batch, Context, Dictionary, FrameCompressor, FrameDecoder,
     StreamingDecoder, build, compress, compress_bound, compress_frames, compress_profile, compress_to_vec, create_dict, create_raw_dict,
     create_raw_dict_from_dir,
     create_raw_dict_from_source, decode_all, decode_all_batch, decode_all_stream, decode_blocks, decode_frames,

@@ -2571,7 +2571,7 @@ extern "C" int b200z_compress_frames_batch_dict(b200z_ctx *c, const uint8_t *inp
                                                 size_t output_cap, int output_mem, b200z_compress_result *results) {
     // ---- everything is checked before any device work
     if (level >= 2 && level <= 4) return B200Z_ERR_REFERENCE_WOULD_PANIC;   // Default / Better / Best: unimplemented!() in the reference
-    if (!c || (level != B200Z_LEVEL_UNCOMPRESSED && level != B200Z_LEVEL_FASTEST)) return B200Z_ERR_INVALID_ARGUMENT;
+    if (!c || (level != B200Z_LEVEL_UNCOMPRESSED && level != B200Z_LEVEL_FASTEST && level != B200Z_LEVEL_LAZY)) return B200Z_ERR_INVALID_ARGUMENT;
     if (dict && dict->ctx != c) { c->err = "dictionary created on another context"; return B200Z_ERR_INVALID_ARGUMENT; }
     if ((nframes && (!frames || !results)) || (input_mem != B200Z_MEM_HOST && input_mem != B200Z_MEM_DEVICE) ||
         (output_mem != B200Z_MEM_HOST && output_mem != B200Z_MEM_DEVICE) || (input_len && !input) || (output_cap && !output) || nframes > 0xffffffffu) {
@@ -2614,7 +2614,7 @@ extern "C" int b200z_compress_frames_batch_dict(b200z_ctx *c, const uint8_t *inp
     CompressResources *rp = nullptr;
     if (int e = compress_get(c, &rp)) return e;
     CompressResources &r = *rp;
-    const bool fast = level == B200Z_LEVEL_FASTEST;
+    const bool fast = level != B200Z_LEVEL_UNCOMPRESSED;   // Fastest or LAZY: the blocks are parsed and encoded
     int e = 0;
     // Uncompressed takes the blocks' results only, not the match and entropy staging
     if ((e = r.frames.ensure(nframes * sizeof(CFrame))) || (e = r.blocks.ensure(nblocks * sizeof(CBlock))) ||
@@ -2685,7 +2685,7 @@ extern "C" int b200z_compress_frames_batch_dict(b200z_ctx *c, const uint8_t *inp
 
 // ---------------------------------------------------------------------------------------------------------------
 // stream compressor (FrameCompressor, frame_compressor.rs:75-276): the source is read into chunks of whole 128 KiB blocks and
-// the frame is written chunk by chunk.  Uncompressed frames the blocks on the host.  Fastest runs k_cmatch -> k_cenc ->
+// the frame is written chunk by chunk.  Uncompressed frames the blocks on the host.  Fastest (or LAZY) runs k_cmatch -> k_cenc ->
 // k_cassemble<true> on each chunk on the ctx stream, uploads on one copy stream and downloads on another, while the calling
 // thread reads and hashes the next chunk and writes the previous one (the pattern of decode_frames_pipelined).
 // ---------------------------------------------------------------------------------------------------------------
@@ -2716,7 +2716,7 @@ struct b200z_frame_compressor {
     size_t desc_bytes() const { return res_off() + sizeof(b200z_compress_result); }
 };
 
-static int fc_valid_level(int level) { return level >= 0 && level <= 4; }   // CompressionLevel: Uncompressed .. Best
+static int fc_valid_level(int level) { return (level >= 0 && level <= 4) || level == B200Z_LEVEL_LAZY; }   // Uncompressed .. Best, LAZY
 static int fc_panic(b200z_ctx *c, const char *what) { c->err = what; return B200Z_ERR_REFERENCE_WOULD_PANIC; }
 
 extern "C" int b200z_frame_compressor_new(b200z_ctx *c, int level, int checksum, b200z_frame_compressor **out) {
@@ -2878,7 +2878,7 @@ static int fc_compress_fast(b200z_frame_compressor *fc, b200z_read_fn rd, void *
         a.results = reinterpret_cast<b200z_compress_result *>(fc->d_desc[s].as<uint8_t>() + fc->res_off());
         a.input = din; a.output = fc->d_out[s].as<uint8_t>();
         fc->stage.bind(a);
-        a.nframes = 1; a.nblocks = m; a.level = B200Z_LEVEL_FASTEST;
+        a.nframes = 1; a.nblocks = m; a.level = fc->level;   // Fastest or LAZY
         if (int le = launch_compress_chunk(a, ks, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_cmatch / k_cenc / k_cassemble<true>");
         CU(c, cudaEventRecord(fc->ev_k[s], ks));
         CU(c, cudaStreamWaitEvent(fc->s_d2h, fc->ev_k[s], 0));
@@ -2931,7 +2931,7 @@ extern "C" int b200z_frame_compressor_compress(b200z_frame_compressor *fc, b200z
                                                b200z_compress_result *result) {
     if (!fc || !rd || !wr) return B200Z_ERR_INVALID_ARGUMENT;
     b200z_ctx *c = fc->ctx;
-    if (fc->level >= 2) return fc_panic(c, "FrameCompressor::compress: compression levels above Fastest are unimplemented!() in the reference");
+    if (fc->level >= 2 && fc->level <= 4) return fc_panic(c, "FrameCompressor::compress: compression levels above Fastest are unimplemented!() in the reference");
     b200z_compress_result r{};
     XXH64State h;
     h.reset();

@@ -1,14 +1,16 @@
 // compress.cu -- sm_90a kernels of the batch compressor (ruzstd's encoding::compress at CompressionLevel::Fastest).
 //
 //   k_cmatch    : one CTA per 128 KiB block: greedy LZ77 parse into literals + sequences (two-table parallel parse)
+//                 (<DICT, true>: the LAZY level's parse, an extension: K-way tables, repeat candidates, a lazy choice)
 //   k_cenc      : one warp per block: Huffman literals, FSE sequences, the Raw / RLE / Compressed decision (encode.cuh)
+//                 (<TABLES, true>: LAZY, repeat-offset codes within each block first)
 //   k_cxxh64    : content checksum of every frame's input (xxh64.cuh; four serial chains per frame)
 //   k_cassemble : one CTA per block: frame header, the block at its prefix-summed offset, the checksum, per-frame results
 //                 (<true>: one chunk of a streamed frame, blocks only; the host writes header, trailer and checksum)
 //   k_cdict     : not a stage: the match table of a dictionary, built once the first time the dictionary is used (EXTENSION)
 //   k_dstats    : not a stage: literal and sequence-code histograms of k_cmatch's parse, for b200z_dict_finalize (EXTENSION)
 //
-// Every block is encoded from its own literals and sequences only (no repeat offsets; Repeat / Treeless modes only in a frame's
+// Every block is encoded from its own literals and sequences only (repeat offsets only at LAZY, within the block; Repeat / Treeless modes only in a frame's
 // first block with a formatted dictionary's tables, which the format makes that block's previous tables), so all
 // blocks of all frames -- including the blocks of one huge frame -- run at the same time.  Matches may still reach back into
 // the previous block: the input is all there from the start.  With a dictionary (an extension: ruzstd's encoder has none), the
@@ -30,6 +32,18 @@ constexpr uint32_t CM_SEED = 16384;  // bytes before its segment a warp's privat
 constexpr uint32_t CM_CAP = 16;      // match bytes a lane verifies before the warp extends the chosen match together
 constexpr uint32_t CM_SMEM = (4u << CM_T1_LOG) + CM_WARPS * (4u << CM_TP_LOG);
 constexpr uint32_t CE_WARPS = 4;
+// the LAZY parse (tests/clazy.py states it rule by rule)
+constexpr uint32_t LZ_T1_LOG = 15;     // its t1 is twice Fastest's
+constexpr uint32_t LZ_TAB_LOG = 10;    // buckets of a warp's table
+constexpr uint32_t LZ_WAYS = 6;        // positions per bucket, u16 relative to the seed base, newest first (3 words)
+constexpr uint32_t LZ_SEED = 32768;    // bytes before its segment a warp's table starts from (stream chunks keep 128 KiB in front)
+constexpr uint32_t LZ_CAP = 32;        // match bytes a lane verifies before the warp extends the chosen match together
+constexpr uint32_t LZ_DEPTH = 4;       // lanes after the first match that compete with it
+constexpr int32_t LZ_LANE_COST = 3;    // gain a later lane gives up per byte it starts later
+constexpr uint32_t LZ_EMPTY = 0xffffu;
+constexpr uint32_t LZ_SMEM = (4u << LZ_T1_LOG) + CM_WARPS * (2u * LZ_WAYS << LZ_TAB_LOG);   // 224 KiB
+static_assert(LZ_SEED + ENC_BLOCK / CM_WARPS < LZ_EMPTY, "a table entry must fit below the empty mark");
+static_assert(LZ_WAYS == 6, "lz_push shifts three words");
 
 __device__ __forceinline__ uint64_t load5(const uint8_t *p) {
     return (uint64_t)__ldg(p) | ((uint64_t)__ldg(p + 1) << 8) | ((uint64_t)__ldg(p + 2) << 16) | ((uint64_t)__ldg(p + 3) << 24) |
@@ -40,6 +54,117 @@ __device__ __forceinline__ uint32_t match_len(const uint8_t *a, const uint8_t *b
     uint32_t n = 0;
     while (n < lim && __ldg(a + n) == __ldg(b + n)) n++;
     return n;
+}
+
+// LAZY: pushes u16 entry v into a bucket held as three words, slot 0 (the newest) in the low half of w0
+__device__ __forceinline__ void lz_push(uint32_t &w0, uint32_t &w1, uint32_t &w2, uint32_t v) {
+    w2 = (w2 << 16) | (w1 >> 16);
+    w1 = (w1 << 16) | (w0 >> 16);
+    w0 = (w0 << 16) | v;
+}
+
+// LAZY: inserts positions q0 + lane (the lanes with `valid`) into the warp's table in position order.  Lanes of one bucket form
+// a group; its last lane pushes the group's last LZ_WAYS positions, oldest first, so the table does not depend on the schedule.
+__device__ __forceinline__ void lz_insert(uint32_t *tab, const uint8_t *src, int32_t q0, bool valid, int32_t base, uint32_t lane) {
+    const uint32_t h = valid ? hash5(src + q0 + (int32_t)lane, LZ_TAB_LOG) : (1u << LZ_TAB_LOG) + lane;   // invalid: a group alone
+    const uint32_t grp = __match_any_sync(0xffffffffu, h);
+    if (valid && lane == 31u - __clz(grp)) {
+        uint32_t *bk = tab + 3 * h;
+        uint32_t w0 = bk[0], w1 = bk[1], w2 = bk[2], m = grp;
+        for (uint32_t c = __popc(grp); c > LZ_WAYS; c--) m &= m - 1;
+        for (; m; m &= m - 1) lz_push(w0, w1, w2, (uint32_t)(q0 + __ffs(m) - 1 - base));
+        bk[0] = w0; bk[1] = w1; bk[2] = w2;
+    }
+    __syncwarp();
+}
+
+// LAZY: extends the chosen match at qj (offset off, ml bytes verified) 32 bytes at a time, up to lim, as the Fastest loop does
+// inline (kept there as it is so that the Fastest kernels compile to the same SASS)
+template <bool DICT>
+__device__ __forceinline__ uint32_t extend_match(const uint8_t *src, uint32_t qj, uint32_t off, uint32_t ml, uint32_t lim, uint32_t back,
+                                                 const uint8_t *dict, uint32_t dict_len, uint32_t lane) {
+    const uint32_t fpos = back + qj;   // an offset beyond the frame's start points into the dictionary
+    const uint8_t *ref = DICT && off > fpos ? dict + dict_len - (off - fpos) : src + qj - off;
+    while (ml < lim) {
+        const uint32_t i = ml + lane;
+        const bool stop = i >= lim || __ldg(src + qj + i) != __ldg(ref + i);
+        const uint32_t sm = __ballot_sync(0xffffffffu, stop);
+        if (sm) { ml += __ffs(sm) - 1; break; }
+        ml += 32;
+    }
+    return min(ml, lim);
+}
+
+// LAZY: one warp's parse of segment [s, e) (see k_cmatch); writes the segment's sequences and literals to its staging and its
+// counts to *nseq_out, *nlit_out, *trail_out
+template <bool DICT>
+__device__ __forceinline__ void cmatch_lazy(const CBlock &blk, const uint8_t *src, uint32_t s, uint32_t e, const uint32_t *t1, uint32_t *tab,
+                                            int32_t base, uint32_t lane, const uint8_t *dict, const uint32_t *dtab, uint32_t dict_len,
+                                            SeqRec *stage, uint8_t *lstage, uint32_t *nseq_out, uint32_t *nlit_out, uint32_t *trail_out) {
+    uint32_t p = s, anchor = s, nseq = 0, nlit = 0;
+    uint32_t r0 = 0, r1 = 0, r2 = 0;   // the segment's three most recent distinct offsets (0: none yet)
+    while (p + ENC_MIN_MATCH <= e) {
+        const uint32_t q = p + lane;
+        const bool valid = q + ENC_MIN_MATCH <= e;
+        int32_t gain = INT_MIN;   // INT_MIN: no candidate of >= 5 bytes
+        uint32_t len = 0, cand = 0, xlim = e - q;
+        if (valid) {
+            const uint32_t lim = min(LZ_CAP, e - q), fpos = blk.back + q;
+            auto take = [&](uint32_t o, const uint8_t *ref, uint32_t l, int32_t cost) {
+                const int32_t g = 4 * (int32_t)l - cost;
+                if (l >= ENC_MIN_MATCH && g > gain) { gain = g; len = l; cand = o; return true; }
+                return false;
+            };
+            auto rep = [&](uint32_t o) {   // the source must lie in the frame and the window
+                if (o && o <= fpos && o <= ENC_WINDOW) take(o, src + q - o, match_len(src + q, src + q - o, lim), 0);
+            };
+            rep(r0); rep(r1); rep(r2);
+            const uint32_t c1 = t1[hash5(src + q, LZ_T1_LOG)];
+            if (c1 < q) take(q - c1, src + c1, match_len(src + q, src + c1, lim), 31 - __clz(q - c1));
+            const uint32_t *bk = tab + 3 * hash5(src + q, LZ_TAB_LOG);
+            const uint32_t w[3] = {bk[0], bk[1], bk[2]};
+#pragma unroll
+            for (uint32_t k = 0; k < LZ_WAYS; k++) {   // newest first
+                const uint32_t rel = (w[k >> 1] >> (16 * (k & 1))) & 0xffffu;
+                const int32_t c = base + (int32_t)rel;
+                if (rel != LZ_EMPTY && c < (int32_t)q) {
+                    const uint32_t o = (uint32_t)((int32_t)q - c);
+                    take(o, src + c, match_len(src + q, src + c, lim), 31 - __clz(o));
+                }
+            }
+            if (DICT && fpos < ENC_WINDOW) {
+                const uint32_t c3 = __ldg(dtab + hash5(src + q, CD_LOG));
+                const uint32_t off3 = fpos + dict_len - (c3 - 1);
+                if (c3 && off3 <= ENC_WINDOW) {
+                    const uint32_t rest = dict_len - (c3 - 1);   // dictionary bytes from the source to the dictionary's end
+                    if (take(off3, dict + (c3 - 1), match_len(src + q, dict + (c3 - 1), min(lim, rest)), 31 - __clz(off3))) xlim = min(xlim, rest);
+                }
+            }
+        }
+        const uint32_t m = __ballot_sync(0xffffffffu, gain != INT_MIN);
+        lz_insert(tab, src, (int32_t)p, valid, base, lane);   // after every lane's lookup (the ballot), before the next round's
+        if (!m) { p += 32; continue; }
+        // the lazy choice: lanes j .. j + LZ_DEPTH with a match score gain - LZ_LANE_COST * (lane - j); the highest wins, the
+        // earlier lane on a tie (a score lies in [-9, 128], so score + 64 fits 8 bits above the lane's 5)
+        const uint32_t j = __ffs(m) - 1, d = lane - j;
+        const bool comp = gain != INT_MIN && lane >= j && d <= LZ_DEPTH;
+        const uint32_t key = comp ? ((uint32_t)(gain - LZ_LANE_COST * (int32_t)d + 64) << 5) | (31 - lane) : 0u;
+        const uint32_t win = 31 - (__reduce_max_sync(0xffffffffu, key) & 31);
+        const uint32_t qj = p + win, off = __shfl_sync(0xffffffffu, cand, win);
+        uint32_t ml = __shfl_sync(0xffffffffu, len, win);
+        const uint32_t lim = __shfl_sync(0xffffffffu, xlim, win);
+        if (ml == LZ_CAP) ml = extend_match<DICT>(src, qj, off, ml, DICT ? lim : e - qj, blk.back, dict, dict_len, lane);
+        for (uint32_t i = anchor + lane; i < qj; i += 32) lstage[nlit + i - anchor] = __ldg(src + i);
+        if (lane == 0) stage[nseq] = SeqRec{qj - anchor, ml, off};
+        nlit += qj - anchor;
+        nseq++;
+        anchor = p = qj + ml;
+        if (off == r1) { r1 = r0; r0 = off; }   // off moves to the front
+        else if (off != r0) { r2 = r1; r1 = r0; r0 = off; }
+        __syncwarp();
+    }
+    for (uint32_t i = anchor + lane; i < e; i += 32) lstage[nlit + i - anchor] = __ldg(src + i);
+    if (lane == 0) { *nseq_out = nseq; *nlit_out = nlit + (e - anchor); *trail_out = e - anchor; }
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -53,8 +178,13 @@ __device__ __forceinline__ uint32_t match_len(const uint8_t *a, const uint8_t *b
 // smaller offset on a tie.  A dictionary match stops at the dictionary's end.  Without DICT the code is the plain parse.
 // Sequences and literals go to per-segment staging; the CTA then packs them, the trailing literals of a segment joining the
 // first sequence after them.  tests/cparse.py states this parse rule by rule; the GPU must produce exactly its sequences.
+// LAZY (an extension, B200Z_LEVEL_LAZY) keeps the blocks, segments, rounds, dictionary lookup and packing, with a t1 over 2^15
+// hashes.  The private table holds the LZ_WAYS most recent positions per hash (seeded from LZ_SEED bytes back, filled in position
+// order); each lane also tries the segment's three most recent distinct offsets; every candidate scores 4 ml - floor(log2 off)
+// (a repeat costs 0), and the first lane with a match competes with the next LZ_DEPTH lanes at LZ_LANE_COST per byte of delay.
+// tests/clazy.py states it rule by rule.
 // ------------------------------------------------------------------------------------------------------------
-template <bool DICT>
+template <bool DICT, bool LAZY>
 __global__ void __launch_bounds__(CM_THREADS, 1)
 k_cmatch(const CBlock *__restrict__ blocks, const uint8_t *__restrict__ input, uint8_t *__restrict__ lit_stage, SeqRec *__restrict__ seq_stage,
          uint8_t *__restrict__ lits, SeqRec *__restrict__ seqs, CBlockInfo *__restrict__ info, const uint8_t *__restrict__ dict,
@@ -74,76 +204,93 @@ k_cmatch(const CBlock *__restrict__ blocks, const uint8_t *__restrict__ input, u
         if (tid == 0) info[b] = CBlockInfo{n, 0, n ? 1u : 0u, 0};
         return;
     }
-    for (uint32_t i = tid; i < (1u << CM_T1_LOG); i += CM_THREADS) t1[i] = 0xffffffffu;
-    for (uint32_t i = tid; i < CM_WARPS << CM_TP_LOG; i += CM_THREADS) tp_all[i] = INT_MIN;
+    constexpr uint32_t T1_LOG = LAZY ? LZ_T1_LOG : CM_T1_LOG;
+    for (uint32_t i = tid; i < (1u << T1_LOG); i += CM_THREADS) t1[i] = 0xffffffffu;
+    if constexpr (LAZY) {
+        uint32_t *tab_all = reinterpret_cast<uint32_t *>(smem_cm + (4u << LZ_T1_LOG));
+        for (uint32_t i = tid; i < CM_WARPS * (3u << LZ_TAB_LOG); i += CM_THREADS) tab_all[i] = 0xffffffffu;
+    } else {
+        for (uint32_t i = tid; i < CM_WARPS << CM_TP_LOG; i += CM_THREADS) tp_all[i] = INT_MIN;
+    }
     __syncthreads();
-    for (uint32_t q = tid; q + ENC_MIN_MATCH <= n; q += CM_THREADS) atomicMin(&t1[hash5(src + q, CM_T1_LOG)], q);
+    for (uint32_t q = tid; q + ENC_MIN_MATCH <= n; q += CM_THREADS) atomicMin(&t1[hash5(src + q, T1_LOG)], q);
     int32_t *tp = tp_all + (w << CM_TP_LOG);
     const uint32_t seglen = (n + CM_WARPS - 1) / CM_WARPS;
     const uint32_t s = min(n, w * seglen), e = min(n, s + seglen);
-    const int32_t seed_lo = max((int32_t)s - (int32_t)CM_SEED, -(int32_t)min(blk.back, CM_SEED));
-    for (int32_t q = seed_lo + (int32_t)lane; q < (int32_t)s && q + (int32_t)ENC_MIN_MATCH <= (int32_t)n; q += 32)   // inside the frame
-        atomicMax(&tp[hash5(src + q, CM_TP_LOG)], q);
-    __syncthreads();
-    SeqRec *stage = seq_stage + ((size_t)b * CM_WARPS + w) * CSEG_SEQS;
-    uint8_t *lstage = lit_stage + (size_t)b * ENC_BLOCK + s;
-    uint32_t p = s, anchor = s, nseq = 0, nlit = 0;
-    while (p + ENC_MIN_MATCH <= e) {
-        const uint32_t q = p + lane;
-        const bool valid = q + ENC_MIN_MATCH <= e;
-        uint32_t len = 0, cand = 0, h2 = 0, xlim = e - q;   // xlim: how far the match may be extended
-        if (valid) {
-            const uint32_t lim = min(CM_CAP, e - q);
-            const uint32_t c1 = t1[hash5(src + q, CM_T1_LOG)];
-            h2 = hash5(src + q, CM_TP_LOG);
-            const int32_t c2 = tp[h2];
-            if (c1 < q) { len = match_len(src + q, src + c1, lim); cand = q - c1; }
-            // the window check cannot fail: c2 >= s - CM_SEED and q < s + seglen <= s + CM_SEED, so a tp offset is below 32 KiB
-            // (offsets up to 128 KiB come from t1 only)
-            if (c2 != INT_MIN && c2 < (int32_t)q && (int32_t)q - c2 <= (int32_t)ENC_WINDOW) {
-                const uint32_t l2 = match_len(src + q, src + c2, lim);
-                if (l2 > len || (l2 == len && (uint32_t)((int32_t)q - c2) < cand)) { len = l2; cand = (uint32_t)((int32_t)q - c2); }
-            }
-            const uint32_t fpos = blk.back + q;   // back < ENC_WINDOW means it is the block's position in the frame
-            if (DICT && fpos < ENC_WINDOW) {
-                const uint32_t c3 = __ldg(dtab + hash5(src + q, CD_LOG));
-                const uint32_t off3 = fpos + dict_len - (c3 - 1);
-                if (c3 && off3 <= ENC_WINDOW) {
-                    const uint32_t rest = dict_len - (c3 - 1);   // dictionary bytes from the source to the dictionary's end
-                    const uint32_t l3 = match_len(src + q, dict + (c3 - 1), min(lim, rest));
-                    if (l3 > len || (l3 == len && off3 < cand)) { len = l3; cand = off3; xlim = min(xlim, rest); }
+    if constexpr (LAZY) {
+        SeqRec *stage = seq_stage + ((size_t)b * CM_WARPS + w) * CSEG_SEQS;
+        uint8_t *lstage = lit_stage + (size_t)b * ENC_BLOCK + s;
+        uint32_t *tab = reinterpret_cast<uint32_t *>(smem_cm + (4u << LZ_T1_LOG)) + w * (3u << LZ_TAB_LOG);
+        const int32_t base = (int32_t)s - (int32_t)LZ_SEED;   // entries hold q - base
+        const int32_t seed_lo = max(base, -(int32_t)blk.back), seed_hi = min((int32_t)s, (int32_t)n - (int32_t)ENC_MIN_MATCH + 1);
+        for (int32_t q0 = seed_lo; q0 < seed_hi; q0 += 32) lz_insert(tab, src, q0, q0 + (int32_t)lane < seed_hi, base, lane);
+        __syncthreads();
+        cmatch_lazy<DICT>(blk, src, s, e, t1, tab, base, lane, dict, dtab, dict_len, stage, lstage, s_nseq + w, s_nlit + w, s_trail + w);
+    } else {
+        const int32_t seed_lo = max((int32_t)s - (int32_t)CM_SEED, -(int32_t)min(blk.back, CM_SEED));
+        for (int32_t q = seed_lo + (int32_t)lane; q < (int32_t)s && q + (int32_t)ENC_MIN_MATCH <= (int32_t)n; q += 32)   // inside the frame
+            atomicMax(&tp[hash5(src + q, CM_TP_LOG)], q);
+        __syncthreads();
+        SeqRec *stage = seq_stage + ((size_t)b * CM_WARPS + w) * CSEG_SEQS;
+        uint8_t *lstage = lit_stage + (size_t)b * ENC_BLOCK + s;
+        uint32_t p = s, anchor = s, nseq = 0, nlit = 0;
+        while (p + ENC_MIN_MATCH <= e) {
+            const uint32_t q = p + lane;
+            const bool valid = q + ENC_MIN_MATCH <= e;
+            uint32_t len = 0, cand = 0, h2 = 0, xlim = e - q;   // xlim: how far the match may be extended
+            if (valid) {
+                const uint32_t lim = min(CM_CAP, e - q);
+                const uint32_t c1 = t1[hash5(src + q, CM_T1_LOG)];
+                h2 = hash5(src + q, CM_TP_LOG);
+                const int32_t c2 = tp[h2];
+                if (c1 < q) { len = match_len(src + q, src + c1, lim); cand = q - c1; }
+                // the window check cannot fail: c2 >= s - CM_SEED and q < s + seglen <= s + CM_SEED, so a tp offset is below 32 KiB
+                // (offsets up to 128 KiB come from t1 only)
+                if (c2 != INT_MIN && c2 < (int32_t)q && (int32_t)q - c2 <= (int32_t)ENC_WINDOW) {
+                    const uint32_t l2 = match_len(src + q, src + c2, lim);
+                    if (l2 > len || (l2 == len && (uint32_t)((int32_t)q - c2) < cand)) { len = l2; cand = (uint32_t)((int32_t)q - c2); }
+                }
+                const uint32_t fpos = blk.back + q;   // back < ENC_WINDOW means it is the block's position in the frame
+                if (DICT && fpos < ENC_WINDOW) {
+                    const uint32_t c3 = __ldg(dtab + hash5(src + q, CD_LOG));
+                    const uint32_t off3 = fpos + dict_len - (c3 - 1);
+                    if (c3 && off3 <= ENC_WINDOW) {
+                        const uint32_t rest = dict_len - (c3 - 1);   // dictionary bytes from the source to the dictionary's end
+                        const uint32_t l3 = match_len(src + q, dict + (c3 - 1), min(lim, rest));
+                        if (l3 > len || (l3 == len && off3 < cand)) { len = l3; cand = off3; xlim = min(xlim, rest); }
+                    }
                 }
             }
-        }
-        __syncwarp();
-        if (valid) atomicMax(&tp[h2], (int32_t)q);
-        const uint32_t m = __ballot_sync(0xffffffffu, len >= ENC_MIN_MATCH);
-        if (!m) { p += 32; __syncwarp(); continue; }
-        const uint32_t j = __ffs(m) - 1;
-        const uint32_t qj = p + j, off = __shfl_sync(0xffffffffu, cand, j);
-        uint32_t ml = __shfl_sync(0xffffffffu, len, j);
-        if (ml == CM_CAP) {   // extend the chosen match 32 bytes at a time
-            const uint32_t lim = DICT ? __shfl_sync(0xffffffffu, xlim, j) : e - qj;
-            const uint32_t fpos = blk.back + qj;   // an offset beyond the frame's start points into the dictionary
-            const uint8_t *ref = DICT && off > fpos ? dict + dict_len - (off - fpos) : src + qj - off;
-            while (ml < lim) {
-                const uint32_t i = ml + lane;
-                const bool stop = i >= lim || __ldg(src + qj + i) != __ldg(ref + i);
-                const uint32_t sm = __ballot_sync(0xffffffffu, stop);
-                if (sm) { ml += __ffs(sm) - 1; break; }
-                ml += 32;
+            __syncwarp();
+            if (valid) atomicMax(&tp[h2], (int32_t)q);
+            const uint32_t m = __ballot_sync(0xffffffffu, len >= ENC_MIN_MATCH);
+            if (!m) { p += 32; __syncwarp(); continue; }
+            const uint32_t j = __ffs(m) - 1;
+            const uint32_t qj = p + j, off = __shfl_sync(0xffffffffu, cand, j);
+            uint32_t ml = __shfl_sync(0xffffffffu, len, j);
+            if (ml == CM_CAP) {   // extend the chosen match 32 bytes at a time
+                const uint32_t lim = DICT ? __shfl_sync(0xffffffffu, xlim, j) : e - qj;
+                const uint32_t fpos = blk.back + qj;   // an offset beyond the frame's start points into the dictionary
+                const uint8_t *ref = DICT && off > fpos ? dict + dict_len - (off - fpos) : src + qj - off;
+                while (ml < lim) {
+                    const uint32_t i = ml + lane;
+                    const bool stop = i >= lim || __ldg(src + qj + i) != __ldg(ref + i);
+                    const uint32_t sm = __ballot_sync(0xffffffffu, stop);
+                    if (sm) { ml += __ffs(sm) - 1; break; }
+                    ml += 32;
+                }
+                ml = min(ml, lim);
             }
-            ml = min(ml, lim);
+            for (uint32_t i = anchor + lane; i < qj; i += 32) lstage[nlit + i - anchor] = __ldg(src + i);
+            if (lane == 0) stage[nseq] = SeqRec{qj - anchor, ml, off};
+            nlit += qj - anchor;
+            nseq++;
+            anchor = p = qj + ml;
+            __syncwarp();
         }
-        for (uint32_t i = anchor + lane; i < qj; i += 32) lstage[nlit + i - anchor] = __ldg(src + i);
-        if (lane == 0) stage[nseq] = SeqRec{qj - anchor, ml, off};
-        nlit += qj - anchor;
-        nseq++;
-        anchor = p = qj + ml;
-        __syncwarp();
+        for (uint32_t i = anchor + lane; i < e; i += 32) lstage[nlit + i - anchor] = __ldg(src + i);
+        if (lane == 0) { s_nseq[w] = nseq; s_nlit[w] = nlit + (e - anchor); s_trail[w] = e - anchor; }
     }
-    for (uint32_t i = anchor + lane; i < e; i += 32) lstage[nlit + i - anchor] = __ldg(src + i);
-    if (lane == 0) { s_nseq[w] = nseq; s_nlit[w] = nlit + (e - anchor); s_trail[w] = e - anchor; }
     __syncthreads();
     if (tid == 0) {
         uint32_t carry = 0, so = 0, lo = 0;
@@ -156,6 +303,8 @@ k_cmatch(const CBlock *__restrict__ blocks, const uint8_t *__restrict__ input, u
         info[b] = CBlockInfo{lo, so, 0, 0};
     }
     __syncthreads();
+    SeqRec *stage = seq_stage + ((size_t)b * CM_WARPS + w) * CSEG_SEQS;   // the segments' staging, packed below
+    uint8_t *lstage = lit_stage + (size_t)b * ENC_BLOCK + s;
     SeqRec *out = seqs + (size_t)b * CBLOCK_SEQS + s_soff[w];
     for (uint32_t i = lane; i < s_nseq[w]; i += 32) {
         SeqRec r = stage[i];
@@ -171,11 +320,40 @@ k_cmatch(const CBlock *__restrict__ blocks, const uint8_t *__restrict__ input, u
 // block type: RLE when all bytes are equal, Compressed when smaller than the input block, else Raw.  A formatted dictionary's
 // tables (dt, B200Z_FLAG_DICT_TABLES) go to a frame's first block only (back == 0); without them (TABLES = false) encode_block gets
 // a constant nullptr, so the plain path carries none of that code.
+// With REPS (LAZY) the warp first writes the block's records with repeat-offset codes to rseqs (rep_pass) and encodes those.
 // ------------------------------------------------------------------------------------------------------------
-template <bool TABLES>
+// LAZY: the decoder's offset history (RFC 8878 3.1.2.5) over one block's sequences, from three unknown slots (0; an offset is
+// >= 1), so no block depends on another's encoding.  A sequence whose offset a known slot can name gets that Offset_Value
+// (LL > 0: rep0 / rep1 / rep2 -> 1 / 2 / 3; LL = 0: rep1 / rep2 / rep0 - 1 -> 1 / 2 / 3), any other offset o is coded raw (o + 3);
+// out[i].of = Offset_Value - 3 (mod 2^32), which encode_block codes as that Offset_Value.  The warp loads 32 records at a time
+// and every lane runs the (uniform) history over them, keeping its own record's code.
+__device__ __forceinline__ void rep_pass(const SeqRec *in, uint32_t nseq, SeqRec *out, uint32_t lane) {
+    uint32_t h0 = 0, h1 = 0, h2 = 0;
+    for (uint32_t b0 = 0; b0 < nseq; b0 += 32) {
+        const uint32_t i = b0 + lane, cnt = min(32u, nseq - b0);
+        const SeqRec r = i < nseq ? in[i] : SeqRec{0, 0, 0};
+        uint32_t mine = 0;
+        for (uint32_t k = 0; k < cnt; k++) {
+            const uint32_t ll = __shfl_sync(0xffffffffu, r.ll, k), o = __shfl_sync(0xffffffffu, r.of, k);
+            uint32_t ov;
+            if (ll) ov = h0 == o ? 1u : h1 == o ? 2u : h2 == o ? 3u : o + 3;
+            else ov = h1 == o ? 1u : h2 == o ? 2u : h0 && h0 - 1 == o ? 3u : o + 3;
+            const uint32_t rep = ov > 3 ? 4u : ov - 1 + (ll == 0);   // 4: raw
+            if (rep == 1) { h1 = h0; h0 = o; }
+            else if (rep == 2) { h2 = h1; h1 = h0; h0 = o; }
+            else if (rep >= 3) { h2 = h1; h1 = h0; h0 = o; }
+            if (k == lane) mine = ov;
+        }
+        if (i < nseq) out[i] = SeqRec{r.ll, r.ml, mine - 3};
+    }
+    __syncwarp();
+}
+
+template <bool TABLES, bool REPS>
 __global__ void __launch_bounds__(CE_WARPS * 32)
 k_cenc(const CBlock *__restrict__ blocks, uint32_t nblocks, const CBlockInfo *__restrict__ info, const uint8_t *__restrict__ lits,
-       const SeqRec *__restrict__ seqs, uint8_t *__restrict__ enc, CBlockInfo *__restrict__ res, const EncDict *__restrict__ dt) {
+       const SeqRec *__restrict__ seqs, uint8_t *__restrict__ enc, CBlockInfo *__restrict__ res, const EncDict *__restrict__ dt,
+       SeqRec *__restrict__ rseqs) {
     __shared__ EncScratch scratch[CE_WARPS];
     const uint32_t w = threadIdx.x >> 5, lane = threadIdx.x & 31, b = blockIdx.x * CE_WARPS + w;
     if (b >= nblocks) return;
@@ -185,7 +363,8 @@ k_cenc(const CBlock *__restrict__ blocks, uint32_t nblocks, const CBlockInfo *__
     uint32_t type = 0, csize = n;
     if (in.type == 1) { type = 1; csize = 1; }
     else if (n) {
-        const uint32_t size = encode_block(scratch[w], lits + (size_t)b * ENC_BLOCK, in.nlit, seqs + (size_t)b * CBLOCK_SEQS, in.nseq,
+        if (REPS) rep_pass(seqs + (size_t)b * CBLOCK_SEQS, in.nseq, rseqs + (size_t)b * CBLOCK_SEQS, lane);
+        const uint32_t size = encode_block(scratch[w], lits + (size_t)b * ENC_BLOCK, in.nlit, REPS ? rseqs + (size_t)b * CBLOCK_SEQS : seqs + (size_t)b * CBLOCK_SEQS, in.nseq,
                                            enc + (size_t)b * ENC_BLOCK, ENC_BLOCK, lane, 32, TABLES ? bdt : nullptr);
         if (size < n) { type = 2; csize = size; }
     }
@@ -301,7 +480,7 @@ static uint32_t cdiv_u(uint64_t a, uint32_t b) { return (uint32_t)((a + b - 1) /
 
 int launch_dict_stats(const CompressArgs &a, unsigned long long *counts, cudaStream_t s, uint64_t *launched) {
     if (!a.nblocks) return 0;
-    k_cmatch<true><<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, a.dict, a.dtab, a.dict_len);
+    k_cmatch<true, false><<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, a.dict, a.dtab, a.dict_len);
     int e = (int)cudaGetLastError();
     if (e) return e;
     ++*launched;
@@ -312,8 +491,10 @@ int launch_dict_stats(const CompressArgs &a, unsigned long long *counts, cudaStr
 }
 
 int init_compress_kernels() {
-    cudaError_t e = cudaFuncSetAttribute(k_cmatch<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CM_SMEM);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cmatch<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CM_SMEM);
+    cudaError_t e = cudaFuncSetAttribute(k_cmatch<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CM_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cmatch<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CM_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cmatch<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LZ_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cmatch<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LZ_SMEM);
     return (int)e;
 }
 
@@ -330,16 +511,23 @@ int launch_dict_table(const uint8_t *dict, uint32_t len, uint32_t *dtab, cudaStr
 const char *const kCompressStageNames[kCompressStages] = {"k_cmatch", "k_cenc", "k_cxxh64", "k_cassemble"};
 
 int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s, uint64_t *launched) {
+    const bool lazy = a.level == B200Z_LEVEL_LAZY;
     switch (stage) {
     case 0:
         if (!a.level || !a.nblocks) return 0;
-        if (a.dtab) k_cmatch<true><<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, a.dict, a.dtab, a.dict_len);
-        else k_cmatch<false><<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, nullptr, nullptr, 0);
+        if (lazy) {
+            if (a.dtab) k_cmatch<true, true><<<a.nblocks, CM_THREADS, LZ_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, a.dict, a.dtab, a.dict_len);
+            else k_cmatch<false, true><<<a.nblocks, CM_THREADS, LZ_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, nullptr, nullptr, 0);
+        } else if (a.dtab) k_cmatch<true, false><<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, a.dict, a.dtab, a.dict_len);
+        else k_cmatch<false, false><<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, nullptr, nullptr, 0);
         break;
-    case 1:
+    case 1:   // LAZY's repeat-offset records go to seq_stage, free once k_cmatch is done
         if (!a.level || !a.nblocks) return 0;
-        if (a.etab) k_cenc<true><<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res, a.etab);
-        else k_cenc<false><<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res, nullptr);
+        if (lazy) {
+            if (a.etab) k_cenc<true, true><<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res, a.etab, a.seq_stage);
+            else k_cenc<false, true><<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res, nullptr, a.seq_stage);
+        } else if (a.etab) k_cenc<true, false><<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res, a.etab, nullptr);
+        else k_cenc<false, false><<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res, nullptr, nullptr);
         break;
     case 2: if (!a.checksum || !a.nframes) return 0; k_cxxh64<<<cdiv_u((uint64_t)a.nframes * 4, 128), 128, 0, s>>>(a.frames, a.input, a.csum, a.nframes); break;
     case 3: if (!a.nblocks) return 0; k_cassemble<false><<<a.nblocks, 256, 0, s>>>(a.frames, a.blocks, a.res, a.enc, a.input, a.csum, a.output, a.results, a.level, a.checksum, a.dict_id); break;
