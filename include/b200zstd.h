@@ -130,7 +130,11 @@ typedef enum b200z_error {
     ,
     /* this build only */
     B200Z_ERR_NO_DEVICE = 230,
-    B200Z_ERR_CUDA = 231
+    B200Z_ERR_CUDA = 231,
+    /* EXTENSION, seekable archives (b200z_seekable_*): the seek table breaks one of the format's rules (the message names it) */
+    B200Z_ERR_SEEKABLE_TABLE = 240,
+    /* EXTENSION, seekable archives: a frame decoded to a size other than its seek-table entry's Decompressed_Size */
+    B200Z_ERR_SEEKABLE_FRAME_SIZE = 241
 } b200z_error;
 
 /* stage that raised the error == nesting path of the reference's FrameDecoderError (errors.rs:472-486) */
@@ -686,6 +690,105 @@ int b200z_dict_finalize(b200z_ctx *ctx, const uint8_t *content, size_t content_l
  * OF codes 0-31, in that order), with the same argument checks */
 int b200z_debug_dict_from_counts(const uint64_t counts[377], const uint8_t *content, size_t content_len, uint32_t dict_id,
                                  uint8_t *dict, size_t dict_cap, size_t *dict_len);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * Seekable archives -- EXTENSION (ruzstd has no seekable support): the zstd seekable format of zstd's contrib/seekable_format.
+ * An archive is independent zstd frames back to back followed by one skippable frame that holds the seek table:
+ *   Skippable_Magic_Number u32 LE 0x184D2A5E, Frame_Size u32 LE = n * (8 or 12) + 9, then per frame Compressed_Size u32,
+ *   Decompressed_Size u32 and, with the Checksum_Flag, the low 32 bits of XXH64 (seed 0) of its plaintext; then the footer
+ *   Number_Of_Frames u32 n, Seek_Table_Descriptor u8 (bit 7 Checksum_Flag, bits 6-2 reserved, must be 0) and
+ *   Seekable_Magic_Number u32 LE 0x8F92EAB1, the archive's last 9 bytes.
+ * Every zstd decoder reads an archive as concatenated frames and a skippable frame (decode_all, tiers 1c and 1d); a reader that
+ * knows the table decodes only the frames a byte range touches (b200z_seekable_read_ranges).  DESIGN.md section 4.10.
+ * ---------------------------------------------------------------------------------------------------------------------------- */
+/* blocks (128 KiB each, a frame's last one shorter) b200z_compress_seekable compresses per submission: a group holds whole frames,
+ * as many as fit in this many blocks, or one frame when a frame alone has more.  The device memory the call holds depends on it
+ * (and on frame_size when one frame has more blocks), not on the archive: the compressor's staging of about 0.9 MB per block of the
+ * largest group -- at most 2048 blocks (1.8 GB), and never more than the input's own blocks -- and with host memory that group's
+ * input (up to 256 MiB) and its frames' bounds (b200z_compress_bound_dict each). */
+#define B200Z_SEEKABLE_GROUP_BLOCKS 2048
+#define B200Z_SEEKABLE_MAX_FRAME_SIZE (1u << 30)
+
+/* b200z_compress_bound_dict of every frame (frame_size bytes each, the last one shorter) plus the seek table (17 bytes and 8 per
+ * frame, 12 with `checksum`); 0 when frame_size is 0 or above B200Z_SEEKABLE_MAX_FRAME_SIZE */
+size_t b200z_seekable_bound(size_t src_size, size_t frame_size, int checksum, const b200z_dict *dict);
+/* Compresses `input` into a seekable archive at `output` (host or device memory, B200Z_MEM_*); *written = the archive's bytes.
+ * The input is cut into frames of frame_size bytes (the last one shorter; an empty input gives no frame, and the archive is the
+ * table alone).  Every frame is byte for byte what b200z_compress_frames_batch_dict writes for that piece with the same level,
+ * checksum, dictionary and B200Z_FLAG_DICT_TABLES; the frames lie back to back from output[0], the table behind them.  With
+ * `checksum` the table carries each frame's checksum (the one its trailer holds) and sets the Checksum_Flag.  The frames go
+ * through in groups of whole frames (B200Z_SEEKABLE_GROUP_BLOCKS); host input is uploaded and host output downloaded group by
+ * group.  Kernels per group: those of b200z_compress_frames_batch_dict (k_cmatch, k_cenc, k_cxxh64 with `checksum`, k_cassemble;
+ * none of the first two at Uncompressed) plus k_cscan; then one k_cseek; all counted in b200z_ctx_kernel_launches.  Checked before
+ * any launch: what b200z_compress_frames_batch_dict checks (levels, dictionary), and B200Z_ERR_INVALID_ARGUMENT for frame_size 0 or
+ * above B200Z_SEEKABLE_MAX_FRAME_SIZE, more than 2^32 - 1 frames, or output_cap < b200z_seekable_bound. */
+int b200z_compress_seekable(b200z_ctx *ctx, const uint8_t *input, size_t input_len, int input_mem, size_t frame_size, int level,
+                            int checksum, const b200z_dict *dict, uint8_t *output, size_t output_cap, int output_mem, size_t *written);
+
+/* An open archive: its table, parsed and checked.  It borrows the archive (host or device memory), which the caller keeps alive and
+ * unchanged until b200z_seekable_close; of a device archive only the table is copied to the host.  B200Z_ERR_SEEKABLE_TABLE, with
+ * the rule in b200z_ctx_last_error_message, when the footer magic, the reserved bits, the skippable magic or Frame_Size is wrong,
+ * when the table does not lie inside the archive, or when the entries' Compressed_Size do not add up to the table's offset. */
+typedef struct b200z_seekable b200z_seekable;
+typedef struct b200z_seek_frame {
+    uint64_t c_off, c_size;   /* the frame's bytes in the archive                                                      */
+    uint64_t d_off, d_size;   /* its plaintext in the archive's content (the Decompressed_Size before it, summed)      */
+    uint32_t has_checksum;    /* the table carries checksums                                                           */
+    uint32_t checksum;
+} b200z_seek_frame;
+int b200z_seekable_open(b200z_ctx *ctx, const uint8_t *archive, size_t len, int mem, b200z_seekable **out);
+uint64_t b200z_seekable_num_frames(const b200z_seekable *s);
+uint64_t b200z_seekable_content_size(const b200z_seekable *s);
+int b200z_seekable_frame(const b200z_seekable *s, uint64_t i, b200z_seek_frame *out);
+void b200z_seekable_close(b200z_seekable *s);
+
+/* one range: plaintext [offset, offset + length) of the archive's content, written at output + out_off */
+typedef struct b200z_range {
+    uint64_t offset, length, out_off;
+} b200z_range;
+typedef struct b200z_range_result {
+    int32_t status;                /* 0, the b200z_error of the first failing frame it needs (in content order), or
+                                      B200Z_ERR_SEEKABLE_FRAME_SIZE when that frame decoded to another size than its entry */
+    int32_t stage;                 /* b200z_stage of the error                                                            */
+    int64_t error_frame;           /* the archive frame that failed, -1 when none                                          */
+    uint64_t frames;               /* archive frames the range touches                                                     */
+    uint64_t checksum_mismatches;  /* B200Z_FLAG_CHECKSUM: touched frames whose GPU checksum differs from their table entry
+                                      or from their own trailer (reported, never enforced)                                 */
+} b200z_range_result;
+/* Reads `n` ranges into `output` (host or device memory).  Checked before any work, B200Z_ERR_INVALID_ARGUMENT: a range that
+ * reaches past the content size or past output_cap, and ranges whose output slots overlap (ranges may overlap in the content).
+ * Every frame the ranges touch is decoded once, in one submission of the batch decoder (b200z_batch_prepare / _run with
+ * b200z_frame_io built from the table; `dicts`, `forced_dict` and `max_window_size` as for b200z_decode_frames_batch) with
+ * out_cap = its Decompressed_Size: a frame that lies wholly inside a range is decoded in place, in the first such range's slot (the
+ * decoder writes a frame's [out_off, out_off + out_cap) only); any other touched frame -- at most two per range -- into device
+ * scratch.  k_range_gather then copies each range's other bytes from scratch or from another range's slot.  Host archives: only
+ * the touched frames' bytes are gathered and uploaded.  Host output: the ranges' slots are staged on the device and copied to
+ * their out_off; no other byte of `output` is written.  With B200Z_FLAG_CHECKSUM, device output must be readable 8 bytes past a
+ * slot that ends at output_cap.  Kernels: the batch pass (b200z_batch_info[6]; with a device archive also the planner's two k_walk
+ * launches), and one k_range_gather when some range has bytes outside its in-place frames; none when no range touches a frame.
+ * Returns 0 when the call ran (outcomes in results[n]). */
+int b200z_seekable_read_ranges(b200z_seekable *s, const b200z_range *ranges, size_t n, const b200z_dict *const *dicts, size_t ndicts,
+                               const b200z_dict *forced_dict, uint64_t max_window_size, uint8_t *output, size_t output_cap, int output_mem,
+                               b200z_range_result *results);
+
+/* Host-only view of the read plan (no context, no device; for CPU tests): the archive's table (host memory, checked as by
+ * b200z_seekable_open) and the ranges (checked as by b200z_seekable_read_ranges, with no output_cap).  plan_frames: every touched
+ * frame once, by ascending frame index; range = the range it is decoded in place for (dst_off in the output), or -1 (dst_off in
+ * scratch: the frames that are not in place, by ascending index, each at a multiple of 16).  pieces: per range in call order, per
+ * touched frame by ascending index that is not in place for that range, the bytes it takes from the frame: len bytes from src_off
+ * (scratch, or the output when the frame is in place for another range) to dst_off in the output.  *scratch_bytes: the scratch's
+ * size.  *nframes / *npieces are set even when the caps are too small (then nothing is written; B200Z_ERR_INVALID_ARGUMENT). */
+typedef struct b200z_seek_plan_frame {
+    uint64_t frame, dst_off;
+    int64_t range;
+} b200z_seek_plan_frame;
+typedef struct b200z_seek_plan_piece {
+    uint64_t dst_off, src_off, len;
+    uint32_t from_scratch, range;
+} b200z_seek_plan_piece;
+int b200z_debug_seekable_plan(const uint8_t *archive, size_t len, const b200z_range *ranges, size_t n, b200z_seek_plan_frame *frames,
+                              size_t frames_cap, size_t *nframes, b200z_seek_plan_piece *pieces, size_t pieces_cap, size_t *npieces,
+                              uint64_t *scratch_bytes);
 
 /* XXH64(seed 0) of a host buffer -- the content-checksum hash the reference feeds on drain
  * (decode_buffer.rs:42,225,290,301); exposed so bindings can verify checksums like tests/decode_corpus.rs:61-74 */

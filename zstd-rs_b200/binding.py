@@ -24,6 +24,8 @@ WRITE_FN = C.CFUNCTYPE(C.c_long, C.c_void_p, C.POINTER(C.c_uint8), C.c_size_t)
 ALL, UPTO_BLOCKS, UPTO_BYTES = 0, 1, 2
 MEM_HOST, MEM_DEVICE = 0, 1
 ERR_SKIP_FRAME = 8
+ERR_INVALID_ARGUMENT = 220
+ERR_SEEKABLE_TABLE, ERR_SEEKABLE_FRAME_SIZE = 240, 241   # EXTENSION: seekable archives
 FLAG_CHECKSUM = 1
 FLAG_PROFILE = 2
 FLAG_DICT_TABLES = 4
@@ -176,6 +178,15 @@ def lib():
         "b200z_dict_train_raw": (C.c_int, [vp, vp, sz, C.c_int, vp, sz, sz, sz, vp, sz, C.POINTER(sz), vp, sz, C.POINTER(sz)]),
         "b200z_dict_finalize": (C.c_int, [vp, vp, sz, vp, sz, C.c_int, vp, sz, C.c_uint32, vp, sz, C.POINTER(sz)]),
         "b200z_debug_dict_from_counts": (C.c_int, [vp, vp, sz, C.c_uint32, vp, sz, C.POINTER(sz)]),
+        "b200z_seekable_bound": (sz, [sz, sz, C.c_int, vp]),
+        "b200z_compress_seekable": (C.c_int, [vp, vp, sz, C.c_int, sz, C.c_int, C.c_int, vp, vp, sz, C.c_int, C.POINTER(sz)]),
+        "b200z_seekable_open": (C.c_int, [vp, vp, sz, C.c_int, pp]),
+        "b200z_seekable_num_frames": (C.c_uint64, [vp]),
+        "b200z_seekable_content_size": (C.c_uint64, [vp]),
+        "b200z_seekable_frame": (C.c_int, [vp, C.c_uint64, vp]),
+        "b200z_seekable_close": (None, [vp]),
+        "b200z_seekable_read_ranges": (C.c_int, [vp, vp, sz, pp, sz, vp, C.c_uint64, vp, sz, C.c_int, vp]),
+        "b200z_debug_seekable_plan": (C.c_int, [vp, sz, vp, sz, vp, sz, C.POINTER(sz), vp, sz, C.POINTER(sz), C.POINTER(C.c_uint64)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)          # AttributeError here == a symbol the header declares is not exported
@@ -575,6 +586,144 @@ def compress_to_vec(ctx, data, level=FASTEST, checksum=True, dict=None, dict_tab
     io = np.array([(0, len(src), 0, cap)], dtype=COMPRESS_IO_DTYPE)
     res = compress_frames(ctx, src, io, out, level, checksum, dict, dict_tables)
     return out[:int(res[0]["dst_size"])].tobytes()
+
+
+# ---- seekable archives (EXTENSION: zstd's seekable format; include/b200zstd.h, DESIGN.md section 4.10)
+SEEKABLE_GROUP_BLOCKS = 2048   # B200Z_SEEKABLE_GROUP_BLOCKS
+SEEKABLE_MAX_FRAME_SIZE = 1 << 30
+SEEK_FRAME_DTYPE = np.dtype([("c_off", "<u8"), ("c_size", "<u8"), ("d_off", "<u8"), ("d_size", "<u8"), ("has_checksum", "<u4"),
+                             ("checksum", "<u4")])
+RANGE_DTYPE = np.dtype([("offset", "<u8"), ("length", "<u8"), ("out_off", "<u8")])
+RANGE_RESULT_DTYPE = np.dtype([("status", "<i4"), ("stage", "<i4"), ("error_frame", "<i8"), ("frames", "<u8"), ("checksum_mismatches", "<u8")])
+SEEK_PLAN_FRAME_DTYPE = np.dtype([("frame", "<u8"), ("dst_off", "<u8"), ("range", "<i8")])
+SEEK_PLAN_PIECE_DTYPE = np.dtype([("dst_off", "<u8"), ("src_off", "<u8"), ("len", "<u8"), ("from_scratch", "<u4"), ("range", "<u4")])
+
+
+def seekable_bound(n, frame_size=131072, checksum=True, dict=None):
+    """b200z_seekable_bound: the largest archive compress_seekable can write for n input bytes (0 for a frame_size out of range)."""
+    return lib().b200z_seekable_bound(n, frame_size, 1 if checksum else 0, dict.h if dict is not None else None)
+
+
+def compress_seekable(ctx, input, output=None, frame_size=131072, level=FASTEST, checksum=True, dict=None, dict_tables=False):
+    """b200z_compress_seekable: a seekable archive of `input` -- frames of frame_size bytes, each what compress_frames writes for that
+    piece, back to back, then the seek table.  input/output: bytes, numpy or torch (host or cuda).  Returns the archive (bytes for a
+    host input, a uint8 CUDA tensor for a device one) when output is None, else the archive's size in bytes."""
+    ip, il, _k1 = _ptr(input)
+    ret = output is None
+    if ret:
+        cap = max(seekable_bound(il, frame_size, checksum, dict), 1)
+        if _is_device(input):
+            import torch
+            output = torch.empty(cap, dtype=torch.uint8, device=input.device)
+        else:
+            output = np.empty(cap, dtype=np.uint8)
+    op, ol, _k2 = _ptr(output)
+    written = C.c_size_t()
+    flags = ctx.L.b200z_ctx_flags(ctx.h)
+    if dict_tables:
+        ctx.L.b200z_ctx_set_flags(ctx.h, flags | FLAG_DICT_TABLES)
+    try:
+        e = ctx.L.b200z_compress_seekable(ctx.h, ip, il, MEM_DEVICE if _is_device(input) else MEM_HOST, frame_size, level, 1 if checksum else 0,
+                                          dict.h if dict is not None else None, op, ol, MEM_DEVICE if _is_device(output) else MEM_HOST,
+                                          C.byref(written))
+    finally:
+        ctx.L.b200z_ctx_set_flags(ctx.h, flags)
+    ctx._chk(e)
+    if not ret:
+        return written.value
+    return output[:written.value] if _is_device(output) else output[:written.value].tobytes()
+
+
+def _ranges_array(ranges):
+    if isinstance(ranges, np.ndarray) and ranges.dtype == RANGE_DTYPE:
+        return np.ascontiguousarray(ranges)
+    return np.array([tuple(r) for r in ranges], dtype=RANGE_DTYPE) if len(ranges) else np.zeros(0, dtype=RANGE_DTYPE)
+
+
+class SeekableArchive:
+    """An open seekable archive (b200z_seekable_open): its table, parsed and checked.  It borrows `archive` (bytes, numpy or torch, host
+    or cuda) and keeps a reference to it.  .num_frames, .content_size, .frames (SEEK_FRAME_DTYPE rows), .read(offset, length) and
+    .read_ranges(ranges, output).  A context manager; close() releases the handle."""
+
+    def __init__(self, ctx, archive):
+        self.ctx = ctx
+        self.h = None
+        ap, al, self._k = _ptr(archive)
+        self._archive = archive
+        h = C.c_void_p()
+        ctx._chk(ctx.L.b200z_seekable_open(ctx.h, ap, al, MEM_DEVICE if _is_device(archive) else MEM_HOST, C.byref(h)))
+        self.h = h
+
+    @property
+    def num_frames(self):
+        return self.ctx.L.b200z_seekable_num_frames(self.h)
+
+    @property
+    def content_size(self):
+        return self.ctx.L.b200z_seekable_content_size(self.h)
+
+    @property
+    def frames(self):
+        out = np.zeros(self.num_frames, dtype=SEEK_FRAME_DTYPE)
+        for i in range(len(out)):
+            self.ctx._chk(self.ctx.L.b200z_seekable_frame(self.h, i, out[i:].ctypes.data))
+        return out
+
+    def read_ranges(self, ranges, output, dicts=None, forced_dict=None, max_window_size=0):
+        """b200z_seekable_read_ranges: RANGE_DTYPE rows (or (offset, length, out_off) tuples) into `output` (numpy or torch, host or
+        cuda).  Returns RANGE_RESULT_DTYPE rows; a range that could not be read is reported there, not raised."""
+        rg = _ranges_array(ranges)
+        res = np.zeros(len(rg), dtype=RANGE_RESULT_DTYPE)
+        op, ol, _k = _ptr(output)
+        darr, nd, forced = _dict_args(dicts, forced_dict)
+        self.ctx._chk(self.ctx.L.b200z_seekable_read_ranges(self.h, rg.ctypes.data, len(rg), darr, nd, forced, max_window_size, op, ol,
+                                                            MEM_DEVICE if _is_device(output) else MEM_HOST, res.ctypes.data))
+        return res
+
+    def read(self, offset, length, dicts=None, forced_dict=None):
+        """Plaintext [offset, offset + length) as bytes; raises B200ZError when a frame it needs fails."""
+        out = np.zeros(max(length, 1), dtype=np.uint8)
+        r = self.read_ranges([(offset, length, 0)], out, dicts, forced_dict)
+        if r[0]["status"]:
+            raise B200ZError(int(r[0]["status"]), int(r[0]["stage"]), f"frame {int(r[0]['error_frame'])}")
+        return out[:length].tobytes()
+
+    def close(self):
+        if getattr(self, "h", None) and self.ctx.h:
+            self.ctx.L.b200z_seekable_close(self.h)
+        self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def seekable_plan(archive, ranges):
+    """Host-only: the read plan b200z_seekable_read_ranges follows for `ranges` on the host archive -- (SEEK_PLAN_FRAME_DTYPE rows,
+    SEEK_PLAN_PIECE_DTYPE rows, scratch bytes).  Raises B200ZError for a corrupt table or invalid ranges."""
+    a = np.frombuffer(bytes(archive), dtype=np.uint8)
+    rg = _ranges_array(ranges)
+    nf, npc, scr = C.c_size_t(), C.c_size_t(), C.c_uint64()
+    fcap, pcap = 16, 16
+    while True:
+        fr = np.zeros(fcap, dtype=SEEK_PLAN_FRAME_DTYPE)
+        pc = np.zeros(pcap, dtype=SEEK_PLAN_PIECE_DTYPE)
+        rc = lib().b200z_debug_seekable_plan(a.ctypes.data if len(a) else None, len(a), rg.ctypes.data if len(rg) else None, len(rg), fr.ctypes.data,
+                                             fcap, C.byref(nf), pc.ctypes.data, pcap, C.byref(npc), C.byref(scr))
+        if rc == 0:
+            return fr[:nf.value], pc[:npc.value], scr.value
+        if rc == ERR_INVALID_ARGUMENT and (nf.value > fcap or npc.value > pcap):
+            fcap, pcap = max(fcap, nf.value), max(pcap, npc.value)
+            continue
+        raise B200ZError(rc, 0, "b200z_debug_seekable_plan")
 
 
 class FrameCompressor:

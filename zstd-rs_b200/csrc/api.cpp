@@ -51,6 +51,7 @@ const ErrName kErrNames[] = {
     EN(ERR_SEQ_MISSING_BYTE_FOR_RLE_ML_TABLE), EN(ERR_EXEC_NOT_ENOUGH_BYTES_FOR_SEQUENCE), EN(ERR_EXEC_ZERO_OFFSET),
     EN(ERR_EXEC_NOT_ENOUGH_BYTES_IN_DICTIONARY), EN(ERR_EXEC_OFFSET_TOO_BIG), EN(ERR_DICT_NOT_ENOUGH_BYTES), EN(ERR_DICT_BAD_MAGIC_NUM),
     EN(ERR_REFERENCE_WOULD_PANIC), EN(ERR_BLOCK_OUTPUT_LIMIT), EN(ERR_INVALID_ARGUMENT), EN(ERR_OUT_OF_MEMORY), EN(ERR_NO_DEVICE), EN(ERR_CUDA),
+    EN(ERR_SEEKABLE_TABLE), EN(ERR_SEEKABLE_FRAME_SIZE),
 };
 #undef EN
 
@@ -2539,6 +2540,9 @@ struct CompressResources {
     DevBuf frames, blocks, csum, results, input, output;
     CompressStaging stage;
     DevBuf dcontent, dtab, dcounts;   // b200z_dict_finalize: the content's tail, its match table and the statistics
+    DevBuf seek_entries, seek_total;  // b200z_compress_seekable: the table's entries and the running archive size
+    DevBuf rd_stage, rd_pieces;       // b200z_seekable_read_ranges: host output's slots and the scratch, the copy pieces
+    PinnedBuf rd_host;                // b200z_seekable_read_ranges: the touched frames of a host archive, host output's slots
     Event ev[kCompressStages + 1];
     float stage_ms[kCompressStages] = {};
     bool profiled = false;
@@ -2556,6 +2560,37 @@ static int compress_get(b200z_ctx *c, CompressResources **out) {
 extern "C" int b200z_compress_last_profile(const b200z_ctx *c, float *stage_ms, size_t n) {
     if (!c || !stage_ms || !c->comp || !c->comp->profiled) return B200Z_ERR_INVALID_ARGUMENT;
     for (size_t i = 0; i < n && i < (size_t)kCompressStages; i++) stage_ms[i] = c->comp->stage_ms[i];
+    return 0;
+}
+
+// The dictionary's part of a compression's CompressArgs (dict_id, the match table, the encoder's tables).  The match table is built
+// once and kept with the dictionary (not one of the timed stages); offsets stay within the 128 KiB window, so the kernels see the
+// content's last ENC_WINDOW bytes only.  The encoder's view of a formatted dictionary's tables is built on the host once and kept
+// with the dictionary (no launch).
+static int compress_dict_args(b200z_ctx *c, const b200z_dict *dict, int level, CompressArgs &a) {
+    const bool fast = level != B200Z_LEVEL_UNCOMPRESSED;
+    const bool match_dict = fast && dict && dict->content_len >= ENC_MIN_MATCH;
+    const uint32_t dict_tail = dict ? (uint32_t)std::min<size_t>(dict->content_len, ENC_WINDOW) : 0;
+    const uint8_t *dict_at = dict ? dict->d_content.as<uint8_t>() + (dict->content_len - dict_tail) : nullptr;
+    if (match_dict && !dict->d_ctab.p) {
+        DevBuf tab;
+        CU(c, tab.alloc(sizeof(uint32_t) << CD_LOG));
+        if (int le = launch_dict_table(dict_at, dict_tail, tab.as<uint32_t>(), c->stream, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_cdict");
+        dict->d_ctab = std::move(tab);
+    }
+    const bool use_tables = fast && dict && dict->has_tables && (c->flags & B200Z_FLAG_DICT_TABLES);
+    if (use_tables && !dict->d_enc.p) {
+        std::unique_ptr<EncDict> ed(new EncDict());
+        const int16_t *probs[3] = {dict->norm[0], dict->norm[1], dict->norm[2]};
+        enc_dict_build(dict->huf_weights, dict->huf_nweights, probs, dict->nnorm, dict->log, *ed);
+        DevBuf enc;
+        CU(c, enc.alloc(sizeof(EncDict)));
+        CU(c, cudaMemcpy(enc.p, ed.get(), sizeof(EncDict), cudaMemcpyHostToDevice));
+        dict->d_enc = std::move(enc);
+    }
+    a.etab = use_tables ? dict->d_enc.as<EncDict>() : nullptr;
+    a.dict_id = compress_dict_id(dict);
+    if (match_dict) { a.dict = dict_at; a.dtab = dict->d_ctab.as<uint32_t>(); a.dict_len = dict_tail; }
     return 0;
 }
 
@@ -2635,37 +2670,13 @@ extern "C" int b200z_compress_frames_batch_dict(b200z_ctx *c, const uint8_t *inp
     }
     CU(c, cudaMemcpyAsync(r.frames.p, hf.data(), nframes * sizeof(CFrame), cudaMemcpyHostToDevice, s));
     CU(c, cudaMemcpyAsync(r.blocks.p, hb.data(), nblocks * sizeof(CBlock), cudaMemcpyHostToDevice, s));
-    // the dictionary's match table, built once and kept with the dictionary (not one of the timed stages).  Offsets stay within
-    // the 128 KiB window, so the kernels see the content's last ENC_WINDOW bytes only.
-    const bool match_dict = fast && dict && dict->content_len >= ENC_MIN_MATCH;
-    const uint32_t dict_tail = dict ? (uint32_t)std::min<size_t>(dict->content_len, ENC_WINDOW) : 0;
-    const uint8_t *dict_at = dict ? dict->d_content.as<uint8_t>() + (dict->content_len - dict_tail) : nullptr;
-    if (match_dict && !dict->d_ctab.p) {
-        DevBuf tab;
-        CU(c, tab.alloc(sizeof(uint32_t) << CD_LOG));
-        if (int le = launch_dict_table(dict_at, dict_tail, tab.as<uint32_t>(), s, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_cdict");
-        dict->d_ctab = std::move(tab);
-    }
-    // the encoder's view of a formatted dictionary's tables, built on the host once and kept with the dictionary (no launch)
-    const bool use_tables = fast && dict && dict->has_tables && (c->flags & B200Z_FLAG_DICT_TABLES);
-    if (use_tables && !dict->d_enc.p) {
-        std::unique_ptr<EncDict> ed(new EncDict());
-        const int16_t *probs[3] = {dict->norm[0], dict->norm[1], dict->norm[2]};
-        enc_dict_build(dict->huf_weights, dict->huf_nweights, probs, dict->nnorm, dict->log, *ed);
-        DevBuf enc;
-        CU(c, enc.alloc(sizeof(EncDict)));
-        CU(c, cudaMemcpy(enc.p, ed.get(), sizeof(EncDict), cudaMemcpyHostToDevice));
-        dict->d_enc = std::move(enc);
-    }
     CompressArgs a{};
+    if ((e = compress_dict_args(c, dict, level, a))) return e;
     a.frames = r.frames.as<CFrame>(); a.blocks = r.blocks.as<CBlock>(); a.input = d_in; a.output = d_out;
-    a.etab = use_tables ? dict->d_enc.as<EncDict>() : nullptr;
     r.stage.bind(a);
     a.csum = r.csum.as<uint64_t>();
     a.results = r.results.as<b200z_compress_result>(); a.nframes = (uint32_t)nframes; a.nblocks = (uint32_t)nblocks; a.level = level;
     a.checksum = checksum ? 1 : 0;
-    a.dict_id = compress_dict_id(dict);
-    if (match_dict) { a.dict = dict_at; a.dtab = dict->d_ctab.as<uint32_t>(); a.dict_len = dict_tail; }
     const bool prof = (c->flags & B200Z_FLAG_PROFILE) != 0;
     if (prof) CU(c, cudaEventRecord(r.ev[0], s));
     for (int st = 0; st < kCompressStages; st++) {
@@ -2680,6 +2691,407 @@ extern "C" int b200z_compress_frames_batch_dict(b200z_ctx *c, const uint8_t *inp
     r.profiled = prof;
     if (prof)
         for (int st = 0; st < kCompressStages; st++) CU(c, cudaEventElapsedTime(&r.stage_ms[st], r.ev[st], r.ev[st + 1]));
+    return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// seekable archives (EXTENSION: zstd's seekable format, DESIGN.md section 4.10).  Writing: the batch compressor's kernels per group of
+// whole frames, with k_cscan packing each group's frames behind the archive so far, and k_cseek writing the table.  Reading: the table
+// is parsed on the host, the ranges become a plan (frames to decode, in place or into scratch, and copy pieces), the frames go through
+// the batch decoder's planner and pass, and k_range_gather copies the pieces.
+// ---------------------------------------------------------------------------------------------------------------
+static uint32_t seek_le32(const uint8_t *p) { return (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24; }
+static uint64_t seek_table_size(uint64_t nframes, bool checksum) { return SEEK_TABLE_FIXED + nframes * (checksum ? 12 : 8); }
+
+extern "C" size_t b200z_seekable_bound(size_t n, size_t frame_size, int checksum, const b200z_dict *dict) {
+    if (!frame_size || frame_size > B200Z_SEEKABLE_MAX_FRAME_SIZE) return 0;
+    const uint64_t full = n / frame_size, rest = n % frame_size;
+    return full * b200z_compress_bound_dict(frame_size, dict) + (rest ? b200z_compress_bound_dict(rest, dict) : 0) +
+           seek_table_size(full + (rest ? 1 : 0), checksum != 0);
+}
+
+extern "C" int b200z_compress_seekable(b200z_ctx *c, const uint8_t *input, size_t input_len, int input_mem, size_t frame_size, int level,
+                                       int checksum, const b200z_dict *dict, uint8_t *output, size_t output_cap, int output_mem, size_t *written) {
+    // ---- everything is checked before any device work, as b200z_compress_frames_batch_dict checks it
+    if (level >= 2 && level <= 4) return B200Z_ERR_REFERENCE_WOULD_PANIC;
+    if (!c || (level != B200Z_LEVEL_UNCOMPRESSED && level != B200Z_LEVEL_FASTEST && level != B200Z_LEVEL_LAZY)) return B200Z_ERR_INVALID_ARGUMENT;
+    if (dict && dict->ctx != c) { c->err = "dictionary created on another context"; return B200Z_ERR_INVALID_ARGUMENT; }
+    if ((input_mem != B200Z_MEM_HOST && input_mem != B200Z_MEM_DEVICE) || (output_mem != B200Z_MEM_HOST && output_mem != B200Z_MEM_DEVICE) ||
+        (input_len && !input) || !output || !written) {
+        c->err = "invalid argument";
+        return B200Z_ERR_INVALID_ARGUMENT;
+    }
+    if (!frame_size || frame_size > B200Z_SEEKABLE_MAX_FRAME_SIZE) { c->err = "frame_size must lie in [1, 2^30]"; return B200Z_ERR_INVALID_ARGUMENT; }
+    const uint64_t nframes = (input_len + frame_size - 1) / frame_size;
+    if (nframes > 0xffffffffull) { c->err = "more than 2^32 - 1 frames"; return B200Z_ERR_INVALID_ARGUMENT; }
+    if (output_cap < b200z_seekable_bound(input_len, frame_size, checksum, dict)) {
+        c->err = "output_cap < b200z_seekable_bound(input_len, frame_size, checksum, dict)";
+        return B200Z_ERR_INVALID_ARGUMENT;
+    }
+    *written = 0;
+    if (int e = c->use()) return e;
+    CompressResources *rp = nullptr;
+    if (int e = compress_get(c, &rp)) return e;
+    CompressResources &r = *rp;
+    const bool fast = level != B200Z_LEVEL_UNCOMPRESSED;
+    const bool sum = checksum != 0;
+    const uint64_t fblocks = std::max<uint64_t>(1, (frame_size + ENC_BLOCK - 1) / ENC_BLOCK);   // blocks of a full frame
+    const uint64_t per_group = std::max<uint64_t>(1, B200Z_SEEKABLE_GROUP_BLOCKS / fblocks);   // frames per group
+    // what the largest group holds -- frames, blocks, input bytes and its frames' bounds -- from the frames the input really has:
+    // every group but the last is full, so the first and the last group are the candidates
+    uint64_t gframes = 1, gblocks = 1, gin = 0, gout = 0;
+    for (uint64_t f0 : {uint64_t(0), nframes ? (nframes - 1) / per_group * per_group : uint64_t(0)}) {
+        const uint64_t f1 = std::min(nframes, f0 + per_group);
+        const uint64_t in0 = std::min<uint64_t>(f0 * frame_size, input_len), in1 = std::min<uint64_t>(f1 * frame_size, input_len);
+        const uint64_t full = f1 > f0 ? (in1 - in0) / frame_size : 0, rest = f1 > f0 ? (in1 - in0) % frame_size : 0;
+        gframes = std::max(gframes, f1 - f0);
+        gblocks = std::max(gblocks, full * fblocks + (rest ? (rest + ENC_BLOCK - 1) / ENC_BLOCK : 0));
+        gin = std::max(gin, in1 - in0);
+        gout = std::max(gout, full * b200z_compress_bound_dict(frame_size, dict) + (rest ? b200z_compress_bound_dict(rest, dict) : 0));
+    }
+    const uint64_t table = seek_table_size(nframes, sum);
+    int e = 0;
+    if ((e = r.frames.ensure(gframes * sizeof(CFrame))) || (e = r.blocks.ensure(gblocks * sizeof(CBlock))) ||
+        (e = fast ? r.stage.ensure(gblocks, true) : r.stage.res.ensure(gblocks * sizeof(CBlockInfo))) ||
+        (e = r.csum.ensure(gframes * 8)) || (e = r.results.ensure(gframes * sizeof(b200z_compress_result))) ||
+        (e = r.seek_entries.ensure(std::max<uint64_t>(table, 16))) || (e = r.seek_total.ensure(8)))
+        return e;
+    if (input_mem == B200Z_MEM_HOST && (e = r.input.ensure(gin + 16))) return e;
+    if (output_mem == B200Z_MEM_HOST && (e = r.output.ensure(std::max(gout, table) + 16))) return e;
+    cudaStream_t s = c->stream;
+    CompressArgs a{};
+    if ((e = compress_dict_args(c, dict, level, a))) return e;
+    a.frames = r.frames.as<CFrame>(); a.blocks = r.blocks.as<CBlock>();
+    r.stage.bind(a);
+    a.csum = r.csum.as<uint64_t>(); a.results = r.results.as<b200z_compress_result>();
+    a.level = level; a.checksum = sum ? 1 : 0;
+    uint64_t *d_total = r.seek_total.as<uint64_t>();
+    CU(c, cudaMemsetAsync(d_total, 0, 8, s));
+    uint64_t origin = 0;        // archive offset of d_out's byte 0 (host output: the group's first byte)
+    std::vector<CFrame> hf;
+    std::vector<CBlock> hb;
+    for (uint64_t f0 = 0; f0 < nframes; f0 += per_group) {
+        const uint64_t f1 = std::min(nframes, f0 + per_group);
+        const uint64_t in0 = f0 * frame_size, in1 = std::min<uint64_t>(f1 * frame_size, input_len);
+        const uint64_t base = input_mem == B200Z_MEM_HOST ? in0 : 0;   // host input: the group is uploaded to r.input's byte 0
+        hf.clear(); hb.clear();
+        for (uint64_t f = f0; f < f1; f++) {   // the plan of b200z_compress_frames_batch_dict for the same pieces
+            const uint64_t off = f * frame_size - base, size = std::min<uint64_t>(frame_size, input_len - f * frame_size);
+            hf.push_back(CFrame{off, size, 0, (uint32_t)hb.size(), 0});
+            uint64_t pos = 0;
+            do {
+                const uint32_t bs = (uint32_t)std::min<uint64_t>(ENC_BLOCK, size - pos);
+                hb.push_back(CBlock{off + pos, bs, (uint32_t)std::min<uint64_t>(pos, ENC_WINDOW), (uint32_t)(f - f0), 0});
+                pos += bs;
+            } while (pos < size);
+            hf.back().nblocks = (uint32_t)hb.size() - hf.back().first_block;
+        }
+        a.input = input;
+        if (input_mem == B200Z_MEM_HOST) {
+            CU(c, cudaMemcpyAsync(r.input.p, input + in0, in1 - in0, cudaMemcpyHostToDevice, s));
+            a.input = r.input.as<uint8_t>();
+        }
+        a.output = output_mem == B200Z_MEM_HOST ? r.output.as<uint8_t>() : output;
+        a.nframes = (uint32_t)hf.size(); a.nblocks = (uint32_t)hb.size();
+        CU(c, cudaMemcpyAsync(r.frames.p, hf.data(), hf.size() * sizeof(CFrame), cudaMemcpyHostToDevice, s));
+        CU(c, cudaMemcpyAsync(r.blocks.p, hb.data(), hb.size() * sizeof(CBlock), cudaMemcpyHostToDevice, s));
+        for (int st = 0; st < kCompressStages; st++) {
+            if (st == 3)
+                if (int le = launch_seek_scan(a, d_total, origin, r.seek_entries.as<uint8_t>(), f0, s, &c->launches))
+                    return c->set_cuda_err((cudaError_t)le, "k_cscan");
+            if (int le = launch_compress_stage(a, st, s, &c->launches)) return c->set_cuda_err((cudaError_t)le, kCompressStageNames[st]);
+        }
+        if (output_mem == B200Z_MEM_HOST) {   // the group's frames, d_out[0, total - origin), to the archive at origin
+            uint64_t total = 0;
+            CU(c, cudaMemcpyAsync(&total, d_total, 8, cudaMemcpyDeviceToHost, s));
+            CU(c, cudaStreamSynchronize(s));
+            CU(c, cudaMemcpy(output + origin, r.output.p, total - origin, cudaMemcpyDeviceToHost));
+            origin = total;
+        }
+    }
+    if (int le = launch_seek_table(r.seek_entries.as<uint8_t>(), nframes, a.checksum, d_total, origin,
+                                   output_mem == B200Z_MEM_HOST ? r.output.as<uint8_t>() : output, s, &c->launches))
+        return c->set_cuda_err((cudaError_t)le, "k_cseek");
+    uint64_t total = 0;
+    CU(c, cudaMemcpyAsync(&total, d_total, 8, cudaMemcpyDeviceToHost, s));
+    CU(c, cudaStreamSynchronize(s));
+    if (output_mem == B200Z_MEM_HOST) CU(c, cudaMemcpy(output + total, r.output.p, table, cudaMemcpyDeviceToHost));
+    *written = total + table;
+    return 0;
+}
+
+// The table of an archive, parsed and checked: the footer (the archive's last 9 bytes) first, then the table frame in front of it
+namespace {
+struct SeekTable {
+    uint64_t n = 0, len = 0;          // frames, archive bytes
+    bool checksum = false;
+    std::vector<uint64_t> coff, doff;   // n + 1 prefix sums of Compressed_Size / Decompressed_Size
+    std::vector<uint32_t> csum;
+};
+}  // namespace
+
+static int seek_fail(std::string *why, const char *rule) {
+    if (why) *why = std::string("seek table: ") + rule;
+    return B200Z_ERR_SEEKABLE_TABLE;
+}
+// the footer: n, the checksum flag, and the size of the table frame (checked to lie inside the archive)
+static int seek_footer(const uint8_t *ft, uint64_t len, SeekTable &t, uint64_t *table_bytes, std::string *why) {
+    if (len < SEEK_TABLE_FIXED) return seek_fail(why, "the archive is shorter than a seek table (17 bytes)");
+    if (seek_le32(ft + 5) != SEEK_FOOTER_MAGIC) return seek_fail(why, "Seekable_Magic_Number is not 0x8F92EAB1");
+    if (ft[4] & 0x7c) return seek_fail(why, "Seek_Table_Descriptor's reserved bits (6-2) are not 0");
+    t.len = len; t.n = seek_le32(ft); t.checksum = (ft[4] & 0x80) != 0;
+    *table_bytes = seek_table_size(t.n, t.checksum);
+    if (*table_bytes > len) return seek_fail(why, "Number_Of_Frames gives a table larger than the archive");
+    return 0;
+}
+// the table frame (table_bytes of it, the footer included): its header and the entries, whose Compressed_Size must add up to its offset
+static int seek_entries(const uint8_t *p, SeekTable &t, std::string *why) {
+    const uint64_t esz = t.checksum ? 12 : 8, tb = seek_table_size(t.n, t.checksum);
+    if (seek_le32(p) != SEEK_SKIPPABLE_MAGIC) return seek_fail(why, "the table frame's Skippable_Magic_Number is not 0x184D2A5E");
+    if (seek_le32(p + 4) != t.n * esz + SEEK_FOOTER) return seek_fail(why, "Frame_Size is not Number_Of_Frames * (8 or 12) + 9");
+    t.coff.assign(t.n + 1, 0); t.doff.assign(t.n + 1, 0); t.csum.assign(t.checksum ? t.n : 0, 0);
+    for (uint64_t i = 0; i < t.n; i++) {
+        const uint8_t *e = p + 8 + i * esz;
+        t.coff[i + 1] = t.coff[i] + seek_le32(e);
+        t.doff[i + 1] = t.doff[i] + seek_le32(e + 4);
+        if (t.checksum) t.csum[i] = seek_le32(e + 8);
+    }
+    if (t.coff[t.n] != t.len - tb) return seek_fail(why, "the frames' Compressed_Size do not add up to the table frame's offset");
+    return 0;
+}
+static int seek_parse_host(const uint8_t *archive, uint64_t len, SeekTable &t, std::string *why) {
+    uint64_t tb = 0;
+    if (int e = seek_footer(len >= SEEK_FOOTER ? archive + len - SEEK_FOOTER : archive, len, t, &tb, why)) return e;
+    return seek_entries(archive + len - tb, t, why);
+}
+
+// The read plan.  Every range is checked first (content and output reach, overlapping output slots); then the frames a range wholly
+// contains are decoded in place for the first such range, the other touched frames into scratch, and each range's remaining bytes
+// become copy pieces.  `touched[r]`: the frames range r touches, ascending.
+namespace {
+struct SeekPlan {
+    std::vector<b200z_seek_plan_frame> frames;
+    std::vector<b200z_seek_plan_piece> pieces;
+    std::vector<std::vector<uint64_t>> touched;
+    uint64_t scratch = 0;
+};
+}  // namespace
+
+static int seek_plan(const SeekTable &t, const b200z_range *ranges, size_t n, uint64_t output_cap, SeekPlan &p, std::string *why) {
+    const uint64_t content = t.doff[t.n];
+    std::vector<std::pair<uint64_t, uint64_t>> slots;
+    for (size_t r = 0; r < n; r++) {
+        const b200z_range &g = ranges[r];
+        if (g.offset > content || g.length > content - g.offset || g.out_off > output_cap || g.length > output_cap - g.out_off) {
+            if (why) *why = "range " + std::to_string(r) + " reaches past the content size or the output";
+            return B200Z_ERR_INVALID_ARGUMENT;
+        }
+        if (g.length) slots.push_back({g.out_off, g.length});
+    }
+    std::sort(slots.begin(), slots.end());
+    for (size_t i = 1; i < slots.size(); i++)
+        if (slots[i - 1].first + slots[i - 1].second > slots[i].first) {
+            if (why) *why = "ranges overlap in the output";
+            return B200Z_ERR_INVALID_ARGUMENT;
+        }
+    p.frames.clear(); p.pieces.clear(); p.scratch = 0;
+    p.touched.assign(n, {});
+    std::map<uint64_t, int64_t> in_place;   // touched frame -> the range it is decoded in place for, or -1
+    for (size_t r = 0; r < n; r++) {
+        const uint64_t lo = ranges[r].offset, hi = lo + ranges[r].length;
+        if (lo == hi) continue;
+        // the first frame holding byte lo: the last one starting at or before it (frames of 0 bytes start where the next one does)
+        uint64_t f = (uint64_t)(std::upper_bound(t.doff.begin(), t.doff.end(), lo) - t.doff.begin()) - 1;
+        for (; f < t.n && t.doff[f] < hi; f++) {
+            if (t.doff[f + 1] == t.doff[f]) continue;
+            p.touched[r].push_back(f);
+            const bool whole = t.doff[f] >= lo && t.doff[f + 1] <= hi;
+            auto it = in_place.find(f);
+            if (it == in_place.end()) in_place[f] = whole ? (int64_t)r : -1;
+            else if (whole && it->second < 0) it->second = (int64_t)r;
+        }
+    }
+    std::map<uint64_t, uint64_t> at;   // frame -> where its plaintext starts (output or scratch)
+    for (const auto &kv : in_place) {
+        const uint64_t f = kv.first;
+        uint64_t dst;
+        if (kv.second >= 0) {
+            const b200z_range &g = ranges[kv.second];
+            dst = g.out_off + (t.doff[f] - g.offset);
+        } else {
+            dst = p.scratch;
+            p.scratch = (p.scratch + (t.doff[f + 1] - t.doff[f]) + 15) & ~15ull;
+        }
+        at[f] = dst;
+        p.frames.push_back(b200z_seek_plan_frame{f, dst, kv.second});
+    }
+    for (size_t r = 0; r < n; r++) {
+        const b200z_range &g = ranges[r];
+        for (uint64_t f : p.touched[r]) {
+            const int64_t owner = in_place[f];
+            if (owner == (int64_t)r) continue;
+            const uint64_t lo = std::max(g.offset, t.doff[f]), hi = std::min(g.offset + g.length, t.doff[f + 1]);
+            p.pieces.push_back(b200z_seek_plan_piece{g.out_off + (lo - g.offset), at[f] + (lo - t.doff[f]), hi - lo, owner < 0 ? 1u : 0u, (uint32_t)r});
+        }
+    }
+    return 0;
+}
+
+extern "C" int b200z_debug_seekable_plan(const uint8_t *archive, size_t len, const b200z_range *ranges, size_t n, b200z_seek_plan_frame *frames,
+                                         size_t frames_cap, size_t *nframes, b200z_seek_plan_piece *pieces, size_t pieces_cap, size_t *npieces,
+                                         uint64_t *scratch_bytes) {
+    if ((!archive && len) || (!ranges && n) || !nframes || !npieces || !scratch_bytes) return B200Z_ERR_INVALID_ARGUMENT;
+    SeekTable t;
+    if (int e = seek_parse_host(archive, len, t, nullptr)) return e;
+    SeekPlan p;
+    if (int e = seek_plan(t, ranges, n, UINT64_MAX, p, nullptr)) return e;
+    *nframes = p.frames.size(); *npieces = p.pieces.size(); *scratch_bytes = p.scratch;
+    if (p.frames.size() > frames_cap || p.pieces.size() > pieces_cap) return B200Z_ERR_INVALID_ARGUMENT;
+    if (!p.frames.empty()) memcpy(frames, p.frames.data(), p.frames.size() * sizeof(b200z_seek_plan_frame));
+    if (!p.pieces.empty()) memcpy(pieces, p.pieces.data(), p.pieces.size() * sizeof(b200z_seek_plan_piece));
+    return 0;
+}
+
+struct b200z_seekable {
+    b200z_ctx *ctx = nullptr;
+    const uint8_t *archive = nullptr;   // borrowed
+    int mem = B200Z_MEM_HOST;
+    SeekTable t;
+};
+
+extern "C" int b200z_seekable_open(b200z_ctx *c, const uint8_t *archive, size_t len, int mem, b200z_seekable **out) {
+    if (!c || !out || (!archive && len) || (mem != B200Z_MEM_HOST && mem != B200Z_MEM_DEVICE)) return B200Z_ERR_INVALID_ARGUMENT;
+    *out = nullptr;
+    std::unique_ptr<b200z_seekable> s(new b200z_seekable());
+    s->ctx = c; s->archive = archive; s->mem = mem;
+    if (mem == B200Z_MEM_HOST) {
+        if (int e = seek_parse_host(archive, len, s->t, &c->err)) return e;
+    } else {   // only the footer, then the table frame, cross to the host
+        if (int e = c->use()) return e;
+        uint8_t ft[SEEK_FOOTER] = {};
+        if (len >= SEEK_FOOTER) CU(c, cudaMemcpy(ft, archive + len - SEEK_FOOTER, SEEK_FOOTER, cudaMemcpyDeviceToHost));
+        uint64_t tb = 0;
+        if (int e = seek_footer(ft, len, s->t, &tb, &c->err)) return e;
+        std::vector<uint8_t> tab(tb);
+        CU(c, cudaMemcpy(tab.data(), archive + len - tb, tb, cudaMemcpyDeviceToHost));
+        if (int e = seek_entries(tab.data(), s->t, &c->err)) return e;
+    }
+    *out = s.release();
+    return 0;
+}
+extern "C" uint64_t b200z_seekable_num_frames(const b200z_seekable *s) { return s ? s->t.n : 0; }
+extern "C" uint64_t b200z_seekable_content_size(const b200z_seekable *s) { return s ? s->t.doff[s->t.n] : 0; }
+extern "C" int b200z_seekable_frame(const b200z_seekable *s, uint64_t i, b200z_seek_frame *out) {
+    if (!s || !out || i >= s->t.n) return B200Z_ERR_INVALID_ARGUMENT;
+    const SeekTable &t = s->t;
+    *out = b200z_seek_frame{t.coff[i], t.coff[i + 1] - t.coff[i], t.doff[i], t.doff[i + 1] - t.doff[i], t.checksum ? 1u : 0u, t.checksum ? t.csum[i] : 0u};
+    return 0;
+}
+extern "C" void b200z_seekable_close(b200z_seekable *s) { delete s; }
+
+extern "C" int b200z_seekable_read_ranges(b200z_seekable *s, const b200z_range *ranges, size_t n, const b200z_dict *const *dicts, size_t ndicts,
+                                          const b200z_dict *forced_dict, uint64_t max_window_size, uint8_t *output, size_t output_cap, int output_mem,
+                                          b200z_range_result *results) {
+    if (!s || (!ranges && n) || (n && !results) || (!dicts && ndicts) || (output_cap && !output) ||
+        (output_mem != B200Z_MEM_HOST && output_mem != B200Z_MEM_DEVICE))
+        return B200Z_ERR_INVALID_ARGUMENT;
+    b200z_ctx *c = s->ctx;
+    const SeekTable &t = s->t;
+    SeekPlan p;
+    if (int e = seek_plan(t, ranges, n, output_cap, p, &c->err)) return e;
+    for (size_t r = 0; r < n; r++) results[r] = b200z_range_result{0, 0, -1, (uint64_t)p.touched[r].size(), 0};
+    if (p.frames.empty()) return 0;
+    if (int e = c->use()) return e;
+    CompressResources *rp = nullptr;
+    if (int e = compress_get(c, &rp)) return e;
+    CompressResources &res = *rp;
+    cudaStream_t st = c->stream;
+    // Host output: the slots are staged on the device packed in call order, so the plan runs on ranges whose out_off is the packed
+    // one; the scratch follows them.  Device output: the scratch is a buffer of its own.
+    const bool host_out = output_mem == B200Z_MEM_HOST;
+    std::vector<b200z_range> packed;
+    uint64_t staged = 0;
+    if (host_out) {
+        packed.assign(ranges, ranges + n);
+        for (b200z_range &g : packed) { g.out_off = staged; staged += g.length; }
+        staged = (staged + 15) & ~15ull;
+        if (int e = seek_plan(t, packed.data(), n, UINT64_MAX, p, &c->err)) return e;
+    }
+    if (int e = res.rd_stage.ensure(staged + p.scratch + 16)) return e;
+    uint8_t *scratch = res.rd_stage.as<uint8_t>() + staged;
+    uint8_t *out_dev = host_out ? res.rd_stage.as<uint8_t>() : output;
+    // The batch writes every frame at base + out_off.  Slots and scratch may be two allocations: base is the lower of the two and
+    // out_off a distance in the one (unified) device address space; each frame writes only [out_off, out_off + its size).
+    const uint64_t out_end = host_out ? staged : output_cap;
+    uint8_t *base = std::min(out_dev, scratch);
+    const uint64_t o_out = (uint64_t)(out_dev - base), o_scr = (uint64_t)(scratch - base);
+    const uint64_t span = std::max(o_out + out_end, o_scr + p.scratch + 16);
+    // the touched frames as b200z_frame_io: host archives gather their bytes, device archives are read where they lie
+    std::vector<b200z_frame_io> io(p.frames.size());
+    uint64_t gathered = 0;
+    for (size_t i = 0; i < p.frames.size(); i++) {
+        const uint64_t f = p.frames[i].frame, cs = t.coff[f + 1] - t.coff[f], ds = t.doff[f + 1] - t.doff[f];
+        io[i].src_off = s->mem == B200Z_MEM_HOST ? gathered : t.coff[f];
+        io[i].src_size = cs;
+        io[i].out_off = (p.frames[i].range >= 0 ? o_out : o_scr) + p.frames[i].dst_off;
+        io[i].out_cap = ds;
+        gathered += cs;
+    }
+    const uint8_t *src = s->archive;
+    size_t src_len = t.len;
+    // the pinned buffer holds a host archive's gathered frames, then host output's staged slots: sized for both uses it has
+    const bool host_arch = s->mem == B200Z_MEM_HOST;
+    if (host_arch || host_out)
+        if (int e = res.rd_host.ensure(std::max<uint64_t>(host_arch ? gathered : 0, staged) + 16)) return e;
+    if (host_arch) {
+        uint8_t *h = res.rd_host.as<uint8_t>();
+        for (size_t i = 0; i < p.frames.size(); i++) memcpy(h + io[i].src_off, s->archive + t.coff[p.frames[i].frame], io[i].src_size);
+        src = h; src_len = gathered;
+    }
+    b200z_batch *bp = nullptr;
+    if (int e = b200z_batch_prepare(c, src, src_len, s->mem, io.data(), io.size(), dicts, ndicts, forced_dict, max_window_size, &bp)) return e;
+    std::unique_ptr<b200z_batch, void (*)(b200z_batch *)> b(bp, b200z_batch_destroy);
+    if (int e = b200z_batch_run(b.get(), base, span)) return e;
+    // the copy pieces, cut to GATHER_CHUNK bytes each
+    std::vector<GatherPiece> gp;
+    for (const b200z_seek_plan_piece &q : p.pieces) {
+        const uint64_t so = (q.from_scratch ? o_scr : o_out) + q.src_off, d = o_out + q.dst_off;
+        for (uint64_t k = 0; k < q.len; k += GATHER_CHUNK)
+            gp.push_back(GatherPiece{so + k, d + k, (uint32_t)std::min<uint64_t>(GATHER_CHUNK, q.len - k), 0});
+    }
+    if (!gp.empty()) {
+        if (int e = res.rd_pieces.ensure(gp.size() * sizeof(GatherPiece))) return e;
+        CU(c, cudaMemcpyAsync(res.rd_pieces.p, gp.data(), gp.size() * sizeof(GatherPiece), cudaMemcpyHostToDevice, st));
+        if (int le = launch_range_gather(res.rd_pieces.as<GatherPiece>(), (uint32_t)gp.size(), base, st, &c->launches))
+            return c->set_cuda_err((cudaError_t)le, "k_range_gather");
+    }
+    std::vector<b200z_frame_result> fr(io.size());
+    if (int e = b200z_batch_finish(b.get(), fr.data())) return e;   // synchronises (and keeps `gp` alive until the copy is done)
+    if (host_out) {
+        uint8_t *h = res.rd_host.as<uint8_t>();
+        CU(c, cudaMemcpy(h, res.rd_stage.p, staged, cudaMemcpyDeviceToHost));
+        for (size_t r = 0; r < n; r++) memcpy(output + ranges[r].out_off, h + packed[r].out_off, ranges[r].length);
+    }
+    // per range: the first failing frame in content order, and the checksum comparisons
+    std::map<uint64_t, size_t> idx;
+    for (size_t i = 0; i < p.frames.size(); i++) idx[p.frames[i].frame] = i;
+    const bool sums = (c->flags & B200Z_FLAG_CHECKSUM) != 0;
+    for (size_t r = 0; r < n; r++) {
+        b200z_range_result &rr = results[r];
+        for (uint64_t f : p.touched[r]) {
+            const b200z_frame_result &x = fr[idx[f]];
+            const uint64_t ds = t.doff[f + 1] - t.doff[f];
+            if (rr.status == 0 && (x.status || x.out_size != ds)) {
+                const bool size = x.status == 0 || x.status == B200Z_ERR_TARGET_TOO_SMALL;   // out_cap is the entry's size
+                rr.status = size ? B200Z_ERR_SEEKABLE_FRAME_SIZE : x.status;
+                rr.stage = size ? B200Z_STAGE_NONE : x.stage;
+                rr.error_frame = (int64_t)f;
+            }
+            if (sums && x.status == 0 && x.has_calculated_checksum &&
+                ((t.checksum && x.calculated_checksum != t.csum[f]) || (x.has_checksum && x.calculated_checksum != x.checksum_from_data)))
+                rr.checksum_mismatches++;
+        }
+    }
     return 0;
 }
 

@@ -75,4 +75,26 @@ int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s, uint
 // which all belong to a.frames[0] (the chunk); no dictionary, no checksum kernel.  Adds the kernels it enqueued to *launched
 int launch_compress_chunk(const CompressArgs &a, cudaStream_t s, uint64_t *launched);
 
+// ---- seekable archives (seekable.cu; EXTENSION, the zstd seekable format)
+constexpr uint32_t SEEK_SKIPPABLE_MAGIC = 0x184D2A5Eu;
+constexpr uint32_t SEEK_FOOTER_MAGIC = 0x8F92EAB1u;
+constexpr uint32_t SEEK_FOOTER = 9;                 // Number_Of_Frames, Seek_Table_Descriptor, Seekable_Magic_Number
+constexpr uint32_t SEEK_TABLE_FIXED = 8 + SEEK_FOOTER;   // the skippable frame's header and the footer
+// k_cscan over a.blocks[a.nblocks] (a group of whole frames, after k_cenc and k_cxxh64): every a.frames[f].dst_off becomes the
+// frame's packed archive offset less `origin`, *total (device) moves past the group, and frame f's table entry goes to
+// entries[(first_frame + f) * (a.checksum ? 12 : 8)].  Adds the kernels it enqueued to *launched
+int launch_seek_scan(const CompressArgs &a, uint64_t *total, uint64_t origin, uint8_t *entries, uint64_t first_frame, cudaStream_t s,
+                     uint64_t *launched);
+// k_cseek: the table frame of the n entries at output + (*total - origin)
+int launch_seek_table(const uint8_t *entries, uint64_t n, int checksum, const uint64_t *total, uint64_t origin, uint8_t *output, cudaStream_t s,
+                      uint64_t *launched);
+// one copy piece of the read plan: len <= GATHER_CHUNK bytes from base + src to base + dst
+struct GatherPiece {
+    uint64_t src, dst;
+    uint32_t len, pad;
+};
+constexpr uint32_t GATHER_CHUNK = 65536;
+// k_range_gather: one CTA per piece
+int launch_range_gather(const GatherPiece *pieces, uint32_t n, uint8_t *base, cudaStream_t s, uint64_t *launched);
+
 }  // namespace b200z
