@@ -134,7 +134,10 @@ typedef enum b200z_error {
     /* EXTENSION, seekable archives (b200z_seekable_*): the seek table breaks one of the format's rules (the message names it) */
     B200Z_ERR_SEEKABLE_TABLE = 240,
     /* EXTENSION, seekable archives: a frame decoded to a size other than its seek-table entry's Decompressed_Size */
-    B200Z_ERR_SEEKABLE_FRAME_SIZE = 241
+    B200Z_ERR_SEEKABLE_FRAME_SIZE = 241,
+    /* EXTENSION, seekable archives from and to callbacks: a read, positional read or write callback failed or came up short (the
+     * message names the callback and the archive offset) */
+    B200Z_ERR_SEEKABLE_IO = 242
 } b200z_error;
 
 /* stage that raised the error == nesting path of the reference's FrameDecoderError (errors.rs:472-486) */
@@ -172,6 +175,10 @@ void b200z_ctx_set_flags(b200z_ctx *ctx, uint32_t flags);
 uint32_t b200z_ctx_flags(const b200z_ctx *ctx);
 /* number of this library's kernel launches since ctx creation (bench.py's gpu_launches) */
 uint64_t b200z_ctx_kernel_launches(const b200z_ctx *ctx);
+/* Bytes of device memory and of pinned host memory the library holds right now, over every context and handle of the process:
+ * exactly what its allocations asked for (each cudaMalloc / cudaMallocHost it made and has not freed), not the driver's rounding.
+ * For tests of what a call keeps, which a card-wide reading cannot isolate on a shared device. */
+void b200z_debug_held_bytes(uint64_t *device, uint64_t *pinned);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Dictionaries (device resident).  Replaces Dictionary::decode_dict (decoding/dictionary.rs:45-126) +
@@ -725,6 +732,47 @@ size_t b200z_seekable_bound(size_t src_size, size_t frame_size, int checksum, co
 int b200z_compress_seekable(b200z_ctx *ctx, const uint8_t *input, size_t input_len, int input_mem, size_t frame_size, int level,
                             int checksum, const b200z_dict *dict, uint8_t *output, size_t output_cap, int output_mem, size_t *written);
 
+/* A seekable archive from a reader to a writer, for sources too large to hold.
+ *   Output:  write_cb receives exactly what b200z_compress_seekable writes for the whole source with the same frame_size, level,
+ *            checksum, dictionary and B200Z_FLAG_DICT_TABLES, whatever the chunk size and however the source splits its reads: a
+ *            frame's bytes depend on its piece and the dictionary only, and the table is written by one k_cseek at the end.
+ *   Source:  read_cb as the stream compressor reads it: a frame is cut after frame_size bytes or where a read returns 0 (the end of
+ *            the source, so only the last frame is shorter); an empty source gives the table alone.
+ *   Groups:  with C = B200Z_PIPELINE_CHUNK_BYTES (read by each call; 64 MiB by default) a group is the most whole frames that hold
+ *            at most C bytes and at most B200Z_SEEKABLE_GROUP_BLOCKS blocks, or one frame when a frame alone is larger: G =
+ *            max(1, min(C / frame_size, B200Z_SEEKABLE_GROUP_BLOCKS / blocks per frame)) * frame_size <= max(C, frame_size) bytes.
+ *            Two slots: while group k compresses on the ctx stream, the calling thread reads group k + 1 and writes group k - 1;
+ *            uploads go on one copy stream and downloads on another.  Each group's frames are packed from its slot's byte 0 by
+ *            k_cscan behind a running-size word of the slot's own; the host learns the packed size from that word's download.
+ *   Kernels: per group, those of a b200z_compress_seekable group (k_cmatch, k_cenc, k_cxxh64 with `checksum`, k_cscan,
+ *            k_cassemble; none of the first two at Uncompressed); then one k_cseek; all counted in b200z_ctx_kernel_launches.
+ *   Memory:  kept by the context and sized by the first group, the largest one the source has.  Device: per slot G input, the
+ *            bounds of G's frames (b200z_compress_bound_dict each) and 32 bytes per frame and 24 per block of descriptors; shared,
+ *            the compressor's staging of about 0.9 MB per block of G.  Pinned host: per slot G input and the bounds of G's frames.
+ *            What grows with the source is the seek table.  With E = 8 bytes per frame (12 with `checksum`): the entries on the
+ *            device, in an array doubled when full, so at most 2 * E per frame after the call; during it the outgrown arrays are
+ *            kept until it ends (freeing one earlier would wait for the whole device), so at most 4 * E per frame, each array its
+ *            own allocation.  At the end the table frame (17 bytes + E per frame) is written on the device, into a buffer the
+ *            context keeps (up to 1.5 times that size, as the compressor's output staging grows), and copied to pageable host
+ *            memory of its size while it is written.  Each group's download takes its frames' bounds (about the group's input),
+ *            not only their packed bytes, so that no host wait stands between the packed size and the bytes.
+ *   Checks:  before any read, write or launch, as b200z_compress_seekable checks them: B200Z_ERR_REFERENCE_WOULD_PANIC for levels
+ *            2-4; B200Z_ERR_INVALID_ARGUMENT for other unknown levels, a dictionary of another context, no callback, and frame_size
+ *            0 or above B200Z_SEEKABLE_MAX_FRAME_SIZE.  A source that gives more than 2^32 - 1 frames fails with
+ *            B200Z_ERR_INVALID_ARGUMENT when it gets there.
+ *   Errors:  a read returning < 0 or more than asked for, or a write returning <= 0, is B200Z_ERR_SEEKABLE_IO, with a message
+ *            naming the callback and the archive offset.  Bytes already written stay written, nothing is left in flight, and the
+ *            context stays usable.  `result` (may be NULL) says what was read and written either way. */
+typedef struct b200z_seekable_stream_result {
+    uint64_t read;      /* plaintext bytes taken from the source             */
+    uint64_t written;   /* archive bytes handed to write_cb (table included) */
+    uint64_t frames;    /* frames in the archive                             */
+    uint64_t groups;    /* GPU submissions the call ran                      */
+} b200z_seekable_stream_result;
+int b200z_compress_seekable_stream(b200z_ctx *ctx, b200z_read_fn read_cb, void *read_user, b200z_write_fn write_cb, void *write_user,
+                                   size_t frame_size, int level, int checksum, const b200z_dict *dict,
+                                   b200z_seekable_stream_result *result);
+
 /* An open archive: its table, parsed and checked.  It borrows the archive (host or device memory), which the caller keeps alive and
  * unchanged until b200z_seekable_close; of a device archive only the table is copied to the host.  B200Z_ERR_SEEKABLE_TABLE, with
  * the rule in b200z_ctx_last_error_message, when the footer magic, the reserved bits, the skippable magic or Frame_Size is wrong,
@@ -737,6 +785,20 @@ typedef struct b200z_seek_frame {
     uint32_t checksum;
 } b200z_seek_frame;
 int b200z_seekable_open(b200z_ctx *ctx, const uint8_t *archive, size_t len, int mem, b200z_seekable **out);
+/* pread semantics: up to len bytes of the archive at offset into buf; returns the bytes read (0 at the end), < 0 on error */
+typedef long (*b200z_read_at_fn)(void *user, uint64_t offset, uint8_t *buf, size_t len);
+/* An archive of `len` bytes behind a positional-read callback (a file too large to hold, for instance).  Open reads the archive's
+ * last 9 bytes (the footer), the table frame's 8-byte header (checked against the footer before anything of the table's size is
+ * allocated or read) and then the table frame, nothing else, and checks them as b200z_seekable_open does, with the same
+ * B200Z_ERR_SEEKABLE_TABLE messages; B200Z_ERR_OUT_OF_MEMORY when a well-formed table does not fit in host memory.  read_at and `user` must stay valid until b200z_seekable_close.  The handle works with
+ * _num_frames, _content_size, _frame and b200z_seekable_read_ranges as a host archive's does: the same plan, one batch submission,
+ * k_range_gather and launch counts, and the same results.  The only difference is where the touched frames' bytes come from: each
+ * run of touched frames adjacent in the archive is fetched by one read_at call (partial reads are retried until a read returns 0)
+ * into the pinned buffer a host archive's frames are gathered to.  A call holds what a host-archive call holds (the touched
+ * frames' compressed bytes in pinned memory, the slots and the scratch), never the archive.  A read_at that fails (< 0, or more
+ * than asked for) or comes up short is B200Z_ERR_SEEKABLE_IO, at open or before any launch of read_ranges; the handle stays
+ * usable. */
+int b200z_seekable_open_source(b200z_ctx *ctx, b200z_read_at_fn read_at, void *user, uint64_t len, b200z_seekable **out);
 uint64_t b200z_seekable_num_frames(const b200z_seekable *s);
 uint64_t b200z_seekable_content_size(const b200z_seekable *s);
 int b200z_seekable_frame(const b200z_seekable *s, uint64_t i, b200z_seek_frame *out);

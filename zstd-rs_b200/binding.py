@@ -20,12 +20,13 @@ _HEADER = os.path.join(_HERE, "..", "include", "b200zstd.h")
 
 READ_FN = C.CFUNCTYPE(C.c_long, C.c_void_p, C.POINTER(C.c_uint8), C.c_size_t)
 WRITE_FN = C.CFUNCTYPE(C.c_long, C.c_void_p, C.POINTER(C.c_uint8), C.c_size_t)
+READ_AT_FN = C.CFUNCTYPE(C.c_long, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint8), C.c_size_t)
 
 ALL, UPTO_BLOCKS, UPTO_BYTES = 0, 1, 2
 MEM_HOST, MEM_DEVICE = 0, 1
 ERR_SKIP_FRAME = 8
 ERR_INVALID_ARGUMENT = 220
-ERR_SEEKABLE_TABLE, ERR_SEEKABLE_FRAME_SIZE = 240, 241   # EXTENSION: seekable archives
+ERR_SEEKABLE_TABLE, ERR_SEEKABLE_FRAME_SIZE, ERR_SEEKABLE_IO = 240, 241, 242   # EXTENSION: seekable archives
 FLAG_CHECKSUM = 1
 FLAG_PROFILE = 2
 FLAG_DICT_TABLES = 4
@@ -98,6 +99,7 @@ def lib():
         "b200z_ctx_last_error_message": (C.c_char_p, [vp]),
         "b200z_ctx_stream": (vp, [vp]),
         "b200z_ctx_kernel_launches": (C.c_uint64, [vp]),
+        "b200z_debug_held_bytes": (None, [C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
         "b200z_ctx_set_flags": (None, [vp, C.c_uint32]),
         "b200z_ctx_flags": (C.c_uint32, [vp]),
         "b200z_dict_create": (C.c_int, [vp, vp, sz, pp]),
@@ -180,7 +182,9 @@ def lib():
         "b200z_debug_dict_from_counts": (C.c_int, [vp, vp, sz, C.c_uint32, vp, sz, C.POINTER(sz)]),
         "b200z_seekable_bound": (sz, [sz, sz, C.c_int, vp]),
         "b200z_compress_seekable": (C.c_int, [vp, vp, sz, C.c_int, sz, C.c_int, C.c_int, vp, vp, sz, C.c_int, C.POINTER(sz)]),
+        "b200z_compress_seekable_stream": (C.c_int, [vp, READ_FN, vp, WRITE_FN, vp, sz, C.c_int, C.c_int, vp, vp]),
         "b200z_seekable_open": (C.c_int, [vp, vp, sz, C.c_int, pp]),
+        "b200z_seekable_open_source": (C.c_int, [vp, READ_AT_FN, vp, C.c_uint64, pp]),
         "b200z_seekable_num_frames": (C.c_uint64, [vp]),
         "b200z_seekable_content_size": (C.c_uint64, [vp]),
         "b200z_seekable_frame": (C.c_int, [vp, C.c_uint64, vp]),
@@ -214,6 +218,13 @@ class B200ZError(Exception):
     def __init__(self, code, stage=0, msg=""):
         self.code, self.stage = code, stage
         super().__init__(f"{lib().b200z_error_name(code).decode()} (stage {stage}) {msg}")
+
+
+def held_bytes():
+    """b200z_debug_held_bytes: (device bytes, pinned host bytes) the library's allocations hold now, over the whole process."""
+    d, p = C.c_uint64(), C.c_uint64()
+    lib().b200z_debug_held_bytes(C.byref(d), C.byref(p))
+    return d.value, p.value
 
 
 def xxh64(data):
@@ -634,6 +645,28 @@ def compress_seekable(ctx, input, output=None, frame_size=131072, level=FASTEST,
     return output[:written.value] if _is_device(output) else output[:written.value].tobytes()
 
 
+SEEKABLE_STREAM_RESULT_DTYPE = np.dtype([("read", "<u8"), ("written", "<u8"), ("frames", "<u8"), ("groups", "<u8")])
+
+
+def compress_seekable_stream(ctx, source, drain, frame_size=131072, level=FASTEST, checksum=True, dict=None, dict_tables=False):
+    """b200z_compress_seekable_stream: the archive compress_seekable writes for everything `source` holds, from the source to `drain`
+    in groups of whole frames (B200Z_PIPELINE_CHUNK_BYTES each), in bounded memory.  Sources and drains as FrameCompressor takes them.
+    Returns the SEEKABLE_STREAM_RESULT_DTYPE row (read, written, frames, groups).  A source or drain that fails raises
+    B200ZError(ERR_SEEKABLE_IO), from the exception it raised."""
+    rd, wr, failure = _source_drain_callbacks(source, drain)
+    res = np.zeros(1, dtype=SEEKABLE_STREAM_RESULT_DTYPE)
+    flags = ctx.L.b200z_ctx_flags(ctx.h)
+    if dict_tables:
+        ctx.L.b200z_ctx_set_flags(ctx.h, flags | FLAG_DICT_TABLES)
+    try:
+        e = ctx.L.b200z_compress_seekable_stream(ctx.h, rd, None, wr, None, frame_size, level, 1 if checksum else 0,
+                                                 dict.h if dict is not None else None, res.ctypes.data)
+    finally:
+        ctx.L.b200z_ctx_set_flags(ctx.h, flags)
+    _raise_chained(ctx, e, failure)
+    return res[0]
+
+
 def _ranges_array(ranges):
     if isinstance(ranges, np.ndarray) and ranges.dtype == RANGE_DTYPE:
         return np.ascontiguousarray(ranges)
@@ -648,11 +681,60 @@ class SeekableArchive:
     def __init__(self, ctx, archive):
         self.ctx = ctx
         self.h = None
+        self._file = None
+        self._failure = []
         ap, al, self._k = _ptr(archive)
         self._archive = archive
         h = C.c_void_p()
         ctx._chk(ctx.L.b200z_seekable_open(ctx.h, ap, al, MEM_DEVICE if _is_device(archive) else MEM_HOST, C.byref(h)))
         self.h = h
+
+    @classmethod
+    def from_source(cls, ctx, f, length=None):
+        """An archive behind a positional-read callback (b200z_seekable_open_source): `f` is a path or a binary file object, read with
+        os.pread on its descriptor when it has one, else with seek() and read().  length: the archive's size, by default the file's.
+        Only the footer and the table are read here, and only the touched frames by read_ranges.  A failed or short read raises
+        B200ZError(ERR_SEEKABLE_IO), from the exception the file raised if any."""
+        self = cls.__new__(cls)
+        self.ctx, self.h, self._k, self._archive, self._failure = ctx, None, None, None, []
+        self._file = open(f, "rb") if isinstance(f, (str, os.PathLike)) else None
+        src = self._file if self._file is not None else f
+        try:
+            fd = src.fileno()
+        except (AttributeError, OSError, io.UnsupportedOperation):
+            fd = None
+        if length is None:
+            length = os.fstat(fd).st_size if fd is not None else src.seek(0, io.SEEK_END)
+
+        def _read_at(_user, offset, buf, n):
+            try:
+                if fd is not None:
+                    b = os.pread(fd, n, offset)
+                else:
+                    src.seek(offset)
+                    b = src.read(n)
+                if b:
+                    C.memmove(buf, b, len(b))
+                return len(b)
+            except Exception as e:
+                failure.append(e)
+                return -1
+
+        failure = self._failure
+        self._read_at = READ_AT_FN(_read_at)
+        h = C.c_void_p()
+        try:
+            self._chk(ctx.L.b200z_seekable_open_source(ctx.h, self._read_at, None, length, C.byref(h)))
+        except BaseException:
+            self.close()
+            raise
+        self.h = h
+        return self
+
+    def _chk(self, e):
+        failure = list(self._failure)
+        self._failure.clear()
+        _raise_chained(self.ctx, e, failure)
 
     @property
     def num_frames(self):
@@ -676,8 +758,8 @@ class SeekableArchive:
         res = np.zeros(len(rg), dtype=RANGE_RESULT_DTYPE)
         op, ol, _k = _ptr(output)
         darr, nd, forced = _dict_args(dicts, forced_dict)
-        self.ctx._chk(self.ctx.L.b200z_seekable_read_ranges(self.h, rg.ctypes.data, len(rg), darr, nd, forced, max_window_size, op, ol,
-                                                            MEM_DEVICE if _is_device(output) else MEM_HOST, res.ctypes.data))
+        self._chk(self.ctx.L.b200z_seekable_read_ranges(self.h, rg.ctypes.data, len(rg), darr, nd, forced, max_window_size, op, ol,
+                                                        MEM_DEVICE if _is_device(output) else MEM_HOST, res.ctypes.data))
         return res
 
     def read(self, offset, length, dicts=None, forced_dict=None):
@@ -692,6 +774,9 @@ class SeekableArchive:
         if getattr(self, "h", None) and self.ctx.h:
             self.ctx.L.b200z_seekable_close(self.h)
         self.h = None
+        if getattr(self, "_file", None) is not None:
+            self._file.close()
+            self._file = None
 
     def __enter__(self):
         return self
@@ -781,38 +866,47 @@ class FrameCompressor:
         panic = [k for k, v in error_names().items() if v == "B200Z_ERR_REFERENCE_WOULD_PANIC"][0]
         if self._source is None or self._drain is None:
             raise B200ZError(panic, 0, "FrameCompressor::compress: no source or no drain set")
-        src = _Reader(self._source).src
-        drain = self._drain
-        failure = []
-
-        def _read(_user, buf, n):
-            try:
-                b = src.read(n)
-                if b:
-                    C.memmove(buf, b, len(b))
-                return len(b)
-            except Exception as e:
-                failure.append(e)
-                return -1
-
-        def _write(_user, buf, n):
-            try:
-                if isinstance(drain, bytearray):
-                    drain.extend(C.string_at(buf, n))
-                    return n
-                r = drain.write(C.string_at(buf, n))
-                return n if r is None else r
-            except Exception as e:
-                failure.append(e)
-                return -1
-
-        rd, wr = READ_FN(_read), WRITE_FN(_write)
+        rd, wr, failure = _source_drain_callbacks(self._source, self._drain)
         res = np.zeros(1, dtype=COMPRESS_RESULT_DTYPE)
         e = self.L.b200z_frame_compressor_compress(self.h, rd, None, wr, None, res.ctypes.data)
-        if e:
-            err = B200ZError(e, 0, self.L.b200z_ctx_last_error_message(self.ctx.h).decode())
-            raise err from (failure[0] if failure else None)
+        _raise_chained(self.ctx, e, failure)
         return res[0]
+
+
+def _source_drain_callbacks(source, drain):
+    """(READ_FN, WRITE_FN, failures) over a source (bytes or a file-like with read()) and a drain (a file-like with write(), or a
+    bytearray, which the bytes are appended to).  An exception either raises makes the callback fail; it is kept in `failures`."""
+    src = _Reader(source).src
+    failure = []
+
+    def _read(_user, buf, n):
+        try:
+            b = src.read(n)
+            if b:
+                C.memmove(buf, b, len(b))
+            return len(b)
+        except Exception as e:
+            failure.append(e)
+            return -1
+
+    def _write(_user, buf, n):
+        try:
+            if isinstance(drain, bytearray):
+                drain.extend(C.string_at(buf, n))
+                return n
+            r = drain.write(C.string_at(buf, n))
+            return n if r is None else r
+        except Exception as e:
+            failure.append(e)
+            return -1
+
+    return READ_FN(_read), WRITE_FN(_write), failure
+
+
+def _raise_chained(ctx, e, failure):
+    """Raises B200ZError for a nonzero code, from the first exception a callback raised."""
+    if e:
+        raise B200ZError(e, 0, ctx.L.b200z_ctx_last_error_message(ctx.h).decode()) from (failure[0] if failure else None)
 
 
 def compress(ctx, source, target, level=FASTEST, checksum=True):

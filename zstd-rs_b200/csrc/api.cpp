@@ -7,8 +7,10 @@
 #include <string.h>
 
 #include <algorithm>
+#include <atomic>
 #include <map>
 #include <memory>
+#include <new>
 #include <string>
 #include <vector>
 
@@ -51,9 +53,12 @@ const ErrName kErrNames[] = {
     EN(ERR_SEQ_MISSING_BYTE_FOR_RLE_ML_TABLE), EN(ERR_EXEC_NOT_ENOUGH_BYTES_FOR_SEQUENCE), EN(ERR_EXEC_ZERO_OFFSET),
     EN(ERR_EXEC_NOT_ENOUGH_BYTES_IN_DICTIONARY), EN(ERR_EXEC_OFFSET_TOO_BIG), EN(ERR_DICT_NOT_ENOUGH_BYTES), EN(ERR_DICT_BAD_MAGIC_NUM),
     EN(ERR_REFERENCE_WOULD_PANIC), EN(ERR_BLOCK_OUTPUT_LIMIT), EN(ERR_INVALID_ARGUMENT), EN(ERR_OUT_OF_MEMORY), EN(ERR_NO_DEVICE), EN(ERR_CUDA),
-    EN(ERR_SEEKABLE_TABLE), EN(ERR_SEEKABLE_FRAME_SIZE),
+    EN(ERR_SEEKABLE_TABLE), EN(ERR_SEEKABLE_FRAME_SIZE), EN(ERR_SEEKABLE_IO),
 };
 #undef EN
+
+// bytes held by every Buf of the process: [0] device, [1] pinned host (b200z_debug_held_bytes)
+std::atomic<uint64_t> g_held[2];
 
 // The owners of the library's CUDA resources: each frees what it holds when it is destroyed, so no path, an error path
 // included, frees by hand.  Buf is device memory (DevBuf) or pinned host memory (PinnedBuf).
@@ -65,7 +70,10 @@ template <bool Pinned> struct Buf {
     Buf &operator=(Buf &&o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }
     ~Buf() { release(); }
     void release() {
-        if (p) Pinned ? cudaFreeHost(p) : cudaFree(p);
+        if (p) {
+            Pinned ? cudaFreeHost(p) : cudaFree(p);
+            g_held[Pinned] -= cap;
+        }
         p = nullptr; cap = 0;
     }
     // exactly n bytes in place of what it held; returns CUDA's error, cleared
@@ -74,6 +82,7 @@ template <bool Pinned> struct Buf {
         const cudaError_t e = Pinned ? cudaMallocHost(&p, n) : cudaMalloc(&p, n);
         if (e != cudaSuccess) { p = nullptr; cudaGetLastError(); return e; }
         cap = n;
+        g_held[Pinned] += n;
         return cudaSuccess;
     }
     // at least n bytes, and at least 1.5 times the old capacity with `grow`; contents are NOT preserved
@@ -184,6 +193,10 @@ extern "C" void b200z_ctx_destroy(b200z_ctx *c) {
 extern "C" const char *b200z_ctx_last_error_message(const b200z_ctx *c) { return c ? c->err.c_str() : ""; }
 extern "C" void *b200z_ctx_stream(const b200z_ctx *c) { return c ? (void *)c->stream.s : nullptr; }
 extern "C" uint64_t b200z_ctx_kernel_launches(const b200z_ctx *c) { return c ? c->launches : 0; }
+extern "C" void b200z_debug_held_bytes(uint64_t *device, uint64_t *pinned) {
+    if (device) *device = g_held[0];
+    if (pinned) *pinned = g_held[1];
+}
 extern "C" void b200z_ctx_set_flags(b200z_ctx *c, uint32_t flags) { if (c) c->flags = flags; }
 extern "C" uint32_t b200z_ctx_flags(const b200z_ctx *c) { return c ? c->flags : 0; }
 extern "C" uint64_t b200z_xxh64(const uint8_t *data, size_t len) { XXH64State s; s.reset(); s.update(data, len); return s.digest(); }
@@ -2536,11 +2549,35 @@ struct CompressStaging {
     }
 };
 
+// The two slots of a host-to-host pipeline around the ctx stream (the stream compressor, the seekable stream writer): slot s serves
+// chunk or group k with k & 1 == s; uploads go on s_h2d, downloads on s_d2h.  A slot's buffers are reused only after the event of
+// the last work that read them: ev_k (kernels: d_in, d_desc), ev_h2d (upload: h_in, h_desc), ev_d2h (download: d_out, h_out).
+struct PipeSlots {
+    Stream s_h2d, s_d2h;
+    Event ev_h2d[2], ev_k[2], ev_d2h[2];
+    PinnedBuf h_in[2], h_out[2], h_desc[2];
+    DevBuf d_in[2], d_out[2], d_desc[2];
+    int create(b200z_ctx *c) {   // the streams and events, once
+        if (!s_h2d && s_h2d.create(c)) return B200Z_ERR_CUDA;
+        if (!s_d2h && s_d2h.create(c)) return B200Z_ERR_CUDA;
+        for (int i = 0; i < 2; i++)
+            for (Event *e : {&ev_h2d[i], &ev_k[i], &ev_d2h[i]})
+                if (!*e && e->create(c)) return B200Z_ERR_CUDA;
+        return 0;
+    }
+    void drain(cudaStream_t ks) {   // leaves nothing in flight on the copy streams and on ks (when given)
+        if (s_h2d) cudaStreamSynchronize(s_h2d);
+        if (ks) cudaStreamSynchronize(ks);
+        if (s_d2h) cudaStreamSynchronize(s_d2h);
+    }
+};
+
 struct CompressResources {
     DevBuf frames, blocks, csum, results, input, output;
     CompressStaging stage;
     DevBuf dcontent, dtab, dcounts;   // b200z_dict_finalize: the content's tail, its match table and the statistics
-    DevBuf seek_entries, seek_total;  // b200z_compress_seekable: the table's entries and the running archive size
+    DevBuf seek_entries, seek_total;  // b200z_compress_seekable(_stream): the table's entries and the running archive size
+    PipeSlots seek_pipe;              // b200z_compress_seekable_stream: d_desc is a group's size word, CFrames and CBlocks
     DevBuf rd_stage, rd_pieces;       // b200z_seekable_read_ranges: host output's slots and the scratch, the copy pieces
     PinnedBuf rd_host;                // b200z_seekable_read_ranges: the touched frames of a host archive, host output's slots
     Event ev[kCompressStages + 1];
@@ -2710,12 +2747,61 @@ extern "C" size_t b200z_seekable_bound(size_t n, size_t frame_size, int checksum
            seek_table_size(full + (rest ? 1 : 0), checksum != 0);
 }
 
-extern "C" int b200z_compress_seekable(b200z_ctx *c, const uint8_t *input, size_t input_len, int input_mem, size_t frame_size, int level,
-                                       int checksum, const b200z_dict *dict, uint8_t *output, size_t output_cap, int output_mem, size_t *written) {
-    // ---- everything is checked before any device work, as b200z_compress_frames_batch_dict checks it
+static uint64_t seek_frame_blocks(uint64_t frame_size) { return std::max<uint64_t>(1, (frame_size + ENC_BLOCK - 1) / ENC_BLOCK); }   // of a full frame
+
+// What a group of `bytes` source bytes from a frame boundary holds: frames, blocks, input bytes and its frames' bounds
+namespace {
+struct SeekGroupSize { uint64_t frames, blocks, in, out; };
+}  // namespace
+static SeekGroupSize seek_group_size(uint64_t bytes, uint64_t frame_size, const b200z_dict *dict) {
+    const uint64_t full = bytes / frame_size, rest = bytes % frame_size;
+    return SeekGroupSize{full + (rest ? 1 : 0), full * seek_frame_blocks(frame_size) + (rest ? (rest + ENC_BLOCK - 1) / ENC_BLOCK : 0), bytes,
+                         full * b200z_compress_bound_dict(frame_size, dict) + (rest ? b200z_compress_bound_dict(rest, dict) : 0)};
+}
+
+// The plan of frames [f0, f1) of a source cut every frame_size bytes and ending at `end`, as b200z_compress_frames_batch_dict plans the
+// same pieces: input offsets less `base`, CBlock.frame counted from f0.  Returns the blocks written to hb.
+static uint32_t seek_group_plan(uint64_t f0, uint64_t f1, uint64_t frame_size, uint64_t end, uint64_t base, CFrame *hf, CBlock *hb) {
+    uint32_t nb = 0;
+    for (uint64_t f = f0; f < f1; f++) {
+        const uint64_t off = f * frame_size - base, size = std::min<uint64_t>(frame_size, end - f * frame_size);
+        CFrame &fr = hf[f - f0];
+        fr = CFrame{off, size, 0, nb, 0};
+        uint64_t pos = 0;
+        do {
+            const uint32_t bs = (uint32_t)std::min<uint64_t>(ENC_BLOCK, size - pos);
+            hb[nb++] = CBlock{off + pos, bs, (uint32_t)std::min<uint64_t>(pos, ENC_WINDOW), (uint32_t)(f - f0), 0};
+            pos += bs;
+        } while (pos < size);
+        fr.nblocks = nb - fr.first_block;
+    }
+    return nb;
+}
+
+// A group's kernels on stream s, once a's frames, blocks, input and output are set: the compressor's stages, with k_cscan before
+// k_cassemble packing the frames behind *total (less origin) and writing their table entries from frame first_frame on
+static int seek_group_run(b200z_ctx *c, const CompressArgs &a, uint64_t *total, uint64_t origin, uint8_t *entries, uint64_t first_frame,
+                          cudaStream_t s) {
+    for (int st = 0; st < kCompressStages; st++) {
+        if (st == 3)
+            if (int le = launch_seek_scan(a, total, origin, entries, first_frame, s, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_cscan");
+        if (int le = launch_compress_stage(a, st, s, &c->launches)) return c->set_cuda_err((cudaError_t)le, kCompressStageNames[st]);
+    }
+    return 0;
+}
+
+// the level and dictionary checks of b200z_compress_frames_batch_dict
+static int seek_check_level(b200z_ctx *c, int level, const b200z_dict *dict) {
     if (level >= 2 && level <= 4) return B200Z_ERR_REFERENCE_WOULD_PANIC;
     if (!c || (level != B200Z_LEVEL_UNCOMPRESSED && level != B200Z_LEVEL_FASTEST && level != B200Z_LEVEL_LAZY)) return B200Z_ERR_INVALID_ARGUMENT;
     if (dict && dict->ctx != c) { c->err = "dictionary created on another context"; return B200Z_ERR_INVALID_ARGUMENT; }
+    return 0;
+}
+
+extern "C" int b200z_compress_seekable(b200z_ctx *c, const uint8_t *input, size_t input_len, int input_mem, size_t frame_size, int level,
+                                       int checksum, const b200z_dict *dict, uint8_t *output, size_t output_cap, int output_mem, size_t *written) {
+    // ---- everything is checked before any device work, as b200z_compress_frames_batch_dict checks it
+    if (int e = seek_check_level(c, level, dict)) return e;
     if ((input_mem != B200Z_MEM_HOST && input_mem != B200Z_MEM_DEVICE) || (output_mem != B200Z_MEM_HOST && output_mem != B200Z_MEM_DEVICE) ||
         (input_len && !input) || !output || !written) {
         c->err = "invalid argument";
@@ -2735,20 +2821,17 @@ extern "C" int b200z_compress_seekable(b200z_ctx *c, const uint8_t *input, size_
     CompressResources &r = *rp;
     const bool fast = level != B200Z_LEVEL_UNCOMPRESSED;
     const bool sum = checksum != 0;
-    const uint64_t fblocks = std::max<uint64_t>(1, (frame_size + ENC_BLOCK - 1) / ENC_BLOCK);   // blocks of a full frame
-    const uint64_t per_group = std::max<uint64_t>(1, B200Z_SEEKABLE_GROUP_BLOCKS / fblocks);   // frames per group
+    const uint64_t per_group = std::max<uint64_t>(1, B200Z_SEEKABLE_GROUP_BLOCKS / seek_frame_blocks(frame_size));   // frames per group
     // what the largest group holds -- frames, blocks, input bytes and its frames' bounds -- from the frames the input really has:
     // every group but the last is full, so the first and the last group are the candidates
-    uint64_t gframes = 1, gblocks = 1, gin = 0, gout = 0;
+    SeekGroupSize g{1, 1, 0, 0};
     for (uint64_t f0 : {uint64_t(0), nframes ? (nframes - 1) / per_group * per_group : uint64_t(0)}) {
         const uint64_t f1 = std::min(nframes, f0 + per_group);
-        const uint64_t in0 = std::min<uint64_t>(f0 * frame_size, input_len), in1 = std::min<uint64_t>(f1 * frame_size, input_len);
-        const uint64_t full = f1 > f0 ? (in1 - in0) / frame_size : 0, rest = f1 > f0 ? (in1 - in0) % frame_size : 0;
-        gframes = std::max(gframes, f1 - f0);
-        gblocks = std::max(gblocks, full * fblocks + (rest ? (rest + ENC_BLOCK - 1) / ENC_BLOCK : 0));
-        gin = std::max(gin, in1 - in0);
-        gout = std::max(gout, full * b200z_compress_bound_dict(frame_size, dict) + (rest ? b200z_compress_bound_dict(rest, dict) : 0));
+        const SeekGroupSize x = seek_group_size(std::min<uint64_t>(f1 * frame_size, input_len) - std::min<uint64_t>(f0 * frame_size, input_len),
+                                                frame_size, dict);
+        g = SeekGroupSize{std::max(g.frames, x.frames), std::max(g.blocks, x.blocks), std::max(g.in, x.in), std::max(g.out, x.out)};
     }
+    const uint64_t gframes = g.frames, gblocks = g.blocks, gin = g.in, gout = g.out;
     const uint64_t table = seek_table_size(nframes, sum);
     int e = 0;
     if ((e = r.frames.ensure(gframes * sizeof(CFrame))) || (e = r.blocks.ensure(gblocks * sizeof(CBlock))) ||
@@ -2768,39 +2851,23 @@ extern "C" int b200z_compress_seekable(b200z_ctx *c, const uint8_t *input, size_
     uint64_t *d_total = r.seek_total.as<uint64_t>();
     CU(c, cudaMemsetAsync(d_total, 0, 8, s));
     uint64_t origin = 0;        // archive offset of d_out's byte 0 (host output: the group's first byte)
-    std::vector<CFrame> hf;
-    std::vector<CBlock> hb;
+    std::vector<CFrame> hf(gframes);
+    std::vector<CBlock> hb(gblocks);
     for (uint64_t f0 = 0; f0 < nframes; f0 += per_group) {
         const uint64_t f1 = std::min(nframes, f0 + per_group);
         const uint64_t in0 = f0 * frame_size, in1 = std::min<uint64_t>(f1 * frame_size, input_len);
         const uint64_t base = input_mem == B200Z_MEM_HOST ? in0 : 0;   // host input: the group is uploaded to r.input's byte 0
-        hf.clear(); hb.clear();
-        for (uint64_t f = f0; f < f1; f++) {   // the plan of b200z_compress_frames_batch_dict for the same pieces
-            const uint64_t off = f * frame_size - base, size = std::min<uint64_t>(frame_size, input_len - f * frame_size);
-            hf.push_back(CFrame{off, size, 0, (uint32_t)hb.size(), 0});
-            uint64_t pos = 0;
-            do {
-                const uint32_t bs = (uint32_t)std::min<uint64_t>(ENC_BLOCK, size - pos);
-                hb.push_back(CBlock{off + pos, bs, (uint32_t)std::min<uint64_t>(pos, ENC_WINDOW), (uint32_t)(f - f0), 0});
-                pos += bs;
-            } while (pos < size);
-            hf.back().nblocks = (uint32_t)hb.size() - hf.back().first_block;
-        }
+        a.nframes = (uint32_t)(f1 - f0);
+        a.nblocks = seek_group_plan(f0, f1, frame_size, input_len, base, hf.data(), hb.data());
         a.input = input;
         if (input_mem == B200Z_MEM_HOST) {
             CU(c, cudaMemcpyAsync(r.input.p, input + in0, in1 - in0, cudaMemcpyHostToDevice, s));
             a.input = r.input.as<uint8_t>();
         }
         a.output = output_mem == B200Z_MEM_HOST ? r.output.as<uint8_t>() : output;
-        a.nframes = (uint32_t)hf.size(); a.nblocks = (uint32_t)hb.size();
-        CU(c, cudaMemcpyAsync(r.frames.p, hf.data(), hf.size() * sizeof(CFrame), cudaMemcpyHostToDevice, s));
-        CU(c, cudaMemcpyAsync(r.blocks.p, hb.data(), hb.size() * sizeof(CBlock), cudaMemcpyHostToDevice, s));
-        for (int st = 0; st < kCompressStages; st++) {
-            if (st == 3)
-                if (int le = launch_seek_scan(a, d_total, origin, r.seek_entries.as<uint8_t>(), f0, s, &c->launches))
-                    return c->set_cuda_err((cudaError_t)le, "k_cscan");
-            if (int le = launch_compress_stage(a, st, s, &c->launches)) return c->set_cuda_err((cudaError_t)le, kCompressStageNames[st]);
-        }
+        CU(c, cudaMemcpyAsync(r.frames.p, hf.data(), a.nframes * sizeof(CFrame), cudaMemcpyHostToDevice, s));
+        CU(c, cudaMemcpyAsync(r.blocks.p, hb.data(), a.nblocks * sizeof(CBlock), cudaMemcpyHostToDevice, s));
+        if (int e2 = seek_group_run(c, a, d_total, origin, r.seek_entries.as<uint8_t>(), f0, s)) return e2;
         if (output_mem == B200Z_MEM_HOST) {   // the group's frames, d_out[0, total - origin), to the archive at origin
             uint64_t total = 0;
             CU(c, cudaMemcpyAsync(&total, d_total, 8, cudaMemcpyDeviceToHost, s));
@@ -2818,6 +2885,149 @@ extern "C" int b200z_compress_seekable(b200z_ctx *c, const uint8_t *input, size_
     if (output_mem == B200Z_MEM_HOST) CU(c, cudaMemcpy(output + total, r.output.p, table, cudaMemcpyDeviceToHost));
     *written = total + table;
     return 0;
+}
+
+// ---- the seekable stream writer: groups of whole frames read from a source, two slots (PipeSlots), the table at the end
+static bool fc_read(b200z_read_fn rd, void *ru, uint8_t *buf, size_t cap, size_t *n, bool *eof);   // the stream compressor's reader
+
+static int seek_io(b200z_ctx *c, const std::string &what) {
+    c->err = what;
+    return B200Z_ERR_SEEKABLE_IO;
+}
+
+// Group k (slot s = k & 1) is read into h_in[s], uploaded with its plan, compressed and packed from d_out[s]'s byte 0 behind the
+// slot's own running-size word (the first 8 bytes of d_desc[s], uploaded as 0), and downloaded with that word; k_cscan writes the
+// entries at their global frame index.  While group k uploads and compresses, the host reads group k + 1 and writes group k - 1.
+// `retired`: entry buffers outgrown during the call, which kernels may still write until the call has synchronised.
+static int seek_stream(b200z_ctx *c, b200z_read_fn rd, void *ru, b200z_write_fn wr, void *wu, uint64_t fs, int level, bool sum,
+                       const b200z_dict *dict, b200z_seekable_stream_result &res, std::vector<DevBuf> &retired) {
+    if (int e = c->use()) return e;
+    CompressResources *rp = nullptr;
+    if (int e = compress_get(c, &rp)) return e;
+    CompressResources &r = *rp;
+    PipeSlots &P = r.seek_pipe;
+    if (P.create(c)) return B200Z_ERR_CUDA;
+    const uint64_t C = sd_chunk_bytes(), esz = sum ? 12 : 8;
+    const uint64_t G = std::max<uint64_t>(1, std::min<uint64_t>(C / fs, B200Z_SEEKABLE_GROUP_BLOCKS / seek_frame_blocks(fs))) * fs;
+    cudaStream_t ks = c->stream;
+    const auto oom = [&](int e) { c->err = "seekable stream: out of memory for groups of " + std::to_string(G) + " bytes"; return e; };
+    int e = 0;
+    for (int i = 0; i < 2; i++)
+        if ((e = P.h_in[i].ensure(G, false))) return oom(e);
+    // the entries so far, doubled when full: the old buffer is copied on the kernel stream and kept until the call ends, since
+    // freeing it earlier (cudaFree) would wait for the whole device in the middle of the pipeline
+    const auto grow_entries = [&](uint64_t need) -> int {
+        if (need <= r.seek_entries.cap) return 0;
+        DevBuf nb;
+        if (nb.alloc(std::max<uint64_t>(need, 2 * r.seek_entries.cap)) != cudaSuccess) return oom(B200Z_ERR_OUT_OF_MEMORY);
+        if (res.frames) CU(c, cudaMemcpyAsync(nb.p, r.seek_entries.p, res.frames * esz, cudaMemcpyDeviceToDevice, ks));
+        std::swap(nb, r.seek_entries);
+        retired.push_back(std::move(nb));
+        return 0;
+    };
+    size_t n[2] = {0, 0};
+    bool eof[2] = {false, false};
+    const auto read_group = [&](int s) -> int {
+        if (!fc_read(rd, ru, P.h_in[s].as<uint8_t>(), G, &n[s], &eof[s]))
+            return seek_io(c, "seekable stream: read_cb failed at source offset " + std::to_string(res.read) + " (archive offset " +
+                                  std::to_string(res.written) + ")");
+        res.read += n[s];
+        return 0;
+    };
+    if ((e = read_group(0)) || (e = grow_entries(16))) return e;
+    // every buffer sized by the first group, the largest one the source has (every group but the last is full)
+    const SeekGroupSize g = seek_group_size(n[0], fs, dict);
+    const uint64_t desc = 8 + g.frames * sizeof(CFrame) + g.blocks * sizeof(CBlock);
+    const bool fast = level != B200Z_LEVEL_UNCOMPRESSED;
+    for (int i = 0; i < 2 && n[0] && !e; i++)
+        if ((e = P.d_in[i].ensure(g.in + 16, false)) || (e = P.d_out[i].ensure(g.out + 16, false)) || (e = P.d_desc[i].ensure(desc, false)) ||
+            (e = P.h_desc[i].ensure(desc, false)) || (e = P.h_out[i].ensure(g.out + 16, false)))
+            break;
+    if (!e && n[0])
+        if (!(e = fast ? r.stage.ensure(g.blocks, true) : r.stage.res.ensure(g.blocks * sizeof(CBlockInfo))) && !(e = r.csum.ensure(g.frames * 8)))
+            e = r.results.ensure(g.frames * sizeof(b200z_compress_result));
+    if (e) return oom(e);
+    CompressArgs a{};
+    if ((e = compress_dict_args(c, dict, level, a))) return e;
+    r.stage.bind(a);
+    a.csum = r.csum.as<uint64_t>(); a.results = r.results.as<b200z_compress_result>();
+    a.level = level; a.checksum = sum ? 1 : 0;
+    const auto enqueue = [&](int s) -> int {
+        const uint64_t nf = (n[s] + fs - 1) / fs;
+        if (res.frames + nf > 0xffffffffull) { c->err = "seekable stream: more than 2^32 - 1 frames"; return B200Z_ERR_INVALID_ARGUMENT; }
+        if (int ge = grow_entries((res.frames + nf) * esz)) return ge;
+        uint8_t *hd = P.h_desc[s].as<uint8_t>(), *dd = P.d_desc[s].as<uint8_t>();
+        memset(hd, 0, 8);
+        CFrame *hf = reinterpret_cast<CFrame *>(hd + 8);
+        const uint32_t nb = seek_group_plan(0, nf, fs, n[s], 0, hf, reinterpret_cast<CBlock *>(hf + nf));
+        CU(c, cudaStreamWaitEvent(P.s_h2d, P.ev_k[s], 0));   // group k - 2's kernels are done with d_in[s] and d_desc[s]
+        CU(c, cudaMemcpyAsync(P.d_in[s].p, P.h_in[s].p, n[s], cudaMemcpyHostToDevice, P.s_h2d));
+        CU(c, cudaMemcpyAsync(dd, hd, 8 + nf * sizeof(CFrame) + nb * sizeof(CBlock), cudaMemcpyHostToDevice, P.s_h2d));
+        CU(c, cudaEventRecord(P.ev_h2d[s], P.s_h2d));
+        CU(c, cudaStreamWaitEvent(ks, P.ev_h2d[s], 0));
+        a.frames = reinterpret_cast<const CFrame *>(dd + 8); a.blocks = reinterpret_cast<const CBlock *>(a.frames + nf);
+        a.input = P.d_in[s].as<uint8_t>(); a.output = P.d_out[s].as<uint8_t>();
+        a.nframes = (uint32_t)nf; a.nblocks = nb;
+        if (int ke = seek_group_run(c, a, reinterpret_cast<uint64_t *>(dd), 0, r.seek_entries.as<uint8_t>(), res.frames, ks)) return ke;
+        CU(c, cudaEventRecord(P.ev_k[s], ks));
+        // the packed size, then the frames: the download takes their bounds, so that no host wait stands between the two
+        CU(c, cudaStreamWaitEvent(P.s_d2h, P.ev_k[s], 0));
+        CU(c, cudaMemcpyAsync(hd, dd, 8, cudaMemcpyDeviceToHost, P.s_d2h));
+        CU(c, cudaMemcpyAsync(P.h_out[s].p, a.output, seek_group_size(n[s], fs, dict).out, cudaMemcpyDeviceToHost, P.s_d2h));
+        CU(c, cudaEventRecord(P.ev_d2h[s], P.s_d2h));
+        res.frames += nf;
+        res.groups++;
+        return 0;
+    };
+    const auto write_group = [&](int s) -> int {
+        CU(c, cudaEventSynchronize(P.ev_d2h[s]));
+        uint64_t packed = 0;
+        memcpy(&packed, P.h_desc[s].p, 8);
+        if (!sd_write(wr, wu, P.h_out[s].as<uint8_t>(), packed, &res.written))
+            return seek_io(c, "seekable stream: write_cb failed at archive offset " + std::to_string(res.written));
+        return 0;
+    };
+    for (uint64_t k = 0;; k++) {
+        const int s = (int)(k & 1);
+        const bool have = n[s] > 0;
+        if (have && (e = enqueue(s))) return e;
+        if (have && !eof[s]) {   // read group k + 1 into the other slot once group k - 1's upload is done with it
+            if (k) CU(c, cudaEventSynchronize(P.ev_h2d[s ^ 1]));
+            if ((e = read_group(s ^ 1))) return e;
+        }
+        if (k && (e = write_group(s ^ 1))) return e;
+        if (!have || eof[s]) {
+            if (have && (e = write_group(s))) return e;
+            break;
+        }
+    }
+    // the table: k_cseek behind a zeroed word into r.output, downloaded and written
+    const uint64_t table = seek_table_size(res.frames, sum);
+    if ((e = r.output.ensure(table + 16)) || (e = r.seek_total.ensure(8))) return oom(e);
+    CU(c, cudaMemsetAsync(r.seek_total.p, 0, 8, ks));
+    if (int le = launch_seek_table(r.seek_entries.as<uint8_t>(), res.frames, a.checksum, r.seek_total.as<uint64_t>(), 0, r.output.as<uint8_t>(), ks,
+                                   &c->launches))
+        return c->set_cuda_err((cudaError_t)le, "k_cseek");
+    std::vector<uint8_t> tab(table);
+    CU(c, cudaMemcpyAsync(tab.data(), r.output.p, table, cudaMemcpyDeviceToHost, ks));
+    CU(c, cudaStreamSynchronize(ks));
+    if (!sd_write(wr, wu, tab.data(), table, &res.written))
+        return seek_io(c, "seekable stream: write_cb failed at archive offset " + std::to_string(res.written));
+    return 0;
+}
+
+extern "C" int b200z_compress_seekable_stream(b200z_ctx *c, b200z_read_fn rd, void *ru, b200z_write_fn wr, void *wu, size_t frame_size, int level,
+                                              int checksum, const b200z_dict *dict, b200z_seekable_stream_result *result) {
+    // ---- everything is checked before any read, write or launch, as b200z_compress_seekable checks it
+    if (int e = seek_check_level(c, level, dict)) return e;
+    if (!rd || !wr) { c->err = "invalid argument"; return B200Z_ERR_INVALID_ARGUMENT; }
+    if (!frame_size || frame_size > B200Z_SEEKABLE_MAX_FRAME_SIZE) { c->err = "frame_size must lie in [1, 2^30]"; return B200Z_ERR_INVALID_ARGUMENT; }
+    b200z_seekable_stream_result res{};
+    std::vector<DevBuf> retired;   // released after the drain below
+    const int e = seek_stream(c, rd, ru, wr, wu, frame_size, level, checksum != 0, dict, res, retired);
+    if (e && c->comp) c->comp->seek_pipe.drain(c->stream);   // leave nothing in flight: the slots are reused by the next call
+    if (result) *result = res;
+    return e;
 }
 
 // The table of an archive, parsed and checked: the footer (the archive's last 9 bytes) first, then the table frame in front of it
@@ -2845,10 +3055,15 @@ static int seek_footer(const uint8_t *ft, uint64_t len, SeekTable &t, uint64_t *
     return 0;
 }
 // the table frame (table_bytes of it, the footer included): its header and the entries, whose Compressed_Size must add up to its offset
+// the table frame's 8-byte header, against the footer's Number_Of_Frames and flag (Frame_Size is a u32, so this bounds the table)
+static int seek_table_header(const uint8_t *p, const SeekTable &t, std::string *why) {
+    if (seek_le32(p) != SEEK_SKIPPABLE_MAGIC) return seek_fail(why, "the table frame's Skippable_Magic_Number is not 0x184D2A5E");
+    if (seek_le32(p + 4) != t.n * (t.checksum ? 12 : 8) + SEEK_FOOTER) return seek_fail(why, "Frame_Size is not Number_Of_Frames * (8 or 12) + 9");
+    return 0;
+}
 static int seek_entries(const uint8_t *p, SeekTable &t, std::string *why) {
     const uint64_t esz = t.checksum ? 12 : 8, tb = seek_table_size(t.n, t.checksum);
-    if (seek_le32(p) != SEEK_SKIPPABLE_MAGIC) return seek_fail(why, "the table frame's Skippable_Magic_Number is not 0x184D2A5E");
-    if (seek_le32(p + 4) != t.n * esz + SEEK_FOOTER) return seek_fail(why, "Frame_Size is not Number_Of_Frames * (8 or 12) + 9");
+    if (int e = seek_table_header(p, t, why)) return e;
     t.coff.assign(t.n + 1, 0); t.doff.assign(t.n + 1, 0); t.csum.assign(t.checksum ? t.n : 0, 0);
     for (uint64_t i = 0; i < t.n; i++) {
         const uint8_t *e = p + 8 + i * esz;
@@ -2954,10 +3169,47 @@ extern "C" int b200z_debug_seekable_plan(const uint8_t *archive, size_t len, con
 
 struct b200z_seekable {
     b200z_ctx *ctx = nullptr;
-    const uint8_t *archive = nullptr;   // borrowed
-    int mem = B200Z_MEM_HOST;
+    const uint8_t *archive = nullptr;   // borrowed; null behind read_at
+    int mem = B200Z_MEM_HOST;           // a host archive, or one behind read_at
+    b200z_read_at_fn read_at = nullptr;
+    void *user = nullptr;
     SeekTable t;
 };
+
+// an archive that is not in host memory: only the footer, then the table frame, are fetched to the host, by fetch(offset, buf, len).
+// The table frame's header is fetched and checked first, so that a corrupt Number_Of_Frames fails before a table of its size is
+// allocated or read; a table that still does not fit in host memory is B200Z_ERR_OUT_OF_MEMORY.
+template <class Fetch>
+static int seek_parse_fetched(uint64_t len, Fetch fetch, SeekTable &t, std::string *why) {
+    uint8_t ft[SEEK_FOOTER] = {}, hd[8] = {};
+    if (len >= SEEK_FOOTER)
+        if (int e = fetch(len - SEEK_FOOTER, ft, (uint64_t)SEEK_FOOTER)) return e;
+    uint64_t tb = 0;
+    if (int e = seek_footer(ft, len, t, &tb, why)) return e;
+    if (int e = fetch(len - tb, hd, (uint64_t)sizeof hd)) return e;
+    if (int e = seek_table_header(hd, t, why)) return e;
+    try {
+        std::vector<uint8_t> tab(tb);
+        if (int e = fetch(len - tb, tab.data(), tb)) return e;
+        return seek_entries(tab.data(), t, why);
+    } catch (const std::bad_alloc &) {
+        if (why) *why = "seek table: " + std::to_string(t.n) + " frames do not fit in host memory";
+        return B200Z_ERR_OUT_OF_MEMORY;
+    }
+}
+
+// len bytes at archive offset `at` through read_at, partial reads retried until one returns 0
+static int seek_read_at(const b200z_seekable *s, uint64_t at, uint8_t *buf, uint64_t len) {
+    for (uint64_t got = 0; got < len;) {
+        const long r = s->read_at(s->user, at + got, buf + got, len - got);
+        if (r < 0 || (uint64_t)r > len - got) return seek_io(s->ctx, "read_at failed at archive offset " + std::to_string(at + got));
+        if (r == 0)
+            return seek_io(s->ctx, "read_at came up short at archive offset " + std::to_string(at + got) + ": " + std::to_string(got) + " of " +
+                                       std::to_string(len) + " bytes from offset " + std::to_string(at));
+        got += (uint64_t)r;
+    }
+    return 0;
+}
 
 extern "C" int b200z_seekable_open(b200z_ctx *c, const uint8_t *archive, size_t len, int mem, b200z_seekable **out) {
     if (!c || !out || (!archive && len) || (mem != B200Z_MEM_HOST && mem != B200Z_MEM_DEVICE)) return B200Z_ERR_INVALID_ARGUMENT;
@@ -2966,16 +3218,24 @@ extern "C" int b200z_seekable_open(b200z_ctx *c, const uint8_t *archive, size_t 
     s->ctx = c; s->archive = archive; s->mem = mem;
     if (mem == B200Z_MEM_HOST) {
         if (int e = seek_parse_host(archive, len, s->t, &c->err)) return e;
-    } else {   // only the footer, then the table frame, cross to the host
+    } else {
         if (int e = c->use()) return e;
-        uint8_t ft[SEEK_FOOTER] = {};
-        if (len >= SEEK_FOOTER) CU(c, cudaMemcpy(ft, archive + len - SEEK_FOOTER, SEEK_FOOTER, cudaMemcpyDeviceToHost));
-        uint64_t tb = 0;
-        if (int e = seek_footer(ft, len, s->t, &tb, &c->err)) return e;
-        std::vector<uint8_t> tab(tb);
-        CU(c, cudaMemcpy(tab.data(), archive + len - tb, tb, cudaMemcpyDeviceToHost));
-        if (int e = seek_entries(tab.data(), s->t, &c->err)) return e;
+        const auto fetch = [&](uint64_t at, uint8_t *buf, uint64_t n) -> int {
+            CU(c, cudaMemcpy(buf, archive + at, n, cudaMemcpyDeviceToHost));
+            return 0;
+        };
+        if (int e = seek_parse_fetched(len, fetch, s->t, &c->err)) return e;
     }
+    *out = s.release();
+    return 0;
+}
+extern "C" int b200z_seekable_open_source(b200z_ctx *c, b200z_read_at_fn read_at, void *user, uint64_t len, b200z_seekable **out) {
+    if (!c || !out || !read_at) return B200Z_ERR_INVALID_ARGUMENT;
+    *out = nullptr;
+    std::unique_ptr<b200z_seekable> s(new b200z_seekable());
+    s->ctx = c; s->read_at = read_at; s->user = user;
+    const auto fetch = [&](uint64_t at, uint8_t *buf, uint64_t n) { return seek_read_at(s.get(), at, buf, n); };
+    if (int e = seek_parse_fetched(len, fetch, s->t, &c->err)) return e;
     *out = s.release();
     return 0;
 }
@@ -3045,7 +3305,16 @@ extern "C" int b200z_seekable_read_ranges(b200z_seekable *s, const b200z_range *
         if (int e = res.rd_host.ensure(std::max<uint64_t>(host_arch ? gathered : 0, staged) + 16)) return e;
     if (host_arch) {
         uint8_t *h = res.rd_host.as<uint8_t>();
-        for (size_t i = 0; i < p.frames.size(); i++) memcpy(h + io[i].src_off, s->archive + t.coff[p.frames[i].frame], io[i].src_size);
+        if (s->read_at) {   // one read_at per run of touched frames adjacent in the archive: they are adjacent in h too
+            for (size_t i = 0, j; i < p.frames.size(); i = j) {
+                const uint64_t at = t.coff[p.frames[i].frame];
+                uint64_t len = io[i].src_size;
+                for (j = i + 1; j < p.frames.size() && t.coff[p.frames[j].frame] == at + len; j++) len += io[j].src_size;
+                if (int e = seek_read_at(s, at, h + io[i].src_off, len)) return e;
+            }
+        } else {
+            for (size_t i = 0; i < p.frames.size(); i++) memcpy(h + io[i].src_off, s->archive + t.coff[p.frames[i].frame], io[i].src_size);
+        }
         src = h; src_len = gathered;
     }
     b200z_batch *bp = nullptr;
@@ -3114,12 +3383,10 @@ struct b200z_frame_compressor {
     bool checksum = true;
     uint64_t chunk = 64ull << 20;   // bytes per chunk, a multiple of ENC_BLOCK
     std::vector<uint8_t> raw;       // Uncompressed: one chunk's part of the frame
-    // Fastest, allocated by its first compress; slot s serves chunks k with k & 1 == s
-    // (b200z_frame_compressor_free synchronises the copy streams before any of these is released)
-    Stream s_h2d, s_d2h;
-    Event ev_h2d[2], ev_k[2], ev_d2h[2];
-    PinnedBuf h_in[2], h_out[2], h_desc[2];   // desc: the chunk's CFrame, its CBlocks, then its b200z_compress_result
-    DevBuf d_in[2], d_out[2], d_desc[2];      // d_in: the previous chunk's last ENC_WINDOW bytes, then the chunk
+    // Fastest, allocated by its first compress (b200z_frame_compressor_free synchronises the copy streams before any of these is
+    // released).  desc: the chunk's CFrame, its CBlocks, then its b200z_compress_result; d_in: the previous chunk's last ENC_WINDOW
+    // bytes, then the chunk
+    PipeSlots p;
     CompressStaging stage;                    // shared: the kernels run in order on one stream
     bool ready = false;
     uint32_t chunk_blocks() const { return (uint32_t)(chunk / ENC_BLOCK); }
@@ -3149,8 +3416,7 @@ extern "C" void b200z_frame_compressor_free(b200z_frame_compressor *fc) {
     if (!fc) return;
     if (fc->ready) {
         cudaSetDevice(fc->device);
-        cudaStreamSynchronize(fc->s_h2d);
-        cudaStreamSynchronize(fc->s_d2h);
+        fc->p.drain(nullptr);
     }
     delete fc;
 }
@@ -3238,16 +3504,12 @@ static int fc_prepare(b200z_frame_compressor *fc) {
     if (fc->ready) return 0;
     b200z_ctx *c = fc->ctx;
     const size_t C = fc->chunk, nb = fc->chunk_blocks(), bound = fc->chunk_bound();
-    if (!fc->s_h2d && fc->s_h2d.create(c)) return B200Z_ERR_CUDA;
-    if (!fc->s_d2h && fc->s_d2h.create(c)) return B200Z_ERR_CUDA;
-    for (int i = 0; i < 2; i++)
-        for (Event *e : {&fc->ev_h2d[i], &fc->ev_k[i], &fc->ev_d2h[i]})
-            if (!*e && e->create(c)) return B200Z_ERR_CUDA;
+    if (fc->p.create(c)) return B200Z_ERR_CUDA;
     int e = 0;
     for (int i = 0; i < 2 && !e; i++)
-        if ((e = fc->d_in[i].ensure(ENC_WINDOW + C + 16, false)) || (e = fc->d_out[i].ensure(bound + 16, false)) ||
-            (e = fc->d_desc[i].ensure(fc->desc_bytes(), false)) || (e = fc->h_in[i].ensure(C, false)) ||
-            (e = fc->h_out[i].ensure(FC_HDR_ROOM + bound + FC_TRAILER, false)) || (e = fc->h_desc[i].ensure(fc->desc_bytes(), false)))
+        if ((e = fc->p.d_in[i].ensure(ENC_WINDOW + C + 16, false)) || (e = fc->p.d_out[i].ensure(bound + 16, false)) ||
+            (e = fc->p.d_desc[i].ensure(fc->desc_bytes(), false)) || (e = fc->p.h_in[i].ensure(C, false)) ||
+            (e = fc->p.h_out[i].ensure(FC_HDR_ROOM + bound + FC_TRAILER, false)) || (e = fc->p.h_desc[i].ensure(fc->desc_bytes(), false)))
             break;
     if (!e) e = fc->stage.ensure(nb, false);
     if (e) { c->err = "FrameCompressor: out of memory for chunks of " + std::to_string(C) + " bytes"; return e; }
@@ -3270,41 +3532,41 @@ static int fc_compress_fast(b200z_frame_compressor *fc, b200z_read_fn rd, void *
     size_t out_n[2] = {0, 0};           // the chunk whose output is in slot s
     auto enqueue = [&](uint64_t k, int s) -> int {
         const uint32_t m = (uint32_t)((n[s] + ENC_BLOCK - 1) / ENC_BLOCK);
-        CFrame *hf = fc->h_desc[s].as<CFrame>();
+        CFrame *hf = fc->p.h_desc[s].as<CFrame>();
         CBlock *hb = reinterpret_cast<CBlock *>(hf + 1);
         *hf = CFrame{ENC_WINDOW, n[s], 0, 0, m};
         for (uint32_t i = 0; i < m; i++) {
             const uint64_t at = (uint64_t)i * ENC_BLOCK;
             hb[i] = CBlock{ENC_WINDOW + at, (uint32_t)std::min<uint64_t>(ENC_BLOCK, n[s] - at), (uint32_t)std::min<uint64_t>(k * C + at, ENC_WINDOW), 0, 0};
         }
-        uint8_t *din = fc->d_in[s].as<uint8_t>();
-        CU(c, cudaStreamWaitEvent(fc->s_h2d, fc->ev_k[s], 0));   // chunk k - 2's kernels are done with d_in[s] and d_desc[s]
-        if (k) CU(c, cudaMemcpyAsync(din, fc->d_in[s ^ 1].as<uint8_t>() + C, ENC_WINDOW, cudaMemcpyDeviceToDevice, fc->s_h2d));
-        CU(c, cudaMemcpyAsync(din + ENC_WINDOW, fc->h_in[s].p, n[s], cudaMemcpyHostToDevice, fc->s_h2d));
-        CU(c, cudaMemcpyAsync(fc->d_desc[s].p, hf, sizeof(CFrame) + m * sizeof(CBlock), cudaMemcpyHostToDevice, fc->s_h2d));
-        CU(c, cudaEventRecord(fc->ev_h2d[s], fc->s_h2d));
-        CU(c, cudaStreamWaitEvent(ks, fc->ev_h2d[s], 0));
+        uint8_t *din = fc->p.d_in[s].as<uint8_t>();
+        CU(c, cudaStreamWaitEvent(fc->p.s_h2d, fc->p.ev_k[s], 0));   // chunk k - 2's kernels are done with d_in[s] and d_desc[s]
+        if (k) CU(c, cudaMemcpyAsync(din, fc->p.d_in[s ^ 1].as<uint8_t>() + C, ENC_WINDOW, cudaMemcpyDeviceToDevice, fc->p.s_h2d));
+        CU(c, cudaMemcpyAsync(din + ENC_WINDOW, fc->p.h_in[s].p, n[s], cudaMemcpyHostToDevice, fc->p.s_h2d));
+        CU(c, cudaMemcpyAsync(fc->p.d_desc[s].p, hf, sizeof(CFrame) + m * sizeof(CBlock), cudaMemcpyHostToDevice, fc->p.s_h2d));
+        CU(c, cudaEventRecord(fc->p.ev_h2d[s], fc->p.s_h2d));
+        CU(c, cudaStreamWaitEvent(ks, fc->p.ev_h2d[s], 0));
         CompressArgs a{};
-        a.frames = fc->d_desc[s].as<CFrame>();
+        a.frames = fc->p.d_desc[s].as<CFrame>();
         a.blocks = reinterpret_cast<const CBlock *>(a.frames + 1);
-        a.results = reinterpret_cast<b200z_compress_result *>(fc->d_desc[s].as<uint8_t>() + fc->res_off());
-        a.input = din; a.output = fc->d_out[s].as<uint8_t>();
+        a.results = reinterpret_cast<b200z_compress_result *>(fc->p.d_desc[s].as<uint8_t>() + fc->res_off());
+        a.input = din; a.output = fc->p.d_out[s].as<uint8_t>();
         fc->stage.bind(a);
         a.nframes = 1; a.nblocks = m; a.level = fc->level;   // Fastest or LAZY
         if (int le = launch_compress_chunk(a, ks, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_cmatch / k_cenc / k_cassemble<true>");
-        CU(c, cudaEventRecord(fc->ev_k[s], ks));
-        CU(c, cudaStreamWaitEvent(fc->s_d2h, fc->ev_k[s], 0));
-        CU(c, cudaMemcpyAsync(fc->h_desc[s].as<uint8_t>() + fc->res_off(), a.results, sizeof(b200z_compress_result), cudaMemcpyDeviceToHost, fc->s_d2h));
-        CU(c, cudaMemcpyAsync(fc->h_out[s].as<uint8_t>() + FC_HDR_ROOM, a.output, n[s] + 3ull * m, cudaMemcpyDeviceToHost, fc->s_d2h));
-        CU(c, cudaEventRecord(fc->ev_d2h[s], fc->s_d2h));
+        CU(c, cudaEventRecord(fc->p.ev_k[s], ks));
+        CU(c, cudaStreamWaitEvent(fc->p.s_d2h, fc->p.ev_k[s], 0));
+        CU(c, cudaMemcpyAsync(fc->p.h_desc[s].as<uint8_t>() + fc->res_off(), a.results, sizeof(b200z_compress_result), cudaMemcpyDeviceToHost, fc->p.s_d2h));
+        CU(c, cudaMemcpyAsync(fc->p.h_out[s].as<uint8_t>() + FC_HDR_ROOM, a.output, n[s] + 3ull * m, cudaMemcpyDeviceToHost, fc->p.s_d2h));
+        CU(c, cudaEventRecord(fc->p.ev_d2h[s], fc->p.s_d2h));
         return 0;
     };
     auto write_chunk = [&](uint64_t k, int s, bool final) -> int {
-        uint8_t *const body = fc->h_out[s].as<uint8_t>() + FC_HDR_ROOM;
+        uint8_t *const body = fc->p.h_out[s].as<uint8_t>() + FC_HDR_ROOM;
         size_t len = 0;
         if (out_n[s]) {
-            CU(c, cudaEventSynchronize(fc->ev_d2h[s]));
-            const b200z_compress_result &cr = *reinterpret_cast<const b200z_compress_result *>(fc->h_desc[s].as<uint8_t>() + fc->res_off());
+            CU(c, cudaEventSynchronize(fc->p.ev_d2h[s]));
+            const b200z_compress_result &cr = *reinterpret_cast<const b200z_compress_result *>(fc->p.h_desc[s].as<uint8_t>() + fc->res_off());
             len = cr.dst_size;
             r.blocks += cr.blocks; r.raw_blocks += cr.raw_blocks; r.rle_blocks += cr.rle_blocks;
         }
@@ -3317,25 +3579,21 @@ static int fc_compress_fast(b200z_frame_compressor *fc, b200z_read_fn rd, void *
         return 0;
     };
     int e = 0;
-    if (!fc_read(rd, ru, fc->h_in[0].as<uint8_t>(), C, &n[0], &eof[0])) e = fc_panic(c, "FrameCompressor::compress: the source's read failed");
-    else h.update(fc->h_in[0].as<uint8_t>(), n[0]);
+    if (!fc_read(rd, ru, fc->p.h_in[0].as<uint8_t>(), C, &n[0], &eof[0])) e = fc_panic(c, "FrameCompressor::compress: the source's read failed");
+    else h.update(fc->p.h_in[0].as<uint8_t>(), n[0]);
     for (uint64_t k = 0; !e; k++) {
         const int s = (int)(k & 1);
         out_n[s] = n[s];
         if (n[s] && (e = enqueue(k, s))) break;
         if (!eof[s]) {   // read chunk k + 1 into the other slot once chunk k - 1's upload is done with it
-            if (k && cudaEventSynchronize(fc->ev_h2d[s ^ 1]) != cudaSuccess) { e = c->set_cuda_err(cudaGetLastError(), "upload"); break; }
-            if (!fc_read(rd, ru, fc->h_in[s ^ 1].as<uint8_t>(), C, &n[s ^ 1], &eof[s ^ 1])) { e = fc_panic(c, "FrameCompressor::compress: the source's read failed"); break; }
-            h.update(fc->h_in[s ^ 1].as<uint8_t>(), n[s ^ 1]);
+            if (k && cudaEventSynchronize(fc->p.ev_h2d[s ^ 1]) != cudaSuccess) { e = c->set_cuda_err(cudaGetLastError(), "upload"); break; }
+            if (!fc_read(rd, ru, fc->p.h_in[s ^ 1].as<uint8_t>(), C, &n[s ^ 1], &eof[s ^ 1])) { e = fc_panic(c, "FrameCompressor::compress: the source's read failed"); break; }
+            h.update(fc->p.h_in[s ^ 1].as<uint8_t>(), n[s ^ 1]);
         }
         if (k && (e = write_chunk(k - 1, s ^ 1, false))) break;
         if (eof[s]) { e = write_chunk(k, s, true); break; }
     }
-    if (e) {   // leave nothing in flight: the buffers are reused by the next compress
-        cudaStreamSynchronize(fc->s_h2d);
-        cudaStreamSynchronize(ks);
-        cudaStreamSynchronize(fc->s_d2h);
-    }
+    if (e) fc->p.drain(ks);   // leave nothing in flight: the buffers are reused by the next compress
     return e;
 }
 
