@@ -6,6 +6,7 @@ import os
 import numpy as np
 import pytest
 
+import intermediates
 from conftest import read_golden
 
 pytestmark = pytest.mark.gpu
@@ -68,30 +69,9 @@ def test_corpus_batch_and_intermediates(pkg, ctx, oracle, manifest, exec_mode):
         r = d.reset(frames[i]); d.decode_blocks(r); d.collect()
         blocks, lits, seqs = d.trace()
         assert res[i]["blocks_decoded"] == len(blocks)
-        hist = [1, 4, 8]   # repeat-offset history at the start of the block (scratch.rs:44)
-        for tb in blocks:
-            if tb["block_type"] == 2:
-                if tb["literals_type"] >= 2:
-                    got_l = b.debug_literals(blk)
-                    assert got_l == lits[tb["lit_offset"]:tb["lit_offset"] + tb["regenerated_size"]], (n, blk)
-                    nlit += 1
-                if tb["num_sequences"]:
-                    got_s = b.debug_sequences(blk)
-                    exp = seqs[tb["seq_offset"]:tb["seq_offset"] + tb["num_sequences"]]
-                    assert np.array_equal(got_s[:, :2], exp[:, :2]), (n, blk)
-                    # offsets: raw offset_values when the block went through k_fse's exact path, otherwise already through
-                    # do_offset_history (oracle column 3), symbolic where they depend on the history at the block's start
-                    if b.debug_block_flags(blk) & 1:
-                        assert np.array_equal(got_s[:, 2], exp[:, 2]), (n, blk)
-                    else:
-                        sym = got_s[:, 2].astype(np.int64)
-                        tag, dec = sym >> 30, sym & ((1 << 30) - 1)
-                        h = np.array([0] + hist, dtype=np.int64)[tag]
-                        actual = np.where(tag == 0, sym, np.maximum(h - dec, 0))
-                        assert np.array_equal(actual, exp[:, 3].astype(np.int64)), (n, blk)
-                    nseq += len(exp)
-                    hist = list(tb["offset_hist_after"])
-            blk += 1
+        blk, nl, ns = intermediates.check_intermediates(b, blk, blocks, lits, seqs, n)
+        nlit += nl
+        nseq += ns
     assert nlit > 1000 and nseq > 1_000_000   # 2458 compressed blocks / 1,031,936 sequences in the corpus
 
 
