@@ -600,6 +600,26 @@ int b200z_compress_frames_batch_dict(b200z_ctx *ctx, const uint8_t *input, size_
                                      uint8_t *output, size_t output_cap, int output_mem, b200z_compress_result *results);
 /* b200z_compress_bound(src_size) + the size of the dictionary ID field the frame carries with `dict` (0, 1, 2 or 4 bytes) */
 size_t b200z_compress_bound_dict(size_t src_size, const b200z_dict *dict);
+/* EXTENSION: long-distance matching (libzstd's --long).  window_log lies in [B200Z_WINDOW_LOG_MIN, B200Z_WINDOW_LOG_MAX]; 17 is the
+ * 128 KiB window every other entry writes. */
+#define B200Z_WINDOW_LOG_MIN 17
+#define B200Z_WINDOW_LOG_MAX 27
+/* b200z_compress_frames_batch_dict with a window of 2^window_log bytes for long matches (EXTENSION; DESIGN.md section 4.11,
+ * tests/cldm.py states the rule).  The regular parse keeps its 128 KiB reach; in every frame larger than 131072 bytes, content-defined
+ * anchors (a gear hash of 64 bytes, about 1 in 128 positions, at most 1 in 16) find the nearest earlier anchor of the same frame
+ * with the same 64-byte hash, and where its offset lies in (131072, 2^window_log] and 64 or more bytes match inside the anchor's
+ * block, that match is forced into the parse.  Long matches never reach into the dictionary.  Each frame's Window_Descriptor
+ * carries min(window_log, max(17, ceil(log2 src_size))), so a frame of 131072 bytes or fewer is exactly what window_log 17
+ * writes, and window_log 17 is exactly b200z_compress_frames_batch_dict.  The compress bound is b200z_compress_bound_dict.  Besides
+ * that entry's checks: B200Z_ERR_INVALID_ARGUMENT, before any launch, for window_log outside [17, 27] and for a window_log
+ * above 17 at B200Z_LEVEL_UNCOMPRESSED.  Accepted at Fastest and LAZY.  With a frame larger than 131072 bytes and window_log > 17
+ * the submission first runs the long-match kernels (k_lanchor twice, k_lscan, four k_lhist / k_lscan / k_lscatter passes of the
+ * key sort, k_lcand, k_lblock: 17 launches, 3 when no anchor is found; counted in b200z_ctx_kernel_launches, not in
+ * b200z_compress_last_profile's four stages), synchronising once to size the anchors' buffers: 44 bytes per anchor (at most one per 16 input bytes of those frames,
+ * about one per 128 on typical data), 1 KiB per block of those frames and 8 bytes per block, kept with the context. */
+int b200z_compress_frames_batch_long(b200z_ctx *ctx, const uint8_t *input, size_t input_len, int input_mem,
+                                     const b200z_compress_io *frames, size_t nframes, int level, int checksum, const b200z_dict *dict,
+                                     int window_log, uint8_t *output, size_t output_cap, int output_mem, b200z_compress_result *results);
 int b200z_compress_num_stages(void);
 const char *b200z_compress_stage_name(int stage);
 /* each kernel's device milliseconds in the last b200z_compress_frames_batch run with B200Z_FLAG_PROFILE set */
@@ -631,6 +651,18 @@ int b200z_frame_compressor_new(b200z_ctx *ctx, int level, int checksum, b200z_fr
 void b200z_frame_compressor_free(b200z_frame_compressor *fc);
 int b200z_frame_compressor_set_compression_level(b200z_frame_compressor *fc, int level);   /* :263; 0-4 or LAZY, else INVALID_ARGUMENT */
 int b200z_frame_compressor_compression_level(const b200z_frame_compressor *fc);            /* :273 */
+/* EXTENSION: long-distance matches up to 2^window_log bytes back (b200z_compress_frames_batch_long's rule) from the next compress
+ * on; window_log in [17, 27], else B200Z_ERR_INVALID_ARGUMENT.  The frame's Window_Descriptor is 2^window_log (its size is unknown
+ * when the header is written).  Every block is what b200z_compress_frames_batch_long writes for the same block of the whole
+ * input compressed as one frame at the same level and window_log, at any chunk size.  compress returns B200Z_ERR_INVALID_ARGUMENT,
+ * before any read, for a window_log above 17 at level Uncompressed.  Above 17 each chunk goes to the device behind the last
+ * H = 2^window_log + 128 bytes before it (a device-to-device copy from the other slot), and the long-match kernels run on the
+ * spans of that history and the chunk (S = ceil(H / 131072) + C / 131072 of them) before k_cmatch.  Memory at window_log > 17,
+ * allocated by the first compress that needs it and kept until _free: device input 2 * (H + C) in place of 2 * (C + 131072),
+ * the anchors' buffers at the density bound, 44 * 8192 * S bytes, 1028 * S + 8 * C / 131072 bytes of counts, and 32 * S bytes
+ * of spans per descriptor slot (two on the device, two pinned); about 0.83 GB more device memory than at 17 for window_log 27 and C = 64 MiB. */
+int b200z_frame_compressor_set_window_log(b200z_frame_compressor *fc, int window_log);
+int b200z_frame_compressor_window_log(const b200z_frame_compressor *fc);
 /* compress :131-224: one frame from read_cb to write_cb.  B200Z_ERR_REFERENCE_WOULD_PANIC for levels 2-4 before any read, write
  * or launch.  result (may be NULL): dst_size = bytes written, blocks (the trailing empty block included), raw / RLE blocks
  * (the empty block is Raw), has_checksum, checksum */

@@ -1,5 +1,6 @@
 """zstd-rs_b200 -- GPU-native (H100, sm_90a) zstd block decompressor behind ruzstd's FrameDecoder / StreamingDecoder API,
-a batch compressor at ruzstd's Uncompressed and Fastest levels and an extension level LAZY (compress_frames / compress_to_vec), a stream compressor behind
+a batch compressor at ruzstd's Uncompressed and Fastest levels and an extension level LAZY (compress_frames / compress_to_vec; with
+long-distance matches up to 2^27 bytes back through window_log, as the stream compressor), a stream compressor behind
 ruzstd's FrameCompressor / encoding::compress API (FrameCompressor, compress), and a raw-content
 dictionary trainer in place of ruzstd::dictionary (create_raw_dict, create_raw_dict_from_source, create_raw_dict_from_dir)
 and a finalizer that turns its content into a zstd-format dictionary (finalize_dict, create_dict).  decode_all_stream decodes a

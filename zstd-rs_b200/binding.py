@@ -169,6 +169,7 @@ def lib():
         "b200z_compress_frames_batch": (C.c_int, [vp, vp, sz, C.c_int, vp, sz, C.c_int, C.c_int, vp, sz, C.c_int, vp]),
         "b200z_compress_frames_batch_dict": (C.c_int, [vp, vp, sz, C.c_int, vp, sz, C.c_int, C.c_int, vp, vp, sz, C.c_int, vp]),
         "b200z_compress_bound_dict": (sz, [sz, vp]),
+        "b200z_compress_frames_batch_long": (C.c_int, [vp, vp, sz, C.c_int, vp, sz, C.c_int, C.c_int, vp, C.c_int, vp, sz, C.c_int, vp]),
         "b200z_compress_num_stages": (C.c_int, []),
         "b200z_compress_stage_name": (C.c_char_p, [C.c_int]),
         "b200z_compress_last_profile": (C.c_int, [vp, C.POINTER(C.c_float), sz]),
@@ -176,6 +177,8 @@ def lib():
         "b200z_frame_compressor_free": (None, [vp]),
         "b200z_frame_compressor_set_compression_level": (C.c_int, [vp, C.c_int]),
         "b200z_frame_compressor_compression_level": (C.c_int, [vp]),
+        "b200z_frame_compressor_set_window_log": (C.c_int, [vp, C.c_int]),
+        "b200z_frame_compressor_window_log": (C.c_int, [vp]),
         "b200z_frame_compressor_compress": (C.c_int, [vp, READ_FN, vp, WRITE_FN, vp, vp]),
         "b200z_dict_train_raw": (C.c_int, [vp, vp, sz, C.c_int, vp, sz, sz, sz, vp, sz, C.POINTER(sz), vp, sz, C.POINTER(sz)]),
         "b200z_dict_finalize": (C.c_int, [vp, vp, sz, vp, sz, C.c_int, vp, sz, C.c_uint32, vp, sz, C.POINTER(sz)]),
@@ -560,17 +563,22 @@ def stream_cut(data, chunk):
         cap = n.value
 
 
+WINDOW_LOG_MIN, WINDOW_LOG_MAX = 17, 27   # B200Z_WINDOW_LOG_MIN / _MAX
+
+
 def compress_bound(n, dict=None):
     """b200z_compress_bound (b200z_compress_bound_dict with a Dictionary): the largest frame compress_frames can write for n input
     bytes."""
     return lib().b200z_compress_bound(n) if dict is None else lib().b200z_compress_bound_dict(n, dict.h)
 
 
-def compress_frames(ctx, input, io, output, level=FASTEST, checksum=True, dict=None, dict_tables=False):
-    """b200z_compress_frames_batch_dict: one zstd frame per COMPRESS_IO_DTYPE row (src_off, src_size, dst_off, dst_cap), every block
+def compress_frames(ctx, input, io, output, level=FASTEST, checksum=True, dict=None, dict_tables=False, window_log=WINDOW_LOG_MIN):
+    """b200z_compress_frames_batch_long: one zstd frame per COMPRESS_IO_DTYPE row (src_off, src_size, dst_off, dst_cap), every block
     of every frame compressed at once, against `dict` (a Dictionary of this context) when given.  dict_tables=True sets
-    FLAG_DICT_TABLES for the call: a formatted dictionary's entropy tables may then code each frame's first block.  input/output:
-    bytes, numpy or torch (host or cuda).  Returns COMPRESS_RESULT_DTYPE rows."""
+    FLAG_DICT_TABLES for the call: a formatted dictionary's entropy tables may then code each frame's first block.  window_log in
+    [17, 27]: above 17, frames larger than 128 KiB also take long-distance matches up to 2^window_log bytes back (17 is
+    b200z_compress_frames_batch_dict's output).  input/output: bytes, numpy or torch (host or cuda).  Returns COMPRESS_RESULT_DTYPE
+    rows."""
     fr = np.ascontiguousarray(io, dtype=COMPRESS_IO_DTYPE)
     res = np.zeros(len(fr), dtype=COMPRESS_RESULT_DTYPE)
     ip, il, _k1 = _ptr(input)
@@ -579,8 +587,8 @@ def compress_frames(ctx, input, io, output, level=FASTEST, checksum=True, dict=N
     if dict_tables:
         ctx.L.b200z_ctx_set_flags(ctx.h, flags | FLAG_DICT_TABLES)
     try:
-        e = ctx.L.b200z_compress_frames_batch_dict(ctx.h, ip, il, MEM_DEVICE if _is_device(input) else MEM_HOST, fr.ctypes.data, len(fr),
-                                                   level, 1 if checksum else 0, dict.h if dict is not None else None, op, ol,
+        e = ctx.L.b200z_compress_frames_batch_long(ctx.h, ip, il, MEM_DEVICE if _is_device(input) else MEM_HOST, fr.ctypes.data, len(fr),
+                                                   level, 1 if checksum else 0, dict.h if dict is not None else None, window_log, op, ol,
                                                    MEM_DEVICE if _is_device(output) else MEM_HOST, res.ctypes.data)
     finally:
         ctx.L.b200z_ctx_set_flags(ctx.h, flags)
@@ -588,14 +596,14 @@ def compress_frames(ctx, input, io, output, level=FASTEST, checksum=True, dict=N
     return res
 
 
-def compress_to_vec(ctx, data, level=FASTEST, checksum=True, dict=None, dict_tables=False):
+def compress_to_vec(ctx, data, level=FASTEST, checksum=True, dict=None, dict_tables=False, window_log=WINDOW_LOG_MIN):
     """Mirror of ruzstd::encoding::compress_to_vec (encoding/mod.rs): one frame holding `data`, as bytes (against `dict` when given,
-    with its entropy tables when dict_tables=True)."""
+    with its entropy tables when dict_tables=True; long-distance matches up to 2^window_log back, see compress_frames)."""
     src = bytes(data)
     cap = compress_bound(len(src), dict)
     out = np.zeros(cap, dtype=np.uint8)
     io = np.array([(0, len(src), 0, cap)], dtype=COMPRESS_IO_DTYPE)
-    res = compress_frames(ctx, src, io, out, level, checksum, dict, dict_tables)
+    res = compress_frames(ctx, src, io, out, level, checksum, dict, dict_tables, window_log)
     return out[:int(res[0]["dst_size"])].tobytes()
 
 
@@ -818,13 +826,15 @@ class FrameCompressor:
     frame is appended to.  An exception raised by the source or the drain fails the call as the reference's unwrap() would,
     with B200ZError(REFERENCE_WOULD_PANIC) raised from it."""
 
-    def __init__(self, ctx, level=FASTEST, checksum=True):
+    def __init__(self, ctx, level=FASTEST, checksum=True, window_log=WINDOW_LOG_MIN):
         self.ctx, self.L = ctx, ctx.L
         self.h = None
         h = C.c_void_p()
         ctx._chk(self.L.b200z_frame_compressor_new(ctx.h, level, 1 if checksum else 0, C.byref(h)))
         self.h = h
         self._source = self._drain = None
+        if window_log != WINDOW_LOG_MIN:
+            self.set_window_log(window_log)
 
     def __del__(self):
         try:
@@ -859,6 +869,15 @@ class FrameCompressor:
         return old
 
     def compression_level(self): return self.L.b200z_frame_compressor_compression_level(self.h)
+
+    def set_window_log(self, window_log):
+        """EXTENSION: long-distance matches up to 2^window_log back from the next compress() on (17: none).  Returns the previous
+        value."""
+        old = self.window_log()
+        self.ctx._chk(self.L.b200z_frame_compressor_set_window_log(self.h, window_log))
+        return old
+
+    def window_log(self): return self.L.b200z_frame_compressor_window_log(self.h)
 
     def compress(self):
         """One frame from the source to the drain.  Returns the COMPRESS_RESULT_DTYPE row: dst_size = bytes written, blocks,
@@ -909,10 +928,10 @@ def _raise_chained(ctx, e, failure):
         raise B200ZError(e, 0, ctx.L.b200z_ctx_last_error_message(ctx.h).decode()) from (failure[0] if failure else None)
 
 
-def compress(ctx, source, target, level=FASTEST, checksum=True):
+def compress(ctx, source, target, level=FASTEST, checksum=True, window_log=WINDOW_LOG_MIN):
     """Mirror of ruzstd::encoding::compress (encoding/mod.rs): one frame from `source` (bytes or a reader) to `target` (a writer
-    or a bytearray) through a FrameCompressor.  Returns its result row."""
-    fc = FrameCompressor(ctx, level, checksum)
+    or a bytearray) through a FrameCompressor (with long-distance matches up to 2^window_log back).  Returns its result row."""
+    fc = FrameCompressor(ctx, level, checksum, window_log)
     fc.set_source(source)
     fc.set_drain(target)
     return fc.compress()

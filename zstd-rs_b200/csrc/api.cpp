@@ -2572,6 +2572,29 @@ struct PipeSlots {
     }
 };
 
+// long-distance matches (window_log > 17): the spans, k_lanchor's counts, the anchors and their sort, the forced matches and
+// each block's share of them
+struct LdmBufs {
+    DevBuf spans, tcount, scount, keys[2], vals[2], hist, pos, frame, cand, forced, off, cnt;
+    static size_t tiles(uint32_t cap) { return std::max<size_t>(1, (cap + LDM_TILE - 1) / LDM_TILE); }
+    // the buffers for `cap` anchors: 44 bytes each, and 4 per 16 anchors of digit counts
+    int ensure(uint32_t cap, bool grow = true) {
+        const size_t n = std::max<uint32_t>(cap, 1);
+        int e = 0;
+        for (int i = 0; i < 2 && !e; i++)
+            if ((e = keys[i].ensure(n * 4, grow)) || (e = vals[i].ensure(n * 4, grow))) return e;
+        if ((e = hist.ensure((tiles(cap) * 256 + 1) * 4, grow)) || (e = pos.ensure(n * 8, grow)) || (e = frame.ensure(n * 4, grow)) ||
+            (e = cand.ensure(n * 4, grow)) || (e = forced.ensure(n * sizeof(LForced), grow)))
+            return e;
+        return 0;
+    }
+    void bind(LdmArgs &l) const {
+        for (int i = 0; i < 2; i++) { l.keys[i] = keys[i].as<uint32_t>(); l.vals[i] = vals[i].as<uint32_t>(); }
+        l.hist = hist.as<uint32_t>(); l.apos = pos.as<uint64_t>(); l.aframe = frame.as<uint32_t>(); l.cand = cand.as<uint32_t>();
+        l.forced = forced.as<LForced>(); l.lf_off = off.as<uint32_t>(); l.lf_cnt = cnt.as<uint32_t>();
+    }
+};
+
 struct CompressResources {
     DevBuf frames, blocks, csum, results, input, output;
     CompressStaging stage;
@@ -2580,6 +2603,7 @@ struct CompressResources {
     PipeSlots seek_pipe;              // b200z_compress_seekable_stream: d_desc is a group's size word, CFrames and CBlocks
     DevBuf rd_stage, rd_pieces;       // b200z_seekable_read_ranges: host output's slots and the scratch, the copy pieces
     PinnedBuf rd_host;                // b200z_seekable_read_ranges: the touched frames of a host archive, host output's slots
+    LdmBufs ldm;                      // b200z_compress_frames_batch_long
     Event ev[kCompressStages + 1];
     float stage_ms[kCompressStages] = {};
     bool profiled = false;
@@ -2641,9 +2665,47 @@ extern "C" int b200z_compress_frames_batch(b200z_ctx *c, const uint8_t *input, s
 extern "C" int b200z_compress_frames_batch_dict(b200z_ctx *c, const uint8_t *input, size_t input_len, int input_mem, const b200z_compress_io *frames,
                                                 size_t nframes, int level, int checksum, const b200z_dict *dict, uint8_t *output,
                                                 size_t output_cap, int output_mem, b200z_compress_result *results) {
+    return b200z_compress_frames_batch_long(c, input, input_len, input_mem, frames, nframes, level, checksum, dict, B200Z_WINDOW_LOG_MIN, output,
+                                            output_cap, output_mem, results);
+}
+
+// The long-distance match stage (ldm.cu) before k_cmatch, over the spans `sp` (LSpan.block indexes the submission's nblocks): anchors
+// counted; with cap == 0 their total is read back to size the buffers (batch), else the buffers hold cap anchors (stream: the
+// density bound).  Then anchors, sort, candidates and the blocks' forced matches into a.lforced / lf_*.
+static int compress_ldm(b200z_ctx *c, LdmBufs &r, CompressArgs &a, const LSpan *d_spans, uint32_t nspans, uint32_t nblocks, uint32_t window_log,
+                        uint32_t cap, cudaStream_t s) {
+    int e = 0;
+    if ((e = r.tcount.ensure((size_t)nspans * LDM_THREADS * sizeof(uint32_t))) || (e = r.scount.ensure((nspans + 1) * sizeof(uint32_t))) ||
+        (e = r.off.ensure(nblocks * sizeof(uint32_t))) ||
+        (e = r.cnt.ensure(nblocks * sizeof(uint32_t))))
+        return e;
+    CU(c, cudaMemsetAsync(r.cnt.p, 0, nblocks * sizeof(uint32_t), s));
+    LdmArgs l{};
+    l.input = a.input; l.spans = d_spans; l.nspans = nspans; l.window_log = window_log; l.tcount = r.tcount.as<uint32_t>();
+    l.scount = r.scount.as<uint32_t>();
+    if (int le = launch_ldm_count(l, s, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_lanchor");
+    l.cap = cap;
+    if (!cap) {
+        CU(c, cudaMemcpyAsync(&l.cap, l.scount + nspans, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+        CU(c, cudaStreamSynchronize(s));
+    }
+    if ((e = r.ensure(l.cap))) return e;
+    r.bind(l);
+    if (int le = launch_ldm_match(l, s, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_lblock");
+    a.lforced = l.forced; a.lf_off = l.lf_off; a.lf_cnt = l.lf_cnt;
+    return 0;
+}
+
+extern "C" int b200z_compress_frames_batch_long(b200z_ctx *c, const uint8_t *input, size_t input_len, int input_mem, const b200z_compress_io *frames,
+                                                size_t nframes, int level, int checksum, const b200z_dict *dict, int window_log, uint8_t *output,
+                                                size_t output_cap, int output_mem, b200z_compress_result *results) {
     // ---- everything is checked before any device work
     if (level >= 2 && level <= 4) return B200Z_ERR_REFERENCE_WOULD_PANIC;   // Default / Better / Best: unimplemented!() in the reference
     if (!c || (level != B200Z_LEVEL_UNCOMPRESSED && level != B200Z_LEVEL_FASTEST && level != B200Z_LEVEL_LAZY)) return B200Z_ERR_INVALID_ARGUMENT;
+    if (window_log < B200Z_WINDOW_LOG_MIN || window_log > B200Z_WINDOW_LOG_MAX || (level == B200Z_LEVEL_UNCOMPRESSED && window_log != B200Z_WINDOW_LOG_MIN)) {
+        c->err = "window_log outside [17, 27], or above 17 at level Uncompressed";
+        return B200Z_ERR_INVALID_ARGUMENT;
+    }
     if (dict && dict->ctx != c) { c->err = "dictionary created on another context"; return B200Z_ERR_INVALID_ARGUMENT; }
     if ((nframes && (!frames || !results)) || (input_mem != B200Z_MEM_HOST && input_mem != B200Z_MEM_DEVICE) ||
         (output_mem != B200Z_MEM_HOST && output_mem != B200Z_MEM_DEVICE) || (input_len && !input) || (output_cap && !output) || nframes > 0xffffffffu) {
@@ -2714,6 +2776,17 @@ extern "C" int b200z_compress_frames_batch_dict(b200z_ctx *c, const uint8_t *inp
     a.csum = r.csum.as<uint64_t>();
     a.results = r.results.as<b200z_compress_result>(); a.nframes = (uint32_t)nframes; a.nblocks = (uint32_t)nblocks; a.level = level;
     a.checksum = checksum ? 1 : 0;
+    a.window_log = (uint32_t)window_log;
+    if (fast && window_log > B200Z_WINDOW_LOG_MIN) {   // the blocks of the frames larger than one block
+        std::vector<LSpan> sp;
+        for (uint32_t b = 0; b < (uint32_t)nblocks; b++)
+            if (hf[hb[b].frame].src_size > ENC_BLOCK) sp.push_back(LSpan{hb[b].src_off, hf[hb[b].frame].src_off, hb[b].size, hb[b].frame, b, 0});
+        if (!sp.empty()) {
+            if ((e = r.ldm.spans.ensure(sp.size() * sizeof(LSpan)))) return e;
+            CU(c, cudaMemcpyAsync(r.ldm.spans.p, sp.data(), sp.size() * sizeof(LSpan), cudaMemcpyHostToDevice, s));
+            if ((e = compress_ldm(c, r.ldm, a, r.ldm.spans.as<LSpan>(), (uint32_t)sp.size(), (uint32_t)nblocks, (uint32_t)window_log, 0, s))) return e;
+        }
+    }
     const bool prof = (c->flags & B200Z_FLAG_PROFILE) != 0;
     if (prof) CU(c, cudaEventRecord(r.ev[0], s));
     for (int st = 0; st < kCompressStages; st++) {
@@ -3381,17 +3454,22 @@ struct b200z_frame_compressor {
     int device = 0;
     int level = B200Z_LEVEL_FASTEST;
     bool checksum = true;
+    uint32_t window_log = B200Z_WINDOW_LOG_MIN;
     uint64_t chunk = 64ull << 20;   // bytes per chunk, a multiple of ENC_BLOCK
     std::vector<uint8_t> raw;       // Uncompressed: one chunk's part of the frame
     // Fastest, allocated by its first compress (b200z_frame_compressor_free synchronises the copy streams before any of these is
-    // released).  desc: the chunk's CFrame, its CBlocks, then its b200z_compress_result; d_in: the previous chunk's last ENC_WINDOW
-    // bytes, then the chunk
+    // released).  desc: the chunk's CFrame, its CBlocks, its long-match spans, then its b200z_compress_result; d_in: the last
+    // `hist` bytes before the chunk (ENC_WINDOW, or 2^window_log + LDM_MARGIN with long matches), then the chunk
     PipeSlots p;
     CompressStaging stage;                    // shared: the kernels run in order on one stream
-    bool ready = false;
+    LdmBufs ldm;                              // shared, sized for the density bound of the spans
+    uint64_t hist = 0;                        // what the buffers were prepared for (0: not yet)
     uint32_t chunk_blocks() const { return (uint32_t)(chunk / ENC_BLOCK); }
+    uint64_t hist_for(uint32_t wl) const { return wl > B200Z_WINDOW_LOG_MIN ? (1ull << wl) + LDM_MARGIN : ENC_WINDOW; }
+    uint32_t max_spans() const { return (uint32_t)((hist + ENC_BLOCK - 1) / ENC_BLOCK) + chunk_blocks(); }
     size_t chunk_bound() const { return chunk + 3ull * chunk_blocks(); }   // the chunk's blocks, packed, at most
-    size_t res_off() const { return sizeof(CFrame) + (size_t)chunk_blocks() * sizeof(CBlock); }
+    size_t span_off() const { return sizeof(CFrame) + (size_t)chunk_blocks() * sizeof(CBlock); }
+    size_t res_off() const { return span_off() + (hist > ENC_WINDOW ? (size_t)max_spans() * sizeof(LSpan) : 0); }
     size_t desc_bytes() const { return res_off() + sizeof(b200z_compress_result); }
 };
 
@@ -3414,7 +3492,7 @@ extern "C" int b200z_frame_compressor_new(b200z_ctx *c, int level, int checksum,
 }
 extern "C" void b200z_frame_compressor_free(b200z_frame_compressor *fc) {
     if (!fc) return;
-    if (fc->ready) {
+    if (fc->hist) {
         cudaSetDevice(fc->device);
         fc->p.drain(nullptr);
     }
@@ -3426,6 +3504,12 @@ extern "C" int b200z_frame_compressor_set_compression_level(b200z_frame_compress
     return 0;
 }
 extern "C" int b200z_frame_compressor_compression_level(const b200z_frame_compressor *fc) { return fc ? fc->level : B200Z_LEVEL_FASTEST; }
+extern "C" int b200z_frame_compressor_set_window_log(b200z_frame_compressor *fc, int window_log) {
+    if (!fc || window_log < B200Z_WINDOW_LOG_MIN || window_log > B200Z_WINDOW_LOG_MAX) return B200Z_ERR_INVALID_ARGUMENT;
+    fc->window_log = (uint32_t)window_log;
+    return 0;
+}
+extern "C" int b200z_frame_compressor_window_log(const b200z_frame_compressor *fc) { return fc ? (int)fc->window_log : B200Z_WINDOW_LOG_MIN; }
 
 // reads up to `cap` bytes, stopping at the first read that returns 0 (*eof; the reference stops there too); false on a read
 // error (< 0, or more than was asked for)
@@ -3451,11 +3535,11 @@ static bool fc_write(b200z_write_fn wr, void *wu, const uint8_t *p, size_t n) { 
     return true;
 }
 static void fc_le(uint8_t *p, uint64_t v, int n) { for (int i = 0; i < n; i++) p[i] = (uint8_t)(v >> (8 * i)); }
-// the frame header (frame_compressor.rs:144-151): no Frame_Content_Size, Single_Segment 0, a 128 KiB window
-static void fc_header(uint8_t *dst, bool checksum) {
+// the frame header (frame_compressor.rs:144-151): no Frame_Content_Size, Single_Segment 0, a 2^window_log window (128 KiB by default)
+static void fc_header(uint8_t *dst, bool checksum, uint32_t window_log) {
     fc_le(dst, 0xFD2FB528u, 4);
     dst[4] = checksum ? 0x04 : 0x00;
-    dst[5] = 0x38;
+    dst[5] = (uint8_t)((window_log - 10) << 3);
 }
 // the end of the frame after its last chunk: the empty last Raw block when the source ended on a block boundary (the reference's
 // uncompressed_data.is_empty() branch, :175-186), then the checksum (:215-223).  Returns the bytes written at dst.
@@ -3491,7 +3575,7 @@ static int fc_compress_raw(b200z_frame_compressor *fc, b200z_read_fn rd, void *r
             r.raw_blocks++;
         }
         uint8_t *start = body;
-        if (k == 0) { start -= FC_HEADER; fc_header(start, fc->checksum); }
+        if (k == 0) { start -= FC_HEADER; fc_header(start, fc->checksum, B200Z_WINDOW_LOG_MIN); }
         if (eof) len += fc_trailer(body + len, n == 0, fc->checksum, h, r);
         const size_t w = (size_t)(body + len - start);
         if (!fc_write(wr, wu, start, w)) return fc_panic(c, "FrameCompressor::compress: the drain's write failed");
@@ -3500,20 +3584,32 @@ static int fc_compress_raw(b200z_frame_compressor *fc, b200z_read_fn rd, void *r
     }
 }
 
+// the buffers for the compressor's window_log: kept while a later compress needs no more history
 static int fc_prepare(b200z_frame_compressor *fc) {
-    if (fc->ready) return 0;
+    if (fc->hist >= fc->hist_for(fc->window_log)) return 0;
     b200z_ctx *c = fc->ctx;
+    fc->hist = fc->hist_for(fc->window_log);
     const size_t C = fc->chunk, nb = fc->chunk_blocks(), bound = fc->chunk_bound();
     if (fc->p.create(c)) return B200Z_ERR_CUDA;
     int e = 0;
     for (int i = 0; i < 2 && !e; i++)
-        if ((e = fc->p.d_in[i].ensure(ENC_WINDOW + C + 16, false)) || (e = fc->p.d_out[i].ensure(bound + 16, false)) ||
+        if ((e = fc->p.d_in[i].ensure(fc->hist + C + 16, false)) || (e = fc->p.d_out[i].ensure(bound + 16, false)) ||
             (e = fc->p.d_desc[i].ensure(fc->desc_bytes(), false)) || (e = fc->p.h_in[i].ensure(C, false)) ||
             (e = fc->p.h_out[i].ensure(FC_HDR_ROOM + bound + FC_TRAILER, false)) || (e = fc->p.h_desc[i].ensure(fc->desc_bytes(), false)))
             break;
     if (!e) e = fc->stage.ensure(nb, false);
-    if (e) { c->err = "FrameCompressor: out of memory for chunks of " + std::to_string(C) + " bytes"; return e; }
-    fc->ready = true;
+    if (!e && fc->hist > ENC_WINDOW) {
+        const uint32_t ns = fc->max_spans();
+        if (!(e = fc->ldm.ensure(ns * LDM_SPAN_CAP, false)) && !(e = fc->ldm.tcount.ensure((size_t)ns * LDM_THREADS * 4, false)) &&
+            !(e = fc->ldm.scount.ensure((ns + 1) * 4, false)) &&
+            !(e = fc->ldm.off.ensure(nb * 4, false)))
+            e = fc->ldm.cnt.ensure(nb * 4, false);
+    }
+    if (e) {
+        fc->hist = 0;
+        c->err = "FrameCompressor: out of memory for chunks of " + std::to_string(C) + " bytes";
+        return e;
+    }
     return 0;
 }
 
@@ -3525,7 +3621,7 @@ static int fc_compress_fast(b200z_frame_compressor *fc, b200z_read_fn rd, void *
                             b200z_compress_result &r) {
     b200z_ctx *c = fc->ctx;
     if (int e = fc_prepare(fc)) return e;
-    const uint64_t C = fc->chunk;
+    const uint64_t C = fc->chunk, H = fc->hist_for(fc->window_log);
     cudaStream_t ks = c->stream;
     size_t n[2] = {0, 0};               // the chunk read into h_in[s]
     bool eof[2] = {false, false};
@@ -3534,16 +3630,26 @@ static int fc_compress_fast(b200z_frame_compressor *fc, b200z_read_fn rd, void *
         const uint32_t m = (uint32_t)((n[s] + ENC_BLOCK - 1) / ENC_BLOCK);
         CFrame *hf = fc->p.h_desc[s].as<CFrame>();
         CBlock *hb = reinterpret_cast<CBlock *>(hf + 1);
-        *hf = CFrame{ENC_WINDOW, n[s], 0, 0, m};
+        *hf = CFrame{H, n[s], 0, 0, m};
         for (uint32_t i = 0; i < m; i++) {
             const uint64_t at = (uint64_t)i * ENC_BLOCK;
-            hb[i] = CBlock{ENC_WINDOW + at, (uint32_t)std::min<uint64_t>(ENC_BLOCK, n[s] - at), (uint32_t)std::min<uint64_t>(k * C + at, ENC_WINDOW), 0, 0};
+            hb[i] = CBlock{H + at, (uint32_t)std::min<uint64_t>(ENC_BLOCK, n[s] - at), (uint32_t)std::min<uint64_t>(k * C + at, ENC_WINDOW), 0, 0};
+        }
+        // long matches: the kept history (from the frame's start while it is shorter than H) and the chunk's blocks, as spans of at
+        // most one block in position order; none until the frame has more than one block
+        const uint64_t vlo = k * C >= H ? 0 : H - k * C;
+        LSpan *hs = reinterpret_cast<LSpan *>(fc->p.h_desc[s].as<uint8_t>() + fc->span_off());
+        uint32_t ns = 0;
+        if (H > ENC_WINDOW && k * C + n[s] > ENC_BLOCK) {
+            for (uint64_t o = vlo; o < H; o += ENC_BLOCK) hs[ns++] = LSpan{o, vlo, (uint32_t)std::min<uint64_t>(ENC_BLOCK, H - o), 0, LDM_NO_BLOCK, 0};
+            for (uint32_t i = 0; i < m; i++) hs[ns++] = LSpan{hb[i].src_off, vlo, hb[i].size, 0, i, 0};
         }
         uint8_t *din = fc->p.d_in[s].as<uint8_t>();
         CU(c, cudaStreamWaitEvent(fc->p.s_h2d, fc->p.ev_k[s], 0));   // chunk k - 2's kernels are done with d_in[s] and d_desc[s]
-        if (k) CU(c, cudaMemcpyAsync(din, fc->p.d_in[s ^ 1].as<uint8_t>() + C, ENC_WINDOW, cudaMemcpyDeviceToDevice, fc->p.s_h2d));
-        CU(c, cudaMemcpyAsync(din + ENC_WINDOW, fc->p.h_in[s].p, n[s], cudaMemcpyHostToDevice, fc->p.s_h2d));
+        if (k) CU(c, cudaMemcpyAsync(din, fc->p.d_in[s ^ 1].as<uint8_t>() + C, H, cudaMemcpyDeviceToDevice, fc->p.s_h2d));
+        CU(c, cudaMemcpyAsync(din + H, fc->p.h_in[s].p, n[s], cudaMemcpyHostToDevice, fc->p.s_h2d));
         CU(c, cudaMemcpyAsync(fc->p.d_desc[s].p, hf, sizeof(CFrame) + m * sizeof(CBlock), cudaMemcpyHostToDevice, fc->p.s_h2d));
+        if (ns) CU(c, cudaMemcpyAsync(fc->p.d_desc[s].as<uint8_t>() + fc->span_off(), hs, ns * sizeof(LSpan), cudaMemcpyHostToDevice, fc->p.s_h2d));
         CU(c, cudaEventRecord(fc->p.ev_h2d[s], fc->p.s_h2d));
         CU(c, cudaStreamWaitEvent(ks, fc->p.ev_h2d[s], 0));
         CompressArgs a{};
@@ -3553,6 +3659,10 @@ static int fc_compress_fast(b200z_frame_compressor *fc, b200z_read_fn rd, void *
         a.input = din; a.output = fc->p.d_out[s].as<uint8_t>();
         fc->stage.bind(a);
         a.nframes = 1; a.nblocks = m; a.level = fc->level;   // Fastest or LAZY
+        if (ns)
+            if (int le = compress_ldm(c, fc->ldm, a, reinterpret_cast<const LSpan *>(fc->p.d_desc[s].as<uint8_t>() + fc->span_off()), ns, m,
+                                      fc->window_log, ns * LDM_SPAN_CAP, ks))
+                return le;
         if (int le = launch_compress_chunk(a, ks, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_cmatch / k_cenc / k_cassemble<true>");
         CU(c, cudaEventRecord(fc->p.ev_k[s], ks));
         CU(c, cudaStreamWaitEvent(fc->p.s_d2h, fc->p.ev_k[s], 0));
@@ -3571,7 +3681,7 @@ static int fc_compress_fast(b200z_frame_compressor *fc, b200z_read_fn rd, void *
             r.blocks += cr.blocks; r.raw_blocks += cr.raw_blocks; r.rle_blocks += cr.rle_blocks;
         }
         uint8_t *start = body;
-        if (k == 0) { start -= FC_HEADER; fc_header(start, fc->checksum); }
+        if (k == 0) { start -= FC_HEADER; fc_header(start, fc->checksum, fc->window_log); }
         if (final) len += fc_trailer(body + len, out_n[s] % ENC_BLOCK == 0, fc->checksum, h, r);
         const size_t w = (size_t)(body + len - start);
         if (!fc_write(wr, wu, start, w)) return fc_panic(c, "FrameCompressor::compress: the drain's write failed");
@@ -3602,6 +3712,10 @@ extern "C" int b200z_frame_compressor_compress(b200z_frame_compressor *fc, b200z
     if (!fc || !rd || !wr) return B200Z_ERR_INVALID_ARGUMENT;
     b200z_ctx *c = fc->ctx;
     if (fc->level >= 2 && fc->level <= 4) return fc_panic(c, "FrameCompressor::compress: compression levels above Fastest are unimplemented!() in the reference");
+    if (fc->level == B200Z_LEVEL_UNCOMPRESSED && fc->window_log != B200Z_WINDOW_LOG_MIN) {
+        c->err = "FrameCompressor::compress: window_log above 17 at level Uncompressed";
+        return B200Z_ERR_INVALID_ARGUMENT;
+    }
     b200z_compress_result r{};
     XXH64State h;
     h.reset();

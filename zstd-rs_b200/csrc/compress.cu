@@ -1,7 +1,8 @@
 // compress.cu -- sm_90a kernels of the batch compressor (ruzstd's encoding::compress at CompressionLevel::Fastest).
 //
 //   k_cmatch    : one CTA per 128 KiB block: greedy LZ77 parse into literals + sequences (two-table parallel parse)
-//                 (<DICT, true>: the LAZY level's parse, an extension: K-way tables, repeat candidates, a lazy choice)
+//                 (<DICT, true>: the LAZY level's parse, an extension: K-way tables, repeat candidates, a lazy choice;
+//                  <DICT, LAZY, true>: with the long-distance matches of ldm.cu forced into the parse, window_log > 17)
 //   k_cenc      : one warp per block: Huffman literals, FSE sequences, the Raw / RLE / Compressed decision (encode.cuh)
 //                 (<TABLES, true>: LAZY, repeat-offset codes within each block first)
 //   k_cxxh64    : content checksum of every frame's input (xxh64.cuh; four serial chains per frame)
@@ -95,21 +96,44 @@ __device__ __forceinline__ uint32_t extend_match(const uint8_t *src, uint32_t qj
     return min(ml, lim);
 }
 
+// long-distance matches: the forced pieces of one segment, in order -- the block's forced matches (ldm.cu) clipped to [s, e),
+// pieces shorter than ENC_MIN_MATCH left to the regular parse.  has: a piece [cs, ce) at offset off is next.
+struct LCursor {
+    const LForced *f;
+    uint32_t k, n, s, e, cs, ce, off;
+    bool has;
+    __device__ __forceinline__ void next() {
+        has = false;
+        while (k < n) {
+            const LForced x = f[k++];
+            if (x.start >= e) { k = n; break; }
+            cs = max(x.start, s);
+            ce = min(x.start + x.len, e);
+            if (ce >= cs + ENC_MIN_MATCH) { off = x.off; has = true; break; }
+        }
+    }
+};
+
 // LAZY: one warp's parse of segment [s, e) (see k_cmatch); writes the segment's sequences and literals to its staging and its
 // counts to *nseq_out, *nlit_out, *trail_out
-template <bool DICT>
+// (LONG: the gaps between the segment's forced pieces, each piece one sequence, as in k_cmatch)
+template <bool DICT, bool LONG>
 __device__ __forceinline__ void cmatch_lazy(const CBlock &blk, const uint8_t *src, uint32_t s, uint32_t e, const uint32_t *t1, uint32_t *tab,
                                             int32_t base, uint32_t lane, const uint8_t *dict, const uint32_t *dtab, uint32_t dict_len,
-                                            SeqRec *stage, uint8_t *lstage, uint32_t *nseq_out, uint32_t *nlit_out, uint32_t *trail_out) {
+                                            SeqRec *stage, uint8_t *lstage, uint32_t *nseq_out, uint32_t *nlit_out, uint32_t *trail_out,
+                                            LCursor &lc) {
     uint32_t p = s, anchor = s, nseq = 0, nlit = 0;
     uint32_t r0 = 0, r1 = 0, r2 = 0;   // the segment's three most recent distinct offsets (0: none yet)
-    while (p + ENC_MIN_MATCH <= e) {
+    uint32_t ee = e;                   // where the regular parse stops: the segment's end, or the next forced piece
+    if constexpr (LONG) { lc.next(); if (lc.has) ee = lc.cs; }
+    while (true) {   // once without LONG; with it, once per forced piece and once after the last (the body keeps its indentation)
+    while (p + ENC_MIN_MATCH <= ee) {
         const uint32_t q = p + lane;
-        const bool valid = q + ENC_MIN_MATCH <= e;
+        const bool valid = q + ENC_MIN_MATCH <= ee;
         int32_t gain = INT_MIN;   // INT_MIN: no candidate of >= 5 bytes
-        uint32_t len = 0, cand = 0, xlim = e - q;
+        uint32_t len = 0, cand = 0, xlim = ee - q;
         if (valid) {
-            const uint32_t lim = min(LZ_CAP, e - q), fpos = blk.back + q;
+            const uint32_t lim = min(LZ_CAP, ee - q), fpos = blk.back + q;
             auto take = [&](uint32_t o, const uint8_t *ref, uint32_t l, int32_t cost) {
                 const int32_t g = 4 * (int32_t)l - cost;
                 if (l >= ENC_MIN_MATCH && g > gain) { gain = g; len = l; cand = o; return true; }
@@ -153,7 +177,7 @@ __device__ __forceinline__ void cmatch_lazy(const CBlock &blk, const uint8_t *sr
         const uint32_t qj = p + win, off = __shfl_sync(0xffffffffu, cand, win);
         uint32_t ml = __shfl_sync(0xffffffffu, len, win);
         const uint32_t lim = __shfl_sync(0xffffffffu, xlim, win);
-        if (ml == LZ_CAP) ml = extend_match<DICT>(src, qj, off, ml, DICT ? lim : e - qj, blk.back, dict, dict_len, lane);
+        if (ml == LZ_CAP) ml = extend_match<DICT>(src, qj, off, ml, DICT ? lim : ee - qj, blk.back, dict, dict_len, lane);
         for (uint32_t i = anchor + lane; i < qj; i += 32) lstage[nlit + i - anchor] = __ldg(src + i);
         if (lane == 0) stage[nseq] = SeqRec{qj - anchor, ml, off};
         nlit += qj - anchor;
@@ -162,6 +186,22 @@ __device__ __forceinline__ void cmatch_lazy(const CBlock &blk, const uint8_t *sr
         if (off == r1) { r1 = r0; r0 = off; }   // off moves to the front
         else if (off != r0) { r2 = r1; r1 = r0; r0 = off; }
         __syncwarp();
+    }
+    if constexpr (!LONG) break;
+    else {
+        if (!lc.has) break;
+        const uint32_t qj = lc.cs, ml = lc.ce - lc.cs, off = lc.off;   // the forced piece, taken as any match is
+        for (uint32_t i = anchor + lane; i < qj; i += 32) lstage[nlit + i - anchor] = __ldg(src + i);
+        if (lane == 0) stage[nseq] = SeqRec{qj - anchor, ml, off};
+        nlit += qj - anchor;
+        nseq++;
+        anchor = p = qj + ml;
+        if (off == r1) { r1 = r0; r0 = off; }
+        else if (off != r0) { r2 = r1; r1 = r0; r0 = off; }
+        lc.next();
+        ee = lc.has ? lc.cs : e;
+        __syncwarp();
+    }
     }
     for (uint32_t i = anchor + lane; i < e; i += 32) lstage[nlit + i - anchor] = __ldg(src + i);
     if (lane == 0) { *nseq_out = nseq; *nlit_out = nlit + (e - anchor); *trail_out = e - anchor; }
@@ -184,11 +224,15 @@ __device__ __forceinline__ void cmatch_lazy(const CBlock &blk, const uint8_t *sr
 // (a repeat costs 0), and the first lane with a match competes with the next LZ_DEPTH lanes at LZ_LANE_COST per byte of delay.
 // tests/clazy.py states it rule by rule.
 // ------------------------------------------------------------------------------------------------------------
-template <bool DICT, bool LAZY>
+// LONG (window_log > 17, ldm.cu): each segment's forced pieces (LCursor) are taken as sequences, with the literals since the last
+// match; the regular parse runs in the gaps between them exactly as it runs up to a segment's end, so no regular match crosses
+// the next forced start.  tests/cldm.py states it.
+template <bool DICT, bool LAZY, bool LONG = false>
 __global__ void __launch_bounds__(CM_THREADS, 1)
 k_cmatch(const CBlock *__restrict__ blocks, const uint8_t *__restrict__ input, uint8_t *__restrict__ lit_stage, SeqRec *__restrict__ seq_stage,
          uint8_t *__restrict__ lits, SeqRec *__restrict__ seqs, CBlockInfo *__restrict__ info, const uint8_t *__restrict__ dict,
-         const uint32_t *__restrict__ dtab, uint32_t dict_len) {
+         const uint32_t *__restrict__ dtab, uint32_t dict_len, const LForced *__restrict__ lforced = nullptr,
+         const uint32_t *__restrict__ lf_off = nullptr, const uint32_t *__restrict__ lf_cnt = nullptr) {
     extern __shared__ __align__(16) uint8_t smem_cm[];
     uint32_t *t1 = reinterpret_cast<uint32_t *>(smem_cm);
     int32_t *tp_all = reinterpret_cast<int32_t *>(smem_cm + (4u << CM_T1_LOG));
@@ -217,6 +261,8 @@ k_cmatch(const CBlock *__restrict__ blocks, const uint8_t *__restrict__ input, u
     int32_t *tp = tp_all + (w << CM_TP_LOG);
     const uint32_t seglen = (n + CM_WARPS - 1) / CM_WARPS;
     const uint32_t s = min(n, w * seglen), e = min(n, s + seglen);
+    LCursor lc{};
+    if constexpr (LONG) lc = LCursor{lforced + lf_off[b], 0, lf_cnt[b], s, e, 0, 0, 0, false};
     if constexpr (LAZY) {
         SeqRec *stage = seq_stage + ((size_t)b * CM_WARPS + w) * CSEG_SEQS;
         uint8_t *lstage = lit_stage + (size_t)b * ENC_BLOCK + s;
@@ -225,7 +271,7 @@ k_cmatch(const CBlock *__restrict__ blocks, const uint8_t *__restrict__ input, u
         const int32_t seed_lo = max(base, -(int32_t)blk.back), seed_hi = min((int32_t)s, (int32_t)n - (int32_t)ENC_MIN_MATCH + 1);
         for (int32_t q0 = seed_lo; q0 < seed_hi; q0 += 32) lz_insert(tab, src, q0, q0 + (int32_t)lane < seed_hi, base, lane);
         __syncthreads();
-        cmatch_lazy<DICT>(blk, src, s, e, t1, tab, base, lane, dict, dtab, dict_len, stage, lstage, s_nseq + w, s_nlit + w, s_trail + w);
+        cmatch_lazy<DICT, LONG>(blk, src, s, e, t1, tab, base, lane, dict, dtab, dict_len, stage, lstage, s_nseq + w, s_nlit + w, s_trail + w, lc);
     } else {
         const int32_t seed_lo = max((int32_t)s - (int32_t)CM_SEED, -(int32_t)min(blk.back, CM_SEED));
         for (int32_t q = seed_lo + (int32_t)lane; q < (int32_t)s && q + (int32_t)ENC_MIN_MATCH <= (int32_t)n; q += 32)   // inside the frame
@@ -234,12 +280,15 @@ k_cmatch(const CBlock *__restrict__ blocks, const uint8_t *__restrict__ input, u
         SeqRec *stage = seq_stage + ((size_t)b * CM_WARPS + w) * CSEG_SEQS;
         uint8_t *lstage = lit_stage + (size_t)b * ENC_BLOCK + s;
         uint32_t p = s, anchor = s, nseq = 0, nlit = 0;
-        while (p + ENC_MIN_MATCH <= e) {
+        uint32_t ee = e;   // where the regular parse stops: the segment's end, or the next forced piece
+        if constexpr (LONG) { lc.next(); if (lc.has) ee = lc.cs; }
+        while (true) {   // as in cmatch_lazy
+        while (p + ENC_MIN_MATCH <= ee) {
             const uint32_t q = p + lane;
-            const bool valid = q + ENC_MIN_MATCH <= e;
-            uint32_t len = 0, cand = 0, h2 = 0, xlim = e - q;   // xlim: how far the match may be extended
+            const bool valid = q + ENC_MIN_MATCH <= ee;
+            uint32_t len = 0, cand = 0, h2 = 0, xlim = ee - q;   // xlim: how far the match may be extended
             if (valid) {
-                const uint32_t lim = min(CM_CAP, e - q);
+                const uint32_t lim = min(CM_CAP, ee - q);
                 const uint32_t c1 = t1[hash5(src + q, CM_T1_LOG)];
                 h2 = hash5(src + q, CM_TP_LOG);
                 const int32_t c2 = tp[h2];
@@ -269,7 +318,7 @@ k_cmatch(const CBlock *__restrict__ blocks, const uint8_t *__restrict__ input, u
             const uint32_t qj = p + j, off = __shfl_sync(0xffffffffu, cand, j);
             uint32_t ml = __shfl_sync(0xffffffffu, len, j);
             if (ml == CM_CAP) {   // extend the chosen match 32 bytes at a time
-                const uint32_t lim = DICT ? __shfl_sync(0xffffffffu, xlim, j) : e - qj;
+                const uint32_t lim = DICT ? __shfl_sync(0xffffffffu, xlim, j) : ee - qj;
                 const uint32_t fpos = blk.back + qj;   // an offset beyond the frame's start points into the dictionary
                 const uint8_t *ref = DICT && off > fpos ? dict + dict_len - (off - fpos) : src + qj - off;
                 while (ml < lim) {
@@ -287,6 +336,20 @@ k_cmatch(const CBlock *__restrict__ blocks, const uint8_t *__restrict__ input, u
             nseq++;
             anchor = p = qj + ml;
             __syncwarp();
+        }
+        if constexpr (!LONG) break;
+        else {
+            if (!lc.has) break;
+            const uint32_t qj = lc.cs;   // the forced piece
+            for (uint32_t i = anchor + lane; i < qj; i += 32) lstage[nlit + i - anchor] = __ldg(src + i);
+            if (lane == 0) stage[nseq] = SeqRec{qj - anchor, lc.ce - qj, lc.off};
+            nlit += qj - anchor;
+            nseq++;
+            anchor = p = lc.ce;
+            lc.next();
+            ee = lc.has ? lc.cs : e;
+            __syncwarp();
+        }
         }
         for (uint32_t i = anchor + lane; i < e; i += 32) lstage[nlit + i - anchor] = __ldg(src + i);
         if (lane == 0) { s_nseq[w] = nseq; s_nlit[w] = nlit + (e - anchor); s_trail[w] = e - anchor; }
@@ -390,7 +453,7 @@ template <bool STREAM>
 __global__ void __launch_bounds__(256)
 k_cassemble(const CFrame *__restrict__ frames, const CBlock *__restrict__ blocks, const CBlockInfo *__restrict__ res, const uint8_t *__restrict__ enc,
             const uint8_t *__restrict__ input, const uint64_t *__restrict__ csum, uint8_t *__restrict__ output, b200z_compress_result *__restrict__ results,
-            int level, int checksum, uint32_t dict_id) {
+            int level, int checksum, uint32_t dict_id, uint32_t window_log) {
     __shared__ uint64_t s_red[3][8];
     const uint32_t b = blockIdx.x, tid = threadIdx.x;
     const CBlock blk = blocks[b];
@@ -422,7 +485,8 @@ k_cassemble(const CFrame *__restrict__ frames, const CBlock *__restrict__ blocks
     if (tid == 0) {
         const uint32_t bh = (last ? 1u : 0u) | (type << 1) | ((type == 1 ? blk.size : csize) << 3);
         dst[0] = (uint8_t)bh; dst[1] = (uint8_t)(bh >> 8); dst[2] = (uint8_t)(bh >> 16);
-        if (!STREAM && b == fr.first_block) write_frame_header(output + fr.dst_off, fr.src_size, checksum != 0, dict_id);
+        if (!STREAM && b == fr.first_block)
+            write_frame_header(output + fr.dst_off, fr.src_size, checksum != 0, dict_id, frame_window_log(fr.src_size, window_log));
     }
     for (uint32_t i = tid; i < csize; i += 256) dst[3 + i] = from[i];
     if (end && tid == 0) {
@@ -495,6 +559,10 @@ int init_compress_kernels() {
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cmatch<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CM_SMEM);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cmatch<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LZ_SMEM);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cmatch<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LZ_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cmatch<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CM_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cmatch<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CM_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cmatch<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LZ_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cmatch<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LZ_SMEM);
     return (int)e;
 }
 
@@ -515,7 +583,12 @@ int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s, uint
     switch (stage) {
     case 0:
         if (!a.level || !a.nblocks) return 0;
-        if (lazy) {
+        if (a.lf_cnt) {
+            const uint32_t smem = lazy ? LZ_SMEM : CM_SMEM;
+            auto k = lazy ? (a.dtab ? k_cmatch<true, true, true> : k_cmatch<false, true, true>) : (a.dtab ? k_cmatch<true, false, true> : k_cmatch<false, false, true>);
+            k<<<a.nblocks, CM_THREADS, smem, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, a.dict, a.dtab, a.dict_len,
+                                                  a.lforced, a.lf_off, a.lf_cnt);
+        } else if (lazy) {
             if (a.dtab) k_cmatch<true, true><<<a.nblocks, CM_THREADS, LZ_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, a.dict, a.dtab, a.dict_len);
             else k_cmatch<false, true><<<a.nblocks, CM_THREADS, LZ_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, nullptr, nullptr, 0);
         } else if (a.dtab) k_cmatch<true, false><<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, a.dict, a.dtab, a.dict_len);
@@ -530,7 +603,7 @@ int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s, uint
         else k_cenc<false, false><<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res, nullptr, nullptr);
         break;
     case 2: if (!a.checksum || !a.nframes) return 0; k_cxxh64<<<cdiv_u((uint64_t)a.nframes * 4, 128), 128, 0, s>>>(a.frames, a.input, a.csum, a.nframes); break;
-    case 3: if (!a.nblocks) return 0; k_cassemble<false><<<a.nblocks, 256, 0, s>>>(a.frames, a.blocks, a.res, a.enc, a.input, a.csum, a.output, a.results, a.level, a.checksum, a.dict_id); break;
+    case 3: if (!a.nblocks) return 0; k_cassemble<false><<<a.nblocks, 256, 0, s>>>(a.frames, a.blocks, a.res, a.enc, a.input, a.csum, a.output, a.results, a.level, a.checksum, a.dict_id, a.window_log); break;
     default: return (int)cudaErrorInvalidValue;
     }
     const int e = (int)cudaGetLastError();
@@ -542,7 +615,7 @@ int launch_compress_chunk(const CompressArgs &a, cudaStream_t s, uint64_t *launc
     if (!a.nblocks) return 0;
     for (int st = 0; st < 2; st++)
         if (int e = launch_compress_stage(a, st, s, launched)) return e;
-    k_cassemble<true><<<a.nblocks, 256, 0, s>>>(a.frames, a.blocks, a.res, a.enc, a.input, nullptr, a.output, a.results, a.level, 0, 0);
+    k_cassemble<true><<<a.nblocks, 256, 0, s>>>(a.frames, a.blocks, a.res, a.enc, a.input, nullptr, a.output, a.results, a.level, 0, 0, 0);
     const int e = (int)cudaGetLastError();
     if (!e) ++*launched;
     return e;

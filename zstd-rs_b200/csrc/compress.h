@@ -27,6 +27,10 @@ struct CBlockInfo {    // k_cmatch: literals, sequences, type 1 when all bytes a
     uint32_t nlit, nseq, type, csize;
 };
 
+struct LForced {       // a forced match of a block: [start, start + len) at offset off, block-relative
+    uint32_t start, len, off;
+};
+
 struct CompressArgs {
     const CFrame *frames;
     const CBlock *blocks;
@@ -48,7 +52,46 @@ struct CompressArgs {
     const uint32_t *dtab;   // [1 << CD_LOG] from k_cdict
     uint32_t dict_len, dict_id;
     const EncDict *etab;    // a formatted dictionary's tables for the frames' first blocks (B200Z_FLAG_DICT_TABLES), else null
+    // long-distance matches (window_log > 17; ldm.cu): block b's forced matches are lforced[lf_off[b], + lf_cnt[b]); lf_cnt null: none,
+    // and k_cmatch is the plain kernel.  window_log (0 counts as 17) sets each frame's Window_Descriptor
+    const LForced *lforced;
+    const uint32_t *lf_off, *lf_cnt;
+    uint32_t window_log;
 };
+
+// ---- long-distance matches (ldm.cu; DESIGN.md section 4.11, tests/cldm.py)
+constexpr uint32_t LDM_LEN = 64;          // bytes hashed at an anchor (the 64 ending at it), verified, and the least a kept match holds
+constexpr uint32_t LDM_MASK_SHIFT = 57;   // a position passes when its gear hash's top 7 bits are 0: about 1 in 128
+constexpr uint32_t LDM_QUIET = 15;        // an anchor passes and no position in the 15 before it does: at most 1 anchor in 16
+constexpr uint32_t LDM_MARGIN = 128;      // bytes before the 2^window_log a stream chunk keeps: >= LDM_LEN - 1 + LDM_QUIET
+constexpr uint32_t LDM_THREADS = 256, LDM_SPAN = ENC_BLOCK / LDM_THREADS;   // k_lanchor: positions per thread
+constexpr uint32_t LDM_SPAN_CAP = LDM_THREADS * (LDM_SPAN / (LDM_QUIET + 1));   // the most anchors a span can hold
+constexpr uint32_t LDM_TILE = 4096;       // pairs per CTA of the key sort
+constexpr uint32_t LDM_NO_BLOCK = 0xffffffffu;
+struct LSpan {         // up to ENC_BLOCK bytes whose anchors k_lanchor lists: a block of a long frame, or history before a stream chunk
+    uint64_t off;      // in `input`
+    uint64_t lo;       // the first byte of its frame in `input` (a stream chunk: of the history kept before it)
+    uint32_t size, frame;
+    uint32_t block;    // its CBlock, whose forced matches k_lblock writes; LDM_NO_BLOCK for history
+    uint32_t pad;
+};
+struct LdmArgs {
+    const uint8_t *input;
+    const LSpan *spans;        // [nspans], in input order within each frame, the frames in submission order
+    uint32_t nspans, window_log;
+    uint32_t *tcount;          // [nspans * LDM_THREADS]: anchors per k_lanchor thread
+    uint32_t *scount;          // [nspans + 1]: anchors per span, then their exclusive prefix sum and the total
+    uint32_t cap;              // anchors the buffers below hold: the total, or (stream) the density bound; grids are sized by it
+    uint32_t *keys[2], *vals[2], *hist;   // the sort's ping-pong pairs [cap] and its digit counts [256 * ceil(cap / LDM_TILE) + 1]
+    uint64_t *apos;            // [cap] input offset of each anchor
+    uint32_t *aframe, *cand;   // [cap] its frame, its candidate offset (0: none)
+    LForced *forced;           // [cap]
+    uint32_t *lf_off, *lf_cnt; // [blocks]: each span's CBlock's share of `forced`; lf_cnt zeroed by the host
+};
+// k_lanchor<false> and k_lscan: tcount, scount and the total; adds the kernels it enqueued to *launched
+int launch_ldm_count(const LdmArgs &a, cudaStream_t s, uint64_t *launched);
+// with the buffers sized for a.cap >= the total: k_lanchor<true>, the sort, k_lcand and k_lblock
+int launch_ldm_match(const LdmArgs &a, cudaStream_t s, uint64_t *launched);
 
 // the dictionary match table: 5-byte hash of a position in the dictionary's last ENC_WINDOW bytes -> that position + 1 (0 = none)
 constexpr uint32_t CD_LOG = 17;

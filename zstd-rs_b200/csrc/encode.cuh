@@ -544,18 +544,26 @@ B200Z_HDN inline uint32_t encode_block(EncScratch &s, const uint8_t *lits, uint3
     return s.total;
 }
 
-// frame header for a frame of `n` bytes: Single_Segment = 0, 128 KiB window, the dictionary ID in the smallest field that holds
+// frame header for a frame of `n` bytes: Single_Segment = 0, a 2^wlog window (128 KiB unless long matches are on), the dictionary ID in the smallest field that holds
 // it (none for ID 0, as ruzstd's minify_val sizes it, encoding/frame_header.rs), Frame_Content_Size in the smallest legal field
 B200Z_HD uint32_t dict_id_field_size(uint32_t dict_id) { return dict_id == 0 ? 0 : dict_id <= 0xffu ? 1 : dict_id <= 0xffffu ? 2 : 4; }
 B200Z_HD uint32_t frame_header_size(uint64_t n, uint32_t dict_id) {
     return 6 + dict_id_field_size(dict_id) + ((n >= 256 && n <= 65791) ? 2 : (n >> 32) ? 8 : 4);
 }
-B200Z_HD uint32_t write_frame_header(uint8_t *dst, uint64_t n, bool checksum, uint32_t dict_id) {
+// the Window_Descriptor's exponent of a frame of n bytes compressed at window_log (0 counts as 17): min(window_log,
+// max(17, ceil(log2 n))), so a frame never advertises more window than its content can use
+B200Z_HD uint32_t frame_window_log(uint64_t n, uint32_t window_log) {
+    if (window_log <= 17) return 17;
+    uint32_t c = 17;
+    while (c < window_log && (1ull << c) < n) c++;
+    return c;
+}
+B200Z_HD uint32_t write_frame_header(uint8_t *dst, uint64_t n, bool checksum, uint32_t dict_id, uint32_t wlog = 17) {
     const uint32_t did = dict_id_field_size(dict_id), fcs = frame_header_size(n, dict_id) - 6 - did;
     const uint32_t flag = fcs == 2 ? 1 : fcs == 4 ? 2 : 3;
     put_le(dst, 4, 0, 0xFD2FB528u, 4);
     dst[4] = (uint8_t)((flag << 6) | (checksum ? 4u : 0u) | (did == 4 ? 3u : did));
-    dst[5] = (uint8_t)((17 - 10) << 3);
+    dst[5] = (uint8_t)((wlog - 10) << 3);
     for (uint32_t i = 0; i < did; i++) dst[6 + i] = (uint8_t)(dict_id >> (8 * i));
     const uint64_t v = fcs == 2 ? n - 256 : n;
     for (uint32_t i = 0; i < fcs; i++) dst[6 + did + i] = (uint8_t)(v >> (8 * i));
