@@ -1614,9 +1614,9 @@ struct SdPlanner {
     }
 };
 
-struct SdSlice { const uint8_t *p; size_t len; };
-long sd_slice_read(void *user, uint8_t *buf, size_t n) {
-    SdSlice *s = (SdSlice *)user;
+struct SliceReader { const uint8_t *p; size_t len; };
+long slice_read(void *user, uint8_t *buf, size_t n) {  // impl Read for &[u8]
+    SliceReader *s = (SliceReader *)user;
     const size_t k = std::min(n, s->len);
     if (k) memcpy(buf, s->p, k);
     s->p += k; s->len -= k;
@@ -1679,13 +1679,30 @@ static int sd_get(b200z_ctx *c, uint64_t C, StreamDecodeResources **out) {
     return 0;
 }
 
-static int sd_write(b200z_write_fn wr, void *wu, const uint8_t *p, size_t n, uint64_t *delivered) {   // write_all; false on a write <= 0
+// The stream entries' I/O.  write_all: false on a write <= 0 or one of more than was asked for; *delivered (when given) counts
+// the bytes written.  read_chunk: reads up to `cap` bytes, stopping at the first read that returns 0 (*eof; the reference's
+// FrameCompressor stops there too); false on a read error (< 0, or more than was asked for).  The frame decoder's read_upto /
+// read_exact take a negative read as the end of the source instead, as ruzstd does.
+static bool write_all(b200z_write_fn wr, void *wu, const uint8_t *p, size_t n, uint64_t *delivered) {
     while (n) {
         const long w = wr(wu, p, n);
-        if (w <= 0 || (size_t)w > n) return 0;
-        p += w; n -= (size_t)w; *delivered += (uint64_t)w;
+        if (w <= 0 || (size_t)w > n) return false;
+        p += w; n -= (size_t)w;
+        if (delivered) *delivered += (uint64_t)w;
     }
-    return 1;
+    return true;
+}
+static bool read_chunk(b200z_read_fn rd, void *ru, uint8_t *buf, size_t cap, size_t *n, bool *eof) {
+    size_t got = 0;
+    *eof = false;
+    while (got < cap) {
+        const long r = rd(ru, buf + got, cap - got);
+        if (r < 0 || (size_t)r > cap - got) return false;
+        if (r == 0) { *eof = true; break; }
+        got += (size_t)r;
+    }
+    *n = got;
+    return true;
 }
 
 extern "C" int b200z_decode_all_stream(b200z_ctx *c, b200z_read_fn rd, void *ru, b200z_write_fn wr, void *wu, const b200z_dict *const *dicts, size_t ndicts,
@@ -1817,7 +1834,7 @@ extern "C" int b200z_decode_all_stream(b200z_ctx *c, b200z_read_fn rd, void *ru,
             // the states are back, so this submission's pass is over; the next one keeps running meanwhile
             CU(c, cudaMemcpyAsync(R->h_out.p, R->d_out[s].as<uint8_t>() + T0, len, cudaMemcpyDeviceToHost, R->s_out));
             CU(c, cudaStreamSynchronize(R->s_out));
-            if (!sd_write(wr, wu, R->h_out.as<uint8_t>(), len, &res.delivered)) {
+            if (!write_all(wr, wu, R->h_out.as<uint8_t>(), len, &res.delivered)) {
                 res.all.status = B200Z_ERR_FAILED_TO_DRAIN_DECODEBUFFER; res.all.stage = B200Z_STAGE_DRAIN;
                 res.all.error_offset = p.frames.front().at; res.all.error_frame = p.frames.front().zi;
                 stopped = true;
@@ -1860,12 +1877,12 @@ extern "C" int b200z_decode_all_stream(b200z_ctx *c, b200z_read_fn rd, void *ru,
 extern "C" int b200z_debug_stream_cut(const uint8_t *input, size_t input_len, uint64_t chunk, b200z_stream_cut *cuts, size_t cap, size_t *n,
                                       b200z_stream_cut_end *end) {
     if (!n || !end || (!input && input_len) || (!cuts && cap) || !chunk) return B200Z_ERR_INVALID_ARGUMENT;
-    SdSlice sr{input, input_len};
+    SliceReader sr{input, input_len};
     SdPlanner pl(chunk, nullptr, 0, nullptr, 0);
     static const FseSlot *const fake = reinterpret_cast<const FseSlot *>(16);   // table pointers are never dereferenced here
     pl.carry_huf = reinterpret_cast<const HufSlot *>(16); pl.carry_fse = fake; pl.predef = fake;
     SdSource src;
-    src.rd = sd_slice_read; src.user = &sr; src.cap = (size_t)pl.bnd.buffer();
+    src.rd = slice_read; src.user = &sr; src.cap = (size_t)pl.bnd.buffer();
     std::vector<uint8_t> buf[2] = {std::vector<uint8_t>(src.cap), std::vector<uint8_t>(src.cap)};
     src.buf = buf[0].data();
     Submission sub;
@@ -2238,17 +2255,6 @@ static int fd_submit(b200z_frame_decoder *d, const TableCursor &cur, uint32_t *f
     return 0;
 }
 
-namespace {
-struct SliceReader { const uint8_t *p; size_t len; };
-long slice_read(void *user, uint8_t *buf, size_t n) {  // impl Read for &[u8]
-    SliceReader *s = (SliceReader *)user;
-    size_t k = std::min(n, s->len);
-    if (k) memcpy(buf, s->p, k);
-    s->p += k; s->len -= k;
-    return (long)k;
-}
-}  // namespace
-
 // decode_blocks (frame_decoder.rs:309-377).  `slice` != null selects decode_from_to's trailer rule (:505-516):
 // the checksum is taken only if its 4 bytes are present, otherwise left for the next call.
 static int fd_decode_blocks_impl(b200z_frame_decoder *d, b200z_read_fn rd, void *user, int strategy, size_t n, int *finished, SliceReader *slice) {
@@ -2565,10 +2571,42 @@ struct PipeSlots {
                 if (!*e && e->create(c)) return B200Z_ERR_CUDA;
         return 0;
     }
+    int ensure(size_t din, size_t hin, size_t dout, size_t hout, size_t desc) {   // each slot's buffers, at their exact sizes
+        int e = 0;
+        for (int i = 0; i < 2 && !e; i++)
+            if ((e = d_in[i].ensure(din, false)) || (e = d_out[i].ensure(dout, false)) || (e = d_desc[i].ensure(desc, false)) ||
+                (e = h_in[i].ensure(hin, false)) || (e = h_out[i].ensure(hout, false)) || (e = h_desc[i].ensure(desc, false)))
+                break;
+        return e;
+    }
     void drain(cudaStream_t ks) {   // leaves nothing in flight on the copy streams and on ks (when given)
         if (s_h2d) cudaStreamSynchronize(s_h2d);
         if (ks) cudaStreamSynchronize(ks);
         if (s_d2h) cudaStreamSynchronize(s_d2h);
+    }
+    // The source through the slots, once the caller has read chunk 0 into slot 0 (n0 bytes; eof0: the source ended there).  For
+    // chunk k in slot s: enqueue(k, s, n) queues a non-empty chunk's upload, kernels and download; read(s ^ 1, n, eof) reads chunk
+    // k + 1 once chunk k - 1's upload is done with the other slot; write(k - 1, s ^ 1, n, false) writes chunk k - 1, n being the
+    // bytes enqueued in its slot.  At the end of the source write(k, s, n, true) writes chunk k, even an empty one.  Each returns 0
+    // or an error code; on an error nothing is left in flight.
+    template <class Enqueue, class Read, class Write>
+    int run(b200z_ctx *c, size_t n0, bool eof0, Enqueue enqueue, Read read, Write write) {
+        size_t n[2] = {n0, 0}, sent[2] = {0, 0};   // the chunk read into h_in[s], and the one whose output is in slot s
+        bool eof[2] = {eof0, false};
+        int e = 0;
+        for (uint64_t k = 0;; k++) {
+            const int s = (int)(k & 1);
+            sent[s] = n[s];
+            if (n[s] && (e = enqueue(k, s, n[s]))) break;
+            if (!eof[s]) {   // a chunk shorter than the slot ends the source, so this one is full
+                if (k && cudaEventSynchronize(ev_h2d[s ^ 1]) != cudaSuccess) { e = c->set_cuda_err(cudaGetLastError(), "upload"); break; }
+                if ((e = read(s ^ 1, n[s ^ 1], eof[s ^ 1]))) break;
+            }
+            if (k && (e = write(k - 1, s ^ 1, sent[s ^ 1], false))) break;
+            if (eof[s]) { e = write(k, s, sent[s], true); break; }
+        }
+        if (e) drain(c->stream);
+        return e;
     }
 };
 
@@ -2607,6 +2645,16 @@ struct CompressResources {
     Event ev[kCompressStages + 1];
     float stage_ms[kCompressStages] = {};
     bool profiled = false;
+    // A submission of whole frames (the batch entry, the seekable writers): the staging, csum and results for `frames` frames in
+    // `blocks` blocks; Uncompressed takes the blocks' results only, not the match and entropy staging
+    int ensure_submission(uint64_t frames, uint64_t blocks, int level) {
+        int e = 0;
+        if ((e = level != B200Z_LEVEL_UNCOMPRESSED ? stage.ensure(blocks, true) : stage.res.ensure(blocks * sizeof(CBlockInfo))) ||
+            (e = csum.ensure(frames * 8)) || (e = results.ensure(frames * sizeof(b200z_compress_result))))
+            return e;
+        return 0;
+    }
+    int bind_submission(b200z_ctx *c, const b200z_dict *dict, int level, bool checksum, CompressArgs &a);
 };
 // the context's, created by its first compression or dictionary finalization
 static int compress_get(b200z_ctx *c, CompressResources **out) {
@@ -2624,11 +2672,11 @@ extern "C" int b200z_compress_last_profile(const b200z_ctx *c, float *stage_ms, 
     return 0;
 }
 
-// The dictionary's part of a compression's CompressArgs (dict_id, the match table, the encoder's tables).  The match table is built
-// once and kept with the dictionary (not one of the timed stages); offsets stay within the 128 KiB window, so the kernels see the
-// content's last ENC_WINDOW bytes only.  The encoder's view of a formatted dictionary's tables is built on the host once and kept
-// with the dictionary (no launch).
-static int compress_dict_args(b200z_ctx *c, const b200z_dict *dict, int level, CompressArgs &a) {
+// A submission's CompressArgs but for its frames, blocks, input, output and counts: the dictionary's part (dict_id, the match table,
+// the encoder's tables), the staging, csum, results, level and checksum.  The match table is built once and kept with the dictionary
+// (not one of the timed stages); offsets stay within the 128 KiB window, so the kernels see the content's last ENC_WINDOW bytes
+// only.  The encoder's view of a formatted dictionary's tables is built on the host once and kept with the dictionary (no launch).
+int CompressResources::bind_submission(b200z_ctx *c, const b200z_dict *dict, int level, bool checksum, CompressArgs &a) {
     const bool fast = level != B200Z_LEVEL_UNCOMPRESSED;
     const bool match_dict = fast && dict && dict->content_len >= ENC_MIN_MATCH;
     const uint32_t dict_tail = dict ? (uint32_t)std::min<size_t>(dict->content_len, ENC_WINDOW) : 0;
@@ -2652,7 +2700,39 @@ static int compress_dict_args(b200z_ctx *c, const b200z_dict *dict, int level, C
     a.etab = use_tables ? dict->d_enc.as<EncDict>() : nullptr;
     a.dict_id = compress_dict_id(dict);
     if (match_dict) { a.dict = dict_at; a.dtab = dict->d_ctab.as<uint32_t>(); a.dict_len = dict_tail; }
+    stage.bind(a);
+    a.csum = csum.as<uint64_t>(); a.results = results.as<b200z_compress_result>();
+    a.level = level; a.checksum = checksum ? 1 : 0;
     return 0;
+}
+
+// The level, window and dictionary rule of every compressing entry, checked before any launch, read or write
+static int compress_check(b200z_ctx *c, int level, int window_log, const b200z_dict *dict) {
+    if (level >= 2 && level <= 4) {   // Default / Better / Best: unimplemented!() in the reference
+        if (c) c->err = "compression levels Default, Better and Best are unimplemented!() in the reference";
+        return B200Z_ERR_REFERENCE_WOULD_PANIC;
+    }
+    if (!c || (level != B200Z_LEVEL_UNCOMPRESSED && level != B200Z_LEVEL_FASTEST && level != B200Z_LEVEL_LAZY)) return B200Z_ERR_INVALID_ARGUMENT;
+    if (window_log < B200Z_WINDOW_LOG_MIN || window_log > B200Z_WINDOW_LOG_MAX || (level == B200Z_LEVEL_UNCOMPRESSED && window_log != B200Z_WINDOW_LOG_MIN)) {
+        c->err = "window_log outside [17, 27], or above 17 at level Uncompressed";
+        return B200Z_ERR_INVALID_ARGUMENT;
+    }
+    if (dict && dict->ctx != c) { c->err = "dictionary created on another context"; return B200Z_ERR_INVALID_ARGUMENT; }
+    return 0;
+}
+
+// One frame's plan: its input [src_off, src_off + size) cut into 128 KiB CBlocks from hb[first_block] on (an empty frame is one empty
+// block), each reaching back to the frame's start or ENC_WINDOW bytes; `before` is the frame's input in front of src_off (a stream
+// chunk's k * C)
+static CFrame plan_frame(uint64_t src_off, uint64_t size, uint64_t dst_off, uint64_t before, uint32_t frame, uint32_t first_block, CBlock *hb) {
+    uint32_t b = first_block;
+    uint64_t pos = 0;
+    do {
+        const uint32_t bs = (uint32_t)std::min<uint64_t>(ENC_BLOCK, size - pos);
+        hb[b++] = CBlock{src_off + pos, bs, (uint32_t)std::min<uint64_t>(before + pos, ENC_WINDOW), frame, 0};
+        pos += bs;
+    } while (pos < size);
+    return CFrame{src_off, size, dst_off, first_block, b - first_block};
 }
 
 extern "C" int b200z_compress_frames_batch(b200z_ctx *c, const uint8_t *input, size_t input_len, int input_mem, const b200z_compress_io *frames,
@@ -2700,13 +2780,7 @@ extern "C" int b200z_compress_frames_batch_long(b200z_ctx *c, const uint8_t *inp
                                                 size_t nframes, int level, int checksum, const b200z_dict *dict, int window_log, uint8_t *output,
                                                 size_t output_cap, int output_mem, b200z_compress_result *results) {
     // ---- everything is checked before any device work
-    if (level >= 2 && level <= 4) return B200Z_ERR_REFERENCE_WOULD_PANIC;   // Default / Better / Best: unimplemented!() in the reference
-    if (!c || (level != B200Z_LEVEL_UNCOMPRESSED && level != B200Z_LEVEL_FASTEST && level != B200Z_LEVEL_LAZY)) return B200Z_ERR_INVALID_ARGUMENT;
-    if (window_log < B200Z_WINDOW_LOG_MIN || window_log > B200Z_WINDOW_LOG_MAX || (level == B200Z_LEVEL_UNCOMPRESSED && window_log != B200Z_WINDOW_LOG_MIN)) {
-        c->err = "window_log outside [17, 27], or above 17 at level Uncompressed";
-        return B200Z_ERR_INVALID_ARGUMENT;
-    }
-    if (dict && dict->ctx != c) { c->err = "dictionary created on another context"; return B200Z_ERR_INVALID_ARGUMENT; }
+    if (int e = compress_check(c, level, window_log, dict)) return e;
     if ((nframes && (!frames || !results)) || (input_mem != B200Z_MEM_HOST && input_mem != B200Z_MEM_DEVICE) ||
         (output_mem != B200Z_MEM_HOST && output_mem != B200Z_MEM_DEVICE) || (input_len && !input) || (output_cap && !output) || nframes > 0xffffffffu) {
         c->err = "invalid argument";
@@ -2732,28 +2806,18 @@ extern "C" int b200z_compress_frames_batch_long(b200z_ctx *c, const uint8_t *inp
     if (int e = c->use()) return e;
     // ---- plan: frames -> 128 KiB blocks
     std::vector<CFrame> hf(nframes);
-    std::vector<CBlock> hb;
-    hb.reserve(nblocks);
-    for (size_t i = 0; i < nframes; i++) {
-        const b200z_compress_io &f = frames[i];
-        hf[i] = CFrame{f.src_off, f.src_size, f.dst_off, (uint32_t)hb.size(), 0};
-        uint64_t pos = 0;
-        do {
-            const uint32_t size = (uint32_t)std::min<uint64_t>(ENC_BLOCK, f.src_size - pos);
-            hb.push_back(CBlock{f.src_off + pos, size, (uint32_t)std::min<uint64_t>(pos, ENC_WINDOW), (uint32_t)i, 0});
-            pos += size;
-        } while (pos < f.src_size);
-        hf[i].nblocks = (uint32_t)hb.size() - hf[i].first_block;
+    std::vector<CBlock> hb(nblocks);
+    for (size_t i = 0, b = 0; i < nframes; i++) {
+        hf[i] = plan_frame(frames[i].src_off, frames[i].src_size, frames[i].dst_off, 0, (uint32_t)i, (uint32_t)b, hb.data());
+        b += hf[i].nblocks;
     }
     CompressResources *rp = nullptr;
     if (int e = compress_get(c, &rp)) return e;
     CompressResources &r = *rp;
     const bool fast = level != B200Z_LEVEL_UNCOMPRESSED;   // Fastest or LAZY: the blocks are parsed and encoded
     int e = 0;
-    // Uncompressed takes the blocks' results only, not the match and entropy staging
     if ((e = r.frames.ensure(nframes * sizeof(CFrame))) || (e = r.blocks.ensure(nblocks * sizeof(CBlock))) ||
-        (e = fast ? r.stage.ensure(nblocks, true) : r.stage.res.ensure(nblocks * sizeof(CBlockInfo))) || (e = r.csum.ensure(nframes * 8)) ||
-        (e = r.results.ensure(nframes * sizeof(b200z_compress_result))))
+        (e = r.ensure_submission(nframes, nblocks, level)))
         return e;
     const uint8_t *d_in = input;
     uint8_t *d_out = output;
@@ -2770,12 +2834,9 @@ extern "C" int b200z_compress_frames_batch_long(b200z_ctx *c, const uint8_t *inp
     CU(c, cudaMemcpyAsync(r.frames.p, hf.data(), nframes * sizeof(CFrame), cudaMemcpyHostToDevice, s));
     CU(c, cudaMemcpyAsync(r.blocks.p, hb.data(), nblocks * sizeof(CBlock), cudaMemcpyHostToDevice, s));
     CompressArgs a{};
-    if ((e = compress_dict_args(c, dict, level, a))) return e;
+    if ((e = r.bind_submission(c, dict, level, checksum != 0, a))) return e;
     a.frames = r.frames.as<CFrame>(); a.blocks = r.blocks.as<CBlock>(); a.input = d_in; a.output = d_out;
-    r.stage.bind(a);
-    a.csum = r.csum.as<uint64_t>();
-    a.results = r.results.as<b200z_compress_result>(); a.nframes = (uint32_t)nframes; a.nblocks = (uint32_t)nblocks; a.level = level;
-    a.checksum = checksum ? 1 : 0;
+    a.nframes = (uint32_t)nframes; a.nblocks = (uint32_t)nblocks;
     a.window_log = (uint32_t)window_log;
     if (fast && window_log > B200Z_WINDOW_LOG_MIN) {   // the blocks of the frames larger than one block
         std::vector<LSpan> sp;
@@ -2810,7 +2871,6 @@ extern "C" int b200z_compress_frames_batch_long(b200z_ctx *c, const uint8_t *inp
 // is parsed on the host, the ranges become a plan (frames to decode, in place or into scratch, and copy pieces), the frames go through
 // the batch decoder's planner and pass, and k_range_gather copies the pieces.
 // ---------------------------------------------------------------------------------------------------------------
-static uint32_t seek_le32(const uint8_t *p) { return (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24; }
 static uint64_t seek_table_size(uint64_t nframes, bool checksum) { return SEEK_TABLE_FIXED + nframes * (checksum ? 12 : 8); }
 
 extern "C" size_t b200z_seekable_bound(size_t n, size_t frame_size, int checksum, const b200z_dict *dict) {
@@ -2832,21 +2892,13 @@ static SeekGroupSize seek_group_size(uint64_t bytes, uint64_t frame_size, const 
                          full * b200z_compress_bound_dict(frame_size, dict) + (rest ? b200z_compress_bound_dict(rest, dict) : 0)};
 }
 
-// The plan of frames [f0, f1) of a source cut every frame_size bytes and ending at `end`, as b200z_compress_frames_batch_dict plans the
-// same pieces: input offsets less `base`, CBlock.frame counted from f0.  Returns the blocks written to hb.
+// The plan of frames [f0, f1) of a source cut every frame_size bytes and ending at `end`: input offsets less `base`, CBlock.frame
+// counted from f0.  Returns the blocks written to hb.
 static uint32_t seek_group_plan(uint64_t f0, uint64_t f1, uint64_t frame_size, uint64_t end, uint64_t base, CFrame *hf, CBlock *hb) {
     uint32_t nb = 0;
     for (uint64_t f = f0; f < f1; f++) {
-        const uint64_t off = f * frame_size - base, size = std::min<uint64_t>(frame_size, end - f * frame_size);
-        CFrame &fr = hf[f - f0];
-        fr = CFrame{off, size, 0, nb, 0};
-        uint64_t pos = 0;
-        do {
-            const uint32_t bs = (uint32_t)std::min<uint64_t>(ENC_BLOCK, size - pos);
-            hb[nb++] = CBlock{off + pos, bs, (uint32_t)std::min<uint64_t>(pos, ENC_WINDOW), (uint32_t)(f - f0), 0};
-            pos += bs;
-        } while (pos < size);
-        fr.nblocks = nb - fr.first_block;
+        hf[f - f0] = plan_frame(f * frame_size - base, std::min<uint64_t>(frame_size, end - f * frame_size), 0, 0, (uint32_t)(f - f0), nb, hb);
+        nb += hf[f - f0].nblocks;
     }
     return nb;
 }
@@ -2863,18 +2915,10 @@ static int seek_group_run(b200z_ctx *c, const CompressArgs &a, uint64_t *total, 
     return 0;
 }
 
-// the level and dictionary checks of b200z_compress_frames_batch_dict
-static int seek_check_level(b200z_ctx *c, int level, const b200z_dict *dict) {
-    if (level >= 2 && level <= 4) return B200Z_ERR_REFERENCE_WOULD_PANIC;
-    if (!c || (level != B200Z_LEVEL_UNCOMPRESSED && level != B200Z_LEVEL_FASTEST && level != B200Z_LEVEL_LAZY)) return B200Z_ERR_INVALID_ARGUMENT;
-    if (dict && dict->ctx != c) { c->err = "dictionary created on another context"; return B200Z_ERR_INVALID_ARGUMENT; }
-    return 0;
-}
-
 extern "C" int b200z_compress_seekable(b200z_ctx *c, const uint8_t *input, size_t input_len, int input_mem, size_t frame_size, int level,
                                        int checksum, const b200z_dict *dict, uint8_t *output, size_t output_cap, int output_mem, size_t *written) {
-    // ---- everything is checked before any device work, as b200z_compress_frames_batch_dict checks it
-    if (int e = seek_check_level(c, level, dict)) return e;
+    // ---- everything is checked before any device work
+    if (int e = compress_check(c, level, B200Z_WINDOW_LOG_MIN, dict)) return e;
     if ((input_mem != B200Z_MEM_HOST && input_mem != B200Z_MEM_DEVICE) || (output_mem != B200Z_MEM_HOST && output_mem != B200Z_MEM_DEVICE) ||
         (input_len && !input) || !output || !written) {
         c->err = "invalid argument";
@@ -2892,7 +2936,6 @@ extern "C" int b200z_compress_seekable(b200z_ctx *c, const uint8_t *input, size_
     CompressResources *rp = nullptr;
     if (int e = compress_get(c, &rp)) return e;
     CompressResources &r = *rp;
-    const bool fast = level != B200Z_LEVEL_UNCOMPRESSED;
     const bool sum = checksum != 0;
     const uint64_t per_group = std::max<uint64_t>(1, B200Z_SEEKABLE_GROUP_BLOCKS / seek_frame_blocks(frame_size));   // frames per group
     // what the largest group holds -- frames, blocks, input bytes and its frames' bounds -- from the frames the input really has:
@@ -2908,19 +2951,15 @@ extern "C" int b200z_compress_seekable(b200z_ctx *c, const uint8_t *input, size_
     const uint64_t table = seek_table_size(nframes, sum);
     int e = 0;
     if ((e = r.frames.ensure(gframes * sizeof(CFrame))) || (e = r.blocks.ensure(gblocks * sizeof(CBlock))) ||
-        (e = fast ? r.stage.ensure(gblocks, true) : r.stage.res.ensure(gblocks * sizeof(CBlockInfo))) ||
-        (e = r.csum.ensure(gframes * 8)) || (e = r.results.ensure(gframes * sizeof(b200z_compress_result))) ||
-        (e = r.seek_entries.ensure(std::max<uint64_t>(table, 16))) || (e = r.seek_total.ensure(8)))
+        (e = r.ensure_submission(gframes, gblocks, level)) || (e = r.seek_entries.ensure(std::max<uint64_t>(table, 16))) ||
+        (e = r.seek_total.ensure(8)))
         return e;
     if (input_mem == B200Z_MEM_HOST && (e = r.input.ensure(gin + 16))) return e;
     if (output_mem == B200Z_MEM_HOST && (e = r.output.ensure(std::max(gout, table) + 16))) return e;
     cudaStream_t s = c->stream;
     CompressArgs a{};
-    if ((e = compress_dict_args(c, dict, level, a))) return e;
+    if ((e = r.bind_submission(c, dict, level, sum, a))) return e;
     a.frames = r.frames.as<CFrame>(); a.blocks = r.blocks.as<CBlock>();
-    r.stage.bind(a);
-    a.csum = r.csum.as<uint64_t>(); a.results = r.results.as<b200z_compress_result>();
-    a.level = level; a.checksum = sum ? 1 : 0;
     uint64_t *d_total = r.seek_total.as<uint64_t>();
     CU(c, cudaMemsetAsync(d_total, 0, 8, s));
     uint64_t origin = 0;        // archive offset of d_out's byte 0 (host output: the group's first byte)
@@ -2961,8 +3000,6 @@ extern "C" int b200z_compress_seekable(b200z_ctx *c, const uint8_t *input, size_
 }
 
 // ---- the seekable stream writer: groups of whole frames read from a source, two slots (PipeSlots), the table at the end
-static bool fc_read(b200z_read_fn rd, void *ru, uint8_t *buf, size_t cap, size_t *n, bool *eof);   // the stream compressor's reader
-
 static int seek_io(b200z_ctx *c, const std::string &what) {
     c->err = what;
     return B200Z_ERR_SEEKABLE_IO;
@@ -2971,9 +3008,8 @@ static int seek_io(b200z_ctx *c, const std::string &what) {
 // Group k (slot s = k & 1) is read into h_in[s], uploaded with its plan, compressed and packed from d_out[s]'s byte 0 behind the
 // slot's own running-size word (the first 8 bytes of d_desc[s], uploaded as 0), and downloaded with that word; k_cscan writes the
 // entries at their global frame index.  While group k uploads and compresses, the host reads group k + 1 and writes group k - 1.
-// `retired`: entry buffers outgrown during the call, which kernels may still write until the call has synchronised.
 static int seek_stream(b200z_ctx *c, b200z_read_fn rd, void *ru, b200z_write_fn wr, void *wu, uint64_t fs, int level, bool sum,
-                       const b200z_dict *dict, b200z_seekable_stream_result &res, std::vector<DevBuf> &retired) {
+                       const b200z_dict *dict, b200z_seekable_stream_result &res) {
     if (int e = c->use()) return e;
     CompressResources *rp = nullptr;
     if (int e = compress_get(c, &rp)) return e;
@@ -2985,10 +3021,10 @@ static int seek_stream(b200z_ctx *c, b200z_read_fn rd, void *ru, b200z_write_fn 
     cudaStream_t ks = c->stream;
     const auto oom = [&](int e) { c->err = "seekable stream: out of memory for groups of " + std::to_string(G) + " bytes"; return e; };
     int e = 0;
-    for (int i = 0; i < 2; i++)
-        if ((e = P.h_in[i].ensure(G, false))) return oom(e);
+    if ((e = P.ensure(0, G, 0, 0, 0))) return oom(e);   // the rest is sized by the first group, once it is read
     // the entries so far, doubled when full: the old buffer is copied on the kernel stream and kept until the call ends, since
     // freeing it earlier (cudaFree) would wait for the whole device in the middle of the pipeline
+    std::vector<DevBuf> retired;
     const auto grow_entries = [&](uint64_t need) -> int {
         if (need <= r.seek_entries.cap) return 0;
         DevBuf nb;
@@ -2998,43 +3034,32 @@ static int seek_stream(b200z_ctx *c, b200z_read_fn rd, void *ru, b200z_write_fn 
         retired.push_back(std::move(nb));
         return 0;
     };
-    size_t n[2] = {0, 0};
-    bool eof[2] = {false, false};
-    const auto read_group = [&](int s) -> int {
-        if (!fc_read(rd, ru, P.h_in[s].as<uint8_t>(), G, &n[s], &eof[s]))
+    const auto read_group = [&](int s, size_t &n, bool &eof) -> int {
+        if (!read_chunk(rd, ru, P.h_in[s].as<uint8_t>(), G, &n, &eof))
             return seek_io(c, "seekable stream: read_cb failed at source offset " + std::to_string(res.read) + " (archive offset " +
                                   std::to_string(res.written) + ")");
-        res.read += n[s];
+        res.read += n;
         return 0;
     };
-    if ((e = read_group(0)) || (e = grow_entries(16))) return e;
+    size_t n0 = 0;
+    bool eof0 = false;
+    if ((e = read_group(0, n0, eof0)) || (e = grow_entries(16))) return e;
     // every buffer sized by the first group, the largest one the source has (every group but the last is full)
-    const SeekGroupSize g = seek_group_size(n[0], fs, dict);
+    const SeekGroupSize g = seek_group_size(n0, fs, dict);
     const uint64_t desc = 8 + g.frames * sizeof(CFrame) + g.blocks * sizeof(CBlock);
-    const bool fast = level != B200Z_LEVEL_UNCOMPRESSED;
-    for (int i = 0; i < 2 && n[0] && !e; i++)
-        if ((e = P.d_in[i].ensure(g.in + 16, false)) || (e = P.d_out[i].ensure(g.out + 16, false)) || (e = P.d_desc[i].ensure(desc, false)) ||
-            (e = P.h_desc[i].ensure(desc, false)) || (e = P.h_out[i].ensure(g.out + 16, false)))
-            break;
-    if (!e && n[0])
-        if (!(e = fast ? r.stage.ensure(g.blocks, true) : r.stage.res.ensure(g.blocks * sizeof(CBlockInfo))) && !(e = r.csum.ensure(g.frames * 8)))
-            e = r.results.ensure(g.frames * sizeof(b200z_compress_result));
-    if (e) return oom(e);
+    if (n0 && ((e = P.ensure(g.in + 16, G, g.out + 16, g.out + 16, desc)) || (e = r.ensure_submission(g.frames, g.blocks, level)))) return oom(e);
     CompressArgs a{};
-    if ((e = compress_dict_args(c, dict, level, a))) return e;
-    r.stage.bind(a);
-    a.csum = r.csum.as<uint64_t>(); a.results = r.results.as<b200z_compress_result>();
-    a.level = level; a.checksum = sum ? 1 : 0;
-    const auto enqueue = [&](int s) -> int {
-        const uint64_t nf = (n[s] + fs - 1) / fs;
+    if ((e = r.bind_submission(c, dict, level, sum, a))) return e;
+    const auto enqueue = [&](uint64_t k, int s, size_t n) -> int {
+        const uint64_t nf = (n + fs - 1) / fs;
         if (res.frames + nf > 0xffffffffull) { c->err = "seekable stream: more than 2^32 - 1 frames"; return B200Z_ERR_INVALID_ARGUMENT; }
         if (int ge = grow_entries((res.frames + nf) * esz)) return ge;
         uint8_t *hd = P.h_desc[s].as<uint8_t>(), *dd = P.d_desc[s].as<uint8_t>();
         memset(hd, 0, 8);
         CFrame *hf = reinterpret_cast<CFrame *>(hd + 8);
-        const uint32_t nb = seek_group_plan(0, nf, fs, n[s], 0, hf, reinterpret_cast<CBlock *>(hf + nf));
+        const uint32_t nb = seek_group_plan(0, nf, fs, n, 0, hf, reinterpret_cast<CBlock *>(hf + nf));
         CU(c, cudaStreamWaitEvent(P.s_h2d, P.ev_k[s], 0));   // group k - 2's kernels are done with d_in[s] and d_desc[s]
-        CU(c, cudaMemcpyAsync(P.d_in[s].p, P.h_in[s].p, n[s], cudaMemcpyHostToDevice, P.s_h2d));
+        CU(c, cudaMemcpyAsync(P.d_in[s].p, P.h_in[s].p, n, cudaMemcpyHostToDevice, P.s_h2d));
         CU(c, cudaMemcpyAsync(dd, hd, 8 + nf * sizeof(CFrame) + nb * sizeof(CBlock), cudaMemcpyHostToDevice, P.s_h2d));
         CU(c, cudaEventRecord(P.ev_h2d[s], P.s_h2d));
         CU(c, cudaStreamWaitEvent(ks, P.ev_h2d[s], 0));
@@ -3046,34 +3071,22 @@ static int seek_stream(b200z_ctx *c, b200z_read_fn rd, void *ru, b200z_write_fn 
         // the packed size, then the frames: the download takes their bounds, so that no host wait stands between the two
         CU(c, cudaStreamWaitEvent(P.s_d2h, P.ev_k[s], 0));
         CU(c, cudaMemcpyAsync(hd, dd, 8, cudaMemcpyDeviceToHost, P.s_d2h));
-        CU(c, cudaMemcpyAsync(P.h_out[s].p, a.output, seek_group_size(n[s], fs, dict).out, cudaMemcpyDeviceToHost, P.s_d2h));
+        CU(c, cudaMemcpyAsync(P.h_out[s].p, a.output, seek_group_size(n, fs, dict).out, cudaMemcpyDeviceToHost, P.s_d2h));
         CU(c, cudaEventRecord(P.ev_d2h[s], P.s_d2h));
         res.frames += nf;
         res.groups++;
         return 0;
     };
-    const auto write_group = [&](int s) -> int {
+    const auto write_group = [&](uint64_t k, int s, size_t n, bool final) -> int {
+        if (!n) return 0;   // the source ended on a group boundary
         CU(c, cudaEventSynchronize(P.ev_d2h[s]));
         uint64_t packed = 0;
         memcpy(&packed, P.h_desc[s].p, 8);
-        if (!sd_write(wr, wu, P.h_out[s].as<uint8_t>(), packed, &res.written))
+        if (!write_all(wr, wu, P.h_out[s].as<uint8_t>(), packed, &res.written))
             return seek_io(c, "seekable stream: write_cb failed at archive offset " + std::to_string(res.written));
         return 0;
     };
-    for (uint64_t k = 0;; k++) {
-        const int s = (int)(k & 1);
-        const bool have = n[s] > 0;
-        if (have && (e = enqueue(s))) return e;
-        if (have && !eof[s]) {   // read group k + 1 into the other slot once group k - 1's upload is done with it
-            if (k) CU(c, cudaEventSynchronize(P.ev_h2d[s ^ 1]));
-            if ((e = read_group(s ^ 1))) return e;
-        }
-        if (k && (e = write_group(s ^ 1))) return e;
-        if (!have || eof[s]) {
-            if (have && (e = write_group(s))) return e;
-            break;
-        }
-    }
+    if ((e = P.run(c, n0, eof0, enqueue, read_group, write_group))) return e;
     // the table: k_cseek behind a zeroed word into r.output, downloaded and written
     const uint64_t table = seek_table_size(res.frames, sum);
     if ((e = r.output.ensure(table + 16)) || (e = r.seek_total.ensure(8))) return oom(e);
@@ -3084,21 +3097,19 @@ static int seek_stream(b200z_ctx *c, b200z_read_fn rd, void *ru, b200z_write_fn 
     std::vector<uint8_t> tab(table);
     CU(c, cudaMemcpyAsync(tab.data(), r.output.p, table, cudaMemcpyDeviceToHost, ks));
     CU(c, cudaStreamSynchronize(ks));
-    if (!sd_write(wr, wu, tab.data(), table, &res.written))
+    if (!write_all(wr, wu, tab.data(), table, &res.written))
         return seek_io(c, "seekable stream: write_cb failed at archive offset " + std::to_string(res.written));
     return 0;
 }
 
 extern "C" int b200z_compress_seekable_stream(b200z_ctx *c, b200z_read_fn rd, void *ru, b200z_write_fn wr, void *wu, size_t frame_size, int level,
                                               int checksum, const b200z_dict *dict, b200z_seekable_stream_result *result) {
-    // ---- everything is checked before any read, write or launch, as b200z_compress_seekable checks it
-    if (int e = seek_check_level(c, level, dict)) return e;
+    // ---- everything is checked before any read, write or launch
+    if (int e = compress_check(c, level, B200Z_WINDOW_LOG_MIN, dict)) return e;
     if (!rd || !wr) { c->err = "invalid argument"; return B200Z_ERR_INVALID_ARGUMENT; }
     if (!frame_size || frame_size > B200Z_SEEKABLE_MAX_FRAME_SIZE) { c->err = "frame_size must lie in [1, 2^30]"; return B200Z_ERR_INVALID_ARGUMENT; }
     b200z_seekable_stream_result res{};
-    std::vector<DevBuf> retired;   // released after the drain below
-    const int e = seek_stream(c, rd, ru, wr, wu, frame_size, level, checksum != 0, dict, res, retired);
-    if (e && c->comp) c->comp->seek_pipe.drain(c->stream);   // leave nothing in flight: the slots are reused by the next call
+    const int e = seek_stream(c, rd, ru, wr, wu, frame_size, level, checksum != 0, dict, res);
     if (result) *result = res;
     return e;
 }
@@ -3120,9 +3131,9 @@ static int seek_fail(std::string *why, const char *rule) {
 // the footer: n, the checksum flag, and the size of the table frame (checked to lie inside the archive)
 static int seek_footer(const uint8_t *ft, uint64_t len, SeekTable &t, uint64_t *table_bytes, std::string *why) {
     if (len < SEEK_TABLE_FIXED) return seek_fail(why, "the archive is shorter than a seek table (17 bytes)");
-    if (seek_le32(ft + 5) != SEEK_FOOTER_MAGIC) return seek_fail(why, "Seekable_Magic_Number is not 0x8F92EAB1");
+    if (rd32le(ft + 5) != SEEK_FOOTER_MAGIC) return seek_fail(why, "Seekable_Magic_Number is not 0x8F92EAB1");
     if (ft[4] & 0x7c) return seek_fail(why, "Seek_Table_Descriptor's reserved bits (6-2) are not 0");
-    t.len = len; t.n = seek_le32(ft); t.checksum = (ft[4] & 0x80) != 0;
+    t.len = len; t.n = rd32le(ft); t.checksum = (ft[4] & 0x80) != 0;
     *table_bytes = seek_table_size(t.n, t.checksum);
     if (*table_bytes > len) return seek_fail(why, "Number_Of_Frames gives a table larger than the archive");
     return 0;
@@ -3130,8 +3141,8 @@ static int seek_footer(const uint8_t *ft, uint64_t len, SeekTable &t, uint64_t *
 // the table frame (table_bytes of it, the footer included): its header and the entries, whose Compressed_Size must add up to its offset
 // the table frame's 8-byte header, against the footer's Number_Of_Frames and flag (Frame_Size is a u32, so this bounds the table)
 static int seek_table_header(const uint8_t *p, const SeekTable &t, std::string *why) {
-    if (seek_le32(p) != SEEK_SKIPPABLE_MAGIC) return seek_fail(why, "the table frame's Skippable_Magic_Number is not 0x184D2A5E");
-    if (seek_le32(p + 4) != t.n * (t.checksum ? 12 : 8) + SEEK_FOOTER) return seek_fail(why, "Frame_Size is not Number_Of_Frames * (8 or 12) + 9");
+    if (rd32le(p) != SEEK_SKIPPABLE_MAGIC) return seek_fail(why, "the table frame's Skippable_Magic_Number is not 0x184D2A5E");
+    if (rd32le(p + 4) != t.n * (t.checksum ? 12 : 8) + SEEK_FOOTER) return seek_fail(why, "Frame_Size is not Number_Of_Frames * (8 or 12) + 9");
     return 0;
 }
 static int seek_entries(const uint8_t *p, SeekTable &t, std::string *why) {
@@ -3140,9 +3151,9 @@ static int seek_entries(const uint8_t *p, SeekTable &t, std::string *why) {
     t.coff.assign(t.n + 1, 0); t.doff.assign(t.n + 1, 0); t.csum.assign(t.checksum ? t.n : 0, 0);
     for (uint64_t i = 0; i < t.n; i++) {
         const uint8_t *e = p + 8 + i * esz;
-        t.coff[i + 1] = t.coff[i] + seek_le32(e);
-        t.doff[i + 1] = t.doff[i] + seek_le32(e + 4);
-        if (t.checksum) t.csum[i] = seek_le32(e + 8);
+        t.coff[i + 1] = t.coff[i] + rd32le(e);
+        t.doff[i + 1] = t.doff[i] + rd32le(e + 4);
+        if (t.checksum) t.csum[i] = rd32le(e + 8);
     }
     if (t.coff[t.n] != t.len - tb) return seek_fail(why, "the frames' Compressed_Size do not add up to the table frame's offset");
     return 0;
@@ -3511,29 +3522,6 @@ extern "C" int b200z_frame_compressor_set_window_log(b200z_frame_compressor *fc,
 }
 extern "C" int b200z_frame_compressor_window_log(const b200z_frame_compressor *fc) { return fc ? (int)fc->window_log : B200Z_WINDOW_LOG_MIN; }
 
-// reads up to `cap` bytes, stopping at the first read that returns 0 (*eof; the reference stops there too); false on a read
-// error (< 0, or more than was asked for)
-static bool fc_read(b200z_read_fn rd, void *ru, uint8_t *buf, size_t cap, size_t *n, bool *eof) {
-    size_t got = 0;
-    *eof = false;
-    while (got < cap) {
-        const long r = rd(ru, buf + got, cap - got);
-        if (r < 0 || (size_t)r > cap - got) return false;
-        if (r == 0) { *eof = true; break; }
-        got += (size_t)r;
-    }
-    *n = got;
-    return true;
-}
-static bool fc_write(b200z_write_fn wr, void *wu, const uint8_t *p, size_t n) {   // write_all
-    while (n) {
-        const long w = wr(wu, p, n);
-        if (w <= 0 || (size_t)w > n) return false;
-        p += w;
-        n -= (size_t)w;
-    }
-    return true;
-}
 static void fc_le(uint8_t *p, uint64_t v, int n) { for (int i = 0; i < n; i++) p[i] = (uint8_t)(v >> (8 * i)); }
 // the frame header (frame_compressor.rs:144-151): no Frame_Content_Size, Single_Segment 0, a 2^window_log window (128 KiB by default)
 static void fc_header(uint8_t *dst, bool checksum, uint32_t window_log) {
@@ -3566,7 +3554,7 @@ static int fc_compress_raw(b200z_frame_compressor *fc, b200z_read_fn rd, void *r
         size_t len = 0, n = 0;
         bool eof = false;
         for (uint32_t i = 0; i < nb && !eof; i++) {
-            if (!fc_read(rd, ru, body + len + 3, ENC_BLOCK, &n, &eof)) return fc_panic(c, "FrameCompressor::compress: the source's read failed");
+            if (!read_chunk(rd, ru, body + len + 3, ENC_BLOCK, &n, &eof)) return fc_panic(c, "FrameCompressor::compress: the source's read failed");
             if (n == 0) break;   // the source ended on a block boundary: the trailer's empty block is the last
             h.update(body + len + 3, n);
             fc_le(body + len, (eof ? 1u : 0u) | ((uint32_t)n << 3), 3);
@@ -3578,7 +3566,7 @@ static int fc_compress_raw(b200z_frame_compressor *fc, b200z_read_fn rd, void *r
         if (k == 0) { start -= FC_HEADER; fc_header(start, fc->checksum, B200Z_WINDOW_LOG_MIN); }
         if (eof) len += fc_trailer(body + len, n == 0, fc->checksum, h, r);
         const size_t w = (size_t)(body + len - start);
-        if (!fc_write(wr, wu, start, w)) return fc_panic(c, "FrameCompressor::compress: the drain's write failed");
+        if (!write_all(wr, wu, start, w, nullptr)) return fc_panic(c, "FrameCompressor::compress: the drain's write failed");
         r.dst_size += w;
         if (eof) return 0;
     }
@@ -3591,12 +3579,7 @@ static int fc_prepare(b200z_frame_compressor *fc) {
     fc->hist = fc->hist_for(fc->window_log);
     const size_t C = fc->chunk, nb = fc->chunk_blocks(), bound = fc->chunk_bound();
     if (fc->p.create(c)) return B200Z_ERR_CUDA;
-    int e = 0;
-    for (int i = 0; i < 2 && !e; i++)
-        if ((e = fc->p.d_in[i].ensure(fc->hist + C + 16, false)) || (e = fc->p.d_out[i].ensure(bound + 16, false)) ||
-            (e = fc->p.d_desc[i].ensure(fc->desc_bytes(), false)) || (e = fc->p.h_in[i].ensure(C, false)) ||
-            (e = fc->p.h_out[i].ensure(FC_HDR_ROOM + bound + FC_TRAILER, false)) || (e = fc->p.h_desc[i].ensure(fc->desc_bytes(), false)))
-            break;
+    int e = fc->p.ensure(fc->hist + C + 16, C, bound + 16, FC_HDR_ROOM + bound + FC_TRAILER, fc->desc_bytes());
     if (!e) e = fc->stage.ensure(nb, false);
     if (!e && fc->hist > ENC_WINDOW) {
         const uint32_t ns = fc->max_spans();
@@ -3613,41 +3596,32 @@ static int fc_prepare(b200z_frame_compressor *fc) {
     return 0;
 }
 
-// Fastest: chunk k (slot s = k & 1) is read into h_in[s] and hashed, uploaded behind the previous chunk's last 128 KiB
-// (for matches that reach back), compressed, downloaded to h_out[s] and written.  While chunk k uploads and compresses, the
-// host reads chunk k + 1 and writes chunk k - 1.  A slot's buffers are reused only after the event of the last work that read
-// them: ev_k (kernels: d_in, d_desc), ev_h2d (upload: h_in, h_desc), ev_d2h (download: d_out, the result, h_out).
+// Fastest: chunk k (slot s = k & 1) is read into h_in[s] and hashed, uploaded behind the previous chunk's last `hist` bytes
+// (for matches that reach back), compressed, downloaded to h_out[s] with its result and written (PipeSlots::run).
 static int fc_compress_fast(b200z_frame_compressor *fc, b200z_read_fn rd, void *ru, b200z_write_fn wr, void *wu, XXH64State &h,
                             b200z_compress_result &r) {
     b200z_ctx *c = fc->ctx;
     if (int e = fc_prepare(fc)) return e;
     const uint64_t C = fc->chunk, H = fc->hist_for(fc->window_log);
     cudaStream_t ks = c->stream;
-    size_t n[2] = {0, 0};               // the chunk read into h_in[s]
-    bool eof[2] = {false, false};
-    size_t out_n[2] = {0, 0};           // the chunk whose output is in slot s
-    auto enqueue = [&](uint64_t k, int s) -> int {
-        const uint32_t m = (uint32_t)((n[s] + ENC_BLOCK - 1) / ENC_BLOCK);
+    auto enqueue = [&](uint64_t k, int s, size_t n) -> int {
         CFrame *hf = fc->p.h_desc[s].as<CFrame>();
         CBlock *hb = reinterpret_cast<CBlock *>(hf + 1);
-        *hf = CFrame{H, n[s], 0, 0, m};
-        for (uint32_t i = 0; i < m; i++) {
-            const uint64_t at = (uint64_t)i * ENC_BLOCK;
-            hb[i] = CBlock{H + at, (uint32_t)std::min<uint64_t>(ENC_BLOCK, n[s] - at), (uint32_t)std::min<uint64_t>(k * C + at, ENC_WINDOW), 0, 0};
-        }
+        *hf = plan_frame(H, n, 0, k * C, 0, 0, hb);
+        const uint32_t m = hf->nblocks;
         // long matches: the kept history (from the frame's start while it is shorter than H) and the chunk's blocks, as spans of at
         // most one block in position order; none until the frame has more than one block
         const uint64_t vlo = k * C >= H ? 0 : H - k * C;
         LSpan *hs = reinterpret_cast<LSpan *>(fc->p.h_desc[s].as<uint8_t>() + fc->span_off());
         uint32_t ns = 0;
-        if (H > ENC_WINDOW && k * C + n[s] > ENC_BLOCK) {
+        if (H > ENC_WINDOW && k * C + n > ENC_BLOCK) {
             for (uint64_t o = vlo; o < H; o += ENC_BLOCK) hs[ns++] = LSpan{o, vlo, (uint32_t)std::min<uint64_t>(ENC_BLOCK, H - o), 0, LDM_NO_BLOCK, 0};
             for (uint32_t i = 0; i < m; i++) hs[ns++] = LSpan{hb[i].src_off, vlo, hb[i].size, 0, i, 0};
         }
         uint8_t *din = fc->p.d_in[s].as<uint8_t>();
         CU(c, cudaStreamWaitEvent(fc->p.s_h2d, fc->p.ev_k[s], 0));   // chunk k - 2's kernels are done with d_in[s] and d_desc[s]
         if (k) CU(c, cudaMemcpyAsync(din, fc->p.d_in[s ^ 1].as<uint8_t>() + C, H, cudaMemcpyDeviceToDevice, fc->p.s_h2d));
-        CU(c, cudaMemcpyAsync(din + H, fc->p.h_in[s].p, n[s], cudaMemcpyHostToDevice, fc->p.s_h2d));
+        CU(c, cudaMemcpyAsync(din + H, fc->p.h_in[s].p, n, cudaMemcpyHostToDevice, fc->p.s_h2d));
         CU(c, cudaMemcpyAsync(fc->p.d_desc[s].p, hf, sizeof(CFrame) + m * sizeof(CBlock), cudaMemcpyHostToDevice, fc->p.s_h2d));
         if (ns) CU(c, cudaMemcpyAsync(fc->p.d_desc[s].as<uint8_t>() + fc->span_off(), hs, ns * sizeof(LSpan), cudaMemcpyHostToDevice, fc->p.s_h2d));
         CU(c, cudaEventRecord(fc->p.ev_h2d[s], fc->p.s_h2d));
@@ -3667,14 +3641,19 @@ static int fc_compress_fast(b200z_frame_compressor *fc, b200z_read_fn rd, void *
         CU(c, cudaEventRecord(fc->p.ev_k[s], ks));
         CU(c, cudaStreamWaitEvent(fc->p.s_d2h, fc->p.ev_k[s], 0));
         CU(c, cudaMemcpyAsync(fc->p.h_desc[s].as<uint8_t>() + fc->res_off(), a.results, sizeof(b200z_compress_result), cudaMemcpyDeviceToHost, fc->p.s_d2h));
-        CU(c, cudaMemcpyAsync(fc->p.h_out[s].as<uint8_t>() + FC_HDR_ROOM, a.output, n[s] + 3ull * m, cudaMemcpyDeviceToHost, fc->p.s_d2h));
+        CU(c, cudaMemcpyAsync(fc->p.h_out[s].as<uint8_t>() + FC_HDR_ROOM, a.output, n + 3ull * m, cudaMemcpyDeviceToHost, fc->p.s_d2h));
         CU(c, cudaEventRecord(fc->p.ev_d2h[s], fc->p.s_d2h));
         return 0;
     };
-    auto write_chunk = [&](uint64_t k, int s, bool final) -> int {
+    auto read = [&](int s, size_t &n, bool &eof) -> int {
+        if (!read_chunk(rd, ru, fc->p.h_in[s].as<uint8_t>(), C, &n, &eof)) return fc_panic(c, "FrameCompressor::compress: the source's read failed");
+        h.update(fc->p.h_in[s].as<uint8_t>(), n);
+        return 0;
+    };
+    auto write = [&](uint64_t k, int s, size_t n, bool final) -> int {
         uint8_t *const body = fc->p.h_out[s].as<uint8_t>() + FC_HDR_ROOM;
         size_t len = 0;
-        if (out_n[s]) {
+        if (n) {
             CU(c, cudaEventSynchronize(fc->p.ev_d2h[s]));
             const b200z_compress_result &cr = *reinterpret_cast<const b200z_compress_result *>(fc->p.h_desc[s].as<uint8_t>() + fc->res_off());
             len = cr.dst_size;
@@ -3682,40 +3661,23 @@ static int fc_compress_fast(b200z_frame_compressor *fc, b200z_read_fn rd, void *
         }
         uint8_t *start = body;
         if (k == 0) { start -= FC_HEADER; fc_header(start, fc->checksum, fc->window_log); }
-        if (final) len += fc_trailer(body + len, out_n[s] % ENC_BLOCK == 0, fc->checksum, h, r);
+        if (final) len += fc_trailer(body + len, n % ENC_BLOCK == 0, fc->checksum, h, r);
         const size_t w = (size_t)(body + len - start);
-        if (!fc_write(wr, wu, start, w)) return fc_panic(c, "FrameCompressor::compress: the drain's write failed");
+        if (!write_all(wr, wu, start, w, nullptr)) return fc_panic(c, "FrameCompressor::compress: the drain's write failed");
         r.dst_size += w;
         return 0;
     };
-    int e = 0;
-    if (!fc_read(rd, ru, fc->p.h_in[0].as<uint8_t>(), C, &n[0], &eof[0])) e = fc_panic(c, "FrameCompressor::compress: the source's read failed");
-    else h.update(fc->p.h_in[0].as<uint8_t>(), n[0]);
-    for (uint64_t k = 0; !e; k++) {
-        const int s = (int)(k & 1);
-        out_n[s] = n[s];
-        if (n[s] && (e = enqueue(k, s))) break;
-        if (!eof[s]) {   // read chunk k + 1 into the other slot once chunk k - 1's upload is done with it
-            if (k && cudaEventSynchronize(fc->p.ev_h2d[s ^ 1]) != cudaSuccess) { e = c->set_cuda_err(cudaGetLastError(), "upload"); break; }
-            if (!fc_read(rd, ru, fc->p.h_in[s ^ 1].as<uint8_t>(), C, &n[s ^ 1], &eof[s ^ 1])) { e = fc_panic(c, "FrameCompressor::compress: the source's read failed"); break; }
-            h.update(fc->p.h_in[s ^ 1].as<uint8_t>(), n[s ^ 1]);
-        }
-        if (k && (e = write_chunk(k - 1, s ^ 1, false))) break;
-        if (eof[s]) { e = write_chunk(k, s, true); break; }
-    }
-    if (e) fc->p.drain(ks);   // leave nothing in flight: the buffers are reused by the next compress
-    return e;
+    size_t n0 = 0;
+    bool eof0 = false;
+    if (int e = read(0, n0, eof0)) return e;
+    return fc->p.run(c, n0, eof0, enqueue, read, write);
 }
 
 extern "C" int b200z_frame_compressor_compress(b200z_frame_compressor *fc, b200z_read_fn rd, void *ru, b200z_write_fn wr, void *wu,
                                                b200z_compress_result *result) {
     if (!fc || !rd || !wr) return B200Z_ERR_INVALID_ARGUMENT;
     b200z_ctx *c = fc->ctx;
-    if (fc->level >= 2 && fc->level <= 4) return fc_panic(c, "FrameCompressor::compress: compression levels above Fastest are unimplemented!() in the reference");
-    if (fc->level == B200Z_LEVEL_UNCOMPRESSED && fc->window_log != B200Z_WINDOW_LOG_MIN) {
-        c->err = "FrameCompressor::compress: window_log above 17 at level Uncompressed";
-        return B200Z_ERR_INVALID_ARGUMENT;
-    }
+    if (int e = compress_check(c, fc->level, (int)fc->window_log, nullptr)) return e;
     b200z_compress_result r{};
     XXH64State h;
     h.reset();
