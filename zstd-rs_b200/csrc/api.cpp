@@ -304,25 +304,22 @@ extern "C" void b200z_dict_destroy(b200z_dict *d) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// A "submission": host-side plan + its device mirror.  Used by the batch entry (many frames, fresh state) and
-// by the FrameDecoder mirror (one frame, a few new blocks, state carried on the device).
+// A "submission": host-side plan + its device mirror.  Every decoding entry plans one.  A frame starts fresh (add_frame) or resumes
+// from a previous submission's state and tables (add_resumed_frame: the stream decoder's first frame, the FrameDecoder mirror's one
+// frame).  Below it, the frame-start and block-read rules of the reference, which every entry's planner applies.
 // ---------------------------------------------------------------------------------------------------------------
 namespace {
+
+// FSE table `which` (0 = LL, 1 = OF, 2 = ML) of a slot
+template <class Slot> auto *fse_at(Slot *s, int which) { return which == 0 ? &s->ll : (which == 1 ? &s->of : &s->ml); }
 
 struct CarrySet {
     const HufSlot *huf = nullptr;
     const FseTab *ll = nullptr, *of = nullptr, *ml = nullptr;
-    const b200z_dict *dict = nullptr;   // the dictionary these tables belong to (null: the frame decoder's carried tables)
+    const b200z_dict *dict = nullptr;   // the dictionary these tables belong to (null: tables carried over from a submission)
+    const FseTab *fse(int which) const { return which == 0 ? ll : (which == 1 ? of : ml); }
 };
 
-// initial cursor of a frame: fresh, or the dictionary's tables (scratch.rs:70-78)
-void cursor_from_carry(TableCursor &cur, const CarrySet &cs, uint32_t carry_idx) {
-    cur = TableCursor();
-    if (cs.huf) { cur.huf.kind = TabRef::CARRY; cur.huf.idx = carry_idx; }
-    if (cs.ll) { cur.ll.kind = TabRef::CARRY; cur.ll.idx = carry_idx; }
-    if (cs.of) { cur.of.kind = TabRef::CARRY; cur.of.idx = carry_idx; }
-    if (cs.ml) { cur.ml.kind = TabRef::CARRY; cur.ml.idx = carry_idx; }
-}
 CarrySet carry_of_dict(const b200z_dict *d) {
     CarrySet cs;
     cs.dict = d;
@@ -357,41 +354,89 @@ struct Submission {
         carries.push_back(carry_of_dict(dict));
         return (int)carries.size() - 1;
     }
-    // Appends a frame whose blocks follow (the caller sets its nblocks), starting from the dictionary's offset history or {1, 4, 8}.
+    // Appends a frame whose blocks follow, starting from the dictionary's offset history or {1, 4, 8}.
     // Returns the table cursor of its first block: the dictionary's tables, if any.
     TableCursor add_frame(const b200z_dict *dict, uint64_t out_off, uint64_t out_cap, uint64_t window) {
         static const uint32_t fresh_hist[3] = {1, 4, 8};
-        FrameDesc fd;
-        memset(&fd, 0, sizeof fd);
-        fd.out_off = out_off; fd.out_cap = out_cap; fd.window_size = window;
-        fd.dict = dict ? dict->d_content.as<uint8_t>() : nullptr; fd.dict_len = dict ? dict->content_len : 0;
-        fd.first_block = (uint32_t)descs.size();
         FrameState st;
         memset(&st, 0, sizeof st);
         memcpy(st.hist, dict ? dict->hist : fresh_hist, sizeof st.hist);
-        frames.push_back(fd); states.push_back(st);
-        TableCursor cur;
-        const int ci = carry_index(dict);
-        if (ci >= 0) cursor_from_carry(cur, carries[ci], (uint32_t)ci);
+        const TableCursor cur = push_frame(dict, window, st, carry_index(dict));
+        frames.back().out_off = out_off; frames.back().out_cap = out_cap;
         return cur;
     }
-    // Appends a block.  A Compressed block is planned from its section headers, as parsed here from its content or by k_walk (`sec`);
-    // `cur` moves on to the tables it leaves current.
-    const BlockDesc &add_block(uint64_t src_off, const BlockHeader &bh, uint32_t frame, uint32_t block_in_frame, const SectionHeaders &sec,
-                               TableCursor &cur) {
+    // Appends a frame that continues from a previous submission, from its state `st` and the tables `cs` its next block starts from;
+    // the caller places it.  Returns the table cursor of that block.
+    TableCursor add_resumed_frame(const FrameState &st, uint64_t window, const b200z_dict *dict, const CarrySet &cs) {
+        carries.push_back(cs);
+        return push_frame(dict, window, st, (int)carries.size() - 1);
+    }
+    // appends a frame's descriptor and state; its first block starts from the tables of carries[ci], if any (scratch.rs:70-78)
+    TableCursor push_frame(const b200z_dict *dict, uint64_t window, const FrameState &st, int ci) {
+        FrameDesc fd;
+        memset(&fd, 0, sizeof fd);
+        fd.window_size = window;
+        fd.dict = dict ? dict->d_content.as<uint8_t>() : nullptr; fd.dict_len = dict ? dict->content_len : 0;
+        fd.first_block = (uint32_t)descs.size();
+        frames.push_back(fd); states.push_back(st);
+        TableCursor cur;
+        if (ci < 0) return cur;
+        const CarrySet &cs = carries[ci];
+        if (cs.huf) { cur.huf.kind = TabRef::CARRY; cur.huf.idx = (uint32_t)ci; }
+        if (cs.ll) { cur.ll.kind = TabRef::CARRY; cur.ll.idx = (uint32_t)ci; }
+        if (cs.of) { cur.of.kind = TabRef::CARRY; cur.of.idx = (uint32_t)ci; }
+        if (cs.ml) { cur.ml.kind = TabRef::CARRY; cur.ml.idx = (uint32_t)ci; }
+        return cur;
+    }
+    // Appends a block to the last frame and counts it there.  A Compressed block is planned from its section headers, as parsed here
+    // from its content or by k_walk (`sec`); `cur` moves on to the tables it leaves current.
+    const BlockDesc &add_block(uint64_t src_off, const BlockHeader &bh, uint32_t block_in_frame, const SectionHeaders &sec, TableCursor &cur) {
         BlockDesc d;
         memset(&d, 0, sizeof d);
         BlockRefs r;
-        d.src_off = src_off; d.src_size = bh.content_size; d.frame = frame; d.btype = bh.type; d.raw_size = bh.decompressed_size;
+        d.src_off = src_off; d.src_size = bh.content_size; d.frame = (uint32_t)frames.size() - 1; d.btype = bh.type; d.raw_size = bh.decompressed_size;
         d.block_in_frame = block_in_frame; d.last = bh.last;
         if (bh.type == BT_COMPRESSED) plan_compressed_block(sec, d, r, cur, n_huf, n_fse, lit_bytes, nseq);
         descs.push_back(d); refs.push_back(r);
+        frames.back().nblocks++;
         return descs.back();
     }
-    const BlockDesc &add_block(uint64_t src_off, const BlockHeader &bh, uint32_t frame, uint32_t block_in_frame, const uint8_t *content,
-                               TableCursor &cur) {
+    const BlockDesc &add_block(uint64_t src_off, const BlockHeader &bh, uint32_t block_in_frame, const uint8_t *content, TableCursor &cur) {
         const SectionHeaders sec = bh.type == BT_COMPRESSED ? parse_section_headers(content, bh.content_size) : SectionHeaders();
-        return add_block(src_off, bh, frame, block_in_frame, sec, cur);
+        return add_block(src_off, bh, block_in_frame, sec, cur);
+    }
+    // The tables a frame's next block starts from after this submission, where its last block left `cur` current: a table built here
+    // (SLOT) is copy_carry's copy at `huf_to` / `fse_to`; the predefined tables and those the frame started from (CARRY) stay put.
+    CarrySet carry_after(const TableCursor &cur, const HufSlot *huf_to, const FseSlot *fse_to, const FseSlot *predef) const {
+        auto fse = [&](const TabRef &t, int which) -> const FseTab * {
+            if (t.kind == TabRef::SLOT) return fse_at(fse_to, which);
+            if (t.kind == TabRef::PREDEF) return fse_at(predef, which);
+            if (t.kind == TabRef::CARRY) return carries[t.idx].fse(which);
+            return nullptr;
+        };
+        CarrySet next;
+        next.huf = cur.huf.kind == TabRef::SLOT ? huf_to : (cur.huf.kind == TabRef::CARRY ? carries[cur.huf.idx].huf : nullptr);
+        next.ll = fse(cur.ll, 0); next.of = fse(cur.of, 1); next.ml = fse(cur.ml, 2);
+        return next;
+    }
+    // Queues on `stream` the device-to-device copies of the tables built here that `cur` names, to where carry_after put them.
+    int copy_carry(b200z_ctx *c, const TableCursor &cur, HufSlot *huf_to, FseSlot *fse_to, cudaStream_t stream) const {
+        if (cur.huf.kind == TabRef::SLOT)
+            CU(c, cudaMemcpyAsync(huf_to, d_huf.as<HufSlot>() + cur.huf.idx, sizeof(HufSlot), cudaMemcpyDeviceToDevice, stream));
+        const TabRef *t[3] = {&cur.ll, &cur.of, &cur.ml};
+        for (int k = 0; k < 3; k++)
+            if (t[k]->kind == TabRef::SLOT)
+                CU(c, cudaMemcpyAsync(fse_at(fse_to, k), fse_at(d_fse.as<FseSlot>() + t[k]->idx, k), sizeof(FseTab), cudaMemcpyDeviceToDevice, stream));
+        return 0;
+    }
+    // Queues on `stream` the copy to host memory of the frame states, or of the aux records of blocks [first, first + n).
+    int download_states(b200z_ctx *c, FrameState *to, cudaStream_t stream) const {
+        if (!states.empty()) CU(c, cudaMemcpyAsync(to, d_states.p, states.size() * sizeof(FrameState), cudaMemcpyDeviceToHost, stream));
+        return 0;
+    }
+    int download_aux(b200z_ctx *c, BlockAux *to, size_t first, size_t n, cudaStream_t stream) const {
+        if (n) CU(c, cudaMemcpyAsync(to, d_aux.as<BlockAux>() + first, n * sizeof(BlockAux), cudaMemcpyDeviceToHost, stream));
+        return 0;
     }
     // resolve table references to device pointers and upload descriptors
     int upload(b200z_ctx *c, cudaStream_t stream = nullptr) {
@@ -452,9 +497,9 @@ struct Submission {
                 return nullptr;
             };
             auto fse = [&](const TabRef &t, int which) -> const FseTab * {
-                if (t.kind == TabRef::SLOT) return which == 0 ? &fs[t.idx].ll : (which == 1 ? &fs[t.idx].of : &fs[t.idx].ml);
-                if (t.kind == TabRef::PREDEF) return which == 0 ? &pd->ll : (which == 1 ? &pd->of : &pd->ml);
-                if (t.kind == TabRef::CARRY) return which == 0 ? carries[t.idx].ll : (which == 1 ? carries[t.idx].of : carries[t.idx].ml);
+                if (t.kind == TabRef::SLOT) return fse_at(fs + t.idx, which);
+                if (t.kind == TabRef::PREDEF) return fse_at(pd, which);
+                if (t.kind == TabRef::CARRY) return carries[t.idx].fse(which);
                 return nullptr;
             };
             d.huf = huf(r.huf);
@@ -488,6 +533,42 @@ struct Submission {
         return a;
     }
 };
+
+// common::MAX_WINDOW_SIZE, the cap of every window limit (FrameDecoder::set_max_window_size, :175-177).  A single-segment frame's
+// window is its content size, which frame_window_size does not bound, so the cap decides for such a frame.
+constexpr uint64_t MAX_WINDOW_SIZE = (1ull << 41) + 7 * (1ull << 38);
+// the window limit of a decoding entry's `max_window`: 0 means the default (frame_decoder.rs:25)
+uint64_t window_limit(uint64_t max_window) { return std::min<uint64_t>(max_window ? max_window : B200Z_DEFAULT_MAX_WINDOW_SIZE, MAX_WINDOW_SIZE); }
+
+// The window rule of FrameDecoderState::new / reset (frame_decoder.rs:103-142): `window` from the header, refused when the header
+// gives none or when it is above `limit`.  Returns 0 or the error, which the reference raises at B200Z_STAGE_FRAME_HEADER.
+int frame_window(const FrameHeader &h, uint64_t limit, uint64_t &window) {
+    if (int e = frame_window_size(h, window)) return e;
+    return window > limit ? B200Z_ERR_WINDOW_SIZE_TOO_BIG : 0;
+}
+
+// The dictionary of a frame on the entries that take a list (FrameDecoder::reset :210-218, then force_dict): the last of `dicts` with
+// the header's ID, or `forced` when given.  B200Z_ERR_DICT_NOT_PROVIDED (stage FRAME_HEADER) when none has the ID, forced or not.
+int frame_dict(const FrameHeader &h, const b200z_dict *const *dicts, size_t ndicts, const b200z_dict *forced, const b200z_dict *&dict) {
+    dict = nullptr;
+    if (h.has_dict_id) {
+        for (size_t k = 0; k < ndicts; k++) if (dicts[k]->id == h.dict_id) dict = dicts[k];
+        if (!dict) return B200Z_ERR_DICT_NOT_PROVIDED;
+    }
+    if (forced) dict = forced;
+    return 0;
+}
+
+// The block-read rule of decode_blocks (BlockDecoder::read_block_header, decode_block_content): `hdr` is null when the 3 header bytes
+// cannot be read, has_body(n) says whether the n content bytes can.  The status word of a block not read whole, or 0 and `bh`.
+template <class HasBody>
+uint32_t read_block(const uint8_t *hdr, BlockHeader &bh, HasBody has_body) {
+    if (!hdr) return mk_status(B200Z_ERR_BLOCK_HEADER_READ, B200Z_STAGE_BLOCK_HEADER);
+    if (int e = parse_block_header(hdr, bh)) return mk_status((uint32_t)e, B200Z_STAGE_BLOCK_HEADER);
+    if (!has_body(bh.content_size))
+        return mk_status(bh.type == BT_COMPRESSED ? B200Z_ERR_BLOCK_CONTENT_READ : B200Z_ERR_BLOCK_BODY_READ, B200Z_STAGE_BLOCK_BODY);
+    return 0;
+}
 
 }  // namespace
 
@@ -536,8 +617,7 @@ static int plan_batch(b200z_batch *b, const uint8_t *in, size_t in_len, const b2
     s.clear();
     b->info.assign(nframes, FramePlanInfo());
     b->block_end_bytes.clear();
-    if (max_window == 0) max_window = B200Z_DEFAULT_MAX_WINDOW_SIZE;
-    max_window = std::min<uint64_t>(max_window, (1ull << 41) + 7 * (1ull << 38));
+    const uint64_t limit = window_limit(max_window);
     for (size_t i = 0; i < nframes; i++) {
         FramePlanInfo &fi = b->info[i];
         const b200z_frame_io &io = frames[i];
@@ -549,14 +629,11 @@ static int plan_batch(b200z_batch *b, const uint8_t *in, size_t in_len, const b2
         const uint32_t wk_end = walk ? wk + walk->wf[i].nblocks : 0;
         int e = parse_frame_header(p, len, fi.hdr, fi.skip_len, consumed);
         if (e) { fi.pre_status = e; fi.pre_stage = B200Z_STAGE_FRAME_HEADER; fi.bytes_read_full = consumed; continue; }
-        if ((e = frame_window_size(fi.hdr, fi.window))) { fi.pre_status = e; fi.pre_stage = B200Z_STAGE_FRAME_HEADER; continue; }
-        if (fi.window > max_window) { fi.pre_status = B200Z_ERR_WINDOW_SIZE_TOO_BIG; fi.pre_stage = B200Z_STAGE_FRAME_HEADER; continue; }
         const b200z_dict *dict = nullptr;
-        if (fi.hdr.has_dict_id) {
-            for (size_t k = 0; k < ndicts; k++) if (dicts[k]->id == fi.hdr.dict_id) dict = dicts[k];
-            if (!dict) { fi.pre_status = B200Z_ERR_DICT_NOT_PROVIDED; fi.pre_stage = B200Z_STAGE_FRAME_HEADER; continue; }
+        if ((e = frame_window(fi.hdr, limit, fi.window)) || (e = frame_dict(fi.hdr, dicts, ndicts, forced, dict))) {
+            fi.pre_status = e; fi.pre_stage = B200Z_STAGE_FRAME_HEADER;
+            continue;
         }
-        if (forced) dict = forced;
 
         fi.sub_frame = (int32_t)s.frames.size();
         TableCursor cur = s.add_frame(dict, io.out_off, io.out_cap, fi.window);
@@ -566,21 +643,17 @@ static int plan_batch(b200z_batch *b, const uint8_t *in, size_t in_len, const b2
         uint64_t pos = consumed, bytes_read = consumed;
         uint32_t bif = 0;
         for (;;) {
-            if (len - pos < 3) { fd.host_status = mk_status(B200Z_ERR_BLOCK_HEADER_READ, B200Z_STAGE_BLOCK_HEADER); break; }
-            BlockHeader bh;
             const WalkBlock *wbk = nullptr;
-            if (walk) {
+            if (walk && len - pos >= 3) {
                 if (wk >= wk_end || walk->wb[wk].pos != pos) return B200Z_ERR_INVALID_ARGUMENT;   // (the walk and the planner follow the same chain)
                 wbk = &walk->wb[wk++];
             }
-            if ((e = parse_block_header(wbk ? wbk->bh : p + pos, bh))) { fd.host_status = mk_status((uint32_t)e, B200Z_STAGE_BLOCK_HEADER); break; }
+            BlockHeader bh;
+            const uint8_t *hdr = len - pos < 3 ? nullptr : (wbk ? wbk->bh : p + pos);
+            if (uint32_t w = read_block(hdr, bh, [&](uint32_t n) { return len - pos - 3 >= n; })) { fd.host_status = w; break; }
             pos += 3;
-            if (len - pos < bh.content_size) {
-                fd.host_status = mk_status(bh.type == BT_COMPRESSED ? B200Z_ERR_BLOCK_CONTENT_READ : B200Z_ERR_BLOCK_BODY_READ, B200Z_STAGE_BLOCK_BODY);
-                break;
-            }
-            const BlockDesc &d = wbk ? s.add_block(io.src_off + pos, bh, (uint32_t)fi.sub_frame, bif++, wbk->sec, cur)
-                                     : s.add_block(io.src_off + pos, bh, (uint32_t)fi.sub_frame, bif++, p + pos, cur);
+            const BlockDesc &d = wbk ? s.add_block(io.src_off + pos, bh, bif++, wbk->sec, cur)
+                                     : s.add_block(io.src_off + pos, bh, bif++, p + pos, cur);
             pos += bh.content_size;
             bytes_read += 3 + bh.content_size;
             b->block_end_bytes.push_back(bytes_read);
@@ -596,7 +669,6 @@ static int plan_batch(b200z_batch *b, const uint8_t *in, size_t in_len, const b2
                 break;
             }
         }
-        fd.nblocks = (uint32_t)s.descs.size() - fd.first_block;
         fi.bytes_read_full = bytes_read;
     }
     return 0;
@@ -838,9 +910,8 @@ extern "C" int b200z_batch_finish(b200z_batch *b, b200z_frame_result *results) {
     if (!b || !results || b->decode_all) return B200Z_ERR_INVALID_ARGUMENT;
     b200z_ctx *c = b->ctx;
     if (int e = c->use()) return e;
-    Submission &s = b->sub;
-    std::vector<FrameState> st(s.states.size());
-    if (!st.empty()) CU(c, cudaMemcpyAsync(st.data(), s.d_states.p, st.size() * sizeof(FrameState), cudaMemcpyDeviceToHost, c->stream));
+    std::vector<FrameState> st(b->sub.states.size());
+    if (int e = b->sub.download_states(c, st.data(), c->stream)) return e;
     CU(c, cudaStreamSynchronize(c->stream));
     for (size_t i = 0; i < b->info.size(); i++) {
         int32_t sf = b->info[i].sub_frame;
@@ -1038,9 +1109,8 @@ static int decode_frames_pipelined(b200z_ctx *c, const uint8_t *input, size_t in
         if (int e = enqueue_pass(c, a, PipelineStreams{km, p->k_side[s], p->k_fork[s], p->k_join[s]}, &b->checksummed, &c->launches)) return e;
         CU(c, cudaEventRecord(p->ev_k[s], km));
         CU(c, cudaStreamWaitEvent(p->s_d2h, p->ev_k[s], 0));
-        size_t nst = b->sub.states.size();
-        if (int e = p->h_states[s].ensure(nst * sizeof(FrameState))) return e;
-        if (nst) CU(c, cudaMemcpyAsync(p->h_states[s].p, b->sub.d_states.p, nst * sizeof(FrameState), cudaMemcpyDeviceToHost, p->s_d2h));
+        if (int e = p->h_states[s].ensure(b->sub.states.size() * sizeof(FrameState))) return e;
+        if (int e = b->sub.download_states(c, p->h_states[s].as<FrameState>(), p->s_d2h)) return e;
         if (ohi > olo) CU(c, cudaMemcpyAsync(output + olo, d_out + olo, ohi - olo, cudaMemcpyDeviceToHost, p->s_d2h));
         CU(c, cudaEventRecord(p->ev_done[s], p->s_d2h));
         pend[s].f0 = f0; pend[s].f1 = f1; pend[s].live = true;
@@ -1276,7 +1346,7 @@ extern "C" int b200z_decode_all_finish(b200z_batch *b, b200z_all_result *sum, b2
     if (int e = c->use()) return e;
     const Submission &s = b->sub;
     std::vector<FrameState> st(s.states.size());
-    if (!st.empty()) CU(c, cudaMemcpyAsync(st.data(), s.d_states.p, st.size() * sizeof(FrameState), cudaMemcpyDeviceToHost, c->stream));
+    if (int e = s.download_states(c, st.data(), c->stream)) return e;
     CU(c, cudaStreamSynchronize(c->stream));
     memset(sum, 0, sizeof *sum);
     sum->error_offset = b->input_len;
@@ -1306,7 +1376,7 @@ extern "C" int b200z_decode_all_finish(b200z_batch *b, b200z_all_result *sum, b2
         const FrameDesc &fd = s.frames[fi.sub_frame];
         std::vector<BlockAux> aux(fd.nblocks);
         if (fd.nblocks) {
-            CU(c, cudaMemcpyAsync(aux.data(), s.d_aux.as<BlockAux>() + fd.first_block, fd.nblocks * sizeof(BlockAux), cudaMemcpyDeviceToHost, c->stream));
+            if (int e = s.download_aux(c, aux.data(), fd.first_block, fd.nblocks, c->stream)) return e;
             CU(c, cudaStreamSynchronize(c->stream));
         }
         uint32_t word = fs->status, n = fs->blocks_done;
@@ -1453,9 +1523,8 @@ struct SdPlanner {
     SdCont cont;
     int32_t zi = -1;
     uint64_t max_window_seen = 0;
-    SdPlanner(uint64_t C, const b200z_dict *const *d, size_t nd, const b200z_dict *f, uint64_t mw) : bnd(C), dicts(d), ndicts(nd), forced(f) {
-        max_window = std::min<uint64_t>(mw ? mw : B200Z_DEFAULT_MAX_WINDOW_SIZE, (1ull << 41) + 7 * (1ull << 38));
-    }
+    SdPlanner(uint64_t C, const b200z_dict *const *d, size_t nd, const b200z_dict *f, uint64_t mw)
+        : bnd(C), dicts(d), ndicts(nd), forced(f), max_window(window_limit(mw)) {}
 
     // the most a block adds to the output: a Raw / RLE block's size, min(128 KiB, window) for a Compressed block
     static uint64_t out_of(const BlockHeader &bh, uint64_t window) { return bh.type == BT_COMPRESSED ? std::min<uint64_t>(131072, window) : bh.decompressed_size; }
@@ -1490,15 +1559,9 @@ struct SdPlanner {
         if (cont.on) {
             // the frame continues from its carried state, tables and tail (k_carry writes its state and placement)
             start_frame(cont.frame, cont.dict, cont.window);
-            FrameDesc fd;
-            memset(&fd, 0, sizeof fd);
-            fd.window_size = cont.window;
-            fd.dict = cont.dict ? cont.dict->d_content.as<uint8_t>() : nullptr; fd.dict_len = cont.dict ? cont.dict->content_len : 0;
             FrameState st;
             memset(&st, 0, sizeof st);
-            s.frames.push_back(fd); s.states.push_back(st);
-            s.carries.push_back(cont.tables);
-            cursor_from_carry(cur, cont.tables, (uint32_t)s.carries.size() - 1);
+            cur = s.add_resumed_frame(st, cont.window, cont.dict, cont.tables);
             checksum = cont.checksum; bif = cont.next_block;
             p.resumed = true; p.resume_window = cont.window;
             active = true;
@@ -1533,15 +1596,10 @@ struct SdPlanner {
                 if (zstd) zi++;
                 const int32_t z = zstd ? zi : -1;
                 uint64_t w = 0;
-                if (!e) e = frame_window_size(h, w);
-                if (!e && w > max_window) e = B200Z_ERR_WINDOW_SIZE_TOO_BIG;
                 const b200z_dict *dict = nullptr;
-                if (!e && h.has_dict_id) {
-                    for (size_t k = 0; k < ndicts; k++) if (dicts[k]->id == h.dict_id) dict = dicts[k];
-                    if (!dict) e = B200Z_ERR_DICT_NOT_PROVIDED;
-                }
+                if (!e) e = frame_window(h, max_window, w);
+                if (!e) e = frame_dict(h, dicts, ndicts, forced, dict);
                 if (e) { fail_at(p, mk_status((uint32_t)e, B200Z_STAGE_FRAME_HEADER), at, z); break; }
-                if (forced) dict = forced;
                 // the frame header goes with the frame's first block: cut in front of it when that block does not fit
                 BlockHeader bh;
                 bool have_bh = src.fill(pos + hs + 3), bh_ok = have_bh && !parse_block_header(src.buf + pos + hs, bh);
@@ -1559,20 +1617,16 @@ struct SdPlanner {
                 active = true;
             }
             // a block of the active frame
-            FrameDesc &fd = s.frames.back();
-            if (!src.fill(pos + 3)) { fd.host_status = mk_status(B200Z_ERR_BLOCK_HEADER_READ, B200Z_STAGE_BLOCK_HEADER); p.ends = true; break; }
             BlockHeader bh;
-            if (int e = parse_block_header(src.buf + pos, bh)) { fd.host_status = mk_status((uint32_t)e, B200Z_STAGE_BLOCK_HEADER); p.ends = true; break; }
-            if (!src.fill(pos + 3 + bh.content_size)) {
-                fd.host_status = mk_status(bh.type == BT_COMPRESSED ? B200Z_ERR_BLOCK_CONTENT_READ : B200Z_ERR_BLOCK_BODY_READ, B200Z_STAGE_BLOCK_BODY);
+            if (uint32_t w = read_block(src.fill(pos + 3) ? src.buf + pos : nullptr, bh, [&](uint32_t n) { return src.fill(pos + 3 + n); })) {
+                s.frames.back().host_status = w;
                 p.ends = true;
                 break;
             }
             const uint64_t in = 3 + bh.content_size + (bh.last && checksum ? 4 : 0), out = out_of(bh, window);
             const uint64_t seqs = seqs_of(bh, src.buf + pos + 3);
             if (!fits(p, in, out, seqs)) break;   // cut at this block end: the frame continues in the next submission
-            const BlockDesc &d = s.add_block(pos + 3, bh, (uint32_t)s.frames.size() - 1, bif++, src.buf + pos + 3, cur);
-            s.frames.back().nblocks++;
+            const BlockDesc &d = s.add_block(pos + 3, bh, bif++, src.buf + pos + 3, cur);
             pos += 3 + bh.content_size;
             p.in_bytes += 3 + bh.content_size; p.out_bound += out; p.nblocks++; p.nseq += seqs;
             if (d.host_status) { p.ends = true; break; }   // the frame fails at this block; nothing after it is looked at
@@ -1599,17 +1653,7 @@ struct SdPlanner {
             cont.next_block = bif;
             cont.dict = fdict;
             // the tables its next block starts from: a table built here is copied to the carry slots after the pass
-            auto fse_of = [](const FseSlot *sl, int which) -> const FseTab * { return which == 0 ? &sl->ll : (which == 1 ? &sl->of : &sl->ml); };
-            auto next_fse = [&](const TabRef &t, int which) -> const FseTab * {
-                if (t.kind == TabRef::SLOT) return fse_of(carry_fse, which);
-                if (t.kind == TabRef::PREDEF) return fse_of(predef, which);
-                if (t.kind == TabRef::CARRY) { const CarrySet &cs = s.carries[t.idx]; return which == 0 ? cs.ll : (which == 1 ? cs.of : cs.ml); }
-                return nullptr;
-            };
-            CarrySet next;
-            next.huf = cur.huf.kind == TabRef::SLOT ? carry_huf : (cur.huf.kind == TabRef::CARRY ? s.carries[cur.huf.idx].huf : nullptr);
-            next.ll = next_fse(cur.ll, 0); next.of = next_fse(cur.of, 1); next.ml = next_fse(cur.ml, 2);
-            cont.tables = next;
+            cont.tables = s.carry_after(cur, carry_huf, carry_fse, predef);
         }
     }
 };
@@ -1760,19 +1804,12 @@ extern "C" int b200z_decode_all_stream(b200z_ctx *c, b200z_read_fn rd, void *ru,
         if (hash)
             if (int le = launch_checksum_stream(a, d_carry + s, d_carry + (s ^ 1), p.resumed, p.continues, c->stream, &c->launches))
                 return c->set_cuda_err((cudaError_t)le, "k_xxh64_stream");
-        if (p.continues) {   // the continuing frame's tables built here, for the next submission (the host knows which: no wait)
-            const TableCursor &t = p.cur_end;
-            if (t.huf.kind == TabRef::SLOT)
-                CU(c, cudaMemcpyAsync(R->d_tab_huf.p, sub.d_huf.as<HufSlot>() + t.huf.idx, sizeof(HufSlot), cudaMemcpyDeviceToDevice, c->stream));
-            FseSlot *dst = R->d_tab_fse.as<FseSlot>();
-            const FseSlot *src_slots = sub.d_fse.as<FseSlot>();
-            if (t.ll.kind == TabRef::SLOT) CU(c, cudaMemcpyAsync(&dst->ll, &src_slots[t.ll.idx].ll, sizeof(FseTab), cudaMemcpyDeviceToDevice, c->stream));
-            if (t.of.kind == TabRef::SLOT) CU(c, cudaMemcpyAsync(&dst->of, &src_slots[t.of.idx].of, sizeof(FseTab), cudaMemcpyDeviceToDevice, c->stream));
-            if (t.ml.kind == TabRef::SLOT) CU(c, cudaMemcpyAsync(&dst->ml, &src_slots[t.ml.idx].ml, sizeof(FseTab), cudaMemcpyDeviceToDevice, c->stream));
-        }
+        // the continuing frame's tables built here, for the next submission (the host knows which: no wait)
+        if (p.continues)
+            if (int e = sub.copy_carry(c, p.cur_end, R->d_tab_huf.as<HufSlot>(), R->d_tab_fse.as<FseSlot>(), c->stream)) return e;
         CU(c, cudaEventRecord(R->ev_k[s], c->stream));
         CU(c, cudaStreamWaitEvent(R->s_d2h, R->ev_k[s], 0));
-        CU(c, cudaMemcpyAsync(R->h_states[s].p, sub.d_states.p, sub.frames.size() * sizeof(FrameState), cudaMemcpyDeviceToHost, R->s_d2h));
+        if (int e = sub.download_states(c, R->h_states[s].as<FrameState>(), R->s_d2h)) return e;
         CU(c, cudaEventRecord(R->ev_d2h[s], R->s_d2h));
         res.submissions++;
         return 0;
@@ -1800,7 +1837,7 @@ extern "C" int b200z_decode_all_stream(b200z_ctx *c, b200z_read_fn rd, void *ru,
                     const uint32_t n = std::min(st[f].blocks_done, fd.nblocks);
                     if (n) {
                         std::vector<BlockAux> aux(n);
-                        CU(c, cudaMemcpyAsync(aux.data(), sub.d_aux.as<BlockAux>() + fd.first_block, n * sizeof(BlockAux), cudaMemcpyDeviceToHost, R->s_out));
+                        if (int e = sub.download_aux(c, aux.data(), fd.first_block, n, R->s_out)) return e;
                         CU(c, cudaStreamSynchronize(R->s_out));
                         for (uint32_t k = 0; k < n; k++) len += aux[k].out_size;
                     }
@@ -1958,10 +1995,9 @@ extern "C" int b200z_decode_blocks_batch(b200z_ctx *c, const b200z_block_desc *b
                 if (sec.lit_off != 0 && (sec.lit_type != bd.literals_type || sec.regen_size != bd.regenerated_size)) return B200Z_ERR_INVALID_ARGUMENT;
                 if (!sec.status && (sec.nseq != bd.num_sequences || (sec.nseq && sec.modes != bd.modes))) return B200Z_ERR_INVALID_ARGUMENT;
             }
-            const BlockDesc &d = s.add_block(bd.src_off, bh, (uint32_t)f, k, sec, cur);
+            const BlockDesc &d = s.add_block(bd.src_off, bh, k, sec, cur);
             if (d.host_status) break;   // decompress_block would have returned here: later blocks of the frame are never reached
         }
-        s.frames.back().nblocks = (uint32_t)s.descs.size() - s.frames.back().first_block;
     }
     DevBuf d_in_own, d_out_own;
     const uint8_t *d_in = compressed;
@@ -1980,8 +2016,8 @@ extern "C" int b200z_decode_blocks_batch(b200z_ctx *c, const b200z_block_desc *b
         return e;
     std::vector<FrameState> st(s.states.size());
     std::vector<BlockAux> aux(s.descs.size());
-    if (!st.empty()) CU(c, cudaMemcpyAsync(st.data(), s.d_states.p, st.size() * sizeof(FrameState), cudaMemcpyDeviceToHost, c->stream));
-    if (!aux.empty()) CU(c, cudaMemcpyAsync(aux.data(), s.d_aux.p, aux.size() * sizeof(BlockAux), cudaMemcpyDeviceToHost, c->stream));
+    if (int e = s.download_states(c, st.data(), c->stream)) return e;
+    if (int e = s.download_aux(c, aux.data(), 0, aux.size(), c->stream)) return e;
     CU(c, cudaStreamSynchronize(c->stream));
     uint64_t lo = UINT64_MAX, hi = 0;
     for (size_t f = 0; f < nframes; f++) {
@@ -2071,7 +2107,7 @@ extern "C" void b200z_frame_decoder_free(b200z_frame_decoder *d) {
     delete d;
 }
 extern "C" void b200z_frame_decoder_set_max_window_size(b200z_frame_decoder *d, uint64_t n) {
-    d->max_window = std::min<uint64_t>(n, (1ull << 41) + 7 * (1ull << 38));
+    d->max_window = std::min<uint64_t>(n, MAX_WINDOW_SIZE);
 }
 extern "C" uint64_t b200z_frame_decoder_max_window_size(const b200z_frame_decoder *d) { return d->max_window; }
 extern "C" uint32_t b200z_frame_decoder_skip_frame_length(const b200z_frame_decoder *d) { return d->skip_len; }
@@ -2106,8 +2142,7 @@ extern "C" int b200z_frame_decoder_reset(b200z_frame_decoder *d, b200z_read_fn r
     if (e == B200Z_ERR_SKIP_FRAME) d->skip_len = skip;
     if (e) return fd_fail(d, e, B200Z_STAGE_FRAME_HEADER);
     uint64_t window = 0;
-    if ((e = frame_window_size(h, window))) return fd_fail(d, e, B200Z_STAGE_FRAME_HEADER);
-    if (window > d->max_window) return fd_fail(d, B200Z_ERR_WINDOW_SIZE_TOO_BIG, B200Z_STAGE_FRAME_HEADER);
+    if ((e = frame_window(h, d->max_window, window))) return fd_fail(d, e, B200Z_STAGE_FRAME_HEADER);
     // FrameDecoderState::new / reset (:103-134)
     d->hdr = h; d->window = window; d->frame_finished = false; d->block_counter = 0;
     d->bytes_read_counter = h.header_size; d->has_check_sum = false; d->using_dict = nullptr;
@@ -2186,23 +2221,15 @@ static int fd_reserve_out(b200z_frame_decoder *d, uint64_t extra) {
     return 0;
 }
 
-// Decode the blocks gathered in d->sub / d->staging on the GPU; updates produced/state/carry tables.
-// Returns 0 or the error of the first failing block (in which case *failed_block is its index in the submission).
-static int fd_submit(b200z_frame_decoder *d, const TableCursor &cur, uint32_t *failed_block, uint32_t *done_blocks) {
+// Decode the blocks gathered in d->sub (its one frame, opened by fd_decode_blocks_impl) / d->staging on the GPU; updates
+// produced/state/carry tables.  Returns 0 or the error of the first failing block; *done_blocks counts the blocks before it.
+static int fd_submit(b200z_frame_decoder *d, const TableCursor &cur, uint32_t *done_blocks) {
     b200z_ctx *c = d->ctx;
     Submission &s = d->sub;
     if (int e = c->use()) return e;
     int e;
     if ((e = d->d_input.ensure(d->staging.size() + 16))) return e;
     CU(c, cudaMemcpyAsync(d->d_input.p, d->staging.data(), d->staging.size(), cudaMemcpyHostToDevice, c->stream));
-    FrameDesc fd;
-    memset(&fd, 0, sizeof fd);
-    fd.out_off = 0; fd.window_size = d->window;
-    fd.dict = d->using_dict ? d->using_dict->d_content.as<uint8_t>() : nullptr; fd.dict_len = d->using_dict ? d->using_dict->content_len : 0;
-    fd.first_block = 0; fd.nblocks = (uint32_t)s.descs.size();
-    d->state.produced = d->produced; d->state.drained = d->drained; d->state.blocks_done = 0; d->state.status = 0;
-    s.frames.assign(1, fd); s.states.assign(1, d->state);
-    s.carries.assign(1, d->carry);
     if ((e = s.upload(c))) return e;
     // stage A: tables + literals + sequences; sizes come back so the output can grow before execution
     PipelineArgs a = s.args(d->d_input.as<uint8_t>(), nullptr, 0);
@@ -2210,7 +2237,7 @@ static int fd_submit(b200z_frame_decoder *d, const TableCursor &cur, uint32_t *f
     int le = launch_pipeline(a_dec, c->stream, &c->launches);
     if (le) return c->set_cuda_err((cudaError_t)le, "launch decode");
     std::vector<BlockAux> aux(s.descs.size());
-    CU(c, cudaMemcpyAsync(aux.data(), s.d_aux.p, aux.size() * sizeof(BlockAux), cudaMemcpyDeviceToHost, c->stream));
+    if ((e = s.download_aux(c, aux.data(), 0, aux.size(), c->stream))) return e;
     CU(c, cudaStreamSynchronize(c->stream));
     uint64_t extra = 0;
     for (size_t i = 0; i < aux.size(); i++) {   // blocks after the first failing one are never executed (nor looked at by the reference)
@@ -2226,32 +2253,18 @@ static int fd_submit(b200z_frame_decoder *d, const TableCursor &cur, uint32_t *f
     le = launch_pipeline(a_ex, c->stream, &c->launches);
     if (le) return c->set_cuda_err((cudaError_t)le, "launch exec");
     // carry the current tables over to the next submission (device-to-device, tables never visit the host)
-    CarrySet next;
-    if (cur.huf.kind == TabRef::SLOT) {
-        CU(c, cudaMemcpyAsync(d->d_carry_huf.p, s.d_huf.as<HufSlot>() + cur.huf.idx, sizeof(HufSlot), cudaMemcpyDeviceToDevice, c->stream));
-        next.huf = d->d_carry_huf.as<HufSlot>();
-    } else if (cur.huf.kind == TabRef::CARRY) next.huf = d->carry.huf;
-    auto carry_fse = [&](const TabRef &t, int which, FseTab *dst, const FseTab *old) -> const FseTab * {
-        const FseTab *src = nullptr;
-        if (t.kind == TabRef::SLOT) { const FseSlot *sl = s.d_fse.as<FseSlot>() + t.idx; src = which == 0 ? &sl->ll : (which == 1 ? &sl->of : &sl->ml); }
-        else if (t.kind == TabRef::PREDEF) { const FseSlot *sl = c->d_predef.as<FseSlot>(); return which == 0 ? &sl->ll : (which == 1 ? &sl->of : &sl->ml); }
-        else if (t.kind == TabRef::CARRY) return old;
-        else return nullptr;
-        if (cudaMemcpyAsync(dst, src, sizeof(FseTab), cudaMemcpyDeviceToDevice, c->stream) != cudaSuccess) return nullptr;
-        return dst;
-    };
-    FseSlot *cf = d->d_carry_fse.as<FseSlot>();
-    next.ll = carry_fse(cur.ll, 0, &cf->ll, d->carry.ll);
-    next.of = carry_fse(cur.of, 1, &cf->of, d->carry.of);
-    next.ml = carry_fse(cur.ml, 2, &cf->ml, d->carry.ml);
+    HufSlot *huf_to = d->d_carry_huf.as<HufSlot>();
+    FseSlot *fse_to = d->d_carry_fse.as<FseSlot>();
+    if ((e = s.copy_carry(c, cur, huf_to, fse_to, c->stream))) return e;
+    const CarrySet next = s.carry_after(cur, huf_to, fse_to, c->d_predef.as<FseSlot>());
     FrameState st;
-    CU(c, cudaMemcpyAsync(&st, s.d_states.p, sizeof(FrameState), cudaMemcpyDeviceToHost, c->stream));
+    if ((e = s.download_states(c, &st, c->stream))) return e;
     CU(c, cudaStreamSynchronize(c->stream));
     d->carry = next;
     d->state = st;
     d->produced = st.produced;
     *done_blocks = st.blocks_done;
-    if (st.status) { *failed_block = st.blocks_done; d->last_stage = (int)status_stage(st.status); return (int)status_code(st.status); }
+    if (st.status) { d->last_stage = (int)status_stage(st.status); return (int)status_code(st.status); }
     return 0;
 }
 
@@ -2270,37 +2283,35 @@ static int fd_decode_blocks_impl(b200z_frame_decoder *d, b200z_read_fn rd, void 
         Submission &s = d->sub;
         s.clear();
         d->staging.clear();
-        TableCursor cur;
-        cursor_from_carry(cur, d->carry, 0);
+        // the frame, resumed from the state and tables the last submission left (placement: fd_submit, once the output is sized)
+        d->state.produced = d->produced; d->state.drained = d->drained; d->state.blocks_done = 0; d->state.status = 0;
+        TableCursor cur = s.add_resumed_frame(d->state, d->window, d->using_dict.get(), d->carry);
         std::vector<uint64_t> bytes_after;  // bytes_read_counter after each gathered block
-        int pending_err = 0, pending_stage = 0;
+        uint32_t pending = 0;               // status word of the block that could not be read
         bool saw_last = false;
         uint64_t brc = d->bytes_read_counter;
         size_t gathered_target = strategy == B200Z_STRATEGY_UPTO_BYTES ? 1 : (strategy == B200Z_STRATEGY_UPTO_BLOCKS ? std::max<size_t>(n, 1) - (d->block_counter - block_counter_before) : SIZE_MAX);
         if (strategy == B200Z_STRATEGY_ALL) gathered_target = 4096;  // bound the staging buffer; loop continues
         while (s.descs.size() < gathered_target) {
             uint8_t hb[3];
-            if (!read_exact(rd, user, hb, 3)) { pending_err = B200Z_ERR_BLOCK_HEADER_READ; pending_stage = B200Z_STAGE_BLOCK_HEADER; break; }
             BlockHeader bh;
-            int e = parse_block_header(hb, bh);
-            if (e) { pending_err = e; pending_stage = B200Z_STAGE_BLOCK_HEADER; break; }
-            brc += 3;
-            size_t off = d->staging.size();
-            d->staging.resize(off + bh.content_size);
-            if (!read_exact(rd, user, d->staging.data() + off, bh.content_size)) {
+            const size_t off = d->staging.size();
+            auto read_body = [&](uint32_t len) {
+                d->staging.resize(off + len);
+                if (read_exact(rd, user, d->staging.data() + off, len)) return true;
                 d->staging.resize(off);
-                pending_err = bh.type == BT_COMPRESSED ? B200Z_ERR_BLOCK_CONTENT_READ : B200Z_ERR_BLOCK_BODY_READ; pending_stage = B200Z_STAGE_BLOCK_BODY;
-                break;
-            }
-            const BlockDesc &bd = s.add_block(off, bh, 0, (uint32_t)(d->block_counter + s.descs.size()), d->staging.data() + off, cur);
-            brc += bh.content_size;
+                return false;
+            };
+            if ((pending = read_block(read_exact(rd, user, hb, 3) ? hb : nullptr, bh, read_body))) break;
+            const BlockDesc &bd = s.add_block(off, bh, (uint32_t)(d->block_counter + s.descs.size()), d->staging.data() + off, cur);
+            brc += 3 + bh.content_size;
             bytes_after.push_back(brc);
             if (bd.host_status) break;
             if (bh.last) { saw_last = true; break; }
         }
-        uint32_t failed = 0, done = 0;
+        uint32_t done = 0;
         int e = 0;
-        if (!s.descs.empty()) e = fd_submit(d, cur, &failed, &done);
+        if (!s.descs.empty()) e = fd_submit(d, cur, &done);
         // counters exactly as the reference leaves them (:325-343)
         if (done > 0) d->bytes_read_counter = bytes_after[done - 1];
         d->block_counter += done;
@@ -2308,10 +2319,10 @@ static int fd_decode_blocks_impl(b200z_frame_decoder *d, b200z_read_fn rd, void 
             if (d->last_stage >= B200Z_STAGE_BLOCK_BODY && d->last_stage <= B200Z_STAGE_EXECUTE) d->bytes_read_counter += 3;
             return fd_fail(d, e, d->last_stage);
         }
-        if (pending_err) {
-            if (pending_stage == B200Z_STAGE_BLOCK_BODY) d->bytes_read_counter += 3;
-            d->state.status = mk_status((uint32_t)pending_err, (uint32_t)pending_stage);
-            return fd_fail(d, pending_err, pending_stage);
+        if (pending) {
+            if (status_stage(pending) == B200Z_STAGE_BLOCK_BODY) d->bytes_read_counter += 3;
+            d->state.status = pending;
+            return fd_fail(d, (int)status_code(pending), (int)status_stage(pending));
         }
         if (saw_last) {
             d->frame_finished = true;
