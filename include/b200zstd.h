@@ -494,6 +494,9 @@ uint32_t b200z_frame_decoder_skip_frame_length(const b200z_frame_decoder *d);
 int b200z_frame_decoder_add_dict(b200z_frame_decoder *d, const uint8_t *raw, size_t len);  /* decode_dict + add_dict :224 */
 int b200z_frame_decoder_add_raw_content_dict(b200z_frame_decoder *d, uint32_t id, const uint8_t *content, size_t len); /* EXTENSION */
 int b200z_frame_decoder_force_dict(b200z_frame_decoder *d, uint32_t dict_id);              /* :229 */
+/* Deviation: after an error, decode_blocks (and decode_from_to, and a StreamingDecoder's read) returns that error again until the
+ * decoder is reset.  The reference keeps no failed state and reads on from the next block header, with whatever tables the failed
+ * block left half built; some such frames make it panic (tests/errcraft.py, reentries()). */
 int b200z_frame_decoder_decode_blocks(b200z_frame_decoder *d, b200z_read_fn read_cb, void *user, int strategy,
                                       size_t n, int *finished);                            /* :309 */
 long b200z_frame_decoder_read(b200z_frame_decoder *d, uint8_t *buf, size_t len);           /* impl Read :615 */

@@ -300,6 +300,9 @@ static void fsed_new(fse_decoder *d, const fse_table *t) {                      
 static int fsed_init_state(fse_decoder *d, brr *bits) {                                           /* :32-40 */
     if (d->table->accuracy_log == 0) return ZO_ERR_FSE_TABLE_IS_UNINITIALIZED;
     uint64_t s = brr_get_bits(bits, d->table->accuracy_log);
+    /* decode[new_state] (:37) past the cells: a description that failed after setting accuracy_log (AccLogTooBig, :230-237)
+     * leaves the previous cells, or none; decode_blocks called again after that error reaches it through a Repeat mode */
+    if (s >= d->table->decode_len) return ZO_ERR_REFERENCE_WOULD_PANIC;
     d->state = d->table->decode[s];
     return 0;
 }

@@ -1052,6 +1052,35 @@ static int pipe_get(b200z_ctx *c, PipeResources **out) {
     return 0;
 }
 
+// Host output: copies the byte ranges [lo, hi) of `ranges` from the device output back to `output`, and nothing between them, so the
+// caller's bytes outside every frame's slot stay as they were.  Ranges that touch or overlap go back in one copy: frames packed back to
+// back cost one copy, as one range over all of them did.  Ranges apart from each other come back one copy each while there are few;
+// past that, one copy of their span lands in a host staging buffer and each range is copied out of it (one PCIe transfer, not one
+// per frame).  `sync`: the staging path and the caller need the bytes now; without it the direct copies stay queued on `stream`.
+static int copy_back_ranges(b200z_ctx *c, cudaStream_t stream, uint8_t *output, const uint8_t *d_out, std::vector<std::pair<uint64_t, uint64_t>> &ranges,
+                            bool sync) {
+    std::sort(ranges.begin(), ranges.end());
+    std::vector<std::pair<uint64_t, uint64_t>> merged;
+    for (const auto &r : ranges) {
+        if (r.second <= r.first) continue;
+        if (!merged.empty() && r.first <= merged.back().second) merged.back().second = std::max(merged.back().second, r.second);
+        else merged.push_back(r);
+    }
+    if (merged.empty()) return 0;
+    const size_t kDirect = 16;
+    if (merged.size() <= kDirect || !sync) {
+        for (const auto &r : merged) CU(c, cudaMemcpyAsync(output + r.first, d_out + r.first, r.second - r.first, cudaMemcpyDeviceToHost, stream));
+        if (sync) CU(c, cudaStreamSynchronize(stream));
+        return 0;
+    }
+    const uint64_t lo = merged.front().first, hi = merged.back().second;
+    std::vector<uint8_t> staging(hi - lo);
+    CU(c, cudaMemcpyAsync(staging.data(), d_out + lo, hi - lo, cudaMemcpyDeviceToHost, stream));
+    CU(c, cudaStreamSynchronize(stream));
+    for (const auto &r : merged) memcpy(output + r.first, staging.data() + (r.first - lo), r.second - r.first);
+    return 0;
+}
+
 static int decode_frames_pipelined(b200z_ctx *c, const uint8_t *input, size_t input_len, const b200z_frame_io *frames, size_t nframes,
                                    const b200z_dict *const *dicts, size_t ndicts, const b200z_dict *forced, uint64_t max_window, uint8_t *output,
                                    size_t output_cap, b200z_frame_result *results, size_t nchunks) {
@@ -1089,16 +1118,16 @@ static int decode_frames_pipelined(b200z_ctx *c, const uint8_t *input, size_t in
         if (int e = retire(s)) return e;
         b200z_batch *b = p->set[s].get();
         if (int e = plan_batch(b, input, input_len, frames + f0, f1 - f0, dicts, ndicts, forced, max_window)) return e;
-        // input byte range and output byte range of this chunk
-        uint64_t ilo = UINT64_MAX, ihi = 0, olo = UINT64_MAX, ohi = 0;
+        // input byte range and the output slots of this chunk (the frames' sizes are not known before the chunk retires)
+        uint64_t ilo = UINT64_MAX, ihi = 0;
+        std::vector<std::pair<uint64_t, uint64_t>> slots;
         for (size_t i = f0; i < f1; i++) {
             if (frames[i].src_off > input_len || frames[i].src_size > input_len - frames[i].src_off) continue;
             ilo = std::min<uint64_t>(ilo, frames[i].src_off); ihi = std::max<uint64_t>(ihi, frames[i].src_off + frames[i].src_size);
-            if (frames[i].out_cap) { olo = std::min<uint64_t>(olo, frames[i].out_off); ohi = std::max<uint64_t>(ohi, frames[i].out_off + frames[i].out_cap); }
+            if (frames[i].out_cap && frames[i].out_off < output_cap)
+                slots.emplace_back(frames[i].out_off, std::min<uint64_t>(frames[i].out_off + std::min<uint64_t>(frames[i].out_cap, output_cap), output_cap));
         }
         if (ihi < ilo) { ilo = ihi = 0; }
-        if (ohi < olo) { olo = ohi = 0; }
-        ohi = std::min<uint64_t>(ohi, output_cap); olo = std::min<uint64_t>(olo, ohi);
         if (int e = p->d_in[s].ensure(ihi - ilo + 32)) return e;
         if (ihi > ilo) CU(c, cudaMemcpyAsync(p->d_in[s].p, input + ilo, ihi - ilo, cudaMemcpyHostToDevice, p->s_h2d));
         if (int e = b->sub.upload(c, p->s_h2d)) return e;
@@ -1111,7 +1140,7 @@ static int decode_frames_pipelined(b200z_ctx *c, const uint8_t *input, size_t in
         CU(c, cudaStreamWaitEvent(p->s_d2h, p->ev_k[s], 0));
         if (int e = p->h_states[s].ensure(b->sub.states.size() * sizeof(FrameState))) return e;
         if (int e = b->sub.download_states(c, p->h_states[s].as<FrameState>(), p->s_d2h)) return e;
-        if (ohi > olo) CU(c, cudaMemcpyAsync(output + olo, d_out + olo, ohi - olo, cudaMemcpyDeviceToHost, p->s_d2h));
+        if (int e = copy_back_ranges(c, p->s_d2h, output, d_out, slots, false)) return e;
         CU(c, cudaEventRecord(p->ev_done[s], p->s_d2h));
         pend[s].f0 = f0; pend[s].f1 = f1; pend[s].live = true;
     }
@@ -1148,15 +1177,12 @@ extern "C" int b200z_decode_frames_batch(b200z_ctx *c, const uint8_t *input, siz
     if ((e = b200z_batch_run(b, dout, output_cap))) return e;
     if ((e = b200z_batch_finish(b, results))) return e;
     if (output_mem != B200Z_MEM_DEVICE) {
-        // one D2H covering every produced byte (frames are normally packed back to back by the caller)
-        uint64_t lo = UINT64_MAX, hi = 0;
+        // every frame's produced bytes (frames are normally packed back to back by the caller: one copy)
+        std::vector<std::pair<uint64_t, uint64_t>> produced;
         for (size_t i = 0; i < nframes; i++)
-            if (results[i].out_size) { lo = std::min<uint64_t>(lo, frames[i].out_off); hi = std::max<uint64_t>(hi, frames[i].out_off + results[i].out_size); }
-        if (hi > lo) {
-            hi = std::min<uint64_t>(hi, output_cap);
-            CU(c, cudaMemcpyAsync(output + lo, dout + lo, hi - lo, cudaMemcpyDeviceToHost, c->stream));
-            CU(c, cudaStreamSynchronize(c->stream));
-        }
+            if (results[i].out_size && frames[i].out_off < output_cap)
+                produced.emplace_back(frames[i].out_off, std::min<uint64_t>(frames[i].out_off + std::min<uint64_t>(results[i].out_size, frames[i].out_cap), output_cap));
+        if ((e = copy_back_ranges(c, c->stream, output, dout, produced, true))) return e;
     }
     return 0;
 }
@@ -2019,12 +2045,14 @@ extern "C" int b200z_decode_blocks_batch(b200z_ctx *c, const b200z_block_desc *b
     if (int e = s.download_states(c, st.data(), c->stream)) return e;
     if (int e = s.download_aux(c, aux.data(), 0, aux.size(), c->stream)) return e;
     CU(c, cudaStreamSynchronize(c->stream));
-    uint64_t lo = UINT64_MAX, hi = 0;
+    // host output: each frame's produced bytes come back (copy_back_ranges), so the caller's bytes between two frames' slots stay as they were
+    std::vector<std::pair<uint64_t, uint64_t>> copy_back;
     for (size_t f = 0; f < nframes; f++) {
         const b200z_block_frame &bf = frames[f];
         const FrameState &fs = st[f];
         if (frame_out_size) frame_out_size[f] = fs.produced;
-        if (fs.produced) { lo = std::min<uint64_t>(lo, bf.out_off); hi = std::max<uint64_t>(hi, bf.out_off + fs.produced); }
+        const uint64_t end = std::min<uint64_t>(bf.out_off + std::min<uint64_t>(fs.produced, bf.out_cap), output_cap);
+        if (end > bf.out_off) copy_back.emplace_back(bf.out_off, end);
         if (!status) continue;
         for (uint32_t k = 0; k < bf.num_blocks; k++) {
             b200z_block_status &o = status[bf.first_block + k];
@@ -2037,10 +2065,8 @@ extern "C" int b200z_decode_blocks_batch(b200z_ctx *c, const b200z_block_desc *b
             o.out_size = d.btype == BT_COMPRESSED ? aux[(size_t)si].out_size : d.raw_size;
         }
     }
-    if (output_mem != B200Z_MEM_DEVICE && hi > lo) {
-        hi = std::min<uint64_t>(hi, output_cap);
-        if (hi > lo) { CU(c, cudaMemcpyAsync(output + lo, d_out + lo, hi - lo, cudaMemcpyDeviceToHost, c->stream)); CU(c, cudaStreamSynchronize(c->stream)); }
-    }
+    if (output_mem != B200Z_MEM_DEVICE)
+        if (int e = copy_back_ranges(c, c->stream, output, d_out, copy_back, true)) return e;
     return 0;
 }
 
