@@ -2,9 +2,10 @@
 repeat-offset pass k_cenc<TABLES, true> runs before encoding, and the frame the compressor must write.
 
 This module restates the rules of zstd-rs_b200/csrc/compress.cu at B200Z_LEVEL_LAZY and DESIGN.md section 4.4 in Python, calling
-nothing in the library.  It shares the Fastest model's hashing, dictionary table, XXH64 and headers (tests/cparse.py).  `parse` gives
-what cparse.parse gives -- per block ("rle", byte, n) or (literals, [(ll, ml, of), ...]) with `of` the actual offset -- and `reps`
-turns a block's sequences into the records the encoder codes: `of` is then Offset_Value - 3 (mod 2^32).  The rules beyond the
+nothing in the library.  It shares the Fastest model's hashing, dictionary table, block and frame drivers, XXH64 and headers
+(tests/cparse.py): `LAZY` is the level cparse.parse and cparse.reference_frame take.  The parse is per block ("rle", byte, n) or
+(literals, [(ll, ml, of), ...]) with `of` the actual offset, and `reps` turns a block's sequences into the records the encoder
+codes: `of` is then Offset_Value - 3 (mod 2^32).  The rules beyond the
 Fastest parse's blocks, t1, segments, dictionary and packing:
 
   t1        as Fastest's, over hash5(p, 15).
@@ -28,16 +29,12 @@ Fastest parse's blocks, t1, segments, dictionary and packing:
             Offset_Value 1, 2, 3.  LL = 0: rep1 -> 1, rep2 -> 2, rep0 - 1 -> 3 (first that is known and equal).  Any other
             sequence is coded raw (o + 3).  The history then moves as the decoder moves it; unknown slots move like known ones.
 
-`reference_frame` assembles the LAZY frame with the host build of encode.cuh.  `cases()` builds the crafted inputs; each case's
-id names the rule it sits on."""
+`cases()` builds the crafted inputs; each case's id names the rule it sits on."""
 import random
-import struct
 
 import cparse
-import seqcraft
 
 BLOCK, WINDOW, MIN_MATCH, CM_WARPS = cparse.BLOCK, cparse.WINDOW, cparse.MIN_MATCH, cparse.CM_WARPS
-CD_LOG = cparse.CD_LOG
 LZ_T1_LOG = 15           # t1, the block's first occurrences (Fastest: 14)
 LZ_TAB_LOG = 10          # buckets of a segment's table
 LZ_WAYS = 6              # K: positions per bucket
@@ -48,23 +45,17 @@ LZ_LANE_COST = 3         # gain a later lane gives up per byte it starts later
 CSEG_SEQS = cparse.CSEG_SEQS
 
 
-def _mlen(a, i, b, j, lim):
-    n = 0
-    while n < lim and a[i + n] == b[j + n]:
-        n += 1
-    return n
-
-
 def _cost(o, rep):
     return 0 if rep else o.bit_length() - 1
 
 
-def _segment(F, base, n, back, s, e, t1, H14, H11, H17, dic):
-    """Parse of segment [s, e) of the block at F[base:base + n]: (literals, sequences, trailing literal count)."""
+def _segment(F, base, n, back, s, e, t1, H15, H10, H17, dic, pieces):
+    """Parse of segment [s, e) of the block at F[base:base + n] with its forced pieces [(cs, ce, off)] (empty: none): (literals,
+    sequences, trailing literal count)."""
     tab = {}
 
     def insert(q):
-        h = H11[base + q]
+        h = H10[base + q]
         b = tab.get(h)
         if b is None:
             tab[h] = [q]
@@ -77,126 +68,91 @@ def _segment(F, base, n, back, s, e, t1, H14, H11, H17, dic):
     reps = []
     seqs, lits = [], []
     p = anchor = s
-    last = e - MIN_MATCH + 1                    # lanes q < last have q + 5 <= e
 
-    def lane(q):
-        """The lane's best candidate (gain, ml, off, xlim), or None."""
-        fq = base + q
-        lim = min(LZ_CAP, e - q)
-        best = None
-        for o in reps:
-            if o <= back + q and o <= WINDOW:
-                ml = _mlen(F, fq, F, fq - o, lim)
-                if ml >= MIN_MATCH and (best is None or 4 * ml > best[0]):
-                    best = (4 * ml, ml, o, e - q)
-        cands = []
-        c1 = t1[H14[fq]]
-        if c1 < q:
-            cands.append(c1)
-        cands += [c for c in tab.get(H11[fq], ()) if c < q]
-        for c in cands:
-            o = q - c
-            ml = _mlen(F, fq, F, fq - o, lim)
-            if ml >= MIN_MATCH:
-                g = 4 * ml - _cost(o, False)
-                if best is None or g > best[0]:
-                    best = (g, ml, o, e - q)
-        if dic is not None and back + q < WINDOW:
-            d = dic.tab.get(H17[fq])
-            if d is not None and back + q + dic.n - d <= WINDOW:
-                o, rest = back + q + dic.n - d, dic.n - d
-                ml = _mlen(F, fq, dic.data, d, min(lim, rest))
-                if ml >= MIN_MATCH:
-                    g = 4 * ml - _cost(o, False)
-                    if best is None or g > best[0]:
-                        best = (g, ml, o, min(e - q, rest))
-        return best
-
-    while p < last:
-        hi = min(p + 32, last)
-        found = None
-        for q in range(p, hi):
-            c = lane(q)
-            if c is not None:
-                found = (q, c)
-                break
-        if found is not None:
-            j = found[0]
-            score = found[1][0]
-            for q in range(j + 1, min(j + LZ_DEPTH + 1, hi)):
-                c = lane(q)
-                if c is not None and c[0] - LZ_LANE_COST * (q - j) > score:
-                    found, score = (q, c), c[0] - LZ_LANE_COST * (q - j)
-        for q in range(p, hi):                  # every valid lane inserts, before or after the chosen one
-            insert(q)
-        if found is None:
-            p += 32
-            continue
-        q, (_, ml, off, xlim) = found
-        if ml == LZ_CAP:
-            fq = base + q
-            if off > back + q:                  # the source lies in the dictionary: stop at its end
-                ref, r0 = dic.data, dic.n - (off - (back + q))
-            else:
-                ref, r0 = F, fq - off
-            while ml < xlim and F[fq + ml] == ref[r0 + ml]:
-                ml += 1
-        lits.append(F[base + anchor:base + q])
-        seqs.append((q - anchor, ml, off))
+    def take(off):
         if off in reps:
             reps.remove(off)
         reps.insert(0, off)
         del reps[3:]
-        anchor = p = q + ml
+
+    def lane(q, stop):
+        """The lane's best candidate (gain, ml, off, xlim), or None."""
+        fq = base + q
+        lim = min(LZ_CAP, stop - q)
+        best = None
+        for o in reps:
+            if o <= back + q and o <= WINDOW:
+                ml = cparse._mlen(F, fq, F, fq - o, lim)
+                if ml >= MIN_MATCH and (best is None or 4 * ml > best[0]):
+                    best = (4 * ml, ml, o, stop - q)
+        cands = []
+        c1 = t1[H15[fq]]
+        if c1 < q:
+            cands.append(c1)
+        cands += [c for c in tab.get(H10[fq], ()) if c < q]
+        for c in cands:
+            o = q - c
+            ml = cparse._mlen(F, fq, F, fq - o, lim)
+            if ml >= MIN_MATCH:
+                g = 4 * ml - _cost(o, False)
+                if best is None or g > best[0]:
+                    best = (g, ml, o, stop - q)
+        if dic is not None and back + q < WINDOW:
+            d = dic.tab.get(H17[fq])
+            if d is not None and back + q + dic.n - d <= WINDOW:
+                o, rest = back + q + dic.n - d, dic.n - d
+                ml = cparse._mlen(F, fq, dic.data, d, min(lim, rest))
+                if ml >= MIN_MATCH:
+                    g = 4 * ml - _cost(o, False)
+                    if best is None or g > best[0]:
+                        best = (g, ml, o, min(stop - q, rest))
+        return best
+
+    for k in range(len(pieces) + 1):
+        stop = pieces[k][0] if k < len(pieces) else e   # the parse runs up to the next piece's start
+        last = stop - MIN_MATCH + 1             # lanes q < last have q + 5 <= stop
+        while p < last:
+            hi = min(p + 32, last)
+            found = None
+            for q in range(p, hi):
+                c = lane(q, stop)
+                if c is not None:
+                    found = (q, c)
+                    break
+            if found is not None:
+                j = found[0]
+                score = found[1][0]
+                for q in range(j + 1, min(j + LZ_DEPTH + 1, hi)):
+                    c = lane(q, stop)
+                    if c is not None and c[0] - LZ_LANE_COST * (q - j) > score:
+                        found, score = (q, c), c[0] - LZ_LANE_COST * (q - j)
+            for q in range(p, hi):              # every valid lane inserts, before or after the chosen one
+                insert(q)
+            if found is None:
+                p += 32
+                continue
+            q, (_, ml, off, xlim) = found
+            if ml == LZ_CAP:
+                fq = base + q
+                if off > back + q:              # the source lies in the dictionary: stop at its end
+                    ref, r0 = dic.data, dic.n - (off - (back + q))
+                else:
+                    ref, r0 = F, fq - off
+                while ml < xlim and F[fq + ml] == ref[r0 + ml]:
+                    ml += 1
+            lits.append(F[base + anchor:base + q])
+            seqs.append((q - anchor, ml, off))
+            take(off)
+            anchor = p = q + ml
+        if k < len(pieces):                     # the piece is one sequence and a repeat offset; the parse resumes at its end
+            cs, ce, off = pieces[k]
+            lits.append(F[base + anchor:base + cs])
+            seqs.append((cs - anchor, ce - cs, off))
+            take(off)
+            anchor = p = ce
     lits.append(F[base + anchor:base + e])
     assert len(seqs) <= CSEG_SEQS
     return b"".join(lits), seqs, e - anchor
-
-
-def parse_block(F, base, n, back, H14, H11, H17, dic):
-    """One block of frame F: ("rle", byte, n), or (literals, [(ll, ml, of), ...]); (b"", []) for the empty block."""
-    blk = F[base:base + n]
-    if n == 0:
-        return (b"", [])
-    if blk.count(blk[:1]) == n:
-        return ("rle", blk[0], n)
-    t1 = [BLOCK] * (1 << LZ_T1_LOG)
-    for q in range(n - MIN_MATCH, -1, -1):      # the smallest position wins
-        t1[H14[base + q]] = q
-    seglen = -(-n // CM_WARPS)
-    lits, seqs, carry = [], [], 0
-    for w in range(CM_WARPS):
-        s = min(n, w * seglen)
-        e = min(n, s + seglen)
-        sl, ss, trail = _segment(F, base, n, back, s, e, t1, H14, H11, H17, dic)
-        lits.append(sl)
-        if ss:
-            ss[0] = (ss[0][0] + carry, ss[0][1], ss[0][2])
-            carry = trail
-        else:
-            carry += trail
-        seqs += ss
-    return (b"".join(lits), seqs)
-
-
-def parse_frame(data, dic=None):
-    """The blocks of one frame (see parse_block); dic: a cparse.Dictionary or None."""
-    F = bytes(data)
-    H14, H11 = cparse.hashes(F, LZ_T1_LOG), cparse.hashes(F, LZ_TAB_LOG)
-    H17 = cparse.hashes(F[:WINDOW + 4], CD_LOG) if dic is not None else None
-    out, pos = [], 0
-    while True:
-        n = min(BLOCK, len(F) - pos)
-        out.append(parse_block(F, pos, n, min(pos, WINDOW), H14, H11, H17, dic))
-        pos += n
-        if pos >= len(F):
-            return out
-
-
-def parse(frames, content=None):
-    """The LAZY parse of every frame of one submission, against a dictionary's content (raw content or a formatted one's)."""
-    dic = cparse.match_dict(content)
-    return [parse_frame(f, dic) for f in frames]
 
 
 def reps(seqs):
@@ -228,33 +184,7 @@ def records(seqs):
     return [(ll, ml, (ov - 3) & 0xFFFFFFFF) for ll, ml, ov in reps(seqs)]
 
 
-def reference_frame(data, blocks, checksum=True, dict_id=0, dict_tables=None):
-    """The LAZY frame for `data` whose parse is `blocks` (parse_frame); dict_tables as cparse.reference_frame."""
-    data = bytes(data)
-    out = cparse.frame_header(len(data), checksum, dict_id)
-    pos = 0
-    for k, b in enumerate(blocks):
-        last = 1 if k + 1 == len(blocks) else 0
-        n = min(BLOCK, len(data) - pos)
-        raw = data[pos:pos + n]
-        if b[0] == "rle":
-            out += struct.pack("<I", last | (1 << 1) | (n << 3))[:3] + bytes([b[1]])
-        else:
-            content = None
-            if n:
-                recs = records(b[1])
-                if dict_tables is not None and k == 0:
-                    content = cparse.encode_with_tables(dict_tables, b[0], recs)
-                else:
-                    content = seqcraft.encode(b[0], recs)[0]
-            if content is not None and len(content) < n:
-                out += struct.pack("<I", last | (2 << 1) | (len(content) << 3))[:3] + content
-            else:
-                out += struct.pack("<I", last | (n << 3))[:3] + raw
-        pos += n
-    if checksum:
-        out += struct.pack("<I", cparse.xxh64(data) & 0xFFFFFFFF)
-    return out
+LAZY = cparse.Level(LZ_T1_LOG, LZ_TAB_LOG, _segment, records)
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -263,16 +193,13 @@ def reference_frame(data, blocks, checksum=True, dict_id=0, dict_tables=None):
 Case, rand, plant, seg_bounds = cparse.Case, cparse.rand, cparse.plant, cparse.seg_bounds
 
 
-def hash5(buf, p, log):
-    return cparse.hash5(buf, p, log)
-
-
 def keep_in_table(buf, first, dst, protect):
     """Changes bytes of buf so that no position in (first, dst) shares position first's bucket with other bytes: its entry is then
     still in the table when the lane at dst looks it up.  Bytes in `protect` are left alone."""
-    target = hash5(buf, first, LZ_TAB_LOG)
+    target = cparse.hash5(buf, first, LZ_TAB_LOG)
     while True:
-        bad = [p for p in range(first + 1, dst) if hash5(buf, p, LZ_TAB_LOG) == target and buf[p:p + 5] != buf[first:first + 5]]
+        bad = [p for p in range(first + 1, dst)
+               if cparse.hash5(buf, p, LZ_TAB_LOG) == target and buf[p:p + 5] != buf[first:first + 5]]
         if not bad:
             return
         for p in bad:
@@ -342,13 +269,13 @@ def buckets(rng):
         plant(buf, z, a, 20)
         protect = set(range(a - 1, a + 21)) | set(range(z - 1, z + 21))
         keep_in_table(buf, a, z, protect)
-        target = hash5(buf, a, LZ_TAB_LOG)
+        target = cparse.hash5(buf, a, LZ_TAB_LOG)
         at = BLOCK + 500
         for _ in range(extra):                  # 5 random bytes with the source's bucket, 100 bytes apart
             while True:
                 cand = bytes(rng.getrandbits(8) for _ in range(5))
                 tmp = bytearray(cand)
-                if hash5(tmp, 0, LZ_TAB_LOG) == target:
+                if cparse.hash5(tmp, 0, LZ_TAB_LOG) == target:
                     break
             buf[at:at + 5] = cand
             at += 100

@@ -25,11 +25,15 @@ the library.  `parse` gives, for every 128 KiB block of every frame of a submiss
             replaces the in-frame candidate when longer, or as long with a smaller offset.
   packing   a segment's trailing literals join the next segment's first sequence, across any segments without sequences; the
             last segments' literals are the block's trailing literals.
+  header    Single_Segment 0; Window_Descriptor exponent min(window_log, max(17, ceil(log2 n))), mantissa 0.
 
-`reference_frame` assembles the frame from the parse (header, blocks through the host build of encode.cuh, checksum), and `xxh64`
-is XXH64 with seed 0.  `cases()` builds the crafted inputs the tests run; each case's id names the constant it sits on."""
+The block and frame drivers are shared by every level: a `Level` names its hash logs, its segment loop (`_segment` here, LAZY's in
+tests/clazy.py) and the records its blocks are coded from.  A segment loop also takes the segment's forced pieces, the long matches
+of tests/cldm.py clipped to it (none at window_log 17).  `reference_frame` assembles the frame from the parse (header, blocks
+through the host build of encode.cuh, checksum), and `xxh64` is XXH64 with seed 0.  `cases()` builds the crafted inputs the tests run; each case's id names the constant it sits on."""
 import atexit
 import bisect
+import collections
 import os
 import random
 import shutil
@@ -43,6 +47,7 @@ import seqcraft
 
 BLOCK = 131072          # ENC_BLOCK
 WINDOW = 131072         # ENC_WINDOW
+WINDOW_LOG_MIN = 17     # B200Z_WINDOW_LOG_MIN (2^17 = WINDOW)
 MIN_MATCH = 5           # ENC_MIN_MATCH
 CM_WARPS = 8            # segments per block
 CM_T1_LOG, CM_TP_LOG, CD_LOG = 14, 12, 17
@@ -90,80 +95,114 @@ def _mlen(a, i, b, j, lim):
     return n
 
 
-def _segment(F, base, n, back, s, e, t1, H14, H12, H17, dic):
-    """Parse of segment [s, e) of the block at F[base:base + n]: (literals, sequences, trailing literal count)."""
+def _segment(F, base, n, back, s, e, t1, H14, H12, H17, dic, pieces):
+    """Parse of segment [s, e) of the block at F[base:base + n] with its forced pieces [(cs, ce, off)] (empty: none): (literals,
+    sequences, trailing literal count)."""
     tp = {}
     for q in range(max(s - CM_SEED, -min(back, CM_SEED)), min(s, n - MIN_MATCH + 1)):
         tp[H12[base + q]] = q
     seqs, lits = [], []
     p = anchor = s
-    last = e - MIN_MATCH + 1                    # lanes q < last have q + 5 <= e
-    while p < last:
-        hi = min(p + 32, last)
-        found = None
-        for q in range(p, hi):
-            fq = base + q
-            lim = min(CM_CAP, e - q)
-            best = cand = 0
-            c1 = t1[H14[fq]]
-            if c1 < q:
-                best, cand = _mlen(F, fq, F, base + c1, lim), q - c1
-            c2 = tp.get(H12[fq])
-            if c2 is not None and c2 < q and q - c2 <= WINDOW:
-                l2 = _mlen(F, fq, F, base + c2, lim)
-                if l2 > best or (l2 == best and q - c2 < cand):
-                    best, cand = l2, q - c2
-            xlim = e - q
-            if dic is not None and back + q < WINDOW:
-                d = dic.tab.get(H17[fq])
-                if d is not None and back + q + dic.n - d <= WINDOW:
-                    off3, rest = back + q + dic.n - d, dic.n - d
-                    l3 = _mlen(F, fq, dic.data, d, min(lim, rest))
-                    if l3 > best or (l3 == best and off3 < cand):
-                        best, cand, xlim = l3, off3, min(xlim, rest)
-            if best >= MIN_MATCH:
-                found = (q, best, cand, xlim)
-                break
-        for q in range(p, hi):                  # every valid lane inserts, before or after the chosen one
-            h = H12[base + q]
-            if tp.get(h, -WINDOW - 1) < q:
-                tp[h] = q
-        if found is None:
-            p += 32
-            continue
-        q, ml, off, xlim = found
-        if ml == CM_CAP:
-            fq = base + q
-            if off > back + q:                  # the source lies in the dictionary: stop at its end
-                ref, r0 = dic.data, dic.n - (off - (back + q))
-            else:
-                ref, r0 = F, fq - off
-            while ml < xlim and F[fq + ml] == ref[r0 + ml]:
-                ml += 1
-        lits.append(F[base + anchor:base + q])
-        seqs.append((q - anchor, ml, off))
-        anchor = p = q + ml
+    for k in range(len(pieces) + 1):
+        stop = pieces[k][0] if k < len(pieces) else e   # the parse runs up to the next piece's start
+        last = stop - MIN_MATCH + 1             # lanes q < last have q + 5 <= stop
+        while p < last:
+            hi = min(p + 32, last)
+            found = None
+            for q in range(p, hi):
+                fq = base + q
+                lim = min(CM_CAP, stop - q)
+                best = cand = 0
+                c1 = t1[H14[fq]]
+                if c1 < q:
+                    best, cand = _mlen(F, fq, F, base + c1, lim), q - c1
+                c2 = tp.get(H12[fq])
+                if c2 is not None and c2 < q and q - c2 <= WINDOW:
+                    l2 = _mlen(F, fq, F, base + c2, lim)
+                    if l2 > best or (l2 == best and q - c2 < cand):
+                        best, cand = l2, q - c2
+                xlim = stop - q
+                if dic is not None and back + q < WINDOW:
+                    d = dic.tab.get(H17[fq])
+                    if d is not None and back + q + dic.n - d <= WINDOW:
+                        off3, rest = back + q + dic.n - d, dic.n - d
+                        l3 = _mlen(F, fq, dic.data, d, min(lim, rest))
+                        if l3 > best or (l3 == best and off3 < cand):
+                            best, cand, xlim = l3, off3, min(xlim, rest)
+                if best >= MIN_MATCH:
+                    found = (q, best, cand, xlim)
+                    break
+            for q in range(p, hi):              # every valid lane inserts, before or after the chosen one
+                h = H12[base + q]
+                if tp.get(h, -WINDOW - 1) < q:
+                    tp[h] = q
+            if found is None:
+                p += 32
+                continue
+            q, ml, off, xlim = found
+            if ml == CM_CAP:
+                fq = base + q
+                if off > back + q:              # the source lies in the dictionary: stop at its end
+                    ref, r0 = dic.data, dic.n - (off - (back + q))
+                else:
+                    ref, r0 = F, fq - off
+                while ml < xlim and F[fq + ml] == ref[r0 + ml]:
+                    ml += 1
+            lits.append(F[base + anchor:base + q])
+            seqs.append((q - anchor, ml, off))
+            anchor = p = q + ml
+        if k < len(pieces):                     # the piece is one sequence; the parse resumes at its end
+            cs, ce, off = pieces[k]
+            lits.append(F[base + anchor:base + cs])
+            seqs.append((cs - anchor, ce - cs, off))
+            anchor = p = ce
     lits.append(F[base + anchor:base + e])
     assert len(seqs) <= CSEG_SEQS
     return b"".join(lits), seqs, e - anchor
 
 
-def parse_block(F, base, n, back, H14, H12, H17, dic):
-    """One block of frame F: ("rle", byte, n), or (literals, [(ll, ml, of), ...]); (b"", []) for the empty block."""
+def raw_offsets(seqs):
+    """Fastest's records: every offset is coded raw (Offset_Value = of + 3), so the encoder takes the sequences as parsed."""
+    return seqs
+
+
+# A level's parse: the hash logs of its t1 and of its segments' tables, its segment loop, and the records its blocks are coded
+# from (reference_frame).  UNCOMPRESSED has no parse: every block is Raw.
+Level = collections.namedtuple("Level", "t1_log tab_log segment records")
+FASTEST = Level(CM_T1_LOG, CM_TP_LOG, _segment, raw_offsets)
+UNCOMPRESSED = None
+
+
+def _pieces(kept, s, e):
+    """A block's kept long matches [(start, length, offset)] clipped to segment [s, e): [(cs, ce, off)], pieces under MIN_MATCH
+    bytes dropped."""
+    out = []
+    for st, ln, off in kept:
+        if st >= e:
+            break
+        cs, ce = max(st, s), min(st + ln, e)
+        if ce >= cs + MIN_MATCH:
+            out.append((cs, ce, off))
+    return out
+
+
+def parse_block(F, base, n, back, level, H_t1, H_tab, H17, dic, kept=()):
+    """One block of frame F: ("rle", byte, n), or (literals, [(ll, ml, of), ...]); (b"", []) for the empty block.  kept: the
+    block's long matches (tests/cldm.py), taken as forced pieces."""
     blk = F[base:base + n]
     if n == 0:
         return (b"", [])
     if blk.count(blk[:1]) == n:
         return ("rle", blk[0], n)
-    t1 = [BLOCK] * (1 << CM_T1_LOG)
+    t1 = [BLOCK] * (1 << level.t1_log)
     for q in range(n - MIN_MATCH, -1, -1):      # the smallest position wins
-        t1[H14[base + q]] = q
+        t1[H_t1[base + q]] = q
     seglen = -(-n // CM_WARPS)
     lits, seqs, carry = [], [], 0
     for w in range(CM_WARPS):
         s = min(n, w * seglen)
         e = min(n, s + seglen)
-        sl, ss, trail = _segment(F, base, n, back, s, e, t1, H14, H12, H17, dic)
+        sl, ss, trail = level.segment(F, base, n, back, s, e, t1, H_t1, H_tab, H17, dic, _pieces(kept, s, e))
         lits.append(sl)
         if ss:
             ss[0] = (ss[0][0] + carry, ss[0][1], ss[0][2])
@@ -174,15 +213,16 @@ def parse_block(F, base, n, back, H14, H12, H17, dic):
     return (b"".join(lits), seqs)
 
 
-def parse_frame(data, dic=None):
-    """The blocks of one frame (see parse_block); dic: a Dictionary or None."""
+def parse_frame(data, level=FASTEST, dic=None, kept=None):
+    """The blocks of one frame at `level` (see parse_block); dic: a Dictionary or None; kept: the frame's long matches, one list
+    per block (cldm.forced), or None."""
     F = bytes(data)
-    H14, H12 = hashes(F, CM_T1_LOG), hashes(F, CM_TP_LOG)
+    H_t1, H_tab = hashes(F, level.t1_log), hashes(F, level.tab_log)
     H17 = hashes(F[:WINDOW + 4], CD_LOG) if dic is not None else None
     out, pos = [], 0
     while True:
         n = min(BLOCK, len(F) - pos)
-        out.append(parse_block(F, pos, n, min(pos, WINDOW), H14, H12, H17, dic))
+        out.append(parse_block(F, pos, n, min(pos, WINDOW), level, H_t1, H_tab, H17, dic, kept[len(out)] if kept else ()))
         pos += n
         if pos >= len(F):
             return out
@@ -193,10 +233,11 @@ def match_dict(content):
     return Dictionary(content) if content is not None and len(content) >= MIN_MATCH else None
 
 
-def parse(frames, content=None):
-    """The parse of every frame of one submission, against a dictionary's content (raw content or a formatted dictionary's)."""
+def parse(frames, content=None, level=FASTEST, kept=None):
+    """The parse of every frame of one submission at `level`, against a dictionary's content (raw content or a formatted
+    dictionary's); kept: per frame, its long matches per block (cldm.forced), or None."""
     dic = match_dict(content)
-    return [parse_frame(f, dic) for f in frames]
+    return [parse_frame(f, level, dic, kept[i] if kept else None) for i, f in enumerate(frames)]
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
@@ -280,34 +321,48 @@ def dict_id_field(dict_id):
     return 0 if dict_id == 0 else 1 if dict_id < 256 else 2 if dict_id < 65536 else 4
 
 
-def frame_header(n, checksum, dict_id=0):
-    """Single_Segment 0, 128 KiB window, the dictionary ID in its smallest field, Frame_Content_Size in its smallest legal one."""
+def frame_window_log(n, window_log):
+    """The Window_Descriptor exponent of a frame of n bytes compressed at window_log: min(window_log, max(17, ceil(log2 n)))."""
+    if window_log <= WINDOW_LOG_MIN:
+        return WINDOW_LOG_MIN
+    c = WINDOW_LOG_MIN
+    while c < window_log and (1 << c) < n:
+        c += 1
+    return c
+
+
+def frame_header(n, checksum, dict_id=0, window_log=WINDOW_LOG_MIN):
+    """Single_Segment 0, the window of frame_window_log (mantissa 0), the dictionary ID in its smallest field, Frame_Content_Size
+    in its smallest legal one."""
     did = dict_id_field(dict_id)
     fcs = struct.pack("<H", n - 256) if 256 <= n <= 65791 else struct.pack("<Q", n) if n >> 32 else struct.pack("<I", n)
     flag = {2: 1, 4: 2, 8: 3}[len(fcs)]
     fhd = (flag << 6) | (4 if checksum else 0) | {0: 0, 1: 1, 2: 2, 4: 3}[did]
-    return struct.pack("<IBB", 0xFD2FB528, fhd, 7 << 3) + dict_id.to_bytes(did, "little") + fcs
+    wd = (frame_window_log(n, window_log) - 10) << 3
+    return struct.pack("<IBB", 0xFD2FB528, fhd, wd) + dict_id.to_bytes(did, "little") + fcs
 
 
-def reference_frame(data, blocks, checksum=True, dict_id=0, dict_tables=None, level=1):
-    """The frame the compressor must write for `data` whose parse is `blocks` (parse_frame).  level 0 writes every block Raw.
-    dict_tables: the formatted dictionary whose tables code the frame's first block (compress_frames(..., dict_tables=True))."""
+def reference_frame(data, blocks, checksum=True, dict_id=0, dict_tables=None, level=FASTEST, window_log=WINDOW_LOG_MIN):
+    """The frame the compressor must write for `data` whose parse at `level` is `blocks` (parse_frame) at window_log.  At
+    UNCOMPRESSED every block is Raw.  dict_tables: the formatted dictionary whose tables code the frame's first block
+    (compress_frames(..., dict_tables=True))."""
     data = bytes(data)
-    out = frame_header(len(data), checksum, dict_id)
+    out = frame_header(len(data), checksum, dict_id, window_log)
     pos = 0
     for k, b in enumerate(blocks):
         last = 1 if k + 1 == len(blocks) else 0
         n = min(BLOCK, len(data) - pos)
         raw = data[pos:pos + n]
-        if level and b[0] == "rle":
+        if level is not UNCOMPRESSED and b[0] == "rle":
             out += struct.pack("<I", last | (1 << 1) | (n << 3))[:3] + bytes([b[1]])
         else:
             content = None
-            if level and n:
+            if level is not UNCOMPRESSED and n:
+                recs = level.records(b[1])
                 if dict_tables is not None and k == 0:
-                    content = encode_with_tables(dict_tables, b[0], b[1])
+                    content = encode_with_tables(dict_tables, b[0], recs)
                 else:
-                    content = seqcraft.encode(b[0], b[1])[0]
+                    content = seqcraft.encode(b[0], recs)[0]
             if content is not None and len(content) < n:
                 out += struct.pack("<I", last | (2 << 1) | (len(content) << 3))[:3] + content
             else:
@@ -332,7 +387,7 @@ def counts(samples, content):
     dic = match_dict(content)
     cnt = np.zeros(DS_BINS, dtype=np.uint64)
     for smp in samples:
-        b = parse_frame(bytes(smp)[:BLOCK], dic)[0]
+        b = parse_frame(bytes(smp)[:BLOCK], FASTEST, dic)[0]
         if b[0] == "rle":
             continue
         lits, seqs = b

@@ -1,7 +1,7 @@
 // Host-side driver of the compressor's Window_Descriptor rule (frame_window_log and write_frame_header in
 // zstd-rs_b200/csrc/encode.cuh), read back with the decoder's parser (parse_frame_header in zstd-rs_b200/csrc/framing.cuh).
 // Arguments: a list of "<content size>:<window_log>".  Prints one line per case: "<header hex> <frame_window_log> <parse status>
-// <window size>"; tests/test_cldm_model.py checks it against tests/cldm.py.
+// <window size>"; tests/test_cldm_model.py checks it against tests/cparse.py.
 #include <cinttypes>
 #include <cstdint>
 #include <cstdio>

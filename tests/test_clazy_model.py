@@ -18,7 +18,7 @@ _parsed = {}
 
 def parsed(c):
     if c.id not in _parsed:
-        _parsed[c.id] = clazy.parse(c.frames, c.content)
+        _parsed[c.id] = cparse.parse(c.frames, c.content, clazy.LAZY)
     return _parsed[c.id]
 
 
@@ -77,7 +77,7 @@ def traced(oracle, f, content=None):
 def test_reference_frame_decodes(oracle, c):
     reps = 0
     for data, blocks in zip(c.frames, parsed(c)):
-        f = clazy.reference_frame(data, blocks)
+        f = cparse.reference_frame(data, blocks, level=clazy.LAZY)
         assert datagen.decompress(f, len(data), raw_dict=c.content) == data
         assert oracle.decode_frame(f, raw_dict=c.content)[0] == data
         seqs = traced(oracle, f, c.content)
@@ -90,16 +90,16 @@ def test_reference_frame_decodes(oracle, c):
 def test_hand_computed_parses():
     # 40 bytes: seglen 5; segment 1 repeats segment 0 (found through t1), its literals carry on
     d = bytes(range(0x20, 0x25)) * 2 + bytes(range(0x60, 0x7e))
-    assert clazy.parse([d]) == [[(d[:5] + d[10:], [(5, 5, 5)])]]
+    assert cparse.parse([d], level=clazy.LAZY) == [[(d[:5] + d[10:], [(5, 5, 5)])]]
     # 256 bytes: seglen 32; a 40-byte repeat inside segment 3 from segment 0 is verified to 32 = e - q and not extended
     d = bytearray(range(256))
     d[100:128] = d[4:32]
     d = bytes(d)
-    assert clazy.parse([d])[0][0][1] == [(100, 28, 96)]
+    assert cparse.parse([d], level=clazy.LAZY)[0][0][1] == [(100, 28, 96)]
     # a dictionary of 5 bytes; all equal, empty, too short
     d = b"hello" + bytes(range(0x60, 0x83))
-    assert clazy.parse([d], b"hello") == [[(d[5:], [(0, 5, 5)])]]
-    assert clazy.parse([b"zzzz", b"", b"abcd"]) == [[("rle", ord("z"), 4)], [(b"", [])], [(b"abcd", [])]]
+    assert cparse.parse([d], b"hello", clazy.LAZY) == [[(d[5:], [(0, 5, 5)])]]
+    assert cparse.parse([b"zzzz", b"", b"abcd"], level=clazy.LAZY) == [[("rle", ord("z"), 4)], [(b"", [])], [(b"abcd", [])]]
 
 
 def test_hand_computed_repeat_codes():
@@ -151,8 +151,8 @@ def test_ratio_at_least_libzstd_level1():
     plain = datagen.c2_text_plain(64 * 131072).tobytes()
     datas = [plain[i:i + 131072] for i in range(0, len(plain), 131072)]
     with ProcessPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as ex:   # parse in parallel, encode here
-        blocks = list(ex.map(clazy.parse_frame, datas))
-    ratio = len(plain) / sum(len(clazy.reference_frame(d, b)) for d, b in zip(datas, blocks))
+        blocks = list(ex.map(cparse.parse_frame, datas, [clazy.LAZY] * len(datas)))
+    ratio = len(plain) / sum(len(cparse.reference_frame(d, b, level=clazy.LAZY)) for d, b in zip(datas, blocks))
     zstd1 = len(plain) / sum(len(datagen.compress(d, level=1, window_log=17)) for d in datas)
     print(f"LAZY model ratio {ratio:.3f}, libzstd level 1 {zstd1:.3f}")
     assert ratio >= zstd1

@@ -7,6 +7,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import clazy
 import cldm
 import cparse
 import datagen
@@ -45,9 +46,10 @@ MIXED = planted(1400000, [(1000000, 1000, 299000), (700000, 400000, 50000), (130
 @pytest.mark.parametrize("lazy", [False, True], ids=["fastest", "lazy"])
 @pytest.mark.parametrize("window_log", [18, 23])
 def test_model_frames_decode_within_their_window(oracle, lazy, window_log):
-    blocks = cldm.parse([MIXED], window_log, lazy=lazy)[0]
-    frame = cldm.reference_frame(MIXED, blocks, window_log, lazy=lazy)
-    wl = cldm.frame_window_log(len(MIXED), window_log)
+    level = clazy.LAZY if lazy else cparse.FASTEST
+    blocks = cldm.parse([MIXED], window_log, level=level)[0]
+    frame = cparse.reference_frame(MIXED, blocks, level=level, window_log=window_log)
+    wl = cparse.frame_window_log(len(MIXED), window_log)
     seqs = decode_checked(oracle, frame, MIXED, wl)
     offs = cldm.offsets(blocks)
     far = [o for o in offs if o > cldm.WINDOW]
@@ -126,8 +128,8 @@ def test_identical_frames_do_not_match_each_other():
 
 def test_small_frames_are_the_regular_parse():
     f = planted(BLOCK, [(100000, 100, 20000)], 9)
-    assert cldm.parse([f], 27) == cparse.parse([f])
-    assert cldm.parse([f], 27, lazy=True) == [cldm.clazy.parse_frame(f)]
+    for level in (cparse.FASTEST, clazy.LAZY):
+        assert cldm.parse([f], 27, level=level) == cparse.parse([f], level=level)
 
 
 def test_window_descriptor_rule(tmp_path):
@@ -143,10 +145,10 @@ def test_window_descriptor_rule(tmp_path):
     for (n, w), row in zip(cases, rows):
         hexhdr, wl, st, ws = row.split()
         want = min(w, max(17, (n - 1).bit_length() if n > 1 else 0))
-        assert int(wl) == want == cldm.frame_window_log(n, w), (n, w)
+        assert int(wl) == want == cparse.frame_window_log(n, w), (n, w)
         assert int(st) == 0 and int(ws) == 1 << want
         hdr = bytes.fromhex(hexhdr)
         assert hdr[5] == (want - 10) << 3
-        assert hdr[:5] + hdr[6:] == cparse.frame_header(n, True)[:5] + cparse.frame_header(n, True)[6:]
+        assert hdr == cparse.frame_header(n, True, window_log=w)
         if n <= BLOCK:
             assert hdr[5] == 0x38

@@ -63,7 +63,7 @@ def test_reference_frame_decodes(oracle, c):
         f = cparse.reference_frame(data, blocks)
         assert datagen.decompress(f, len(data), raw_dict=c.content) == data
         assert oracle.decode_frame(f, raw_dict=c.content)[0] == data
-        assert cparse.reference_frame(data, blocks, level=0) == oracle_free_raw(data)
+        assert cparse.reference_frame(data, blocks, level=cparse.UNCOMPRESSED) == oracle_free_raw(data)
 
 
 def oracle_free_raw(data):

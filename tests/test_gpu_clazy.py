@@ -1,74 +1,32 @@
 """The LAZY level on the GPU against its plain model (tests/clazy.py): every frame is the model's reference_frame byte for byte --
 in one submission and one frame per submission, from host and device memory, against raw-content and formatted dictionaries
-with and without their tables.  The frames round-trip through libzstd, the oracle and this library's decoder in both execution
-modes and FrameDecoder; the output does not depend on the run or the batch; the ratio on 64 frames of C2b-shaped text is at
-least libzstd level 1's and above Fastest's; FrameCompressor at LAZY writes the batch compressor's blocks; and an unknown level
-is refused before any launch."""
+with and without their tables, by the checks test_gpu_cparse.py runs at Fastest.  The frames round-trip through libzstd, the
+oracle and this library's decoder in both execution modes and FrameDecoder; the output does not depend on the run or the batch;
+the ratio on 64 frames of C2b-shaped text is at least libzstd level 1's and above Fastest's; FrameCompressor at LAZY writes the
+batch compressor's blocks; and an unknown level is refused before any launch."""
 import numpy as np
 import pytest
 
-import clazy
 import datagen
 from test_compress import batch_decode, check_frames
 from test_gpu_compress_stream import _chunk, check_fastest, run
-from test_gpu_cparse import compress
+from test_gpu_cparse import check_reference_frames, check_reference_frames_with_dictionaries, compress
 
 pytestmark = pytest.mark.gpu
 
-CASES = clazy.cases()
-PLAIN = [c for c in CASES if c.content is None]
-WITH_DICT = [c for c in CASES if c.content is not None]
 MIB = 1 << 20
-
-
-@pytest.fixture(scope="module")
-def model():
-    return {c.id: clazy.parse(c.frames, c.content) for c in CASES}
-
-
-_refs = {}
-
-
-def reference(c, model, i, **kw):
-    key = (c.id, i, tuple(sorted((k, v if not isinstance(v, bytes) else hash(v)) for k, v in kw.items())))
-    if key not in _refs:
-        _refs[key] = clazy.reference_frame(c.frames[i], model[c.id][i], **kw)
-    return _refs[key]
 
 
 def lazy(pkg, ctx, datas, **kw):
     return compress(pkg, ctx, datas, level=pkg.LAZY, **kw)
 
 
-def test_frames_are_the_models(pkg, ctx, model):
-    frames, _ = lazy(pkg, ctx, [f for c in PLAIN for f in c.frames])
-    at = 0
-    for c in PLAIN:
-        for i in range(len(c.frames)):
-            assert frames[at + i] == reference(c, model, i), f"{c.id} frame {i}"
-        at += len(c.frames)
-    for c in PLAIN:                                                     # one frame per submission, host and device
-        for i, data in enumerate(c.frames):
-            for device in (False, True):
-                assert lazy(pkg, ctx, [data], device=device)[0][0] == reference(c, model, i), f"{c.id} frame {i} device={device}"
+def test_frames_are_the_models(pkg, ctx):
+    check_reference_frames(pkg, ctx, "lazy")
 
 
-def test_frames_with_dictionaries_are_the_models(pkg, ctx, model):
-    for c in WITH_DICT:
-        R = pkg.Dictionary.raw_content(ctx, 1, c.content)
-        for device in (False, True):
-            frames, _ = lazy(pkg, ctx, c.frames, dict=R, device=device)
-            for i, f in enumerate(frames):
-                assert f == reference(c, model, i), f"{c.id} frame {i} raw content device={device}"
-        if len(c.content) < 8:                                           # the finalizer's smallest content
-            continue
-        fin = pkg.finalize_dict(ctx, c.content, c.frames[:50])
-        F = pkg.Dictionary.decode_dict(ctx, fin)
-        for tables in (False, True):
-            frames, _ = lazy(pkg, ctx, c.frames, dict=F, dict_tables=tables)
-            for i, f in enumerate(frames):
-                want = reference(c, model, i, dict_id=F.id, dict_tables=fin if tables else None)
-                assert f == want, f"{c.id} frame {i} finalized dictionary tables={tables}"
+def test_frames_with_dictionaries_are_the_models(pkg, ctx):
+    check_reference_frames_with_dictionaries(pkg, ctx, "lazy")
 
 
 @pytest.fixture(scope="module")

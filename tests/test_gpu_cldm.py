@@ -9,10 +9,13 @@ import struct
 import numpy as np
 import pytest
 
+import clazy
 import cldm
+import cparse
 import datagen
 import streamframe as SF
 from test_gpu_compress_stream import Sink, Source, _chunk
+from test_gpu_cparse import compress
 
 pytestmark = pytest.mark.gpu
 
@@ -59,30 +62,12 @@ _models = {}
 def model(frames, wl, lazy, content=None):
     key = (tuple(map(len, frames)), hash(tuple(frames)), wl, lazy, content and hash(content))
     if key not in _models:
-        _models[key] = cldm.parse(frames, wl, content, lazy)
+        _models[key] = cldm.parse(frames, wl, content, clazy.LAZY if lazy else cparse.FASTEST)
     return _models[key]
 
 
-def long_frames(pkg, ctx, datas, window_log, level=1, checksum=True, device=False, dict=None, dict_tables=False):
-    """compress_many with window_log: (frames, results)."""
-    io_ = np.zeros(len(datas), dtype=pkg.binding.COMPRESS_IO_DTYPE)
-    so = oo = 0
-    for i, d in enumerate(datas):
-        cap = pkg.compress_bound(len(d), dict)
-        io_[i] = (so, len(d), oo, cap)
-        so += len(d)
-        oo += cap
-    src = np.frombuffer(b"".join(datas) + b"\0", dtype=np.uint8)[:so]
-    out = np.zeros(oo + 1, dtype=np.uint8)
-    if device:
-        import torch
-        src_t, out_t = torch.from_numpy(src.copy()).cuda(), torch.zeros(oo + 1, dtype=torch.uint8, device="cuda")
-        res = pkg.compress_frames(ctx, src_t, io_, out_t, level, checksum, dict, dict_tables, window_log)
-        out = out_t.cpu().numpy()
-    else:
-        res = pkg.compress_frames(ctx, src, io_, out, level, checksum, dict, dict_tables, window_log)
-    frames = [out[int(r["dst_off"]):int(r["dst_off"]) + int(x["dst_size"])].tobytes() for r, x in zip(io_, res)]
-    return frames, res
+def reference(data, blocks, window_log, lazy, **kw):
+    return cparse.reference_frame(data, blocks, level=clazy.LAZY if lazy else cparse.FASTEST, window_log=window_log, **kw)
 
 
 def check_decodes(pkg, ctx, oracle, datas, frames, window_log):
@@ -90,7 +75,7 @@ def check_decodes(pkg, ctx, oracle, datas, frames, window_log):
     FrameDecoder."""
     dec = pkg.FrameDecoder(ctx)
     for d, f in zip(datas, frames):
-        wl = cldm.frame_window_log(len(d), window_log)
+        wl = cparse.frame_window_log(len(d), window_log)
         assert f[5] == (wl - 10) << 3
         o = oracle.FrameDecoder()
         o.set_max_window_size(1 << 27)
@@ -110,16 +95,16 @@ def test_frames_equal_the_model(pkg, ctx, oracle, lazy, window_log):
     level = pkg.LAZY if lazy else pkg.FASTEST
     blocks = model(plain, window_log, lazy)
     before = ctx.kernel_launches()
-    frames, res = long_frames(pkg, ctx, plain, window_log, level)
+    frames, res = compress(pkg, ctx, plain, level=level, window_log=window_log)
     assert ctx.kernel_launches() - before == 17 + 4   # the long-match kernels, then the four stages
     for i, (d, f) in enumerate(zip(plain, frames)):
-        assert f == cldm.reference_frame(d, blocks[i], window_log, lazy=lazy), f"frame {i}"
+        assert f == reference(d, blocks[i], window_log, lazy), f"frame {i}"
     far = [o for o in cldm.offsets(blocks[0]) if o > B]
     assert far and max(far) <= 1 << window_log
     if window_log >= 23:
         assert 4 * MIB in far
-    frames2, _ = long_frames(pkg, ctx, plain[:1], window_log, level, checksum=False, device=True)
-    assert frames2[0] == cldm.reference_frame(big, blocks[0], window_log, checksum=False, lazy=lazy)
+    frames2, _ = compress(pkg, ctx, plain[:1], level=level, window_log=window_log, checksum=False, device=True)
+    assert frames2[0] == reference(big, blocks[0], window_log, lazy, checksum=False)
     if window_log == 23:
         check_decodes(pkg, ctx, oracle, plain, frames, window_log)
 
@@ -132,14 +117,14 @@ def test_frames_with_dictionaries_equal_the_model(pkg, ctx, lazy):
     datas = [mid, big[:2 * MIB]]
     blocks = model(datas, 23, lazy, content)
     R = pkg.Dictionary.raw_content(ctx, 1, content)
-    frames, _ = long_frames(pkg, ctx, datas, 23, level, dict=R)
+    frames, _ = compress(pkg, ctx, datas, dict=R, level=level, window_log=23)
     for i, d in enumerate(datas):
-        assert frames[i] == cldm.reference_frame(d, blocks[i], 23, lazy=lazy), f"raw content frame {i}"
+        assert frames[i] == reference(d, blocks[i], 23, lazy), f"raw content frame {i}"
     fin = pkg.finalize_dict(ctx, content, [mid[i:i + 4096] for i in range(0, 400000, 4096)])
     F = pkg.Dictionary.decode_dict(ctx, fin)
-    frames, _ = long_frames(pkg, ctx, datas, 23, level, dict=F, dict_tables=True)
+    frames, _ = compress(pkg, ctx, datas, dict=F, dict_tables=True, level=level, window_log=23)
     for i, d in enumerate(datas):
-        assert frames[i] == cldm.reference_frame(d, blocks[i], 23, dict_id=F.id, dict_tables=fin, lazy=lazy), f"formatted frame {i}"
+        assert frames[i] == reference(d, blocks[i], 23, lazy, dict_id=F.id, dict_tables=fin), f"formatted frame {i}"
 
 
 def test_window_17_is_the_dict_entry(pkg, ctx):
@@ -147,7 +132,7 @@ def test_window_17_is_the_dict_entry(pkg, ctx):
     L = pkg.lib()
     datas = plain
     for level in (pkg.UNCOMPRESSED, pkg.FASTEST, pkg.LAZY):
-        frames, _ = long_frames(pkg, ctx, datas, 17, level)
+        frames, _ = compress(pkg, ctx, datas, level=level, window_log=17)
         io_ = np.zeros(len(datas), dtype=pkg.binding.COMPRESS_IO_DTYPE)
         so = oo = 0
         for i, d in enumerate(datas):
@@ -166,9 +151,9 @@ def test_c2b_shaped_frames_are_unchanged_at_27(pkg, ctx):
     plain = datagen.c2_text_plain(8192 * B).tobytes()
     datas = [plain[i:i + B] for i in range(0, len(plain), B)]
     for level in (pkg.FASTEST, pkg.LAZY):
-        a, _ = long_frames(pkg, ctx, datas, 17, level)
+        a, _ = compress(pkg, ctx, datas, level=level, window_log=17)
         before = ctx.kernel_launches()
-        b, _ = long_frames(pkg, ctx, datas, 27, level)
+        b, _ = compress(pkg, ctx, datas, level=level, window_log=27)
         assert ctx.kernel_launches() - before == 4   # the four stages, no long-match kernel
         assert a == b
         assert all(f[5] == 0x38 for f in b[:16])
@@ -199,7 +184,7 @@ def test_stream_equals_the_batch_blocks(pkg, ctx, oracle, monkeypatch, chunk):
 
 def test_round_trips(pkg, ctx, oracle, tmp_path):
     big, mid, plain = inputs()
-    frames, res = long_frames(pkg, ctx, plain, 24, pkg.FASTEST)
+    frames, res = compress(pkg, ctx, plain, level=pkg.FASTEST, window_log=24)
     check_decodes(pkg, ctx, oracle, plain, frames, 24)
     whole = b"".join(frames)
     out = bytearray()
@@ -258,11 +243,11 @@ def test_bad_arguments_are_refused_before_any_launch(pkg, ctx):
 
 def test_deterministic_across_runs_and_batch_shapes(pkg, ctx):
     big, mid, plain = inputs()
-    a, _ = long_frames(pkg, ctx, plain, 23, pkg.FASTEST)
-    b, _ = long_frames(pkg, ctx, plain, 23, pkg.FASTEST)
-    c, _ = long_frames(pkg, ctx, plain[::-1], 23, pkg.FASTEST)
+    a, _ = compress(pkg, ctx, plain, window_log=23)
+    b, _ = compress(pkg, ctx, plain, window_log=23)
+    c, _ = compress(pkg, ctx, plain[::-1], window_log=23)
     assert a == b == c[::-1]
-    assert [long_frames(pkg, ctx, [d], 23, pkg.FASTEST)[0][0] for d in plain] == a
+    assert [compress(pkg, ctx, [d], window_log=23)[0][0] for d in plain] == a
 
 
 class Repeat(io.RawIOBase):

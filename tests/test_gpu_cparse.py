@@ -2,43 +2,47 @@
 sequences (through the oracle's trace) are the model's, and every frame is reference_frame's byte for byte -- which also pins the
 Raw blocks' parse, k_cenc's 32-lane encode_block against the 1-lane host build, k_cassemble's layout and k_cxxh64 -- in one
 submission, one frame per submission, from host and device memory, against raw-content and formatted dictionaries with and without
-their tables.  The dictionary finalizer's statistics are the model's counts, and both checksum kernels (k_cxxh64, k_xxh64) equal
-the plain XXH64 at the lengths where their stripe loops change shape, at every address residue mod 8."""
+their tables.  The frame checks take the level; test_gpu_clazy.py runs them at LAZY (tests/clazy.py).  The dictionary finalizer's
+statistics are the model's counts, and both checksum kernels (k_cxxh64, k_xxh64) equal the plain XXH64 at the lengths where their
+stripe loops change shape, at every address residue mod 8."""
 import ctypes as C
 import struct
 
 import numpy as np
 import pytest
 
+import clazy
 import cparse
 import datagen
 from conftest import read_golden
 
 pytestmark = pytest.mark.gpu
 
-CASES = cparse.cases()
+LEVELS = {"fastest": (cparse.FASTEST, cparse.cases()), "lazy": (clazy.LAZY, clazy.cases())}
+CASES = LEVELS["fastest"][1]
 PLAIN = [c for c in CASES if c.content is None]
 WITH_DICT = [c for c in CASES if c.content is not None]
 
-
-@pytest.fixture(scope="module")
-def model():
-    return {c.id: cparse.parse(c.frames, c.content) for c in CASES}
+_models, _refs = {}, {}
 
 
-_refs = {}
+def model(name, c):
+    """The parse of case c at the level, computed once."""
+    if (name, c.id) not in _models:
+        _models[name, c.id] = cparse.parse(c.frames, c.content, LEVELS[name][0])
+    return _models[name, c.id]
 
 
-def reference(c, model, i, **kw):
-    """reference_frame of frame i of case c, cached per options."""
-    key = (c.id, i, tuple(sorted((k, v if not isinstance(v, bytes) else hash(v)) for k, v in kw.items())))
+def reference(name, c, i, **kw):
+    """reference_frame of frame i of case c at the level, cached per options."""
+    key = (name, c.id, i, tuple(sorted((k, v if not isinstance(v, bytes) else hash(v)) for k, v in kw.items())))
     if key not in _refs:
-        _refs[key] = cparse.reference_frame(c.frames[i], model[c.id][i], **kw)
+        _refs[key] = cparse.reference_frame(c.frames[i], model(name, c)[i], level=LEVELS[name][0], **kw)
     return _refs[key]
 
 
-def compress(pkg, ctx, datas, dict=None, dict_tables=False, device=False, level=1, checksum=True):
-    """compress_frames over datas laid out back to back; returns the frames and the result rows."""
+def compress(pkg, ctx, datas, dict=None, dict_tables=False, device=False, level=1, checksum=True, window_log=cparse.WINDOW_LOG_MIN):
+    """compress_frames over datas laid out back to back at window_log; returns the frames and the result rows."""
     io = np.zeros(len(datas), dtype=pkg.binding.COMPRESS_IO_DTYPE)
     so = oo = 0
     parts = []
@@ -53,10 +57,10 @@ def compress(pkg, ctx, datas, dict=None, dict_tables=False, device=False, level=
     if device:
         import torch
         src_t, out_t = torch.from_numpy(src.copy()).cuda(), torch.zeros(out.size, dtype=torch.uint8, device="cuda")
-        res = pkg.compress_frames(ctx, src_t, io, out_t, level, checksum, dict=dict, dict_tables=dict_tables)
+        res = pkg.compress_frames(ctx, src_t, io, out_t, level, checksum, dict=dict, dict_tables=dict_tables, window_log=window_log)
         out = out_t.cpu().numpy()
     else:
-        res = pkg.compress_frames(ctx, src, io, out, level, checksum, dict=dict, dict_tables=dict_tables)
+        res = pkg.compress_frames(ctx, src, io, out, level, checksum, dict=dict, dict_tables=dict_tables, window_log=window_log)
     assert (res["status"] == 0).all()
     return [out[io[i]["dst_off"]:io[i]["dst_off"] + res[i]["dst_size"]].tobytes() for i in range(len(datas))], res
 
@@ -83,9 +87,10 @@ def traced_blocks(oracle, f, content=None, formatted=None):
     return out
 
 
-def check_parse(c, model, frames, oracle, content=None, formatted=None):
+def check_parse(c, blocks, frames, oracle, content=None, formatted=None):
+    """Every Compressed block of the GPU's frames of case c has the literals and sequences of `blocks`, the model's parse."""
     for i, f in enumerate(frames):
-        want = model[c.id][i]
+        want = blocks[i]
         got = traced_blocks(oracle, f, content, formatted)
         assert len(got) == len(want), (c.id, i)
         for k, ((btype, lits, seqs), w) in enumerate(zip(got, want)):
@@ -101,48 +106,64 @@ def check_parse(c, model, frames, oracle, content=None, formatted=None):
                 assert lits == w[0], f"{c.id} frame {i} block {k}: literals differ"
 
 
-def test_parse_is_the_models(pkg, ctx, oracle, model):
+def test_parse_is_the_models(pkg, ctx, oracle):
     frames, _ = compress(pkg, ctx, [f for c in PLAIN for f in c.frames])
     at = 0
     for c in PLAIN:
-        check_parse(c, model, frames[at:at + len(c.frames)], oracle)
+        check_parse(c, model("fastest", c), frames[at:at + len(c.frames)], oracle)
         at += len(c.frames)
     for c in WITH_DICT:
         D = pkg.Dictionary.raw_content(ctx, 1, c.content)
         frames, _ = compress(pkg, ctx, c.frames, dict=D)
-        check_parse(c, model, frames, oracle, content=c.content)
+        check_parse(c, model("fastest", c), frames, oracle, content=c.content)
 
 
-def test_frames_are_the_reference(pkg, ctx, model):
-    frames, _ = compress(pkg, ctx, [f for c in PLAIN for f in c.frames])
+def check_reference_frames(pkg, ctx, name):
+    """The frames of every case without a dictionary at the level (LEVELS) are reference_frame's: in one submission, and one
+    frame per submission from host and device memory."""
+    level = getattr(pkg, name.upper())
+    plain = [c for c in LEVELS[name][1] if c.content is None]
+    frames, _ = compress(pkg, ctx, [f for c in plain for f in c.frames], level=level)
     at = 0
-    for c in PLAIN:
+    for c in plain:
         for i in range(len(c.frames)):
-            assert frames[at + i] == reference(c, model, i), f"{c.id} frame {i}"
+            assert frames[at + i] == reference(name, c, i), f"{c.id} frame {i}"
         at += len(c.frames)
-    for c in PLAIN:                                                     # one frame per submission, host and device
+    for c in plain:                                                     # one frame per submission, host and device
         for i, data in enumerate(c.frames):
             for device in (False, True):
-                assert compress(pkg, ctx, [data], device=device)[0][0] == reference(c, model, i), f"{c.id} frame {i} device={device}"
+                assert compress(pkg, ctx, [data], device=device, level=level)[0][0] == reference(name, c, i), \
+                    f"{c.id} frame {i} device={device}"
 
 
-def test_frames_with_dictionaries_are_the_reference(pkg, ctx, model):
-    for c in WITH_DICT:
+def check_reference_frames_with_dictionaries(pkg, ctx, name):
+    """The frames of every case with a dictionary at the level (LEVELS) are reference_frame's: against its raw content from host
+    and device memory, and against the finalized dictionary with and without its tables."""
+    level = getattr(pkg, name.upper())
+    for c in [c for c in LEVELS[name][1] if c.content is not None]:
         R = pkg.Dictionary.raw_content(ctx, 1, c.content)
         for device in (False, True):
-            frames, _ = compress(pkg, ctx, c.frames, dict=R, device=device)
+            frames, _ = compress(pkg, ctx, c.frames, dict=R, device=device, level=level)
             for i, f in enumerate(frames):
-                assert f == reference(c, model, i), f"{c.id} frame {i} raw content device={device}"
+                assert f == reference(name, c, i), f"{c.id} frame {i} raw content device={device}"
         if len(c.content) < 8:                                           # the finalizer's smallest content
             continue
         fin = pkg.finalize_dict(ctx, c.content, c.frames[:50])
         assert fin.endswith(c.content)
         F = pkg.Dictionary.decode_dict(ctx, fin)
         for tables in (False, True):
-            frames, _ = compress(pkg, ctx, c.frames, dict=F, dict_tables=tables)
+            frames, _ = compress(pkg, ctx, c.frames, dict=F, dict_tables=tables, level=level)
             for i, f in enumerate(frames):
-                want = reference(c, model, i, dict_id=F.id, dict_tables=fin if tables else None)
+                want = reference(name, c, i, dict_id=F.id, dict_tables=fin if tables else None)
                 assert f == want, f"{c.id} frame {i} finalized dictionary tables={tables}"
+
+
+def test_frames_are_the_reference(pkg, ctx):
+    check_reference_frames(pkg, ctx, "fastest")
+
+
+def test_frames_with_dictionaries_are_the_reference(pkg, ctx):
+    check_reference_frames_with_dictionaries(pkg, ctx, "fastest")
 
 
 def test_golden_formatted_dictionary(pkg, ctx, oracle, manifest):
@@ -154,14 +175,14 @@ def test_golden_formatted_dictionary(pkg, ctx, oracle, manifest):
     datas = [oracle.decode_frame(read_golden("dict_tests", "files", x), dict_raw=dic)[0] for x in names]
     datas.append(content[-3000:-1000] + content[-64:] + bytes(range(256)))
     c = cparse.Case("golden", "dict_tests-dictionary", datas, content)
-    model = {c.id: cparse.parse(c.frames, content)}
+    blocks = cparse.parse(c.frames, content)
     D = pkg.Dictionary.decode_dict(ctx, dic)
     assert D.id == did.value and D.content_size == len(content)
     for tables in (False, True):
         frames, _ = compress(pkg, ctx, datas, dict=D, dict_tables=tables)
-        check_parse(c, model, frames, oracle, formatted=dic)
+        check_parse(c, blocks, frames, oracle, formatted=dic)
         for i, f in enumerate(frames):
-            assert f == cparse.reference_frame(datas[i], model[c.id][i], dict_id=D.id, dict_tables=dic if tables else None), \
+            assert f == cparse.reference_frame(datas[i], blocks[i], dict_id=D.id, dict_tables=dic if tables else None), \
                 f"{names[i] if i < len(names) else 'crafted'} tables={tables}"
 
 
@@ -202,7 +223,7 @@ def test_checksums_at_every_residue(pkg, ctx):
                 frames, res = compress_at(pkg, ctx, datas, r, device)
                 for n, d, f, x, w in zip(LENGTHS, datas, frames, res, want):
                     assert x["checksum"] == w and struct.unpack("<I", f[-4:])[0] == w, (n, r, device)
-                    assert f == cparse.reference_frame(d, [None] * max(1, -(-n // cparse.BLOCK)), level=0), (n, r)
+                    assert f == cparse.reference_frame(d, [None] * max(1, -(-n // cparse.BLOCK)), level=cparse.UNCOMPRESSED), (n, r)
             io = np.zeros(len(frames), dtype=pkg.binding.FRAME_IO_DTYPE)
             so = oo = 0
             for i, (f, d) in enumerate(zip(frames, datas)):
