@@ -1,14 +1,15 @@
 #!/usr/bin/env python3
 """bench_compress.py -- input GB/s of the batch compressor (b200z_compress_frames_batch, ruzstd's Fastest level, checksum on).
 
-    python bench_compress.py [--steps K] [--warmup W] [--skip-cpu] [--level fastest|lazy]
+    python bench_compress.py [--steps K] [--warmup W] [--skip-cpu] [--level fastest|lazy|opt]
 
 The workload is the C2b plaintext (1 GiB of enwik9-shaped text, datagen.c2_text_plain), device-resident, in two shapes:
 8192 frames of 128 KiB and one 1 GiB frame (C2a's plaintext shape, where the content checksum is four serial chains).
 Prints one JSON line: per shape the input GB/s (CUDA events around the call, median of the steps), the ratio, each kernel's
 milliseconds, (input + output bytes) / t against the HBM peak, the card's name and power limit, and `cpu_baseline`:
 libzstd 1.5.5 level 1 on the same 128 KiB pieces, one thread and all host threads.  --level lazy measures the LAZY extension
-level instead, and adds libzstd level 3 to the baseline.  Nothing is written to the tree.
+level instead, and adds libzstd level 3 to the baseline; --level opt measures the OPT extension level and adds libzstd levels 3
+and 16 (btopt, the price-based parse).  Nothing is written to the tree.
 """
 import argparse
 import json
@@ -63,7 +64,7 @@ def libzstd_compress_baseline(datas, level=1):
 
 
 def run_compress(args):
-    """b200z_compress_frames_batch at the Fastest (or LAZY) level on the 1 GiB C2b plaintext, device-resident, in two shapes:
+    """b200z_compress_frames_batch at the Fastest (or LAZY, or OPT) level on the 1 GiB C2b plaintext, device-resident, in two shapes:
     8192 frames of 128 KiB (C2b) and one 1 GiB frame (C2a's plaintext shape).  Each output is first decoded on the GPU and must
     equal the input; then the call is timed with CUDA events after warm-up, and one more run with a CUDA event between kernels
     gives each kernel's time."""
@@ -78,8 +79,8 @@ def run_compress(args):
     plain = datagen.c2_text_plain(total)
     d_in = torch.from_numpy(plain).cuda()
     peak, peak_src = bench.measured_peak()
-    level = pkg.LAZY if args.level == "lazy" else pkg.FASTEST
-    line = {"metric": "compress_GBps", "unit": "GB/s", "level": "LAZY" if args.level == "lazy" else "Fastest", "checksum": True, "card": card_info(), "input_bytes": total, "shapes": {}}
+    level, name = {"fastest": (pkg.FASTEST, "Fastest"), "lazy": (pkg.LAZY, "LAZY"), "opt": (pkg.OPT, "OPT")}[args.level]
+    line = {"metric": "compress_GBps", "unit": "GB/s", "level": name, "checksum": True, "card": card_info(), "input_bytes": total, "shapes": {}}
     for shape, frame_bytes in (("c2b", args.frame_bytes), ("c2a", total)):
         nfr = total // frame_bytes
         io = np.zeros(nfr, dtype=pkg.binding.COMPRESS_IO_DTYPE)
@@ -122,8 +123,10 @@ def run_compress(args):
     if not args.skip_cpu:
         pieces = [plain[i:i + args.frame_bytes] for i in range(0, total, args.frame_bytes)]
         line["cpu_baseline"] = libzstd_compress_baseline(pieces)
-        if args.level == "lazy":
+        if args.level in ("lazy", "opt"):
             line["cpu_baseline_level3"] = libzstd_compress_baseline(pieces, 3)
+        if args.level == "opt":
+            line["cpu_baseline_level16"] = libzstd_compress_baseline(pieces, 16)
     ctx.close()
     print(json.dumps(line))
 
@@ -135,7 +138,7 @@ def main():
     ap.add_argument("--frame-bytes", type=int, default=131072)
     ap.add_argument("--c2a-bytes", type=int, default=1 << 30, help="total plaintext bytes (both shapes)")
     ap.add_argument("--skip-cpu", action="store_true")
-    ap.add_argument("--level", choices=("fastest", "lazy"), default="fastest")
+    ap.add_argument("--level", choices=("fastest", "lazy", "opt"), default="fastest")
     run_compress(ap.parse_args())
     return 0
 

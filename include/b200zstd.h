@@ -568,6 +568,22 @@ typedef struct b200z_compress_result {
  * them byte for byte.  Accepted by the batch entries (with or without a dictionary and B200Z_FLAG_DICT_TABLES) and the stream
  * compressor; b200z_dict_finalize keeps the Fastest parse. */
 #define B200Z_LEVEL_LAZY 5
+/* EXTENSION (not a ruzstd level): a price-based ("optimal") parse.  Same framing, window, blocks, compress bound, 8 segments per
+ * block, 5-byte minimum match, dictionary reach, forced long-distance pieces, packing and repeat-offset coding as LAZY; no match
+ * crosses its segment's end and no block depends on another block's encoding.  The finder gives every position a list of
+ * candidates that depends on the input only: the nearest earlier positions of the frame with the same 13-bit 5-byte hash, up to
+ * 24 of them within the 128 KiB window (the previous block included), each verified for up to 32 bytes; the up to 4 longest of
+ * strictly increasing length, each with the smallest offset for its length (and the dictionary's entry in a frame's first
+ * 128 KiB).  Each segment is then parsed by a forward dynamic program over its positions: a literal costs its byte's share of the
+ * block's byte histogram in bits, a match a fixed weight plus its offset code's bits (a repeat, one of the path's three most
+ * recent distinct offsets, verified at that position, a smaller weight); the cheapest path wins, and a candidate of 32 bytes is
+ * taken at once and extended.  A program spans at most 256 positions before it closes.  DESIGN.md section 4.4 states the rule
+ * and tests/copt.py models it byte for byte.  One kernel (k_copt, stage 0 of b200z_compress_last_profile) replaces k_cmatch, so a
+ * submission launches as many kernels as at LAZY.  Its grid is the CTAs resident on the device at once (one per SM), striding
+ * over the blocks; each keeps a chain of (131072 + 131072) * 4 bytes, 1 MiB, in device memory held by the context (132 MiB on
+ * 132 SMs), allocated by the first compression at this level.  Accepted wherever LAZY is; b200z_dict_finalize keeps the
+ * Fastest parse.  Levels 6, 8 and up stay B200Z_ERR_INVALID_ARGUMENT. */
+#define B200Z_LEVEL_OPT 7
 /* context flag: b200z_compress_frames_batch records a CUDA event between its kernels and keeps each kernel's milliseconds
  * for b200z_compress_last_profile (profiling aid for bench.py; it synchronises anyway) */
 #define B200Z_FLAG_PROFILE 2u
@@ -585,7 +601,7 @@ size_t b200z_compress_bound(size_t src_size);
  * content checksum.  Returns 0 when the submission ran (results[nframes] filled).  Checked before any launch:
  * B200Z_ERR_INVALID_ARGUMENT for a range outside `input` / `output`, dst_cap < b200z_compress_bound(src_size), overlapping
  * destination ranges or an unknown level; B200Z_ERR_REFERENCE_WOULD_PANIC for the levels the reference does not implement.
- * Levels: Uncompressed, Fastest and the extension B200Z_LEVEL_LAZY. */
+ * Levels: Uncompressed, Fastest and the extensions B200Z_LEVEL_LAZY and B200Z_LEVEL_OPT. */
 int b200z_compress_frames_batch(b200z_ctx *ctx, const uint8_t *input, size_t input_len, int input_mem,
                                 const b200z_compress_io *frames, size_t nframes, int level, int checksum,
                                 uint8_t *output, size_t output_cap, int output_mem, b200z_compress_result *results);
@@ -615,7 +631,7 @@ size_t b200z_compress_bound_dict(size_t src_size, const b200z_dict *dict);
  * carries min(window_log, max(17, ceil(log2 src_size))), so a frame of 131072 bytes or fewer is exactly what window_log 17
  * writes, and window_log 17 is exactly b200z_compress_frames_batch_dict.  The compress bound is b200z_compress_bound_dict.  Besides
  * that entry's checks: B200Z_ERR_INVALID_ARGUMENT, before any launch, for window_log outside [17, 27] and for a window_log
- * above 17 at B200Z_LEVEL_UNCOMPRESSED.  Accepted at Fastest and LAZY.  With a frame larger than 131072 bytes and window_log > 17
+ * above 17 at B200Z_LEVEL_UNCOMPRESSED.  Accepted at Fastest, LAZY and OPT.  With a frame larger than 131072 bytes and window_log > 17
  * the submission first runs the long-match kernels (k_lanchor twice, k_lscan, four k_lhist / k_lscan / k_lscatter passes of the
  * key sort, k_lcand, k_lblock: 17 launches, 3 when no anchor is found; counted in b200z_ctx_kernel_launches, not in
  * b200z_compress_last_profile's four stages), synchronising once to size the anchors' buffers: 44 bytes per anchor (at most one per 16 input bytes of those frames,
@@ -636,10 +652,10 @@ int b200z_compress_last_profile(const b200z_ctx *ctx, float *stage_ms, size_t n)
  * a multiple of 128 KiB (0 included) ends with an empty last Raw block (01 00 00); then the low 32 bits of XXH64 (seed 0) of the
  * plaintext when the checksum is on.  Level Uncompressed writes Raw blocks, byte for byte the reference's frame, on the host
  * only (no kernel, no device copy).  Level Fastest writes every block's type and body as b200z_compress_frames_batch does for the
- * same block of the same input compressed as one frame, and so does level LAZY (EXTENSION) at LAZY.
+ * same block of the same input compressed as one frame, and so do levels LAZY and OPT (EXTENSION) at theirs.
  * The source is read into chunks of whole blocks: B200Z_PIPELINE_CHUNK_BYTES (read by _new) rounded down to a multiple of
  * 131072, at least 131072; 64 MiB by default.  At Fastest (and LAZY) each non-empty chunk is uploaded and compressed by three kernels
- * (k_cmatch, k_cenc, k_cassemble) on the ctx stream, counted in b200z_ctx_kernel_launches, while the host reads and hashes the
+ * (k_cmatch, k_cenc, k_cassemble; at OPT k_copt in k_cmatch's place, with its chain slots allocated by the first OPT compress) on the ctx stream, counted in b200z_ctx_kernel_launches, while the host reads and hashes the
  * next chunk and writes the previous one: one write_cb pass per chunk (header in the first, trailer in the last), not per block.
  * Memory, allocated by the first Fastest compress and kept until _free, depends on the chunk C only.  Device: 2 * (C + 131072)
  * input, 2 * (C + 3 * C / 131072) output, and the compressor's staging for C / 131072 blocks (about 0.9 MB per block); about
@@ -649,10 +665,10 @@ int b200z_compress_last_profile(const b200z_ctx *ctx, float *stage_ms, size_t n)
  * written, and the compressor stays usable.  Hashing and matching state reset with every compress.
  * ---------------------------------------------------------------------------------------------------------- */
 typedef struct b200z_frame_compressor b200z_frame_compressor;
-/* FrameCompressor::new :77.  B200Z_ERR_INVALID_ARGUMENT for a level outside 0-4 and B200Z_LEVEL_LAZY */
+/* FrameCompressor::new :77.  B200Z_ERR_INVALID_ARGUMENT for a level outside 0-4, B200Z_LEVEL_LAZY and B200Z_LEVEL_OPT */
 int b200z_frame_compressor_new(b200z_ctx *ctx, int level, int checksum, b200z_frame_compressor **out);
 void b200z_frame_compressor_free(b200z_frame_compressor *fc);
-int b200z_frame_compressor_set_compression_level(b200z_frame_compressor *fc, int level);   /* :263; 0-4 or LAZY, else INVALID_ARGUMENT */
+int b200z_frame_compressor_set_compression_level(b200z_frame_compressor *fc, int level);   /* :263; 0-4, LAZY or OPT, else INVALID_ARGUMENT */
 int b200z_frame_compressor_compression_level(const b200z_frame_compressor *fc);            /* :273 */
 /* EXTENSION: long-distance matches up to 2^window_log bytes back (b200z_compress_frames_batch_long's rule) from the next compress
  * on; window_log in [17, 27], else B200Z_ERR_INVALID_ARGUMENT.  The frame's Window_Descriptor is 2^window_log (its size is unknown

@@ -2575,20 +2575,22 @@ extern "C" size_t b200z_compress_bound_dict(size_t n, const b200z_dict *d) { ret
 extern "C" int b200z_compress_num_stages(void) { return kCompressStages; }
 extern "C" const char *b200z_compress_stage_name(int stage) { return stage >= 0 && stage < kCompressStages ? kCompressStageNames[stage] : ""; }
 
-// k_cmatch / k_cenc staging for nblocks blocks (CompressArgs)
+// k_cmatch / k_cenc staging for nblocks blocks (CompressArgs), and at OPT k_copt's chain slots
 struct CompressStaging {
     DevBuf lit_stage, seq_stage, lits, seqs, info, res;
-    int ensure(uint64_t nblocks, bool grow) {
+    DevBuf opt_prev;   // OPT: opt_ctas() slots of OPT_SPAN words, allocated by the first OPT submission and kept
+    int ensure(uint64_t nblocks, bool grow, int level = B200Z_LEVEL_FASTEST) {
         int e = 0;
         if ((e = lit_stage.ensure(nblocks * ENC_BLOCK, grow)) || (e = seq_stage.ensure(nblocks * CBLOCK_SEQS * sizeof(SeqRec), grow)) ||
             (e = lits.ensure(nblocks * ENC_BLOCK, grow)) || (e = seqs.ensure(nblocks * CBLOCK_SEQS * sizeof(SeqRec), grow)) ||
             (e = info.ensure(nblocks * sizeof(CBlockInfo), grow)) || (e = res.ensure(nblocks * sizeof(CBlockInfo), grow)))
             return e;
+        if (level == B200Z_LEVEL_OPT && (e = opt_prev.ensure((uint64_t)opt_ctas() * OPT_SPAN * sizeof(int32_t)))) return e;
         return 0;
     }
     void bind(CompressArgs &a) const {
         a.lit_stage = lit_stage.as<uint8_t>(); a.seq_stage = seq_stage.as<SeqRec>(); a.lits = lits.as<uint8_t>(); a.seqs = seqs.as<SeqRec>();
-        a.enc = a.lit_stage; a.info = info.as<CBlockInfo>(); a.res = res.as<CBlockInfo>();
+        a.enc = a.lit_stage; a.info = info.as<CBlockInfo>(); a.res = res.as<CBlockInfo>(); a.opt_prev = opt_prev.as<int32_t>();
     }
 };
 
@@ -2686,7 +2688,7 @@ struct CompressResources {
     // `blocks` blocks; Uncompressed takes the blocks' results only, not the match and entropy staging
     int ensure_submission(uint64_t frames, uint64_t blocks, int level) {
         int e = 0;
-        if ((e = level != B200Z_LEVEL_UNCOMPRESSED ? stage.ensure(blocks, true) : stage.res.ensure(blocks * sizeof(CBlockInfo))) ||
+        if ((e = level != B200Z_LEVEL_UNCOMPRESSED ? stage.ensure(blocks, true, level) : stage.res.ensure(blocks * sizeof(CBlockInfo))) ||
             (e = csum.ensure(frames * 8)) || (e = results.ensure(frames * sizeof(b200z_compress_result))))
             return e;
         return 0;
@@ -2749,7 +2751,8 @@ static int compress_check(b200z_ctx *c, int level, int window_log, const b200z_d
         if (c) c->err = "compression levels Default, Better and Best are unimplemented!() in the reference";
         return B200Z_ERR_REFERENCE_WOULD_PANIC;
     }
-    if (!c || (level != B200Z_LEVEL_UNCOMPRESSED && level != B200Z_LEVEL_FASTEST && level != B200Z_LEVEL_LAZY)) return B200Z_ERR_INVALID_ARGUMENT;
+    if (!c || (level != B200Z_LEVEL_UNCOMPRESSED && level != B200Z_LEVEL_FASTEST && level != B200Z_LEVEL_LAZY && level != B200Z_LEVEL_OPT))
+        return B200Z_ERR_INVALID_ARGUMENT;
     if (window_log < B200Z_WINDOW_LOG_MIN || window_log > B200Z_WINDOW_LOG_MAX || (level == B200Z_LEVEL_UNCOMPRESSED && window_log != B200Z_WINDOW_LOG_MIN)) {
         c->err = "window_log outside [17, 27], or above 17 at level Uncompressed";
         return B200Z_ERR_INVALID_ARGUMENT;
@@ -2851,7 +2854,7 @@ extern "C" int b200z_compress_frames_batch_long(b200z_ctx *c, const uint8_t *inp
     CompressResources *rp = nullptr;
     if (int e = compress_get(c, &rp)) return e;
     CompressResources &r = *rp;
-    const bool fast = level != B200Z_LEVEL_UNCOMPRESSED;   // Fastest or LAZY: the blocks are parsed and encoded
+    const bool fast = level != B200Z_LEVEL_UNCOMPRESSED;   // Fastest, LAZY or OPT: the blocks are parsed and encoded
     int e = 0;
     if ((e = r.frames.ensure(nframes * sizeof(CFrame))) || (e = r.blocks.ensure(nblocks * sizeof(CBlock))) ||
         (e = r.ensure_submission(nframes, nblocks, level)))
@@ -3521,7 +3524,7 @@ struct b200z_frame_compressor {
     size_t desc_bytes() const { return res_off() + sizeof(b200z_compress_result); }
 };
 
-static int fc_valid_level(int level) { return (level >= 0 && level <= 4) || level == B200Z_LEVEL_LAZY; }   // Uncompressed .. Best, LAZY
+static int fc_valid_level(int level) { return (level >= 0 && level <= 4) || level == B200Z_LEVEL_LAZY || level == B200Z_LEVEL_OPT; }   // Uncompressed .. Best, LAZY, OPT
 static int fc_panic(b200z_ctx *c, const char *what) { c->err = what; return B200Z_ERR_REFERENCE_WOULD_PANIC; }
 
 extern "C" int b200z_frame_compressor_new(b200z_ctx *c, int level, int checksum, b200z_frame_compressor **out) {
@@ -3639,6 +3642,7 @@ static int fc_compress_fast(b200z_frame_compressor *fc, b200z_read_fn rd, void *
                             b200z_compress_result &r) {
     b200z_ctx *c = fc->ctx;
     if (int e = fc_prepare(fc)) return e;
+    if (int e = fc->stage.ensure(fc->chunk_blocks(), false, fc->level)) return e;   // OPT's chain slots, whenever the level became OPT
     const uint64_t C = fc->chunk, H = fc->hist_for(fc->window_log);
     cudaStream_t ks = c->stream;
     auto enqueue = [&](uint64_t k, int s, size_t n) -> int {
@@ -3669,7 +3673,7 @@ static int fc_compress_fast(b200z_frame_compressor *fc, b200z_read_fn rd, void *
         a.results = reinterpret_cast<b200z_compress_result *>(fc->p.d_desc[s].as<uint8_t>() + fc->res_off());
         a.input = din; a.output = fc->p.d_out[s].as<uint8_t>();
         fc->stage.bind(a);
-        a.nframes = 1; a.nblocks = m; a.level = fc->level;   // Fastest or LAZY
+        a.nframes = 1; a.nblocks = m; a.level = fc->level;   // Fastest, LAZY or OPT
         if (ns)
             if (int le = compress_ldm(c, fc->ldm, a, reinterpret_cast<const LSpan *>(fc->p.d_desc[s].as<uint8_t>() + fc->span_off()), ns, m,
                                       fc->window_log, ns * LDM_SPAN_CAP, ks))

@@ -3,8 +3,11 @@
 //   k_cmatch    : one CTA per 128 KiB block: greedy LZ77 parse into literals + sequences (two-table parallel parse)
 //                 (<DICT, true>: the LAZY level's parse, an extension: K-way tables, repeat candidates, a lazy choice;
 //                  <DICT, LAZY, true>: with the long-distance matches of ldm.cu forced into the parse, window_log > 17)
+//   k_copt      : OPT (an extension): in k_cmatch's place, a grid of the resident CTAs striding over the blocks: per block a hash chain
+//                 over the block and the 128 KiB before it, then one warp per segment parses it by a price-based forward DP
+//                 (<DICT, LONG>: as k_cmatch's)
 //   k_cenc      : one warp per block: Huffman literals, FSE sequences, the Raw / RLE / Compressed decision (encode.cuh)
-//                 (<TABLES, true>: LAZY, repeat-offset codes within each block first)
+//                 (<TABLES, true>: LAZY and OPT, repeat-offset codes within each block first)
 //   k_cxxh64    : content checksum of every frame's input (xxh64.cuh; four serial chains per frame)
 //   k_cassemble : one CTA per block: frame header, the block at its prefix-summed offset, the checksum, per-frame results
 //                 (<true>: one chunk of a streamed frame, blocks only; the host writes header, trailer and checksum)
@@ -19,6 +22,8 @@
 #include <cuda_runtime.h>
 #include <limits.h>
 #include <stdint.h>
+
+#include <algorithm>
 
 #include "compress.h"
 #include "encode.cuh"
@@ -45,6 +50,26 @@ constexpr uint32_t LZ_EMPTY = 0xffffu;
 constexpr uint32_t LZ_SMEM = (4u << LZ_T1_LOG) + CM_WARPS * (2u * LZ_WAYS << LZ_TAB_LOG);   // 224 KiB
 static_assert(LZ_SEED + ENC_BLOCK / CM_WARPS < LZ_EMPTY, "a table entry must fit below the empty mark");
 static_assert(LZ_WAYS == 6, "lz_push shifts three words");
+// the OPT parse (tests/copt.py states it rule by rule)
+constexpr uint32_t OPT_HASH_LOG = 13;   // H: the chain's hash
+constexpr uint32_t OPT_DEPTH = 24;      // D: chain entries a position visits
+constexpr uint32_t OPT_CANDS = 4;       // M: candidates kept per position
+constexpr uint32_t OPT_SUFF = 32;       // bytes a candidate is verified for; a candidate this long is taken at once
+constexpr uint32_t OPT_WIN = 256;       // W: nodes one DP spans before it closes
+constexpr uint32_t OPT_NODES = OPT_WIN + OPT_SUFF;      // node a + k for k < OPT_NODES: a DP's reach
+constexpr uint32_t OPT_PATH = OPT_WIN / ENC_MIN_MATCH + 1;   // the most matches a closed DP's path holds
+constexpr uint32_t OPT_INF = 1u << 30;
+constexpr uint32_t OPT_MATCH_W = 1024, OPT_OF_W = 512, OPT_REP_W0 = 256, OPT_REP_W1 = 512, OPT_REP_W2 = 768;   // prices in 1/256 bit
+constexpr int32_t OPT_NONE = INT_MIN, OPT_FIX = INT_MIN + 1;   // prev: no earlier position; none in the stripe (resolved next)
+constexpr uint32_t OPT_SMEM = CM_WARPS * (2u << OPT_HASH_LOG);  // the stripes' u16 heads (128 KiB), then the warps' DP state
+struct OptWarp {       // one warp's DP state (k_copt's second phase)
+    uint32_t cost[OPT_NODES], link[OPT_NODES], off[OPT_NODES], rep[3][OPT_NODES];   // link: from | length << 16 (0: a literal)
+    uint32_t cand[32 * OPT_CANDS];                                                  // the chunk's lists: length << 18 | offset
+    uint32_t path_pos[OPT_PATH], path_ml[OPT_PATH], path_off[OPT_PATH];
+};
+static_assert(CM_WARPS * sizeof(OptWarp) <= OPT_SMEM, "the DP state reuses the heads' shared memory");
+static_assert(OPT_SPAN / CM_WARPS <= 0xffffu, "a stripe position must fit below the empty head");
+static_assert(OPT_SUFF == 32 && OPT_SUFF - 1 <= 34, "one lane per length, and no length below OPT_SUFF has ML extra bits");
 
 __device__ __forceinline__ uint64_t load5(const uint8_t *p) {
     return (uint64_t)__ldg(p) | ((uint64_t)__ldg(p + 1) << 8) | ((uint64_t)__ldg(p + 2) << 16) | ((uint64_t)__ldg(p + 3) << 24) |
@@ -379,6 +404,278 @@ k_cmatch(const CBlock *__restrict__ blocks, const uint8_t *__restrict__ input, u
 }
 
 // ------------------------------------------------------------------------------------------------------------
+// k_copt (OPT, an extension, B200Z_LEVEL_OPT): the price-based parse.  The CTAs stride over the blocks; for each block:
+//   chain  prev[q] for every position q in [-min(back, 131072), n - 4) is the nearest earlier position of the frame with the same
+//          hash5(q, OPT_HASH_LOG), in the CTA's global slot.  Warp w builds stripe w of that range in position order 32 positions at
+//          a time (__match_any_sync finds a lane's predecessor inside the round, a u16 head table per stripe the one before), then
+//          the positions without one in their stripe take the last occurrence of the nearest earlier stripe's table.
+//   prices the block's byte histogram prices a literal; a match pays OPT_MATCH_W plus its offset's code bits, or a repeat's weight.
+//   parse  warp w parses segment w as a forward DP (opt_segment) over its parts between forced pieces.
+// The packing is k_cmatch's.  tests/copt.py states the rule; the GPU must produce exactly its sequences.
+// ------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t opt_log2(uint32_t x) {   // 256 floor(log2 x) + the 8 bits after the leading one (x >= 1)
+    const uint32_t k = 31 - __clz(x);
+    return 256 * k + ((k <= 8 ? x << (8 - k) : x >> (k - 8)) & 255u);
+}
+
+// the finder's list of each position cb + lane (q + 5 <= stop), lengths increasing, into wk.cand
+template <bool DICT>
+__device__ __forceinline__ void opt_chunk(OptWarp &wk, const int32_t *prev, int32_t lo, const CBlock &blk, const uint8_t *src, uint32_t cb,
+                                          uint32_t stop, const uint8_t *dict, const uint32_t *dtab, uint32_t dict_len, uint32_t lane) {
+    const uint32_t q = cb + lane;
+    uint32_t k0 = 0, k1 = 0, k2 = 0, k3 = 0, cnt = 0;
+    auto push = [&](uint32_t v) {
+        if (cnt == OPT_CANDS) { k0 = k1; k1 = k2; k2 = k3; cnt--; }   // the shortest drops out
+        if (cnt == 0) k0 = v; else if (cnt == 1) k1 = v; else if (cnt == 2) k2 = v; else k3 = v;
+        cnt++;
+    };
+    if (q + ENC_MIN_MATCH <= stop) {
+        const uint32_t lim = min(OPT_SUFF, stop - q);
+        uint32_t best = ENC_MIN_MATCH - 1;
+        int32_t c = prev[(int32_t)q - lo];
+        for (uint32_t seen = 0; c >= lo && (int32_t)q - c <= (int32_t)ENC_WINDOW && seen < OPT_DEPTH; seen++) {
+            const uint32_t ln = match_len(src + q, src + c, lim);
+            if (ln > best) {
+                push(ln << 18 | (uint32_t)((int32_t)q - c));
+                best = ln;
+                if (ln == lim) break;
+            }
+            c = prev[c - lo];
+        }
+        const uint32_t fpos = blk.back + q;
+        if (DICT && fpos < ENC_WINDOW) {
+            const uint32_t c3 = __ldg(dtab + hash5(src + q, CD_LOG));
+            const uint32_t off3 = fpos + dict_len - (c3 - 1);
+            if (c3 && off3 <= ENC_WINDOW) {
+                const uint32_t ln = match_len(src + q, dict + (c3 - 1), min(lim, dict_len - (c3 - 1)));
+                if (ln > best) push(ln << 18 | off3);
+            }
+        }
+    }
+    uint32_t *out = wk.cand + lane * OPT_CANDS;
+    out[0] = cnt > 0 ? k0 : 0u; out[1] = cnt > 1 ? k1 : 0u; out[2] = cnt > 2 ? k2 : 0u; out[3] = cnt > 3 ? k3 : 0u;
+    __syncwarp();
+}
+
+// the length of repeat o at i (>= 5, else 0), verified for min(OPT_SUFF, stop - i) bytes; the source must lie in the frame
+__device__ __forceinline__ uint32_t opt_rep(const uint8_t *src, uint32_t i, uint32_t o, uint32_t lim, uint32_t back, uint32_t lane) {
+    const bool ok = o && o <= back + i && o <= ENC_WINDOW;
+    const bool stop = !ok || lane >= lim || __ldg(src + i + lane) != __ldg(src + i + lane - o);
+    const uint32_t m = __ballot_sync(0xffffffffu, stop);
+    const uint32_t ln = m ? __ffs(m) - 1 : 32u;
+    return ok && ln >= ENC_MIN_MATCH ? ln : 0u;
+}
+
+// one warp's parse of segment [s, e) (see k_copt): the DPs of each part, forced pieces between them; staging as cmatch_lazy's
+template <bool DICT, bool LONG>
+__device__ __forceinline__ void opt_segment(OptWarp &wk, const int32_t *prev, int32_t lo, const uint32_t *lit, const CBlock &blk, const uint8_t *src,
+                                            uint32_t s, uint32_t e, const uint8_t *dict, const uint32_t *dtab, uint32_t dict_len, SeqRec *stage,
+                                            uint8_t *lstage, uint32_t *nseq_out, uint32_t *nlit_out, uint32_t *trail_out, LCursor &lc, uint32_t lane) {
+    uint32_t p = s, anchor = s, nseq = 0, nlit = 0;
+    uint32_t r0 = 0, r1 = 0, r2 = 0;   // the reps at p (0: none yet)
+    auto push_rep = [&](uint32_t o) {
+        if (o == r1) { r1 = r0; r0 = o; }
+        else if (o != r0) { r2 = r1; r1 = r0; r0 = o; }
+    };
+    auto emit = [&](uint32_t q, uint32_t ml, uint32_t off) {
+        for (uint32_t i = anchor + lane; i < q; i += 32) lstage[nlit + i - anchor] = __ldg(src + i);
+        if (lane == 0) stage[nseq] = SeqRec{q - anchor, ml, off};
+        nlit += q - anchor;
+        nseq++;
+        anchor = q + ml;
+    };
+    uint32_t stop = e;
+    if constexpr (LONG) { lc.next(); if (lc.has) stop = lc.cs; }
+    while (true) {
+        while (p < stop) {   // one DP from a = p
+            const uint32_t a = p;
+            uint32_t end = min(stop, a + OPT_WIN);
+            for (uint32_t k = lane; k < OPT_NODES; k += 32) wk.cost[k] = OPT_INF;
+            __syncwarp();
+            if (lane == 0) { wk.cost[0] = 0; wk.rep[0][0] = r0; wk.rep[1][0] = r1; wk.rep[2][0] = r2; }
+            uint32_t cb = a;
+            opt_chunk<DICT>(wk, prev, lo, blk, src, cb, stop, dict, dtab, dict_len, lane);
+            uint32_t tml = 0, toff = 0;   // a match taken at once at `end`
+            for (uint32_t i = a; i < end; i++) {
+                if (i >= cb + 32) { cb = i; opt_chunk<DICT>(wk, prev, lo, blk, src, cb, stop, dict, dtab, dict_len, lane); }
+                const uint32_t k = i - a, ci = wk.cost[k], x0 = wk.rep[0][k], x1 = wk.rep[1][k], x2 = wk.rep[2][k];
+                const uint32_t *cl = wk.cand + (i - cb) * OPT_CANDS;
+                const uint32_t c0 = cl[0], c1 = cl[1], c2 = cl[2], c3 = cl[3];
+                uint32_t l0 = 0, l1 = 0, l2 = 0;
+                if (i + ENC_MIN_MATCH <= stop) {
+                    const uint32_t lim = min(OPT_SUFF, stop - i);
+                    l0 = opt_rep(src, i, x0, lim, blk.back, lane);
+                    l1 = opt_rep(src, i, x1, lim, blk.back, lane);
+                    l2 = opt_rep(src, i, x2, lim, blk.back, lane);
+                }
+                // a candidate of OPT_SUFF bytes closes the DP: the longest, the first of rep0, rep1, rep2, the finder's on a tie
+                const uint32_t ctop = c3 ? c3 : c2 ? c2 : c1 ? c1 : c0;
+                if (l0 >= OPT_SUFF && l0 > tml) { tml = l0; toff = x0; }
+                if (l1 >= OPT_SUFF && l1 > tml) { tml = l1; toff = x1; }
+                if (l2 >= OPT_SUFF && l2 > tml) { tml = l2; toff = x2; }
+                if ((ctop >> 18) >= OPT_SUFF && (ctop >> 18) > tml) { tml = ctop >> 18; toff = ctop & 0x3ffffu; }
+                if (tml) { end = i; break; }
+                // lane l relaxes node i + l: the literal (l = 1), a match of l bytes (l >= 5)
+                uint32_t c = OPT_INF, off = 0;
+                if (lane == 1) c = ci + lit[__ldg(src + i)];
+                else if (lane >= ENC_MIN_MATCH) {
+                    uint32_t best = OPT_INF;
+                    if (l0 >= lane) { best = OPT_REP_W0; off = x0; }
+                    if (l1 >= lane && OPT_REP_W1 < best) { best = OPT_REP_W1; off = x1; }
+                    if (l2 >= lane && OPT_REP_W2 < best) { best = OPT_REP_W2; off = x2; }
+                    const uint32_t f = (c0 >> 18) >= lane ? c0 : (c1 >> 18) >= lane ? c1 : (c2 >> 18) >= lane ? c2 : (c3 >> 18) >= lane ? c3 : 0u;
+                    if (f) {
+                        const uint32_t o = f & 0x3ffffu, pr = 256 * (31 - __clz(o + 3)) + OPT_OF_W;
+                        if (pr < best) { best = pr; off = o; }
+                    }
+                    if (best != OPT_INF) c = ci + OPT_MATCH_W + best;
+                }
+                const uint32_t t = k + lane;
+                if (c != OPT_INF && c < wk.cost[t]) {
+                    wk.cost[t] = c;
+                    wk.link[t] = k | (lane == 1 ? 0u : lane << 16);
+                    wk.off[t] = off;
+                    if (lane == 1 || off == x0) { wk.rep[0][t] = x0; wk.rep[1][t] = x1; wk.rep[2][t] = x2; }
+                    else if (off == x1) { wk.rep[0][t] = off; wk.rep[1][t] = x0; wk.rep[2][t] = x2; }
+                    else { wk.rep[0][t] = off; wk.rep[1][t] = x0; wk.rep[2][t] = x1; }
+                }
+                __syncwarp();
+            }
+            // close at `end`: the path's matches (lane 0 walks it back), then the taken match
+            uint32_t np = 0;
+            if (lane == 0) {
+                for (uint32_t k = end - a; k;) {
+                    const uint32_t lk = wk.link[k], f = lk & 0xffffu;
+                    if (lk >> 16) { wk.path_pos[np] = a + f; wk.path_ml[np] = lk >> 16; wk.path_off[np] = wk.off[k]; np++; }
+                    k = f;
+                }
+            }
+            np = __shfl_sync(0xffffffffu, np, 0);
+            __syncwarp();
+            for (uint32_t j = np; j-- > 0;) emit(wk.path_pos[j], wk.path_ml[j], wk.path_off[j]);
+            r0 = wk.rep[0][end - a]; r1 = wk.rep[1][end - a]; r2 = wk.rep[2][end - a];
+            p = end;
+            if (tml) {
+                const uint32_t fpos = blk.back + end;
+                const uint32_t xlim = DICT && toff > fpos ? min(stop - end, toff - fpos) : stop - end;   // a dictionary source: to its end
+                const uint32_t ml = extend_match<DICT>(src, end, toff, tml, xlim, blk.back, dict, dict_len, lane);
+                emit(end, ml, toff);
+                push_rep(toff);
+                p = end + ml;
+            }
+            __syncwarp();
+        }
+        if constexpr (!LONG) break;
+        else {
+            if (!lc.has) break;
+            emit(lc.cs, lc.ce - lc.cs, lc.off);   // the forced piece, taken as any match is
+            push_rep(lc.off);
+            p = lc.ce;
+            lc.next();
+            stop = lc.has ? lc.cs : e;
+            __syncwarp();
+        }
+    }
+    for (uint32_t i = anchor + lane; i < e; i += 32) lstage[nlit + i - anchor] = __ldg(src + i);
+    if (lane == 0) { *nseq_out = nseq; *nlit_out = nlit + (e - anchor); *trail_out = e - anchor; }
+}
+
+template <bool DICT, bool LONG>
+__global__ void __launch_bounds__(CM_THREADS, 1)
+k_copt(const CBlock *__restrict__ blocks, uint32_t nblocks, const uint8_t *__restrict__ input, uint8_t *__restrict__ lit_stage,
+       SeqRec *__restrict__ seq_stage, uint8_t *__restrict__ lits, SeqRec *__restrict__ seqs, CBlockInfo *__restrict__ info,
+       const uint8_t *__restrict__ dict, const uint32_t *__restrict__ dtab, uint32_t dict_len, int32_t *opt_prev,
+       const LForced *__restrict__ lforced, const uint32_t *__restrict__ lf_off, const uint32_t *__restrict__ lf_cnt) {
+    extern __shared__ __align__(16) uint8_t smem_co[];
+    __shared__ uint32_t s_nseq[CM_WARPS], s_nlit[CM_WARPS], s_trail[CM_WARPS], s_add[CM_WARPS], s_soff[CM_WARPS], s_loff[CM_WARPS];
+    __shared__ uint32_t s_lit[256];
+    const uint32_t tid = threadIdx.x, w = tid >> 5, lane = tid & 31;
+    int32_t *prev = opt_prev + (size_t)blockIdx.x * OPT_SPAN;
+    uint16_t *heads = reinterpret_cast<uint16_t *>(smem_co);
+    OptWarp &wk = reinterpret_cast<OptWarp *>(smem_co)[w];
+    for (uint32_t b = blockIdx.x; b < nblocks; b += gridDim.x) {
+        const CBlock blk = blocks[b];
+        const uint8_t *src = input + blk.src_off;
+        const uint32_t n = blk.size;
+        bool same = true;
+        for (uint32_t i = tid; i < n; i += CM_THREADS) same &= __ldg(src + i) == __ldg(src);
+        same = __syncthreads_and(same);
+        if (n == 0 || same) {
+            if (tid == 0) info[b] = CBlockInfo{n, 0, n ? 1u : 0u, 0};
+            continue;
+        }
+        // prices: the block's byte histogram
+        for (uint32_t i = tid; i < 256; i += CM_THREADS) s_lit[i] = 0;
+        for (uint32_t i = tid; i < CM_WARPS << OPT_HASH_LOG; i += CM_THREADS) heads[i] = 0xffffu;
+        __syncthreads();
+        for (uint32_t i = tid; i < n; i += CM_THREADS) atomicAdd(&s_lit[__ldg(src + i)], 1u);
+        // the chain, stripe w
+        const int32_t lo = -(int32_t)min(blk.back, ENC_WINDOW), hi = (int32_t)n - 4;
+        const int32_t slen = (hi - lo + (int32_t)CM_WARPS - 1) / (int32_t)CM_WARPS;
+        const int32_t s0 = lo + (int32_t)w * slen, s1 = min(hi, s0 + slen);
+        uint16_t *hd = heads + (w << OPT_HASH_LOG);
+        for (int32_t c0 = s0; c0 < s1; c0 += 32) {
+            const int32_t q = c0 + (int32_t)lane;
+            const bool valid = q < s1;
+            const uint32_t h = valid ? hash5(src + q, OPT_HASH_LOG) : (1u << OPT_HASH_LOG) + lane;
+            const uint32_t grp = __match_any_sync(0xffffffffu, h), lower = grp & ((1u << lane) - 1);
+            int32_t pv = OPT_FIX;
+            if (lower) pv = c0 + 31 - __clz(lower);
+            else if (valid && hd[h] != 0xffffu) pv = s0 + hd[h];
+            __syncwarp();
+            if (valid && lane == 31 - __clz(grp)) hd[h] = (uint16_t)(q - s0);
+            if (valid) prev[q - lo] = pv;
+            __syncwarp();
+        }
+        __syncthreads();
+        if (tid < 256) s_lit[tid] = s_lit[tid] ? opt_log2(n) - opt_log2(s_lit[tid]) : OPT_INF;
+        for (int32_t q = s0 + (int32_t)lane; q < s1; q += 32) {
+            if (prev[q - lo] != OPT_FIX) continue;
+            const uint32_t h = hash5(src + q, OPT_HASH_LOG);
+            int32_t pv = OPT_NONE;
+            for (int32_t v = (int32_t)w - 1; v >= 0; v--) {
+                const uint32_t r = heads[((uint32_t)v << OPT_HASH_LOG) + h];
+                if (r != 0xffffu) { pv = lo + v * slen + (int32_t)r; break; }
+            }
+            prev[q - lo] = pv;
+        }
+        __syncthreads();   // the chain is complete; the heads' memory becomes the warps' DP state
+        const uint32_t seglen = (n + CM_WARPS - 1) / CM_WARPS;
+        const uint32_t s = min(n, w * seglen), e = min(n, s + seglen);
+        LCursor lc{};
+        if constexpr (LONG) lc = LCursor{lforced + lf_off[b], 0, lf_cnt[b], s, e, 0, 0, 0, false};
+        {
+            SeqRec *stage = seq_stage + ((size_t)b * CM_WARPS + w) * CSEG_SEQS;
+            uint8_t *lstage = lit_stage + (size_t)b * ENC_BLOCK + s;
+            opt_segment<DICT, LONG>(wk, prev, lo, s_lit, blk, src, s, e, dict, dtab, dict_len, stage, lstage, s_nseq + w, s_nlit + w, s_trail + w, lc, lane);
+        }
+        __syncthreads();
+        if (tid == 0) {   // k_cmatch's packing
+            uint32_t carry = 0, so = 0, lo2 = 0;
+            for (uint32_t v = 0; v < CM_WARPS; v++) {
+                s_soff[v] = so; s_loff[v] = lo2;
+                so += s_nseq[v]; lo2 += s_nlit[v];
+                if (s_nseq[v]) { s_add[v] = carry; carry = s_trail[v]; }
+                else { s_add[v] = 0; carry += s_trail[v]; }
+            }
+            info[b] = CBlockInfo{lo2, so, 0, 0};
+        }
+        __syncthreads();
+        SeqRec *stage = seq_stage + ((size_t)b * CM_WARPS + w) * CSEG_SEQS;
+        uint8_t *lstage = lit_stage + (size_t)b * ENC_BLOCK + s;
+        SeqRec *out = seqs + (size_t)b * CBLOCK_SEQS + s_soff[w];
+        for (uint32_t i = lane; i < s_nseq[w]; i += 32) {
+            SeqRec r = stage[i];
+            if (i == 0) r.ll += s_add[w];
+            out[i] = r;
+        }
+        uint8_t *lout = lits + (size_t)b * ENC_BLOCK + s_loff[w];
+        for (uint32_t i = lane; i < s_nlit[w]; i += 32) lout[i] = lstage[i];
+        __syncthreads();   // before the next block's histogram, heads and counts
+    }
+}
+
+// ------------------------------------------------------------------------------------------------------------
 // k_cenc: one warp per block encodes its literals and sequences (encode_block) into the block's staging slot and decides the
 // block type: RLE when all bytes are equal, Compressed when smaller than the input block, else Raw.  A formatted dictionary's
 // tables (dt, B200Z_FLAG_DICT_TABLES) go to a frame's first block only (back == 0); without them (TABLES = false) encode_block gets
@@ -540,6 +837,8 @@ k_dstats(const CBlockInfo *__restrict__ info, const uint8_t *__restrict__ lits, 
         if (h[i]) atomicAdd(&counts[i], (unsigned long long)h[i]);
 }
 
+static uint32_t g_opt_ctas = 1;   // init_compress_kernels: the SMs times k_copt's CTAs per SM
+
 static uint32_t cdiv_u(uint64_t a, uint32_t b) { return (uint32_t)((a + b - 1) / b); }
 
 int launch_dict_stats(const CompressArgs &a, unsigned long long *counts, cudaStream_t s, uint64_t *launched) {
@@ -563,8 +862,19 @@ int init_compress_kernels() {
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cmatch<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CM_SMEM);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cmatch<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LZ_SMEM);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_cmatch<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LZ_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_copt<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OPT_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_copt<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OPT_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_copt<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OPT_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_copt<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OPT_SMEM);
+    int dev = 0, sms = 0, per = 0;
+    if (e == cudaSuccess) e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, k_copt<true, true>, CM_THREADS, OPT_SMEM);
+    if (e == cudaSuccess) g_opt_ctas = (uint32_t)std::max(1, sms * per);
     return (int)e;
 }
+
+uint32_t opt_ctas() { return g_opt_ctas; }
 
 int launch_dict_table(const uint8_t *dict, uint32_t len, uint32_t *dtab, cudaStream_t s, uint64_t *launched) {
     int e = (int)cudaMemsetAsync(dtab, 0, sizeof(uint32_t) << CD_LOG, s);
@@ -579,11 +889,15 @@ int launch_dict_table(const uint8_t *dict, uint32_t len, uint32_t *dtab, cudaStr
 const char *const kCompressStageNames[kCompressStages] = {"k_cmatch", "k_cenc", "k_cxxh64", "k_cassemble"};
 
 int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s, uint64_t *launched) {
-    const bool lazy = a.level == B200Z_LEVEL_LAZY;
+    const bool lazy = a.level == B200Z_LEVEL_LAZY, opt = a.level == B200Z_LEVEL_OPT;
     switch (stage) {
     case 0:
         if (!a.level || !a.nblocks) return 0;
-        if (a.lf_cnt) {
+        if (opt) {
+            auto k = a.lf_cnt ? (a.dtab ? k_copt<true, true> : k_copt<false, true>) : (a.dtab ? k_copt<true, false> : k_copt<false, false>);
+            k<<<std::min(a.nblocks, g_opt_ctas), CM_THREADS, OPT_SMEM, s>>>(a.blocks, a.nblocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info,
+                                                                         a.dict, a.dtab, a.dict_len, a.opt_prev, a.lforced, a.lf_off, a.lf_cnt);
+        } else if (a.lf_cnt) {
             const uint32_t smem = lazy ? LZ_SMEM : CM_SMEM;
             auto k = lazy ? (a.dtab ? k_cmatch<true, true, true> : k_cmatch<false, true, true>) : (a.dtab ? k_cmatch<true, false, true> : k_cmatch<false, false, true>);
             k<<<a.nblocks, CM_THREADS, smem, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, a.dict, a.dtab, a.dict_len,
@@ -594,9 +908,9 @@ int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s, uint
         } else if (a.dtab) k_cmatch<true, false><<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, a.dict, a.dtab, a.dict_len);
         else k_cmatch<false, false><<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, nullptr, nullptr, 0);
         break;
-    case 1:   // LAZY's repeat-offset records go to seq_stage, free once k_cmatch is done
+    case 1:   // LAZY's and OPT's repeat-offset records go to seq_stage, free once k_cmatch / k_copt is done
         if (!a.level || !a.nblocks) return 0;
-        if (lazy) {
+        if (lazy || opt) {
             if (a.etab) k_cenc<true, true><<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res, a.etab, a.seq_stage);
             else k_cenc<false, true><<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res, nullptr, a.seq_stage);
         } else if (a.etab) k_cenc<true, false><<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res, a.etab, nullptr);

@@ -57,7 +57,14 @@ struct CompressArgs {
     const LForced *lforced;
     const uint32_t *lf_off, *lf_cnt;
     uint32_t window_log;
+    // OPT (EXTENSION): k_copt's chain of the block it works on, one OPT_SPAN slot per CTA of its grid (opt_ctas())
+    int32_t *opt_prev;
 };
+
+// ---- OPT (compress.cu): a CTA's chain covers the block and the ENC_WINDOW bytes before it
+constexpr uint32_t OPT_SPAN = ENC_WINDOW + ENC_BLOCK;
+// k_copt's grid: the CTAs resident on the device at once (after init_compress_kernels); the CTAs stride over the blocks
+uint32_t opt_ctas();
 
 // ---- long-distance matches (ldm.cu; DESIGN.md section 4.11, tests/cldm.py)
 constexpr uint32_t LDM_LEN = 64;          // bytes hashed at an anchor (the 64 ending at it), verified, and the least a kept match holds
