@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """bench_compress.py -- input GB/s of the batch compressor (b200z_compress_frames_batch, ruzstd's Fastest level, checksum on).
 
-    python bench_compress.py [--steps K] [--warmup W] [--skip-cpu] [--level fastest|lazy|opt]
+    python bench_compress.py [--steps K] [--warmup W] [--skip-cpu] [--level fastest|lazy|opt|ultra] [--window-log N]
 
 The workload is the C2b plaintext (1 GiB of enwik9-shaped text, datagen.c2_text_plain), device-resident, in two shapes:
 8192 frames of 128 KiB and one 1 GiB frame (C2a's plaintext shape, where the content checksum is four serial chains).
@@ -9,7 +9,10 @@ Prints one JSON line: per shape the input GB/s (CUDA events around the call, med
 milliseconds, (input + output bytes) / t against the HBM peak, the card's name and power limit, and `cpu_baseline`:
 libzstd 1.5.5 level 1 on the same 128 KiB pieces, one thread and all host threads.  --level lazy measures the LAZY extension
 level instead, and adds libzstd level 3 to the baseline; --level opt measures the OPT extension level and adds libzstd levels 3
-and 16 (btopt, the price-based parse).  Nothing is written to the tree.
+and 16 (btopt, the price-based parse).  --level ultra measures the ULTRA extension level on the one-frame shape at --window-log
+(23 by default) against OPT at the same window_log, the two alternated step by step in one run; its far-stage kernels' times come
+from torch.profiler, and the baselines are libzstd levels 3, 16 and 19 at that window_log (one frame per 64 MiB piece, the pieces
+on all host threads).  Nothing is written to the tree.
 """
 import argparse
 import json
@@ -131,6 +134,87 @@ def run_compress(args):
     print(json.dumps(line))
 
 
+FAR_KERNELS = ("k_fkey", "k_lhist", "k_lscan", "k_lscatter", "k_fstart", "k_copt", "k_lanchor", "k_lcand", "k_lblock")
+
+
+def libzstd_window_baseline(plain, level, window_log, piece=64 << 20):
+    """libzstd 1.5.5 at `level` and window_log, one frame per `piece` bytes, the pieces on all host threads."""
+    import datagen as G
+    from concurrent.futures import ThreadPoolExecutor
+    pieces = [plain[i:i + piece].tobytes() for i in range(0, len(plain), piece)]
+    with ThreadPoolExecutor(max_workers=bench.host_threads()) as ex:
+        t0 = time.perf_counter()
+        sizes = list(ex.map(lambda d: len(G.compress(d, level=level, window_log=window_log)), pieces))
+        dt = time.perf_counter() - t0
+    return {"kind": f"libzstd 1.5.5 level {level}, window_log {window_log}, {piece >> 20} MiB frames", "all_cores_GBps": len(plain) / dt / GB,
+            "cores": bench.host_threads(), "ratio": len(plain) / sum(sizes)}
+
+
+def run_ultra(args):
+    """ULTRA and OPT on one frame of the C2b plaintext at --window-log, alternated; each output decodes on the GPU to the input."""
+    import torch
+    import _pkg
+    import datagen
+    from torch.profiler import ProfilerActivity, profile
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_compress.py needs a CUDA device: the product path has no CPU fallback")
+    pkg = _pkg.load()
+    ctx = pkg.Context(0)
+    total, wl = args.c2a_bytes, args.window_log
+    plain = datagen.c2_text_plain(total)
+    d_in = torch.from_numpy(plain).cuda()
+    io = np.zeros(1, dtype=pkg.binding.COMPRESS_IO_DTYPE)
+    cap = pkg.compress_bound(total)
+    io[0] = (0, total, 0, cap)
+    d_out = torch.empty(cap, dtype=torch.uint8, device="cuda")
+    line = {"metric": "compress_GBps", "unit": "GB/s", "level": "ULTRA", "window_log": wl, "checksum": True, "card": card_info(),
+            "input_bytes": total, "frames": 1, "levels": {}}
+    levels = (("ULTRA", pkg.ULTRA), ("OPT", pkg.OPT))
+    for name, level in levels:
+        res = pkg.compress_frames(ctx, d_in, io, d_out, level, window_log=wl)
+        assert (res["status"] == 0).all()
+        dio = np.zeros(1, dtype=pkg.binding.FRAME_IO_DTYPE)
+        dio["src_off"], dio["src_size"], dio["out_off"], dio["out_cap"] = 0, res["dst_size"], 0, total
+        back = torch.empty(total + 16, dtype=torch.uint8, device="cuda")
+        dres = pkg.decode_frames(ctx, d_out, dio, back)
+        assert (dres["status"] == 0).all() and torch.equal(back[:total], d_in), f"{name}: GPU decode differs from the input"
+        del back
+        line["levels"][name] = {"ratio": total / int(res["dst_size"][0]), "output_bytes": int(res["dst_size"][0]), "times": []}
+        for _ in range(args.warmup):
+            pkg.compress_frames(ctx, d_in, io, d_out, level, window_log=wl)
+    stream = torch.cuda.ExternalStream(ctx.stream())
+    for _ in range(args.steps):
+        for name, level in levels:
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record(stream)
+            pkg.compress_frames(ctx, d_in, io, d_out, level, window_log=wl)
+            b.record(stream)
+            b.synchronize()
+            line["levels"][name]["times"].append(a.elapsed_time(b))
+    for name, level in levels:
+        r = line["levels"][name]
+        t = float(np.median(r["times"]))
+        r.update({"ms": t, "ms_min_max": [min(r["times"]), max(r["times"])], "value": total / (t / 1e3) / GB})
+        ctx.set_flags(pkg.binding.FLAG_PROFILE)
+        pkg.compress_frames(ctx, d_in, io, d_out, level, window_log=wl)
+        r["stage_ms"] = pkg.compress_profile(ctx)
+        ctx.set_flags(0)
+        with profile(activities=[ProfilerActivity.CUDA]) as pr:
+            pkg.compress_frames(ctx, d_in, io, d_out, level, window_log=wl)
+            torch.cuda.synchronize()
+        ms = {}
+        for ev in pr.key_averages():
+            k = next((k for k in FAR_KERNELS if k in ev.key), None)
+            if k:
+                ms[k] = ms.get(k, 0.0) + ev.device_time_total / 1e3
+        r["kernel_ms_profiler"] = ms
+    line["value"], line["ratio"] = line["levels"]["ULTRA"]["value"], line["levels"]["ULTRA"]["ratio"]
+    if not args.skip_cpu:
+        line["cpu_baselines"] = [libzstd_window_baseline(plain, lv, wl) for lv in (3, 16, 19)]
+    ctx.close()
+    print(json.dumps(line))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=10)
@@ -138,8 +222,10 @@ def main():
     ap.add_argument("--frame-bytes", type=int, default=131072)
     ap.add_argument("--c2a-bytes", type=int, default=1 << 30, help="total plaintext bytes (both shapes)")
     ap.add_argument("--skip-cpu", action="store_true")
-    ap.add_argument("--level", choices=("fastest", "lazy", "opt"), default="fastest")
-    run_compress(ap.parse_args())
+    ap.add_argument("--level", choices=("fastest", "lazy", "opt", "ultra"), default="fastest")
+    ap.add_argument("--window-log", type=int, default=23, help="--level ultra: the window_log of both levels and the baselines")
+    args = ap.parse_args()
+    (run_ultra if args.level == "ultra" else run_compress)(args)
     return 0
 
 

@@ -584,6 +584,19 @@ typedef struct b200z_compress_result {
  * 132 SMs), allocated by the first compression at this level.  Accepted wherever LAZY is; b200z_dict_finalize keeps the
  * Fastest parse.  Levels 6, 8 and up stay B200Z_ERR_INVALID_ARGUMENT. */
 #define B200Z_LEVEL_OPT 7
+/* EXTENSION: ULTRA, OPT's parse with a far finder.  Where a frame's window Wf (2^its Window_Descriptor exponent) is larger than
+ * 131072 -- window_log > 17 and a frame larger than 131072 bytes, or the stream compressor at window_log > 17 -- each position's
+ * finder, after OPT's chain and unless that found a 32-byte match, also walks the earlier positions of the frame with the same
+ * 32-bit hash of their 8 bytes (key8; a position is keyed when its 8 bytes end inside its 128 KiB block), nearest first from
+ * the first beyond 131072, at most 8 of them and none beyond Wf; and a repeat offset reaches up to Wf.  Elsewhere (window_log 17,
+ * frames of 131072 bytes or fewer, the seekable writers) ULTRA writes OPT's frames and launches OPT's kernels.
+ * The far stage runs per group of whole blocks -- at most B200Z_PIPELINE_CHUNK_BYTES (64 MiB by default, rounded down to whole
+ * blocks) of the submission's blocks, or one stream chunk -- before each group's k_copt: k_fkey, the long-distance matches'
+ * radix sort (four passes of k_lhist, k_lscan, k_lscatter) and k_fstart, 14 kernels, then one k_copt per group.  These kernels
+ * are counted in b200z_ctx_kernel_launches; b200z_compress_last_profile's stage 0 is the sum of the groups' k_copt times only.
+ * Its memory, kept with the context (stream compressor: with the compressor), is 20 bytes per keyed position of the largest
+ * group (the group's bytes and the Wf before it) and 16 per block.  Accepted wherever OPT is. */
+#define B200Z_LEVEL_ULTRA 10
 /* context flag: b200z_compress_frames_batch records a CUDA event between its kernels and keeps each kernel's milliseconds
  * for b200z_compress_last_profile (profiling aid for bench.py; it synchronises anyway) */
 #define B200Z_FLAG_PROFILE 2u
@@ -601,7 +614,7 @@ size_t b200z_compress_bound(size_t src_size);
  * content checksum.  Returns 0 when the submission ran (results[nframes] filled).  Checked before any launch:
  * B200Z_ERR_INVALID_ARGUMENT for a range outside `input` / `output`, dst_cap < b200z_compress_bound(src_size), overlapping
  * destination ranges or an unknown level; B200Z_ERR_REFERENCE_WOULD_PANIC for the levels the reference does not implement.
- * Levels: Uncompressed, Fastest and the extensions B200Z_LEVEL_LAZY and B200Z_LEVEL_OPT. */
+ * Levels: Uncompressed, Fastest and the extensions B200Z_LEVEL_LAZY, B200Z_LEVEL_OPT and B200Z_LEVEL_ULTRA. */
 int b200z_compress_frames_batch(b200z_ctx *ctx, const uint8_t *input, size_t input_len, int input_mem,
                                 const b200z_compress_io *frames, size_t nframes, int level, int checksum,
                                 uint8_t *output, size_t output_cap, int output_mem, b200z_compress_result *results);
@@ -665,10 +678,10 @@ int b200z_compress_last_profile(const b200z_ctx *ctx, float *stage_ms, size_t n)
  * written, and the compressor stays usable.  Hashing and matching state reset with every compress.
  * ---------------------------------------------------------------------------------------------------------- */
 typedef struct b200z_frame_compressor b200z_frame_compressor;
-/* FrameCompressor::new :77.  B200Z_ERR_INVALID_ARGUMENT for a level outside 0-4, B200Z_LEVEL_LAZY and B200Z_LEVEL_OPT */
+/* FrameCompressor::new :77.  B200Z_ERR_INVALID_ARGUMENT for a level outside 0-4, B200Z_LEVEL_LAZY, B200Z_LEVEL_OPT and B200Z_LEVEL_ULTRA */
 int b200z_frame_compressor_new(b200z_ctx *ctx, int level, int checksum, b200z_frame_compressor **out);
 void b200z_frame_compressor_free(b200z_frame_compressor *fc);
-int b200z_frame_compressor_set_compression_level(b200z_frame_compressor *fc, int level);   /* :263; 0-4, LAZY or OPT, else INVALID_ARGUMENT */
+int b200z_frame_compressor_set_compression_level(b200z_frame_compressor *fc, int level);   /* :263; 0-4, LAZY, OPT or ULTRA, else INVALID_ARGUMENT */
 int b200z_frame_compressor_compression_level(const b200z_frame_compressor *fc);            /* :273 */
 /* EXTENSION: long-distance matches up to 2^window_log bytes back (b200z_compress_frames_batch_long's rule) from the next compress
  * on; window_log in [17, 27], else B200Z_ERR_INVALID_ARGUMENT.  The frame's Window_Descriptor is 2^window_log (its size is unknown

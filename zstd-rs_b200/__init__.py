@@ -1,5 +1,5 @@
 """zstd-rs_b200 -- GPU-native (H100, sm_90a) zstd block decompressor behind ruzstd's FrameDecoder / StreamingDecoder API,
-a batch compressor at ruzstd's Uncompressed and Fastest levels and extension levels LAZY and OPT (compress_frames / compress_to_vec; with
+a batch compressor at ruzstd's Uncompressed and Fastest levels and extension levels LAZY, OPT and ULTRA (compress_frames / compress_to_vec; with
 long-distance matches up to 2^27 bytes back through window_log, as the stream compressor), a stream compressor behind
 ruzstd's FrameCompressor / encoding::compress API (FrameCompressor, compress), and a raw-content
 dictionary trainer in place of ruzstd::dictionary (create_raw_dict, create_raw_dict_from_source, create_raw_dict_from_dir)
@@ -16,7 +16,7 @@ There is no CPU decode path: every decode call needs a CUDA device and fails lou
 Import name: ``zstd_rs_b200`` (the directory name has a hyphen; see ``_pkg.py`` at the repo root).
 """
 from .binding import (  # noqa: F401
-    ALL, FASTEST, LAZY, OPT, UNCOMPRESSED, UPTO_BLOCKS, UPTO_BYTES, AllBatch, B200ZError, Batch, Context, Dictionary, FrameCompressor, FrameDecoder,
+    ALL, FASTEST, LAZY, OPT, ULTRA, UNCOMPRESSED, UPTO_BLOCKS, UPTO_BYTES, AllBatch, B200ZError, Batch, Context, Dictionary, FrameCompressor, FrameDecoder,
     SeekableArchive, StreamingDecoder, build, compress, compress_bound, compress_frames, compress_profile, compress_seekable, compress_seekable_stream, compress_to_vec, create_dict, create_raw_dict,
     create_raw_dict_from_dir,
     create_raw_dict_from_source, decode_all, decode_all_batch, decode_all_stream, decode_blocks, decode_frames,

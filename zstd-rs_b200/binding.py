@@ -34,6 +34,7 @@ HUF_DEBUG_BYTES, FSE_DEBUG_BYTES = 3088, 1040   # B200Z_DEBUG_HUF_BYTES / B200Z_
 UNCOMPRESSED, FASTEST = 0, 1   # CompressionLevel (ruzstd encoding/mod.rs:24-67); Default / Better / Best are not implemented there
 LAZY = 5   # EXTENSION (B200Z_LEVEL_LAZY): a deeper parse with a lazy choice and repeat offsets; not ruzstd's output
 OPT = 7    # EXTENSION (B200Z_LEVEL_OPT): a price-based parse over full-window match chains; not ruzstd's output
+ULTRA = 10  # EXTENSION (B200Z_LEVEL_ULTRA): OPT's parse with far matches from the frame's whole window (window_log > 17)
 
 
 class FrameIO(C.Structure):

@@ -12,6 +12,7 @@
 #include <memory>
 #include <new>
 #include <string>
+#include <deque>
 #include <vector>
 
 #include "../../include/b200zstd.h"
@@ -2578,14 +2579,14 @@ extern "C" const char *b200z_compress_stage_name(int stage) { return stage >= 0 
 // k_cmatch / k_cenc staging for nblocks blocks (CompressArgs), and at OPT k_copt's chain slots
 struct CompressStaging {
     DevBuf lit_stage, seq_stage, lits, seqs, info, res;
-    DevBuf opt_prev;   // OPT: opt_ctas() slots of OPT_SPAN words, allocated by the first OPT submission and kept
+    DevBuf opt_prev;   // OPT and ULTRA: opt_ctas() slots of OPT_SPAN words, allocated by the first such submission and kept
     int ensure(uint64_t nblocks, bool grow, int level = B200Z_LEVEL_FASTEST) {
         int e = 0;
         if ((e = lit_stage.ensure(nblocks * ENC_BLOCK, grow)) || (e = seq_stage.ensure(nblocks * CBLOCK_SEQS * sizeof(SeqRec), grow)) ||
             (e = lits.ensure(nblocks * ENC_BLOCK, grow)) || (e = seqs.ensure(nblocks * CBLOCK_SEQS * sizeof(SeqRec), grow)) ||
             (e = info.ensure(nblocks * sizeof(CBlockInfo), grow)) || (e = res.ensure(nblocks * sizeof(CBlockInfo), grow)))
             return e;
-        if (level == B200Z_LEVEL_OPT && (e = opt_prev.ensure((uint64_t)opt_ctas() * OPT_SPAN * sizeof(int32_t)))) return e;
+        if ((level == B200Z_LEVEL_OPT || level == B200Z_LEVEL_ULTRA) && (e = opt_prev.ensure((uint64_t)opt_ctas() * OPT_SPAN * sizeof(int32_t)))) return e;
         return 0;
     }
     void bind(CompressArgs &a) const {
@@ -2672,6 +2673,46 @@ struct LdmBufs {
     }
 };
 
+// ULTRA's far stage (compress.h): the largest group's pairs, sort counts and walk starts, and the pieces and per-block FBlocks
+struct FarBufs {
+    DevBuf pieces, fblk, total, keys[2], vals[2], hist, start;
+    // 16 bytes per pair, 4 per virtual position, 4 per 16 pairs of digit counts, and the pieces and blocks
+    int ensure(uint64_t npairs, uint64_t nvirt, uint64_t npieces, uint64_t nblocks, bool grow = true) {
+        const size_t n = std::max<uint64_t>(npairs, 1);
+        int e = 0;
+        for (int i = 0; i < 2 && !e; i++)
+            if ((e = keys[i].ensure(n * 4, grow)) || (e = vals[i].ensure(n * 4, grow))) return e;
+        if ((e = hist.ensure((LdmBufs::tiles((uint32_t)n) * 256 + 1) * 4, grow)) || (e = start.ensure(std::max<uint64_t>(nvirt, 1) * 4, grow)) ||
+            (e = total.ensure(4, grow)) || (e = pieces.ensure(std::max<uint64_t>(npieces, 1) * sizeof(FPiece), grow)) ||
+            (e = fblk.ensure(std::max<uint64_t>(nblocks, 1) * sizeof(FBlock), grow)))
+            return e;
+        return 0;
+    }
+    FarArgs args(const uint8_t *input, const FPiece *d_pieces, uint32_t npieces, uint32_t npairs) const {
+        FarArgs f{};
+        f.input = input; f.pieces = d_pieces; f.npieces = npieces; f.npairs = npairs; f.total = total.as<uint32_t>();
+        for (int i = 0; i < 2; i++) { f.keys[i] = keys[i].as<uint32_t>(); f.vals[i] = vals[i].as<uint32_t>(); }
+        f.hist = hist.as<uint32_t>(); f.start = start.as<uint32_t>();
+        return f;
+    }
+    void bind(CompressArgs &a, const FBlock *d_fblk) const {
+        a.fblk = d_fblk; a.fkeys = keys[0].as<uint32_t>(); a.fvals = vals[0].as<uint32_t>(); a.fstart = start.as<uint32_t>();
+    }
+};
+// the pieces of one group: adds FPiece{off, vbase, pbase, size} for a 128 KiB block and moves vbase and pbase past it
+static void far_piece(std::vector<FPiece> &pc, uint64_t off, uint32_t size, uint64_t &vbase, uint64_t &pbase) {
+    pc.push_back(FPiece{off, (uint32_t)vbase, (uint32_t)pbase, size, 0});
+    vbase += size;
+    pbase += size >= FAR_KEY ? size - (FAR_KEY - 1) : 0;
+}
+// the group size: B200Z_PIPELINE_CHUNK_BYTES rounded down to whole blocks (64 MiB by default), so that a group's virtual positions
+// (its bytes and at most 2^27 before them) fit in 32 bits
+static uint64_t far_group_bytes() {
+    uint64_t C = 64ull << 20;
+    if (const char *ev = getenv("B200Z_PIPELINE_CHUNK_BYTES")) C = strtoull(ev, nullptr, 10);
+    return std::min<uint64_t>(1ull << 31, std::max<uint64_t>(ENC_BLOCK, C / ENC_BLOCK * ENC_BLOCK));
+}
+
 struct CompressResources {
     DevBuf frames, blocks, csum, results, input, output;
     CompressStaging stage;
@@ -2681,6 +2722,8 @@ struct CompressResources {
     DevBuf rd_stage, rd_pieces;       // b200z_seekable_read_ranges: host output's slots and the scratch, the copy pieces
     PinnedBuf rd_host;                // b200z_seekable_read_ranges: the touched frames of a host archive, host output's slots
     LdmBufs ldm;                      // b200z_compress_frames_batch_long
+    FarBufs far;                      // b200z_compress_frames_batch_long at ULTRA
+    std::deque<Event> far_ev;         // profiled ULTRA submissions: around each group's k_copt
     Event ev[kCompressStages + 1];
     float stage_ms[kCompressStages] = {};
     bool profiled = false;
@@ -2751,7 +2794,8 @@ static int compress_check(b200z_ctx *c, int level, int window_log, const b200z_d
         if (c) c->err = "compression levels Default, Better and Best are unimplemented!() in the reference";
         return B200Z_ERR_REFERENCE_WOULD_PANIC;
     }
-    if (!c || (level != B200Z_LEVEL_UNCOMPRESSED && level != B200Z_LEVEL_FASTEST && level != B200Z_LEVEL_LAZY && level != B200Z_LEVEL_OPT))
+    if (!c || (level != B200Z_LEVEL_UNCOMPRESSED && level != B200Z_LEVEL_FASTEST && level != B200Z_LEVEL_LAZY && level != B200Z_LEVEL_OPT &&
+               level != B200Z_LEVEL_ULTRA))
         return B200Z_ERR_INVALID_ARGUMENT;
     if (window_log < B200Z_WINDOW_LOG_MIN || window_log > B200Z_WINDOW_LOG_MAX || (level == B200Z_LEVEL_UNCOMPRESSED && window_log != B200Z_WINDOW_LOG_MIN)) {
         c->err = "window_log outside [17, 27], or above 17 at level Uncompressed";
@@ -2814,6 +2858,39 @@ static int compress_ldm(b200z_ctx *c, LdmBufs &r, CompressArgs &a, const LSpan *
     if (int le = launch_ldm_match(l, s, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_lblock");
     a.lforced = l.forced; a.lf_off = l.lf_off; a.lf_cnt = l.lf_cnt;
     return 0;
+}
+
+// ULTRA's groups over a submission's blocks hb[nblocks] (frames hf): consecutive blocks of at most C bytes in all.  A group's
+// pieces are, for each frame of it whose window Wf is beyond 131072, the frame's blocks in the Wf bytes before its first block in the
+// group, then its blocks in the group, numbered on in one virtual space; fb[b] is block b's FBlock.  Returns whether any block has
+// a far walk (else ULTRA is OPT and no far stage runs).
+struct FarGroup { uint32_t b0, b1, p0, p1; uint64_t npairs, nvirt; };
+static bool far_plan(const CFrame *hf, const CBlock *hb, uint32_t nblocks, uint32_t window_log, uint64_t C, std::vector<FarGroup> &groups,
+                     std::vector<FPiece> &pieces, std::vector<FBlock> &fb) {
+    bool any = false;
+    fb.resize(nblocks);
+    for (uint32_t b = 0; b < nblocks;) {
+        FarGroup g{b, b, (uint32_t)pieces.size(), 0, 0, 0};
+        uint64_t bytes = 0, vbase = 0, pbase = 0;
+        while (b < nblocks && (b == g.b0 || bytes + hb[b].size <= C)) {
+            const CFrame &f = hf[hb[b].frame];
+            const uint64_t wf = 1ull << frame_window_log(f.src_size, window_log), pos = hb[b].src_off - f.src_off;
+            if (wf > ENC_WINDOW) {
+                if (b == g.b0 || hb[b - 1].frame != hb[b].frame)   // the frame's first block in the group: its history first
+                    for (uint32_t j = b - (uint32_t)(std::min(pos, wf) / ENC_BLOCK); j < b; j++) far_piece(pieces, hb[j].src_off, hb[j].size, vbase, pbase);
+                fb[b] = FBlock{(uint32_t)vbase, (uint32_t)std::min(pos, wf), (uint32_t)wf, 0};
+                far_piece(pieces, hb[b].src_off, hb[b].size, vbase, pbase);
+                any = true;
+            } else {
+                fb[b] = FBlock{FAR_NONE, hb[b].back, ENC_WINDOW, 0};
+            }
+            bytes += hb[b].size;
+            b++;
+        }
+        g.b1 = b; g.p1 = (uint32_t)pieces.size(); g.npairs = pbase; g.nvirt = vbase;
+        groups.push_back(g);
+    }
+    return any;
 }
 
 extern "C" int b200z_compress_frames_batch_long(b200z_ctx *c, const uint8_t *input, size_t input_len, int input_mem, const b200z_compress_io *frames,
@@ -2888,10 +2965,50 @@ extern "C" int b200z_compress_frames_batch_long(b200z_ctx *c, const uint8_t *inp
             if ((e = compress_ldm(c, r.ldm, a, r.ldm.spans.as<LSpan>(), (uint32_t)sp.size(), (uint32_t)nblocks, (uint32_t)window_log, 0, s))) return e;
         }
     }
+    // ULTRA: the groups of whole blocks, each with the pieces of its far frames (their history, then their blocks in the group)
+    std::vector<FarGroup> groups;
+    std::vector<FPiece> pieces;
+    std::vector<FBlock> fb;
+    if (level == B200Z_LEVEL_ULTRA && window_log > B200Z_WINDOW_LOG_MIN &&
+        far_plan(hf.data(), hb.data(), (uint32_t)nblocks, (uint32_t)window_log, far_group_bytes(), groups, pieces, fb)) {
+        uint64_t mp = 0, mv = 0;
+        for (const FarGroup &g : groups) { mp = std::max(mp, g.npairs); mv = std::max(mv, g.nvirt); }
+        if ((e = r.far.ensure(mp, mv, pieces.size(), nblocks))) return e;
+        CU(c, cudaMemcpyAsync(r.far.pieces.p, pieces.data(), pieces.size() * sizeof(FPiece), cudaMemcpyHostToDevice, s));
+        CU(c, cudaMemcpyAsync(r.far.fblk.p, fb.data(), fb.size() * sizeof(FBlock), cudaMemcpyHostToDevice, s));
+    } else {
+        groups.clear();
+    }
     const bool prof = (c->flags & B200Z_FLAG_PROFILE) != 0;
-    if (prof) CU(c, cudaEventRecord(r.ev[0], s));
+    if (prof) {
+        CU(c, cudaEventRecord(r.ev[0], s));
+        while (r.far_ev.size() < 2 * groups.size()) {
+            r.far_ev.emplace_back();
+            if (r.far_ev.back().create(c, cudaEventDefault)) { r.far_ev.pop_back(); return B200Z_ERR_CUDA; }
+        }
+    }
     for (int st = 0; st < kCompressStages; st++) {
-        if (int le = launch_compress_stage(a, st, s, &c->launches)) return c->set_cuda_err((cudaError_t)le, kCompressStageNames[st]);
+        if (st == 0 && !groups.empty()) {   // per group: its far stage, then k_copt over its blocks
+            for (size_t g = 0; g < groups.size(); g++) {
+                const FarGroup &G = groups[g];
+                if (G.p1 > G.p0) {
+                    const FarArgs fa = r.far.args(d_in, r.far.pieces.as<FPiece>() + G.p0, G.p1 - G.p0, (uint32_t)G.npairs);
+                    if (int le = launch_far_stage(fa, s, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_fkey / k_fstart");
+                }
+                CompressArgs ga = a;
+                const size_t b0 = G.b0;
+                ga.blocks = a.blocks + b0; ga.nblocks = G.b1 - G.b0;
+                ga.lit_stage = a.lit_stage + b0 * ENC_BLOCK; ga.seq_stage = a.seq_stage + b0 * CBLOCK_SEQS;
+                ga.lits = a.lits + b0 * ENC_BLOCK; ga.seqs = a.seqs + b0 * CBLOCK_SEQS; ga.info = a.info + b0;
+                ga.lf_off = a.lf_off + b0; ga.lf_cnt = a.lf_cnt + b0;
+                r.far.bind(ga, r.far.fblk.as<FBlock>() + b0);
+                if (prof) CU(c, cudaEventRecord(r.far_ev[2 * g], s));
+                if (int le = launch_compress_stage(ga, 0, s, &c->launches)) return c->set_cuda_err((cudaError_t)le, kCompressStageNames[0]);
+                if (prof) CU(c, cudaEventRecord(r.far_ev[2 * g + 1], s));
+            }
+        } else if (int le = launch_compress_stage(a, st, s, &c->launches)) {
+            return c->set_cuda_err((cudaError_t)le, kCompressStageNames[st]);
+        }
         if (prof) CU(c, cudaEventRecord(r.ev[st + 1], s));
     }
     CU(c, cudaMemcpyAsync(results, r.results.p, nframes * sizeof(b200z_compress_result), cudaMemcpyDeviceToHost, s));
@@ -2900,8 +3017,17 @@ extern "C" int b200z_compress_frames_batch_long(b200z_ctx *c, const uint8_t *inp
         for (size_t i = 0; i < nframes; i++)
             CU(c, cudaMemcpy(output + frames[i].dst_off, d_out + frames[i].dst_off, results[i].dst_size, cudaMemcpyDeviceToHost));
     r.profiled = prof;
-    if (prof)
+    if (prof) {
         for (int st = 0; st < kCompressStages; st++) CU(c, cudaEventElapsedTime(&r.stage_ms[st], r.ev[st], r.ev[st + 1]));
+        if (!groups.empty()) {   // stage 0 is the groups' k_copt, not their far stages
+            r.stage_ms[0] = 0;
+            for (size_t g = 0; g < groups.size(); g++) {
+                float ms = 0;
+                CU(c, cudaEventElapsedTime(&ms, r.far_ev[2 * g], r.far_ev[2 * g + 1]));
+                r.stage_ms[0] += ms;
+            }
+        }
+    }
     return 0;
 }
 
@@ -3514,6 +3640,9 @@ struct b200z_frame_compressor {
     PipeSlots p;
     CompressStaging stage;                    // shared: the kernels run in order on one stream
     LdmBufs ldm;                              // shared, sized for the density bound of the spans
+    FarBufs far;                              // ULTRA, shared: sized for a chunk and the 2^window_log bytes before it
+    std::vector<FPiece> far_pieces;           // ULTRA: the chunk's pieces and blocks, uploaded on the kernel stream
+    std::vector<FBlock> far_blocks;
     uint64_t hist = 0;                        // what the buffers were prepared for (0: not yet)
     uint32_t chunk_blocks() const { return (uint32_t)(chunk / ENC_BLOCK); }
     uint64_t hist_for(uint32_t wl) const { return wl > B200Z_WINDOW_LOG_MIN ? (1ull << wl) + LDM_MARGIN : ENC_WINDOW; }
@@ -3524,7 +3653,9 @@ struct b200z_frame_compressor {
     size_t desc_bytes() const { return res_off() + sizeof(b200z_compress_result); }
 };
 
-static int fc_valid_level(int level) { return (level >= 0 && level <= 4) || level == B200Z_LEVEL_LAZY || level == B200Z_LEVEL_OPT; }   // Uncompressed .. Best, LAZY, OPT
+static int fc_valid_level(int level) {   // Uncompressed .. Best, LAZY, OPT, ULTRA
+    return (level >= 0 && level <= 4) || level == B200Z_LEVEL_LAZY || level == B200Z_LEVEL_OPT || level == B200Z_LEVEL_ULTRA;
+}
 static int fc_panic(b200z_ctx *c, const char *what) { c->err = what; return B200Z_ERR_REFERENCE_WOULD_PANIC; }
 
 extern "C" int b200z_frame_compressor_new(b200z_ctx *c, int level, int checksum, b200z_frame_compressor **out) {
@@ -3643,7 +3774,15 @@ static int fc_compress_fast(b200z_frame_compressor *fc, b200z_read_fn rd, void *
     b200z_ctx *c = fc->ctx;
     if (int e = fc_prepare(fc)) return e;
     if (int e = fc->stage.ensure(fc->chunk_blocks(), false, fc->level)) return e;   // OPT's chain slots, whenever the level became OPT
-    const uint64_t C = fc->chunk, H = fc->hist_for(fc->window_log);
+    const uint64_t C = fc->chunk, H = fc->hist_for(fc->window_log), Wf = 1ull << fc->window_log;
+    const bool ultra = fc->level == B200Z_LEVEL_ULTRA && fc->window_log > B200Z_WINDOW_LOG_MIN;
+    if (ultra) {   // a chunk and the Wf bytes before it, whenever the level became ULTRA
+        const uint64_t v = Wf + C;
+        if (int e = fc->far.ensure(v, v, Wf / ENC_BLOCK + fc->chunk_blocks(), fc->chunk_blocks(), false)) {
+            c->err = "FrameCompressor: out of memory for ULTRA's far stage";
+            return e;
+        }
+    }
     cudaStream_t ks = c->stream;
     auto enqueue = [&](uint64_t k, int s, size_t n) -> int {
         CFrame *hf = fc->p.h_desc[s].as<CFrame>();
@@ -3678,6 +3817,23 @@ static int fc_compress_fast(b200z_frame_compressor *fc, b200z_read_fn rd, void *
             if (int le = compress_ldm(c, fc->ldm, a, reinterpret_cast<const LSpan *>(fc->p.d_desc[s].as<uint8_t>() + fc->span_off()), ns, m,
                                       fc->window_log, ns * LDM_SPAN_CAP, ks))
                 return le;
+        if (ultra && ns) {   // ULTRA's far stage over the last min(k * C, Wf) bytes of the frame and the chunk: one group
+            std::vector<FPiece> &pc = fc->far_pieces;
+            std::vector<FBlock> &fb = fc->far_blocks;
+            pc.clear(); fb.clear();
+            const uint64_t hl = std::min(k * C, Wf);
+            uint64_t vbase = 0, pbase = 0;
+            for (uint64_t o = H - hl; o < H; o += ENC_BLOCK) far_piece(pc, o, ENC_BLOCK, vbase, pbase);
+            for (uint32_t i = 0; i < m; i++) {
+                fb.push_back(FBlock{(uint32_t)vbase, (uint32_t)std::min(k * C + (uint64_t)i * ENC_BLOCK, Wf), (uint32_t)Wf, 0});
+                far_piece(pc, hb[i].src_off, hb[i].size, vbase, pbase);
+            }
+            CU(c, cudaMemcpyAsync(fc->far.pieces.p, pc.data(), pc.size() * sizeof(FPiece), cudaMemcpyHostToDevice, ks));
+            CU(c, cudaMemcpyAsync(fc->far.fblk.p, fb.data(), fb.size() * sizeof(FBlock), cudaMemcpyHostToDevice, ks));
+            if (int le = launch_far_stage(fc->far.args(din, fc->far.pieces.as<FPiece>(), (uint32_t)pc.size(), (uint32_t)pbase), ks, &c->launches))
+                return c->set_cuda_err((cudaError_t)le, "k_fkey / k_fstart");
+            fc->far.bind(a, fc->far.fblk.as<FBlock>());
+        }
         if (int le = launch_compress_chunk(a, ks, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_cmatch / k_cenc / k_cassemble<true>");
         CU(c, cudaEventRecord(fc->p.ev_k[s], ks));
         CU(c, cudaStreamWaitEvent(fc->p.s_d2h, fc->p.ev_k[s], 0));

@@ -5,7 +5,7 @@
 //                  <DICT, LAZY, true>: with the long-distance matches of ldm.cu forced into the parse, window_log > 17)
 //   k_copt      : OPT (an extension): in k_cmatch's place, a grid of the resident CTAs striding over the blocks: per block a hash chain
 //                 over the block and the 128 KiB before it, then one warp per segment parses it by a price-based forward DP
-//                 (<DICT, LONG>: as k_cmatch's)
+//                 (<DICT, LONG>: as k_cmatch's; <DICT, true, true>: ULTRA, with the far walk over ldm.cu's far stage)
 //   k_cenc      : one warp per block: Huffman literals, FSE sequences, the Raw / RLE / Compressed decision (encode.cuh)
 //                 (<TABLES, true>: LAZY and OPT, repeat-offset codes within each block first)
 //   k_cxxh64    : content checksum of every frame's input (xxh64.cuh; four serial chains per frame)
@@ -64,7 +64,7 @@ constexpr int32_t OPT_NONE = INT_MIN, OPT_FIX = INT_MIN + 1;   // prev: no earli
 constexpr uint32_t OPT_SMEM = CM_WARPS * (2u << OPT_HASH_LOG);  // the stripes' u16 heads (128 KiB), then the warps' DP state
 struct OptWarp {       // one warp's DP state (k_copt's second phase)
     uint32_t cost[OPT_NODES], link[OPT_NODES], off[OPT_NODES], rep[3][OPT_NODES];   // link: from | length << 16 (0: a literal)
-    uint32_t cand[32 * OPT_CANDS];                                                  // the chunk's lists: length << 18 | offset
+    uint32_t cand[32 * OPT_CANDS];                                                  // the chunk's lists (cand_pack)
     uint32_t path_pos[OPT_PATH], path_ml[OPT_PATH], path_off[OPT_PATH];
 };
 static_assert(CM_WARPS * sizeof(OptWarp) <= OPT_SMEM, "the DP state reuses the heads' shared memory");
@@ -418,10 +418,23 @@ __device__ __forceinline__ uint32_t opt_log2(uint32_t x) {   // 256 floor(log2 x
     return 256 * k + ((k <= 8 ? x << (8 - k) : x >> (k - 8)) & 255u);
 }
 
+// a finder candidate in one word (0: none): length << 18 | offset at OPT (offsets <= 131072); at ULTRA (FAR) (length - 1) << 27 |
+// (offset - 1), which holds offsets up to 2^27 and lengths 5..32
+template <bool FAR> __device__ __forceinline__ uint32_t cand_pack(uint32_t ln, uint32_t o) { return FAR ? (ln - 1) << 27 | (o - 1) : ln << 18 | o; }
+template <bool FAR> __device__ __forceinline__ uint32_t cand_len(uint32_t c) { return FAR ? (c >> 27) + 1 : c >> 18; }   // FAR: 1 for none
+template <bool FAR> __device__ __forceinline__ uint32_t cand_off(uint32_t c) { return FAR ? (c & 0x7ffffffu) + 1 : c & 0x3ffffu; }
+
+// ULTRA's far walk: the group's sorted (key8, virtual position) pairs and, per virtual position, where its walk starts (ldm.cu)
+struct FarView {
+    FBlock fb;
+    const uint32_t *keys, *vals, *start;
+};
+
 // the finder's list of each position cb + lane (q + 5 <= stop), lengths increasing, into wk.cand
-template <bool DICT>
+template <bool DICT, bool FAR>
 __device__ __forceinline__ void opt_chunk(OptWarp &wk, const int32_t *prev, int32_t lo, const CBlock &blk, const uint8_t *src, uint32_t cb,
-                                          uint32_t stop, const uint8_t *dict, const uint32_t *dtab, uint32_t dict_len, uint32_t lane) {
+                                          uint32_t stop, const uint8_t *dict, const uint32_t *dtab, uint32_t dict_len, const FarView &fv,
+                                          uint32_t lane) {
     const uint32_t q = cb + lane;
     uint32_t k0 = 0, k1 = 0, k2 = 0, k3 = 0, cnt = 0;
     auto push = [&](uint32_t v) {
@@ -432,15 +445,35 @@ __device__ __forceinline__ void opt_chunk(OptWarp &wk, const int32_t *prev, int3
     if (q + ENC_MIN_MATCH <= stop) {
         const uint32_t lim = min(OPT_SUFF, stop - q);
         uint32_t best = ENC_MIN_MATCH - 1;
+        bool full = false;   // a verification reached its limit
         int32_t c = prev[(int32_t)q - lo];
         for (uint32_t seen = 0; c >= lo && (int32_t)q - c <= (int32_t)ENC_WINDOW && seen < OPT_DEPTH; seen++) {
             const uint32_t ln = match_len(src + q, src + c, lim);
             if (ln > best) {
-                push(ln << 18 | (uint32_t)((int32_t)q - c));
+                push(cand_pack<FAR>(ln, (uint32_t)((int32_t)q - c)));
                 best = ln;
-                if (ln == lim) break;
+                if (ln == lim) { full = true; break; }
             }
             c = prev[c - lo];
+        }
+        // ULTRA: the same key8's earlier positions beyond 131072, nearest first, consecutive sorted pairs read backwards
+        if (FAR && !full && fv.fb.vbase != FAR_NONE) {
+            const uint32_t vq = fv.fb.vbase + q;
+            uint32_t k = fv.start[vq];
+            if (k != FAR_NONE) {
+                const uint32_t key = fv.keys[k], reach = min(fv.fb.wf, fv.fb.back + q);
+                for (uint32_t seen = 0; seen < FAR_DEPTH; seen++) {
+                    const uint32_t d = vq - fv.vals[k];
+                    if (d > reach) break;
+                    const uint32_t ln = match_len(src + q, src + q - d, lim);
+                    if (ln > best) {
+                        push(cand_pack<FAR>(ln, d));
+                        best = ln;
+                        if (ln == lim) break;
+                    }
+                    if (k == 0 || fv.keys[--k] != key) break;
+                }
+            }
         }
         const uint32_t fpos = blk.back + q;
         if (DICT && fpos < ENC_WINDOW) {
@@ -448,7 +481,7 @@ __device__ __forceinline__ void opt_chunk(OptWarp &wk, const int32_t *prev, int3
             const uint32_t off3 = fpos + dict_len - (c3 - 1);
             if (c3 && off3 <= ENC_WINDOW) {
                 const uint32_t ln = match_len(src + q, dict + (c3 - 1), min(lim, dict_len - (c3 - 1)));
-                if (ln > best) push(ln << 18 | off3);
+                if (ln > best) push(cand_pack<FAR>(ln, off3));
             }
         }
     }
@@ -457,9 +490,10 @@ __device__ __forceinline__ void opt_chunk(OptWarp &wk, const int32_t *prev, int3
     __syncwarp();
 }
 
-// the length of repeat o at i (>= 5, else 0), verified for min(OPT_SUFF, stop - i) bytes; the source must lie in the frame
-__device__ __forceinline__ uint32_t opt_rep(const uint8_t *src, uint32_t i, uint32_t o, uint32_t lim, uint32_t back, uint32_t lane) {
-    const bool ok = o && o <= back + i && o <= ENC_WINDOW;
+// the length of repeat o at i (>= 5, else 0), verified for min(OPT_SUFF, stop - i) bytes; the source must lie in the frame and in
+// the window wf (131072 at OPT, the frame's at ULTRA)
+__device__ __forceinline__ uint32_t opt_rep(const uint8_t *src, uint32_t i, uint32_t o, uint32_t lim, uint32_t back, uint32_t wf, uint32_t lane) {
+    const bool ok = o && o <= back + i && o <= wf;
     const bool stop = !ok || lane >= lim || __ldg(src + i + lane) != __ldg(src + i + lane - o);
     const uint32_t m = __ballot_sync(0xffffffffu, stop);
     const uint32_t ln = m ? __ffs(m) - 1 : 32u;
@@ -467,10 +501,13 @@ __device__ __forceinline__ uint32_t opt_rep(const uint8_t *src, uint32_t i, uint
 }
 
 // one warp's parse of segment [s, e) (see k_copt): the DPs of each part, forced pieces between them; staging as cmatch_lazy's
-template <bool DICT, bool LONG>
+template <bool DICT, bool LONG, bool FAR>
 __device__ __forceinline__ void opt_segment(OptWarp &wk, const int32_t *prev, int32_t lo, const uint32_t *lit, const CBlock &blk, const uint8_t *src,
                                             uint32_t s, uint32_t e, const uint8_t *dict, const uint32_t *dtab, uint32_t dict_len, SeqRec *stage,
-                                            uint8_t *lstage, uint32_t *nseq_out, uint32_t *nlit_out, uint32_t *trail_out, LCursor &lc, uint32_t lane) {
+                                            uint8_t *lstage, uint32_t *nseq_out, uint32_t *nlit_out, uint32_t *trail_out, LCursor &lc,
+                                            const FarView &fv, uint32_t lane) {
+    // the frame before the block that repeats may reach, and their window: at ULTRA the far stage's (up to Wf), else 131072
+    const uint32_t rback = FAR ? fv.fb.back : blk.back, rwf = FAR ? fv.fb.wf : ENC_WINDOW;
     uint32_t p = s, anchor = s, nseq = 0, nlit = 0;
     uint32_t r0 = 0, r1 = 0, r2 = 0;   // the reps at p (0: none yet)
     auto push_rep = [&](uint32_t o) {
@@ -494,26 +531,26 @@ __device__ __forceinline__ void opt_segment(OptWarp &wk, const int32_t *prev, in
             __syncwarp();
             if (lane == 0) { wk.cost[0] = 0; wk.rep[0][0] = r0; wk.rep[1][0] = r1; wk.rep[2][0] = r2; }
             uint32_t cb = a;
-            opt_chunk<DICT>(wk, prev, lo, blk, src, cb, stop, dict, dtab, dict_len, lane);
+            opt_chunk<DICT, FAR>(wk, prev, lo, blk, src, cb, stop, dict, dtab, dict_len, fv, lane);
             uint32_t tml = 0, toff = 0;   // a match taken at once at `end`
             for (uint32_t i = a; i < end; i++) {
-                if (i >= cb + 32) { cb = i; opt_chunk<DICT>(wk, prev, lo, blk, src, cb, stop, dict, dtab, dict_len, lane); }
+                if (i >= cb + 32) { cb = i; opt_chunk<DICT, FAR>(wk, prev, lo, blk, src, cb, stop, dict, dtab, dict_len, fv, lane); }
                 const uint32_t k = i - a, ci = wk.cost[k], x0 = wk.rep[0][k], x1 = wk.rep[1][k], x2 = wk.rep[2][k];
                 const uint32_t *cl = wk.cand + (i - cb) * OPT_CANDS;
                 const uint32_t c0 = cl[0], c1 = cl[1], c2 = cl[2], c3 = cl[3];
                 uint32_t l0 = 0, l1 = 0, l2 = 0;
                 if (i + ENC_MIN_MATCH <= stop) {
                     const uint32_t lim = min(OPT_SUFF, stop - i);
-                    l0 = opt_rep(src, i, x0, lim, blk.back, lane);
-                    l1 = opt_rep(src, i, x1, lim, blk.back, lane);
-                    l2 = opt_rep(src, i, x2, lim, blk.back, lane);
+                    l0 = opt_rep(src, i, x0, lim, rback, rwf, lane);
+                    l1 = opt_rep(src, i, x1, lim, rback, rwf, lane);
+                    l2 = opt_rep(src, i, x2, lim, rback, rwf, lane);
                 }
                 // a candidate of OPT_SUFF bytes closes the DP: the longest, the first of rep0, rep1, rep2, the finder's on a tie
                 const uint32_t ctop = c3 ? c3 : c2 ? c2 : c1 ? c1 : c0;
                 if (l0 >= OPT_SUFF && l0 > tml) { tml = l0; toff = x0; }
                 if (l1 >= OPT_SUFF && l1 > tml) { tml = l1; toff = x1; }
                 if (l2 >= OPT_SUFF && l2 > tml) { tml = l2; toff = x2; }
-                if ((ctop >> 18) >= OPT_SUFF && (ctop >> 18) > tml) { tml = ctop >> 18; toff = ctop & 0x3ffffu; }
+                if (cand_len<FAR>(ctop) >= OPT_SUFF && cand_len<FAR>(ctop) > tml) { tml = cand_len<FAR>(ctop); toff = cand_off<FAR>(ctop); }
                 if (tml) { end = i; break; }
                 // lane l relaxes node i + l: the literal (l = 1), a match of l bytes (l >= 5)
                 uint32_t c = OPT_INF, off = 0;
@@ -523,9 +560,11 @@ __device__ __forceinline__ void opt_segment(OptWarp &wk, const int32_t *prev, in
                     if (l0 >= lane) { best = OPT_REP_W0; off = x0; }
                     if (l1 >= lane && OPT_REP_W1 < best) { best = OPT_REP_W1; off = x1; }
                     if (l2 >= lane && OPT_REP_W2 < best) { best = OPT_REP_W2; off = x2; }
-                    const uint32_t f = (c0 >> 18) >= lane ? c0 : (c1 >> 18) >= lane ? c1 : (c2 >> 18) >= lane ? c2 : (c3 >> 18) >= lane ? c3 : 0u;
+                    uint32_t f;   // the first finder candidate of >= lane bytes (OPT's expression kept as it was: the same SASS)
+                    if constexpr (FAR) f = cand_len<FAR>(c0) >= lane ? c0 : cand_len<FAR>(c1) >= lane ? c1 : cand_len<FAR>(c2) >= lane ? c2 : cand_len<FAR>(c3) >= lane ? c3 : 0u;
+                    else f = (c0 >> 18) >= lane ? c0 : (c1 >> 18) >= lane ? c1 : (c2 >> 18) >= lane ? c2 : (c3 >> 18) >= lane ? c3 : 0u;
                     if (f) {
-                        const uint32_t o = f & 0x3ffffu, pr = 256 * (31 - __clz(o + 3)) + OPT_OF_W;
+                        const uint32_t o = cand_off<FAR>(f), pr = 256 * (31 - __clz(o + 3)) + OPT_OF_W;
                         if (pr < best) { best = pr; off = o; }
                     }
                     if (best != OPT_INF) c = ci + OPT_MATCH_W + best;
@@ -556,9 +595,9 @@ __device__ __forceinline__ void opt_segment(OptWarp &wk, const int32_t *prev, in
             r0 = wk.rep[0][end - a]; r1 = wk.rep[1][end - a]; r2 = wk.rep[2][end - a];
             p = end;
             if (tml) {
-                const uint32_t fpos = blk.back + end;
+                const uint32_t fpos = rback + end;
                 const uint32_t xlim = DICT && toff > fpos ? min(stop - end, toff - fpos) : stop - end;   // a dictionary source: to its end
-                const uint32_t ml = extend_match<DICT>(src, end, toff, tml, xlim, blk.back, dict, dict_len, lane);
+                const uint32_t ml = extend_match<DICT>(src, end, toff, tml, xlim, rback, dict, dict_len, lane);
                 emit(end, ml, toff);
                 push_rep(toff);
                 p = end + ml;
@@ -580,12 +619,14 @@ __device__ __forceinline__ void opt_segment(OptWarp &wk, const int32_t *prev, in
     if (lane == 0) { *nseq_out = nseq; *nlit_out = nlit + (e - anchor); *trail_out = e - anchor; }
 }
 
-template <bool DICT, bool LONG>
+template <bool DICT, bool LONG, bool FAR = false>
 __global__ void __launch_bounds__(CM_THREADS, 1)
 k_copt(const CBlock *__restrict__ blocks, uint32_t nblocks, const uint8_t *__restrict__ input, uint8_t *__restrict__ lit_stage,
        SeqRec *__restrict__ seq_stage, uint8_t *__restrict__ lits, SeqRec *__restrict__ seqs, CBlockInfo *__restrict__ info,
        const uint8_t *__restrict__ dict, const uint32_t *__restrict__ dtab, uint32_t dict_len, int32_t *opt_prev,
-       const LForced *__restrict__ lforced, const uint32_t *__restrict__ lf_off, const uint32_t *__restrict__ lf_cnt) {
+       const LForced *__restrict__ lforced, const uint32_t *__restrict__ lf_off, const uint32_t *__restrict__ lf_cnt,
+       const FBlock *__restrict__ fblk, const uint32_t *__restrict__ fkeys, const uint32_t *__restrict__ fvals,
+       const uint32_t *__restrict__ fstart) {
     extern __shared__ __align__(16) uint8_t smem_co[];
     __shared__ uint32_t s_nseq[CM_WARPS], s_nlit[CM_WARPS], s_trail[CM_WARPS], s_add[CM_WARPS], s_soff[CM_WARPS], s_loff[CM_WARPS];
     __shared__ uint32_t s_lit[256];
@@ -644,10 +685,13 @@ k_copt(const CBlock *__restrict__ blocks, uint32_t nblocks, const uint8_t *__res
         const uint32_t s = min(n, w * seglen), e = min(n, s + seglen);
         LCursor lc{};
         if constexpr (LONG) lc = LCursor{lforced + lf_off[b], 0, lf_cnt[b], s, e, 0, 0, 0, false};
+        FarView fv{};
+        if constexpr (FAR) fv = FarView{fblk[b], fkeys, fvals, fstart};
         {
             SeqRec *stage = seq_stage + ((size_t)b * CM_WARPS + w) * CSEG_SEQS;
             uint8_t *lstage = lit_stage + (size_t)b * ENC_BLOCK + s;
-            opt_segment<DICT, LONG>(wk, prev, lo, s_lit, blk, src, s, e, dict, dtab, dict_len, stage, lstage, s_nseq + w, s_nlit + w, s_trail + w, lc, lane);
+            opt_segment<DICT, LONG, FAR>(wk, prev, lo, s_lit, blk, src, s, e, dict, dtab, dict_len, stage, lstage, s_nseq + w, s_nlit + w, s_trail + w, lc,
+                                         fv, lane);
         }
         __syncthreads();
         if (tid == 0) {   // k_cmatch's packing
@@ -866,6 +910,8 @@ int init_compress_kernels() {
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_copt<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OPT_SMEM);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_copt<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OPT_SMEM);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_copt<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OPT_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_copt<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OPT_SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_copt<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OPT_SMEM);
     int dev = 0, sms = 0, per = 0;
     if (e == cudaSuccess) e = cudaGetDevice(&dev);
     if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -889,14 +935,21 @@ int launch_dict_table(const uint8_t *dict, uint32_t len, uint32_t *dtab, cudaStr
 const char *const kCompressStageNames[kCompressStages] = {"k_cmatch", "k_cenc", "k_cxxh64", "k_cassemble"};
 
 int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s, uint64_t *launched) {
-    const bool lazy = a.level == B200Z_LEVEL_LAZY, opt = a.level == B200Z_LEVEL_OPT;
+    const bool lazy = a.level == B200Z_LEVEL_LAZY, opt = a.level == B200Z_LEVEL_OPT || a.level == B200Z_LEVEL_ULTRA;
     switch (stage) {
     case 0:
         if (!a.level || !a.nblocks) return 0;
-        if (opt) {
+        if (opt && a.fblk) {   // ULTRA with a far stage (always with the long-distance matches: both need window_log > 17)
+            if (!a.lf_cnt) return (int)cudaErrorInvalidValue;
+            auto k = a.dtab ? k_copt<true, true, true> : k_copt<false, true, true>;
+            k<<<std::min(a.nblocks, g_opt_ctas), CM_THREADS, OPT_SMEM, s>>>(a.blocks, a.nblocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info,
+                                                                         a.dict, a.dtab, a.dict_len, a.opt_prev, a.lforced, a.lf_off, a.lf_cnt,
+                                                                         a.fblk, a.fkeys, a.fvals, a.fstart);
+        } else if (opt) {
             auto k = a.lf_cnt ? (a.dtab ? k_copt<true, true> : k_copt<false, true>) : (a.dtab ? k_copt<true, false> : k_copt<false, false>);
             k<<<std::min(a.nblocks, g_opt_ctas), CM_THREADS, OPT_SMEM, s>>>(a.blocks, a.nblocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info,
-                                                                         a.dict, a.dtab, a.dict_len, a.opt_prev, a.lforced, a.lf_off, a.lf_cnt);
+                                                                         a.dict, a.dtab, a.dict_len, a.opt_prev, a.lforced, a.lf_off, a.lf_cnt,
+                                                                         nullptr, nullptr, nullptr, nullptr);
         } else if (a.lf_cnt) {
             const uint32_t smem = lazy ? LZ_SMEM : CM_SMEM;
             auto k = lazy ? (a.dtab ? k_cmatch<true, true, true> : k_cmatch<false, true, true>) : (a.dtab ? k_cmatch<true, false, true> : k_cmatch<false, false, true>);
@@ -908,7 +961,7 @@ int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s, uint
         } else if (a.dtab) k_cmatch<true, false><<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, a.dict, a.dtab, a.dict_len);
         else k_cmatch<false, false><<<a.nblocks, CM_THREADS, CM_SMEM, s>>>(a.blocks, a.input, a.lit_stage, a.seq_stage, a.lits, a.seqs, a.info, nullptr, nullptr, 0);
         break;
-    case 1:   // LAZY's and OPT's repeat-offset records go to seq_stage, free once k_cmatch / k_copt is done
+    case 1:   // LAZY's, OPT's and ULTRA's repeat-offset records go to seq_stage, free once k_cmatch / k_copt is done
         if (!a.level || !a.nblocks) return 0;
         if (lazy || opt) {
             if (a.etab) k_cenc<true, true><<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res, a.etab, a.seq_stage);

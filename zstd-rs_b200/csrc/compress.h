@@ -31,6 +31,13 @@ struct LForced {       // a forced match of a block: [start, start + len) at off
     uint32_t start, len, off;
 };
 
+struct FBlock {        // one block of a k_copt<..., true, true> launch
+    uint32_t vbase;    // its first byte's virtual position; FAR_NONE: no far walk (its frame's window is 131072)
+    uint32_t back;     // the frame's bytes before the block that repeats and far matches may reach: min(its offset in the frame, wf)
+    uint32_t wf;       // its frame's window (131072 when vbase is FAR_NONE)
+    uint32_t pad;
+};
+
 struct CompressArgs {
     const CFrame *frames;
     const CBlock *blocks;
@@ -59,6 +66,10 @@ struct CompressArgs {
     uint32_t window_log;
     // OPT (EXTENSION): k_copt's chain of the block it works on, one OPT_SPAN slot per CTA of its grid (opt_ctas())
     int32_t *opt_prev;
+    // ULTRA (EXTENSION): a group's far stage (ldm.cu) for k_copt<..., true, true>: fblk[nblocks] per block, the sorted pairs and the
+    // walks' starts; fblk null: k_copt is OPT's kernel (no block of the submission has a window beyond 131072)
+    const FBlock *fblk;
+    const uint32_t *fkeys, *fvals, *fstart;
 };
 
 // ---- OPT (compress.cu): a CTA's chain covers the block and the ENC_WINDOW bytes before it
@@ -99,6 +110,33 @@ struct LdmArgs {
 int launch_ldm_count(const LdmArgs &a, cudaStream_t s, uint64_t *launched);
 // with the buffers sized for a.cap >= the total: k_lanchor<true>, the sort, k_lcand and k_lblock
 int launch_ldm_match(const LdmArgs &a, cudaStream_t s, uint64_t *launched);
+
+// ---- ULTRA's far stage (ldm.cu; DESIGN.md section 4.4, tests/cultra.py): per group of whole blocks (at most
+// B200Z_PIPELINE_CHUNK_BYTES of them, or a stream chunk) and the Wf bytes of its frame before its first block, the keyed positions'
+// (key8, virtual position) pairs sorted by key (the LDM sort), then where each position's far walk starts in the sorted pairs.
+// A group's positions are numbered in a virtual space: each frame's part (its history, then its blocks) is contiguous in it, so a
+// distance in the virtual space is a distance in the frame.
+constexpr uint32_t FAR_DEPTH = 8;          // D_F: far entries a position visits, collisions counted
+constexpr uint32_t FAR_KEY = 8;            // bytes key8 hashes; a position is keyed when they end inside its 128 KiB block
+constexpr uint32_t FAR_NONE = 0xffffffffu;
+constexpr uint32_t FAR_LAUNCHES = 14;      // kernels per group: k_fkey, four sort passes of three, k_fstart
+struct FPiece {        // one 128 KiB (or shorter last) block of a frame in a group, history or the group's own
+    uint64_t off;      // in `input`
+    uint32_t vbase;    // its first byte's virtual position
+    uint32_t pbase;    // its first pair
+    uint32_t size;     // bytes; the first size - 7 (if any) are keyed
+    uint32_t pad;
+};
+struct FarArgs {
+    const uint8_t *input;
+    const FPiece *pieces;
+    uint32_t npieces, npairs;
+    uint32_t *total;                       // [1]: npairs, written by k_fkey for the sort
+    uint32_t *keys[2], *vals[2], *hist;    // the sort's ping-pong pairs [npairs] and its digit counts [256 * ceil(npairs / LDM_TILE) + 1]
+    uint32_t *start;                       // [virtual positions]: the sorted index a position's far walk starts at, or FAR_NONE
+};
+// the group's far stage: k_fkey, the sort, k_fstart (FAR_LAUNCHES kernels); adds the kernels it enqueued to *launched
+int launch_far_stage(const FarArgs &f, cudaStream_t s, uint64_t *launched);
 
 // the dictionary match table: 5-byte hash of a position in the dictionary's last ENC_WINDOW bytes -> that position + 1 (0 = none)
 constexpr uint32_t CD_LOG = 17;

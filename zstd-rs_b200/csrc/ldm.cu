@@ -13,8 +13,17 @@
 //   k_lblock   : one warp per span of a block: verify, extend inside the block, trim to the prefix max of earlier ends,
 //                coalesce, and write the block's forced matches for k_cmatch<..., true>
 // The anchors' total stays on the device (scount[nspans]); grids are sized by the capacity and read it.
+//
+// ULTRA's far stage (compress.h, tests/cultra.py), per group:
+//   k_fkey     : one CTA per piece (a 128 KiB block of the group's virtual space): (key8, virtual position) of every keyed position
+//                into the pairs, in position order; the piece's unkeyed tail gets no far walk
+//   the sort   : k_lhist / k_lscan / k_lscatter as above, four passes: equal keys stay in position order
+//   k_fstart   : per sorted pair (position q), the sorted index of the nearest earlier pair with the same key and q - p > ENC_WINDOW,
+//                or FAR_NONE: a backward gallop then a binary search inside the key's run
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <algorithm>
 
 #include "compress.h"
 
@@ -262,6 +271,53 @@ k_lblock(const LSpan *__restrict__ spans, const uint8_t *__restrict__ input, con
     }
 }
 
+__global__ void __launch_bounds__(256)
+k_fkey(const FPiece *__restrict__ pieces, const uint8_t *__restrict__ input, uint32_t npairs, uint32_t *__restrict__ total,
+       uint32_t *__restrict__ keys, uint32_t *__restrict__ vals, uint32_t *__restrict__ start) {
+    const FPiece pc = pieces[blockIdx.x];
+    if (blockIdx.x == 0 && threadIdx.x == 0) *total = npairs;
+    const uint32_t keyed = pc.size >= FAR_KEY ? pc.size - (FAR_KEY - 1) : 0u;
+    const uint8_t *src = input + pc.off;
+    for (uint32_t x = threadIdx.x; x < pc.size; x += 256) {
+        if (x < keyed) {
+            uint64_t v = 0;
+            for (int k = 0; k < 8; k++) v |= (uint64_t)__ldg(src + x + k) << (8 * k);
+            keys[pc.pbase + x] = (uint32_t)((v * LDM_KEY_MUL) >> 32);
+            vals[pc.pbase + x] = pc.vbase + x;
+        } else {
+            start[pc.vbase + x] = FAR_NONE;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(256)
+k_fstart(const uint32_t *__restrict__ keys, const uint32_t *__restrict__ vals, uint32_t npairs, uint32_t *__restrict__ start) {
+    const uint32_t k = blockIdx.x * 256 + threadIdx.x;
+    if (k >= npairs) return;
+    const uint32_t key = keys[k], q = vals[k];
+    // past(t): pair t is before q's walk -- another (smaller) key, or the same key at q - p > ENC_WINDOW.  It holds for every t below
+    // some T and for none in [T, k); the walk starts at T - 1 when that pair has q's key
+    auto past = [&](uint32_t t) { return keys[t] != key || q - vals[t] > ENC_WINDOW; };
+    uint32_t hi = k, lo = 0;
+    uint64_t step = 1;   // [lo, hi): T lies in (lo, hi], past(lo) when lo < hi
+    bool found = false;
+    while (hi >= step) {
+        const uint32_t t = hi - step;
+        if (past(t)) { lo = t; found = true; break; }
+        hi = t;
+        step <<= 1;
+    }
+    if (!found) {   // every pair from hi on is within the run and near; below hi only pair 0 .. hi - 1 remain
+        if (hi == 0 || !past(0)) { start[q] = FAR_NONE; return; }
+        lo = 0;
+    }
+    while (hi - lo > 1) {   // past(lo), !past(hi) (or hi is where the gallop stopped)
+        const uint32_t m = lo + (hi - lo) / 2;
+        if (past(m)) lo = m; else hi = m;
+    }
+    start[q] = keys[lo] == key ? lo : FAR_NONE;
+}
+
 static uint32_t cdiv_l(uint64_t a, uint32_t b) { return (uint32_t)((a + b - 1) / b); }
 static int counted(uint64_t *launched) {
     const int e = (int)cudaGetLastError();
@@ -295,6 +351,23 @@ int launch_ldm_match(const LdmArgs &a, cudaStream_t s, uint64_t *launched) {
         if (int e = counted(launched)) return e;
     }
     k_lblock<<<a.nspans, 32, 0, s>>>(a.spans, a.input, a.scount, a.apos, a.cand, a.forced, a.lf_off, a.lf_cnt);
+    return counted(launched);
+}
+
+int launch_far_stage(const FarArgs &f, cudaStream_t s, uint64_t *launched) {
+    k_fkey<<<f.npieces, 256, 0, s>>>(f.pieces, f.input, f.npairs, f.total, f.keys[0], f.vals[0], f.start);
+    if (int e = counted(launched)) return e;
+    const uint32_t ntiles = std::max(1u, cdiv_l(f.npairs, LDM_TILE));
+    for (uint32_t pass = 0; pass < 4; pass++) {
+        const uint32_t in = pass & 1;
+        k_lhist<<<ntiles, LS_THREADS, 0, s>>>(f.keys[in], f.total, 8 * pass, f.hist);
+        if (int e = counted(launched)) return e;
+        k_lscan<<<1, LSCAN_THREADS, 0, s>>>(f.hist, ntiles * 256);
+        if (int e = counted(launched)) return e;
+        k_lscatter<<<ntiles, LS_THREADS, 0, s>>>(f.keys[in], f.vals[in], f.total, 8 * pass, f.hist, f.keys[in ^ 1], f.vals[in ^ 1]);
+        if (int e = counted(launched)) return e;
+    }
+    k_fstart<<<std::max(1u, cdiv_l(f.npairs, 256)), 256, 0, s>>>(f.keys[0], f.vals[0], f.npairs, f.start);
     return counted(launched);
 }
 
