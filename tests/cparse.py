@@ -30,20 +30,15 @@ the library.  `parse` gives, for every 128 KiB block of every frame of a submiss
 The block and frame drivers are shared by every level: a `Level` names its hash logs, its segment loop (`_segment` here, LAZY's in
 tests/clazy.py) and the records its blocks are coded from.  A segment loop also takes the segment's forced pieces, the long matches
 of tests/cldm.py clipped to it (none at window_log 17).  `reference_frame` assembles the frame from the parse (header, blocks
-through the host build of encode.cuh, checksum), and `xxh64` is XXH64 with seed 0.  `cases()` builds the crafted inputs the tests run; each case's id names the constant it sits on."""
-import atexit
+through tests/cenc.py's plain statement of the entropy stage, checksum), and `xxh64` is XXH64 with seed 0.  `cases()` builds the crafted inputs the tests run; each case's id names the constant it sits on."""
 import bisect
 import collections
-import os
 import random
-import shutil
 import struct
-import subprocess
-import tempfile
 
 import numpy as np
 
-import seqcraft
+import cenc
 
 BLOCK = 131072          # ENC_BLOCK
 WINDOW = 131072         # ENC_WINDOW
@@ -285,36 +280,15 @@ def xxh64(data):
     return h ^ (h >> 32)
 
 
-_dict_exe = None
-
-
-def dict_encoder():
-    """Path of tests/host/encode_dict_test.cpp compiled for the host, once per process, in a temporary directory."""
-    global _dict_exe
-    if _dict_exe is None:
-        d = tempfile.mkdtemp(prefix="cparse")
-        atexit.register(shutil.rmtree, d, True)
-        exe = os.path.join(d, "encode_dict_test")
-        subprocess.check_call([seqcraft.NVCC, "-x", "cu", "-std=c++17", "-O2", "-w", "-o", exe,
-                               os.path.join(seqcraft.HERE, "host", "encode_dict_test.cpp")])
-        _dict_exe = exe
-    return _dict_exe
+_tables = {}
 
 
 def encode_with_tables(formatted, lits, seqs):
-    """Content of a frame's first Compressed block coded with a formatted dictionary's tables (encode_dict_test)."""
-    exe = dict_encoder()
-    d = os.path.dirname(exe)
-    dpath, src, dst = os.path.join(d, "dict"), os.path.join(d, "in.bin"), os.path.join(d, "out.bin")
-    with open(dpath, "wb") as f:
-        f.write(bytes(formatted))
-    with open(src, "wb") as f:
-        f.write(struct.pack("<I", len(lits)) + bytes(lits) + struct.pack("<I", len(seqs)) +
-                b"".join(struct.pack("<3I", ll, ml, of) for ll, ml, of in seqs))
-    out = subprocess.run([exe, dpath, src, dst], capture_output=True, text=True, timeout=120)
-    assert out.returncode == 0 and out.stdout.startswith("ok"), out.stdout + out.stderr
-    with open(dst, "rb") as fh:
-        return fh.read()
+    """Content of a frame's first Compressed block coded with a formatted dictionary's tables (tests/cenc.py)."""
+    key = bytes(formatted)
+    if key not in _tables:
+        _tables[key] = cenc.Tables(key)
+    return cenc.encode_block(lits, seqs, _tables[key])[0]
 
 
 def dict_id_field(dict_id):
@@ -362,7 +336,7 @@ def reference_frame(data, blocks, checksum=True, dict_id=0, dict_tables=None, le
                 if dict_tables is not None and k == 0:
                     content = encode_with_tables(dict_tables, b[0], recs)
                 else:
-                    content = seqcraft.encode(b[0], recs)[0]
+                    content = cenc.encode_block(b[0], recs)[0]
             if content is not None and len(content) < n:
                 out += struct.pack("<I", last | (2 << 1) | (len(content) << 3))[:3] + content
             else:

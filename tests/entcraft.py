@@ -13,8 +13,11 @@ The reference is written from RFC 8878, independent of the oracle and of tables.
   huf_table(weights)    -- section 4.2.1: max_bits, the implicit last weight, ranges longest code first and then by symbol
 Frames follow seqcraft.frame's conventions (window log, content size, checksum); sequences are (ll, ml, Offset_Value) and the
 content comes from seqcraft.execute.  `cases()` builds the crafted set; each id names the edge it sits on."""
+import bisect
 import random
 import struct
+
+import numpy as np
 
 import seqcraft as S
 
@@ -183,16 +186,39 @@ def read_ncount(data):
     return log, norm, (r.pos + 7) // 8
 
 
-def _pick_state(tab, sym, target):
-    """Encoding through the decoding table: the state of `sym` whose [baseline, baseline + 2^nb) holds `target`."""
+def _encoder(tab):
+    """Encoding through the decoding table: {symbol: [state of the symbol whose [baseline, baseline + 2^nb) holds target, for
+    every target in [0, 2^log)]} -- the ranges of one symbol's states cover the table exactly once."""
+    enc = {}
     for x, (s, nb, base) in enumerate(tab):
-        if s == sym and base <= target < base + (1 << nb):
-            return x
-    raise AssertionError("no state")
+        enc.setdefault(s, [None] * len(tab))[base:base + (1 << nb)] = [x] * (1 << nb)
+    return enc
 
 
 def _first_state(tab, sym, min_nb=0):
     return next(x for x, (s, nb, _) in enumerate(tab) if s == sym and nb >= min_nb)
+
+
+def huf_fse_weights(weights, log, norm, first=_first_state):
+    """The FSE-compressed form of a weight list (the description's body without its size byte): the table description, then
+    two interleaved states, weight i from state i & 1.  first(tab, sym): the state a chain ends in (its symbol is decoded last);
+    the update after weight n-2 reads past the stream's start, so that state needs nb >= 1."""
+    tab, n = fse_table(norm, log), len(weights)
+    assert n >= 2
+    st = [None] * n
+    st[n - 1] = first(tab, weights[n - 1])
+    st[n - 2] = first(tab, weights[n - 2])
+    assert tab[st[n - 2]][1] >= 1
+    enc = _encoder(tab)
+    for i in range(n - 3, -1, -1):
+        st[i] = enc[weights[i]][st[i + 2]]
+    w = BitW()
+    for i in range(n - 3, -1, -1):
+        _, nb, base = tab[st[i]]
+        w.add(st[i + 2] - base, nb)
+    w.add(st[1], log)
+    w.add(st[0], log)
+    return write_ncount(norm, log) + w.backward()
 
 
 def write_huf_desc(weights, desc):
@@ -203,21 +229,7 @@ def write_huf_desc(weights, desc):
         ws = list(weights) + [0]
         return bytes([127 + n]) + bytes((ws[i] << 4) | ws[i + 1] for i in range(0, n, 2))
     _, log, norm = desc
-    tab, n = fse_table(norm, log), len(weights)
-    assert n >= 2
-    # two interleaved states: weight i comes from state i & 1; the update after weight n-2 reads past the stream's start
-    st = [None] * n
-    st[n - 1] = _first_state(tab, weights[n - 1])
-    st[n - 2] = _first_state(tab, weights[n - 2], 1)
-    for i in range(n - 3, -1, -1):
-        st[i] = _pick_state(tab, weights[i], st[i + 2])
-    w = BitW()
-    for i in range(n - 3, -1, -1):
-        _, nb, base = tab[st[i]]
-        w.add(st[i + 2] - base, nb)
-    w.add(st[1], log)
-    w.add(st[0], log)
-    body = write_ncount(norm, log) + w.backward()
+    body = huf_fse_weights(weights, log, norm, lambda tab, s: _first_state(tab, s, 1))
     assert len(body) < 128
     return bytes([len(body)]) + body
 
@@ -265,15 +277,24 @@ class Huf:
 
 
 def huf_stream(table, data):
+    """One Huffman stream: the codes of data's bytes from the last to the first, LSB first, then the end marker (packed with
+    numpy: each code's bit j lands at the code's start + j)."""
     mb, entries = table
-    code = {}
+    code, ln = np.zeros(256, dtype=np.int64), np.zeros(256, dtype=np.int64)
     for i, (s, nb) in enumerate(entries):
-        if s not in code:
-            code[s] = (i >> (mb - nb), nb)
-    w = BitW()
-    for b in reversed(data):
-        w.add(*code[b])
-    return w.backward()
+        if not ln[s]:
+            code[s], ln[s] = i >> (mb - nb), nb
+    d = np.frombuffer(bytes(data), dtype=np.uint8)[::-1]
+    c, n = code[d], ln[d]
+    assert n.all(), "a byte without a code"
+    start = np.cumsum(n) - n
+    total = int(n.sum())
+    bits = np.zeros(total + 1, dtype=np.uint8)
+    for j in range(mb):
+        m = n > j
+        bits[start[m] + j] = (c[m] >> j) & 1
+    bits[total] = 1
+    return np.packbits(bits, bitorder="little").tobytes()
 
 
 def lit_payload(table, data, streams):
@@ -298,15 +319,25 @@ def lit_header(lt, regen, comp=None, streams=1, sf=None):
     return (lt | (sf << 2) | (regen << 4) | (comp << (4 + bits))).to_bytes(n, "little")
 
 
+LL_BASE = [b for b, _ in LL_CODES]
+ML_BASE = [b for b, _ in ML_CODES]
+
+
 def seq_codes(ll, ml, ov):
-    llc = max(c for c, (b, _) in enumerate(LL_CODES) if b <= ll)
-    mlc = max(c for c, (b, _) in enumerate(ML_CODES) if b <= ml)
+    llc = bisect.bisect_right(LL_BASE, ll) - 1
+    mlc = bisect.bisect_right(ML_BASE, ml) - 1
     ofc = ov.bit_length() - 1
     return (llc, ll - LL_CODES[llc][0], LL_CODES[llc][1]), (ofc, ov - (1 << ofc), ofc), (mlc, ml - ML_CODES[mlc][0], ML_CODES[mlc][1])
 
 
-def seq_bitstream(seqs, tabs):
-    """tabs: per kind (ll, of, ml) the decoding table, or ("rle", code)."""
+def seq_count(n):
+    """Number_of_Sequences in 1, 2 or 3 bytes."""
+    return bytes([n]) if n < 128 else (bytes([(n >> 8) + 128, n & 0xFF]) if n < 0x7F00 else bytes([255]) + struct.pack("<H", n - 0x7F00))
+
+
+def seq_bitstream(seqs, tabs, first=_first_state):
+    """tabs: per kind (ll, of, ml) the decoding table, or ("rle", code).  first(tab, code): the state each chain ends in (the
+    decoder's initial state; any state of the last sequence's code is legal)."""
     cs = [seq_codes(*q) for q in seqs]      # per sequence: ((llc, extra, nb), (ofc, ...), (mlc, ...))
     n = len(cs)
     states = [[None] * n for _ in range(3)]
@@ -314,9 +345,10 @@ def seq_bitstream(seqs, tabs):
         if tabs[k][0] == "rle":
             assert all(c[k][0] == tabs[k][1] for c in cs), "a code other than the RLE code"
             continue
-        states[k][n - 1] = _first_state(tabs[k], cs[n - 1][k][0])
+        enc, st = _encoder(tabs[k]), states[k]
+        st[n - 1] = first(tabs[k], cs[n - 1][k][0])
         for i in range(n - 2, -1, -1):
-            states[k][i] = _pick_state(tabs[k], cs[i][k][0], states[k][i + 1])
+            st[i] = enc[cs[i][k][0]][st[i + 1]]
     w = BitW()
     for i in range(n - 1, -1, -1):
         if i < n - 1:
@@ -375,7 +407,7 @@ def block_content(b, state):
         pay = b.raw["lit_payload"] if "lit_payload" in b.raw else lit_payload(table, b.lits, b.streams)
         out += lit_header(2 if b.lit == "huf" else 3, len(b.lits), len(desc) + len(pay), b.streams, b.sf) + desc + pay
     n = len(b.seqs)
-    out += bytes([n]) if n < 128 else (bytes([(n >> 8) + 128, n & 0xFF]) if n < 0x7F00 else bytes([255]) + struct.pack("<H", n - 0x7F00))
+    out += seq_count(n)
     if n:
         out.append(sum({"pre": 0, "rle": 1, "fse": 2, "rep": 3}[m[0]] << (6 - 2 * k) for k, m in enumerate(b.modes)))
         enc = []

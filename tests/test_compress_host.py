@@ -1,13 +1,14 @@
 """CPU checks of the compressor's format layer: zstd-rs_b200/csrc/encode.cuh (the code k_cenc runs on the GPU) compiled for the
 host encodes crafted literal and sequence sets into Compressed blocks (tests/seqcraft.py); each is wrapped in a frame and must decode to the
-expected bytes with the oracle (ruzstd's decode semantics) and with libzstd.  Also: compress_bound and the layout of the new
-C-ABI structs."""
+expected bytes with the oracle (ruzstd's decode semantics) and with libzstd, and must be tests/cenc.py's block byte for byte.
+Also: compress_bound and the layout of the new C-ABI structs."""
 import os
 import random
 import subprocess
 
 import pytest
 
+import cenc
 import datagen
 import seqcraft
 from conftest import ROOT
@@ -26,6 +27,7 @@ def roundtrip(oracle, lits, seqs, history=b""):
     expect = seqcraft.execute(blocks)
     assert expect is not seqcraft.ERROR and len(expect) - len(history) <= 131072
     fr, [(huf, modes)] = seqcraft.frame(blocks)
+    assert cenc.encode_block(lits, seqs) == tuple(seqcraft.encode(lits, seqs)), "the host build is not the plain model"
     assert oracle.decode_frame(fr)[0] == expect
     assert datagen.decompress(fr, len(expect)) == expect
     return huf, modes

@@ -1,8 +1,8 @@
 """encode_block with a formatted dictionary's tables, on the host (tests/host/encode_dict_test.cpp, no GPU): crafted literal and
 sequence sets against a crafted dictionary, each block wrapped in a frame that carries the dictionary's ID, must decode to the
-plain LZ77 result (seqcraft.execute) with the oracle and with libzstd.  Covered: the three literal choices (Raw, own Huffman,
-Treeless with 1 and 4 streams), a literal byte the dictionary's Huffman table lacks, and each sequence table as Repeat /
-Compressed / RLE, including a code the dictionary's FSE table lacks."""
+plain LZ77 result (seqcraft.execute) with the oracle and with libzstd, and be tests/cenc.py's block byte for byte.  Covered: the
+three literal choices (Raw, own Huffman, Treeless with 1 and 4 streams), a literal byte the dictionary's Huffman table lacks, and
+each sequence table as Repeat / Compressed / RLE, including a code the dictionary's FSE table lacks."""
 import os
 import random
 import shutil
@@ -12,6 +12,7 @@ import tempfile
 
 import pytest
 
+import cenc
 import datagen
 import entcraft
 import seqcraft
@@ -55,6 +56,7 @@ def encode(tool, lits, seqs):
 def round_trip(oracle, tool, lits, seqs):
     """Encodes one first block, frames it with the dictionary's ID, and checks both decoders; returns (literals mode, modes)."""
     content, lit_mode, modes = encode(tool, lits, seqs)
+    assert cenc.encode_block(lits, seqs, cenc.Tables(tool[2])) == (content, lit_mode, modes), "the host build is not the plain model"
     plain = seqcraft.execute([("cmp", bytes(lits), seqs)])
     assert plain is not seqcraft.ERROR
     hdr = struct.pack("<IBBII", 0xFD2FB528, (2 << 6) | 3, (17 - 10) << 3, DICT_ID, len(plain))
