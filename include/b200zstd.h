@@ -607,6 +607,21 @@ typedef struct b200z_compress_result {
  * encoder's view of the tables is built on the host by the dictionary's first use with the flag (no kernel launch) and kept
  * until b200z_dict_destroy. */
 #define B200Z_FLAG_DICT_TABLES 4u
+/* context flag (EXTENSION; libzstd's --patch-from; DESIGN.md section 4.11, tests/cpatch.py states the rule):
+ * b200z_compress_frames_batch_long with a dictionary and window_log > 17 lets long matches take their source anywhere in the last
+ * 2^27 bytes of the dictionary's content D, at every level that runs the long-match stage (Fastest, LAZY, OPT, ULTRA).  Every
+ * block of every frame, also of frames of 131072 bytes or fewer, then has anchors; an anchor without an earlier anchor of its
+ * frame with the same key takes D's last anchor with that key, and its match may run back across D's end.  Each frame's
+ * Window_Descriptor carries min(window_log, max(17, ceil(log2(src_size + |D|)))), so every offset lies within the window and within
+ * position + |D|.  Repeat offsets never take their source from D, and ULTRA's far walk stays in the frame.  The first such use of a
+ * dictionary builds its anchors on the ctx stream: k_lanchor twice, k_lscan, four k_lhist / k_lscan / k_lscatter passes of the key
+ * sort and k_ldict, 16 launches (2 when D has no anchor, none when it is empty), counted in b200z_ctx_kernel_launches, with one synchronisation to size
+ * them; their scratch is the context's long-match buffers (44 bytes per anchor, kept with the context).  The sorted anchors,
+ * 8 bytes each (at most one per 16 bytes of D's last 2^27, about one per 128 on typical data), are kept with the dictionary until
+ * b200z_dict_destroy and reported by b200z_debug_held_bytes; a later submission launches exactly what it launches without them.
+ * Without a dictionary, at window_log 17 or at Uncompressed the flag changes no byte written.  b200z_frame_compressor_* (no
+ * dictionary) and the seekable writers (no window_log) are unaffected by it. */
+#define B200Z_FLAG_DICT_LONG 8u
 
 /* the largest frame b200z_compress_frames_batch can write for src_size bytes: src_size + 14 + 3 * max(1, ceil(src_size / 131072)) + 4 */
 size_t b200z_compress_bound(size_t src_size);
@@ -640,7 +655,8 @@ size_t b200z_compress_bound_dict(size_t src_size, const b200z_dict *dict);
  * tests/cldm.py states the rule).  The regular parse keeps its 128 KiB reach; in every frame larger than 131072 bytes, content-defined
  * anchors (a gear hash of 64 bytes, about 1 in 128 positions, at most 1 in 16) find the nearest earlier anchor of the same frame
  * with the same 64-byte hash, and where its offset lies in (131072, 2^window_log] and 64 or more bytes match inside the anchor's
- * block, that match is forced into the parse.  Long matches never reach into the dictionary.  Each frame's Window_Descriptor
+ * block, that match is forced into the parse.  Long matches reach into the dictionary only with B200Z_FLAG_DICT_LONG (see there;
+ * the header below then covers the dictionary too).  Each frame's Window_Descriptor
  * carries min(window_log, max(17, ceil(log2 src_size))), so a frame of 131072 bytes or fewer is exactly what window_log 17
  * writes, and window_log 17 is exactly b200z_compress_frames_batch_dict.  The compress bound is b200z_compress_bound_dict.  Besides
  * that entry's checks: B200Z_ERR_INVALID_ARGUMENT, before any launch, for window_log outside [17, 27] and for a window_log

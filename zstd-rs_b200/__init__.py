@@ -17,9 +17,9 @@ Import name: ``zstd_rs_b200`` (the directory name has a hyphen; see ``_pkg.py`` 
 """
 from .binding import (  # noqa: F401
     ALL, FASTEST, LAZY, OPT, ULTRA, UNCOMPRESSED, UPTO_BLOCKS, UPTO_BYTES, AllBatch, B200ZError, Batch, Context, Dictionary, FrameCompressor, FrameDecoder,
-    SeekableArchive, StreamingDecoder, build, compress, compress_bound, compress_frames, compress_profile, compress_seekable, compress_seekable_stream, compress_to_vec, create_dict, create_raw_dict,
+    SeekableArchive, StreamingDecoder, build, compress, compress_bound, compress_frames, compress_patch_from, compress_profile, compress_seekable, compress_seekable_stream, compress_to_vec, create_dict, create_raw_dict,
     create_raw_dict_from_dir,
     create_raw_dict_from_source, decode_all, decode_all_batch, decode_all_stream, decode_blocks, decode_frames,
-    dict_from_counts, error_names, finalize_dict, lib, lib_path, seekable_bound, seekable_plan, xxh64,
+    dict_from_counts, patch_window_log, error_names, finalize_dict, lib, lib_path, seekable_bound, seekable_plan, xxh64,
 )
 from . import binding  # noqa: F401

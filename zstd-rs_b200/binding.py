@@ -30,6 +30,7 @@ ERR_SEEKABLE_TABLE, ERR_SEEKABLE_FRAME_SIZE, ERR_SEEKABLE_IO = 240, 241, 242   #
 FLAG_CHECKSUM = 1
 FLAG_PROFILE = 2
 FLAG_DICT_TABLES = 4
+FLAG_DICT_LONG = 8   # EXTENSION (B200Z_FLAG_DICT_LONG): long matches into the dictionary's last 2^27 bytes (libzstd's --patch-from)
 HUF_DEBUG_BYTES, FSE_DEBUG_BYTES = 3088, 1040   # B200Z_DEBUG_HUF_BYTES / B200Z_DEBUG_FSE_BYTES: one raw huff0 / FSE table
 UNCOMPRESSED, FASTEST = 0, 1   # CompressionLevel (ruzstd encoding/mod.rs:24-67); Default / Better / Best are not implemented there
 LAZY = 5   # EXTENSION (B200Z_LEVEL_LAZY): a deeper parse with a lazy choice and repeat offsets; not ruzstd's output
@@ -574,20 +575,22 @@ def compress_bound(n, dict=None):
     return lib().b200z_compress_bound(n) if dict is None else lib().b200z_compress_bound_dict(n, dict.h)
 
 
-def compress_frames(ctx, input, io, output, level=FASTEST, checksum=True, dict=None, dict_tables=False, window_log=WINDOW_LOG_MIN):
+def compress_frames(ctx, input, io, output, level=FASTEST, checksum=True, dict=None, dict_tables=False, window_log=WINDOW_LOG_MIN,
+                    dict_long=False):
     """b200z_compress_frames_batch_long: one zstd frame per COMPRESS_IO_DTYPE row (src_off, src_size, dst_off, dst_cap), every block
     of every frame compressed at once, against `dict` (a Dictionary of this context) when given.  dict_tables=True sets
     FLAG_DICT_TABLES for the call: a formatted dictionary's entropy tables may then code each frame's first block.  window_log in
     [17, 27]: above 17, frames larger than 128 KiB also take long-distance matches up to 2^window_log bytes back (17 is
-    b200z_compress_frames_batch_dict's output).  input/output: bytes, numpy or torch (host or cuda).  Returns COMPRESS_RESULT_DTYPE
-    rows."""
+    b200z_compress_frames_batch_dict's output).  dict_long=True sets FLAG_DICT_LONG for the call: with `dict` and window_log > 17
+    the long matches of every frame also reach into the dictionary's last 2^27 bytes, and each frame's window covers the
+    dictionary (compress_patch_from).  input/output: bytes, numpy or torch (host or cuda).  Returns COMPRESS_RESULT_DTYPE rows."""
     fr = np.ascontiguousarray(io, dtype=COMPRESS_IO_DTYPE)
     res = np.zeros(len(fr), dtype=COMPRESS_RESULT_DTYPE)
     ip, il, _k1 = _ptr(input)
     op, ol, _k2 = _ptr(output)
     flags = ctx.L.b200z_ctx_flags(ctx.h)
-    if dict_tables:
-        ctx.L.b200z_ctx_set_flags(ctx.h, flags | FLAG_DICT_TABLES)
+    if dict_tables or dict_long:
+        ctx.L.b200z_ctx_set_flags(ctx.h, flags | (FLAG_DICT_TABLES if dict_tables else 0) | (FLAG_DICT_LONG if dict_long else 0))
     try:
         e = ctx.L.b200z_compress_frames_batch_long(ctx.h, ip, il, MEM_DEVICE if _is_device(input) else MEM_HOST, fr.ctypes.data, len(fr),
                                                    level, 1 if checksum else 0, dict.h if dict is not None else None, window_log, op, ol,
@@ -598,15 +601,42 @@ def compress_frames(ctx, input, io, output, level=FASTEST, checksum=True, dict=N
     return res
 
 
-def compress_to_vec(ctx, data, level=FASTEST, checksum=True, dict=None, dict_tables=False, window_log=WINDOW_LOG_MIN):
+def compress_to_vec(ctx, data, level=FASTEST, checksum=True, dict=None, dict_tables=False, window_log=WINDOW_LOG_MIN, dict_long=False):
     """Mirror of ruzstd::encoding::compress_to_vec (encoding/mod.rs): one frame holding `data`, as bytes (against `dict` when given,
-    with its entropy tables when dict_tables=True; long-distance matches up to 2^window_log back, see compress_frames)."""
+    with its entropy tables when dict_tables=True; long-distance matches up to 2^window_log back, into the dictionary too when
+    dict_long=True, see compress_frames)."""
     src = bytes(data)
     cap = compress_bound(len(src), dict)
     out = np.zeros(cap, dtype=np.uint8)
     io = np.array([(0, len(src), 0, cap)], dtype=COMPRESS_IO_DTYPE)
-    res = compress_frames(ctx, src, io, out, level, checksum, dict, dict_tables, window_log)
+    res = compress_frames(ctx, src, io, out, level, checksum, dict, dict_tables, window_log, dict_long)
     return out[:int(res[0]["dst_size"])].tobytes()
+
+
+def patch_window_log(reference_size, data_size):
+    """The window_log compress_patch_from uses: min(27, max(17, ceil(log2(reference_size + data_size))))."""
+    return min(WINDOW_LOG_MAX, max(WINDOW_LOG_MIN, (reference_size + data_size - 1).bit_length()))
+
+
+def compress_patch_from(ctx, reference, data, level=FASTEST, checksum=True):
+    """What `zstd --patch-from=reference` does: one frame of `data` compressed against `reference` as a raw-content dictionary, with
+    long-distance matches into all of it (the last 2^27 bytes of a larger one) at window_log patch_window_log(len(reference),
+    len(data)), as bytes.  The frame carries no dictionary ID, so it is decoded with the reference forced and a window limit of at
+    least the frame's window (2^window_log):
+
+        R = Dictionary.raw_content(ctx, 0, reference)
+        decode_frames(ctx, frame, io, out, forced_dict=R, max_window_size=1 << 27)      # or decode_all(..., forced_dict=R, ...)
+        d = FrameDecoder(ctx); d.add_raw_content_dict(1, reference); d.force_dict(1); d.set_max_window_size(1 << 27)
+        d.decode_all(frame, len(data))
+
+    libzstd decodes the same frame with ZSTD_decompress_usingDict (the reference as raw content) or ZSTD_DCtx_refPrefix, with
+    ZSTD_d_windowLogMax at least the frame's window_log."""
+    ref = bytes(reference)
+    D = Dictionary.raw_content(ctx, 0, ref)
+    try:
+        return compress_to_vec(ctx, data, level, checksum, D, window_log=patch_window_log(len(ref), len(data)), dict_long=True)
+    finally:
+        del D
 
 
 # ---- seekable archives (EXTENSION: zstd's seekable format; include/b200zstd.h, DESIGN.md section 4.10)

@@ -222,6 +222,11 @@ struct b200z_dict {
     int16_t norm[3][64] = {};
     uint32_t nnorm[3] = {}, log[3] = {};
     mutable DevBuf d_enc;
+    // B200Z_FLAG_DICT_LONG: the anchors of the content's last min(len, 2^27) bytes, sorted by key: nlanch keys, then nlanch distances
+    // from the content's end (ldm.cu k_ldict), built by the first long-match compression with the flag (lanch_built) and kept
+    mutable DevBuf d_lanch;
+    mutable uint32_t nlanch = 0;
+    mutable bool lanch_built = false;
 };
 
 static int dict_upload_content(b200z_dict *d, const uint8_t *content, size_t len) {
@@ -2837,7 +2842,7 @@ extern "C" int b200z_compress_frames_batch_dict(b200z_ctx *c, const uint8_t *inp
 // counted; with cap == 0 their total is read back to size the buffers (batch), else the buffers hold cap anchors (stream: the
 // density bound).  Then anchors, sort, candidates and the blocks' forced matches into a.lforced / lf_*.
 static int compress_ldm(b200z_ctx *c, LdmBufs &r, CompressArgs &a, const LSpan *d_spans, uint32_t nspans, uint32_t nblocks, uint32_t window_log,
-                        uint32_t cap, cudaStream_t s) {
+                        uint32_t cap, cudaStream_t s, const b200z_dict *ldict = nullptr) {
     int e = 0;
     if ((e = r.tcount.ensure((size_t)nspans * LDM_THREADS * sizeof(uint32_t))) || (e = r.scount.ensure((nspans + 1) * sizeof(uint32_t))) ||
         (e = r.off.ensure(nblocks * sizeof(uint32_t))) ||
@@ -2847,6 +2852,11 @@ static int compress_ldm(b200z_ctx *c, LdmBufs &r, CompressArgs &a, const LSpan *
     LdmArgs l{};
     l.input = a.input; l.spans = d_spans; l.nspans = nspans; l.window_log = window_log; l.tcount = r.tcount.as<uint32_t>();
     l.scount = r.scount.as<uint32_t>();
+    if (ldict) {   // B200Z_FLAG_DICT_LONG: candidates and sources in the dictionary too
+        l.dict_long = true;
+        l.ld = LDict{ldict->d_lanch.as<uint32_t>(), ldict->d_lanch.as<uint32_t>() + ldict->nlanch, ldict->nlanch, a.frames};
+        l.ds = LDictSrc{ldict->d_content.as<uint8_t>(), ldict->content_len};
+    }
     if (int le = launch_ldm_count(l, s, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_lanchor");
     l.cap = cap;
     if (!cap) {
@@ -2857,6 +2867,43 @@ static int compress_ldm(b200z_ctx *c, LdmBufs &r, CompressArgs &a, const LSpan *
     r.bind(l);
     if (int le = launch_ldm_match(l, s, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_lblock");
     a.lforced = l.forced; a.lf_off = l.lf_off; a.lf_cnt = l.lf_cnt;
+    return 0;
+}
+
+// B200Z_FLAG_DICT_LONG: the dictionary's anchors, by its first use with the flag.  k_lanchor counts them over spans of at most one
+// block of the content's last min(len, 2^27) bytes; their total is read back; then k_lanchor fills them, the key sort orders them
+// (the scratch is the context's long-match buffers) and k_ldict keeps (key, distance from the end) with the dictionary: 8 bytes per
+// anchor, LDM_DICT_LAUNCHES kernels (2 when there is none)
+static int dict_long_anchors(b200z_ctx *c, LdmBufs &r, const b200z_dict *d, cudaStream_t s) {
+    if (d->lanch_built) return 0;
+    const uint64_t len = d->content_len, lo = len - std::min<uint64_t>(len, LDM_DICT_REACH);
+    std::vector<LSpan> sp;
+    for (uint64_t o = lo; o < len; o += ENC_BLOCK) sp.push_back(LSpan{o, lo, (uint32_t)std::min<uint64_t>(ENC_BLOCK, len - o), 0, LDM_NO_BLOCK, 0});
+    if (!sp.empty()) {
+        const uint32_t ns = (uint32_t)sp.size();
+        int e = 0;
+        if ((e = r.spans.ensure(ns * sizeof(LSpan))) || (e = r.tcount.ensure((size_t)ns * LDM_THREADS * sizeof(uint32_t))) ||
+            (e = r.scount.ensure((ns + 1) * sizeof(uint32_t))))
+            return e;
+        CU(c, cudaMemcpyAsync(r.spans.p, sp.data(), ns * sizeof(LSpan), cudaMemcpyHostToDevice, s));
+        LdmArgs l{};
+        l.input = d->d_content.as<uint8_t>(); l.spans = r.spans.as<LSpan>(); l.nspans = ns; l.window_log = B200Z_WINDOW_LOG_MAX;
+        l.tcount = r.tcount.as<uint32_t>(); l.scount = r.scount.as<uint32_t>();
+        if (int le = launch_ldm_count(l, s, &c->launches)) return c->set_cuda_err((cudaError_t)le, "k_lanchor");
+        CU(c, cudaMemcpyAsync(&l.cap, l.scount + ns, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+        CU(c, cudaStreamSynchronize(s));
+        if (l.cap) {
+            if ((e = r.ensure(l.cap))) return e;
+            r.bind(l);
+            DevBuf keep;
+            CU(c, keep.alloc((size_t)l.cap * 2 * sizeof(uint32_t)));
+            if (int le = launch_ldm_dict(l, len, keep.as<uint32_t>(), keep.as<uint32_t>() + l.cap, s, &c->launches))
+                return c->set_cuda_err((cudaError_t)le, "k_ldict");
+            d->d_lanch = std::move(keep);
+            d->nlanch = l.cap;
+        }
+    }
+    d->lanch_built = true;
     return 0;
 }
 
@@ -2955,14 +3002,22 @@ extern "C" int b200z_compress_frames_batch_long(b200z_ctx *c, const uint8_t *inp
     a.frames = r.frames.as<CFrame>(); a.blocks = r.blocks.as<CBlock>(); a.input = d_in; a.output = d_out;
     a.nframes = (uint32_t)nframes; a.nblocks = (uint32_t)nblocks;
     a.window_log = (uint32_t)window_log;
-    if (fast && window_log > B200Z_WINDOW_LOG_MIN) {   // the blocks of the frames larger than one block
+    // B200Z_FLAG_DICT_LONG: long matches reach into the dictionary's content, and every frame's window covers it
+    const bool dlong = fast && dict && window_log > B200Z_WINDOW_LOG_MIN && (c->flags & B200Z_FLAG_DICT_LONG);
+    if (dlong) {
+        if ((e = dict_long_anchors(c, r.ldm, dict, s))) return e;
+        a.ldict = dict->d_content.as<uint8_t>(); a.ldict_len = dict->content_len;
+    }
+    if (fast && window_log > B200Z_WINDOW_LOG_MIN) {   // the blocks of the frames larger than one block (with the dictionary's reach: all)
         std::vector<LSpan> sp;
         for (uint32_t b = 0; b < (uint32_t)nblocks; b++)
-            if (hf[hb[b].frame].src_size > ENC_BLOCK) sp.push_back(LSpan{hb[b].src_off, hf[hb[b].frame].src_off, hb[b].size, hb[b].frame, b, 0});
+            if (dlong || hf[hb[b].frame].src_size > ENC_BLOCK) sp.push_back(LSpan{hb[b].src_off, hf[hb[b].frame].src_off, hb[b].size, hb[b].frame, b, 0});
         if (!sp.empty()) {
             if ((e = r.ldm.spans.ensure(sp.size() * sizeof(LSpan)))) return e;
             CU(c, cudaMemcpyAsync(r.ldm.spans.p, sp.data(), sp.size() * sizeof(LSpan), cudaMemcpyHostToDevice, s));
-            if ((e = compress_ldm(c, r.ldm, a, r.ldm.spans.as<LSpan>(), (uint32_t)sp.size(), (uint32_t)nblocks, (uint32_t)window_log, 0, s))) return e;
+            if ((e = compress_ldm(c, r.ldm, a, r.ldm.spans.as<LSpan>(), (uint32_t)sp.size(), (uint32_t)nblocks, (uint32_t)window_log, 0, s,
+                                  dlong ? dict : nullptr)))
+                return e;
         }
     }
     // ULTRA: the groups of whole blocks, each with the pieces of its far frames (their history, then their blocks in the group)

@@ -10,7 +10,8 @@
 //                 (<TABLES, true>: LAZY and OPT, repeat-offset codes within each block first)
 //   k_cxxh64    : content checksum of every frame's input (xxh64.cuh; four serial chains per frame)
 //   k_cassemble : one CTA per block: frame header, the block at its prefix-summed offset, the checksum, per-frame results
-//                 (<true>: one chunk of a streamed frame, blocks only; the host writes header, trailer and checksum)
+//                 (<true, false>: one chunk of a streamed frame, blocks only; the host writes header, trailer and checksum;
+//                 <false, true>: B200Z_FLAG_DICT_LONG, the Window_Descriptor covers the dictionary's content and the frame)
 //   k_cdict     : not a stage: the match table of a dictionary, built once the first time the dictionary is used (EXTENSION)
 //   k_dstats    : not a stage: literal and sequence-code histograms of k_cmatch's parse, for b200z_dict_finalize (EXTENSION)
 //
@@ -788,13 +789,14 @@ __global__ void k_cxxh64(const CFrame *__restrict__ frames, const uint8_t *__res
 // whole CTA); the first block also writes the frame header, the last one the checksum and the frame's result.
 // With STREAM (b200z_frame_compressor) a CFrame is one chunk of a frame whose header, trailing empty block and checksum the host
 // writes: the blocks are packed from the chunk's dst_off, and only a chunk that ends inside a block (the source ended there)
-// sets the last-block bit on its last block.  Its result holds the chunk's packed size and block counts.
+// sets the last-block bit on its last block.  Its result holds the chunk's packed size and block counts.  With DLONG
+// (B200Z_FLAG_DICT_LONG) the Window_Descriptor is frame_window_log of src_size + ldict_len.
 // ------------------------------------------------------------------------------------------------------------
-template <bool STREAM>
+template <bool STREAM, bool DLONG>
 __global__ void __launch_bounds__(256)
 k_cassemble(const CFrame *__restrict__ frames, const CBlock *__restrict__ blocks, const CBlockInfo *__restrict__ res, const uint8_t *__restrict__ enc,
             const uint8_t *__restrict__ input, const uint64_t *__restrict__ csum, uint8_t *__restrict__ output, b200z_compress_result *__restrict__ results,
-            int level, int checksum, uint32_t dict_id, uint32_t window_log) {
+            int level, int checksum, uint32_t dict_id, uint32_t window_log, uint64_t ldict_len) {
     __shared__ uint64_t s_red[3][8];
     const uint32_t b = blockIdx.x, tid = threadIdx.x;
     const CBlock blk = blocks[b];
@@ -827,7 +829,8 @@ k_cassemble(const CFrame *__restrict__ frames, const CBlock *__restrict__ blocks
         const uint32_t bh = (last ? 1u : 0u) | (type << 1) | ((type == 1 ? blk.size : csize) << 3);
         dst[0] = (uint8_t)bh; dst[1] = (uint8_t)(bh >> 8); dst[2] = (uint8_t)(bh >> 16);
         if (!STREAM && b == fr.first_block)
-            write_frame_header(output + fr.dst_off, fr.src_size, checksum != 0, dict_id, frame_window_log(fr.src_size, window_log));
+            write_frame_header(output + fr.dst_off, fr.src_size, checksum != 0, dict_id,
+                               frame_window_log(DLONG ? fr.src_size + ldict_len : fr.src_size, window_log));
     }
     for (uint32_t i = tid; i < csize; i += 256) dst[3 + i] = from[i];
     if (end && tid == 0) {
@@ -970,7 +973,11 @@ int launch_compress_stage(const CompressArgs &a, int stage, cudaStream_t s, uint
         else k_cenc<false, false><<<cdiv_u(a.nblocks, CE_WARPS), CE_WARPS * 32, 0, s>>>(a.blocks, a.nblocks, a.info, a.lits, a.seqs, a.enc, a.res, nullptr, nullptr);
         break;
     case 2: if (!a.checksum || !a.nframes) return 0; k_cxxh64<<<cdiv_u((uint64_t)a.nframes * 4, 128), 128, 0, s>>>(a.frames, a.input, a.csum, a.nframes); break;
-    case 3: if (!a.nblocks) return 0; k_cassemble<false><<<a.nblocks, 256, 0, s>>>(a.frames, a.blocks, a.res, a.enc, a.input, a.csum, a.output, a.results, a.level, a.checksum, a.dict_id, a.window_log); break;
+    case 3:
+        if (!a.nblocks) return 0;
+        if (a.ldict_len) k_cassemble<false, true><<<a.nblocks, 256, 0, s>>>(a.frames, a.blocks, a.res, a.enc, a.input, a.csum, a.output, a.results, a.level, a.checksum, a.dict_id, a.window_log, a.ldict_len);
+        else k_cassemble<false, false><<<a.nblocks, 256, 0, s>>>(a.frames, a.blocks, a.res, a.enc, a.input, a.csum, a.output, a.results, a.level, a.checksum, a.dict_id, a.window_log, 0);
+        break;
     default: return (int)cudaErrorInvalidValue;
     }
     const int e = (int)cudaGetLastError();
@@ -982,7 +989,7 @@ int launch_compress_chunk(const CompressArgs &a, cudaStream_t s, uint64_t *launc
     if (!a.nblocks) return 0;
     for (int st = 0; st < 2; st++)
         if (int e = launch_compress_stage(a, st, s, launched)) return e;
-    k_cassemble<true><<<a.nblocks, 256, 0, s>>>(a.frames, a.blocks, a.res, a.enc, a.input, nullptr, a.output, a.results, a.level, 0, 0, 0);
+    k_cassemble<true, false><<<a.nblocks, 256, 0, s>>>(a.frames, a.blocks, a.res, a.enc, a.input, nullptr, a.output, a.results, a.level, 0, 0, 0, 0);
     const int e = (int)cudaGetLastError();
     if (!e) ++*launched;
     return e;

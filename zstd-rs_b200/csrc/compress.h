@@ -70,6 +70,10 @@ struct CompressArgs {
     // walks' starts; fblk null: k_copt is OPT's kernel (no block of the submission has a window beyond 131072)
     const FBlock *fblk;
     const uint32_t *fkeys, *fvals, *fstart;
+    // B200Z_FLAG_DICT_LONG (ldm.cu): long matches reach into the dictionary's whole content ldict[ldict_len] (device), and each
+    // frame's Window_Descriptor covers ldict_len + its size; ldict_len 0 and ldict null: they do not
+    const uint8_t *ldict;
+    uint64_t ldict_len;
 };
 
 // ---- OPT (compress.cu): a CTA's chain covers the block and the ENC_WINDOW bytes before it
@@ -93,6 +97,19 @@ struct LSpan {         // up to ENC_BLOCK bytes whose anchors k_lanchor lists: a
     uint32_t block;    // its CBlock, whose forced matches k_lblock writes; LDM_NO_BLOCK for history
     uint32_t pad;
 };
+// B200Z_FLAG_DICT_LONG: the dictionary's anchors, built once per dictionary (launch_ldm_dict) and kept with it, for k_lcand<true>;
+// its content for k_lblock<true>, whose sources lie in the virtual stream D || X
+constexpr uint64_t LDM_DICT_REACH = 1ull << B200Z_WINDOW_LOG_MAX;   // the dictionary bytes, from its end, whose anchors are listed
+struct LDict {
+    const uint32_t *keys;   // [n] the anchors' keys, ascending; equal keys in position order
+    const uint32_t *dist;   // [n] |D| minus each anchor's position in D (1 .. 2^27)
+    uint32_t n;
+    const CFrame *frames;   // the submission's frames: an anchor's position in its frame is its input offset less src_off
+};
+struct LDictSrc {
+    const uint8_t *d;       // D's content (device), allocated with 16 bytes of padding
+    uint64_t len;           // |D|
+};
 struct LdmArgs {
     const uint8_t *input;
     const LSpan *spans;        // [nspans], in input order within each frame, the frames in submission order
@@ -105,11 +122,18 @@ struct LdmArgs {
     uint32_t *aframe, *cand;   // [cap] its frame, its candidate offset (0: none)
     LForced *forced;           // [cap]
     uint32_t *lf_off, *lf_cnt; // [blocks]: each span's CBlock's share of `forced`; lf_cnt zeroed by the host
+    bool dict_long;            // B200Z_FLAG_DICT_LONG: k_lcand<true> and k_lblock<true> over ld and ds
+    LDict ld;
+    LDictSrc ds;
 };
 // k_lanchor<false> and k_lscan: tcount, scount and the total; adds the kernels it enqueued to *launched
 int launch_ldm_count(const LdmArgs &a, cudaStream_t s, uint64_t *launched);
 // with the buffers sized for a.cap >= the total: k_lanchor<true>, the sort, k_lcand and k_lblock
 int launch_ldm_match(const LdmArgs &a, cudaStream_t s, uint64_t *launched);
+// a dictionary's anchors (B200Z_FLAG_DICT_LONG), after launch_ldm_count over the spans of D's last min(|D|, 2^27) bytes (input: D,
+// a.cap >= their total > 0): k_lanchor<true>, the sort and k_ldict, which writes the sorted keys[a.cap] and dist[a.cap] of |D| = dlen
+constexpr uint32_t LDM_DICT_LAUNCHES = 16;   // launch_ldm_count's 2, then k_lanchor<true>, four sort passes of three and k_ldict
+int launch_ldm_dict(const LdmArgs &a, uint64_t dlen, uint32_t *keys, uint32_t *dist, cudaStream_t s, uint64_t *launched);
 
 // ---- ULTRA's far stage (ldm.cu; DESIGN.md section 4.4, tests/cultra.py): per group of whole blocks (at most
 // B200Z_PIPELINE_CHUNK_BYTES of them, or a stream chunk) and the Wf bytes of its frame before its first block, the keyed positions'

@@ -9,9 +9,11 @@
 //   k_lscan    : one CTA: exclusive prefix sum of a u32 array in place (4,096 at a time, coalesced), its total after it
 //   k_lhist / k_lscatter : one stable LSD radix pass (8 bits) of the (key, anchor index) pairs, LDM_TILE pairs per CTA
 //   k_lcand    : per sorted pair, the predecessor with the same key -- the nearest earlier anchor with that key -- when it lies
-//                in the same frame at an offset in (ENC_WINDOW, 2^window_log]
+//                in the same frame at an offset in (ENC_WINDOW, 2^window_log]; <true> (B200Z_FLAG_DICT_LONG): without a
+//                predecessor in the frame, the dictionary's last anchor with the key (a binary search of its sorted keys)
 //   k_lblock   : one warp per span of a block: verify, extend inside the block, trim to the prefix max of earlier ends,
-//                coalesce, and write the block's forced matches for k_cmatch<..., true>
+//                coalesce, and write the block's forced matches for k_cmatch<..., true>; <true>: the source is D || X
+//   k_ldict    : per sorted pair of a dictionary's anchors, its key and distance from D's end, kept with the dictionary
 // The anchors' total stays on the device (scount[nspans]); grids are sized by the capacity and read it.
 //
 // ULTRA's far stage (compress.h, tests/cultra.py), per group:
@@ -195,27 +197,52 @@ k_lscatter(const uint32_t *__restrict__ kin, const uint32_t *__restrict__ vin, c
     }
 }
 
+template <bool DICT>
 __global__ void __launch_bounds__(256)
 k_lcand(const uint32_t *__restrict__ keys, const uint32_t *__restrict__ vals, const uint32_t *__restrict__ total, const uint64_t *__restrict__ apos,
-        const uint32_t *__restrict__ aframe, uint64_t reach, uint32_t *__restrict__ cand) {
+        const uint32_t *__restrict__ aframe, uint64_t reach, uint32_t *__restrict__ cand, LDict ld) {
     const uint32_t k = blockIdx.x * 256 + threadIdx.x;
     if (k >= *total) return;
     const uint32_t i = vals[k];
     uint32_t c = 0;
+    bool near = false;   // an earlier anchor of the frame has the key (in range or not)
     if (k > 0 && keys[k - 1] == keys[k]) {
         const uint32_t j = vals[k - 1];   // the stable sort keeps equal keys in anchor order: j < i
         const uint64_t off = apos[i] - apos[j];
+        near = aframe[j] == aframe[i];
         if (aframe[j] == aframe[i] && off > ENC_WINDOW && off <= reach) c = (uint32_t)off;
     }
+    if constexpr (DICT) {
+        if (!near && ld.n) {   // the dictionary's last pair with the key: the first with a larger key, less one
+            const uint32_t key = keys[k];
+            uint32_t lo = 0, hi = ld.n;
+            while (lo < hi) {
+                const uint32_t m = lo + (hi - lo) / 2;
+                if (ld.keys[m] <= key) lo = m + 1; else hi = m;
+            }
+            if (lo && ld.keys[lo - 1] == key) {
+                const uint64_t off = apos[i] - ld.frames[aframe[i]].src_off + ld.dist[lo - 1];
+                if (off > ENC_WINDOW && off <= reach) c = (uint32_t)off;
+            }
+        }
+    }
     cand[i] = c;
+}
+
+// byte x (block-relative) of the source `off` back in the virtual stream D || X: in the frame, or before its start (fb: the frame's
+// bytes before the block) at D's end.  Byte loads only: nothing before D's first byte or past its end is read
+__device__ __forceinline__ uint8_t ldict_src(const uint8_t *src, uint64_t fb, int32_t x, uint32_t off, const LDictSrc &ds) {
+    const int64_t q = (int64_t)fb + x - (int64_t)off;   // the source's position in the frame
+    return q >= 0 ? __ldg(src + ((int64_t)x - (int64_t)off)) : __ldg(ds.d + (int64_t)ds.len + q);
 }
 
 // one warp per span; spans of history (no block) write nothing.  The span's anchors are scount[sp] up to the next span's first
 // (scount[nspans]: the total).  Block-relative positions are signed where a 64-byte window may start
 // in the previous block.
+template <bool DICT>
 __global__ void __launch_bounds__(32)
 k_lblock(const LSpan *__restrict__ spans, const uint8_t *__restrict__ input, const uint32_t *__restrict__ scount, const uint64_t *__restrict__ apos,
-         const uint32_t *__restrict__ cand, LForced *__restrict__ forced, uint32_t *__restrict__ lf_off, uint32_t *__restrict__ lf_cnt) {
+         const uint32_t *__restrict__ cand, LForced *__restrict__ forced, uint32_t *__restrict__ lf_off, uint32_t *__restrict__ lf_cnt, LDictSrc ds) {
     const uint32_t sp = blockIdx.x, lane = threadIdx.x;
     const LSpan span = spans[sp];
     if (span.block == LDM_NO_BLOCK) return;
@@ -234,22 +261,33 @@ k_lblock(const LSpan *__restrict__ spans, const uint8_t *__restrict__ input, con
         if (nk && off == last.off && at < (int32_t)(last.start + last.len)) continue;
         const uint8_t *ref = src - off;
         const int32_t w0 = at - (int32_t)LDM_LEN + 1;
-        const bool eq = __ldg(src + w0 + lane) == __ldg(ref + w0 + lane) && __ldg(src + w0 + 32 + lane) == __ldg(ref + w0 + 32 + lane);
+        bool eq;
+        if constexpr (DICT)
+            eq = __ldg(src + w0 + lane) == ldict_src(src, fb, w0 + (int32_t)lane, off, ds) &&
+                 __ldg(src + w0 + 32 + lane) == ldict_src(src, fb, w0 + 32 + (int32_t)lane, off, ds);
+        else
+            eq = __ldg(src + w0 + lane) == __ldg(ref + w0 + lane) && __ldg(src + w0 + 32 + lane) == __ldg(ref + w0 + 32 + lane);
         if (!__all_sync(0xffffffffu, eq)) continue;
         int32_t e = at + 1;
         while (true) {
             const int32_t x = e + (int32_t)lane;
-            const uint32_t sm = __ballot_sync(0xffffffffu, x >= n || __ldg(src + x) != __ldg(ref + x));
+            uint32_t sm;
+            if constexpr (DICT) sm = __ballot_sync(0xffffffffu, x >= n || __ldg(src + x) != ldict_src(src, fb, x, off, ds));
+            else sm = __ballot_sync(0xffffffffu, x >= n || __ldg(src + x) != __ldg(ref + x));
             if (sm) { e += __ffs(sm) - 1; break; }
             e += 32;
         }
         // backward from the window's start, not below the prefix max of earlier ends (the match is trimmed there anyway), the
-        // block's start, nor where the source would leave the frame
-        const int32_t lo = max(maxend, off > fb ? (int32_t)(off - fb) : 0);
+        // block's start, nor where the source would leave the frame (DICT: D)
+        int32_t lo;
+        if constexpr (DICT) lo = max(maxend, off > fb + ds.len ? (int32_t)(off - fb - ds.len) : 0);
+        else lo = max(maxend, off > fb ? (int32_t)(off - fb) : 0);
         int32_t s = max(w0, lo);
         while (s > lo) {
             const int32_t x = s - 1 - (int32_t)lane;
-            const uint32_t sm = __ballot_sync(0xffffffffu, x < lo || __ldg(src + x) != __ldg(ref + x));
+            uint32_t sm;
+            if constexpr (DICT) sm = __ballot_sync(0xffffffffu, x < lo || __ldg(src + x) != ldict_src(src, fb, x, off, ds));
+            else sm = __ballot_sync(0xffffffffu, x < lo || __ldg(src + x) != __ldg(ref + x));
             if (sm) { s -= __ffs(sm) - 1; break; }
             s -= 32;
         }
@@ -269,6 +307,15 @@ k_lblock(const LSpan *__restrict__ spans, const uint8_t *__restrict__ input, con
         lf_off[span.block] = a0;
         lf_cnt[span.block] = nk;
     }
+}
+
+__global__ void __launch_bounds__(256)
+k_ldict(const uint32_t *__restrict__ keys, const uint32_t *__restrict__ vals, const uint32_t *__restrict__ total, const uint64_t *__restrict__ apos,
+        uint64_t dlen, uint32_t *__restrict__ dkeys, uint32_t *__restrict__ ddist) {
+    const uint32_t k = blockIdx.x * 256 + threadIdx.x;
+    if (k >= *total) return;
+    dkeys[k] = keys[k];
+    ddist[k] = (uint32_t)(dlen - apos[vals[k]]);
 }
 
 __global__ void __launch_bounds__(256)
@@ -332,25 +379,40 @@ int launch_ldm_count(const LdmArgs &a, cudaStream_t s, uint64_t *launched) {
     return counted(launched);
 }
 
+// k_lanchor<true> and the four passes of the key sort over a.cap anchors: the sorted pairs end in keys[0] / vals[0]
+static int anchors_sorted(const LdmArgs &a, cudaStream_t s, uint64_t *launched) {
+    const uint32_t *total = a.scount + a.nspans;
+    k_lanchor<true><<<a.nspans, LDM_THREADS, 0, s>>>(a.spans, a.input, a.tcount, a.scount, a.keys[0], a.vals[0], a.apos, a.aframe);
+    if (int e = counted(launched)) return e;
+    const uint32_t ntiles = cdiv_l(a.cap, LDM_TILE);
+    for (uint32_t pass = 0; pass < 4; pass++) {
+        const uint32_t in = pass & 1;
+        k_lhist<<<ntiles, LS_THREADS, 0, s>>>(a.keys[in], total, 8 * pass, a.hist);
+        if (int e = counted(launched)) return e;
+        k_lscan<<<1, LSCAN_THREADS, 0, s>>>(a.hist, ntiles * 256);
+        if (int e = counted(launched)) return e;
+        k_lscatter<<<ntiles, LS_THREADS, 0, s>>>(a.keys[in], a.vals[in], total, 8 * pass, a.hist, a.keys[in ^ 1], a.vals[in ^ 1]);
+        if (int e = counted(launched)) return e;
+    }
+    return 0;
+}
+
 int launch_ldm_match(const LdmArgs &a, cudaStream_t s, uint64_t *launched) {
     const uint32_t *total = a.scount + a.nspans;
     if (a.cap) {
-        k_lanchor<true><<<a.nspans, LDM_THREADS, 0, s>>>(a.spans, a.input, a.tcount, a.scount, a.keys[0], a.vals[0], a.apos, a.aframe);
-        if (int e = counted(launched)) return e;
-        const uint32_t ntiles = cdiv_l(a.cap, LDM_TILE);
-        for (uint32_t pass = 0; pass < 4; pass++) {
-            const uint32_t in = pass & 1;
-            k_lhist<<<ntiles, LS_THREADS, 0, s>>>(a.keys[in], total, 8 * pass, a.hist);
-            if (int e = counted(launched)) return e;
-            k_lscan<<<1, LSCAN_THREADS, 0, s>>>(a.hist, ntiles * 256);
-            if (int e = counted(launched)) return e;
-            k_lscatter<<<ntiles, LS_THREADS, 0, s>>>(a.keys[in], a.vals[in], total, 8 * pass, a.hist, a.keys[in ^ 1], a.vals[in ^ 1]);
-            if (int e = counted(launched)) return e;
-        }
-        k_lcand<<<cdiv_l(a.cap, 256), 256, 0, s>>>(a.keys[0], a.vals[0], total, a.apos, a.aframe, 1ull << a.window_log, a.cand);
+        if (int e = anchors_sorted(a, s, launched)) return e;
+        if (a.dict_long) k_lcand<true><<<cdiv_l(a.cap, 256), 256, 0, s>>>(a.keys[0], a.vals[0], total, a.apos, a.aframe, 1ull << a.window_log, a.cand, a.ld);
+        else k_lcand<false><<<cdiv_l(a.cap, 256), 256, 0, s>>>(a.keys[0], a.vals[0], total, a.apos, a.aframe, 1ull << a.window_log, a.cand, LDict{});
         if (int e = counted(launched)) return e;
     }
-    k_lblock<<<a.nspans, 32, 0, s>>>(a.spans, a.input, a.scount, a.apos, a.cand, a.forced, a.lf_off, a.lf_cnt);
+    if (a.dict_long) k_lblock<true><<<a.nspans, 32, 0, s>>>(a.spans, a.input, a.scount, a.apos, a.cand, a.forced, a.lf_off, a.lf_cnt, a.ds);
+    else k_lblock<false><<<a.nspans, 32, 0, s>>>(a.spans, a.input, a.scount, a.apos, a.cand, a.forced, a.lf_off, a.lf_cnt, LDictSrc{});
+    return counted(launched);
+}
+
+int launch_ldm_dict(const LdmArgs &a, uint64_t dlen, uint32_t *keys, uint32_t *dist, cudaStream_t s, uint64_t *launched) {
+    if (int e = anchors_sorted(a, s, launched)) return e;
+    k_ldict<<<cdiv_l(a.cap, 256), 256, 0, s>>>(a.keys[0], a.vals[0], a.scount + a.nspans, a.apos, dlen, keys, dist);
     return counted(launched);
 }
 
